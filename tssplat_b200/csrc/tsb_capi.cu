@@ -2,7 +2,6 @@
 #include <cuda_runtime.h>
 
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -59,19 +58,21 @@ int fail(tsb_handle_t h, int code, const std::string &msg) {
   return code;
 }
 
-template <class T>
-int upload(tsb_handle_t h, const T *src, size_t count, const T **out, size_t min_elems = 1) {
-  const size_t bytes = std::max(count, min_elems) * sizeof(T);
+// Copies src to a new device array of at least min_elems elements and points dst (the kernel's typed view of
+// the data, e.g. float4 over 4 floats) at it.
+template <class T, class A, class D>
+int upload(tsb_handle_t h, const std::vector<T, A> &src, D *&dst, size_t min_elems = 1) {
+  const size_t bytes = std::max(src.size(), min_elems) * sizeof(T);
   void *d = nullptr;
   cudaError_t e = cudaMalloc(&d, bytes);
   if (e != cudaSuccess) return fail(h, TSB_E_NOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e));
   h->allocs.push_back(d);
   h->info.device_bytes += int64_t(bytes);
-  if (count) {
-    e = cudaMemcpy(d, src, count * sizeof(T), cudaMemcpyHostToDevice);
+  if (!src.empty()) {
+    e = cudaMemcpy(d, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice);
     if (e != cudaSuccess) return fail(h, TSB_E_CUDA, std::string("cudaMemcpy: ") + cudaGetErrorString(e));
   }
-  *out = static_cast<const T *>(d);
+  dst = static_cast<D *>(d);
   return TSB_OK;
 }
 
@@ -89,13 +90,6 @@ int alloc_zero(tsb_handle_t h, size_t elems, T **out) {
   return TSB_OK;
 }
 
-int env_int(const char *name, int dflt) {
-  const char *e = std::getenv(name);
-  return e && *e ? std::atoi(e) : dflt;
-}
-
-struct Choice { int nw, ring, smem, ctas, global; };
-
 }  // namespace
 
 extern "C" {
@@ -105,24 +99,20 @@ int tsb_create(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t ne
   if (!out) return fail(nullptr, TSB_E_INVALID, "out is null");
   *out = nullptr;
   tsb::PlanConfig pc;
-  int nw = env_int("TSSPLAT_B200_WARPS", 16), ring = env_int("TSSPLAT_B200_RING_SLOTS", 2);
-  const int cpc = std::max(1, std::min(8, env_int("TSSPLAT_B200_CELLS_PER_CHUNK", 6)));
-  int tet_cost_x100 = env_int("TSSPLAT_B200_TET_COST_X100", 0);
+  int nw = 16, ring = 2;
   if (opt) {
     if (opt->warps_per_cta != 0) nw = opt->warps_per_cta;
     if (opt->ring_slots != 0) ring = opt->ring_slots;
-    if (opt->tet_cost_x100 > 0) tet_cost_x100 = opt->tet_cost_x100;
+    if (opt->tet_cost_x100 > 0) pc.tet_cost = float(opt->tet_cost_x100) / 100.f;
     pc.laplacian_scale = opt->laplacian_scale ? 1 : 0;
     pc.force_global = opt->force_global ? 1 : 0;
     pc.enable_amips = opt->enable_amips ? 1 : 0;
   }
-  if (env_int("TSSPLAT_B200_FORCE_GLOBAL", 0)) pc.force_global = 1;
-  pc.max_lanes_per_row = std::max(1, std::min(4, env_int("TSSPLAT_B200_LANES_PER_ROW", pc.max_lanes_per_row)));
-  if (env_int("TSSPLAT_B200_TETCELL_COST_X100", 0) > 0) pc.tetcell_cost = float(env_int("TSSPLAT_B200_TETCELL_COST_X100", 0)) / 100.f;
   if (nw != 8 && nw != 16) return fail(nullptr, TSB_E_INVALID, "warps_per_cta must be 8 or 16");
   if (ring < 2 || ring > 8) return fail(nullptr, TSB_E_INVALID, "ring_slots must be in [2, 8]");
-  if (tet_cost_x100 > 0) pc.tet_cost = float(tet_cost_x100) / 100.f;
   pc.nw = nw;
+  pc.ring_cells = ring * tsb::kCellsPerChunk;   // the requested ring, also when the callback below shrinks it
+  const int cpc = tsb::kCellsPerChunk;
 
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev) {
@@ -139,76 +129,52 @@ int tsb_create(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t ne
 
   // Called by the plan builder once the component sizes are known: pick the ring size that lets the
   // staging area fit, query occupancy, return the persistent grid.
-  Choice ch{nw, ring, 0, 0, 0};
-  std::string cb_err;
-  pc.grid_cb = [&](int /*vh*/, int area_verts, bool &global_mode) -> int {
+  int slots = ring, smem = 0, ctas_per_sm = 0;
+  pc.grid_cb = [&](int area_verts, bool &global_mode, int &grid, std::string &err) -> int {
     if (!global_mode) {
       int r = ring;
       while (r > 2 && tsb::energy_smem_bytes(nw, r, cpc, area_verts, false) > smem_optin) --r;
       if (tsb::energy_smem_bytes(nw, r, cpc, area_verts, false) > smem_optin) global_mode = true;
-      else ch.ring = r;
+      else slots = r;
     }
-    ch.global = global_mode ? 1 : 0;
-    if (global_mode) while (ch.ring > 2 && tsb::energy_smem_bytes(nw, ch.ring, cpc, 0, true) > smem_optin) --ch.ring;
-    ch.smem = tsb::energy_smem_bytes(nw, ch.ring, cpc, global_mode ? 0 : area_verts, global_mode);
+    if (global_mode) while (slots > 2 && tsb::energy_smem_bytes(nw, slots, cpc, 0, true) > smem_optin) --slots;
+    smem = tsb::energy_smem_bytes(nw, slots, cpc, global_mode ? 0 : area_verts, global_mode);
     int ctas = 0;
-    cudaError_t e = tsb::energy_occupancy(nw, ch.smem, global_mode, pc.enable_amips != 0, &ctas);
+    cudaError_t e = tsb::energy_occupancy(nw, smem, global_mode, pc.enable_amips != 0, &ctas);
     if (e != cudaSuccess || ctas < 1) {
-      cb_err = std::string("kernel does not fit the device: ") + (e != cudaSuccess ? cudaGetErrorString(e) : "occupancy 0");
-      return 0;
+      err = std::string("kernel does not fit the device: ") + (e != cudaSuccess ? cudaGetErrorString(e) : "occupancy 0");
+      return TSB_E_CUDA;
     }
-    const int want = env_int("TSSPLAT_B200_CTAS_PER_SM", nw == 16 ? 1 : 2);
-    ch.ctas = std::max(1, std::min(ctas, want));
-    return ch.ctas * sms;
+    ctas_per_sm = std::min(ctas, nw == 16 ? 1 : 2);
+    grid = ctas_per_sm * sms;
+    return TSB_OK;
   };
 
-  pc.ring_cells = env_int("TSSPLAT_B200_NO_SPLIT", 0) ? 0 : ring * cpc;
-  pc.rb_cap_div = std::max(1, env_int("TSSPLAT_B200_RB_CAP_DIV", pc.rb_cap_div));
-  if (env_int("TSSPLAT_B200_SEG_OVERHEAD_X100", -1) >= 0) pc.seg_overhead = float(env_int("TSSPLAT_B200_SEG_OVERHEAD_X100", 25)) / 100.f;
   tsb::HostPlan plan;
   std::string err;
   int rc = tsb::build_plan(rest_xyz, tets, n, nele, pc, plan, err);
-  if (rc != TSB_OK) return fail(nullptr, cb_err.empty() ? rc : TSB_E_CUDA, cb_err.empty() ? err : cb_err);
+  if (rc != TSB_OK) return fail(nullptr, rc, err);
 
   tsb_handle_t h = new tsb_handle_s();
   h->device = device;
   tsb::KParams &kp = h->kp;
 #define TSB_TRY(expr) do { rc = (expr); if (rc != TSB_OK) { g_create_err = h->err; tsb_destroy(h); return rc; } } while (0)
-  TSB_TRY(upload(h, plan.stream.data(), plan.stream.size(), &kp.stream, 16));
-  {
-    const float *x4 = nullptr;
-    TSB_TRY(upload(h, plan.X4.data(), plan.X4.size(), &x4, 4));
-    kp.X4 = reinterpret_cast<const float4 *>(x4);
-    const tsb::SegHdr *sg = nullptr;
-    TSB_TRY(upload(h, plan.segs.data(), plan.segs.size(), &sg, 1));
-    kp.segs = sg;
-    const int32_t *cs = nullptr;
-    TSB_TRY(upload(h, plan.cta_seg.data(), plan.cta_seg.size(), &cs, 2));
-    kp.cta_seg = reinterpret_cast<const int2 *>(cs);
-    const uint32_t *wd = nullptr;
-    TSB_TRY(upload(h, plan.wdesc.data(), plan.wdesc.size(), &wd, 2));
-    kp.wdesc = reinterpret_cast<const uint2 *>(wd);
-    const uint16_t *wsg = nullptr;
-    TSB_TRY(upload(h, plan.wseg.data(), plan.wseg.size(), &wsg, 2));
-    kp.wseg = reinterpret_cast<const ushort2 *>(wsg);
-  }
-  TSB_TRY(upload(h, plan.vlist.data(), plan.vlist.size(), &kp.vlist, 1));
-  TSB_TRY(upload(h, plan.pos16.data(), plan.pos16.size(), &kp.pos16, 2));
-  TSB_TRY(upload(h, plan.pos_gid.data(), plan.pos_gid.size(), &kp.pos_gid, 1));
-  TSB_TRY(upload(h, plan.orphans.data(), plan.orphans.size(), &kp.orphans, 1));
+  TSB_TRY(upload(h, plan.stream, kp.stream, 16));
+  TSB_TRY(upload(h, plan.X4, kp.X4, 4));
+  TSB_TRY(upload(h, plan.segs, kp.segs));
+  TSB_TRY(upload(h, plan.cta_seg, kp.cta_seg, 2));
+  TSB_TRY(upload(h, plan.wdesc, kp.wdesc, 2));
+  TSB_TRY(upload(h, plan.wseg, kp.wseg, 2));
+  TSB_TRY(upload(h, plan.vlist, kp.vlist));
+  TSB_TRY(upload(h, plan.pos16, kp.pos16, 2));
+  TSB_TRY(upload(h, plan.pos_gid, kp.pos_gid));
+  TSB_TRY(upload(h, plan.orphans, kp.orphans));
   if (pc.enable_amips) {
-    const float *bt = nullptr;
-    TSB_TRY(upload(h, plan.Bt.data(), plan.Bt.size(), &bt, 4));
-    kp.Bt = reinterpret_cast<const float4 *>(bt);
-    TSB_TRY(upload(h, plan.wtc0.data(), plan.wtc0.size(), &kp.wtc0, 1));
+    TSB_TRY(upload(h, plan.Bt, kp.Bt, 4));
+    TSB_TRY(upload(h, plan.wtc0, kp.wtc0));
   }
   TSB_TRY(alloc_zero(h, size_t(plan.n_components), &kp.done));
-  {
-    std::vector<unsigned long long> init(size_t(plan.grid) * 4, tsb::kEnergySentinel);
-    const unsigned long long *ce = nullptr;
-    TSB_TRY(upload(h, init.data(), init.size(), &ce, 2));
-    kp.cta_energy = reinterpret_cast<double *>(const_cast<unsigned long long *>(ce));
-  }
+  TSB_TRY(upload(h, std::vector<unsigned long long>(size_t(plan.grid) * 4, tsb::kEnergySentinel), kp.cta_energy, 2));
 #ifdef TSB_TRACE
   TSB_TRY(alloc_zero(h, size_t(plan.grid) * 16, &kp.trace));
 #endif
@@ -221,17 +187,17 @@ int tsb_create(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t ne
   kp.n_components = plan.n_components;
   kp.n = plan.n;
   kp.vh = plan.vh;
-  kp.ring_bytes = tsb::energy_ring_bytes(ch.ring, cpc, plan.mode_global != 0);
+  kp.ring_bytes = tsb::energy_ring_bytes(slots, cpc, plan.mode_global != 0);
   kp.cells_per_chunk = cpc;
-  kp.ring_slots = ch.ring;
+  kp.ring_slots = slots;
   kp.stage_bytes = plan.mode_global ? 0 : plan.area_verts * 32;
-  h->lc = tsb::LaunchConfig{nw, plan.grid, ch.smem, plan.mode_global, 0};
+  h->lc = tsb::LaunchConfig{nw, plan.grid, smem, plan.mode_global, 0};
   h->amips = pc.enable_amips != 0;
 
   tsb_info_t &I = h->info;
   I.n = plan.n; I.nele = plan.nele; I.n_components = plan.n_components; I.grid = plan.grid;
-  I.warps_per_cta = nw; I.ctas_per_sm = ch.ctas; I.mode_global = plan.mode_global; I.smem_bytes = ch.smem;
-  I.ring_slots = ch.ring; I.n_segments = int32_t(plan.segs.size()); I.n_boundary_faces = plan.n_boundary_faces;
+  I.warps_per_cta = nw; I.ctas_per_sm = ctas_per_sm; I.mode_global = plan.mode_global; I.smem_bytes = smem;
+  I.ring_slots = slots; I.n_segments = int32_t(plan.segs.size()); I.n_boundary_faces = plan.n_boundary_faces;
   I.max_component_vertices = plan.max_comp_verts; I.nnz = plan.nnz; I.nnz_padded = plan.nnz_padded;
   // bytes one launch requests: the warp streams, rest positions + x per staged component copy, grad
   int64_t staged = 0;

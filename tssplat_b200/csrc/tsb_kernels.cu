@@ -28,7 +28,6 @@
 
 #include <cmath>
 #include <cstdint>
-#include <cstdlib>
 
 #include "tsb_kernels.cuh"
 
@@ -713,8 +712,7 @@ cudaError_t launch_variant(const KParams &p, const LaunchConfig &lc, cudaStream_
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  static const int no_pdl = std::getenv("TSSPLAT_B200_NO_PDL") != nullptr;     // developer A/B switch
-  attr[0].val.programmaticStreamSerializationAllowed = no_pdl ? 0 : 1;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, energy_grad_kernel<NW, MINB, GLOBAL, AMIPS>, p);

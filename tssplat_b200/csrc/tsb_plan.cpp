@@ -5,12 +5,8 @@
 
 #include <algorithm>
 #include <atomic>
-#include <chrono>
-#include <cstdio>
 #include <cmath>
-#include <cstdlib>
 #include <cstring>
-#include <functional>
 #include <numeric>
 #include <thread>
 
@@ -45,8 +41,12 @@ struct UnionFind {
   }
 };
 
-// B = Dm^-1 (row-major) and det(Dm).  Returns false for a degenerate tet.
-bool invert3(const double *m, double *o, double *det) {
+// B = Dm^-1 (row-major) and det(Dm) of the tet with vertices v[0..3] in this order (Dm column k = X_{k+1} - X_0).
+// Returns false for a degenerate tet.
+bool rest_inverse(const float *rest, const int32_t *v, double *o, double *det) {
+  double m[9];
+  for (int r = 0; r < 3; ++r)
+    for (int k = 0; k < 3; ++k) m[3 * r + k] = double(rest[3 * size_t(v[k + 1]) + r]) - double(rest[3 * size_t(v[0]) + r]);
   const double c00 = m[4] * m[8] - m[5] * m[7], c01 = m[5] * m[6] - m[3] * m[8], c02 = m[3] * m[7] - m[4] * m[6];
   const double d = m[0] * c00 + m[1] * c01 + m[2] * c02;
   if (d == 0.0 || !std::isfinite(d)) return false;
@@ -124,18 +124,13 @@ void build_rows(const Mesh &M, Comp &C) {
   const int nv = int(C.verts.size()), nt = int(C.tets.size());
   // hat gradients of every tet of the component (fp64)
   std::vector<double> A(size_t(nt) * 12);
-  {
-    for (int tl = 0; tl < nt; ++tl) {
-      const int32_t *v = M.tets + 4 * size_t(C.tets[tl]);
-      double Dm[9], B[9], det;
-      for (int r = 0; r < 3; ++r)
-        for (int k = 0; k < 3; ++k) Dm[3 * r + k] = double(M.rest[3 * size_t(v[k + 1]) + r]) - double(M.rest[3 * size_t(v[0]) + r]);
-      invert3(Dm, B, &det);   // validated earlier
-      double *a = &A[size_t(tl) * 12];
-      for (int c = 0; c < 3; ++c) {
-        a[3 + c] = B[c]; a[6 + c] = B[3 + c]; a[9 + c] = B[6 + c];
-        a[c] = -(B[c] + B[3 + c] + B[6 + c]);
-      }
+  for (int tl = 0; tl < nt; ++tl) {
+    double B[9], det;
+    rest_inverse(M.rest, M.tets + 4 * size_t(C.tets[tl]), B, &det);   // validated earlier
+    double *a = &A[size_t(tl) * 12];
+    for (int c = 0; c < 3; ++c) {
+      a[3 + c] = B[c]; a[6 + c] = B[3 + c]; a[9 + c] = B[6 + c];
+      a[c] = -(B[c] + B[3 + c] + B[6 + c]);
     }
   }
   // local tet lookup through a sorted search (component tets are ascending)
@@ -566,10 +561,8 @@ void emit_tc(std::vector<uint8_t> &s, const Mesh &M, const Comp &C, int t0, int 
     const int32_t *v0 = M.tets + 4 * size_t(t);
     int32_t v[4];
     for (int c = 0; c < 4; ++c) v[c] = v0[kPerm[perm_of[i]][c]];
-    double Dm[9], B[9], det;
-    for (int r = 0; r < 3; ++r)
-      for (int c = 0; c < 3; ++c) Dm[3 * r + c] = double(M.rest[3 * size_t(v[c + 1]) + r]) - double(M.rest[3 * size_t(v[0]) + r]);
-    invert3(Dm, B, &det);
+    double B[9], det;
+    rest_inverse(M.rest, v, B, &det);
     for (int c = 0; c < 4; ++c)
       put<IDX>(s, o + ((size_t(l) * TPL + k) * 4 + c) * sizeof(IDX), kGlobal ? IDX(v[c]) : IDX(xbase_bytes + C.pos[M.local_of[v[c]]] * 16));
     put<float>(s, o + DOFF + (size_t(l) * TPL + k) * 4, float(1.0 / det));
@@ -579,263 +572,247 @@ void emit_tc(std::vector<uint8_t> &s, const Mesh &M, const Comp &C, int t0, int 
   }
 }
 
-}  // namespace
+constexpr int kMaxHostThreads = 32;
+constexpr double kRowCost = 2.0;        // cost of one vertex row (header, store) in operator entries (CTA-level cut)
+constexpr float kTetCellCost = 1.3f;    // cost of one tet cell relative to one quad cell (warp-level deal)
+constexpr float kSegOverhead = 0.60f;   // fixed cost of every (CTA, component) segment, as a fraction of the mean CTA cost
+constexpr int kMaxLanesPerRow = 4;      // rows may be split over up to this many adjacent lanes (latency regime only)
+constexpr int kRbCapDiv = 2;            // latency regime: a row block is at most ring_cells / kRbCapDiv quad cells
 
-// run fn(begin, end) over [0, count) on up to `nth` threads (contiguous ranges of at least `grain` items)
+// Runs fn(begin, end) over [0, count) in chunks of `grain` items, handed out in order to up to `nth` host threads
+// (the calling one included) as they become free.  The items of every phase are independent, so the plan does not
+// depend on how they are split.
 template <class F>
-static void parallel_ranges(size_t count, int nth, size_t grain, F fn) {
-  nth = int(std::max<size_t>(1, std::min<size_t>(size_t(std::max(nth, 1)), count / grain + 1)));
-  if (nth == 1) { fn(size_t(0), count); return; }
+void parallel_for(size_t count, size_t grain, int nth, F fn) {
+  const size_t chunks = (count + grain - 1) / grain;
+  std::atomic<size_t> next{0};
+  auto work = [&] {
+    for (size_t c = next++; c < chunks; c = next++) fn(c * grain, std::min(count, (c + 1) * grain));
+  };
   std::vector<std::thread> th;
-  const size_t per = (count + size_t(nth) - 1) / size_t(nth);
-  for (int k = 0; k < nth; ++k) {
-    const size_t b = std::min(count, per * size_t(k)), e = std::min(count, b + per);
-    if (b < e) th.emplace_back([=] { fn(b, e); });
-  }
+  for (size_t k = 1; k < std::min(chunks, size_t(nth)); ++k) th.emplace_back(work);
+  work();
   for (auto &t : th) t.join();
 }
 
-int build_plan(const float *rest, const int32_t *tets, int32_t n, int32_t nele, const PlanConfig &cfg,
-               HostPlan &P, std::string &err) {
-  const bool timing = std::getenv("TSSPLAT_B200_PLAN_TIMING") != nullptr;     // developer aid: phase times on stderr
-  auto t_last = std::chrono::steady_clock::now();
-#define TSB_T(name) do { if (timing) { auto t_now = std::chrono::steady_clock::now(); std::fprintf(stderr, "[plan] %-16s %.3f s\n", name, std::chrono::duration<double>(t_now - t_last).count()); t_last = t_now; } } while (0)
-  if (!rest || !tets || n <= 0 || nele <= 0) { err = "null input or non-positive size"; return TSB_E_INVALID; }
-  if (cfg.nw < 1 || cfg.nw > kMaxWarps || cfg.grid < 1) { err = "bad plan configuration"; return TSB_E_INVALID; }
-  if (n >= 0xFFFFFF) { err = "more than 16.7 M vertices in one handle (row-block headers hold 24-bit row ids): shard the mesh"; return TSB_E_INVALID; }
-  P = HostPlan();
-  P.n = n; P.nele = nele; P.laplacian_scale = cfg.laplacian_scale ? 1 : 0;
-  P.nw = cfg.nw;
-  const int NW = cfg.nw;
+// What is wrong with the tet with vertices v[0..3], or nullptr.  Checked in this order: vertex index out of
+// range, repeated vertex, zero rest volume.
+const char *tet_problem(const float *rest, const int32_t *v, int32_t n) {
+  for (int k = 0; k < 4; ++k)
+    if (v[k] < 0 || v[k] >= n) return "has a vertex index out of range";
+  if (v[0] == v[1] || v[0] == v[2] || v[0] == v[3] || v[1] == v[2] || v[1] == v[3] || v[2] == v[3]) return "repeats a vertex";
+  double B[9], det;
+  if (!rest_inverse(rest, v, B, &det) || !std::isfinite(float(1.0 / det))) return "has zero rest volume";
+  return nullptr;
+}
 
-  // ---- validate (parallel; the lowest offending tet is reported, like a serial scan would) ---------------
-  {
-    const int nth_v = cfg.threads > 0 ? cfg.threads : int(std::thread::hardware_concurrency());
-    std::atomic<int> bad_tet{nele};
-    parallel_ranges(size_t(nele), nth_v, 8192, [&](size_t b, size_t e) {
-      for (size_t t = b; t < e; ++t) {
-        const int32_t *v = tets + 4 * t;
-        bool bad = false;
-        for (int k = 0; k < 4; ++k) bad |= v[k] < 0 || v[k] >= n;
-        if (!bad) {
-          bad = v[0] == v[1] || v[0] == v[2] || v[0] == v[3] || v[1] == v[2] || v[1] == v[3] || v[2] == v[3];
-          if (!bad) {
-            double Dm[9], Bi[9], det;
-            for (int r = 0; r < 3; ++r)
-              for (int k = 0; k < 3; ++k) Dm[3 * r + k] = double(rest[3 * size_t(v[k + 1]) + r]) - double(rest[3 * size_t(v[0]) + r]);
-            bad = !invert3(Dm, Bi, &det) || !std::isfinite(float(1.0 / det));
-          }
-        }
-        if (bad) {
-          int cur = bad_tet.load();
-          while (int(t) < cur && !bad_tet.compare_exchange_weak(cur, int(t))) {}
-          return;       // later tets of this range cannot be the lowest
-        }
+// Reports the lowest offending tet, like a serial scan would.
+int validate(const float *rest, const int32_t *tets, int32_t n, int32_t nele, int nth, std::string &err) {
+  std::atomic<int> bad_tet{nele};
+  parallel_for(size_t(nele), 8192, nth, [&](size_t b, size_t e) {
+    for (size_t t = b; t < e; ++t)
+      if (tet_problem(rest, tets + 4 * t, n)) {
+        int cur = bad_tet.load();
+        while (int(t) < cur && !bad_tet.compare_exchange_weak(cur, int(t))) {}
+        return;       // later tets of this chunk cannot be the lowest
       }
-    });
-    if (bad_tet.load() < nele) {
-      const int t = bad_tet.load();
-      const int32_t *v = tets + 4 * size_t(t);
-      for (int k = 0; k < 4; ++k)
-        if (v[k] < 0 || v[k] >= n) { err = "tet " + std::to_string(t) + " has a vertex index out of range"; return TSB_E_MESH; }
-      if (v[0] == v[1] || v[0] == v[2] || v[0] == v[3] || v[1] == v[2] || v[1] == v[3] || v[2] == v[3]) {
-        err = "tet " + std::to_string(t) + " repeats a vertex"; return TSB_E_MESH;
-      }
-      err = "tet " + std::to_string(t) + " has zero rest volume"; return TSB_E_MESH;
-    }
-  }
+  });
+  const int t = bad_tet.load();
+  if (t == nele) return TSB_OK;
+  err = "tet " + std::to_string(t) + " " + tet_problem(rest, tets + 4 * size_t(t), n);
+  return TSB_E_MESH;
+}
 
-  TSB_T("validate");
-  // ---- face adjacency (neighbour tet across each face) and vertex components -----------------------
-  Mesh M{rest, tets, n, nele, std::vector<int32_t>(size_t(nele) * 4, -1), std::vector<int32_t>(size_t(n), -1), P.laplacian_scale};
-  UnionFind uf(n);
-  std::vector<uint8_t> used(n, 0);
-  for (int t = 0; t < nele; ++t) {
-    const int32_t *v = tets + 4 * size_t(t);
+// Vertex components (union-find over the tets), numbered by their lowest vertex, with their vertices and tets in
+// ascending order; vertices no tet references become orphans.
+std::vector<Comp> find_components(Mesh &M, HostPlan &P) {
+  UnionFind uf(M.n);
+  std::vector<uint8_t> used(M.n, 0);
+  for (int t = 0; t < M.nele; ++t) {
+    const int32_t *v = M.tets + 4 * size_t(t);
     uf.unite(v[0], v[1]); uf.unite(v[0], v[2]); uf.unite(v[0], v[3]);
     used[v[0]] = used[v[1]] = used[v[2]] = used[v[3]] = 1;
   }
-  TSB_T("union-find");
   std::vector<Comp> comps;
-  {
-    std::vector<int32_t> label(n, -1);
-    for (int v = 0; v < n; ++v) {
-      if (!used[v]) { P.orphans.push_back(v); continue; }
-      const int r = uf.find(v);
-      if (label[r] < 0) { label[r] = int32_t(comps.size()); comps.emplace_back(); }
-      Comp &C = comps[label[r]];
-      M.local_of[v] = int32_t(C.verts.size());
-      C.verts.push_back(v);
-    }
-    for (int t = 0; t < nele; ++t) comps[label[uf.find(tets[4 * size_t(t)])]].tets.push_back(t);
-    for (Comp &C : comps) {
-      for (size_t k = 0; k < C.verts.size(); ++k)
-        if (C.verts[k] != C.verts[0] + int32_t(k)) { C.contiguous = 0; break; }
-      P.max_comp_verts = std::max<int32_t>(P.max_comp_verts, int32_t(C.verts.size()));
-      if (!C.contiguous) P.contiguous = 0;
-    }
+  std::vector<int32_t> label(M.n, -1);
+  for (int v = 0; v < M.n; ++v) {
+    if (!used[v]) { P.orphans.push_back(v); continue; }
+    const int r = uf.find(v);
+    if (label[r] < 0) { label[r] = int32_t(comps.size()); comps.emplace_back(); }
+    Comp &C = comps[label[r]];
+    M.local_of[v] = int32_t(C.verts.size());
+    C.verts.push_back(v);
   }
-  const int NC = int(comps.size());
-  P.n_components = NC;
-  TSB_T("components");
-  // ---- face adjacency, operator rows and bank-aware staging positions, component-parallel ---------------
-  bool global_mode = cfg.force_global || P.max_comp_verts > cfg.area_cap || P.max_comp_verts > kMaxStagedVerts;
-  const bool identity_first = global_mode || std::getenv("TSSPLAT_B200_NO_PLACEMENT") != nullptr;
-  {
-    int nth = cfg.threads > 0 ? cfg.threads : int(std::thread::hardware_concurrency());
-    nth = std::max(1, std::min({nth, 32, NC}));
-    std::atomic<int> next{0};
-    std::atomic<int64_t> boundary{0};
-    std::atomic<int> bad{0};
-    auto work = [&]() {
-      for (int c = next.fetch_add(1); c < NC; c = next.fetch_add(1)) {
-        const int64_t bf = build_adjacency(M, comps[c]);
-        if (bf < 0) { bad.store(1); continue; }
-        boundary.fetch_add(bf);
-        build_rows(M, comps[c]);
-        place_vertices(comps[c], identity_first);
-      }
-    };
-    if (nth == 1) {
-      work();
-    } else {
-      std::vector<std::thread> th;
-      for (int i = 0; i < nth; ++i) th.emplace_back(work);
-      for (auto &t : th) t.join();
-    }
-    if (bad.load()) { err = "non-manifold mesh: a face is shared by more than two tets"; return TSB_E_MESH; }
-    P.n_boundary_faces = int32_t(boundary.load());
+  for (int t = 0; t < M.nele; ++t) comps[label[uf.find(M.tets[4 * size_t(t)])]].tets.push_back(t);
+  for (Comp &C : comps) {
+    for (size_t k = 0; k < C.verts.size(); ++k)
+      if (C.verts[k] != C.verts[0] + int32_t(k)) { C.contiguous = 0; break; }
+    P.max_comp_verts = std::max<int32_t>(P.max_comp_verts, int32_t(C.verts.size()));
+    if (!C.contiguous) P.contiguous = 0;
   }
+  P.n_components = int32_t(comps.size());
+  return comps;
+}
 
-  TSB_T("adjacency+rows+placement");
-  // ---- mode, bank-aware staging positions, staging capacities, grid ------------------------------------
-  auto place_all = [&](bool identity, bool redo) {
-    int vh = 0, mx = 0;
-    for (Comp &C : comps) {
-      if (redo) place_vertices(C, identity);
-      mx = std::max(mx, C.npos);
-      if (C.npos <= cfg.vh_cap) vh = std::max(vh, C.npos);
+// Face adjacency, operator rows and staging positions of every component.  Components differ a lot in size, so
+// they are handed out to the threads one at a time.
+int build_components(Mesh &M, std::vector<Comp> &comps, bool identity, int nth, HostPlan &P, std::string &err) {
+  std::atomic<int64_t> boundary{0};
+  std::atomic<bool> bad{false};
+  parallel_for(comps.size(), 1, nth, [&](size_t c0, size_t c1) {
+    for (size_t c = c0; c < c1; ++c) {
+      const int64_t bf = build_adjacency(M, comps[c]);
+      if (bf < 0) { bad = true; continue; }
+      boundary += bf;
+      build_rows(M, comps[c]);
+      place_vertices(comps[c], identity);
     }
-    P.vh = vh;
-    P.area_verts = std::max(2 * vh, mx);
-    return mx;
-  };
+  });
+  if (bad) { err = "non-manifold mesh: a face is shared by more than two tets"; return TSB_E_MESH; }
+  P.n_boundary_faces = int32_t(boundary.load());
+  for (const Comp &C : comps) P.nnz += int64_t(C.col.size());
+  return TSB_OK;
+}
+
+// Staging capacities, STAGED or GLOBAL mode (GLOBAL stores global vertex ids: identity placement, no staging) and
+// the grid.
+int choose_layout(std::vector<Comp> &comps, const PlanConfig &cfg, bool global_mode, HostPlan &P, std::string &err) {
   if (!global_mode) {
-    const int mx = place_all(identity_first, false);
-    if (mx > cfg.area_cap || mx > kMaxStagedVerts) global_mode = true;     // colouring padded a borderline component over the cap
+    int mx = 0;
+    for (const Comp &C : comps) {
+      mx = std::max(mx, C.npos);
+      if (C.npos <= cfg.vh_cap) P.vh = std::max(P.vh, C.npos);
+    }
+    P.area_verts = std::max(2 * P.vh, mx);
+    global_mode = mx > cfg.area_cap || mx > kMaxStagedVerts;     // colouring padded a borderline component over the cap
   }
   int G = cfg.grid;
-  if (cfg.grid_cb) G = cfg.grid_cb(P.vh, P.area_verts, global_mode);   // the caller sizes shared memory / occupancy
+  if (cfg.grid_cb) {
+    const int rc = cfg.grid_cb(P.area_verts, global_mode, G, err);
+    if (rc != TSB_OK) return rc;
+  }
   if (G < 1) { err = "bad grid size"; return TSB_E_INVALID; }
   P.grid = G;
   P.mode_global = global_mode ? 1 : 0;
-  const bool GLOBAL = global_mode;
-  if (GLOBAL) { place_all(true, !identity_first); P.vh = 0; P.area_verts = 0; }
+  if (global_mode) {
+    for (Comp &C : comps) place_vertices(C, true);
+    P.vh = 0; P.area_verts = 0;
+  }
+  return TSB_OK;
+}
 
-  TSB_T("placement");
-  // ---- cost stream and its G cuts --------------------------------------------------------------------
-  const double CR = 2.0, CT = double(cfg.tet_cost);
-  std::vector<double> crow(NC), ctot(NC), cbase(size_t(NC) + 1, 0.0);
+struct Cut { int comp; double f; };   // a point of the cost stream: fraction f of component comp
+
+// Fills CTAs greedily up to capacity T, of which every segment a CTA opens costs F.  Returns the number of CTAs
+// used and, with `out`, the cut where each of the first G begins.
+int fill_ctas(const std::vector<double> &ctot, double T, double F, int G, std::vector<Cut> *out) {
+  const int NC = int(ctot.size());
+  int b = 0, c = 0;
+  double f = 0.0;                       // position inside component c
+  if (out) (*out)[0] = {0, 0.0};
+  while (c < NC) {
+    double cap = T - F;                 // first segment of this CTA
+    while (c < NC && cap > 0) {
+      const double rem = (1.0 - f) * ctot[c];
+      if (rem <= cap * 1.02) {          // take the rest of the component (2% slack avoids slivers)
+        cap -= rem; ++c; f = 0.0;
+        if (c < NC) { cap -= F; if (cap < 0.10 * T) break; }      // not worth opening another segment
+      } else {
+        const double eps = std::min(0.05, 0.15 * T / std::max(ctot[c], 1e-30));
+        double nf = f + cap / ctot[c];
+        if (nf - f < eps) break;        // sliver: leave it to the next CTA
+        if (nf > 1.0 - eps) nf = 1.0;
+        f = nf; cap = 0;
+        if (f >= 1.0) { ++c; f = 0.0; }
+      }
+    }
+    ++b;
+    if (out && b <= G) (*out)[b] = (c >= NC) ? Cut{NC - 1, 1.0} : Cut{c, f};
+    if (b > 4 * G + 8) break;
+  }
+  return b;
+}
+
+// The G + 1 cuts of the cost stream (operator entries + kRowCost per row + tet_cost per tet, component after
+// component); CTA b takes [cuts[b], cuts[b + 1]).  Every segment a CTA touches costs a fixed overhead F on top of
+// its share of the stream (staging its component, a second set of partially filled row blocks): CTAs are filled
+// up to a capacity T that includes F per segment, and T is found by bisection so that exactly G CTAs consume the
+// stream.
+std::vector<Cut> cut_stream(const std::vector<Comp> &comps, double tet_cost, int G) {
+  const int NC = int(comps.size());
+  std::vector<double> ctot(NC);
+  double W = 0.0;
   for (int c = 0; c < NC; ++c) {
     const Comp &C = comps[c];
-    crow[c] = double(C.col.size()) + CR * double(C.verts.size());
-    ctot[c] = crow[c] + CT * double(C.tets.size());
-    cbase[c + 1] = cbase[c] + ctot[c];
-    P.nnz += int64_t(C.col.size());
+    ctot[c] = double(C.col.size()) + kRowCost * double(C.verts.size()) + tet_cost * double(C.tets.size());
+    W += ctot[c];
   }
-  const double W = cbase[NC];
-  // cut b (1..G-1) -> (component, fraction), snapped to the component boundary when it would leave a sliver
-  struct Cut { int comp; double f; };
+  const double F = double(kSegOverhead) * W / G;
+  double lo = W / G, hi = W + F * (NC + 1) + 1.0;      // hi: one CTA could take everything
+  for (int it = 0; it < 64; ++it) {
+    const double mid = 0.5 * (lo + hi);
+    if (fill_ctas(ctot, mid, F, G, nullptr) <= G) hi = mid; else lo = mid;
+  }
   std::vector<Cut> cuts(size_t(G) + 1);
-  cuts[0] = {0, 0.0};
-  cuts[G] = {NC - 1, 1.0};
-  {
-    // Every segment a CTA touches costs a fixed overhead F on top of its share of the stream (staging its
-    // component, a second set of partially filled row blocks): CTAs are filled greedily up to a capacity T
-    // that includes F per segment, and T is found by bisection so that exactly G CTAs consume the stream.
-    const double F = double(cfg.seg_overhead) * W / G;
-    auto fill = [&](double T, std::vector<Cut> *out) -> int {
-      int b = 0, c = 0;
-      double f = 0.0;                       // position inside component c
-      if (out) (*out)[0] = {0, 0.0};
-      while (c < NC) {
-        double cap = T - F;                 // first segment of this CTA
-        while (c < NC && cap > 0) {
-          const double rem = (1.0 - f) * ctot[c];
-          if (rem <= cap * 1.02) {          // take the rest of the component (2% slack avoids slivers)
-            cap -= rem; ++c; f = 0.0;
-            if (c < NC) { cap -= F; if (cap < 0.10 * T) break; }      // not worth opening another segment
-          } else {
-            const double eps = std::min(0.05, 0.15 * T / std::max(ctot[c], 1e-30));
-            double nf = f + cap / ctot[c];
-            if (nf - f < eps) break;        // sliver: leave it to the next CTA
-            if (nf > 1.0 - eps) nf = 1.0;
-            f = nf; cap = 0;
-            if (f >= 1.0) { ++c; f = 0.0; }
-          }
-        }
-        ++b;
-        if (out && b <= G) (*out)[b] = (c >= NC) ? Cut{NC - 1, 1.0} : Cut{c, f};
-        if (b > 4 * G + 8) break;
-      }
-      return b;
-    };
-    double lo = W / G, hi = W + F * (NC + 1) + 1.0;      // hi: one CTA could take everything
-    for (int it = 0; it < 64; ++it) {
-      const double mid = 0.5 * (lo + hi);
-      if (fill(mid, nullptr) <= G) hi = mid; else lo = mid;
-    }
-    const int used = fill(hi, &cuts);
-    for (int b = std::min(used, G); b <= G; ++b) cuts[b] = {NC - 1, 1.0};   // unused CTAs (tiny meshes) get nothing
-    cuts[G] = {NC - 1, 1.0};
-    for (int b = 1; b <= G; ++b) {   // monotone
-      const Cut &a = cuts[b - 1];
-      Cut &d = cuts[b];
-      if (d.comp < a.comp || (d.comp == a.comp && d.f < a.f)) d = a;
-    }
+  const int used = fill_ctas(ctot, hi, F, G, &cuts);
+  for (int b = std::min(used, G); b <= G; ++b) cuts[b] = {NC - 1, 1.0};   // unused CTAs (tiny meshes) get nothing
+  for (int b = 1; b <= G; ++b) {   // monotone
+    const Cut &a = cuts[b - 1];
+    Cut &d = cuts[b];
+    if (d.comp < a.comp || (d.comp == a.comp && d.f < a.f)) d = a;
   }
+  return cuts;
+}
 
-  // ---- segments --------------------------------------------------------------------------------------
-  struct Seg { int comp; int r0, r1, t0, t1; };
+struct Seg { int comp; int r0, r1, t0, t1; };   // rows [r0, r1) and tets [t0, t1) of a component
+
+// Row of component C at fraction f of its row cost (rc: cumulative row costs, built on first use).
+int row_at(const Comp &C, double f, std::vector<double> &rc) {
+  const int nv = int(C.verts.size());
+  if (f <= 0.0) return 0;
+  if (f >= 1.0) return nv;
+  if (rc.empty()) {
+    rc.resize(size_t(nv) + 1, 0.0);
+    for (int i = 0; i < nv; ++i) rc[i + 1] = rc[i] + double(C.rptr[i + 1] - C.rptr[i]) + kRowCost;
+  }
+  return int(std::lower_bound(rc.begin(), rc.end(), f * rc[nv]) - rc.begin());
+}
+
+int tet_at(const Comp &C, double f) {
+  const int nt = int(C.tets.size());
+  if (f <= 0.0) return 0;
+  if (f >= 1.0) return nt;
+  return int(std::llround(f * nt));
+}
+
+// The segments of every CTA, in CTA order (their range in P.cta_seg).
+std::vector<Seg> make_segments(const std::vector<Comp> &comps, const std::vector<Cut> &cuts, HostPlan &P) {
   std::vector<Seg> segs;
-  P.cta_seg.assign(size_t(G) * 2, 0);
-  std::vector<std::vector<double>> rowcum(NC);
-  auto row_at = [&](int c, double f) -> int {
-    const Comp &C = comps[c];
-    const int nv = int(C.verts.size());
-    if (f <= 0.0) return 0;
-    if (f >= 1.0) return nv;
-    std::vector<double> &rc = rowcum[c];
-    if (rc.empty()) {
-      rc.resize(size_t(nv) + 1, 0.0);
-      for (int i = 0; i < nv; ++i) rc[i + 1] = rc[i] + double(C.rptr[i + 1] - C.rptr[i]) + CR;
-    }
-    return int(std::lower_bound(rc.begin(), rc.end(), f * rc[nv]) - rc.begin());
-  };
-  auto tet_at = [&](int c, double f) -> int {
-    const int nt = int(comps[c].tets.size());
-    if (f <= 0.0) return 0;
-    if (f >= 1.0) return nt;
-    return int(std::llround(f * nt));
-  };
-  std::vector<int32_t> nseg_of(NC, 0);
-  for (int b = 0; b < G; ++b) {
+  std::vector<std::vector<double>> rowcum(comps.size());
+  P.cta_seg.assign(size_t(P.grid) * 2, 0);
+  for (int b = 0; b < P.grid; ++b) {
     P.cta_seg[2 * size_t(b)] = int32_t(segs.size());
     const Cut lo = cuts[b], hi = cuts[b + 1];
     for (int c = lo.comp; c <= hi.comp; ++c) {
       const double f0 = (c == lo.comp) ? lo.f : 0.0, f1 = (c == hi.comp) ? hi.f : 1.0;
       if (f1 <= f0) continue;
-      Seg s{c, row_at(c, f0), row_at(c, f1), tet_at(c, f0), tet_at(c, f1)};
+      const Comp &C = comps[c];
+      Seg s{c, row_at(C, f0, rowcum[c]), row_at(C, f1, rowcum[c]), tet_at(C, f0), tet_at(C, f1)};
       if (s.r1 <= s.r0 && s.t1 <= s.t0) continue;
       segs.push_back(s);
-      ++nseg_of[c];
     }
     P.cta_seg[2 * size_t(b) + 1] = int32_t(segs.size());
   }
-  const int NS = int(segs.size());
+  return segs;
+}
 
-  // ---- staging tables ----------------------------------------------------------------------------------
-  std::vector<int32_t> x4off(size_t(NC) + 1, 0), p4off(size_t(NC) + 1, 0);
+// Staging tables (STAGED: rest position, global id and staging position of every component vertex; GLOBAL: rest
+// positions by vertex id) and the segment headers.
+void staging_tables(const Mesh &M, const std::vector<Comp> &comps, const std::vector<Seg> &segs, HostPlan &P) {
+  const int NC = int(comps.size());
+  const bool GLOBAL = P.mode_global != 0;
+  std::vector<int32_t> x4off(size_t(NC) + 1, 0), p4off(size_t(NC) + 1, 0), nseg_of(NC, 0);
+  for (const Seg &g : segs) ++nseg_of[g.comp];
   if (!GLOBAL) {
     for (int c = 0; c < NC; ++c) x4off[c + 1] = x4off[c] + int32_t(comps[c].verts.size());
     P.X4.assign(size_t(x4off[NC]) * 4, 0.f);
@@ -846,18 +823,18 @@ int build_plan(const float *rest, const int32_t *tets, int32_t n, int32_t nele, 
     for (int c = 0; c < NC; ++c)
       for (size_t k = 0; k < comps[c].verts.size(); ++k) {
         const int32_t v = comps[c].verts[k];
-        for (int r = 0; r < 3; ++r) P.X4[(size_t(x4off[c]) + k) * 4 + r] = rest[3 * size_t(v) + r];
+        for (int r = 0; r < 3; ++r) P.X4[(size_t(x4off[c]) + k) * 4 + r] = M.rest[3 * size_t(v) + r];
         P.vlist[size_t(x4off[c]) + k] = v;
         P.pos16[size_t(x4off[c]) + k] = uint16_t(comps[c].pos[k]);
         P.pos_gid[size_t(p4off[c]) + comps[c].pos[k]] = v;
       }
   } else {
-    P.X4.assign(size_t(n) * 4, 0.f);
-    for (int v = 0; v < n; ++v)
-      for (int r = 0; r < 3; ++r) P.X4[size_t(v) * 4 + r] = rest[3 * size_t(v) + r];
+    P.X4.assign(size_t(M.n) * 4, 0.f);
+    for (int v = 0; v < M.n; ++v)
+      for (int r = 0; r < 3; ++r) P.X4[size_t(v) * 4 + r] = M.rest[3 * size_t(v) + r];
   }
-  P.segs.resize(NS);
-  for (int s = 0; s < NS; ++s) {
+  P.segs.resize(segs.size());
+  for (size_t s = 0; s < segs.size(); ++s) {
     const Seg &g = segs[s];
     const Comp &C = comps[g.comp];
     SegHdr &h = P.segs[s];
@@ -870,130 +847,144 @@ int build_plan(const float *rest, const int32_t *tets, int32_t n, int32_t nele, 
     h.npos = C.npos;
     h.p4off = GLOBAL ? 0 : p4off[g.comp];
   }
+}
 
-  TSB_T("segments+tables");
-  // ---- per-warp streams ----------------------------------------------------------------------------------
-  P.wseg.assign(size_t(NS) * NW * 2, 0);
-  P.wdesc.assign(size_t(G) * NW * 2, 0);
-  std::vector<std::vector<uint8_t>> wstream(size_t(G) * NW);
-  std::vector<std::vector<float>> wB(cfg.enable_amips ? size_t(G) * NW : 0);
+struct RB { int first, nrows, L, len4; };   // row block: rows[first, first + nrows), L lanes per row
+
+// Row blocks of a segment's rows (sorted by length) that has ntc tet cells.  L lanes per row (1, 2 or 4) is chosen
+// PER BLOCK: in the latency regime (the segment's cells fit the per-warp TMA rings, so nothing is ever refilled
+// mid-kernel) long rows are split over adjacent lanes until a block is at most `rb_cap` quad cells, which bounds
+// every warp's serial chain; in the streaming regime blocks are never split (fewest padded entries).
+int row_blocks(const std::vector<RowRef> &rows, int ntc, int NW, int ring_cells, std::vector<RB> &rbs, bool &latency,
+               std::string &err) {
+  int64_t cells1 = ntc;                        // cells of this segment with L = 1 everywhere
+  for (size_t i = 0; i < rows.size(); i += 32) cells1 += rb_len4(rows.data() + i, int(std::min<size_t>(32, rows.size() - i)), 1);
+  latency = cells1 * 10 <= int64_t(ring_cells) * NW * 9;
+  const int rb_cap = latency ? std::max(3, ring_cells / kRbCapDiv) : 62;
+  rbs.clear();
+  for (size_t i = 0; i < rows.size();) {
+    int L = 1;
+    while (L < kMaxLanesPerRow && rb_len4(rows.data() + i, 1, L) > rb_cap) L *= 2;
+    if (rb_len4(rows.data() + i, 1, L) > 62) { err = "a vertex has more than 980 operator neighbours"; return TSB_E_MESH; }
+    const int nr = int(std::min<size_t>(size_t(32 / L), rows.size() - i));
+    rbs.push_back(RB{int(i), nr, L, rb_len4(rows.data() + i, nr, L)});
+    i += nr;
+  }
+  return TSB_OK;
+}
+
+// What one CTA adds to the plan's counters, and the error that stopped it.
+struct CtaStats {
+  int64_t nnz_padded = 0, n_cells = 0, n_rb = 0, n_tetcells = 0, gwf[2] = {0, 0}, twf[2] = {0, 0};
+  int rc = TSB_OK;
+  std::string err;
+};
+
+// The streams of CTA b's warps (streams[w]; AMIPS: their rest inverses rest_inv[w]) and the CTA's entries of P.wseg.
+// Row blocks (longest first) and then tet cells go to the least loaded warp; loads carry over the CTA's segments,
+// which balances every warp's whole stream.
+void emit_cta(const Mesh &M, const std::vector<Comp> &comps, const std::vector<Seg> &segs, int ring_cells, int b,
+              HostPlan &P, std::vector<uint8_t> *streams, std::vector<float> *rest_inv, CtaStats &ES) {
+  const bool GLOBAL = P.mode_global != 0;
+  const int NW = P.nw;
   const int TPC = GLOBAL ? 32 : 64;                        // tets per tet cell
-  const double CTC = double(cfg.tetcell_cost) * (GLOBAL ? 0.6 : 1.0);
-  struct EmitStats { int64_t nnz_padded = 0, n_cells = 0, n_rb = 0, n_tetcells = 0, gwf[2] = {0, 0}, twf[2] = {0, 0}; int rc = TSB_OK; std::string err; };
-  // CTAs are independent: emit them on all host threads (each thread owns a contiguous range of CTAs)
-  auto emit_ctas = [&](int b_begin, int b_end, EmitStats &ES) {
+  const double CTC = double(kTetCellCost) * (GLOBAL ? 0.6 : 1.0);
+  const int s0 = P.cta_seg[2 * size_t(b)], s1 = P.cta_seg[2 * size_t(b) + 1];
   std::vector<RowRef> rows;
+  std::vector<RB> rbs;
   std::vector<int> rb_of_warp[kMaxWarps];
   LaneSlots lane_slots;
   double load[kMaxWarps] = {0};
-  for (int b = b_begin; b < b_end; ++b) {
-    for (int s = P.cta_seg[2 * size_t(b)]; s < P.cta_seg[2 * size_t(b) + 1]; ++s) {
-      const Seg &g = segs[s];
-      const Comp &C = comps[g.comp];
-      const int32_t *gid = GLOBAL ? C.verts.data() : nullptr;
-      // where this segment's component will sit in the CTA's staging area (must match the kernel:
-      // "whole" components start at 0, others alternate between the two halves by position in the CTA)
-      const int li = s - P.cta_seg[2 * size_t(b)];
-      const bool whole = P.segs[s].whole != 0;
-      const int ubase_bytes = GLOBAL ? 0 : (whole ? 0 : (li & 1) * 2 * P.vh * 16);
-      const int xbase_bytes = GLOBAL ? 0 : ubase_bytes + (whole ? C.npos : P.vh) * 16;
-      if (!GLOBAL && xbase_bytes + C.npos * 16 > 65536) { ES.err = "internal: staging offsets exceed 16 bits"; ES.rc = TSB_E_INVALID; return; }
-      rows.clear();
-      for (int r = g.r0; r < g.r1; ++r) rows.push_back(RowRef{r, C.rptr[r + 1] - C.rptr[r]});
-      std::stable_sort(rows.begin(), rows.end(), [](const RowRef &a, const RowRef &c) { return a.len > c.len; });
-      // Row blocks.  L lanes per row (1, 2 or 4) is chosen PER BLOCK: in the latency regime (the CTA's whole
-      // work fits the per-warp TMA rings, so nothing is ever refilled mid-kernel) long rows are split over
-      // adjacent lanes until a block is at most `rb_cap` quad cells, which bounds every warp's serial chain;
-      // in the streaming regime blocks are never split (fewest padded entries).
-      struct RB { int first, nrows, L, len4; };
-      std::vector<RB> rbs;
-      bool seg_latency = false;
-      {
-        const int ntc_total = (g.t1 - g.t0 + TPC - 1) / TPC;
-        int64_t cells1 = ntc_total;                        // cells of this segment with L = 1 everywhere
-        for (size_t i = 0; i < rows.size(); i += 32) cells1 += rb_len4(rows.data() + i, int(std::min<size_t>(32, rows.size() - i)), 1);
-        const bool latency_regime = cfg.ring_cells > 0 && cells1 * 10 <= int64_t(cfg.ring_cells) * NW * 9;
-        const int rb_cap = latency_regime ? std::max(3, cfg.ring_cells / cfg.rb_cap_div) : 62;
-        seg_latency = latency_regime;
-        size_t i = 0;
-        while (i < rows.size()) {
-          int L = 1;
-          while (L < 4 && rb_len4(rows.data() + i, 1, L) > (L < cfg.max_lanes_per_row ? rb_cap : 62)) L *= 2;
-          if (rb_len4(rows.data() + i, 1, L) > 62) { ES.err = "a vertex has more than 980 operator neighbours"; ES.rc = TSB_E_MESH; return; }
-          const int nr = int(std::min<size_t>(size_t(32 / L), rows.size() - i));
-          rbs.push_back(RB{int(i), nr, L, rb_len4(rows.data() + i, nr, L)});
-          i += nr;
-        }
+  for (int s = s0; s < s1; ++s) {
+    const Seg &g = segs[s];
+    const Comp &C = comps[g.comp];
+    const int32_t *gid = GLOBAL ? C.verts.data() : nullptr;
+    // where this segment's component will sit in the CTA's staging area (must match the kernel:
+    // "whole" components start at 0, others alternate between the two halves by position in the CTA)
+    const bool whole = P.segs[s].whole != 0;
+    const int ubase_bytes = GLOBAL ? 0 : (whole ? 0 : ((s - s0) & 1) * 2 * P.vh * 16);
+    const int xbase_bytes = GLOBAL ? 0 : ubase_bytes + (whole ? C.npos : P.vh) * 16;
+    if (!GLOBAL && xbase_bytes + C.npos * 16 > 65536) { ES.err = "internal: staging offsets exceed 16 bits"; ES.rc = TSB_E_INVALID; return; }
+    rows.clear();
+    for (int r = g.r0; r < g.r1; ++r) rows.push_back(RowRef{r, C.rptr[r + 1] - C.rptr[r]});
+    std::stable_sort(rows.begin(), rows.end(), [](const RowRef &a, const RowRef &c) { return a.len > c.len; });
+    const int ntc = (g.t1 - g.t0 + TPC - 1) / TPC;
+    bool latency = false;
+    if ((ES.rc = row_blocks(rows, ntc, NW, ring_cells, rbs, latency, ES.err)) != TSB_OK) return;
+    const int nrb = int(rbs.size());
+    for (int w = 0; w < NW; ++w) rb_of_warp[w].clear();
+    {
+      std::vector<int> order(nrb);
+      std::iota(order.begin(), order.end(), 0);
+      std::stable_sort(order.begin(), order.end(), [&](int a, int c) { return rbs[a].len4 > rbs[c].len4; });
+      for (int k : order) {                  // LPT: longest block first
+        int w = int(std::min_element(load, load + NW) - load);
+        load[w] += double(rbs[k].len4) + (latency ? 0.0 : 0.5);
+        rb_of_warp[w].push_back(k);
       }
-      const int nrb = int(rbs.size());
-      const int ntc = (g.t1 - g.t0 + TPC - 1) / TPC;
-      if (s == P.cta_seg[2 * size_t(b)]) for (int w = 0; w < NW; ++w) load[w] = 0.0;   // loads carry over the CTA's segments:
-      for (int w = 0; w < NW; ++w) rb_of_warp[w].clear();                               // balances every warp's whole stream
-      {
-        std::vector<int> order(nrb);
-        std::iota(order.begin(), order.end(), 0);
-        std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return rbs[a].len4 > rbs[b].len4; });
-        for (int k : order) {                  // LPT: longest block first
-          int w = int(std::min_element(load, load + NW) - load);
-          load[w] += double(rbs[k].len4) + (seg_latency ? 0.0 : 0.5);
-          rb_of_warp[w].push_back(k);
-        }
-      }
-      int tc_cnt[kMaxWarps] = {0};
-      const int NWT = NW > 1 ? NW - 1 : 1;     // the last warp signals "rows stored" and takes no tets (it must never wait on itself)
-      for (int k = 0; k < ntc; ++k) {
-        int w = int(std::min_element(load, load + NWT) - load);
-        load[w] += seg_latency ? 1.0 : CTC;     // latency regime: balance the CELL count so that every stream fits its ring
-        ++tc_cnt[w];
-      }
-      int tnext = g.t0;
-      for (int w = 0; w < NW; ++w) {
-        std::vector<uint8_t> &st = wstream[size_t(b) * NW + w];
-        for (int k : rb_of_warp[w]) {
-          const RB &rb = rbs[k];
-          const int len4 = GLOBAL ? emit_rb<uint32_t>(st, C, rows.data() + rb.first, rb.nrows, rb.L, gid, 0, lane_slots, nullptr)
-                                  : emit_rb<uint16_t>(st, C, rows.data() + rb.first, rb.nrows, rb.L, nullptr, ubase_bytes, lane_slots, ES.gwf);
-          ES.nnz_padded += int64_t(len4) * 4 * 32;
-          ES.n_cells += len4;
-        }
-        for (int k = 0; k < tc_cnt[w]; ++k) {
-          const int nt = std::min(TPC, g.t1 - tnext);
-          std::vector<float> *bo = cfg.enable_amips ? &wB[size_t(b) * NW + w] : nullptr;
-          if (GLOBAL) emit_tc<uint32_t>(st, M, C, tnext, nt, 0, nullptr, bo);
-          else emit_tc<uint16_t>(st, M, C, tnext, nt, xbase_bytes, ES.twf, bo);
-          tnext += nt;
-        }
-        if (rb_of_warp[w].size() > 0xFFFF || tc_cnt[w] > 0xFFFF) { ES.err = "segment too large for the stream descriptors"; ES.rc = TSB_E_INVALID; return; }
-        P.wseg[(size_t(s) * NW + w) * 2] = uint16_t(rb_of_warp[w].size());
-        P.wseg[(size_t(s) * NW + w) * 2 + 1] = uint16_t(tc_cnt[w]);
-      }
-      ES.n_rb += nrb;
-      ES.n_tetcells += ntc;
-      ES.n_cells += ntc;
     }
+    int tc_cnt[kMaxWarps] = {0};
+    const int NWT = NW > 1 ? NW - 1 : 1;     // the last warp signals "rows stored" and takes no tets (it must never wait on itself)
+    for (int k = 0; k < ntc; ++k) {
+      int w = int(std::min_element(load, load + NWT) - load);
+      load[w] += latency ? 1.0 : CTC;        // latency regime: balance the CELL count so that every stream fits its ring
+      ++tc_cnt[w];
+    }
+    int tnext = g.t0;
+    for (int w = 0; w < NW; ++w) {
+      std::vector<uint8_t> &st = streams[w];
+      for (int k : rb_of_warp[w]) {
+        const RB &rb = rbs[k];
+        const int len4 = GLOBAL ? emit_rb<uint32_t>(st, C, rows.data() + rb.first, rb.nrows, rb.L, gid, 0, lane_slots, nullptr)
+                                : emit_rb<uint16_t>(st, C, rows.data() + rb.first, rb.nrows, rb.L, nullptr, ubase_bytes, lane_slots, ES.gwf);
+        ES.nnz_padded += int64_t(len4) * 4 * 32;
+        ES.n_cells += len4;
+      }
+      for (int k = 0; k < tc_cnt[w]; ++k) {
+        const int nt = std::min(TPC, g.t1 - tnext);
+        std::vector<float> *bo = rest_inv ? &rest_inv[w] : nullptr;
+        if (GLOBAL) emit_tc<uint32_t>(st, M, C, tnext, nt, 0, nullptr, bo);
+        else emit_tc<uint16_t>(st, M, C, tnext, nt, xbase_bytes, ES.twf, bo);
+        tnext += nt;
+      }
+      if (rb_of_warp[w].size() > 0xFFFF || tc_cnt[w] > 0xFFFF) { ES.err = "segment too large for the stream descriptors"; ES.rc = TSB_E_INVALID; return; }
+      P.wseg[(size_t(s) * NW + w) * 2] = uint16_t(rb_of_warp[w].size());
+      P.wseg[(size_t(s) * NW + w) * 2 + 1] = uint16_t(tc_cnt[w]);
+    }
+    ES.n_rb += nrb;
+    ES.n_tetcells += ntc;
+    ES.n_cells += ntc;
   }
-  };
-  {
-    int nth = cfg.threads > 0 ? cfg.threads : int(std::thread::hardware_concurrency());
-    nth = std::max(1, std::min({nth, 32, G}));
-    std::vector<EmitStats> stats(nth);
-    std::vector<std::thread> th;
-    for (int i = 0; i < nth; ++i) {
-      const int b0 = int(int64_t(G) * i / nth), b1 = int(int64_t(G) * (i + 1) / nth);
-      if (nth == 1) emit_ctas(b0, b1, stats[i]);
-      else th.emplace_back([&, b0, b1, i]() { emit_ctas(b0, b1, stats[i]); });
-    }
-    for (auto &t : th) t.join();
-    for (const EmitStats &e : stats) {
-      if (e.rc != TSB_OK) { err = e.err; return e.rc; }
-      P.nnz_padded += e.nnz_padded; P.n_cells += e.n_cells; P.n_rb += e.n_rb; P.n_tetcells += e.n_tetcells;
-      P.gather_wavefronts[0] += e.gwf[0]; P.gather_wavefronts[1] += e.gwf[1];
-      P.tet_wavefronts[0] += e.twf[0]; P.tet_wavefronts[1] += e.twf[1];
-    }
+}
+
+// Every CTA's warp streams (wstream[b * nw + w]; AMIPS, when wB is not empty: the rest inverses in wB alike).
+// CTAs are independent and emitted in parallel; the first failing CTA's error is reported.
+int emit_ctas(const Mesh &M, const std::vector<Comp> &comps, const std::vector<Seg> &segs, int ring_cells, int nth,
+              HostPlan &P, std::vector<std::vector<uint8_t>> &wstream, std::vector<std::vector<float>> &wB, std::string &err) {
+  const size_t NW = size_t(P.nw);
+  P.wseg.assign(segs.size() * NW * 2, 0);
+  std::vector<CtaStats> stats(P.grid);
+  parallel_for(size_t(P.grid), 1, nth, [&](size_t b0, size_t b1) {
+    for (size_t b = b0; b < b1; ++b)
+      emit_cta(M, comps, segs, ring_cells, int(b), P, &wstream[b * NW], wB.empty() ? nullptr : &wB[b * NW], stats[b]);
+  });
+  for (const CtaStats &e : stats) {
+    if (e.rc != TSB_OK) { err = e.err; return e.rc; }
+    P.nnz_padded += e.nnz_padded; P.n_cells += e.n_cells; P.n_rb += e.n_rb; P.n_tetcells += e.n_tetcells;
+    P.gather_wavefronts[0] += e.gwf[0]; P.gather_wavefronts[1] += e.gwf[1];
+    P.tet_wavefronts[0] += e.twf[0]; P.tet_wavefronts[1] += e.twf[1];
   }
-  if (cfg.enable_amips) {       // rest inverses in (CTA, warp) order + the first tet cell of every (segment, warp)
-    P.wtc0.assign(size_t(NS) * NW, 0);
-    const size_t per_cell = size_t(3) * TPC * 4;
+  return TSB_OK;
+}
+
+// The plan's byte stream (the warp streams in (CTA, warp) order) and its descriptors; AMIPS: the rest inverses in
+// the same order and the first tet cell of every (segment, warp).
+int concat_streams(const std::vector<std::vector<uint8_t>> &wstream, const std::vector<std::vector<float>> &wB, int nth,
+                   HostPlan &P, std::string &err) {
+  const int G = P.grid, NW = P.nw;
+  if (!wB.empty()) {
+    P.wtc0.assign(P.segs.size() * NW, 0);
+    const size_t per_cell = size_t(3) * (P.mode_global ? 32 : 64) * 4;
     size_t cells = 0;
     for (int b = 0; b < G; ++b)
       for (int w = 0; w < NW; ++w) {
@@ -1006,28 +997,52 @@ int build_plan(const float *rest, const int32_t *tets, int32_t n, int32_t nele, 
       }
     if (P.Bt.size() != cells * per_cell) { err = "internal: AMIPS rest-inverse blocks out of step with the tet cells"; return TSB_E_INVALID; }
   }
-  TSB_T("emission");
   size_t total = 0;
   for (const auto &st : wstream) total += st.size();
   if (total / 16 > 0xFFFFFFFFull) { err = "plan stream exceeds 64 GiB"; return TSB_E_NOMEM; }
   P.stream.resize(std::max<size_t>(total, 16));
-  {
-    std::vector<size_t> offs(wstream.size() + 1, 0);
-    for (size_t i = 0; i < wstream.size(); ++i) {
-      if (wstream[i].size() > 0xFFFFFFFFull) { err = "warp stream exceeds 4 GiB"; return TSB_E_NOMEM; }
-      P.wdesc[2 * i] = uint32_t(offs[i] / 16);
-      P.wdesc[2 * i + 1] = uint32_t(wstream[i].size());
-      offs[i + 1] = offs[i] + wstream[i].size();
-    }
-    const int nth_c = cfg.threads > 0 ? cfg.threads : int(std::thread::hardware_concurrency());
-    uint8_t *dst = P.stream.data();
-    parallel_ranges(wstream.size(), total > (size_t(8) << 20) ? std::min(nth_c, 32) : 1, 16, [&](size_t b, size_t e) {
-      for (size_t i = b; i < e; ++i)
-        if (!wstream[i].empty()) std::memcpy(dst + offs[i], wstream[i].data(), wstream[i].size());
-    });
+  P.wdesc.assign(wstream.size() * 2, 0);
+  std::vector<size_t> offs(wstream.size() + 1, 0);
+  for (size_t i = 0; i < wstream.size(); ++i) {
+    if (wstream[i].size() > 0xFFFFFFFFull) { err = "warp stream exceeds 4 GiB"; return TSB_E_NOMEM; }
+    P.wdesc[2 * i] = uint32_t(offs[i] / 16);
+    P.wdesc[2 * i + 1] = uint32_t(wstream[i].size());
+    offs[i + 1] = offs[i] + wstream[i].size();
   }
-  TSB_T("concat");
+  uint8_t *dst = P.stream.data();
+  parallel_for(wstream.size(), 16, total > (size_t(8) << 20) ? nth : 1, [&](size_t b, size_t e) {
+    for (size_t i = b; i < e; ++i)
+      if (!wstream[i].empty()) std::memcpy(dst + offs[i], wstream[i].data(), wstream[i].size());
+  });
   return TSB_OK;
+}
+
+}  // namespace
+
+int build_plan(const float *rest, const int32_t *tets, int32_t n, int32_t nele, const PlanConfig &cfg,
+               HostPlan &P, std::string &err) {
+  if (!rest || !tets || n <= 0 || nele <= 0) { err = "null input or non-positive size"; return TSB_E_INVALID; }
+  if (cfg.nw < 1 || cfg.nw > kMaxWarps || cfg.grid < 1) { err = "bad plan configuration"; return TSB_E_INVALID; }
+  if (n >= 0xFFFFFF) { err = "more than 16.7 M vertices in one handle (row-block headers hold 24-bit row ids): shard the mesh"; return TSB_E_INVALID; }
+  P = HostPlan();
+  P.n = n; P.nele = nele; P.laplacian_scale = cfg.laplacian_scale ? 1 : 0;
+  P.nw = cfg.nw;
+  const int nth = std::clamp(int(std::thread::hardware_concurrency()), 1, kMaxHostThreads);
+
+  int rc = validate(rest, tets, n, nele, nth, err);
+  if (rc != TSB_OK) return rc;
+  Mesh M{rest, tets, n, nele, std::vector<int32_t>(size_t(nele) * 4, -1), std::vector<int32_t>(size_t(n), -1), P.laplacian_scale};
+  std::vector<Comp> comps = find_components(M, P);
+  // components too large to stage keep global ids (identity placement) from the start
+  const bool global_mode = cfg.force_global || P.max_comp_verts > cfg.area_cap || P.max_comp_verts > kMaxStagedVerts;
+  if ((rc = build_components(M, comps, global_mode, nth, P, err)) != TSB_OK) return rc;
+  if ((rc = choose_layout(comps, cfg, global_mode, P, err)) != TSB_OK) return rc;
+  const std::vector<Seg> segs = make_segments(comps, cut_stream(comps, double(cfg.tet_cost), P.grid), P);
+  staging_tables(M, comps, segs, P);
+  std::vector<std::vector<uint8_t>> wstream(size_t(P.grid) * P.nw);
+  std::vector<std::vector<float>> wB(cfg.enable_amips ? wstream.size() : 0);
+  if ((rc = emit_ctas(M, comps, segs, cfg.ring_cells, nth, P, wstream, wB, err)) != TSB_OK) return rc;
+  return concat_streams(wstream, wB, nth, P, err);
 }
 
 }  // namespace tsb

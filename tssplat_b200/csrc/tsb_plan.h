@@ -11,21 +11,23 @@
 //
 // Work decomposition.  The mesh is cut into connected components (= tet-spheres; they share no
 // vertices, geometry/tetmesh_geometry.py:305-331).  The cost stream of all components is cut into
-// `grid` equal pieces, one per persistent CTA; the piece of a component that lands in a CTA is a
-// *segment*: a contiguous range of the component's vertex rows and of its tets.  A CTA stages the
-// displacement u = x - X and the position x of the WHOLE component of each of its segments in
-// shared memory (32 B per vertex), so every gather is a shared-memory read.  Inside a segment the
-// rows are sorted by length, grouped into row blocks (RB) of 32 rows (one lane per row), and the RBs
-// plus the tet blocks (32 tets) are dealt to the CTA's warps so that every warp has the same cost.
+// `grid` pieces, one per persistent CTA, with a fixed charge per piece so that cuts snap to component
+// boundaries where they can; the piece of a component that lands in a CTA is a *segment*: a
+// contiguous range of the component's vertex rows and of its tets.  A CTA stages the displacement
+// u = x - X and the position x of the WHOLE component of each of its segments in shared memory
+// (32 B per vertex), so every gather is a shared-memory read.  Inside a segment the rows are sorted
+// by length and grouped into row blocks (RB) of 32 lanes, and the RBs plus the tet cells (64 tets
+// STAGED, 32 GLOBAL) are dealt to the CTA's warps so that every warp has the same cost.
 //
-// Stream format v2 (per warp, segments back to back): a sequence of fixed-size CELLS, three cells per
-// TMA chunk, so that no block ever straddles a chunk or the ring end.
+// Stream format v2 (per warp, segments back to back): a sequence of fixed-size CELLS, pulled through
+// the warp's ring kCellsPerChunk cells per TMA copy; a cell is the unit, so no block depends on where
+// a chunk or the ring ends.
 //   STAGED (component-local vertex ids, stored as 16-bit BYTE OFFSETS from the start of the CTA's staging
 //           area -- the plan knows which half-buffer a segment will use, so the kernel's gather address is
 //           just smem_base + offset; row entries point at u, tet entries at x -- hence <= 1023 vertices
 //           per double-buffered component and <= 2047 per "whole" component), cell = 768 B:
 //     quad cell : u16 idx[32][4] | f32 w[32][4]     4 operator entries per lane
-//     tet cell  : u16 idx[32][2][4] | f32 inv_det[32][2]   2 tets per lane (padding: idx 0, inv_det 0)
+//     tet cell  : u16 idx[32][2][4] | f32 inv_det[32][2]   2 tets per lane (padding: 4 x vertex 0, inv_det 0)
 //   GLOBAL (mesh-global 32-bit vertex ids), cell = 1024 B:
 //     quad cell : u32 idx[32][4] | f32 w[32][4]
 //     tet cell  : u32 idx[32][4] | f32 inv_det[32] | pad   1 tet per lane
@@ -33,9 +35,10 @@
 // idx = the lane's own row (so the gather returns u_i and the entry contributes exactly 0), and the
 // weight's BIT PATTERN holds global row id (24 bits, 0xFFFFFF = idle lane) | len4 << 24 | log2(L) << 30
 // (finite as a float because len4 <= 62, and it multiplies an exact 0).
-// L = lanes per row (1, 2 or 4; the lanes of a row are adjacent and split its entries round-robin): the
-// planner raises L when a segment has fewer row blocks than the CTA has warps, which shortens the
-// per-warp serial chain at small problem sizes.  Padding slots: idx = own row, w = 0.
+// L = lanes per row (1, 2 or 4; the lanes of a row are adjacent and split its entries round-robin), chosen
+// per block: when a segment's cells fit 90% of its CTA's rings (the latency regime of small problems) long
+// rows are split until a block is at most half a ring, which shortens the per-warp serial chain; otherwise
+// L = 1 unless a row needs more than 62 quad cells.  Padding slots: idx = a wildcard vertex, w = 0.
 #pragma once
 #include <cstdint>
 #include <functional>
@@ -51,6 +54,7 @@ constexpr int kCellStaged = 768, kCellGlobal = 1024;   // bytes per stream cell
 constexpr int kMaxHalfVerts = 1023;                    // 64 * vh <= 65535 (16-bit byte offsets into the staging area)
 constexpr int kMaxStagedVerts = 2047;                  // 32 * nv <= 65535
 constexpr int kMaxWarps = 16;
+constexpr int kCellsPerChunk = 6;                      // cells per TMA bulk copy = per ring slot (tsb_options_t.ring_slots)
 
 // One segment (32 bytes).  comp indexes the per-component "rows done" counters; vbase >= 0 when the
 // component's vertices are contiguous in the caller's numbering (then global id = vbase + local id),
@@ -70,20 +74,16 @@ static_assert(sizeof(SegHdr) == 32, "SegHdr must be 32 bytes");
 struct PlanConfig {
   int32_t nw = 16;              // warps per CTA
   int32_t grid = 132;           // persistent CTAs (used when grid_cb is empty; H100 SXM: 132 SMs)
-  // Called once the component sizes are known: (half capacity, staging-area vertices, global mode in/out)
-  // -> grid.  Lets the caller size shared memory and query occupancy before the work is cut.
-  std::function<int(int, int, bool &)> grid_cb;
+  // Called once the component sizes are known, with the staging area the plan needs (vertices) and the mode
+  // (true = GLOBAL; the callback may switch to it).  Sets grid and returns TSB_OK, or returns a TSB_E_* code
+  // with a message in err.  Lets the caller size shared memory and query occupancy before the work is cut.
+  std::function<int(int area_verts, bool &global_mode, int &grid, std::string &err)> grid_cb;
   int32_t vh_cap = kMaxHalfVerts;   // max vertices of a double-buffered ("half") component
   int32_t area_cap = kMaxStagedVerts;   // max vertices of any staged component (whole staging area)
   int32_t laplacian_scale = 0;
   int32_t force_global = 0;     // 1: skip staging, gather from global memory (testing / huge components)
   float tet_cost = 3.0f;        // cost of one tet relative to one operator entry (CTA-level cut)
-  float tetcell_cost = 1.3f;    // cost of one tet cell relative to one quad cell (warp-level deal)
-  int32_t max_lanes_per_row = 4;   // rows may be split over up to this many adjacent lanes (latency regime only)
-  int32_t ring_cells = 12;         // cells one warp's TMA ring holds (decides the latency / streaming regime)
-  float seg_overhead = 0.60f;      // fixed cost of every (CTA, component) segment, as a fraction of the mean CTA cost
-  int32_t rb_cap_div = 2;          // latency regime: a row block is at most ring_cells / rb_cap_div cells
-  int32_t threads = 0;          // host threads for the build (0 = hardware concurrency, capped)
+  int32_t ring_cells = 2 * kCellsPerChunk;   // cells one warp's TMA ring holds (decides the latency / streaming regime)
   int32_t enable_amips = 0;     // also emit the per-tet rest inverses (AMIPS term; 48 B per tet)
 };
 
