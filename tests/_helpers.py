@@ -65,9 +65,68 @@ class COracle:
         return float(c1) * terms[0] + float(c2) * terms[1] + float(c3) * terms[2], terms, g
 
 
+def rigid_motion(x, shift=0.0, angle=0.0, pivot_dist=5.0):
+    """x (float32 [n,3]) moved rigidly in fp64, rounded once: rotated by `angle` rad about an oblique axis through a
+    pivot `pivot_dist` away from the centroid, then translated by `shift` along an oblique direction."""
+    x = np.asarray(x, dtype=np.float64).reshape(-1, 3)
+    axis = np.array([0.3, -0.5, 0.81])
+    axis /= np.linalg.norm(axis)
+    K = np.array([[0, -axis[2], axis[1]], [axis[2], 0, -axis[0]], [-axis[1], axis[0], 0]])
+    R = np.eye(3) + np.sin(angle) * K + (1 - np.cos(angle)) * K @ K
+    pivot = x.mean(axis=0) + pivot_dist * np.array([0.6, 0.8, 0.0])
+    d = np.array([1.0, -0.6, 0.3]) / np.linalg.norm([1.0, -0.6, 0.3])
+    return ((x - pivot) @ R.T + pivot + shift * d).astype(np.float32)
+
+
+# The moved inputs of the displacement-precision tests: (name, shift, rotation angle about a pivot 5 units away)
+RIGID_MOTIONS = [("rest_pose", 0.0, 0.0), ("shift1", 1.0, 0.0), ("shift10", 10.0, 0.0), ("rot1_far_pivot", 0.0, 1.0)]
+
+
+def min_abs_J(rest, tets, x):
+    """Smallest |det F| over the tets at x (fp64 on the fp32 inputs)."""
+    from tssplat_b200.mesh import _signed_volumes
+    t = np.asarray(tets).astype(np.int64).reshape(-1, 4)
+    X = np.asarray(rest, dtype=np.float32).reshape(-1, 3).astype(np.float64)
+    x = np.asarray(x, dtype=np.float32).reshape(-1, 3).astype(np.float64)
+    return float(np.abs(_signed_volumes(x, t) / _signed_volumes(X, t)).min())
+
+
+def mirror_components(x, tets, every=2):
+    """x with every `every`-th connected component mirrored through its centroid's z plane: all its tets inverted
+    (J near -1) while the others keep J > 0, with |J| far from 0 (no fp32 sign flips, a well-conditioned J^(-2/3))."""
+    from tssplat_b200.mesh import connected_components
+    x = np.array(x, dtype=np.float32).reshape(-1, 3)
+    lab = connected_components(len(x), np.asarray(tets).reshape(-1, 4))
+    used = np.unique(np.asarray(tets).reshape(-1))
+    for k, c in enumerate(np.unique(lab[used])):
+        if k % every == 0:
+            m = lab == c
+            zc = x[m, 2].mean()
+            x[m, 2] = 2 * zc - x[m, 2]
+    return x
+
+
+def pole_mesh(m):
+    """One centre vertex (id 0, at the origin) with a tet to every face of the convex hull of m Fibonacci points on
+    the unit sphere: the centre's operator row has m entries (the longest row the stream format must carry)."""
+    from scipy.spatial import ConvexHull
+    k = np.arange(m) + 0.5
+    phi = np.arccos(1 - 2 * k / m)
+    th = np.pi * (1 + 5 ** 0.5) * k
+    P = np.stack([np.cos(th) * np.sin(phi), np.sin(th) * np.sin(phi), np.cos(phi)], axis=1)
+    f = ConvexHull(P).simplices.astype(np.int64)
+    vol = np.einsum("ij,ij->i", P[f[:, 0]], np.cross(P[f[:, 1]], P[f[:, 2]]))
+    f[vol < 0] = f[vol < 0][:, [0, 2, 1]]
+    verts = np.concatenate([np.zeros((1, 3)), P])
+    tets = np.concatenate([np.zeros((len(f), 1), np.int64), f + 1], axis=1)
+    return verts, tets.astype(np.int32)
+
+
 PLAN_DEBUG_SO = os.path.join(ROOT, "tests", "native", "libtsb_plan_debug.so")
+CELLS_PER_CHUNK = 6      # tsb_plan.h kCellsPerChunk: cells per ring slot
 _ARRAYS = {"stream": np.uint8, "X4": np.float32, "vlist": np.int32, "segs": np.int32, "cta_seg": np.int32,
-           "wdesc": np.uint32, "wseg": np.uint16, "orphans": np.int32, "pos16": np.uint16, "pos_gid": np.int32}
+           "wdesc": np.uint32, "wseg": np.uint16, "orphans": np.int32, "pos16": np.uint16, "pos_gid": np.int32,
+           "Bt": np.float32, "wtc0": np.int32}
 _SCALARS = ("n", "nele", "n_components", "n_boundary_faces", "laplacian_scale", "mode_global", "nw", "grid", "vh",
             "area_verts", "max_comp_verts", "contiguous", "nnz", "nnz_padded", "n_rb", "n_tetcells",
             "gather_wf", "gather_wf_ideal", "tet_wf", "tet_wf_ideal")
@@ -75,13 +134,15 @@ _SEG = ("comp", "vbase", "nv", "x4off", "expected", "whole", "npos", "p4off")
 
 
 def build_host_plan(rest, tets, nw=16, grid=132, laplacian_scale=0, force_global=0, vh_cap=0, area_cap=0,
-                    tet_cost=0.0):
+                    tet_cost=0.0, ring_slots=0, enable_amips=0):
     """Run the product's host plan builder (tssplat_b200/csrc/tsb_plan.cpp, no CUDA) through the
-    test-only inspection library and copy its arrays out as numpy."""
+    test-only inspection library and copy its arrays out as numpy.  ring_slots: the ring a handle
+    requests (row splitting depends on it); 0 = the default."""
     lib = C.CDLL(PLAN_DEBUG_SO)
-    lib.tsbdbg_build.restype = C.c_int
-    lib.tsbdbg_build.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                 C.c_int32, C.c_int32, C.c_int32, C.c_float, C.POINTER(C.c_void_p)]
+    lib.tsbdbg_build_ex.restype = C.c_int
+    lib.tsbdbg_build_ex.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                    C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_int32,
+                                    C.POINTER(C.c_void_p)]
     lib.tsbdbg_array.restype = C.c_int
     lib.tsbdbg_array.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64),
                                  C.POINTER(C.c_int32)]
@@ -91,9 +152,9 @@ def build_host_plan(rest, tets, nw=16, grid=132, laplacian_scale=0, force_global
     rest = np.ascontiguousarray(np.asarray(rest, dtype=np.float32).reshape(-1))
     tets = np.ascontiguousarray(np.asarray(tets, dtype=np.int32).reshape(-1))
     d = C.c_void_p()
-    rc = lib.tsbdbg_build(rest.ctypes.data, tets.ctypes.data, rest.size // 3, tets.size // 4, int(nw), int(grid),
-                          int(laplacian_scale), int(force_global), int(vh_cap), int(area_cap), float(tet_cost),
-                          C.byref(d))
+    rc = lib.tsbdbg_build_ex(rest.ctypes.data, tets.ctypes.data, rest.size // 3, tets.size // 4, int(nw), int(grid),
+                             int(laplacian_scale), int(force_global), int(vh_cap), int(area_cap), float(tet_cost),
+                             int(ring_slots) * CELLS_PER_CHUNK, int(enable_amips), C.byref(d))
     if rc != 0:
         raise RuntimeError(lib.tsbdbg_last_error().decode())
     try:
@@ -114,10 +175,25 @@ def build_host_plan(rest, tets, nw=16, grid=132, laplacian_scale=0, force_global
     return plan
 
 
-def emulate_kernel(plan, x, c1, c2, order, gradH=1.0, dtype=np.float64):
+def _rel_u(x, X, xr, Xr):
+    """The kernel's staged displacement (rel_u in tsb_kernels.cu, the same fp32 operations): (x - X) - c with x - X
+    kept exactly as a TwoSum pair, c = fp32(x_r - X_r) of the component's reference vertex r."""
+    f = lambda a: np.asarray(a, dtype=np.float32)
+    x, X = np.broadcast_arrays(f(x), f(X))
+    c = f(xr) - f(Xr)
+    s = x - X
+    bb = s - x
+    e = (x - (s - bb)) + (-X - bb)
+    return (s - c) + e
+
+
+def emulate_kernel(plan, x, c1, c2, order, gradH=1.0, dtype=np.float64, c3=None):
     """numpy re-enactment of energy_grad_kernel (tsb_kernels.cu) on the host plan: every CTA, every
     warp walks its cell stream exactly as the kernel does (row blocks, then tet cells, segment by
-    segment), with the same formulas.  Returns (energy_total, smooth, barrier, grad[n,3])."""
+    segment), with the same formulas.  Returns (energy_total, smooth, barrier, grad[n,3]); with c3
+    (the AMIPS coefficient; the plan must be built with enable_amips) it also evaluates the AMIPS term of
+    every J > 0 tet from the plan's per-cell rest inverses (Bt, wtc0) and returns
+    (energy_total, smooth, barrier, amips, grad[n,3])."""
     G, NW, glob = plan["grid"], plan["nw"], bool(plan["mode_global"])
     IB = 4 if glob else 2
     idt = np.uint32 if glob else np.uint16
@@ -129,7 +205,11 @@ def emulate_kernel(plan, x, c1, c2, order, gradH=1.0, dtype=np.float64):
     grad = np.full((n, 3), np.nan, dtype=dtype)
     grad[plan["orphans"]] = 0.0
     bar_add = np.zeros((n, 3), dtype=dtype)
-    es = eb = 0.0
+    es = eb = ea = 0.0
+    if c3 is not None:
+        Bt = plan["Bt"].reshape(-1, 3, 32 * TPL, 4)                  # [tet cell][row of Dm^-1][lane * TPL + slot]
+        wtc0 = plan["wtc0"].reshape(-1, NW)
+        assert len(Bt) == plan["n_tetcells"], "AMIPS: one rest-inverse block per tet cell"
     X4 = plan["X4"].reshape(-1, 4)
     wdesc = plan["wdesc"].reshape(G, NW, 2)
     wseg = plan["wseg"].reshape(-1, NW, 2)
@@ -146,7 +226,8 @@ def emulate_kernel(plan, x, c1, c2, order, gradH=1.0, dtype=np.float64):
             nv = h["nv"]
             if glob:
                 gids = np.arange(n)
-                U = (x - X4[:, :3]).astype(dtype)                       # float32 subtraction, like the kernel
+                ref = X4.view(np.int32)[:, 3]                          # each vertex's reference vertex (bits in .w)
+                U = _rel_u(x, X4[:, :3], x[ref], X4[ref, :3]).astype(dtype)
                 Pp = x.astype(dtype)
                 to_local = lambda a, base=None: a.astype(np.int64)
             else:
@@ -158,7 +239,8 @@ def emulate_kernel(plan, x, c1, c2, order, gradH=1.0, dtype=np.float64):
                 assert np.array_equal(gids[spos], vg)
                 U = np.full((npos, 3), np.nan, dtype=dtype)                                 # unused positions hold garbage
                 Pp = np.full((npos, 3), np.nan, dtype=dtype)
-                U[spos] = (x[vg] - X4[h["x4off"]:h["x4off"] + nv, :3]).astype(dtype)
+                Xc = X4[h["x4off"]:h["x4off"] + nv, :3]
+                U[spos] = _rel_u(x[vg], Xc, x[vg[0]], Xc[0]).astype(dtype)
                 Pp[spos] = x[vg].astype(dtype)
                 assert npos <= 2047 and npos <= plan["area_verts"] and (h["whole"] or npos <= plan["vh"])
                 nv = npos
@@ -213,7 +295,7 @@ def emulate_kernel(plan, x, c1, c2, order, gradH=1.0, dtype=np.float64):
                     es += 0.5 * np.einsum("lr,lr->", ui[lead] - uref, tot[lead[::L]])
                     rows_seen += int(lead.sum())
                 assert ntc == 0 or w < NW - 1 or NW == 1, "the signalling warp must own no tets"
-                for _ in range(ntc):
+                for tc in range(ntc):
                     idx = st[p:p + 128 * IB * TPL].view(idt).reshape(32 * TPL, 4)
                     idx = to_local(idx) if glob else to_local(idx, xb)
                     idet = st[p + 128 * IB * TPL:p + 128 * IB * TPL + 128 * TPL].view(np.float32).astype(dtype)
@@ -230,10 +312,27 @@ def emulate_kernel(plan, x, c1, c2, order, gradH=1.0, dtype=np.float64):
                     g1, g2, g3 = k * c23, k * np.cross(e3, e1), k * np.cross(e1, e2)
                     for g, col in ((-(g1 + g2 + g3), 0), (g1, 1), (g2, 2), (g3, 3)):
                         np.add.at(bar_add, gids[idx[inv, col]], g[inv])
+                    if c3 is not None:
+                        # psi = tr(F^T F) / (3 J^(2/3)) - 1,  F = Ds B,  dpsi/dF = 2 / (3 J^(2/3)) (F - tr / (3 J) cof F)
+                        ok = J > 0
+                        B = Bt[int(wtc0[s, w]) + tc][:, ok, :3].transpose(1, 0, 2).astype(dtype)   # [tet][k][c]
+                        F = np.stack([e1[ok], e2[ok], e3[ok]], axis=2) @ B                       # Ds[:, k] = e_{k+1}
+                        Jp = J[ok]
+                        tr = (F * F).sum(axis=(1, 2))
+                        j23 = np.cbrt(Jp) ** 2
+                        ea += (tr / (3 * j23) - 1).sum()
+                        cof = np.linalg.det(F)[:, None, None] * np.linalg.inv(F).transpose(0, 2, 1)
+                        P = (2 / (3 * j23) * c3 * gradH)[:, None, None] * (F - (tr / (3 * Jp))[:, None, None] * cof)
+                        gk = P @ B.transpose(0, 2, 1)                                             # [tet][r][k]: vertex k+1
+                        for k in range(3):
+                            np.add.at(bar_add, gids[idx[ok, k + 1]], gk[:, :, k])
+                        np.add.at(bar_add, gids[idx[ok, 0]], -gk.sum(axis=2))
                 pos[w] = p
             rows_done[h["comp"]] += 1
         assert pos == end, "a warp did not consume exactly its stream"
     for sg in plan["segs"]:
         assert rows_done[sg["comp"]] == sg["expected"], "rows-done counter would never reach `expected`"
     assert rows_seen == n - len(plan["orphans"]) and not np.isnan(grad).any()
+    if c3 is not None:
+        return c1 * es + c2 * eb + c3 * ea, es, eb, ea, grad + bar_add
     return c1 * es + c2 * eb, es, eb, grad + bar_add

@@ -11,7 +11,8 @@ import numpy as np
 import pytest
 import torch
 
-from _helpers import GOLDEN, COracle
+from _helpers import (GOLDEN, RIGID_MOTIONS, COracle, build_host_plan, min_abs_J, mirror_components, pole_mesh,
+                      rigid_motion)
 from tssplat_b200.mesh import concat_spheres, make_pack, make_tet_sphere, perturb
 
 pytestmark = pytest.mark.gpu
@@ -28,6 +29,8 @@ def ext():
 def _check(ext, verts, tets, x_np, c1, c2, order, gradH=1.0, scale=0, rel=REL, **kw):
     sp = ext.TetSpheres(np.ascontiguousarray(verts, dtype=np.float32).reshape(-1),
                         np.ascontiguousarray(tets, dtype=np.int32).reshape(-1), laplacian_scale=scale, **kw)
+    if kw.get("ring_slots"):
+        assert sp.info["ring_slots"] == kw["ring_slots"], "the ring was shrunk: this variant would not test its depth"
     x = torch.from_numpy(np.asarray(x_np, dtype=np.float32)).cuda()
     e, g = sp.energy_grad(x, c1, c2, order, gradH)
     torch.cuda.synchronize()
@@ -42,8 +45,42 @@ def _check(ext, verts, tets, x_np, c1, c2, order, gradH=1.0, scale=0, rel=REL, *
     return sp, e, g
 
 
+# Rings deeper than 2 slots only keep their depth where shared memory holds them (tsb_create shrinks them otherwise):
+# 8 warps, 3-4 slots, staged or global; _check asserts the depth.
 VARIANTS = [dict(), dict(warps_per_cta=8), dict(force_global=True), dict(warps_per_cta=8, force_global=True),
-            dict(ring_slots=4)]
+            dict(warps_per_cta=8, ring_slots=3), dict(warps_per_cta=8, ring_slots=4),
+            dict(warps_per_cta=8, force_global=True, ring_slots=3), dict(warps_per_cta=8, force_global=True, ring_slots=4)]
+
+
+def _cpu_plan(sp, verts, tets, ring_slots=0, force_global=False, enable_amips=False):
+    """The host plan of handle sp, rebuilt on the CPU with the handle's warps and grid (and the ring it requested: row
+    splitting depends on it); it must agree with the handle, so what it shows is what the kernel ran."""
+    I = sp.info
+    plan = build_host_plan(verts, tets, nw=I["warps_per_cta"], grid=I["grid"], force_global=int(force_global),
+                           ring_slots=ring_slots, enable_amips=int(enable_amips))
+    assert plan["mode_global"] == I["mode_global"] and len(plan["segs"]) == I["n_segments"]
+    assert plan["nnz_padded"] == I["nnz_padded"]
+    return plan
+
+
+def _segment_patterns(plan):
+    """The set of per-CTA segment sequences, each segment 'whole' (whole staging area) or 'half' (double-buffered)."""
+    cs = plan["cta_seg"].reshape(-1, 2)
+    return {tuple("whole" if plan["segs"][s]["whole"] else "half" for s in range(a, b)) for a, b in cs if b > a}
+
+
+def _check_amips(sp, verts, tets, x_np, order, c=(2e-4, 3e-4, 1e-4), gradH=0.8, rel=2e-5):
+    """The AMIPS term (J > 0 tets, beside the barrier of J < 0 tets) against the fp64 oracle.  Inputs keep |J| clear of
+    0, where the sign of J and J^(-2/3) are ill-conditioned in fp32.  Returns the oracle's terms."""
+    assert min_abs_J(verts, tets, x_np) > 0.05
+    e, g = sp.energy_grad(torch.from_numpy(np.ascontiguousarray(x_np, dtype=np.float32)).cuda(), c[0], c[1], order, gradH,
+                          c3=c[2])
+    eo, terms, go = COracle(verts, tets).energy_grad_ex(x_np, *c, order, gradH=gradH)
+    e, g = e.cpu().numpy().astype(np.float64), g.cpu().numpy().astype(np.float64)
+    assert e[3] == pytest.approx(terms[2], rel=rel) and e[0] == pytest.approx(eo, rel=rel)
+    assert e[2] == pytest.approx(terms[1], rel=rel, abs=1e-30)
+    assert np.linalg.norm(g - go) <= rel * np.linalg.norm(go), np.linalg.norm(g - go) / np.linalg.norm(go)
+    return terms
 
 
 @pytest.mark.parametrize("kw", VARIANTS, ids=lambda k: "-".join(f"{a}{b}" for a, b in k.items()) or "default")
@@ -52,6 +89,127 @@ def test_parity_small_pack(ext, kw, sig, order):
     """Every kernel variant (16 / 8 warps per CTA, components staged in shared memory / global gathers)."""
     pack = make_pack(3, 1024, seed=1)
     _check(ext, pack.verts, pack.tets, perturb(pack, sigma_rel=sig, seed=1), 2e-4 / 3, 2e-4, order, gradH=0.7, **kw)
+
+
+@pytest.mark.parametrize("kw", [dict(), dict(warps_per_cta=8), dict(force_global=True)],
+                         ids=lambda k: "-".join(f"{a}{b}" for a, b in k.items()) or "default")
+def test_displacement_precision_far_from_rest(ext, kw):
+    """Spheres moved rigidly far from their rest pose (translations of 1 and 10, a 1 rad rotation about a pivot 5
+    units away) keep the kernel within 1e-5 of the oracle: the staged displacement is centred per component, so the
+    rigid part never enters a rounded fp32 difference (uncentred, the gradient error reaches 2.7e-4)."""
+    pack = make_pack(3, 1024, seed=1)
+    sp = ext.TetSpheres(pack.verts.reshape(-1), pack.tets.reshape(-1), **kw)
+    orc = COracle(pack.verts, pack.tets)
+    for sig in (0.02, 0.35):
+        x0 = perturb(pack, sigma_rel=sig, seed=1)
+        for name, shift, angle in RIGID_MOTIONS:
+            x_np = rigid_motion(x0, shift, angle)
+            e, g = sp.energy_grad(torch.from_numpy(x_np).cuda(), 2e-4 / 3, 2e-4, 2, 0.7)
+            eo, terms, go = orc.energy_grad(x_np, 2e-4 / 3, 2e-4, 2, gradH=0.7)
+            e, g = e.cpu().numpy().astype(np.float64), g.cpu().numpy().astype(np.float64)
+            assert e[0] == pytest.approx(eo, rel=REL) and e[1] == pytest.approx(terms[0], rel=REL), (sig, name)
+            assert np.linalg.norm(g - go) <= REL * np.linalg.norm(go), (sig, name, np.linalg.norm(g - go) / np.linalg.norm(go))
+    e, g = sp.energy_grad(torch.from_numpy(pack.verts).cuda(), 1.0, 1.0, 2)          # rest pose: exactly 0
+    assert float(e[0]) == 0.0 and float(g.abs().max()) == 0.0
+
+
+def _whole_area_meshes():
+    """Components staged in the whole staging area (1024..2047 positions): one alone; two mixed with 600 double-buffered
+    twelve-tet spheres so that CTAs hold both kinds of segment; one of 2041 vertices that bank colouring pads past
+    2047 staging positions, which sends the mesh to the global-gather mode."""
+    tiny = make_pack(600, 12, seed=3, unique=6)
+    a, b = tiny.slice_spheres(0, 300), tiny.slice_spheres(300, 600)
+    mixed = concat_spheres([(a.verts, a.tets), make_tet_sphere(1500, 7000), (b.verts, b.tets), make_tet_sphere(1501, 7700)])
+    alone, near_cap = make_tet_sphere(1502, 7000), make_tet_sphere(1510, 10000)
+    return {"alone": (alone[0].astype(np.float32), alone[1]), "mixed": (mixed.verts, mixed.tets),
+            "near_cap": (near_cap[0].astype(np.float32), near_cap[1])}
+
+
+@pytest.mark.parametrize("nw", [16, 8])
+def test_whole_area_staging(ext, nw):
+    """Whole-area staging (its own staging pass, u / x bases, hand-overs and gradient-id base) against the oracle, at
+    orders 2 and 4, benign and inverted, with and without AMIPS.  The handle's plan, rebuilt on the CPU, proves the
+    path: whole segments, CTAs that mix whole and double-buffered segments, and the padded near-cap mesh in GLOBAL."""
+    for name, (v, t) in _whole_area_meshes().items():
+        sp = ext.TetSpheres(v.reshape(-1), t.reshape(-1), warps_per_cta=nw, enable_amips=True)
+        plan = _cpu_plan(sp, v, t, enable_amips=True)
+        pats = _segment_patterns(plan)
+        if name == "near_cap":
+            assert sp.info["max_component_vertices"] <= 2047 and sp.info["mode_global"] == 1
+        else:
+            assert sp.info["mode_global"] == 0 and any("whole" in p for p in pats), pats
+        if name == "mixed":
+            assert any("whole" in p and "half" in p for p in pats), pats
+        orc = COracle(v, t)
+        for sig, order in ((0.02, 2), (0.35, 2), (0.35, 4)):
+            x_np = perturb(v, t, sig, 4)
+            e, g = sp.energy_grad(torch.from_numpy(x_np).cuda(), 2e-4, 3e-4, order, 0.9)
+            eo, terms, go = orc.energy_grad(x_np, 2e-4, 3e-4, order, gradH=0.9)
+            e, g = e.cpu().numpy().astype(np.float64), g.cpu().numpy().astype(np.float64)
+            assert (terms[1] > 0) == (sig > 0.1), (name, sig)
+            assert e[0] == pytest.approx(eo, rel=REL) and e[2] == pytest.approx(terms[1], rel=REL, abs=1e-30), (name, sig, order)
+            assert np.linalg.norm(g - go) <= REL * np.linalg.norm(go), (name, sig, order)
+        x_np = perturb(v, t, 0.05, 4)
+        if name == "mixed":          # inverted (mirrored) components next to AMIPS ones
+            x_np = mirror_components(x_np, t)
+        for order in (2, 4):
+            _check_amips(sp, v, t, x_np, order)
+
+
+@pytest.mark.parametrize("kw", [dict(), dict(warps_per_cta=8), dict(force_global=True), dict(warps_per_cta=8, ring_slots=4),
+                                dict(warps_per_cta=8, force_global=True, ring_slots=4)],
+                         ids=lambda k: "-".join(f"{a}{b}" for a, b in k.items()) or "default")
+def test_high_valence_row(ext, kw):
+    """A 'pole' vertex with 988 operator neighbours: one 4-lane row block of 62 quad cells, which wraps the warp's
+    ring several times inside the block (with 4-slot rings too)."""
+    v, t = pole_mesh(988)
+    v = v.astype(np.float32)
+    x_np = perturb(v, t, 0.3, 2)
+    sp, e, g = _check(ext, v, t, x_np, 1e-3, 2e-3, 2, gradH=0.6, **kw)
+    plan = _cpu_plan(sp, v, t, ring_slots=kw.get("ring_slots", 0), force_global=kw.get("force_global", False))
+    from test_host_logic import _block_headers
+    assert (62, 4) in _block_headers(plan)
+    assert e[2] > 0
+    _check(ext, v, t, perturb(v, t, 0.05, 2), 1e-3, 2e-3, 4, **kw)
+
+
+def test_level1_helpers_at_scale(ext):
+    """tsb_scale, tsb_grad_limit and tsb_adam_uniform_step past their grid cap (132 x 8 CTAs of 256 threads: the
+    grid-stride loops only run beyond 270 k elements) at the 1024-sphere gradient size, and at odd counts."""
+    from tssplat_b200 import _capi
+    st = torch.cuda.current_stream().cuda_stream
+    torch.manual_seed(5)
+    for count in (2_600_003, 1, 257):
+        g = torch.randn(count, device="cuda") * 0.01
+        g[count // 2] = 0.7                                                     # the maximum sits deep in the array
+        out = torch.empty_like(g)
+        gh = torch.tensor([1.5], device="cuda")
+        assert _capi.lib.tsb_scale(g.data_ptr(), count, 0.5, gh.data_ptr(), out.data_ptr(), st) == 0
+        torch.cuda.synchronize()
+        assert torch.equal(out, (0.5 * 1.5) * g)
+        ref = g.clone()
+        ext.grad_limit(g, 0.001, 0.05)
+        assert float(g.abs().max()) == pytest.approx(0.05, rel=1e-6)
+        assert torch.allclose(g, ref * (0.05 / ref.abs().max()), rtol=1e-6)
+        p = torch.randn(count, device="cuda")
+        p_ref, g1r, g2r = p.clone(), torch.zeros_like(p), torch.zeros_like(p)
+        g1, g2, work = torch.zeros_like(p), torch.zeros_like(p), torch.zeros(4, device="cuda")
+        lr, b1, b2, limit = 0.2, 0.9, 0.999, 0.01
+        for step in range(1, 4):
+            grad = torch.randn(count, device="cuda") * (0.1 if step != 2 else 10.0)
+            grad[(count * step) // 4] = 30.0
+            g1r.mul_(b1).add_(grad, alpha=1 - b1)
+            g2r.mul_(b2).add_(grad.square(), alpha=1 - b2)
+            gr = (g1r / (1 - b1 ** step)) / (1e-8 + (g2r / (1 - b2 ** step)).sqrt().max())
+            s = gr.abs().max()
+            if s > limit:
+                gr = gr * (limit / s)
+            p_ref.sub_(gr, alpha=lr)
+            assert _capi.lib.tsb_adam_uniform_step(p.data_ptr(), grad.data_ptr(), g1.data_ptr(), g2.data_ptr(), count,
+                                                   lr, b1, b2, step, limit, work.data_ptr(), st) == 0
+        torch.cuda.synchronize()
+        assert torch.allclose(p, p_ref, rtol=1e-5, atol=1e-7) and torch.allclose(g1, g1r, rtol=1e-5, atol=1e-6)
+        assert torch.allclose(g2, g2r, rtol=1e-5, atol=1e-8) and torch.all(work == 0)
 
 
 def test_parity_coefficient_range_and_scale(ext):
@@ -268,10 +426,9 @@ def test_full_size_properties_64_spheres(ext):
     if np.linalg.det(q) < 0:
         q[:, 0] = -q[:, 0]
     xr = (x_np.astype(np.float64) @ q.T + np.array([0.3, -0.2, 0.1])).astype(np.float32)
-    e2, g2 = sp.energy_grad(torch.from_numpy(xr).cuda(), c1, c2, 2)
-    assert float(e2[0]) == pytest.approx(e[0], rel=2e-5)
-    g2 = g2.cpu().numpy().astype(np.float64)
-    assert np.linalg.norm(g2 - g @ q.T) <= 5e-5 * np.linalg.norm(g)
+    _, e2, g2 = _check(ext, pack.verts, pack.tets, xr, c1, c2, 2)                   # the moved input against the oracle
+    assert e2[0] == pytest.approx(e[0], rel=REL)
+    assert np.linalg.norm(g2 - g @ q.T) <= REL * np.linalg.norm(g)
     # block-diagonality: spheres 10..13 as their own handle give the same gradient slice
     sub = pack.slice_spheres(10, 14)
     v0, v1 = int(pack.vert_offsets[10]), int(pack.vert_offsets[14])
@@ -455,26 +612,31 @@ def test_amips_term_default_off(ext):
     fp64 restatements (oracle/tet_energy_oracle.{py,c}), the known answers and "c3 = 0 changes nothing"."""
     pack = make_pack(3, 1024, seed=8)
     v, t = pack.verts, pack.tets
-    sp = ext.TetSpheres(v.reshape(-1), t.reshape(-1), enable_amips=True)
-    plain = ext.TetSpheres(v.reshape(-1), t.reshape(-1))
     orc = COracle(v, t)
-    for sig, order in ((0.05, 2), (0.2, 4)):
-        x_np = perturb(pack, sigma_rel=sig, seed=4)
-        x = torch.from_numpy(x_np).cuda()
-        e, g = sp.energy_grad(x, 2e-4, 3e-4, order, 0.8, c3=1e-4)
-        eo, terms, go = orc.energy_grad_ex(x_np, 2e-4, 3e-4, 1e-4, order, gradH=0.8)
-        e, g = e.cpu().numpy().astype(np.float64), g.cpu().numpy().astype(np.float64)
-        assert e[3] == pytest.approx(terms[2], rel=2e-5) and e[0] == pytest.approx(eo, rel=2e-5)
-        assert np.linalg.norm(g - go) <= 2e-5 * np.linalg.norm(go)
-        # c3 = 0 on the AMIPS-enabled handle == the plain handle, bit for bit (no inverted tets at sigma 0.05)
-        e0, g0 = sp.energy_grad(x, 2e-4, 3e-4, order, 0.8)
-        e1, g1 = plain.energy_grad(x, 2e-4, 3e-4, order, 0.8)
-        assert torch.equal(e0, e1) and (sig > 0.1 or torch.equal(g0, g1))
+    for kw in ({}, {"warps_per_cta": 8}, {"force_global": True}):       # STAGED (2 tets per lane) and GLOBAL (1)
+        sp = ext.TetSpheres(v.reshape(-1), t.reshape(-1), enable_amips=True, **kw)
+        plain = ext.TetSpheres(v.reshape(-1), t.reshape(-1), **kw)
+        for sig, order in ((0.05, 2), (0.2, 4)):
+            x_np = perturb(pack, sigma_rel=sig, seed=4)
+            x = torch.from_numpy(x_np).cuda()
+            e, g = sp.energy_grad(x, 2e-4, 3e-4, order, 0.8, c3=1e-4)
+            eo, terms, go = orc.energy_grad_ex(x_np, 2e-4, 3e-4, 1e-4, order, gradH=0.8)
+            e, g = e.cpu().numpy().astype(np.float64), g.cpu().numpy().astype(np.float64)
+            assert e[3] == pytest.approx(terms[2], rel=2e-5) and e[0] == pytest.approx(eo, rel=2e-5), kw
+            assert np.linalg.norm(g - go) <= 2e-5 * np.linalg.norm(go), kw
+            # c3 = 0 on the AMIPS-enabled handle == the plain handle, bit for bit (no inverted tets at sigma 0.05)
+            e0, g0 = sp.energy_grad(x, 2e-4, 3e-4, order, 0.8)
+            e1, g1 = plain.energy_grad(x, 2e-4, 3e-4, order, 0.8)
+            assert torch.equal(e0, e1) and (sig > 0.1 or torch.equal(g0, g1))
+        # a mirrored (fully inverted) sphere beside two AMIPS ones, in the same launch
+        terms = _check_amips(sp, v, t, mirror_components(perturb(pack, sigma_rel=0.05, seed=4), t), 2)
+        assert terms[1] > 0 and terms[2] > 0
+    sp = ext.TetSpheres(v.reshape(-1), t.reshape(-1), enable_amips=True)
     rest = torch.from_numpy(v).cuda()
     e, g = sp.energy_grad(rest, 0.0, 0.0, 2, c3=1.0)                       # rest state: minimum, zero gradient
     assert abs(float(e[3])) < 1e-3 and float(g.abs().max()) < 1e-3
     with pytest.raises(RuntimeError, match="enable_amips"):
-        plain.energy_grad(rest, 1.0, 1.0, 2, c3=0.5)
+        ext.TetSpheres(v.reshape(-1), t.reshape(-1)).energy_grad(rest, 1.0, 1.0, 2, c3=0.5)
 
 
 def test_handles_with_different_staging_sizes_coexist(ext):
@@ -588,13 +750,17 @@ def test_randomised_ragged_meshes_on_gpu(ext):
         V, T = _ragged_mesh(rng, int(rng.integers(1, 7)), 1200)
         orc = COracle(V, T)
         for kw in ({}, {"warps_per_cta": 8}, {"force_global": True}):
-            sp = ext.TetSpheres(V.reshape(-1), T.reshape(-1), **kw)
+            sp = ext.TetSpheres(V.reshape(-1), T.reshape(-1), enable_amips=True, **kw)
             for sig, order in ((0.03, 2), (0.4, 4)):
                 x_np = (V + rng.normal(0, sig * 0.2, V.shape)).astype(np.float32)
                 e, g = sp.energy_grad(torch.from_numpy(x_np).cuda(), 3e-4, 2e-4, order, 1.3)
                 eo, _, go = orc.energy_grad(x_np, 3e-4, 2e-4, order, gradH=1.3)
                 assert float(e[0]) == pytest.approx(eo, rel=REL, abs=1e-12), (seed, kw, sig)
                 assert np.linalg.norm(g.cpu().numpy() - go) <= REL * max(np.linalg.norm(go), 1e-12), (seed, kw, sig)
+            # AMIPS: every other component mirrored (inverted), all stretched so that the AMIPS sum does not cancel (per
+            # tet psi = tr / (3 J^(2/3)) - 1 is a difference of O(1) fp32 values; here psi is near 0.08)
+            x_np = V * np.array([1.3, 1.0, 0.8], dtype=np.float32) + rng.normal(0, 0.002, V.shape)
+            _check_amips(sp, V, T, mirror_components(x_np, T), 2, gradH=1.3)
 
 
 def test_thousands_of_tiny_components(ext):
@@ -603,11 +769,19 @@ def test_thousands_of_tiny_components(ext):
     pk = make_pack(2600, 12, seed=3, unique=6)
     orc = COracle(pk.verts, pk.tets)
     rng = np.random.default_rng(0)
-    for kw in ({}, {"warps_per_cta": 8}, {"force_global": True}):
-        sp = ext.TetSpheres(pk.verts.reshape(-1), pk.tets.reshape(-1), **kw)
+    x_amips = mirror_components(perturb(pk, sigma_rel=0.05, seed=4), pk.tets)
+    for kw in ({}, {"warps_per_cta": 8}, {"force_global": True}, {"ring_slots": 3}):    # 16 warps x 3 slots fits here
+        sp = ext.TetSpheres(pk.verts.reshape(-1), pk.tets.reshape(-1), enable_amips=True, **kw)
+        if "ring_slots" in kw:
+            assert sp.info["ring_slots"] == kw["ring_slots"]
+        plan = _cpu_plan(sp, pk.verts, pk.tets, ring_slots=kw.get("ring_slots", 0), force_global=kw.get("force_global", False))
+        cs = plan["cta_seg"].reshape(-1, 2)
+        if sp.info["warps_per_cta"] == 16:                      # 132 CTAs: AMIPS's tet-cell offsets past the segment table
+            assert (cs[:, 1] - cs[:, 0]).max() > 16
         for sig, order in ((0.02, 2), (0.3, 4)):
             x_np = (pk.verts + rng.normal(0, sig, pk.verts.shape)).astype(np.float32)
             e, g = sp.energy_grad(torch.from_numpy(x_np).cuda(), 2e-4, 3e-4, order)
             eo, _, go = orc.energy_grad(x_np, 2e-4, 3e-4, order)
             assert float(e[0]) == pytest.approx(eo, rel=REL), (kw, sig)
             assert np.linalg.norm(g.cpu().numpy() - go) <= REL * np.linalg.norm(go), (kw, sig)
+        _check_amips(sp, pk.verts, pk.tets, x_amips, 4)

@@ -8,7 +8,8 @@ import re
 import numpy as np
 import pytest
 
-from _helpers import GOLDEN, ROOT, COracle, build_host_plan, emulate_kernel
+from _helpers import (GOLDEN, RIGID_MOTIONS, ROOT, COracle, build_host_plan, emulate_kernel, min_abs_J, pole_mesh,
+                      rigid_motion)
 from tssplat_b200 import _capi
 from tssplat_b200.mesh import (concat_spheres, connected_components, load_veg, make_pack, make_tet_sphere, perturb,
                                save_veg)
@@ -37,9 +38,10 @@ PLAN_VARIANTS = [dict(nw=16, grid=132), dict(nw=8, grid=5), dict(nw=16, grid=7, 
 @pytest.mark.parametrize("kw", PLAN_VARIANTS, ids=lambda k: "-".join(f"{a}{b}" for a, b in k.items()))
 def test_plan_reenactment_matches_oracle(kw):
     """The product's plan builder (operator rows, bank-aware placement, segments, warp streams) walked in
-    numpy exactly as the kernel walks it, against the fp64 C oracle."""
+    numpy exactly as the kernel walks it, against the fp64 C oracle; with the AMIPS term, the per-cell rest
+    inverses (Bt, wtc0) walked the same way."""
     pack = make_pack(3, 768, seed=2)
-    plan = build_host_plan(pack.verts, pack.tets, **kw)
+    plan = build_host_plan(pack.verts, pack.tets, enable_amips=1, **kw)
     assert plan["n_components"] == 3 and plan["mode_global"] == kw.get("force_global", 0)
     orc = COracle(pack.verts, pack.tets)
     for sig, order in ((0.02, 2), (0.35, 4)):
@@ -49,6 +51,72 @@ def test_plan_reenactment_matches_oracle(kw):
         assert E == pytest.approx(Eo, rel=2e-6)          # fp32 operator entries, fp64 arithmetic
         assert es == pytest.approx(terms[0], rel=2e-6) and eb == pytest.approx(terms[1], rel=2e-6, abs=1e-300)
         assert np.linalg.norm(g - go) <= 2e-6 * np.linalg.norm(go)
+        # AMIPS (J > 0 tets) next to the barrier (J < 0 tets) in the same cells; |J| stays clear of 0, where the
+        # sign of J and J^(-2/3) are ill-conditioned
+        assert min_abs_J(pack.verts, pack.tets, x) > 1e-4
+        E, es, eb, ea, g = emulate_kernel(plan, x, 2e-4, 3e-4, order, gradH=0.7, c3=1e-4)
+        Eo, terms, go = orc.energy_grad_ex(x, 2e-4, 3e-4, 1e-4, order, gradH=0.7)
+        assert terms[2] > 0 and ea == pytest.approx(terms[2], rel=2e-6) and E == pytest.approx(Eo, rel=2e-6)
+        assert np.linalg.norm(g - go) <= 2e-6 * np.linalg.norm(go)
+
+
+@pytest.mark.parametrize("sig", [0.02, 0.35])
+@pytest.mark.parametrize("force_global", [0, 1])
+def test_displacement_precision_far_from_rest(sig, force_global):
+    """Spheres moved rigidly far from their rest pose (translations of 1 and 10, a 1 rad rotation about a pivot 5
+    units away) keep the precision of an unmoved sphere: the staged displacement is centred on a reference vertex of
+    each component, so the rigid part never enters a rounded fp32 difference.  Without the centring the gradient
+    error reaches 2.7e-4 at a translation of 10."""
+    pack = make_pack(3, 1024, seed=1)
+    plan = build_host_plan(pack.verts, pack.tets, force_global=force_global)
+    orc = COracle(pack.verts, pack.tets)
+    x0 = perturb(pack, sigma_rel=sig, seed=1)
+    for name, shift, angle in RIGID_MOTIONS:
+        x = rigid_motion(x0, shift, angle)
+        E, es, eb, g = emulate_kernel(plan, x, 2e-4 / 3, 2e-4, 2, gradH=0.7)
+        Eo, terms, go = orc.energy_grad(x, 2e-4 / 3, 2e-4, 2, gradH=0.7)
+        assert E == pytest.approx(Eo, rel=5e-6), name
+        assert np.linalg.norm(g - go) <= 5e-6 * np.linalg.norm(go), (name, np.linalg.norm(g - go) / np.linalg.norm(go))
+    # at rest the staged displacement is exactly 0: energy and gradient exactly 0
+    E, es, eb, g = emulate_kernel(plan, pack.verts, 1.0, 1.0, 2)
+    assert E == 0.0 and np.all(g == 0.0)
+
+
+def test_high_valence_rows():
+    """A 'pole' vertex with 988 operator neighbours: its row needs 4 lanes and 62 quad cells, the longest block
+    the stream format holds (several ring wraps inside one block).  989 neighbours are rejected."""
+    v, t = pole_mesh(988)
+    orc = COracle(v, t)
+    x = perturb(v, t, 0.3, 2)
+    for kw in (dict(nw=16, grid=132), dict(nw=8, grid=264), dict(nw=16, grid=132, force_global=1)):
+        plan = build_host_plan(v, t, **kw)
+        hdr = _block_headers(plan)
+        assert any(len4 == 62 and L == 4 for len4, L in hdr), "the pole row must be one 4-lane, 62-cell block"
+        E, es, eb, g = emulate_kernel(plan, x, 1e-3, 2e-3, 2)
+        Eo, terms, go = orc.energy_grad(x, 1e-3, 2e-3, 2)
+        assert terms[1] > 0 and E == pytest.approx(Eo, rel=2e-6)
+        assert np.linalg.norm(g - go) <= 2e-6 * np.linalg.norm(go)
+    with pytest.raises(RuntimeError, match="more than 988 operator neighbours"):
+        build_host_plan(*pole_mesh(989))
+
+
+def _block_headers(plan):
+    """(len4, lanes per row) of every row block in the plan's streams."""
+    G, NW, glob = plan["grid"], plan["nw"], bool(plan["mode_global"])
+    CELL, WOFF = (1024, 512) if glob else (768, 256)
+    wdesc, wseg, cs = plan["wdesc"].reshape(G, NW, 2), plan["wseg"].reshape(-1, NW, 2), plan["cta_seg"].reshape(G, 2)
+    out = []
+    for b in range(G):
+        for w in range(NW):
+            p = int(wdesc[b, w, 0]) * 16
+            for s in range(cs[b, 0], cs[b, 1]):
+                for _ in range(int(wseg[s, w, 0])):
+                    hdr = int(plan["stream"][p + WOFF:p + WOFF + 4].view(np.uint32)[0])
+                    len4 = (hdr >> 24) & 63
+                    out.append((len4, 1 << (hdr >> 30)))
+                    p += len4 * CELL
+                p += int(wseg[s, w, 1]) * CELL
+    return out
 
 
 def test_plan_operator_is_the_reference_matrix():

@@ -5,7 +5,7 @@
 // cuda_forward_det, Sasum, SpMV c1.GTLTLG.x, SpMV G.x again, cuda_backward_det, SpMV G^T, Sscal,
 // with three host syncs).
 //
-// Math (DESIGN.md section 3).  With u = x - X (X = rest positions):
+// Math (DESIGN.md section 3).  With u = x - X (X = rest positions; staged as u - u_r per component, in fp64):
 //   smoothness  1/2 x^T M x = 1/2 u^T M u        M = G^T L^T L G  (tet_spheres.cpp:148; M X = 0: affine maps are in its null space)
 //   M has zero row sums, so with d_ij = u_j - u_i
 //       (M u)_i        = sum_{j != i} M_ij d_ij
@@ -79,6 +79,17 @@ struct f32x2 { float lo, hi; };
 __device__ __forceinline__ f32x2 pk2(float lo, float hi) { return f32x2{lo, hi}; }
 __device__ __forceinline__ float sum2(f32x2 v) { return v.lo + v.hi; }
 __device__ __forceinline__ void fma2_acc(f32x2 &acc, f32x2 a, f32x2 b) { acc.lo = fmaf(a.lo, b.lo, acc.lo); acc.hi = fmaf(a.hi, b.hi, acc.hi); }
+
+// Staged displacement of a vertex whose component is shifted by c (any value shared by the component: the operator's
+// differences and the energy do not see it; the kernel takes c = u of the component's reference vertex):
+// (x - X) - c to within about one rounding of the exact value.  x - X is kept exactly as s + e (TwoSum); when the
+// component has moved far from rest, s and c are close and s - c is exact (Sterbenz), so the rigid displacement never
+// enters a rounded difference.  At rest (x = X, c = 0) the result is exactly 0.
+__device__ __forceinline__ float rel_u(float x, float X, float c) {
+  const float s = x - X, bb = s - x;
+  const float e = (x - (s - bb)) + (-X - bb);
+  return (s - c) + e;
+}
 
 template <bool GLOBAL> struct Fmt;
 template <> struct Fmt<false> { static constexpr uint32_t CELL = kCellStaged, IB = 2, TPL = 2; };   // 16-bit smem byte offsets
@@ -219,6 +230,13 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
 
   double des = 0.0, deb = 0.0, dea = 0.0;     // per-lane energy partials (smoothness, barrier, AMIPS)
 
+  // staged u = rel_u(x_i, X_i, c) with c = fp32(x_r - X_r) of the component's local vertex r = 0 (tsb_plan.cpp,
+  // staging_tables): the component's rigid displacement never enters a rounded difference
+  auto load_ref = [&](const SegHdr &h, float (&r)[3]) {
+    const size_t gr = size_t(h.vbase >= 0 ? h.vbase : __ldg(&p.vlist[h.x4off]));
+    const float4 Xr = __ldg(&p.X4[h.x4off]);
+    r[0] = __ldcg(p.x + 3 * gr) - Xr.x; r[1] = __ldcg(p.x + 3 * gr + 1) - Xr.y; r[2] = __ldcg(p.x + 3 * gr + 2) - Xr.z;
+  };
   auto load_x = [&](const SegHdr &h) {      // x of a double-buffered component -> registers
 #pragma unroll
     for (int k = 0; k < SV; ++k) {
@@ -231,24 +249,28 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
   };
   auto store_staged = [&](const SegHdr &h, int li) {
     float4 *ub = stage + ubase_of(h, li), *xb = stage + xbase_of(h, li);
+    float pr[3];                            // loaded here, not with px: kept out of the segment loop's live registers
+    load_ref(h, pr);
 #pragma unroll
     for (int k = 0; k < SV; ++k) {
       const int v = tid + k * NT;
       if (v < h.nv) {
         const uint32_t pos = __float_as_uint(pX[k].w);
-        ub[pos] = make_float4(px[k][0] - pX[k].x, px[k][1] - pX[k].y, px[k][2] - pX[k].z, 0.f);
+        ub[pos] = make_float4(rel_u(px[k][0], pX[k].x, pr[0]), rel_u(px[k][1], pX[k].y, pr[1]), rel_u(px[k][2], pX[k].z, pr[2]), 0.f);
         xb[pos] = make_float4(px[k][0], px[k][1], px[k][2], 0.f);
       }
     }
   };
   auto stage_direct = [&](const SegHdr &h, int li) {   // any size, no register prefetch
     float4 *ub = stage + ubase_of(h, li), *xb = stage + xbase_of(h, li);
+    float r[3];
+    load_ref(h, r);
     for (int v = tid; v < h.nv; v += NT) {
       const float4 X = __ldg(&p.X4[h.x4off + v]);
       const size_t gi = size_t(h.vbase >= 0 ? h.vbase + v : __ldg(&p.vlist[h.x4off + v]));
       const float x0 = __ldcg(p.x + 3 * gi), x1 = __ldcg(p.x + 3 * gi + 1), x2 = __ldcg(p.x + 3 * gi + 2);
       const uint32_t pos = __ldg(&p.pos16[h.x4off + v]);
-      ub[pos] = make_float4(x0 - X.x, x1 - X.y, x2 - X.z, 0.f);
+      ub[pos] = make_float4(rel_u(x0, X.x, r[0]), rel_u(x1, X.y, r[1]), rel_u(x2, X.z, r[2]), 0.f);
       xb[pos] = make_float4(x0, x1, x2, 0.f);
     }
   };
@@ -266,7 +288,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
         load_x(hcur); store_staged(hcur, 0);
       } else {
         // both components' loads in flight together (second register set), then both stores
-        float qx[SV][3];
+        float qx[SV][3], qr[3];
         float4 qX[SV];
 #pragma unroll
         for (int k = 0; k < SV; ++k) {
@@ -274,6 +296,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
           if (v < h1.nv) { qX[k] = __ldg(&p.X4[h1.x4off + v]); qX[k].w = __uint_as_float(uint32_t(__ldg(&p.pos16[h1.x4off + v]))); }
         }
         load_x(hcur);
+        load_ref(h1, qr);
 #pragma unroll
         for (int k = 0; k < SV; ++k) {
           const int v = tid + k * NT;
@@ -289,7 +312,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
           const int v = tid + k * NT;
           if (v < h1.nv) {
             const uint32_t pos = __float_as_uint(qX[k].w);
-            ub[pos] = make_float4(qx[k][0] - qX[k].x, qx[k][1] - qX[k].y, qx[k][2] - qX[k].z, 0.f);
+            ub[pos] = make_float4(rel_u(qx[k][0], qX[k].x, qr[0]), rel_u(qx[k][1], qX[k].y, qr[1]), rel_u(qx[k][2], qX[k].z, qr[2]), 0.f);
             xb[pos] = make_float4(qx[k][0], qx[k][1], qx[k][2], 0.f);
           }
         }
@@ -609,13 +632,17 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
 #endif
 }
 
-// GLOBAL mode pre-pass: u = x - X and x as float4 per vertex.
+// GLOBAL mode pre-pass: u = rel_u(x, X, c), c = fp32(x_r - X_r) of the component's reference vertex r = X4[v].w (see
+// staging_tables in tsb_plan.cpp), and x as float4 per vertex.
 __global__ void prestage_kernel(const float *__restrict__ x, const float4 *__restrict__ X4, float4 *__restrict__ u4,
                                 float4 *__restrict__ x4, int n) {
   for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < n; v += gridDim.x * blockDim.x) {
     const float4 X = X4[v];
+    const size_t r = size_t(__float_as_uint(X.w));
+    const float4 Xr = X4[r];
     const float a = x[3 * size_t(v)], b = x[3 * size_t(v) + 1], c = x[3 * size_t(v) + 2];
-    u4[v] = make_float4(a - X.x, b - X.y, c - X.z, 0.f);
+    const float c0 = x[3 * r] - Xr.x, c1 = x[3 * r + 1] - Xr.y, c2 = x[3 * r + 2] - Xr.z;
+    u4[v] = make_float4(rel_u(a, X.x, c0), rel_u(b, X.y, c1), rel_u(c, X.z, c2), 0.f);
     x4[v] = make_float4(a, b, c, 0.f);
   }
 }

@@ -11,7 +11,7 @@ namespace tsb {
 struct KParams {
   // plan (read-only, built once by tsb_create)
   const unsigned char *stream;  // per-warp byte streams (operator rows + tet blocks)
-  const float4 *X4;             // rest positions, float4 per staged vertex (STAGED: component-major; GLOBAL: by vertex id)
+  const float4 *X4;             // rest positions (STAGED: component-major; GLOBAL: by vertex id, .w = reference vertex)
   const int32_t *vlist;         // STAGED: global vertex id per staged vertex (used when a component is not contiguous)
   const uint16_t *pos16;        // STAGED: staging position per staged vertex (bank-aware placement)
   const int32_t *pos_gid;       // STAGED: global vertex id per staging position

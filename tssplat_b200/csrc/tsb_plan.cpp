@@ -808,6 +808,13 @@ std::vector<Seg> make_segments(const std::vector<Comp> &comps, const std::vector
 
 // Staging tables (STAGED: rest position, global id and staging position of every component vertex; GLOBAL: rest
 // positions by vertex id) and the segment headers.
+//
+// The kernel stages u_i - c instead of u_i = x_i - X_i, with c = fp32(x_r - X_r) of the component's reference vertex r
+// (its local vertex 0), formed from the exact difference x_i - X_i (a TwoSum pair, rel_u in tsb_kernels.cu) and
+// rounded once: a sphere that has moved far from its rest pose would otherwise lose ulp(|x - X|) in every staged u,
+// and every operator difference u_j - u_i inherits that error.  A shift shared by the component's vertices changes neither the differences nor the energy,
+// and at rest u is still exactly 0.  STAGED: r is the first vertex of the component's X4 / vlist range; GLOBAL: X4's
+// .w holds the bit pattern of r's global id (the pre-pass has no segment header to find it in).
 void staging_tables(const Mesh &M, const std::vector<Comp> &comps, const std::vector<Seg> &segs, HostPlan &P) {
   const int NC = int(comps.size());
   const bool GLOBAL = P.mode_global != 0;
@@ -830,8 +837,12 @@ void staging_tables(const Mesh &M, const std::vector<Comp> &comps, const std::ve
       }
   } else {
     P.X4.assign(size_t(M.n) * 4, 0.f);
-    for (int v = 0; v < M.n; ++v)
+    for (int32_t v = 0; v < M.n; ++v) {     // vertices no tet references are their own reference (never gathered)
       for (int r = 0; r < 3; ++r) P.X4[size_t(v) * 4 + r] = M.rest[3 * size_t(v) + r];
+      std::memcpy(&P.X4[size_t(v) * 4 + 3], &v, 4);
+    }
+    for (const Comp &C : comps)
+      for (const int32_t v : C.verts) std::memcpy(&P.X4[size_t(v) * 4 + 3], &C.verts[0], 4);
   }
   P.segs.resize(segs.size());
   for (size_t s = 0; s < segs.size(); ++s) {
@@ -865,7 +876,7 @@ int row_blocks(const std::vector<RowRef> &rows, int ntc, int NW, int ring_cells,
   for (size_t i = 0; i < rows.size();) {
     int L = 1;
     while (L < kMaxLanesPerRow && rb_len4(rows.data() + i, 1, L) > rb_cap) L *= 2;
-    if (rb_len4(rows.data() + i, 1, L) > 62) { err = "a vertex has more than 980 operator neighbours"; return TSB_E_MESH; }
+    if (rb_len4(rows.data() + i, 1, L) > 62) { err = "a vertex has more than 988 operator neighbours"; return TSB_E_MESH; }
     const int nr = int(std::min<size_t>(size_t(32 / L), rows.size() - i));
     rbs.push_back(RB{int(i), nr, L, rb_len4(rows.data() + i, nr, L)});
     i += nr;

@@ -113,7 +113,8 @@ struct HostPlan {
   int64_t tet_wavefronts[2] = {0, 0};
 
   std::vector<uint8_t, NoInitAlloc<uint8_t>> stream;   // all warp streams, 16-byte aligned (filled by parallel copies)
-  std::vector<float> X4;            // 4 floats per staged vertex (X, Y, Z, 0), component-major
+  std::vector<float> X4;            // STAGED: (X, Y, Z, 0) per staged vertex, component-major; GLOBAL: (X, Y, Z, bits
+                                    // of the id of the component's reference vertex) by vertex id
   std::vector<int32_t> vlist;       // global id per staged vertex (same order as X4)
   // Bank-aware placement: vertex k of a component is staged at position pos16[x4off + k] of its u / x
   // arrays; positions are chosen so that (position mod 8) -- the 16-byte shared-memory bank group of
