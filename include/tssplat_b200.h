@@ -42,7 +42,9 @@ typedef struct {
   int32_t tet_cost_x100;    /* load-balance weight of one tet vs one operator entry, x100 (0 = default) */
   int32_t enable_amips;     /* 1: also keep the per-tet rest inverses (48 B/tet) so that tsb_energy_grad_ex
                                may add the AMIPS term; 0 (default): c3 must be 0                    */
-  int32_t reserved[2];
+  int32_t deterministic;    /* 1: bitwise repeatable gradient, also with inverted tets and AMIPS (see
+                               tsb_energy_grad); costs a second launch and 64 B/tet of device memory */
+  int32_t reserved[1];
 } tsb_options_t;
 
 /* Energy terms of tsb_energy_grad_ex.  c3 weighs the AMIPS term that BASELINE.json's north_star names:
@@ -105,7 +107,17 @@ int tsb_get_info(tsb_handle_t h, tsb_info_t *info);
  * owns counters and scratch, like the reference's TetSpheres: tet_spheres.h:37); launches on one
  * stream are chained with programmatic dependent launch.  Results are bitwise repeatable when no tet
  * is inverted; inverted tets add their barrier gradient with red.global.add.f32 (order-dependent
- * rounding in the affected vertices only). */
+ * rounding in the affected vertices only).
+ * Deterministic handles (tsb_options_t.deterministic = 1): every contributing tet (inverted, or any tet
+ * with J > 0 when the AMIPS term is on) stores its corner vectors in handle scratch, and a second
+ * kernel on the same stream adds them to each vertex in a fixed order; grad_out_dev == NULL runs the
+ * energy kernel alone.  The energies and the gradient are then a pure function of (plan, x, the
+ * coefficients, gradH): bitwise identical across launches, streams, CUDA-graph replays and handles
+ * created from the same mesh with the same options, for tsb_energy_grad, tsb_energy_grad_ex and
+ * tsb_energy_grad_host alike.  The energies, and the gradient rows no contributing tet touches, are
+ * bitwise those of a default handle with the same options.  The guarantee holds for one handle
+ * configuration only: warps_per_cta, force_global (or a mesh that needs global gathers) and
+ * ring_slots change the plan, and with it the summation order and the tets' vertex order. */
 int tsb_energy_grad(tsb_handle_t h, const float *x_dev, float c1, float c2, int32_t order,
                     float gradH, const float *gradH_dev, float *energy_out_dev,
                     float *grad_out_dev, void *stream);
@@ -113,7 +125,7 @@ int tsb_energy_grad(tsb_handle_t h, const float *x_dev, float c1, float c2, int3
 /* tsb_energy_grad plus the optional AMIPS term.  energy_out_dev: device float32 [4] = total, smoothness,
  * barrier, AMIPS (unweighted sums; total = c1*smooth + c2*barrier + c3*amips).  With terms->c3 == 0 the launch
  * is the very kernel tsb_energy_grad runs.  c3 != 0 needs a handle created with enable_amips = 1; its gradient
- * is added with red.global.add.f32 for every tet (order-dependent rounding). */
+ * is added with red.global.add.f32 for every tet (order-dependent rounding), except on a deterministic handle. */
 int tsb_energy_grad_ex(tsb_handle_t h, const float *x_dev, const tsb_terms_t *terms, float gradH,
                        const float *gradH_dev, float *energy_out_dev, float *grad_out_dev, void *stream);
 

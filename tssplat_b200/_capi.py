@@ -26,7 +26,8 @@ EXPORTED_SYMBOLS = (
 
 class tsb_options_t(C.Structure):
     _fields_ = [("warps_per_cta", C.c_int32), ("laplacian_scale", C.c_int32), ("ring_slots", C.c_int32),
-                ("force_global", C.c_int32), ("tet_cost_x100", C.c_int32), ("enable_amips", C.c_int32), ("reserved", C.c_int32 * 2)]
+                ("force_global", C.c_int32), ("tet_cost_x100", C.c_int32), ("enable_amips", C.c_int32),
+                ("deterministic", C.c_int32), ("reserved", C.c_int32 * 1)]
 
 
 class tsb_terms_t(C.Structure):

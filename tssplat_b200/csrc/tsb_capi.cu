@@ -23,6 +23,8 @@ struct tsb_handle_s {
   cudaEvent_t ev_run[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr};
   unsigned host_calls = 0;
   bool amips = false;
+  bool det = false;             // deterministic gradient: DET energy kernel + det_gather_kernel
+  tsb::DetParams dp{};
   tsb_info_t info{};
   std::vector<void *> allocs;
   std::string err;
@@ -107,6 +109,7 @@ int tsb_create(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t ne
     pc.laplacian_scale = opt->laplacian_scale ? 1 : 0;
     pc.force_global = opt->force_global ? 1 : 0;
     pc.enable_amips = opt->enable_amips ? 1 : 0;
+    pc.deterministic = opt->deterministic ? 1 : 0;
   }
   if (nw != 8 && nw != 16) return fail(nullptr, TSB_E_INVALID, "warps_per_cta must be 8 or 16");
   if (ring < 2 || ring > 8) return fail(nullptr, TSB_E_INVALID, "ring_slots must be in [2, 8]");
@@ -140,7 +143,7 @@ int tsb_create(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t ne
     if (global_mode) while (slots > 2 && tsb::energy_smem_bytes(nw, slots, cpc, 0, true) > smem_optin) --slots;
     smem = tsb::energy_smem_bytes(nw, slots, cpc, global_mode ? 0 : area_verts, global_mode);
     int ctas = 0;
-    cudaError_t e = tsb::energy_occupancy(nw, smem, global_mode, pc.enable_amips != 0, &ctas);
+    cudaError_t e = tsb::energy_occupancy(nw, smem, global_mode, pc.enable_amips != 0, pc.deterministic != 0, &ctas);
     if (e != cudaSuccess || ctas < 1) {
       err = std::string("kernel does not fit the device: ") + (e != cudaSuccess ? cudaGetErrorString(e) : "occupancy 0");
       return TSB_E_CUDA;
@@ -173,6 +176,25 @@ int tsb_create(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t ne
     TSB_TRY(upload(h, plan.Bt, kp.Bt, 4));
     TSB_TRY(upload(h, plan.wtc0, kp.wtc0));
   }
+  if (pc.deterministic) {
+    // 48 B of corner vectors per tet slot, 8 B of ballot per tet cell, the vertex lists (16 B per tet) and their rows
+    const size_t slots = size_t(plan.n_tetcells) * (plan.mode_global ? 32 : 64);
+    tsb::DetParams &dp = h->dp;
+    if (!pc.enable_amips) TSB_TRY(upload(h, plan.wtc0, kp.wtc0));
+    TSB_TRY(alloc_zero(h, slots * 3, &kp.det_scratch));
+    TSB_TRY(alloc_zero(h, size_t(plan.n_tetcells), &kp.det_ballot));
+    TSB_TRY(alloc_zero(h, size_t(plan.n_components), &kp.det_flag));
+    TSB_TRY(upload(h, plan.det_rowptr, dp.rowptr));
+    TSB_TRY(upload(h, plan.det_vert, dp.vert));
+    TSB_TRY(upload(h, plan.det_comp_row, dp.comp_row));
+    TSB_TRY(upload(h, plan.det_ent, dp.ent));
+    TSB_TRY(upload(h, plan.det_chunk, dp.chunk, 2));
+    dp.scratch = kp.det_scratch;
+    dp.ballot = kp.det_ballot;
+    dp.flag = kp.det_flag;
+    dp.n_chunks = int32_t(plan.det_chunk.size() / 2);
+    dp.tpl_log = plan.mode_global ? 0 : 1;
+  }
   TSB_TRY(alloc_zero(h, size_t(plan.n_components), &kp.done));
   TSB_TRY(upload(h, std::vector<unsigned long long>(size_t(plan.grid) * 4, tsb::kEnergySentinel), kp.cta_energy, 2));
 #ifdef TSB_TRACE
@@ -191,8 +213,9 @@ int tsb_create(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t ne
   kp.cells_per_chunk = cpc;
   kp.ring_slots = slots;
   kp.stage_bytes = plan.mode_global ? 0 : plan.area_verts * 32;
-  h->lc = tsb::LaunchConfig{nw, plan.grid, smem, plan.mode_global, 0};
+  h->lc = tsb::LaunchConfig{nw, plan.grid, smem, plan.mode_global, 0, 0};
   h->amips = pc.enable_amips != 0;
+  h->det = pc.deterministic != 0;
 
   tsb_info_t &I = h->info;
   I.n = plan.n; I.nele = plan.nele; I.n_components = plan.n_components; I.grid = plan.grid;
@@ -242,8 +265,13 @@ static int energy_grad_impl(tsb_handle_t h, const float *x_dev, float c1, float 
   kp.c1 = c1; kp.c2 = c2; kp.c3 = c3; kp.gradH = gradH; kp.order = order; kp.energy4 = energy4;
   tsb::LaunchConfig lc = h->lc;
   lc.amips = c3 != 0.f ? 1 : 0;          // c3 == 0: the very instantiation tsb_energy_grad always ran
+  lc.det = h->det && grad_out_dev ? 1 : 0;   // energy only: the default kernel computes the same energies
   cudaError_t e = tsb::launch_energy_grad(kp, lc, static_cast<cudaStream_t>(stream));
   if (e != cudaSuccess) return fail(h, TSB_E_CUDA, std::string("energy_grad launch: ") + cudaGetErrorString(e));
+  if (lc.det) {
+    e = tsb::launch_det_gather(h->dp, grad_out_dev, static_cast<cudaStream_t>(stream));
+    if (e != cudaSuccess) return fail(h, TSB_E_CUDA, std::string("deterministic gather launch: ") + cudaGetErrorString(e));
+  }
   return TSB_OK;
 }
 

@@ -143,7 +143,10 @@ struct WarpStream {
   }
 };
 
-template <int NW, int MINB, bool GLOBAL, bool AMIPS>
+// DET (deterministic gradient, tsb_options_t.deterministic): a contributing tet stores its four corner vectors at its
+// tet slot instead of adding them to grad, every tet cell stores its activity ballot, and the component is flagged;
+// det_gather_kernel then adds them in a fixed order.  Tets never touch grad, so there is no rows-done protocol.
+template <int NW, int MINB, bool GLOBAL, bool AMIPS, bool DET = false>
 __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParams p) {
   using F = Fmt<GLOBAL>;
   constexpr int NT = NW * 32;
@@ -415,7 +418,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
       }
     }
     if (s == cs.x) TSB_STAMP(5);
-    if (grad) {   // all warps' rows of this segment are stored -> ONE release of the component's counter, sent by
+    if (!DET && grad) {   // all warps' rows of this segment are stored -> ONE release of the component's counter, sent by
                   // the last warp (which owns no tets, so it never waits on its own signal)
       const int bar_id = 1 + (li & 1);      // segments 0 and 1 may be in flight together: two barrier ids
       if (warp == NW - 1) {
@@ -428,8 +431,17 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
 
     // ---- barrier: TPL tets per lane ---------------------------------------------------------------------
     bool waited = false;
-    const int tcell0 = amips_on ? __ldg(&p.wtc0[size_t(s) * NW + warp]) : 0;
+    const int tcell0 = (amips_on || (DET && grad)) ? __ldg(&p.wtc0[size_t(s) * NW + warp]) : 0;
+    // DET: corner vectors c0..c3 of the tet in slot lane * TPL + t of tet cell tcell0 + tc
+    auto det_store = [&](int tc, int t, float c0x, float c0y, float c0z, float c1x, float c1y, float c1z, float c2x, float c2y,
+                         float c2z, float c3x, float c3y, float c3z) {
+      float4 *d = p.det_scratch + 3 * (size_t(tcell0 + tc) * (32 * F::TPL) + lane * F::TPL + t);
+      d[0] = make_float4(c0x, c0y, c0z, c1x);
+      d[1] = make_float4(c1y, c1z, c2x, c2y);
+      d[2] = make_float4(c2z, c3x, c3y, c3z);
+    };
     for (int tc = 0; tc < int(wseg.y); ++tc) {
+      uint32_t dmask = 0;   // DET: bit t = this lane's tet t contributed
       uint32_t tj[F::TPL][4];
       float tdet[F::TPL];
       if (GLOBAL) {
@@ -467,6 +479,11 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
             const float g1x = k * c1x, g1y = k * c1y, g1z = k * c1z;
             const float g2x = k * (e3y * e1z - e3z * e1y), g2y = k * (e3z * e1x - e3x * e1z), g2z = k * (e3x * e1y - e3y * e1x);
             const float g3x = k * (e1y * e2z - e1z * e2y), g3y = k * (e1z * e2x - e1x * e2z), g3z = k * (e1x * e2y - e1y * e2x);
+            if constexpr (DET) {
+              det_store(tc, t, -(g1x + g2x + g3x), -(g1y + g2y + g3y), -(g1z + g2z + g3z), g1x, g1y, g1z, g2x, g2y, g2z, g3x, g3y, g3z);
+              dmask |= 1u << t;
+              continue;
+            }
             if (!waited) {   // every row of this component must be stored before we add to it
               const unsigned int need = unsigned(hcur.expected);
               while (ld_acquire(p.done + hcur.comp) < need) __nanosleep(40);
@@ -512,6 +529,19 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
             Pm[2][0] = a * (Fm[2][0] - bq * (Fm[0][1] * Fm[1][2] - Fm[0][2] * Fm[1][1]));
             Pm[2][1] = a * (Fm[2][1] - bq * (Fm[0][2] * Fm[1][0] - Fm[0][0] * Fm[1][2]));
             Pm[2][2] = a * (Fm[2][2] - bq * (Fm[0][0] * Fm[1][1] - Fm[0][1] * Fm[1][0]));
+            if constexpr (DET) {
+              float gk[3][3], g0[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+              for (int k = 0; k < 3; ++k)
+#pragma unroll
+                for (int r = 0; r < 3; ++r) {
+                  gk[k][r] = Pm[r][0] * bb[k][0] + Pm[r][1] * bb[k][1] + Pm[r][2] * bb[k][2];
+                  g0[r] -= gk[k][r];
+                }
+              det_store(tc, t, g0[0], g0[1], g0[2], gk[0][0], gk[0][1], gk[0][2], gk[1][0], gk[1][1], gk[1][2], gk[2][0], gk[2][1], gk[2][2]);
+              dmask |= 1u << t;
+              continue;
+            }
             if (!waited) {
               const unsigned int need = unsigned(hcur.expected);
               while (ld_acquire(p.done + hcur.comp) < need) __nanosleep(40);
@@ -533,6 +563,13 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
           }
         }
       }
+      if (DET && grad) {   // every launch with a gradient rewrites every cell's ballot: inactive slots are never read
+        const unsigned m0 = __ballot_sync(0xffffffffu, dmask & 1u), m1 = F::TPL > 1 ? __ballot_sync(0xffffffffu, dmask & 2u) : 0u;
+        if (lane == 0) {
+          p.det_ballot[tcell0 + tc] = (static_cast<unsigned long long>(m1) << 32) | m0;
+          if (m0 | m1) p.det_flag[hcur.comp] = 1u;
+        }
+      }
     }
     if (s == cs.x) TSB_STAMP(6);
 
@@ -552,7 +589,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
             __syncthreads();
           }
         }
-      } else if (grad) {
+      } else if (!DET && grad) {
         __syncthreads();     // keeps the named barrier's generations apart
       }
     }
@@ -624,7 +661,8 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
       p.energy_out[2] = float(b);
       if (p.energy4) p.energy_out[3] = float(c3sum);
     }
-    for (int c = lane; c < p.n_components; c += 32) p.done[c] = 0u;   // every CTA has finished: safe to re-arm
+    if (!DET)
+      for (int c = lane; c < p.n_components; c += 32) p.done[c] = 0u;   // every CTA has finished: safe to re-arm
   }
   TSB_STAMP(10);
 #ifdef TSB_TRACE
@@ -644,6 +682,49 @@ __global__ void prestage_kernel(const float *__restrict__ x, const float4 *__res
     const float c0 = x[3 * r] - Xr.x, c1 = x[3 * r + 1] - Xr.y, c2 = x[3 * r + 2] - Xr.z;
     u4[v] = make_float4(rel_u(a, X.x, c0), rel_u(b, X.y, c1), rel_u(c, X.z, c2), 0.f);
     x4[v] = make_float4(a, b, c, 0.f);
+  }
+}
+
+// Deterministic gather, after a DET launch on the same stream: CTA = a run of <= kDetChunkRows vertex rows of one
+// component (thread = row).  Unflagged components are skipped without reading their lists.  A row sums the corner
+// vectors of its list's active entries in list order, starting from +0, and adds the sum to grad: it is the only
+// writer of its row, so the result does not depend on scheduling.  The last CTA of a flagged component to finish
+// clears the flag (flag = 1 + number of CTAs done, so every CTA reads it before it is cleared).
+__global__ void __launch_bounds__(kDetChunkRows) det_gather_kernel(const DetParams d, float *__restrict__ grad) {
+  asm volatile("griddepcontrol.wait;" ::: "memory");       // everything below reads what the energy kernel wrote
+                                                             // (a no-op under the plain launch used now)
+  const int2 ch = __ldg(&d.chunk[blockIdx.x]);               // (component, first row)
+  const unsigned flag = __ldcg(d.flag + ch.x);
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  if (!flag) return;
+  const int row0 = __ldg(&d.comp_row[ch.x]), row_end = __ldg(&d.comp_row[ch.x + 1]);
+  const int r = ch.y + int(threadIdx.x);
+  if (r < row_end) {
+    const int b = __ldg(&d.rowptr[r]), e = __ldg(&d.rowptr[r + 1]);
+    const float *sc = reinterpret_cast<const float *>(d.scratch);
+    const uint32_t tpl_mask = (1u << d.tpl_log) - 1u, cell_log = 5 + d.tpl_log;
+    float ax = 0.f, ay = 0.f, az = 0.f;
+    bool any = false;
+#pragma unroll 4
+    for (int i = b; i < e; ++i) {
+      const uint32_t ent = __ldg(&d.ent[i]), slot = ent >> 2, k = ent & 3u;
+      const uint32_t sic = slot & ((1u << cell_log) - 1u);                  // lane * TPL + t
+      const unsigned long long m = __ldcg(d.ballot + (slot >> cell_log));
+      const bool act = (m >> (((sic & tpl_mask) << 5) | (sic >> d.tpl_log))) & 1ull;
+      // inactive slots hold stale values: loaded anyway (no dependence on the ballot), never added
+      const float *c = sc + size_t(slot) * 12 + k * 3;
+      const float cx = __ldcg(c), cy = __ldcg(c + 1), cz = __ldcg(c + 2);
+      if (act) { ax += cx; ay += cy; az += cz; any = true; }
+    }
+    if (any) {
+      const size_t v = 3 * size_t(__ldg(&d.vert[r]));
+      grad[v] += ax; grad[v + 1] += ay; grad[v + 2] += az;
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const unsigned nchunks = unsigned((row_end - row0 + kDetChunkRows - 1) / kDetChunkRows);
+    if (nchunks == 1 || atomicAdd(d.flag + ch.x, 1u) == nchunks) d.flag[ch.x] = 0u;
   }
 }
 
@@ -730,7 +811,7 @@ inline int grid_for(int64_t count, int block) {
   return int(g < 1 ? 1 : (g > kMaxGrid ? kMaxGrid : g));
 }
 
-template <int NW, int MINB, bool GLOBAL, bool AMIPS>
+template <int NW, int MINB, bool GLOBAL, bool AMIPS, bool DET = false>
 cudaError_t launch_variant(const KParams &p, const LaunchConfig &lc, cudaStream_t stream) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(unsigned(lc.grid));
@@ -742,11 +823,24 @@ cudaError_t launch_variant(const KParams &p, const LaunchConfig &lc, cudaStream_
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, energy_grad_kernel<NW, MINB, GLOBAL, AMIPS>, p);
+  return cudaLaunchKernelEx(&cfg, energy_grad_kernel<NW, MINB, GLOBAL, AMIPS, DET>, p);
 }
 
 template <int NW, int MINB, bool GLOBAL>
-cudaError_t occupancy_variant(int smem_bytes, bool amips, int *ctas_per_sm) {
+cudaError_t launch_det_variant(const KParams &p, const LaunchConfig &lc, cudaStream_t stream) {
+  return lc.amips ? launch_variant<NW, MINB, GLOBAL, true, true>(p, lc, stream) : launch_variant<NW, MINB, GLOBAL, false, true>(p, lc, stream);
+}
+
+// occupancy of the deterministic instantiations (opts them in to the device's shared memory maximum like the others)
+template <int NW, int MINB, bool GLOBAL, bool AMIPS>
+cudaError_t occupancy_det(int smem_bytes, int optin, int *ctas_per_sm) {
+  cudaError_t e = cudaFuncSetAttribute(energy_grad_kernel<NW, MINB, GLOBAL, AMIPS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
+  if (e != cudaSuccess) { *ctas_per_sm = 0; cudaGetLastError(); return cudaSuccess; }
+  return cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, energy_grad_kernel<NW, MINB, GLOBAL, AMIPS, true>, NW * 32, size_t(smem_bytes));
+}
+
+template <int NW, int MINB, bool GLOBAL>
+cudaError_t occupancy_variant(int smem_bytes, bool amips, bool det, int *ctas_per_sm) {
   // opt in to the device maximum once (the attribute is per function, not per handle: handles with different
   // staging sizes share the kernel)
   int dev = 0, optin = 0;
@@ -761,6 +855,13 @@ cudaError_t occupancy_variant(int smem_bytes, bool amips, int *ctas_per_sm) {
   e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, energy_grad_kernel<NW, MINB, GLOBAL, false>, NW * 32, size_t(smem_bytes));
   if (e == cudaSuccess && amips) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, energy_grad_kernel<NW, MINB, GLOBAL, true>, NW * 32, size_t(smem_bytes));
   *ctas_per_sm = a < b ? a : b;
+  if (e == cudaSuccess && det) {
+    int c = 0, d = 1 << 30;
+    e = occupancy_det<NW, MINB, GLOBAL, false>(smem_bytes, optin, &c);
+    if (e == cudaSuccess && amips) e = occupancy_det<NW, MINB, GLOBAL, true>(smem_bytes, optin, &d);
+    if (c < *ctas_per_sm) *ctas_per_sm = c;
+    if (d < *ctas_per_sm) *ctas_per_sm = d;
+  }
   return e;
 }
 
@@ -772,9 +873,9 @@ int energy_smem_bytes(int nw, int ring_slots, int cells_per_chunk, int area_vert
   return smem_total(global ? 0 : area_verts * 32, nw, energy_ring_bytes(ring_slots, cells_per_chunk, global));
 }
 
-cudaError_t energy_occupancy(int nw, int smem_bytes, bool global, bool amips, int *ctas_per_sm) {
-  if (nw == 16) return global ? occupancy_variant<16, 1, true>(smem_bytes, amips, ctas_per_sm) : occupancy_variant<16, 1, false>(smem_bytes, amips, ctas_per_sm);
-  if (nw == 8) return global ? occupancy_variant<8, 2, true>(smem_bytes, amips, ctas_per_sm) : occupancy_variant<8, 2, false>(smem_bytes, amips, ctas_per_sm);
+cudaError_t energy_occupancy(int nw, int smem_bytes, bool global, bool amips, bool det, int *ctas_per_sm) {
+  if (nw == 16) return global ? occupancy_variant<16, 1, true>(smem_bytes, amips, det, ctas_per_sm) : occupancy_variant<16, 1, false>(smem_bytes, amips, det, ctas_per_sm);
+  if (nw == 8) return global ? occupancy_variant<8, 2, true>(smem_bytes, amips, det, ctas_per_sm) : occupancy_variant<8, 2, false>(smem_bytes, amips, det, ctas_per_sm);
   return cudaErrorInvalidValue;
 }
 
@@ -783,13 +884,23 @@ cudaError_t launch_energy_grad(const KParams &p, const LaunchConfig &lc, cudaStr
     prestage_kernel<<<grid_for(p.n, 256), 256, 0, stream>>>(p.x, p.X4, p.u4g, p.x4g, p.n);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
+    if (lc.det) return lc.nw == 16 ? launch_det_variant<16, 1, true>(p, lc, stream) : launch_det_variant<8, 2, true>(p, lc, stream);
     if (lc.nw == 16) return lc.amips ? launch_variant<16, 1, true, true>(p, lc, stream) : launch_variant<16, 1, true, false>(p, lc, stream);
     if (lc.nw == 8) return lc.amips ? launch_variant<8, 2, true, true>(p, lc, stream) : launch_variant<8, 2, true, false>(p, lc, stream);
     return cudaErrorInvalidValue;
   }
+  if (lc.det) return lc.nw == 16 ? launch_det_variant<16, 1, false>(p, lc, stream) : launch_det_variant<8, 2, false>(p, lc, stream);
   if (lc.nw == 16) return lc.amips ? launch_variant<16, 1, false, true>(p, lc, stream) : launch_variant<16, 1, false, false>(p, lc, stream);
   if (lc.nw == 8) return lc.amips ? launch_variant<8, 2, false, true>(p, lc, stream) : launch_variant<8, 2, false, false>(p, lc, stream);
   return cudaErrorInvalidValue;
+}
+
+// A plain launch (the gather starts when the energy kernel has finished); its early launch_dependents still lets the
+// next energy launch start its plan prefetch while the gather runs.  Launching the gather with programmatic dependent
+// launch as well measured 5x slower at 64 x 4096 with inverted tets (DESIGN.md section 3).
+cudaError_t launch_det_gather(const DetParams &d, float *grad, cudaStream_t stream) {
+  det_gather_kernel<<<unsigned(d.n_chunks), kDetChunkRows, 0, stream>>>(d, grad);
+  return cudaGetLastError();
 }
 
 cudaError_t launch_scale(const float *g, int64_t count, float gradH, const float *gradH_dev, float *out, cudaStream_t s) {

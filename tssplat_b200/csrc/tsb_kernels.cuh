@@ -42,6 +42,11 @@ struct KParams {
   int32_t cells_per_chunk;      // cells per TMA bulk copy (= per ring slot)
   int32_t ring_slots;
   int32_t stage_bytes;          // STAGED: bytes of the staging area at the start of shared memory
+  // deterministic gradient only (tsb_options_t.deterministic): per-handle scratch the DET instantiation fills and
+  // det_gather_kernel consumes.  Tet slot (wtc0 + tc) * (tets per cell) + lane * TPL + t (tsb_plan.h).
+  float4 *det_scratch;          // [3 * slots] corner vectors of a contributing tet: (c0.xyz, c1.x) (c1.yz, c2.xy) (c2.z, c3.xyz)
+  unsigned long long *det_ballot;   // [tet cells] bit t * 32 + lane: the tet in slot lane * TPL + t contributed
+  unsigned int *det_flag;       // [n_components] nonzero: a tet of the component contributed (the gather clears it)
 #ifdef TSB_TRACE
   unsigned long long *trace;    // profiling build only: [grid][16] phase stamps
 #endif
@@ -53,15 +58,31 @@ struct LaunchConfig {
   int smem_bytes;  // dynamic shared memory
   int global;      // GLOBAL mode
   int amips;       // launch the AMIPS-capable instantiation
+  int det;         // launch the deterministic instantiation (tets store their corners instead of adding them)
+};
+
+// The deterministic gather's plan (HostPlan::det_*, uploaded) and the scratch it shares with the energy kernel.
+struct DetParams {
+  const int32_t *rowptr, *vert, *comp_row;
+  const uint32_t *ent;              // slot * 4 + corner
+  const int2 *chunk;                // (component, first row) of every CTA
+  const float4 *scratch;
+  const unsigned long long *ballot;
+  unsigned int *flag;
+  int32_t n_chunks;
+  int32_t tpl_log;                  // log2(tets per lane): 1 STAGED, 0 GLOBAL
 };
 
 // Dynamic shared memory the kernel needs for a configuration (ring_slots chunks of cells_per_chunk cells per warp).
 int energy_ring_bytes(int ring_slots, int cells_per_chunk, bool global);
 int energy_smem_bytes(int nw, int ring_slots, int cells_per_chunk, int area_verts, bool global);
 constexpr unsigned long long kEnergySentinel = 0x7FF8F00DBAADC0DEull;   // initial value of cta_energy
-// Max co-resident CTAs per SM for a configuration (0 if it does not fit); also opts in to the smem size.
-cudaError_t energy_occupancy(int nw, int smem_bytes, bool global, bool amips, int *ctas_per_sm);
+// Max co-resident CTAs per SM for a configuration (0 if it does not fit); also opts in to the smem size.  det: the
+// deterministic instantiations count too.
+cudaError_t energy_occupancy(int nw, int smem_bytes, bool global, bool amips, bool det, int *ctas_per_sm);
 cudaError_t launch_energy_grad(const KParams &p, const LaunchConfig &lc, cudaStream_t stream);
+// grad[v] += the active corner vectors of v's list, in list order, for every flagged component (after a DET launch).
+cudaError_t launch_det_gather(const DetParams &d, float *grad, cudaStream_t stream);
 
 cudaError_t launch_scale(const float *g, int64_t count, float gradH, const float *gradH_dev, float *out, cudaStream_t s);
 cudaError_t launch_grad_limit(float *g, int64_t count, float thr, float s, float *work4, cudaStream_t st);

@@ -467,9 +467,11 @@ int emit_rb(std::vector<uint8_t> &s, const Comp &C, const RowRef *rows, int nrow
   return len4;
 }
 
-// Appends one tet cell: STAGED 64 tets (2 per lane), GLOBAL 32 tets.
+// Appends one tet cell: STAGED 64 tets (2 per lane), GLOBAL 32 tets.  Vout (deterministic gradient): the global vertex
+// of every (tet slot, corner) of the cell, in the streamed vertex order, -1 for padding.
 template <class IDX>
-void emit_tc(std::vector<uint8_t> &s, const Mesh &M, const Comp &C, int t0, int nt, int xbase_bytes, int64_t *stat, std::vector<float> *Bout) {
+void emit_tc(std::vector<uint8_t> &s, const Mesh &M, const Comp &C, int t0, int nt, int xbase_bytes, int64_t *stat, std::vector<float> *Bout,
+             std::vector<int32_t> *Vout) {
   constexpr bool kGlobal = sizeof(IDX) == 4;
   constexpr size_t CELL = kGlobal ? kCellGlobal : kCellStaged;
   constexpr int TPL = kGlobal ? 1 : 2;
@@ -483,8 +485,9 @@ void emit_tc(std::vector<uint8_t> &s, const Mesh &M, const Comp &C, int t0, int 
   // bank groups in each of its 4 gathers (greedy over the 24 permutations).
   static const uint8_t kPerm[24][4] = {{0,1,2,3},{0,1,3,2},{0,2,1,3},{0,2,3,1},{0,3,1,2},{0,3,2,1},{1,0,2,3},{1,0,3,2},{1,2,0,3},{1,2,3,0},{1,3,0,2},{1,3,2,0},
                                        {2,0,1,3},{2,0,3,1},{2,1,0,3},{2,1,3,0},{2,3,0,1},{2,3,1,0},{3,0,1,2},{3,0,2,1},{3,1,0,2},{3,1,2,0},{3,2,0,1},{3,2,1,0}};
-  size_t bo = 0;
+  size_t bo = 0, vo = 0;
   if (Bout) { bo = Bout->size(); Bout->resize(bo + size_t(3) * 32 * TPL * 4, 0.f); }   // [row][lane*TPL + k] float4
+  if (Vout) { vo = Vout->size(); Vout->resize(vo + size_t(32) * TPL * 4, -1); }       // [lane*TPL + k][corner]
   // choose the vertex order of every tet: min-conflicts over each group of 8 lanes x one tet slot
   std::vector<uint8_t> perm_of(size_t(nt), 0);
   if (!kGlobal) {
@@ -566,6 +569,8 @@ void emit_tc(std::vector<uint8_t> &s, const Mesh &M, const Comp &C, int t0, int 
     for (int c = 0; c < 4; ++c)
       put<IDX>(s, o + ((size_t(l) * TPL + k) * 4 + c) * sizeof(IDX), kGlobal ? IDX(v[c]) : IDX(xbase_bytes + C.pos[M.local_of[v[c]]] * 16));
     put<float>(s, o + DOFF + (size_t(l) * TPL + k) * 4, float(1.0 / det));
+    if (Vout)
+      for (int c = 0; c < 4; ++c) (*Vout)[vo + size_t(i) * 4 + c] = v[c];
     if (Bout)
       for (int r = 0; r < 3; ++r)
         for (int c = 0; c < 3; ++c) (*Bout)[bo + (size_t(r) * 32 * TPL + size_t(l) * TPL + k) * 4 + c] = float(B[3 * r + c]);
@@ -891,11 +896,13 @@ struct CtaStats {
   std::string err;
 };
 
-// The streams of CTA b's warps (streams[w]; AMIPS: their rest inverses rest_inv[w]) and the CTA's entries of P.wseg.
+// The streams of CTA b's warps (streams[w]; AMIPS: their rest inverses rest_inv[w]; deterministic gradient: their tet
+// corners' vertices tet_verts[w]) and the CTA's entries of P.wseg.
 // Row blocks (longest first) and then tet cells go to the least loaded warp; loads carry over the CTA's segments,
 // which balances every warp's whole stream.
 void emit_cta(const Mesh &M, const std::vector<Comp> &comps, const std::vector<Seg> &segs, int ring_cells, int b,
-              HostPlan &P, std::vector<uint8_t> *streams, std::vector<float> *rest_inv, CtaStats &ES) {
+              HostPlan &P, std::vector<uint8_t> *streams, std::vector<float> *rest_inv, std::vector<int32_t> *tet_verts,
+              CtaStats &ES) {
   const bool GLOBAL = P.mode_global != 0;
   const int NW = P.nw;
   const int TPC = GLOBAL ? 32 : 64;                        // tets per tet cell
@@ -954,8 +961,9 @@ void emit_cta(const Mesh &M, const std::vector<Comp> &comps, const std::vector<S
       for (int k = 0; k < tc_cnt[w]; ++k) {
         const int nt = std::min(TPC, g.t1 - tnext);
         std::vector<float> *bo = rest_inv ? &rest_inv[w] : nullptr;
-        if (GLOBAL) emit_tc<uint32_t>(st, M, C, tnext, nt, 0, nullptr, bo);
-        else emit_tc<uint16_t>(st, M, C, tnext, nt, xbase_bytes, ES.twf, bo);
+        std::vector<int32_t> *vo = tet_verts ? &tet_verts[w] : nullptr;
+        if (GLOBAL) emit_tc<uint32_t>(st, M, C, tnext, nt, 0, nullptr, bo, vo);
+        else emit_tc<uint16_t>(st, M, C, tnext, nt, xbase_bytes, ES.twf, bo, vo);
         tnext += nt;
       }
       if (rb_of_warp[w].size() > 0xFFFF || tc_cnt[w] > 0xFFFF) { ES.err = "segment too large for the stream descriptors"; ES.rc = TSB_E_INVALID; return; }
@@ -968,16 +976,19 @@ void emit_cta(const Mesh &M, const std::vector<Comp> &comps, const std::vector<S
   }
 }
 
-// Every CTA's warp streams (wstream[b * nw + w]; AMIPS, when wB is not empty: the rest inverses in wB alike).
+// Every CTA's warp streams (wstream[b * nw + w]; AMIPS, when wB is not empty: the rest inverses in wB alike;
+// deterministic gradient, when wV is not empty: the tet corners' vertices in wV alike).
 // CTAs are independent and emitted in parallel; the first failing CTA's error is reported.
 int emit_ctas(const Mesh &M, const std::vector<Comp> &comps, const std::vector<Seg> &segs, int ring_cells, int nth,
-              HostPlan &P, std::vector<std::vector<uint8_t>> &wstream, std::vector<std::vector<float>> &wB, std::string &err) {
+              HostPlan &P, std::vector<std::vector<uint8_t>> &wstream, std::vector<std::vector<float>> &wB,
+              std::vector<std::vector<int32_t>> &wV, std::string &err) {
   const size_t NW = size_t(P.nw);
   P.wseg.assign(segs.size() * NW * 2, 0);
   std::vector<CtaStats> stats(P.grid);
   parallel_for(size_t(P.grid), 1, nth, [&](size_t b0, size_t b1) {
     for (size_t b = b0; b < b1; ++b)
-      emit_cta(M, comps, segs, ring_cells, int(b), P, &wstream[b * NW], wB.empty() ? nullptr : &wB[b * NW], stats[b]);
+      emit_cta(M, comps, segs, ring_cells, int(b), P, &wstream[b * NW], wB.empty() ? nullptr : &wB[b * NW],
+               wV.empty() ? nullptr : &wV[b * NW], stats[b]);
   });
   for (const CtaStats &e : stats) {
     if (e.rc != TSB_OK) { err = e.err; return e.rc; }
@@ -988,12 +999,12 @@ int emit_ctas(const Mesh &M, const std::vector<Comp> &comps, const std::vector<S
   return TSB_OK;
 }
 
-// The plan's byte stream (the warp streams in (CTA, warp) order) and its descriptors; AMIPS: the rest inverses in
-// the same order and the first tet cell of every (segment, warp).
-int concat_streams(const std::vector<std::vector<uint8_t>> &wstream, const std::vector<std::vector<float>> &wB, int nth,
-                   HostPlan &P, std::string &err) {
+// The plan's byte stream (the warp streams in (CTA, warp) order) and its descriptors; AMIPS or deterministic
+// gradient (number_cells): the first tet cell of every (segment, warp), and AMIPS: the rest inverses in that order.
+int concat_streams(const std::vector<std::vector<uint8_t>> &wstream, const std::vector<std::vector<float>> &wB,
+                   bool number_cells, int nth, HostPlan &P, std::string &err) {
   const int G = P.grid, NW = P.nw;
-  if (!wB.empty()) {
+  if (number_cells) {
     P.wtc0.assign(P.segs.size() * NW, 0);
     const size_t per_cell = size_t(3) * (P.mode_global ? 32 : 64) * 4;
     size_t cells = 0;
@@ -1003,10 +1014,12 @@ int concat_streams(const std::vector<std::vector<uint8_t>> &wstream, const std::
           P.wtc0[size_t(sgi) * NW + w] = int32_t(cells);
           cells += P.wseg[(size_t(sgi) * NW + w) * 2 + 1];
         }
-        const auto &v = wB[size_t(b) * NW + w];
-        P.Bt.insert(P.Bt.end(), v.begin(), v.end());
+        if (!wB.empty()) {
+          const auto &v = wB[size_t(b) * NW + w];
+          P.Bt.insert(P.Bt.end(), v.begin(), v.end());
+        }
       }
-    if (P.Bt.size() != cells * per_cell) { err = "internal: AMIPS rest-inverse blocks out of step with the tet cells"; return TSB_E_INVALID; }
+    if (!wB.empty() && P.Bt.size() != cells * per_cell) { err = "internal: AMIPS rest-inverse blocks out of step with the tet cells"; return TSB_E_INVALID; }
   }
   size_t total = 0;
   for (const auto &st : wstream) total += st.size();
@@ -1025,6 +1038,44 @@ int concat_streams(const std::vector<std::vector<uint8_t>> &wstream, const std::
     for (size_t i = b; i < e; ++i)
       if (!wstream[i].empty()) std::memcpy(dst + offs[i], wstream[i].data(), wstream[i].size());
   });
+  return TSB_OK;
+}
+
+// The deterministic gather's vertex -> (tet slot, corner) lists (HostPlan::det_*).  wV holds the corners' vertices of
+// every tet cell in (CTA, warp, segment) order, the order in which concat_streams numbers the cells, so entry i of
+// the concatenation is slot i / 4, corner i % 4; visiting the entries in that order sorts every list.
+int det_lists(const std::vector<Comp> &comps, const std::vector<std::vector<int32_t>> &wV, HostPlan &P, std::string &err) {
+  size_t total = 0;
+  for (const auto &v : wV) total += v.size();
+  const size_t slots = size_t(P.n_tetcells) * (P.mode_global ? 32 : 64);
+  if (total != 4 * slots) { err = "internal: tet-corner lists out of step with the tet cells"; return TSB_E_INVALID; }
+  if (total > 0xFFFFFFFFull || size_t(P.nele) * 4 > 0x7FFFFFFFull) { err = "too many tets for the deterministic gradient's lists"; return TSB_E_INVALID; }
+  const int NC = int(comps.size());
+  std::vector<int32_t> row_of(size_t(P.n), -1);
+  P.det_comp_row.assign(size_t(NC) + 1, 0);
+  P.det_vert.clear();
+  P.det_chunk.clear();
+  for (int c = 0; c < NC; ++c) {
+    const int32_t r0 = int32_t(P.det_vert.size());
+    for (const int32_t v : comps[c].verts) { row_of[v] = int32_t(P.det_vert.size()); P.det_vert.push_back(v); }
+    P.det_comp_row[c + 1] = int32_t(P.det_vert.size());
+    for (int32_t r = r0; r < P.det_comp_row[c + 1]; r += kDetChunkRows) { P.det_chunk.push_back(c); P.det_chunk.push_back(r); }
+  }
+  const size_t rows = P.det_vert.size();
+  P.det_rowptr.assign(rows + 1, 0);
+  for (const auto &wv : wV)
+    for (const int32_t v : wv)
+      if (v >= 0) ++P.det_rowptr[row_of[v] + 1];
+  for (size_t r = 0; r < rows; ++r) P.det_rowptr[r + 1] += P.det_rowptr[r];
+  if (P.det_rowptr[rows] != 4 * P.nele) { err = "internal: the streamed tets are not the mesh's tets"; return TSB_E_INVALID; }
+  P.det_ent.assign(size_t(P.det_rowptr[rows]), 0);
+  std::vector<int32_t> cur(P.det_rowptr.begin(), P.det_rowptr.end() - 1);
+  uint32_t ent = 0;
+  for (const auto &wv : wV)
+    for (const int32_t v : wv) {
+      if (v >= 0) P.det_ent[size_t(cur[row_of[v]]++)] = ent;
+      ++ent;
+    }
   return TSB_OK;
 }
 
@@ -1052,8 +1103,10 @@ int build_plan(const float *rest, const int32_t *tets, int32_t n, int32_t nele, 
   staging_tables(M, comps, segs, P);
   std::vector<std::vector<uint8_t>> wstream(size_t(P.grid) * P.nw);
   std::vector<std::vector<float>> wB(cfg.enable_amips ? wstream.size() : 0);
-  if ((rc = emit_ctas(M, comps, segs, cfg.ring_cells, nth, P, wstream, wB, err)) != TSB_OK) return rc;
-  return concat_streams(wstream, wB, nth, P, err);
+  std::vector<std::vector<int32_t>> wV(cfg.deterministic ? wstream.size() : 0);
+  if ((rc = emit_ctas(M, comps, segs, cfg.ring_cells, nth, P, wstream, wB, wV, err)) != TSB_OK) return rc;
+  if ((rc = concat_streams(wstream, wB, cfg.enable_amips || cfg.deterministic, nth, P, err)) != TSB_OK) return rc;
+  return cfg.deterministic ? det_lists(comps, wV, P, err) : TSB_OK;
 }
 
 }  // namespace tsb

@@ -55,6 +55,7 @@ constexpr int kMaxHalfVerts = 1023;                    // 64 * vh <= 65535 (16-b
 constexpr int kMaxStagedVerts = 2047;                  // 32 * nv <= 65535
 constexpr int kMaxWarps = 16;
 constexpr int kCellsPerChunk = 6;                      // cells per TMA bulk copy = per ring slot (tsb_options_t.ring_slots)
+constexpr int kDetChunkRows = 256;                     // deterministic gather: vertex rows per chunk (= threads per CTA)
 
 // One segment (32 bytes).  comp indexes the per-component "rows done" counters; vbase >= 0 when the
 // component's vertices are contiguous in the caller's numbering (then global id = vbase + local id),
@@ -85,6 +86,7 @@ struct PlanConfig {
   float tet_cost = 3.0f;        // cost of one tet relative to one operator entry (CTA-level cut)
   int32_t ring_cells = 2 * kCellsPerChunk;   // cells one warp's TMA ring holds (decides the latency / streaming regime)
   int32_t enable_amips = 0;     // also emit the per-tet rest inverses (AMIPS term; 48 B per tet)
+  int32_t deterministic = 0;    // also emit the vertex -> (tet slot, corner) lists of the deterministic gather (16 B per tet)
 };
 
 // std::allocator whose construct() default-initialises: resize() of a byte vector does not zero-fill
@@ -130,7 +132,15 @@ struct HostPlan {
   // AMIPS only: rest inverses B = Dm^-1 of every streamed tet (in its streamed vertex order), one block of
   // 3 rows x (tets per cell) float4 per tet cell, and the first tet cell of every (segment, warp)
   std::vector<float> Bt;
-  std::vector<int32_t> wtc0;
+  std::vector<int32_t> wtc0;        // also emitted for the deterministic gradient (it numbers the tet slots)
+  // Deterministic gradient only.  Tet slot of a streamed tet: (wtc0[s, w] + tc) * (tets per cell) + lane * TPL + t.
+  // Rows are the vertices of every component (components in order, vertices ascending); row r lists the entries
+  // slot * 4 + corner of the non-padding tets whose streamed corner is det_vert[r], ascending.  Orphans have no row.
+  std::vector<int32_t> det_rowptr;  // [rows + 1]
+  std::vector<int32_t> det_vert;    // [rows] global vertex id
+  std::vector<uint32_t> det_ent;    // [4 * nele] slot * 4 + corner
+  std::vector<int32_t> det_comp_row;   // [n_components + 1] first row of every component
+  std::vector<int32_t> det_chunk;   // [2 * chunks] (component, first row) of every run of <= kDetChunkRows rows
 };
 
 // Returns 0 on success, TSB_E_* otherwise (message in err).

@@ -16,16 +16,16 @@ extern "C" {
 
 const char *tsbdbg_last_error() { return g_err.c_str(); }
 
-/* tsbdbg_build plus ring_cells (the ring tsb_create requests: ring_slots * kCellsPerChunk; 0 = the default) and
-   enable_amips (emit the AMIPS rest inverses "Bt" / "wtc0") */
-int tsbdbg_build_ex(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele, int32_t nw, int32_t grid,
-                    int32_t laplacian_scale, int32_t force_global, int32_t vh_cap, int32_t area_cap, float tet_cost,
-                    int32_t ring_cells, int32_t enable_amips, tsbdbg_plan **out) {
+/* tsbdbg_build_ex plus deterministic (emit the deterministic gather's lists "det_*" and the tet-cell numbering "wtc0") */
+int tsbdbg_build_det(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele, int32_t nw, int32_t grid,
+                     int32_t laplacian_scale, int32_t force_global, int32_t vh_cap, int32_t area_cap, float tet_cost,
+                     int32_t ring_cells, int32_t enable_amips, int32_t deterministic, tsbdbg_plan **out) {
   if (!out) return TSB_E_INVALID;
   *out = nullptr;
   tsb::PlanConfig pc;
   pc.nw = nw; pc.grid = grid; pc.laplacian_scale = laplacian_scale; pc.force_global = force_global;
   pc.enable_amips = enable_amips ? 1 : 0;
+  pc.deterministic = deterministic ? 1 : 0;
   if (vh_cap > 0) pc.vh_cap = vh_cap;
   if (area_cap > 0) pc.area_cap = area_cap;
   if (tet_cost > 0) pc.tet_cost = tet_cost;
@@ -35,6 +35,15 @@ int tsbdbg_build_ex(const float *rest_xyz, const int32_t *tets, int32_t n, int32
   if (rc != TSB_OK) { delete d; return rc; }
   *out = d;
   return TSB_OK;
+}
+
+/* tsbdbg_build plus ring_cells (the ring tsb_create requests: ring_slots * kCellsPerChunk; 0 = the default) and
+   enable_amips (emit the AMIPS rest inverses "Bt" / "wtc0") */
+int tsbdbg_build_ex(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele, int32_t nw, int32_t grid,
+                    int32_t laplacian_scale, int32_t force_global, int32_t vh_cap, int32_t area_cap, float tet_cost,
+                    int32_t ring_cells, int32_t enable_amips, tsbdbg_plan **out) {
+  return tsbdbg_build_det(rest_xyz, tets, n, nele, nw, grid, laplacian_scale, force_global, vh_cap, area_cap, tet_cost,
+                          ring_cells, enable_amips, 0, out);
 }
 
 int tsbdbg_build(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele, int32_t nw, int32_t grid,
@@ -52,6 +61,8 @@ int tsbdbg_array(tsbdbg_plan *d, const char *name, const void **ptr, int64_t *co
   ARR("stream", P.stream, 1) ARR("X4", P.X4, 4) ARR("vlist", P.vlist, 4) ARR("segs", P.segs, 4) ARR("cta_seg", P.cta_seg, 4)
   ARR("wdesc", P.wdesc, 4) ARR("wseg", P.wseg, 2) ARR("orphans", P.orphans, 4) ARR("pos16", P.pos16, 2) ARR("pos_gid", P.pos_gid, 4)
   ARR("Bt", P.Bt, 4) ARR("wtc0", P.wtc0, 4)
+  ARR("det_rowptr", P.det_rowptr, 4) ARR("det_vert", P.det_vert, 4) ARR("det_ent", P.det_ent, 4)
+  ARR("det_comp_row", P.det_comp_row, 4) ARR("det_chunk", P.det_chunk, 4)
 #undef ARR
   return TSB_E_INVALID;
 }

@@ -48,15 +48,16 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
     """``SmoothnessBarrierEnergy(tet_v, tet_f, FLAGS)`` (``energies/smooth_barrier.py:34-67``).
 
     ``tet_v``: numpy [n,3] REST positions; ``tet_f``: numpy [nele,4]; ``FLAGS``: mapping or object
-    with ``smooth_eng_coeff``, ``barrier_coeff``, ``increase_order_iter`` (``config/gso.yaml:9-11``).
+    with ``smooth_eng_coeff``, ``barrier_coeff``, ``increase_order_iter`` (``config/gso.yaml:9-11``), and optionally
+    ``deterministic`` (default False): a bitwise repeatable gradient (``TetSpheres(..., deterministic=True)``).
     """
 
     def __init__(self, tet_v, tet_f, FLAGS) -> None:
         super().__init__()
         v_flat = np.asarray(tet_v).flatten().astype(np.float32)
         f_flat = np.asarray(tet_f).flatten().astype(np.int32)
-        self.tet_sp = tet_spheres_ext.TetSpheres(v_flat, f_flat)
         self.FLAGS = SimpleNamespace(**FLAGS) if isinstance(FLAGS, dict) else FLAGS
+        self.tet_sp = tet_spheres_ext.TetSpheres(v_flat, f_flat, deterministic=bool(getattr(self.FLAGS, "deterministic", False)))
         self.smooth_eng_func = SmoothnessBarrierFunc          # the reference instantiates it; .apply is static
 
     def coeff_scheduler(self, it):

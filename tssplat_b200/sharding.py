@@ -65,17 +65,21 @@ class ShardedEnergy:
 
     ``energy_grad(x_local)`` returns (energy[3] device tensor holding the GLOBAL sums once
     ``wait()`` has been called, local gradient [n_local,3]).
+
+    ``deterministic=True`` makes each rank's gradient and local energies bitwise repeatable
+    (``TetSpheres(..., deterministic=True)``); the NCCL all-reduce of the energies is outside that guarantee.
     """
 
     def __init__(self, pack: TetPack, rank: Optional[int] = None, world_size: Optional[int] = None,
-                 device=None, group=None, warps_per_cta: int = 0):
+                 device=None, group=None, warps_per_cta: int = 0, deterministic: bool = False):
         from . import tet_spheres_ext as ext   # needs the CUDA library + a GPU
         self.group = group
         self.rank = dist.get_rank(group) if rank is None else rank
         self.world_size = dist.get_world_size(group) if world_size is None else world_size
         self.local, self.sphere_range = shard_pack(pack, self.rank, self.world_size)
         self.tet_sp = ext.TetSpheres(self.local.verts.reshape(-1), self.local.tets.reshape(-1),
-                                     device=device, warps_per_cta=warps_per_cta) if self.local.nele else None
+                                     device=device, warps_per_cta=warps_per_cta,
+                                     deterministic=deterministic) if self.local.nele else None
         self._work = None
         if device is None:
             device = torch.device("cuda", torch.cuda.current_device())

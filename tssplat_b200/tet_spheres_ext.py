@@ -58,10 +58,15 @@ class TetSpheres:
     positions), ``elements`` 1-D C-contiguous int32 of length 4*nele, 0-based
     (``tet_spheres.cpp:234-258``).  ``TetSpheres(filename)`` loads a ``.veg`` file
     (``tet_spheres.cpp:108-117``).
+
+    ``deterministic=True``: the gradient is bitwise repeatable also with inverted tets and the AMIPS term (a second
+    launch adds the tets' contributions in a fixed order; see ``tsb_energy_grad`` in the header).  Callers that set
+    ``torch.use_deterministic_algorithms(True)`` should pass it: the flag is not followed automatically.
     """
 
     def __init__(self, vertices, elements=None, *, device=None, warps_per_cta: int = 0,
-                 laplacian_scale: int = 0, force_global: bool = False, ring_slots: int = 0, enable_amips: bool = False):
+                 laplacian_scale: int = 0, force_global: bool = False, ring_slots: int = 0, enable_amips: bool = False,
+                 deterministic: bool = False):
         self._h = None
         if isinstance(vertices, (str, bytes)) and elements is None:
             v, t = load_veg(vertices if isinstance(vertices, str) else vertices.decode())
@@ -88,7 +93,7 @@ class TetSpheres:
         torch.cuda.init()
         opt = _capi.tsb_options_t(warps_per_cta=int(warps_per_cta), laplacian_scale=int(laplacian_scale),
                                   ring_slots=int(ring_slots), force_global=int(bool(force_global)),
-                                  enable_amips=int(bool(enable_amips)))
+                                  enable_amips=int(bool(enable_amips)), deterministic=int(bool(deterministic)))
         h = C.c_void_p()
         rc = _capi.lib.tsb_create(vertices.ctypes.data, elements.ctypes.data, vertices.size // 3,
                                   elements.size // 4, C.byref(opt), self.device.index, C.byref(h))
@@ -100,6 +105,7 @@ class TetSpheres:
         self.n = int(info.n)
         self.nele = int(info.nele)
         self.n3 = 3 * self.n
+        self.deterministic = bool(deterministic)
         self._cache_key = None
         self._cache_grad: Optional[torch.Tensor] = None
         # energies of the last 32 launches (a ring, so a loss tensor stays valid while it is being logged)
