@@ -3,9 +3,10 @@
     python tools/trace_phases.py build          # here (no GPU): nvcc -> tssplat_b200/libtssplat_b200_trace.so
     python tools/trace_phases.py run [S ...]    # on the GPU box
 
-Thread 0 of every CTA stamps clock64 at: 1 entry, 2 prologue done (TMA issued), 3 after
+Thread 0 of every CTA stamps clock64 at: 1 entry, 2 prologue done (first TMA chunk issued), 3 after
 griddepcontrol.wait, 4 first component staged, 5 warp-0 rows of first segment done, 6 warp-0 tets done,
-7 all segments done, 8 CTA energy barrier, 9 ticket atomic returned, 10 exit; 0/11 = globaltimer."""
+7 all segments done, 8 CTA energy barrier, 9 ticket atomic returned, 10 exit; 0/11 = globaltimer.  Lane 0 of warp w
+stamps clock64 in slot 16 + w when its last chunk wait returns (the wait for the last chunk of its stream)."""
 import ctypes as C
 import os
 import subprocess
@@ -14,6 +15,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 TRACE_LIB = os.path.join(ROOT, "tssplat_b200", "libtssplat_b200_trace.so")
+SLOTS = 32                    # tsb_kernels.cuh kTraceSlots: 16 phase stamps, then one per warp
 
 
 def build():
@@ -47,7 +49,7 @@ def run(sizes):
                 for _ in range(20):
                     lib.tsb_energy_grad(sp._h, x.data_ptr(), 2e-4 / S, 2e-4, 2, 1.0, None, energy.data_ptr(), grad.data_ptr(), st.cuda_stream)
                 st.synchronize()
-            tr = np.zeros((G, 16), dtype=np.uint64)
+            tr = np.zeros((G, SLOTS), dtype=np.uint64)
             lib.tsb_trace_read(sp._h, tr.ctypes.data, tr.size)
             tr = tr.astype(np.int64)
             dur_ns = tr[:, 11].max() - tr[:, 0].min()
@@ -71,6 +73,17 @@ def run(sizes):
                 nseg = np.diff(pl["cta_seg"].reshape(G, 2), axis=1).ravel()
                 ws_ = pl["wseg"].reshape(-1, NWp, 2)
                 rbs = np.array([ws_[a:b, :, 0].sum() for a, b in pl["cta_seg"].reshape(G, 2)])
+                # CTAs whose slowest warp has more cells than its ring holds: that warp waits on a ring refill
+                big = cells.max(1) > 2 * 6
+                busy = cells.sum(1) > 0
+                wmax = cells.argmax(1)
+                lw = tr[np.arange(G), 16 + wmax]
+                last = np.where(lw > 0, (lw - tr[:, 3]) / 1.965, np.nan)    # its last chunk wait, after the gdc.wait
+                for nm, m in (("slowest warp > 12 cells", big & busy), ("slowest warp <= 12 cells", ~big & busy)):
+                    if m.any():
+                        lm = last[m][np.isfinite(last[m])]      # empty when the warp's whole stream is one chunk
+                        print(f"    {nm:25s}: {m.sum():3d} CTAs  post-wait median {np.median(post[m]):.0f} max {post[m].max():.0f} ns  " +
+                              (f"last chunk wait of that warp median {np.median(lm):.0f} max {lm.max():.0f} ns after gdc.wait" if lm.size else "no chunk wait"))
                 for k in sorted(set(nseg.tolist())):
                     m = nseg == k
                     print(f"    CTAs with {k} segment(s): {m.sum():3d}  post-wait mean {post[m].mean():.0f} ns  total cells {cells[m].sum(1).mean():.0f}  "

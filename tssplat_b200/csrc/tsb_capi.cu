@@ -198,7 +198,7 @@ int tsb_create(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t ne
   TSB_TRY(alloc_zero(h, size_t(plan.n_components), &kp.done));
   TSB_TRY(upload(h, std::vector<unsigned long long>(size_t(plan.grid) * 4, tsb::kEnergySentinel), kp.cta_energy, 2));
 #ifdef TSB_TRACE
-  TSB_TRY(alloc_zero(h, size_t(plan.grid) * 16, &kp.trace));
+  TSB_TRY(alloc_zero(h, size_t(plan.grid) * tsb::kTraceSlots, &kp.trace));
 #endif
   if (plan.mode_global) {
     TSB_TRY(alloc_zero(h, size_t(plan.n), &kp.u4g));
@@ -390,11 +390,11 @@ int tsb_adam_uniform_step(float *p_dev, const float *grad_dev, float *g1_dev, fl
 }
 
 #ifdef TSB_TRACE
-/* profiling build only: copy the [grid][16] phase stamps of the last launch to the host */
+/* profiling build only: copy the [grid][kTraceSlots] phase stamps of the last launch to the host */
 int tsb_trace_read(tsb_handle_t h, unsigned long long *out, int64_t count) {
   if (!h || !out) return TSB_E_INVALID;
   DeviceGuard guard(h->device);
-  const int64_t have = int64_t(h->info.grid) * 16;
+  const int64_t have = int64_t(h->info.grid) * tsb::kTraceSlots;
   return cudaMemcpy(out, h->kp.trace, size_t(std::min(count, have)) * 8, cudaMemcpyDeviceToHost) == cudaSuccess ? TSB_OK : TSB_E_CUDA;
 }
 #endif

@@ -19,8 +19,9 @@
 //
 // Execution.  Persistent CTAs (1 per SM x 16 warps, or 2 x 8).  Every warp owns a private byte
 // stream of operator rows and tet blocks (tsb_plan.h) and pulls it through a private shared-memory
-// ring with TMA bulk copies (cp.async.bulk + mbarrier complete_tx), issued by its lane 0, first
-// chunks before griddepcontrol.wait: plan data streams from HBM while the previous kernel drains.
+// ring with TMA bulk copies (cp.async.bulk + mbarrier complete_tx), issued by its lane 0: the first
+// chunk before griddepcontrol.wait (plan data streams from HBM while the previous kernel drains), the rest of the
+// ring once the loads of x have been issued, so that x does not queue behind them.
 // Per segment the CTA stages u and x of the whole component in shared memory (float4 each; the next
 // component is prefetched through registers), so all gathers are LDS.128.  Energies: per-lane fp64
 // partials -> per-CTA pair -> last-arriving CTA folds them in fixed order (deterministic).
@@ -54,10 +55,11 @@ constexpr int align_up(int v, int a) { return (v + a - 1) / a * a; }
 constexpr int kMaxSlots = 8;
 constexpr unsigned long long kSentinel = kEnergySentinel;   // "no partial yet" marker in cta_energy (a NaN payload)
 
-// Profiling build only (-DTSB_TRACE, tools/trace_phases.py): thread 0 of every CTA stamps its phases.
+// Profiling build only (-DTSB_TRACE, tools/trace_phases.py): thread 0 of every CTA stamps its phases in slots 0..15 of
+// the CTA's kTraceSlots, lane 0 of warp w the return of its last chunk wait in slot 16 + w.
 #ifdef TSB_TRACE
 __device__ __forceinline__ unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
-#define TSB_STAMP(i) do { if (tid == 0 && p.trace) p.trace[blockIdx.x * 16 + (i)] = (i) == 0 ? gtime() : (unsigned long long)clock64(); } while (0)
+#define TSB_STAMP(i) do { if (tid == 0 && p.trace) p.trace[blockIdx.x * kTraceSlots + (i)] = (i) == 0 ? gtime() : (unsigned long long)clock64(); } while (0)
 #else
 #define TSB_STAMP(i) do { } while (0)
 #endif
@@ -107,6 +109,9 @@ struct WarpStream {
   uint32_t chunk_bytes, cpc, nslot;
   uint32_t cc, slot, phase, cells_left;
   int lane;
+#ifdef TSB_TRACE
+  unsigned long long *trace_last;  // lane 0: clock64 when the warp's latest chunk wait returned
+#endif
 
   __device__ __forceinline__ void request(uint32_t smem_dst, uint32_t bar) {   // lane 0 only
     const uint32_t bytes = min(chunk_bytes, bytes_left);
@@ -122,6 +127,13 @@ struct WarpStream {
     do {
       asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}" : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
     } while (!ok);
+  }
+  // Lane 0 requests the chunk of slot 0 before griddepcontrol.wait and those of the other slots here, once the CTA's
+  // x loads have been issued: with the plan HBM-cold, the loads that stage x would otherwise queue behind every
+  // warp's whole ring of plan data, although the warp needs only its first chunk before the staged x.
+  __device__ __forceinline__ void request_rest() {
+    if (lane == 0)
+      for (uint32_t i = 1; i < nslot && bytes_left; ++i) request(smem_u32(ring) + i * chunk_bytes, bars + i * 8);
   }
   __device__ __forceinline__ void begin() {       // first chunk has landed
     if (cells_left) wait(bars, 0);
@@ -139,6 +151,9 @@ struct WarpStream {
       if (lane == 0 && bytes_left) request(smem_u32(cell) - chunk_bytes, bars + slot * 8);
       if (++slot == nslot) { slot = 0; cell = ring; phase ^= 1u; }
       if (cells_left) wait(bars + slot * 8, phase);
+#ifdef TSB_TRACE
+      if (cells_left && trace_last) *trace_last = (unsigned long long)clock64();
+#endif
     }
   }
 };
@@ -173,12 +188,15 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
     ws.cpc = uint32_t(p.cells_per_chunk);
     ws.chunk_bytes = ws.cpc * CELL;
     ws.nslot = uint32_t(p.ring_slots);
+#ifdef TSB_TRACE
+    ws.trace_last = (lane == 0 && p.trace) ? p.trace + blockIdx.x * kTraceSlots + 16 + warp : nullptr;
+#endif
     ws.cell = ws.ring;
     ws.cc = 0; ws.slot = 0; ws.phase = 0; ws.lane = lane;
     if (lane == 0) {
       for (uint32_t i = 0; i < ws.nslot; ++i) asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(ws.bars + i * 8), "r"(1) : "memory");
       mbar_fence_init();
-      for (uint32_t i = 0; i < ws.nslot && ws.bytes_left; ++i) ws.request(smem_u32(ws.ring) + i * ws.chunk_bytes, ws.bars + i * 8);
+      if (ws.bytes_left) ws.request(smem_u32(ws.ring), ws.bars);   // slot 0; the others: request_rest()
     }
     __syncwarp();
   }
@@ -250,10 +268,8 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
       }
     }
   };
-  auto store_staged = [&](const SegHdr &h, int li) {
+  auto store_staged_ref = [&](const SegHdr &h, int li, const float (&pr)[3]) {
     float4 *ub = stage + ubase_of(h, li), *xb = stage + xbase_of(h, li);
-    float pr[3];                            // loaded here, not with px: kept out of the segment loop's live registers
-    load_ref(h, pr);
 #pragma unroll
     for (int k = 0; k < SV; ++k) {
       const int v = tid + k * NT;
@@ -263,6 +279,11 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
         xb[pos] = make_float4(px[k][0], px[k][1], px[k][2], 0.f);
       }
     }
+  };
+  auto store_staged = [&](const SegHdr &h, int li) {
+    float pr[3];                            // loaded here, not with px: kept out of the segment loop's live registers
+    load_ref(h, pr);
+    store_staged_ref(h, li, pr);
   };
   auto stage_direct = [&](const SegHdr &h, int li) {   // any size, no register prefetch
     float4 *ub = stage + ubase_of(h, li), *xb = stage + xbase_of(h, li);
@@ -287,11 +308,15 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
       if (cs.x + 1 < cs.y && !hcur.whole) eager2 = !h1.whole;
       if (hcur.whole) {
         stage_direct(hcur, 0);
+        ws.request_rest();
       } else if (!eager2) {
-        load_x(hcur); store_staged(hcur, 0);
+        float pr[3];
+        load_x(hcur); load_ref(hcur, pr);
+        ws.request_rest();
+        store_staged_ref(hcur, 0, pr);
       } else {
         // both components' loads in flight together (second register set), then both stores
-        float qx[SV][3], qr[3];
+        float qx[SV][3], qr[3], pr[3];
         float4 qX[SV];
 #pragma unroll
         for (int k = 0; k < SV; ++k) {
@@ -308,7 +333,9 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
             qx[k][0] = __ldcg(p.x + 3 * gi); qx[k][1] = __ldcg(p.x + 3 * gi + 1); qx[k][2] = __ldcg(p.x + 3 * gi + 2);
           }
         }
-        store_staged(hcur, 0);
+        load_ref(hcur, pr);
+        ws.request_rest();
+        store_staged_ref(hcur, 0, pr);
         float4 *ub = stage + ubase_of(h1, 1), *xb = stage + xbase_of(h1, 1);
 #pragma unroll
         for (int k = 0; k < SV; ++k) {
@@ -320,10 +347,13 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
           }
         }
       }
+    } else {
+      ws.request_rest();
     }
     __syncthreads();
     TSB_STAMP(4);
   } else {
+    ws.request_rest();
     __syncthreads();      // segment tables visible
   }
   ws.begin();
@@ -401,7 +431,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
         left -= n;
       }
 #ifdef TSB_TRACE
-      if (s == cs.x && rb == 0) { TSB_STAMP(14); if (tid == 0 && p.trace) p.trace[blockIdx.x * 16 + 15] = len4 | (uint32_t(wseg.x) << 16) | (uint32_t(wseg.y) << 24); }
+      if (s == cs.x && rb == 0) { TSB_STAMP(14); if (tid == 0 && p.trace) p.trace[blockIdx.x * kTraceSlots + 15] = len4 | (uint32_t(wseg.x) << 16) | (uint32_t(wseg.y) << 24); }
 #endif
       float ax = sum2(AX), ay = sum2(AY), az = sum2(AZ);
       for (uint32_t o = 1; o < (1u << llog); o <<= 1) {   // the L lanes of a row are adjacent
@@ -666,7 +696,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
   }
   TSB_STAMP(10);
 #ifdef TSB_TRACE
-  if (tid == 0 && p.trace) p.trace[blockIdx.x * 16 + 11] = gtime();
+  if (tid == 0 && p.trace) p.trace[blockIdx.x * kTraceSlots + 11] = gtime();
 #endif
 }
 

@@ -48,9 +48,10 @@ struct KParams {
   unsigned long long *det_ballot;   // [tet cells] bit t * 32 + lane: the tet in slot lane * TPL + t contributed
   unsigned int *det_flag;       // [n_components] nonzero: a tet of the component contributed (the gather clears it)
 #ifdef TSB_TRACE
-  unsigned long long *trace;    // profiling build only: [grid][16] phase stamps
+  unsigned long long *trace;    // profiling build only: [grid][kTraceSlots] phase stamps
 #endif
 };
+constexpr int kTraceSlots = 16 + kMaxWarps;   // profiling build: 16 phase stamps of thread 0, then one per warp
 
 struct LaunchConfig {
   int nw;          // warps per CTA (8 or 16)
