@@ -129,6 +129,32 @@ int tsb_energy_grad(tsb_handle_t h, const float *x_dev, float c1, float c2, int3
 int tsb_energy_grad_ex(tsb_handle_t h, const float *x_dev, const tsb_terms_t *terms, float gradH,
                        const float *gradH_dev, float *energy_out_dev, float *grad_out_dev, void *stream);
 
+/* Geometry statistics of one connected component (= one tet-sphere), from tsb_energy_grad_spheres.  40 bytes. */
+typedef struct {
+  double smooth;        /* 1/2 u^T M u restricted to the component's rows (unweighted, like energy_out[1])     */
+  double barrier;       /* sum over its tets of max(-J,0)^order                                                 */
+  double amips;         /* sum of the AMIPS term over its J > 0 tets; 0 unless terms->c3 != 0                   */
+  float min_J;          /* smallest det F over its tets (the kernel's fp32 J, the value the barrier tests)      */
+  int32_t n_inverted;   /* tets with J < 0 (exactly the tets that contribute to the barrier)                    */
+  int32_t n_tets;       /* tets of the component                                                                 */
+  int32_t first_vertex; /* its lowest vertex id: identifies the component in the caller's numbering              */
+} tsb_sphere_stats_t;
+
+/* tsb_energy_grad_ex plus per-sphere statistics: the same launch (same argument checks, same energy_out_dev and
+ * grad_out_dev, which may be NULL) also writes one tsb_sphere_stats_t per connected component to spheres_out_dev
+ * (device memory, [info.n_components], required: NULL is TSB_E_INVALID).  Records are in component order, which is
+ * the order of the components' lowest vertex ids (so for spheres concatenated one after the other, record k is
+ * sphere k); vertices no tet references belong to no record.  Every record is rewritten by every call; no host
+ * sync.  The per-component sums are folded in fp64 in a fixed order, so the records are a pure function of (plan,
+ * x, order, c3 != 0): bitwise identical across launches and CUDA-graph replays, on default and deterministic
+ * handles, with or without grad_out_dev.  Summed over the components they give energy_out's terms up to fp64
+ * rounding; energy_out itself may differ from tsb_energy_grad_ex's by one fp32 ulp (the fp64 partials are summed
+ * per sphere first), and grad_out is computed exactly as there.
+ * Cost: per-segment warp reductions in the energy kernel plus one small kernel (DESIGN.md section 5). */
+int tsb_energy_grad_spheres(tsb_handle_t h, const float *x_dev, const tsb_terms_t *terms, float gradH,
+                            const float *gradH_dev, float *energy_out_dev, float *grad_out_dev,
+                            tsb_sphere_stats_t *spheres_out_dev, void *stream);
+
 /* Same computation for callers whose vertex positions live in HOST memory (e.g. a CPU-side
  * optimiser): copies x_host -> device, runs the fused launch, copies energy[3] and grad back,
  * asynchronously; the outputs are valid once `stream` has been synchronised and the host buffers

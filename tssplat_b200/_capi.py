@@ -17,7 +17,7 @@ TSB_OK, TSB_E_INVALID, TSB_E_MESH, TSB_E_CUDA, TSB_E_NOMEM = 0, -1, -2, -3, -4
 
 # every symbol include/tssplat_b200.h declares (tests check the library exports each one)
 EXPORTED_SYMBOLS = (
-    "tsb_create", "tsb_destroy", "tsb_last_error", "tsb_get_info", "tsb_energy_grad", "tsb_energy_grad_ex", "tsb_energy_grad_host", "tsb_scale",
+    "tsb_create", "tsb_destroy", "tsb_last_error", "tsb_get_info", "tsb_energy_grad", "tsb_energy_grad_ex", "tsb_energy_grad_spheres", "tsb_energy_grad_host", "tsb_scale",
     "tsb_grad_limit", "tsb_adam_uniform_step",
     "tsb_surface_create", "tsb_surface_destroy", "tsb_surface_last_error", "tsb_surface_forward", "tsb_surface_backward",
     "tsb_surface_extract", "tsb_free_host", "tsb_setup_last_error",
@@ -32,6 +32,11 @@ class tsb_options_t(C.Structure):
 
 class tsb_terms_t(C.Structure):
     _fields_ = [("c1", C.c_float), ("c2", C.c_float), ("order", C.c_int32), ("c3", C.c_float), ("reserved", C.c_int32 * 4)]
+
+
+class tsb_sphere_stats_t(C.Structure):
+    _fields_ = [("smooth", C.c_double), ("barrier", C.c_double), ("amips", C.c_double), ("min_J", C.c_float),
+                ("n_inverted", C.c_int32), ("n_tets", C.c_int32), ("first_vertex", C.c_int32)]
 
 
 class tsb_info_t(C.Structure):
@@ -66,6 +71,8 @@ def _load() -> C.CDLL:
     lib.tsb_energy_grad.argtypes = [vp, vp, f32, f32, i32, f32, vp, vp, vp, vp]
     lib.tsb_energy_grad_ex.restype = C.c_int
     lib.tsb_energy_grad_ex.argtypes = [vp, vp, C.POINTER(tsb_terms_t), f32, vp, vp, vp, vp]
+    lib.tsb_energy_grad_spheres.restype = C.c_int
+    lib.tsb_energy_grad_spheres.argtypes = [vp, vp, C.POINTER(tsb_terms_t), f32, vp, vp, vp, vp, vp]
     lib.tsb_energy_grad_host.restype = C.c_int
     lib.tsb_energy_grad_host.argtypes = [vp, vp, f32, f32, i32, f32, vp, vp, vp]
     lib.tsb_scale.restype = C.c_int

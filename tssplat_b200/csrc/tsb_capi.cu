@@ -10,6 +10,8 @@
 #include "tsb_kernels.cuh"
 #include "tsb_plan.h"
 
+static_assert(sizeof(tsb_sphere_stats_t) == 40, "tsb_sphere_stats_t must be 40 bytes");
+
 struct tsb_handle_s {
   int device = 0;
   tsb::KParams kp{};
@@ -25,6 +27,7 @@ struct tsb_handle_s {
   bool amips = false;
   bool det = false;             // deterministic gradient: DET energy kernel + det_gather_kernel
   tsb::DetParams dp{};
+  tsb::SphParams sp{};          // per-sphere statistics: the fold's tables (records: kp.sph_rec)
   tsb_info_t info{};
   std::vector<void *> allocs;
   std::string err;
@@ -196,6 +199,14 @@ int tsb_create(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t ne
     dp.tpl_log = plan.mode_global ? 0 : 1;
   }
   TSB_TRY(alloc_zero(h, size_t(plan.n_components), &kp.done));
+  // per-sphere statistics: 12 B per component of tables, 32 B per (segment, warp) of records
+  TSB_TRY(upload(h, plan.comp_seg, h->sp.comp_seg));
+  TSB_TRY(upload(h, plan.comp_first_vertex, h->sp.comp_first_vertex));
+  TSB_TRY(upload(h, plan.comp_ntets, h->sp.comp_ntets));
+  TSB_TRY(alloc_zero(h, plan.segs.size() * size_t(nw), &kp.sph_rec));
+  h->sp.rec = kp.sph_rec;
+  h->sp.n_components = plan.n_components;
+  h->sp.nw = nw;
   TSB_TRY(upload(h, std::vector<unsigned long long>(size_t(plan.grid) * 4, tsb::kEnergySentinel), kp.cta_energy, 2));
 #ifdef TSB_TRACE
   TSB_TRY(alloc_zero(h, size_t(plan.grid) * tsb::kTraceSlots, &kp.trace));
@@ -213,7 +224,7 @@ int tsb_create(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t ne
   kp.cells_per_chunk = cpc;
   kp.ring_slots = slots;
   kp.stage_bytes = plan.mode_global ? 0 : plan.area_verts * 32;
-  h->lc = tsb::LaunchConfig{nw, plan.grid, smem, plan.mode_global, 0, 0};
+  h->lc = tsb::LaunchConfig{nw, plan.grid, smem, plan.mode_global, 0, 0, 0};
   h->amips = pc.enable_amips != 0;
   h->det = pc.deterministic != 0;
 
@@ -252,7 +263,8 @@ int tsb_get_info(tsb_handle_t h, tsb_info_t *info) {
 }
 
 static int energy_grad_impl(tsb_handle_t h, const float *x_dev, float c1, float c2, float c3, int32_t order, float gradH,
-                            const float *gradH_dev, float *energy_out_dev, int energy4, float *grad_out_dev, void *stream) {
+                            const float *gradH_dev, float *energy_out_dev, int energy4, float *grad_out_dev,
+                            tsb_sphere_stats_t *spheres_out_dev, void *stream) {
   if (!h) return TSB_E_INVALID;
   if (!x_dev || !energy_out_dev) return fail(h, TSB_E_INVALID, "x_dev and energy_out_dev must be non-null");
   if (order != 2 && order != 4)
@@ -266,25 +278,40 @@ static int energy_grad_impl(tsb_handle_t h, const float *x_dev, float c1, float 
   tsb::LaunchConfig lc = h->lc;
   lc.amips = c3 != 0.f ? 1 : 0;          // c3 == 0: the very instantiation tsb_energy_grad always ran
   lc.det = h->det && grad_out_dev ? 1 : 0;   // energy only: the default kernel computes the same energies
+  lc.sph = spheres_out_dev ? 1 : 0;
   cudaError_t e = tsb::launch_energy_grad(kp, lc, static_cast<cudaStream_t>(stream));
   if (e != cudaSuccess) return fail(h, TSB_E_CUDA, std::string("energy_grad launch: ") + cudaGetErrorString(e));
   if (lc.det) {
     e = tsb::launch_det_gather(h->dp, grad_out_dev, static_cast<cudaStream_t>(stream));
     if (e != cudaSuccess) return fail(h, TSB_E_CUDA, std::string("deterministic gather launch: ") + cudaGetErrorString(e));
   }
+  if (lc.sph) {
+    e = tsb::launch_sphere_fold(h->sp, spheres_out_dev, static_cast<cudaStream_t>(stream));
+    if (e != cudaSuccess) return fail(h, TSB_E_CUDA, std::string("sphere fold launch: ") + cudaGetErrorString(e));
+  }
   return TSB_OK;
 }
 
 int tsb_energy_grad(tsb_handle_t h, const float *x_dev, float c1, float c2, int32_t order, float gradH,
                     const float *gradH_dev, float *energy_out_dev, float *grad_out_dev, void *stream) {
-  return energy_grad_impl(h, x_dev, c1, c2, 0.f, order, gradH, gradH_dev, energy_out_dev, 0, grad_out_dev, stream);
+  return energy_grad_impl(h, x_dev, c1, c2, 0.f, order, gradH, gradH_dev, energy_out_dev, 0, grad_out_dev, nullptr, stream);
 }
 
 int tsb_energy_grad_ex(tsb_handle_t h, const float *x_dev, const tsb_terms_t *terms, float gradH, const float *gradH_dev,
                        float *energy_out_dev, float *grad_out_dev, void *stream) {
   if (!h) return TSB_E_INVALID;
   if (!terms) return fail(h, TSB_E_INVALID, "terms is null");
-  return energy_grad_impl(h, x_dev, terms->c1, terms->c2, terms->c3, terms->order, gradH, gradH_dev, energy_out_dev, 1, grad_out_dev, stream);
+  return energy_grad_impl(h, x_dev, terms->c1, terms->c2, terms->c3, terms->order, gradH, gradH_dev, energy_out_dev, 1, grad_out_dev,
+                          nullptr, stream);
+}
+
+int tsb_energy_grad_spheres(tsb_handle_t h, const float *x_dev, const tsb_terms_t *terms, float gradH, const float *gradH_dev,
+                            float *energy_out_dev, float *grad_out_dev, tsb_sphere_stats_t *spheres_out_dev, void *stream) {
+  if (!h) return TSB_E_INVALID;
+  if (!terms) return fail(h, TSB_E_INVALID, "terms is null");
+  if (!spheres_out_dev) return fail(h, TSB_E_INVALID, "spheres_out_dev must be non-null");
+  return energy_grad_impl(h, x_dev, terms->c1, terms->c2, terms->c3, terms->order, gradH, gradH_dev, energy_out_dev, 1, grad_out_dev,
+                          spheres_out_dev, stream);
 }
 
 int tsb_energy_grad_host(tsb_handle_t h, const float *x_host, float c1, float c2, int32_t order, float gradH,

@@ -161,7 +161,10 @@ struct WarpStream {
 // DET (deterministic gradient, tsb_options_t.deterministic): a contributing tet stores its four corner vectors at its
 // tet slot instead of adding them to grad, every tet cell stores its activity ballot, and the component is flagged;
 // det_gather_kernel then adds them in a fixed order.  Tets never touch grad, so there is no rows-done protocol.
-template <int NW, int MINB, bool GLOBAL, bool AMIPS, bool DET = false>
+// SPH (tsb_energy_grad_spheres): at the end of every segment each warp reduces its lanes' energy partials, inverted-tet
+// count and smallest J, and lane 0 stores them as the (segment, warp) record; the running totals move to the warp's
+// red[] slot, so the CTA fold below is unchanged.  sphere_fold_kernel turns the records into per-component statistics.
+template <int NW, int MINB, bool GLOBAL, bool AMIPS, bool DET = false, bool SPH = false>
 __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParams p) {
   using F = Fmt<GLOBAL>;
   constexpr int NT = NW * 32;
@@ -250,6 +253,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
   }
 
   double des = 0.0, deb = 0.0, dea = 0.0;     // per-lane energy partials (smoothness, barrier, AMIPS)
+  if (SPH && lane == 0) { red[3 * warp] = 0.0; red[3 * warp + 1] = 0.0; red[3 * warp + 2] = 0.0; }
 
   // staged u = rel_u(x_i, X_i, c) with c = fp32(x_r - X_r) of the component's local vertex r = 0 (tsb_plan.cpp,
   // staging_tables): the component's rigid displacement never enters a rounded difference
@@ -368,7 +372,12 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
     if (s + 1 < cs.y) {
       hn = seg_at(s + 1);
       if (!GLOBAL) {
-        pre = !hcur.whole && !hn.whole && !(li == 0 && eager2);
+        if constexpr (SPH) {   // eager2 read back from the segment table: not kept live through the loop (register budget)
+          const bool e2 = cs.y - cs.x >= 2 && !segtab[0].whole && !segtab[1].whole;
+          pre = !hcur.whole && !hn.whole && !(li == 0 && e2);
+        } else {
+          pre = !hcur.whole && !hn.whole && !(li == 0 && eager2);
+        }
         if (pre) {
 #pragma unroll
           for (int k = 0; k < SV; ++k) {
@@ -470,6 +479,8 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
       d[1] = make_float4(c1y, c1z, c2x, c2y);
       d[2] = make_float4(c2z, c3x, c3y, c3z);
     };
+    int mnK = 0x7F800000;   // SPH: the warp's smallest J of a real tet in the segment (as an int key), its J < 0 count
+    int nneg = 0;
     for (int tc = 0; tc < int(wseg.y); ++tc) {
       uint32_t dmask = 0;   // DET: bit t = this lane's tet t contributed
       uint32_t tj[F::TPL][4];
@@ -500,6 +511,13 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
         const float e3x = x3.x - x0.x, e3y = x3.y - x0.y, e3z = x3.z - x0.z;
         const float c1x = e2y * e3z - e2z * e3y, c1y = e2z * e3x - e2x * e3z, c1z = e2x * e3y - e2y * e3x;   // e2 x e3
         const float J = (e1x * c1x + e1y * c1y + e1z * c1z) * idet;
+        if constexpr (SPH) {
+          // warp-uniform accumulators (no per-lane register).  J as an int key whose signed order is J's order;
+          // padding tets (1/det(Dm) = 0, J = 0) are not part of the sphere and enter as +inf
+          const int kJ = idet == 0.f ? 0x7F800000 : (__float_as_int(J) < 0 ? __float_as_int(J) ^ 0x7FFFFFFF : __float_as_int(J));
+          mnK = min(mnK, __reduce_min_sync(0xffffffffu, kJ));
+          nneg += __popc(__ballot_sync(0xffffffffu, J < 0.f));
+        }
         if (J < 0.f) {
           const float m = -J, m2 = m * m;
           deb += double(order2 ? m2 : m2 * m2);
@@ -602,10 +620,27 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
       }
     }
     if (s == cs.x) TSB_STAMP(6);
+    if (SPH && lane == 0) {
+      p.sph_rec[size_t(s) * NW + warp].min_J = __int_as_float(mnK < 0 ? mnK ^ 0x7FFFFFFF : mnK);
+      p.sph_rec[size_t(s) * NW + warp].n_inverted = nneg;
+    }
 
     // ---- hand the staging buffers over ------------------------------------------------------------------
     if (s + 1 < cs.y) {      // (after the last segment the energy fold's own barrier is the only one needed)
-      if (!GLOBAL) {
+      if (!GLOBAL && SPH) {   // the same as below, with eager2 read back from the segment table
+        const bool e2 = cs.y - cs.x >= 2 && !segtab[0].whole && !segtab[1].whole;
+        if (!(li == 0 && e2)) {
+          if (pre) {
+            if (li == 1 && e2) __syncthreads();
+            store_staged(hn, li + 1);
+          }
+          __syncthreads();
+          if (!pre) {
+            stage_direct(hn, li + 1);
+            __syncthreads();
+          }
+        }
+      } else if (!GLOBAL) {
         if (li == 0 && eager2) {
           // segment 1 is already staged: no barrier
         } else {
@@ -623,15 +658,28 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
         __syncthreads();     // keeps the named barrier's generations apart
       }
     }
+    // SPH: this warp's record of the segment (every warp writes one, also with no work in it); after the handover, so
+    // that the next component's prefetch registers are no longer live
+    if constexpr (SPH) {
+      const double ws = warp_sum(des), wb = warp_sum(deb), wa = AMIPS ? warp_sum(dea) : 0.0;
+      if (lane == 0) {
+        SphRec &r = p.sph_rec[size_t(s) * NW + warp];
+        r.smooth = ws; r.barrier = wb; r.amips = wa;
+        red[3 * warp] += ws; red[3 * warp + 1] += wb; red[3 * warp + 2] += wa;
+      }
+      des = 0.0; deb = 0.0; dea = 0.0;
+    }
     hcur = hn;
   }
 
   // ---- energies: lanes -> warp -> CTA partial; CTA 0 folds all partials in fixed order ---------------------
   TSB_STAMP(7);
-  des = warp_sum(des);
-  deb = warp_sum(deb);
-  if (AMIPS) dea = warp_sum(dea);
-  if (lane == 0) { red[3 * warp] = des; red[3 * warp + 1] = deb; red[3 * warp + 2] = dea; }
+  if constexpr (!SPH) {   // SPH: red[] already holds the warp's sums, segment by segment
+    des = warp_sum(des);
+    deb = warp_sum(deb);
+    if (AMIPS) dea = warp_sum(dea);
+    if (lane == 0) { red[3 * warp] = des; red[3 * warp + 1] = deb; red[3 * warp + 2] = dea; }
+  }
   __syncthreads();
   TSB_STAMP(8);
   if (tid == 0) {
@@ -758,6 +806,41 @@ __global__ void __launch_bounds__(kDetChunkRows) det_gather_kernel(const DetPara
   }
 }
 
+// Per-sphere statistics, after an SPH launch on the same stream: one warp per component.  Lane l sums the component's
+// (segment, warp) records l, l + 32, ... in that order, a shuffle tree combines the lanes: the result depends on the
+// records alone, never on scheduling.  Every output record is rewritten.
+constexpr int kFoldWarps = 8;
+__global__ void __launch_bounds__(kFoldWarps * 32) sphere_fold_kernel(const SphParams sp, tsb_sphere_stats_t *__restrict__ out) {
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // the next energy launch writes records only after its wait
+  const int c = blockIdx.x * kFoldWarps + int(threadIdx.x >> 5), lane = int(threadIdx.x & 31);
+  if (c >= sp.n_components) return;
+  const int r0 = __ldg(&sp.comp_seg[c]) * sp.nw, r1 = __ldg(&sp.comp_seg[c + 1]) * sp.nw;
+  double a = 0.0, b = 0.0, d = 0.0;
+  float m = INFINITY;
+  int k = 0;
+  for (int r = r0 + lane; r < r1; r += 32) {
+    const SphRec e = sp.rec[r];
+    a += e.smooth; b += e.barrier; d += e.amips;
+    m = fminf(m, e.min_J);
+    k += e.n_inverted;
+  }
+  a = warp_sum(a); b = warp_sum(b); d = warp_sum(d);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fminf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  k = __reduce_add_sync(0xffffffffu, k);
+  if (lane == 0) {
+    tsb_sphere_stats_t r;
+    r.smooth = 0.5 * a;            // as the CTA fold: 1/2 u^T M u
+    r.barrier = b;
+    r.amips = d;
+    r.min_J = m;
+    r.n_inverted = k;
+    r.n_tets = __ldg(&sp.comp_ntets[c]);
+    r.first_vertex = __ldg(&sp.comp_first_vertex[c]);
+    out[c] = r;
+  }
+}
+
 // ---- level-1 helpers -------------------------------------------------------------------------------
 __global__ void scale_kernel(const float *__restrict__ g, int64_t count, float gradH, const float *gradH_dev,
                              float *__restrict__ out) {
@@ -841,7 +924,7 @@ inline int grid_for(int64_t count, int block) {
   return int(g < 1 ? 1 : (g > kMaxGrid ? kMaxGrid : g));
 }
 
-template <int NW, int MINB, bool GLOBAL, bool AMIPS, bool DET = false>
+template <int NW, int MINB, bool GLOBAL, bool AMIPS, bool DET = false, bool SPH = false>
 cudaError_t launch_variant(const KParams &p, const LaunchConfig &lc, cudaStream_t stream) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(unsigned(lc.grid));
@@ -853,7 +936,7 @@ cudaError_t launch_variant(const KParams &p, const LaunchConfig &lc, cudaStream_
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, energy_grad_kernel<NW, MINB, GLOBAL, AMIPS, DET>, p);
+  return cudaLaunchKernelEx(&cfg, energy_grad_kernel<NW, MINB, GLOBAL, AMIPS, DET, SPH>, p);
 }
 
 template <int NW, int MINB, bool GLOBAL>
@@ -861,12 +944,32 @@ cudaError_t launch_det_variant(const KParams &p, const LaunchConfig &lc, cudaStr
   return lc.amips ? launch_variant<NW, MINB, GLOBAL, true, true>(p, lc, stream) : launch_variant<NW, MINB, GLOBAL, false, true>(p, lc, stream);
 }
 
-// occupancy of the deterministic instantiations (opts them in to the device's shared memory maximum like the others)
-template <int NW, int MINB, bool GLOBAL, bool AMIPS>
+template <int NW, int MINB, bool GLOBAL>
+cudaError_t launch_sph_variant(const KParams &p, const LaunchConfig &lc, cudaStream_t stream) {
+  if (lc.det)
+    return lc.amips ? launch_variant<NW, MINB, GLOBAL, true, true, true>(p, lc, stream) : launch_variant<NW, MINB, GLOBAL, false, true, true>(p, lc, stream);
+  return lc.amips ? launch_variant<NW, MINB, GLOBAL, true, false, true>(p, lc, stream) : launch_variant<NW, MINB, GLOBAL, false, false, true>(p, lc, stream);
+}
+
+// occupancy of the deterministic and SPH instantiations (opts them in to the device's shared memory maximum like the others)
+template <int NW, int MINB, bool GLOBAL, bool AMIPS, bool DET = true, bool SPH = false>
 cudaError_t occupancy_det(int smem_bytes, int optin, int *ctas_per_sm) {
-  cudaError_t e = cudaFuncSetAttribute(energy_grad_kernel<NW, MINB, GLOBAL, AMIPS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
+  cudaError_t e = cudaFuncSetAttribute(energy_grad_kernel<NW, MINB, GLOBAL, AMIPS, DET, SPH>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
   if (e != cudaSuccess) { *ctas_per_sm = 0; cudaGetLastError(); return cudaSuccess; }
-  return cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, energy_grad_kernel<NW, MINB, GLOBAL, AMIPS, true>, NW * 32, size_t(smem_bytes));
+  return cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, energy_grad_kernel<NW, MINB, GLOBAL, AMIPS, DET, SPH>, NW * 32, size_t(smem_bytes));
+}
+
+// the SPH instantiations a handle may launch: AMIPS ones when amips, DET ones when det
+template <int NW, int MINB, bool GLOBAL>
+cudaError_t occupancy_sph(int smem_bytes, int optin, bool amips, bool det, int *ctas_per_sm) {
+  int v[4] = {1 << 30, 1 << 30, 1 << 30, 1 << 30};
+  cudaError_t e = occupancy_det<NW, MINB, GLOBAL, false, false, true>(smem_bytes, optin, &v[0]);
+  if (e == cudaSuccess && amips) e = occupancy_det<NW, MINB, GLOBAL, true, false, true>(smem_bytes, optin, &v[1]);
+  if (e == cudaSuccess && det) e = occupancy_det<NW, MINB, GLOBAL, false, true, true>(smem_bytes, optin, &v[2]);
+  if (e == cudaSuccess && det && amips) e = occupancy_det<NW, MINB, GLOBAL, true, true, true>(smem_bytes, optin, &v[3]);
+  for (int k = 0; k < 4; ++k)
+    if (v[k] < *ctas_per_sm) *ctas_per_sm = v[k];
+  return e;
 }
 
 template <int NW, int MINB, bool GLOBAL>
@@ -892,6 +995,7 @@ cudaError_t occupancy_variant(int smem_bytes, bool amips, bool det, int *ctas_pe
     if (c < *ctas_per_sm) *ctas_per_sm = c;
     if (d < *ctas_per_sm) *ctas_per_sm = d;
   }
+  if (e == cudaSuccess) e = occupancy_sph<NW, MINB, GLOBAL>(smem_bytes, optin, amips, det, ctas_per_sm);
   return e;
 }
 
@@ -914,11 +1018,13 @@ cudaError_t launch_energy_grad(const KParams &p, const LaunchConfig &lc, cudaStr
     prestage_kernel<<<grid_for(p.n, 256), 256, 0, stream>>>(p.x, p.X4, p.u4g, p.x4g, p.n);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
+    if (lc.sph) return lc.nw == 16 ? launch_sph_variant<16, 1, true>(p, lc, stream) : launch_sph_variant<8, 2, true>(p, lc, stream);
     if (lc.det) return lc.nw == 16 ? launch_det_variant<16, 1, true>(p, lc, stream) : launch_det_variant<8, 2, true>(p, lc, stream);
     if (lc.nw == 16) return lc.amips ? launch_variant<16, 1, true, true>(p, lc, stream) : launch_variant<16, 1, true, false>(p, lc, stream);
     if (lc.nw == 8) return lc.amips ? launch_variant<8, 2, true, true>(p, lc, stream) : launch_variant<8, 2, true, false>(p, lc, stream);
     return cudaErrorInvalidValue;
   }
+  if (lc.sph) return lc.nw == 16 ? launch_sph_variant<16, 1, false>(p, lc, stream) : launch_sph_variant<8, 2, false>(p, lc, stream);
   if (lc.det) return lc.nw == 16 ? launch_det_variant<16, 1, false>(p, lc, stream) : launch_det_variant<8, 2, false>(p, lc, stream);
   if (lc.nw == 16) return lc.amips ? launch_variant<16, 1, false, true>(p, lc, stream) : launch_variant<16, 1, false, false>(p, lc, stream);
   if (lc.nw == 8) return lc.amips ? launch_variant<8, 2, false, true>(p, lc, stream) : launch_variant<8, 2, false, false>(p, lc, stream);
@@ -930,6 +1036,11 @@ cudaError_t launch_energy_grad(const KParams &p, const LaunchConfig &lc, cudaStr
 // launch as well measured 5x slower at 64 x 4096 with inverted tets (DESIGN.md section 3).
 cudaError_t launch_det_gather(const DetParams &d, float *grad, cudaStream_t stream) {
   det_gather_kernel<<<unsigned(d.n_chunks), kDetChunkRows, 0, stream>>>(d, grad);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_sphere_fold(const SphParams &sp, tsb_sphere_stats_t *out, cudaStream_t stream) {
+  sphere_fold_kernel<<<unsigned((sp.n_components + kFoldWarps - 1) / kFoldWarps), kFoldWarps * 32, 0, stream>>>(sp, out);
   return cudaGetLastError();
 }
 

@@ -4,9 +4,19 @@
 
 #include <cstdint>
 
+#include "../../include/tssplat_b200.h"
 #include "tsb_plan.h"
 
 namespace tsb {
+
+// What one warp saw of one segment (SPH instantiation): its lanes' energy partials in fp64 (smoothness not yet
+// halved), the smallest J of its real tets (+inf: none) and how many of them have J < 0.  32 bytes.
+struct __align__(16) SphRec {
+  double smooth, barrier, amips;
+  float min_J;
+  int32_t n_inverted;
+};
+static_assert(sizeof(SphRec) == 32, "SphRec must be 32 bytes");
 
 struct KParams {
   // plan (read-only, built once by tsb_create)
@@ -47,6 +57,8 @@ struct KParams {
   float4 *det_scratch;          // [3 * slots] corner vectors of a contributing tet: (c0.xyz, c1.x) (c1.yz, c2.xy) (c2.z, c3.xyz)
   unsigned long long *det_ballot;   // [tet cells] bit t * 32 + lane: the tet in slot lane * TPL + t contributed
   unsigned int *det_flag;       // [n_components] nonzero: a tet of the component contributed (the gather clears it)
+  // per-sphere statistics only (the SPH instantiation, tsb_energy_grad_spheres): one record per (segment, warp)
+  SphRec *sph_rec;              // [n_segments * nw], rewritten by every SPH launch, read by sphere_fold_kernel
 #ifdef TSB_TRACE
   unsigned long long *trace;    // profiling build only: [grid][kTraceSlots] phase stamps
 #endif
@@ -60,6 +72,17 @@ struct LaunchConfig {
   int global;      // GLOBAL mode
   int amips;       // launch the AMIPS-capable instantiation
   int det;         // launch the deterministic instantiation (tets store their corners instead of adding them)
+  int sph;         // launch the SPH instantiation (it also writes the per-(segment, warp) sphere records)
+};
+
+// sphere_fold_kernel's inputs (HostPlan::comp_*, uploaded, and the records of the SPH launch before it).
+struct SphParams {
+  const SphRec *rec;
+  const int32_t *comp_seg;          // [n_components + 1] first segment of every component
+  const int32_t *comp_first_vertex; // [n_components]
+  const int32_t *comp_ntets;        // [n_components]
+  int32_t n_components;
+  int32_t nw;
 };
 
 // The deterministic gather's plan (HostPlan::det_*, uploaded) and the scratch it shares with the energy kernel.
@@ -84,6 +107,8 @@ cudaError_t energy_occupancy(int nw, int smem_bytes, bool global, bool amips, bo
 cudaError_t launch_energy_grad(const KParams &p, const LaunchConfig &lc, cudaStream_t stream);
 // grad[v] += the active corner vectors of v's list, in list order, for every flagged component (after a DET launch).
 cudaError_t launch_det_gather(const DetParams &d, float *grad, cudaStream_t stream);
+// One tsb_sphere_stats_t per component from the records of the SPH launch before it on the same stream.
+cudaError_t launch_sphere_fold(const SphParams &sp, tsb_sphere_stats_t *out, cudaStream_t stream);
 
 cudaError_t launch_scale(const float *g, int64_t count, float gradH, const float *gradH_dev, float *out, cudaStream_t s);
 cudaError_t launch_grad_limit(float *g, int64_t count, float thr, float s, float *work4, cudaStream_t st);

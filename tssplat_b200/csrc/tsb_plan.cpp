@@ -811,6 +811,30 @@ std::vector<Seg> make_segments(const std::vector<Comp> &comps, const std::vector
   return segs;
 }
 
+// Per-component tables of the sphere statistics: first segment, lowest vertex and tet count of every component.
+int component_tables(const std::vector<Comp> &comps, const std::vector<Seg> &segs, HostPlan &P, std::string &err) {
+  const int NC = int(comps.size());
+  P.comp_seg.assign(size_t(NC) + 1, 0);
+  P.comp_first_vertex.resize(size_t(NC));
+  P.comp_ntets.resize(size_t(NC));
+  for (int c = 0; c < NC; ++c) {
+    P.comp_first_vertex[c] = comps[c].verts[0];
+    P.comp_ntets[c] = int32_t(comps[c].tets.size());
+  }
+  // every component has >= 1 segment and its segments are consecutive: seg s starts component segs[s].comp exactly
+  // when the component changes
+  int c = -1;
+  for (size_t s = 0; s < segs.size(); ++s) {
+    if (segs[s].comp == c) continue;
+    if (segs[s].comp != c + 1) { err = "internal: the segments of a component are not consecutive"; return TSB_E_INVALID; }
+    c = segs[s].comp;
+    P.comp_seg[c] = int32_t(s);
+  }
+  if (c != NC - 1) { err = "internal: a component has no segment"; return TSB_E_INVALID; }
+  P.comp_seg[NC] = int32_t(segs.size());
+  return TSB_OK;
+}
+
 // Staging tables (STAGED: rest position, global id and staging position of every component vertex; GLOBAL: rest
 // positions by vertex id) and the segment headers.
 //
@@ -1101,6 +1125,7 @@ int build_plan(const float *rest, const int32_t *tets, int32_t n, int32_t nele, 
   if ((rc = choose_layout(comps, cfg, global_mode, P, err)) != TSB_OK) return rc;
   const std::vector<Seg> segs = make_segments(comps, cut_stream(comps, double(cfg.tet_cost), P.grid), P);
   staging_tables(M, comps, segs, P);
+  if ((rc = component_tables(comps, segs, P, err)) != TSB_OK) return rc;
   std::vector<std::vector<uint8_t>> wstream(size_t(P.grid) * P.nw);
   std::vector<std::vector<float>> wB(cfg.enable_amips ? wstream.size() : 0);
   std::vector<std::vector<int32_t>> wV(cfg.deterministic ? wstream.size() : 0);

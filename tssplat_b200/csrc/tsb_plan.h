@@ -129,6 +129,11 @@ struct HostPlan {
   std::vector<uint32_t> wdesc;      // [2*grid*nw] (stream offset / 16, stream bytes)
   std::vector<uint16_t> wseg;       // [2*nsegs*nw] (row blocks, tet cells) of each warp in each segment
   std::vector<int32_t> orphans;     // vertices no tet references (their gradient is zero)
+  // Per component (per-sphere statistics).  Cuts run along the component-major cost stream and segs is CTA-major, so
+  // the segments of a component are consecutive: component c owns segs[comp_seg[c], comp_seg[c + 1]).
+  std::vector<int32_t> comp_seg;          // [n_components + 1]
+  std::vector<int32_t> comp_first_vertex; // [n_components] lowest vertex id (components are numbered by it)
+  std::vector<int32_t> comp_ntets;        // [n_components]
   // AMIPS only: rest inverses B = Dm^-1 of every streamed tet (in its streamed vertex order), one block of
   // 3 rows x (tets per cell) float4 per tet cell, and the first tet cell of every (segment, warp)
   std::vector<float> Bt;

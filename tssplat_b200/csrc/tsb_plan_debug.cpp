@@ -63,6 +63,7 @@ int tsbdbg_array(tsbdbg_plan *d, const char *name, const void **ptr, int64_t *co
   ARR("Bt", P.Bt, 4) ARR("wtc0", P.wtc0, 4)
   ARR("det_rowptr", P.det_rowptr, 4) ARR("det_vert", P.det_vert, 4) ARR("det_ent", P.det_ent, 4)
   ARR("det_comp_row", P.det_comp_row, 4) ARR("det_chunk", P.det_chunk, 4)
+  ARR("comp_seg", P.comp_seg, 4) ARR("comp_first_vertex", P.comp_first_vertex, 4) ARR("comp_ntets", P.comp_ntets, 4)
 #undef ARR
   return TSB_E_INVALID;
 }

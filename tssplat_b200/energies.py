@@ -67,8 +67,20 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         multiplier = math.pow(2, abs(math.sin(phase)) * 4)
         return self.FLAGS.smooth_eng_coeff * multiplier, self.FLAGS.barrier_coeff * multiplier
 
+    def order_at(self, it) -> int:
+        return 4 if it > self.FLAGS.increase_order_iter else 2     # smooth_barrier.py:61-63
+
+    def sphere_stats(self, x, it):
+        """Per-sphere geometry statistics at ``x`` (``tet_spheres_ext.SphereStats`` of device tensors, no host sync):
+        each sphere's smoothness and barrier terms, inverted-tet count and smallest det F, with the barrier order
+        ``forward(x, it, ...)`` uses at ``it``.  An energy-only launch, outside autograd; it leaves the fused-gradient
+        cache alone.  Meant to be logged every N iterations next to the loss."""
+        c1, c2 = self.coeff_scheduler(it)
+        _, _, stats = self.tet_sp.energy_grad_spheres(x.detach(), c1, c2, self.order_at(it), want_grad=False)
+        return stats
+
     def forward(self, x, it, c1, c2):
-        order = 4 if it > self.FLAGS.increase_order_iter else 2     # smooth_barrier.py:61-63
+        order = self.order_at(it)
         if (use_native_autograd and self.smooth_eng_func is SmoothnessBarrierFunc and tet_spheres_ext.fuse_backward_into_forward
                 and not tet_spheres_ext.return_cpu_scalar):
             ns = self.tet_sp.native_state()        # C++ torch::autograd::Function over the same C ABI (csrc/torch_binding.cpp)

@@ -24,7 +24,7 @@ Deliberate differences from the reference (SURVEY.md section 2.4), all on error 
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional
+from typing import NamedTuple, Optional
 
 import numpy as np
 import torch
@@ -32,7 +32,7 @@ import torch
 from . import _capi
 from .mesh import load_veg
 
-__all__ = ["TetSpheres", "forward", "backward", "random_x", "grad_limit", "energy_grad_host"]
+__all__ = ["TetSpheres", "SphereStats", "forward", "backward", "random_x", "grad_limit", "energy_grad_host"]
 
 return_cpu_scalar = False
 _limit_work = {}       # (device, stream) -> float32[4] scratch of grad_limit (caller-owned in the C ABI)
@@ -49,6 +49,21 @@ def _stream_ptr(device) -> int:
     if _raw_stream is not None:
         return int(_raw_stream(device.index if isinstance(device, torch.device) else int(device)))
     return int(torch.cuda.current_stream(device).cuda_stream)
+
+
+class SphereStats(NamedTuple):
+    """Geometry statistics per connected component (= tet-sphere), device tensors of length S = number of components,
+    in the order of the components' lowest vertex ids (``tsb_sphere_stats_t`` in ``include/tssplat_b200.h``)."""
+    smooth: torch.Tensor        # f64: 1/2 u^T M u over the sphere's rows (unweighted)
+    barrier: torch.Tensor       # f64: sum of max(-J, 0)^order over its tets
+    amips: torch.Tensor         # f64: AMIPS sum over its J > 0 tets (0 unless c3 != 0)
+    min_J: torch.Tensor         # f32: smallest det F of its tets
+    n_inverted: torch.Tensor    # i32: tets with J < 0
+    n_tets: torch.Tensor        # i32
+    first_vertex: torch.Tensor  # i32: lowest vertex id of the sphere
+
+
+_STATS_BYTES = C.sizeof(_capi.tsb_sphere_stats_t)     # 40
 
 
 class TetSpheres:
@@ -183,6 +198,35 @@ class TetSpheres:
             _capi.check(rc, self._h, "tet_spheres_ext")
         del keep
         return energy, grad
+
+    def energy_grad_spheres(self, x: torch.Tensor, c1: float, c2: float, order: int, gradH=1.0, want_grad: bool = True,
+                            c3: float = 0.0):
+        """``energy_grad`` plus per-sphere statistics (``tsb_energy_grad_spheres``): returns (energy[4] = total / smooth /
+        barrier / AMIPS, grad or None, ``SphereStats``), all on the device, without a host sync.  Every call allocates
+        fresh output tensors (this is a diagnostic call, not the training step).  The records of a sharded run
+        (``ShardedEnergy``) cover the rank's own ``sphere_range`` and carry ``first_vertex`` in the rank's local
+        numbering."""
+        xc = self._check_x(x)
+        S = int(self.info["n_components"])
+        energy = torch.empty(4, dtype=torch.float32, device=self.device)
+        grad = torch.empty((self.n, 3), dtype=torch.float32, device=self.device) if want_grad else None
+        raw = torch.empty((S, _STATS_BYTES), dtype=torch.uint8, device=self.device)
+        gh_val, gh_ptr, keep = 1.0, None, None
+        if isinstance(gradH, torch.Tensor) and gradH.is_cuda:
+            keep = gradH.detach().to(device=self.device, dtype=torch.float32).reshape(-1)[:1].contiguous()
+            gh_ptr = keep.data_ptr()
+        else:
+            gh_val = float(gradH)
+        terms = _capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
+        rc = _capi.lib.tsb_energy_grad_spheres(self._h, xc.data_ptr(), C.byref(terms), gh_val, gh_ptr, energy.data_ptr(),
+                                               grad.data_ptr() if want_grad else None, raw.data_ptr(),
+                                               _stream_ptr(self.device))
+        if rc:
+            _capi.check(rc, self._h, "tet_spheres_ext.energy_grad_spheres")
+        del keep
+        f64, f32, i32 = (raw[:, 0:24].view(torch.float64), raw[:, 24:28].view(torch.float32), raw[:, 28:40].view(torch.int32))
+        stats = SphereStats(f64[:, 0], f64[:, 1], f64[:, 2], f32[:, 0], i32[:, 0], i32[:, 1], i32[:, 2])
+        return energy, grad, stats
 
 
 def energy_grad_host(tet_sp: TetSpheres, x_host: torch.Tensor, c1: float, c2: float, order: int, gradH: float,
