@@ -124,9 +124,16 @@ def pole_mesh(m):
 
 PLAN_DEBUG_SO = os.path.join(ROOT, "tests", "native", "libtsb_plan_debug.so")
 CELLS_PER_CHUNK = 6      # tsb_plan.h kCellsPerChunk: cells per ring slot
+# Stream cells (tsb_plan.h): (cell bytes, bytes per index, tets per lane) of the STAGED (16-bit smem offsets) and
+# GLOBAL (32-bit vertex ids) formats.  A cell holds 128 indices, then (at WOFF = 128 * bytes per index) 128 weights or
+# the tets' 1/det(Dm); word 0 of each lane's first weight quad of a row block is the block header.
+CELL_FORMAT = {False: (768, 2, 2), True: (1024, 4, 1)}
 _ARRAYS = {"stream": np.uint8, "X4": np.float32, "vlist": np.int32, "segs": np.int32, "cta_seg": np.int32,
            "wdesc": np.uint32, "wseg": np.uint16, "orphans": np.int32, "pos16": np.uint16, "pos_gid": np.int32,
-           "Bt": np.float32, "wtc0": np.int32}
+           "Bt": np.float32, "wtc0": np.int32, "comp_seg": np.int32, "comp_first_vertex": np.int32,
+           "comp_ntets": np.int32}
+_DET_ARRAYS = {"det_rowptr": np.int32, "det_vert": np.int32, "det_ent": np.uint32, "det_comp_row": np.int32,
+               "det_chunk": np.int32}
 _SCALARS = ("n", "nele", "n_components", "n_boundary_faces", "laplacian_scale", "mode_global", "nw", "grid", "vh",
             "area_verts", "max_comp_verts", "contiguous", "nnz", "nnz_padded", "n_rb", "n_tetcells",
             "gather_wf", "gather_wf_ideal", "tet_wf", "tet_wf_ideal")
@@ -134,15 +141,15 @@ _SEG = ("comp", "vbase", "nv", "x4off", "expected", "whole", "npos", "p4off")
 
 
 def build_host_plan(rest, tets, nw=16, grid=132, laplacian_scale=0, force_global=0, vh_cap=0, area_cap=0,
-                    tet_cost=0.0, ring_slots=0, enable_amips=0):
+                    tet_cost=0.0, ring_slots=0, enable_amips=0, deterministic=0):
     """Run the product's host plan builder (tssplat_b200/csrc/tsb_plan.cpp, no CUDA) through the
     test-only inspection library and copy its arrays out as numpy.  ring_slots: the ring a handle
-    requests (row splitting depends on it); 0 = the default."""
+    requests (row splitting depends on it); 0 = the default.  deterministic: also build (and return)
+    the deterministic gather's det_* arrays."""
     lib = C.CDLL(PLAN_DEBUG_SO)
-    lib.tsbdbg_build_ex.restype = C.c_int
-    lib.tsbdbg_build_ex.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                    C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_int32,
-                                    C.POINTER(C.c_void_p)]
+    lib.tsbdbg_build_det.restype = C.c_int
+    lib.tsbdbg_build_det.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 8 + [C.c_float] + [C.c_int32] * 3 + \
+                                    [C.POINTER(C.c_void_p)]
     lib.tsbdbg_array.restype = C.c_int
     lib.tsbdbg_array.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64),
                                  C.POINTER(C.c_int32)]
@@ -152,14 +159,14 @@ def build_host_plan(rest, tets, nw=16, grid=132, laplacian_scale=0, force_global
     rest = np.ascontiguousarray(np.asarray(rest, dtype=np.float32).reshape(-1))
     tets = np.ascontiguousarray(np.asarray(tets, dtype=np.int32).reshape(-1))
     d = C.c_void_p()
-    rc = lib.tsbdbg_build_ex(rest.ctypes.data, tets.ctypes.data, rest.size // 3, tets.size // 4, int(nw), int(grid),
-                             int(laplacian_scale), int(force_global), int(vh_cap), int(area_cap), float(tet_cost),
-                             int(ring_slots) * CELLS_PER_CHUNK, int(enable_amips), C.byref(d))
+    rc = lib.tsbdbg_build_det(rest.ctypes.data, tets.ctypes.data, rest.size // 3, tets.size // 4, int(nw), int(grid),
+                              int(laplacian_scale), int(force_global), int(vh_cap), int(area_cap), float(tet_cost),
+                              int(ring_slots) * CELLS_PER_CHUNK, int(enable_amips), int(deterministic), C.byref(d))
     if rc != 0:
         raise RuntimeError(lib.tsbdbg_last_error().decode())
     try:
         plan = {}
-        for name, dt in _ARRAYS.items():
+        for name, dt in {**_ARRAYS, **(_DET_ARRAYS if deterministic else {})}.items():
             ptr, cnt, eb = C.c_void_p(), C.c_int64(), C.c_int32()
             assert lib.tsbdbg_array(d, name.encode(), C.byref(ptr), C.byref(cnt), C.byref(eb)) == 0, name
             nbytes = cnt.value * eb.value
@@ -173,6 +180,44 @@ def build_host_plan(rest, tets, nw=16, grid=132, laplacian_scale=0, force_global
         lib.tsbdbg_free(d)
     plan["segs"] = [dict(zip(_SEG, row)) for row in plan["segs"].reshape(-1, 8).tolist()]
     return plan
+
+
+def walk_streams(plan):
+    """Walk every warp's cell stream as energy_grad_kernel does: CTA -> warp -> segment -> the segment's row blocks,
+    then its tet cells.  Returns (blocks, cells): blocks = (byte offset, the 32 lanes' header words) of every row
+    block, cells = (byte offset, CTA, segment, warp, index among the warp's tet cells of the segment) of every tet
+    cell.  Asserts that each warp consumes exactly its stream."""
+    G, NW = plan["grid"], plan["nw"]
+    CELL, IB, _ = CELL_FORMAT[bool(plan["mode_global"])]
+    WOFF = 128 * IB
+    st = plan["stream"]
+    wdesc, wseg, cta_seg = plan["wdesc"].reshape(G, NW, 2), plan["wseg"].reshape(-1, NW, 2), plan["cta_seg"].reshape(G, 2)
+    blocks, cells = [], []
+    for b in range(G):
+        for w in range(NW):
+            p = int(wdesc[b, w, 0]) * 16
+            for s in range(cta_seg[b, 0], cta_seg[b, 1]):
+                nrb, ntc = (int(v) for v in wseg[s, w])
+                for _ in range(nrb):
+                    hdr = st[p + WOFF:p + WOFF + 512].view(np.uint32).reshape(32, 4)[:, 0].copy()
+                    blocks.append((p, hdr))
+                    p += int((hdr[0] >> 24) & 63) * CELL
+                for tc in range(ntc):
+                    cells.append((p, b, s, w, tc))
+                    p += CELL
+            assert p == int(wdesc[b, w, 0]) * 16 + int(wdesc[b, w, 1]), "a warp did not consume exactly its stream"
+    return blocks, cells
+
+
+def tet_cell(plan, p):
+    """(streamed ids [32 * TPL, 4] as int64, 1/det(Dm) [32 * TPL]) of the tet cell at byte offset p: staging byte
+    offsets (STAGED) or vertex ids (GLOBAL), in slot order lane * TPL + t."""
+    glob = bool(plan["mode_global"])
+    _, IB, TPL = CELL_FORMAT[glob]
+    n = 128 * IB * TPL
+    st = plan["stream"]
+    ids = st[p:p + n].view(np.uint32 if glob else np.uint16).reshape(32 * TPL, 4).astype(np.int64)
+    return ids, st[p + n:p + n + 128 * TPL].view(np.float32)
 
 
 def _rel_u(x, X, xr, Xr):

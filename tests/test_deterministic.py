@@ -13,81 +13,29 @@ import _helpers as H
 from _helpers import COracle, build_host_plan, emulate_kernel, min_abs_J, mirror_components
 from tssplat_b200.mesh import connected_components, make_pack, perturb
 
-_DET_ARRAYS = {"det_rowptr": np.int32, "det_vert": np.int32, "det_ent": np.uint32, "det_comp_row": np.int32,
-               "det_chunk": np.int32}
 CHUNK_ROWS = 256            # tsb_plan.h kDetChunkRows
 SHARED = ("stream", "X4", "vlist", "segs", "cta_seg", "wdesc", "wseg", "orphans", "pos16", "pos_gid", "Bt")
-
-
-def build_det_plan(rest, tets, nw=16, grid=132, laplacian_scale=0, force_global=0, vh_cap=0, area_cap=0, ring_slots=0,
-                   enable_amips=0):
-    """build_host_plan with deterministic = 1 (tsbdbg_build_det), plus the det_* arrays."""
-    lib = C.CDLL(H.PLAN_DEBUG_SO)
-    lib.tsbdbg_build_det.restype = C.c_int
-    lib.tsbdbg_build_det.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 8 + [C.c_float] + [C.c_int32] * 3 + \
-                                    [C.POINTER(C.c_void_p)]
-    lib.tsbdbg_array.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_int32)]
-    lib.tsbdbg_scalars.argtypes = [C.c_void_p, C.c_void_p]
-    lib.tsbdbg_free.argtypes = [C.c_void_p]
-    lib.tsbdbg_last_error.restype = C.c_char_p
-    rest = np.ascontiguousarray(np.asarray(rest, dtype=np.float32).reshape(-1))
-    tets = np.ascontiguousarray(np.asarray(tets, dtype=np.int32).reshape(-1))
-    d = C.c_void_p()
-    rc = lib.tsbdbg_build_det(rest.ctypes.data, tets.ctypes.data, rest.size // 3, tets.size // 4, nw, grid, laplacian_scale,
-                              force_global, vh_cap, area_cap, 0.0, ring_slots * H.CELLS_PER_CHUNK, enable_amips, 1, C.byref(d))
-    if rc != 0:
-        raise RuntimeError(lib.tsbdbg_last_error().decode())
-    plan = {}
-    try:
-        for name, dt in {**H._ARRAYS, **_DET_ARRAYS}.items():
-            ptr, cnt, eb = C.c_void_p(), C.c_int64(), C.c_int32()
-            assert lib.tsbdbg_array(d, name.encode(), C.byref(ptr), C.byref(cnt), C.byref(eb)) == 0, name
-            nbytes = cnt.value * eb.value
-            plan[name] = np.frombuffer(bytes((C.c_char * nbytes).from_address(ptr.value)) if nbytes else b"", dtype=dt).copy()
-        sc = np.zeros(20, np.int64)
-        lib.tsbdbg_scalars(d, sc.ctypes.data)
-        plan.update({k: int(v) for k, v in zip(H._SCALARS, sc)})
-    finally:
-        lib.tsbdbg_free(d)
-    plan["segs_raw"] = plan["segs"]
-    plan["segs"] = [dict(zip(H._SEG, row)) for row in plan["segs"].reshape(-1, 8).tolist()]
-    return plan
 
 
 def stream_tets(plan):
     """Walk every warp's stream as the kernel does and return, per tet slot (wtc0[s, w] + tc) * TPC + lane * TPL + t,
     the global ids of its four streamed corners (-1 for padding tets) and its 1/det(Dm)."""
-    G, NW, glob = plan["grid"], plan["nw"], bool(plan["mode_global"])
-    IB, CELL, TPL = (4, 1024, 1) if glob else (2, 768, 2)
-    idt = np.uint32 if glob else np.uint16
-    TPC = 32 * TPL
-    st = plan["stream"]
-    wdesc = plan["wdesc"].reshape(G, NW, 2)
-    wseg = plan["wseg"].reshape(-1, NW, 2)
-    wtc0 = plan["wtc0"].reshape(-1, NW)
-    cta_seg = plan["cta_seg"].reshape(G, 2)
+    glob = bool(plan["mode_global"])
+    TPC = 32 * H.CELL_FORMAT[glob][2]
+    wtc0 = plan["wtc0"].reshape(-1, plan["nw"])
+    cta_seg = plan["cta_seg"].reshape(-1, 2)
     verts = np.full((plan["n_tetcells"] * TPC, 4), -2, np.int64)
     idet = np.zeros(plan["n_tetcells"] * TPC, np.float32)
-    for b in range(G):
-        for w in range(NW):
-            p = int(wdesc[b, w, 0]) * 16
-            for s in range(cta_seg[b, 0], cta_seg[b, 1]):
-                h = plan["segs"][s]
-                nrb, ntc = (int(v) for v in wseg[s, w])
-                for _ in range(nrb):
-                    p += int((st[p + 128 * IB:p + 128 * IB + 4].view(np.uint32)[0] >> 24) & 63) * CELL
-                for tc in range(ntc):
-                    idx = st[p:p + 128 * IB * TPL].view(idt).reshape(TPC, 4).astype(np.int64)
-                    d = st[p + 128 * IB * TPL:p + 128 * IB * TPL + 4 * TPC].view(np.float32)
-                    if not glob:
-                        li = s - cta_seg[b, 0]
-                        xb = h["npos"] if h["whole"] else (li & 1) * 2 * plan["vh"] + plan["vh"]
-                        idx = plan["pos_gid"][h["p4off"] + idx // 16 - xb].astype(np.int64)
-                    sl = (int(wtc0[s, w]) + tc) * TPC
-                    verts[sl:sl + TPC] = np.where((d == 0)[:, None], -1, idx)
-                    idet[sl:sl + TPC] = d
-                    p += CELL
-            assert p == int(wdesc[b, w, 0]) * 16 + int(wdesc[b, w, 1])
+    for p, b, s, w, tc in H.walk_streams(plan)[1]:
+        idx, d = H.tet_cell(plan, p)
+        if not glob:
+            h = plan["segs"][s]
+            li = s - cta_seg[b, 0]
+            xb = h["npos"] if h["whole"] else (li & 1) * 2 * plan["vh"] + plan["vh"]
+            idx = plan["pos_gid"][h["p4off"] + idx // 16 - xb].astype(np.int64)
+        sl = (int(wtc0[s, w]) + tc) * TPC
+        verts[sl:sl + TPC] = np.where((d == 0)[:, None], -1, idx)
+        idet[sl:sl + TPC] = d
     assert (verts >= -1).all(), "a tet cell was not visited"
     return verts, idet
 
@@ -132,11 +80,11 @@ def test_det_lists_structure(mesh, kw, amips):
     """Every (non-padding streamed tet, corner) is listed exactly once, under the global vertex the stream names; lists
     are ascending; padding and orphans are absent; rows are grouped by component; the default plan is unchanged."""
     V, T = _mesh(mesh)
-    plan = build_det_plan(V, T, enable_amips=amips, **kw)
+    plan = build_host_plan(V, T, enable_amips=amips, deterministic=1, **kw)
     ref = build_host_plan(V, T, enable_amips=amips, **kw)
     for k in SHARED:
         if k == "segs":
-            assert plan["segs_raw"].tobytes() == np.array([list(s.values()) for s in ref["segs"]], np.int32).tobytes()
+            assert plan["segs"] == ref["segs"]
         else:
             assert plan[k].tobytes() == ref[k].tobytes(), k
     assert all(plan[k] == ref[k] for k in H._SCALARS)
@@ -228,7 +176,7 @@ def test_det_reenactment_matches_oracle(kw):
     """Store at the slots, gather in list order: the result is the oracle's gradient (barrier orders 2 and 4 on
     inverted input; AMIPS beside the barrier)."""
     pack = make_pack(3, 768, seed=2)
-    plan = build_det_plan(pack.verts, pack.tets, enable_amips=1, **kw)
+    plan = build_host_plan(pack.verts, pack.tets, enable_amips=1, deterministic=1, **kw)
     orc = COracle(pack.verts, pack.tets)
     for order in (2, 4):
         x = perturb(pack, sigma_rel=0.35, seed=1)

@@ -21,7 +21,7 @@ import numpy as np
 import pytest
 import scipy.sparse as sps
 
-from _helpers import COracle, build_host_plan, emulate_kernel, mirror_components
+from _helpers import COracle, build_host_plan, emulate_kernel, mirror_components, walk_streams
 from oracle.tet_energy_oracle import build_G, rest_inverse, tet_laplacian
 from tssplat_b200.mesh import connected_components, make_pack, perturb
 
@@ -444,24 +444,6 @@ def top():
     return pk, ids, rest, T, RowScale(pk.verts, pk.tets, ids=ids), COracle(pk.verts, pk.tets)
 
 
-def _headers(plan):
-    """The 32 lanes' header words of every row block of the plan's streams."""
-    G, NW, glob = plan["grid"], plan["nw"], bool(plan["mode_global"])
-    CELL, WOFF = (1024, 512) if glob else (768, 256)
-    wdesc, wseg, cs = plan["wdesc"].reshape(G, NW, 2), plan["wseg"].reshape(-1, NW, 2), plan["cta_seg"].reshape(G, 2)
-    out = []
-    for b in range(G):
-        for w in range(NW):
-            p = int(wdesc[b, w, 0]) * 16
-            for s in range(cs[b, 0], cs[b, 1]):
-                for _ in range(int(wseg[s, w, 0])):
-                    hdr = plan["stream"][p + WOFF:p + WOFF + 512].view(np.uint32).reshape(32, 4)[:, 0].copy()
-                    out.append(hdr)
-                    p += int((hdr[0] >> 24) & 63) * CELL
-                p += int(wseg[s, w, 1]) * CELL
-    return np.array(out)
-
-
 @pytest.mark.parametrize("force_global", [0, 1])
 def test_top_range_plan_headers(top, force_global):
     """The block headers' row ids are the relabelled vertex ids (bits 20..23 set), and every header read as fp32 is
@@ -471,7 +453,7 @@ def test_top_range_plan_headers(top, force_global):
     assert plan["n"] == TOP_N and plan["mode_global"] == force_global and len(plan["orphans"]) == TOP_N - pk.n
     if not force_global:
         assert any(s["vbase"] < 0 for s in plan["segs"]) and any(s["vbase"] >= 1 << 23 for s in plan["segs"])
-    hdr = _headers(plan)
+    hdr = np.array([h for _, h in walk_streams(plan)[0]])   # the 32 lanes' header words of every row block
     rid = hdr & 0xFFFFFF
     assert np.array_equal(np.unique(rid[rid != 0xFFFFFF]), np.sort(ids))
     assert np.isfinite(hdr.view(np.float32)).all()

@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 from _helpers import (GOLDEN, RIGID_MOTIONS, ROOT, COracle, build_host_plan, emulate_kernel, min_abs_J, pole_mesh,
-                      rigid_motion)
+                      rigid_motion, walk_streams)
 from tssplat_b200 import _capi
 from tssplat_b200.mesh import (concat_spheres, connected_components, load_veg, make_pack, make_tet_sphere, perturb,
                                save_veg)
@@ -102,21 +102,7 @@ def test_high_valence_rows():
 
 def _block_headers(plan):
     """(len4, lanes per row) of every row block in the plan's streams."""
-    G, NW, glob = plan["grid"], plan["nw"], bool(plan["mode_global"])
-    CELL, WOFF = (1024, 512) if glob else (768, 256)
-    wdesc, wseg, cs = plan["wdesc"].reshape(G, NW, 2), plan["wseg"].reshape(-1, NW, 2), plan["cta_seg"].reshape(G, 2)
-    out = []
-    for b in range(G):
-        for w in range(NW):
-            p = int(wdesc[b, w, 0]) * 16
-            for s in range(cs[b, 0], cs[b, 1]):
-                for _ in range(int(wseg[s, w, 0])):
-                    hdr = int(plan["stream"][p + WOFF:p + WOFF + 4].view(np.uint32)[0])
-                    len4 = (hdr >> 24) & 63
-                    out.append((len4, 1 << (hdr >> 30)))
-                    p += len4 * CELL
-                p += int(wseg[s, w, 1]) * CELL
-    return out
+    return [((int(h[0]) >> 24) & 63, 1 << (int(h[0]) >> 30)) for _, h in walk_streams(plan)[0]]
 
 
 def test_plan_operator_is_the_reference_matrix():

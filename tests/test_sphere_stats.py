@@ -17,30 +17,6 @@ REL = 1e-5
 
 
 # ---- helpers -------------------------------------------------------------------------------------------------------
-def _comp_tables(rest, tets, **kw):
-    """The plan's comp_seg / comp_first_vertex / comp_ntets (tsb_plan_debug.cpp), next to build_host_plan's arrays."""
-    lib = C.CDLL(H.PLAN_DEBUG_SO)
-    lib.tsbdbg_build_ex.restype = C.c_int
-    lib.tsbdbg_build_ex.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 8 + [C.c_float, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
-    lib.tsbdbg_array.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_int32)]
-    lib.tsbdbg_free.argtypes = [C.c_void_p]
-    rest = np.ascontiguousarray(np.asarray(rest, dtype=np.float32).reshape(-1))
-    tets = np.ascontiguousarray(np.asarray(tets, dtype=np.int32).reshape(-1))
-    d = C.c_void_p()
-    rc = lib.tsbdbg_build_ex(rest.ctypes.data, tets.ctypes.data, rest.size // 3, tets.size // 4, kw.get("nw", 16),
-                             kw.get("grid", 132), 0, kw.get("force_global", 0), 0, 0, 0.0, 0, 0, C.byref(d))
-    assert rc == 0
-    out = {}
-    try:
-        for name in ("comp_seg", "comp_first_vertex", "comp_ntets"):
-            ptr, cnt, eb = C.c_void_p(), C.c_int64(), C.c_int32()
-            assert lib.tsbdbg_array(d, name.encode(), C.byref(ptr), C.byref(cnt), C.byref(eb)) == 0, name
-            out[name] = np.ctypeslib.as_array((C.c_int32 * cnt.value).from_address(ptr.value)).copy() if cnt.value else np.zeros(0, np.int32)
-    finally:
-        lib.tsbdbg_free(d)
-    return out
-
-
 def _components(n, tets):
     """(vertex ids, tet ids) of every connected component, in order of the lowest vertex id."""
     t = np.asarray(tets).reshape(-1, 4)
@@ -70,26 +46,8 @@ def _a_veg():
 
 
 def _tet_cells(plan):
-    """(vertex ids [slots, 4], 1/det(Dm) [slots]) of every tet slot of every tet cell, walking each warp's stream."""
-    G, NW, glob = plan["grid"], plan["nw"], bool(plan["mode_global"])
-    IB, TPL, CELL = (4, 1, 1024) if glob else (2, 2, 768)
-    idt = np.uint32 if glob else np.uint16
-    st, wdesc = plan["stream"], plan["wdesc"].reshape(G, NW, 2)
-    wseg, cta_seg = plan["wseg"].reshape(-1, NW, 2), plan["cta_seg"].reshape(G, 2)
-    ids, idets = [], []
-    for b in range(G):
-        for w in range(NW):
-            p = int(wdesc[b, w, 0]) * 16
-            for s in range(cta_seg[b, 0], cta_seg[b, 1]):
-                nrb, ntc = (int(v) for v in wseg[s, w])
-                for _ in range(nrb):
-                    hdr = st[p + 128 * IB:p + 128 * IB + 4].view(np.uint32)[0]
-                    p += CELL * int((hdr >> 24) & 63)
-                for _ in range(ntc):
-                    ids.append(st[p:p + 128 * IB * TPL].view(idt).reshape(32 * TPL, 4).astype(np.int64))
-                    idets.append(st[p + 128 * IB * TPL:p + 128 * IB * TPL + 128 * TPL].view(np.float32))
-                    p += CELL
-            assert p == int(wdesc[b, w, 0]) * 16 + int(wdesc[b, w, 1])
+    """(streamed ids [slots, 4], 1/det(Dm) [slots]) of every tet slot of every tet cell, walking each warp's stream."""
+    ids, idets = zip(*(H.tet_cell(plan, c[0]) for c in H.walk_streams(plan)[1]))
     return np.concatenate(ids), np.concatenate(idets)
 
 
@@ -106,18 +64,17 @@ PLAN_CASES = {
 def test_component_tables(case):
     verts, tets, kw = PLAN_CASES[case]()
     plan = build_host_plan(verts, tets, **kw)
-    tab = _comp_tables(verts, tets, **kw)
     comps = _components(len(verts), tets)
     NC, nseg = len(comps), len(plan["segs"])
     assert plan["n_components"] == NC and bool(plan["mode_global"]) == bool(kw.get("force_global"))
-    cs = tab["comp_seg"]
+    cs = plan["comp_seg"]
     assert len(cs) == NC + 1 and cs[0] == 0 and cs[-1] == nseg
     assert np.all(np.diff(cs) >= 1), "every component has a segment"
     owner = np.repeat(np.arange(NC), np.diff(cs))          # each segment lies in exactly one component range
     assert np.array_equal(owner, [sg["comp"] for sg in plan["segs"]])
-    assert np.array_equal(tab["comp_first_vertex"], [v[0] for v, _ in comps])
-    assert np.array_equal(tab["comp_ntets"], [len(t) for _, t in comps])
-    assert tab["comp_ntets"].sum() == len(np.asarray(tets).reshape(-1, 4))
+    assert np.array_equal(plan["comp_first_vertex"], [v[0] for v, _ in comps])
+    assert np.array_equal(plan["comp_ntets"], [len(t) for _, t in comps])
+    assert plan["comp_ntets"].sum() == len(np.asarray(tets).reshape(-1, 4))
     if case == "large_split":
         assert np.diff(cs).max() > 10, "the large spheres must be split over many CTAs"
 

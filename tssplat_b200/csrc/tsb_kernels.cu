@@ -27,8 +27,10 @@
 // partials -> per-CTA pair -> last-arriving CTA folds them in fixed order (deterministic).
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdint>
+#include <utility>
 
 #include "tsb_kernels.cuh"
 
@@ -207,6 +209,15 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
   // float4 index of a segment's u / x arrays inside the staging area (must match tsb_plan.cpp)
   auto ubase_of = [&](const SegHdr &h, int li) -> int { return h.whole ? 0 : (li & 1) * 2 * vh; };
   auto xbase_of = [&](const SegHdr &h, int li) -> int { return h.whole ? h.npos : (li & 1) * 2 * vh + vh; };
+  // global id of a segment's local vertex v
+  auto gid_of = [&](const SegHdr &h, int v) -> size_t { return size_t(h.vbase >= 0 ? h.vbase + v : __ldg(&p.vlist[h.x4off + v])); };
+  auto load_rest = [&](const SegHdr &h, float4 (&X)[SV]) {   // rest positions (.w: staging position) -> registers
+#pragma unroll
+    for (int k = 0; k < SV; ++k) {
+      const int v = tid + k * NT;
+      if (v < h.nv) { X[k] = __ldg(&p.X4[h.x4off + v]); X[k].w = __uint_as_float(uint32_t(__ldg(&p.pos16[h.x4off + v]))); }
+    }
+  };
 
   // the CTA's segment headers and this warp's block counts, cached in shared memory (plan data: before the wait)
   SegHdr *segtab = reinterpret_cast<SegHdr *>(smem + off_segtab(stage_bytes, NW, ring));
@@ -227,13 +238,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
   if (cs.x < cs.y) {
     hcur = p.segs[cs.x];
     if (!GLOBAL && cs.x + 1 < cs.y) h1 = p.segs[cs.x + 1];
-    if (!GLOBAL && !hcur.whole) {   // rest positions of the first component: plan data, loaded before the wait
-#pragma unroll
-      for (int k = 0; k < SV; ++k) {
-        const int v = tid + k * NT;
-        if (v < hcur.nv) { pX[k] = __ldg(&p.X4[hcur.x4off + v]); pX[k].w = __uint_as_float(uint32_t(__ldg(&p.pos16[hcur.x4off + v]))); }
-      }
-    }
+    if (!GLOBAL && !hcur.whole) load_rest(hcur, pX);   // first component: plan data, loaded before the wait
   }
   TSB_STAMP(2);
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -258,36 +263,37 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
   // staged u = rel_u(x_i, X_i, c) with c = fp32(x_r - X_r) of the component's local vertex r = 0 (tsb_plan.cpp,
   // staging_tables): the component's rigid displacement never enters a rounded difference
   auto load_ref = [&](const SegHdr &h, float (&r)[3]) {
-    const size_t gr = size_t(h.vbase >= 0 ? h.vbase : __ldg(&p.vlist[h.x4off]));
+    const size_t gr = gid_of(h, 0);
     const float4 Xr = __ldg(&p.X4[h.x4off]);
     r[0] = __ldcg(p.x + 3 * gr) - Xr.x; r[1] = __ldcg(p.x + 3 * gr + 1) - Xr.y; r[2] = __ldcg(p.x + 3 * gr + 2) - Xr.z;
   };
-  auto load_x = [&](const SegHdr &h) {      // x of a double-buffered component -> registers
+  auto load_x = [&](const SegHdr &h, float (&x)[SV][3]) {      // x of a double-buffered component -> registers
 #pragma unroll
     for (int k = 0; k < SV; ++k) {
       const int v = tid + k * NT;
       if (v < h.nv) {
-        const size_t gi = size_t(h.vbase >= 0 ? h.vbase + v : __ldg(&p.vlist[h.x4off + v]));
-        px[k][0] = __ldcg(p.x + 3 * gi); px[k][1] = __ldcg(p.x + 3 * gi + 1); px[k][2] = __ldcg(p.x + 3 * gi + 2);
+        const size_t gi = gid_of(h, v);
+        x[k][0] = __ldcg(p.x + 3 * gi); x[k][1] = __ldcg(p.x + 3 * gi + 1); x[k][2] = __ldcg(p.x + 3 * gi + 2);
       }
     }
   };
-  auto store_staged_ref = [&](const SegHdr &h, int li, const float (&pr)[3]) {
+  // registers (x, X from load_x / load_rest) -> the component's half-buffer, relative to the reference displacement ref
+  auto store_staged_ref = [&](const SegHdr &h, int li, const float (&x)[SV][3], const float4 (&X)[SV], const float (&ref)[3]) {
     float4 *ub = stage + ubase_of(h, li), *xb = stage + xbase_of(h, li);
 #pragma unroll
     for (int k = 0; k < SV; ++k) {
       const int v = tid + k * NT;
       if (v < h.nv) {
-        const uint32_t pos = __float_as_uint(pX[k].w);
-        ub[pos] = make_float4(rel_u(px[k][0], pX[k].x, pr[0]), rel_u(px[k][1], pX[k].y, pr[1]), rel_u(px[k][2], pX[k].z, pr[2]), 0.f);
-        xb[pos] = make_float4(px[k][0], px[k][1], px[k][2], 0.f);
+        const uint32_t pos = __float_as_uint(X[k].w);
+        ub[pos] = make_float4(rel_u(x[k][0], X[k].x, ref[0]), rel_u(x[k][1], X[k].y, ref[1]), rel_u(x[k][2], X[k].z, ref[2]), 0.f);
+        xb[pos] = make_float4(x[k][0], x[k][1], x[k][2], 0.f);
       }
     }
   };
   auto store_staged = [&](const SegHdr &h, int li) {
     float pr[3];                            // loaded here, not with px: kept out of the segment loop's live registers
     load_ref(h, pr);
-    store_staged_ref(h, li, pr);
+    store_staged_ref(h, li, px, pX, pr);
   };
   auto stage_direct = [&](const SegHdr &h, int li) {   // any size, no register prefetch
     float4 *ub = stage + ubase_of(h, li), *xb = stage + xbase_of(h, li);
@@ -295,7 +301,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
     load_ref(h, r);
     for (int v = tid; v < h.nv; v += NT) {
       const float4 X = __ldg(&p.X4[h.x4off + v]);
-      const size_t gi = size_t(h.vbase >= 0 ? h.vbase + v : __ldg(&p.vlist[h.x4off + v]));
+      const size_t gi = gid_of(h, v);
       const float x0 = __ldcg(p.x + 3 * gi), x1 = __ldcg(p.x + 3 * gi + 1), x2 = __ldcg(p.x + 3 * gi + 2);
       const uint32_t pos = __ldg(&p.pos16[h.x4off + v]);
       ub[pos] = make_float4(rel_u(x0, X.x, r[0]), rel_u(x1, X.y, r[1]), rel_u(x2, X.z, r[2]), 0.f);
@@ -315,41 +321,21 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
         ws.request_rest();
       } else if (!eager2) {
         float pr[3];
-        load_x(hcur); load_ref(hcur, pr);
+        load_x(hcur, px); load_ref(hcur, pr);
         ws.request_rest();
-        store_staged_ref(hcur, 0, pr);
+        store_staged_ref(hcur, 0, px, pX, pr);
       } else {
         // both components' loads in flight together (second register set), then both stores
         float qx[SV][3], qr[3], pr[3];
         float4 qX[SV];
-#pragma unroll
-        for (int k = 0; k < SV; ++k) {
-          const int v = tid + k * NT;
-          if (v < h1.nv) { qX[k] = __ldg(&p.X4[h1.x4off + v]); qX[k].w = __uint_as_float(uint32_t(__ldg(&p.pos16[h1.x4off + v]))); }
-        }
-        load_x(hcur);
+        load_rest(h1, qX);
+        load_x(hcur, px);
         load_ref(h1, qr);
-#pragma unroll
-        for (int k = 0; k < SV; ++k) {
-          const int v = tid + k * NT;
-          if (v < h1.nv) {
-            const size_t gi = size_t(h1.vbase >= 0 ? h1.vbase + v : __ldg(&p.vlist[h1.x4off + v]));
-            qx[k][0] = __ldcg(p.x + 3 * gi); qx[k][1] = __ldcg(p.x + 3 * gi + 1); qx[k][2] = __ldcg(p.x + 3 * gi + 2);
-          }
-        }
+        load_x(h1, qx);
         load_ref(hcur, pr);
         ws.request_rest();
-        store_staged_ref(hcur, 0, pr);
-        float4 *ub = stage + ubase_of(h1, 1), *xb = stage + xbase_of(h1, 1);
-#pragma unroll
-        for (int k = 0; k < SV; ++k) {
-          const int v = tid + k * NT;
-          if (v < h1.nv) {
-            const uint32_t pos = __float_as_uint(qX[k].w);
-            ub[pos] = make_float4(rel_u(qx[k][0], qX[k].x, qr[0]), rel_u(qx[k][1], qX[k].y, qr[1]), rel_u(qx[k][2], qX[k].z, qr[2]), 0.f);
-            xb[pos] = make_float4(qx[k][0], qx[k][1], qx[k][2], 0.f);
-          }
-        }
+        store_staged_ref(hcur, 0, px, pX, pr);
+        store_staged_ref(h1, 1, qx, qX, qr);
       }
     } else {
       ws.request_rest();
@@ -360,6 +346,11 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
     ws.request_rest();
     __syncthreads();      // segment tables visible
   }
+  // SPH reads eager2 back from the segment table: it is not kept live through the segment loop (register budget)
+  auto eager2_of = [&]() -> bool {
+    if constexpr (SPH) return cs.y - cs.x >= 2 && !segtab[0].whole && !segtab[1].whole;
+    else return eager2;
+  };
   ws.begin();
   TSB_STAMP(12);
 
@@ -372,19 +363,11 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
     if (s + 1 < cs.y) {
       hn = seg_at(s + 1);
       if (!GLOBAL) {
-        if constexpr (SPH) {   // eager2 read back from the segment table: not kept live through the loop (register budget)
-          const bool e2 = cs.y - cs.x >= 2 && !segtab[0].whole && !segtab[1].whole;
-          pre = !hcur.whole && !hn.whole && !(li == 0 && e2);
-        } else {
-          pre = !hcur.whole && !hn.whole && !(li == 0 && eager2);
-        }
+        const bool e2 = eager2_of();
+        pre = !hcur.whole && !hn.whole && !(li == 0 && e2);
         if (pre) {
-#pragma unroll
-          for (int k = 0; k < SV; ++k) {
-            const int v = tid + k * NT;
-            if (v < hn.nv) { pX[k] = __ldg(&p.X4[hn.x4off + v]); pX[k].w = __uint_as_float(uint32_t(__ldg(&p.pos16[hn.x4off + v]))); }
-          }
-          load_x(hn);
+          load_rest(hn, pX);
+          load_x(hn, px);
         }
       }
     }
@@ -470,6 +453,13 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
 
     // ---- barrier: TPL tets per lane ---------------------------------------------------------------------
     bool waited = false;
+    auto wait_rows = [&] {   // every row of this component must be stored before we add to it
+      if (!waited) {
+        const unsigned int need = unsigned(hcur.expected);
+        while (ld_acquire(p.done + hcur.comp) < need) __nanosleep(40);
+        waited = true;
+      }
+    };
     const int tcell0 = (amips_on || (DET && grad)) ? __ldg(&p.wtc0[size_t(s) * NW + warp]) : 0;
     // DET: corner vectors c0..c3 of the tet in slot lane * TPL + t of tet cell tcell0 + tc
     auto det_store = [&](int tc, int t, float c0x, float c0y, float c0z, float c1x, float c1y, float c1z, float c2x, float c2y,
@@ -532,11 +522,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
               dmask |= 1u << t;
               continue;
             }
-            if (!waited) {   // every row of this component must be stored before we add to it
-              const unsigned int need = unsigned(hcur.expected);
-              while (ld_acquire(p.done + hcur.comp) < need) __nanosleep(40);
-              waited = true;
-            }
+            wait_rows();
             const size_t v0 = 3 * gid_x(tj[t][0]), v1 = 3 * gid_x(tj[t][1]), v2 = 3 * gid_x(tj[t][2]), v3 = 3 * gid_x(tj[t][3]);
             atomicAdd(grad + v0, -(g1x + g2x + g3x)); atomicAdd(grad + v0 + 1, -(g1y + g2y + g3y)); atomicAdd(grad + v0 + 2, -(g1z + g2z + g3z));
             atomicAdd(grad + v1, g1x); atomicAdd(grad + v1 + 1, g1y); atomicAdd(grad + v1 + 2, g1z);
@@ -590,11 +576,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
               dmask |= 1u << t;
               continue;
             }
-            if (!waited) {
-              const unsigned int need = unsigned(hcur.expected);
-              while (ld_acquire(p.done + hcur.comp) < need) __nanosleep(40);
-              waited = true;
-            }
+            wait_rows();
             float g0[3] = {0.f, 0.f, 0.f};
 #pragma unroll
             for (int k = 0; k < 3; ++k) {       // vertex k+1 pulls with P a_{k+1},  a_{k+1} = row k of B
@@ -627,25 +609,13 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
 
     // ---- hand the staging buffers over ------------------------------------------------------------------
     if (s + 1 < cs.y) {      // (after the last segment the energy fold's own barrier is the only one needed)
-      if (!GLOBAL && SPH) {   // the same as below, with eager2 read back from the segment table
-        const bool e2 = cs.y - cs.x >= 2 && !segtab[0].whole && !segtab[1].whole;
-        if (!(li == 0 && e2)) {
-          if (pre) {
-            if (li == 1 && e2) __syncthreads();
-            store_staged(hn, li + 1);
-          }
-          __syncthreads();
-          if (!pre) {
-            stage_direct(hn, li + 1);
-            __syncthreads();
-          }
-        }
-      } else if (!GLOBAL) {
-        if (li == 0 && eager2) {
+      if (!GLOBAL) {
+        const bool e2 = eager2_of();
+        if (li == 0 && e2) {
           // segment 1 is already staged: no barrier
         } else {
           if (pre) {
-            if (li == 1 && eager2) __syncthreads();     // half 0 is reused: every warp must have left segment 0
+            if (li == 1 && e2) __syncthreads();    // half 0 is reused: every warp must have left segment 0
             store_staged(hn, li + 1);
           }
           __syncthreads();
@@ -924,79 +894,22 @@ inline int grid_for(int64_t count, int block) {
   return int(g < 1 ? 1 : (g > kMaxGrid ? kMaxGrid : g));
 }
 
-template <int NW, int MINB, bool GLOBAL, bool AMIPS, bool DET = false, bool SPH = false>
-cudaError_t launch_variant(const KParams &p, const LaunchConfig &lc, cudaStream_t stream) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(unsigned(lc.grid));
-  cfg.blockDim = dim3(NW * 32);
-  cfg.dynamicSmemBytes = size_t(lc.smem_bytes);
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, energy_grad_kernel<NW, MINB, GLOBAL, AMIPS, DET, SPH>, p);
+// ---- the energy_grad_kernel instantiations, by flag bits f = AMIPS | DET << 1 | SPH << 2 ---------------------------
+using EnergyKernel = void (*)(KParams);
+
+template <int NW, int MINB, bool GLOBAL, int... F>
+const EnergyKernel *flag_table(std::integer_sequence<int, F...>) {
+  static const EnergyKernel table[] = {energy_grad_kernel<NW, MINB, GLOBAL, bool(F & 1), bool(F & 2), bool(F & 4)>...};
+  return table;
 }
 
-template <int NW, int MINB, bool GLOBAL>
-cudaError_t launch_det_variant(const KParams &p, const LaunchConfig &lc, cudaStream_t stream) {
-  return lc.amips ? launch_variant<NW, MINB, GLOBAL, true, true>(p, lc, stream) : launch_variant<NW, MINB, GLOBAL, false, true>(p, lc, stream);
-}
-
-template <int NW, int MINB, bool GLOBAL>
-cudaError_t launch_sph_variant(const KParams &p, const LaunchConfig &lc, cudaStream_t stream) {
-  if (lc.det)
-    return lc.amips ? launch_variant<NW, MINB, GLOBAL, true, true, true>(p, lc, stream) : launch_variant<NW, MINB, GLOBAL, false, true, true>(p, lc, stream);
-  return lc.amips ? launch_variant<NW, MINB, GLOBAL, true, false, true>(p, lc, stream) : launch_variant<NW, MINB, GLOBAL, false, false, true>(p, lc, stream);
-}
-
-// occupancy of the deterministic and SPH instantiations (opts them in to the device's shared memory maximum like the others)
-template <int NW, int MINB, bool GLOBAL, bool AMIPS, bool DET = true, bool SPH = false>
-cudaError_t occupancy_det(int smem_bytes, int optin, int *ctas_per_sm) {
-  cudaError_t e = cudaFuncSetAttribute(energy_grad_kernel<NW, MINB, GLOBAL, AMIPS, DET, SPH>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
-  if (e != cudaSuccess) { *ctas_per_sm = 0; cudaGetLastError(); return cudaSuccess; }
-  return cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, energy_grad_kernel<NW, MINB, GLOBAL, AMIPS, DET, SPH>, NW * 32, size_t(smem_bytes));
-}
-
-// the SPH instantiations a handle may launch: AMIPS ones when amips, DET ones when det
-template <int NW, int MINB, bool GLOBAL>
-cudaError_t occupancy_sph(int smem_bytes, int optin, bool amips, bool det, int *ctas_per_sm) {
-  int v[4] = {1 << 30, 1 << 30, 1 << 30, 1 << 30};
-  cudaError_t e = occupancy_det<NW, MINB, GLOBAL, false, false, true>(smem_bytes, optin, &v[0]);
-  if (e == cudaSuccess && amips) e = occupancy_det<NW, MINB, GLOBAL, true, false, true>(smem_bytes, optin, &v[1]);
-  if (e == cudaSuccess && det) e = occupancy_det<NW, MINB, GLOBAL, false, true, true>(smem_bytes, optin, &v[2]);
-  if (e == cudaSuccess && det && amips) e = occupancy_det<NW, MINB, GLOBAL, true, true, true>(smem_bytes, optin, &v[3]);
-  for (int k = 0; k < 4; ++k)
-    if (v[k] < *ctas_per_sm) *ctas_per_sm = v[k];
-  return e;
-}
-
-template <int NW, int MINB, bool GLOBAL>
-cudaError_t occupancy_variant(int smem_bytes, bool amips, bool det, int *ctas_per_sm) {
-  // opt in to the device maximum once (the attribute is per function, not per handle: handles with different
-  // staging sizes share the kernel)
-  int dev = 0, optin = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  if (e != cudaSuccess) return e;
-  if (smem_bytes > optin) { *ctas_per_sm = 0; return cudaSuccess; }   // does not fit
-  e = cudaFuncSetAttribute(energy_grad_kernel<NW, MINB, GLOBAL, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
-  if (e == cudaSuccess && amips) e = cudaFuncSetAttribute(energy_grad_kernel<NW, MINB, GLOBAL, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
-  if (e != cudaSuccess) { *ctas_per_sm = 0; cudaGetLastError(); return cudaSuccess; }
-  int a = 0, b = 1 << 30;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, energy_grad_kernel<NW, MINB, GLOBAL, false>, NW * 32, size_t(smem_bytes));
-  if (e == cudaSuccess && amips) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, energy_grad_kernel<NW, MINB, GLOBAL, true>, NW * 32, size_t(smem_bytes));
-  *ctas_per_sm = a < b ? a : b;
-  if (e == cudaSuccess && det) {
-    int c = 0, d = 1 << 30;
-    e = occupancy_det<NW, MINB, GLOBAL, false>(smem_bytes, optin, &c);
-    if (e == cudaSuccess && amips) e = occupancy_det<NW, MINB, GLOBAL, true>(smem_bytes, optin, &d);
-    if (c < *ctas_per_sm) *ctas_per_sm = c;
-    if (d < *ctas_per_sm) *ctas_per_sm = d;
-  }
-  if (e == cudaSuccess) e = occupancy_sph<NW, MINB, GLOBAL>(smem_bytes, optin, amips, det, ctas_per_sm);
-  return e;
+// 16 warps run one CTA per SM, 8 warps two; nullptr for any other nw
+EnergyKernel energy_kernel(int nw, bool global, bool amips, bool det, bool sph) {
+  constexpr std::make_integer_sequence<int, 8> flags{};
+  const int f = int(amips) | int(det) << 1 | int(sph) << 2;
+  if (nw == 16) return (global ? flag_table<16, 1, true>(flags) : flag_table<16, 1, false>(flags))[f];
+  if (nw == 8) return (global ? flag_table<8, 2, true>(flags) : flag_table<8, 2, false>(flags))[f];
+  return nullptr;
 }
 
 }  // namespace
@@ -1008,27 +921,52 @@ int energy_smem_bytes(int nw, int ring_slots, int cells_per_chunk, int area_vert
 }
 
 cudaError_t energy_occupancy(int nw, int smem_bytes, bool global, bool amips, bool det, int *ctas_per_sm) {
-  if (nw == 16) return global ? occupancy_variant<16, 1, true>(smem_bytes, amips, det, ctas_per_sm) : occupancy_variant<16, 1, false>(smem_bytes, amips, det, ctas_per_sm);
-  if (nw == 8) return global ? occupancy_variant<8, 2, true>(smem_bytes, amips, det, ctas_per_sm) : occupancy_variant<8, 2, false>(smem_bytes, amips, det, ctas_per_sm);
-  return cudaErrorInvalidValue;
+  if (!energy_kernel(nw, global, false, false, false)) return cudaErrorInvalidValue;
+  // opt in to the device maximum (the attribute is per function, not per handle: handles with different staging sizes
+  // share the kernel)
+  int dev = 0, optin = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  if (e != cudaSuccess) return e;
+  *ctas_per_sm = 0;
+  if (smem_bytes > optin) return cudaSuccess;   // does not fit
+  // every instantiation the handle may launch: AMIPS ones when amips, DET ones when det, with and without SPH
+  int ctas = 1 << 30;
+  for (int f = 0; f < 8; ++f) {
+    if (((f & 1) && !amips) || ((f & 2) && !det)) continue;
+    const EnergyKernel k = energy_kernel(nw, global, f & 1, f & 2, f & 4);
+    if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, optin) != cudaSuccess) {
+      cudaGetLastError();
+      return cudaSuccess;   // does not fit
+    }
+    int c = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, k, nw * 32, size_t(smem_bytes));
+    if (e != cudaSuccess) return e;
+    ctas = std::min(ctas, c);
+  }
+  *ctas_per_sm = ctas;
+  return cudaSuccess;
 }
 
 cudaError_t launch_energy_grad(const KParams &p, const LaunchConfig &lc, cudaStream_t stream) {
+  const EnergyKernel k = energy_kernel(lc.nw, lc.global, lc.amips, lc.det, lc.sph);
+  if (!k) return cudaErrorInvalidValue;
   if (lc.global) {
     prestage_kernel<<<grid_for(p.n, 256), 256, 0, stream>>>(p.x, p.X4, p.u4g, p.x4g, p.n);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
-    if (lc.sph) return lc.nw == 16 ? launch_sph_variant<16, 1, true>(p, lc, stream) : launch_sph_variant<8, 2, true>(p, lc, stream);
-    if (lc.det) return lc.nw == 16 ? launch_det_variant<16, 1, true>(p, lc, stream) : launch_det_variant<8, 2, true>(p, lc, stream);
-    if (lc.nw == 16) return lc.amips ? launch_variant<16, 1, true, true>(p, lc, stream) : launch_variant<16, 1, true, false>(p, lc, stream);
-    if (lc.nw == 8) return lc.amips ? launch_variant<8, 2, true, true>(p, lc, stream) : launch_variant<8, 2, true, false>(p, lc, stream);
-    return cudaErrorInvalidValue;
   }
-  if (lc.sph) return lc.nw == 16 ? launch_sph_variant<16, 1, false>(p, lc, stream) : launch_sph_variant<8, 2, false>(p, lc, stream);
-  if (lc.det) return lc.nw == 16 ? launch_det_variant<16, 1, false>(p, lc, stream) : launch_det_variant<8, 2, false>(p, lc, stream);
-  if (lc.nw == 16) return lc.amips ? launch_variant<16, 1, false, true>(p, lc, stream) : launch_variant<16, 1, false, false>(p, lc, stream);
-  if (lc.nw == 8) return lc.amips ? launch_variant<8, 2, false, true>(p, lc, stream) : launch_variant<8, 2, false, false>(p, lc, stream);
-  return cudaErrorInvalidValue;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(unsigned(lc.grid));
+  cfg.blockDim = dim3(unsigned(lc.nw * 32));
+  cfg.dynamicSmemBytes = size_t(lc.smem_bytes);
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  return cudaLaunchKernelEx(&cfg, k, p);
 }
 
 // A plain launch (the gather starts when the energy kernel has finished); its early launch_dependents still lets the

@@ -101,8 +101,9 @@ struct DetParams {
 int energy_ring_bytes(int ring_slots, int cells_per_chunk, bool global);
 int energy_smem_bytes(int nw, int ring_slots, int cells_per_chunk, int area_verts, bool global);
 constexpr unsigned long long kEnergySentinel = 0x7FF8F00DBAADC0DEull;   // initial value of cta_energy
-// Max co-resident CTAs per SM for a configuration (0 if it does not fit); also opts in to the smem size.  det: the
-// deterministic instantiations count too.
+// Max co-resident CTAs per SM for a configuration (0 if it does not fit): the minimum over every instantiation a handle
+// may launch (AMIPS ones when amips, deterministic ones when det, each with and without the sphere records); also opts
+// them in to the smem size.
 cudaError_t energy_occupancy(int nw, int smem_bytes, bool global, bool amips, bool det, int *ctas_per_sm);
 cudaError_t launch_energy_grad(const KParams &p, const LaunchConfig &lc, cudaStream_t stream);
 // grad[v] += the active corner vectors of v's list, in list order, for every flagged component (after a DET launch).

@@ -16,7 +16,9 @@ extern "C" {
 
 const char *tsbdbg_last_error() { return g_err.c_str(); }
 
-/* tsbdbg_build_ex plus deterministic (emit the deterministic gather's lists "det_*" and the tet-cell numbering "wtc0") */
+/* The plan tsb_create would build.  ring_cells: the ring it requests (ring_slots * kCellsPerChunk; 0 = the default);
+   enable_amips: emit the AMIPS rest inverses "Bt" and the tet-cell numbering "wtc0"; deterministic: emit the
+   deterministic gather's lists "det_*" and "wtc0".  vh_cap, area_cap, tet_cost: 0 = the default. */
 int tsbdbg_build_det(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele, int32_t nw, int32_t grid,
                      int32_t laplacian_scale, int32_t force_global, int32_t vh_cap, int32_t area_cap, float tet_cost,
                      int32_t ring_cells, int32_t enable_amips, int32_t deterministic, tsbdbg_plan **out) {
@@ -37,8 +39,8 @@ int tsbdbg_build_det(const float *rest_xyz, const int32_t *tets, int32_t n, int3
   return TSB_OK;
 }
 
-/* tsbdbg_build plus ring_cells (the ring tsb_create requests: ring_slots * kCellsPerChunk; 0 = the default) and
-   enable_amips (emit the AMIPS rest inverses "Bt" / "wtc0") */
+/* tsbdbg_build_det with deterministic = 0: the entry point earlier test helpers call, so that they keep running
+   against this library */
 int tsbdbg_build_ex(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele, int32_t nw, int32_t grid,
                     int32_t laplacian_scale, int32_t force_global, int32_t vh_cap, int32_t area_cap, float tet_cost,
                     int32_t ring_cells, int32_t enable_amips, tsbdbg_plan **out) {
@@ -46,13 +48,7 @@ int tsbdbg_build_ex(const float *rest_xyz, const int32_t *tets, int32_t n, int32
                           ring_cells, enable_amips, 0, out);
 }
 
-int tsbdbg_build(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele, int32_t nw, int32_t grid,
-                 int32_t laplacian_scale, int32_t force_global, int32_t vh_cap, int32_t area_cap, float tet_cost,
-                 tsbdbg_plan **out) {
-  return tsbdbg_build_ex(rest_xyz, tets, n, nele, nw, grid, laplacian_scale, force_global, vh_cap, area_cap, tet_cost, 0, 0, out);
-}
-
-/* name -> (pointer, element count, element bytes); TSB_E_INVALID for an unknown name */
+/* name ->(pointer, element count, element bytes); TSB_E_INVALID for an unknown name */
 int tsbdbg_array(tsbdbg_plan *d, const char *name, const void **ptr, int64_t *count, int32_t *elem_bytes) {
   if (!d || !name || !ptr || !count || !elem_bytes) return TSB_E_INVALID;
   const tsb::HostPlan &P = d->plan;

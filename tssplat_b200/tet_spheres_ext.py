@@ -166,6 +166,14 @@ class TetSpheres:
             raise RuntimeError(f"vertexPositions has {x.numel()} entries, expected {self.n3}")
         return x if x.is_contiguous() else x.contiguous()            # tet_spheres_cuda.cu:124
 
+    def _gradH_arg(self, gradH):
+        """gradH as the C ABI takes it: (host value, device pointer or None, tensor to keep alive until the launch is
+        enqueued).  A CUDA tensor is read on the device (its first entry, as fp32); anything else is a host float."""
+        if isinstance(gradH, torch.Tensor) and gradH.is_cuda:
+            keep = gradH.detach().to(device=self.device, dtype=torch.float32).reshape(-1)[:1].contiguous()
+            return 1.0, keep.data_ptr(), keep
+        return float(gradH), None, None
+
     def energy_grad(self, x: torch.Tensor, c1: float, c2: float, order: int, gradH=1.0,
                     want_grad: bool = True, c3: float = 0.0):
         """The fused launch.  Returns (energy[3] = total/smooth/barrier on device, grad or None); with ``c3``
@@ -177,15 +185,7 @@ class TetSpheres:
         energy = self._ring4[i] if c3 else self._ring3[i]
         e_ptr = self._ring_ptr + 16 * i
         grad = torch.empty((self.n, 3), dtype=torch.float32, device=self.device) if want_grad else None
-        gh_val, gh_ptr, keep = 1.0, None, None
-        if isinstance(gradH, torch.Tensor):
-            if gradH.is_cuda:
-                keep = gradH.detach().to(device=self.device, dtype=torch.float32).reshape(-1)[:1].contiguous()
-                gh_ptr = keep.data_ptr()
-            else:
-                gh_val = float(gradH)
-        else:
-            gh_val = float(gradH)
+        gh_val, gh_ptr, keep = self._gradH_arg(gradH)
         if c3:
             terms = _capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
             rc = _capi.lib.tsb_energy_grad_ex(self._h, xc.data_ptr(), C.byref(terms), gh_val, gh_ptr, e_ptr,
@@ -211,12 +211,7 @@ class TetSpheres:
         energy = torch.empty(4, dtype=torch.float32, device=self.device)
         grad = torch.empty((self.n, 3), dtype=torch.float32, device=self.device) if want_grad else None
         raw = torch.empty((S, _STATS_BYTES), dtype=torch.uint8, device=self.device)
-        gh_val, gh_ptr, keep = 1.0, None, None
-        if isinstance(gradH, torch.Tensor) and gradH.is_cuda:
-            keep = gradH.detach().to(device=self.device, dtype=torch.float32).reshape(-1)[:1].contiguous()
-            gh_ptr = keep.data_ptr()
-        else:
-            gh_val = float(gradH)
+        gh_val, gh_ptr, keep = self._gradH_arg(gradH)
         terms = _capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
         rc = _capi.lib.tsb_energy_grad_spheres(self._h, xc.data_ptr(), C.byref(terms), gh_val, gh_ptr, energy.data_ptr(),
                                                grad.data_ptr() if want_grad else None, raw.data_ptr(),
