@@ -194,7 +194,8 @@ int tsb_adam_uniform_step(float *p_dev, const float *grad_dev, float *g1_dev, fl
 /* ---- "Next" row (f)2: surface gather + vertex-normal splat ------------------------------------------------
  * Replaces `tet_v[surface_vid]` (geometry/tetmesh_geometry.py:33) and `_compute_vertex_normal`
  * (geometry/tetmesh_geometry.py:39-66) and their autograd backward.  surface_vid: host int32 [nsv] tet-mesh
- * vertex of each surface vertex (unique); surface_f: host int32 [3*nsf] triangles over surface-vertex ids.
+ * vertex of each surface vertex, each id at most once (a repeat is rejected with TSB_E_MESH: every gradient row has
+ * one writer); surface_f: host int32 [3*nsf] triangles over surface-vertex ids.
  * One handle may serve one stream at a time (it owns a backward scratch array). */
 typedef struct tsb_surface_s *tsb_surface_t;
 int tsb_surface_create(const int32_t *surface_vid, int32_t nsv, const int32_t *surface_f, int32_t nsf,

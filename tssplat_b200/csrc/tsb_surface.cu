@@ -136,7 +136,16 @@ int tsb_surface_create(const int32_t *surface_vid, int32_t nsv, const int32_t *s
   *out = nullptr;
   if (!surface_vid || !surface_f || nsv <= 0 || nsf <= 0 || n_tet_vertices <= 0) return sfail(nullptr, TSB_E_INVALID, "null input or non-positive size");
   std::vector<int32_t> svid(surface_vid, surface_vid + nsv), faces(surface_f, surface_f + 3 * size_t(nsf));
-  for (int32_t v : svid) if (v < 0 || v >= n_tet_vertices) return sfail(nullptr, TSB_E_MESH, "surface_vid out of range");
+  {
+    // one writer per gradient row: a repeated id would have two threads of surface_backward_kernel store the same row
+    std::vector<uint8_t> seen(size_t(n_tet_vertices), 0);
+    for (int32_t i = 0; i < nsv; ++i) {
+      const int32_t v = svid[i];
+      if (v < 0 || v >= n_tet_vertices) return sfail(nullptr, TSB_E_MESH, "surface_vid out of range");
+      if (seen[size_t(v)]) return sfail(nullptr, TSB_E_MESH, "surface_vid repeats tet vertex " + std::to_string(v) + " (entry " + std::to_string(i) + ")");
+      seen[size_t(v)] = 1;
+    }
+  }
   std::vector<int32_t> inc_ptr(size_t(nsv) + 1, 0), inc(3 * size_t(nsf));
   for (int32_t v : faces) {
     if (v < 0 || v >= nsv) return sfail(nullptr, TSB_E_MESH, "surface face index out of range");
