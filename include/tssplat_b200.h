@@ -20,7 +20,7 @@
 extern "C" {
 #endif
 
-#define TSB_VERSION 2
+#define TSB_VERSION 3
 
 enum {
   TSB_OK = 0,
@@ -154,6 +154,23 @@ typedef struct {
 int tsb_energy_grad_spheres(tsb_handle_t h, const float *x_dev, const tsb_terms_t *terms, float gradH,
                             const float *gradH_dev, float *energy_out_dev, float *grad_out_dev,
                             tsb_sphere_stats_t *spheres_out_dev, void *stream);
+
+/* Hessian-vector product of the smoothness and barrier energy (no counterpart in the reference):
+ *   hv_out   = gradH * (*gradH_dev) * H(x) v       ([n,3] fp32, fully overwritten, required)
+ *   curv_out = v^T H v as { c1*vMv + c2*vHbv, vMv, vHbv }   (optional device float[3]; NOT scaled by gradH)
+ * with H(x) = c1 M + c2 sum_t H_t(x): M = G^T L^T L G (the smoothness Hessian: 1/2 x^T M x has Hessian M), and H_t the
+ * Hessian of max(-J_t, 0)^order, nonzero only for tets whose fp32 J (the value tsb_energy_grad tests) is negative.
+ * vMv = v^T M v and vHbv = sum_t v^T H_t v.  H_t is the exact, indefinite tet Hessian (no SPD projection).
+ * The AMIPS term is NOT part of the product: tsb_hvp differentiates c1*smooth + c2*barrier only, also on handles
+ * created with enable_amips.  x_dev, v_dev: device float32 [3n], contiguous; order 2 or 4; vertices no tet references
+ * get zero rows.  The launch streams the same plan as tsb_energy_grad (one kernel, plus the gather on deterministic
+ * handles) and works on every handle: it leaves the handle's scratch as the next tsb_energy_grad expects, so the
+ * two may be chained on one stream.  Rows no inverted tet touches are bitwise repeatable on every handle (and equal
+ * across default and deterministic handles of the same options); inverted tets add their H_t v with
+ * red.global.add.f32 on a default handle, and through the deterministic gather on a deterministic handle, where hv
+ * and curv are then bitwise identical across launches, streams and CUDA-graph replays.  DESIGN.md section 5. */
+int tsb_hvp(tsb_handle_t h, const float *x_dev, const float *v_dev, float c1, float c2, int32_t order,
+            float gradH, const float *gradH_dev, float *hv_out_dev, float *curv_out_dev, void *stream);
 
 /* Same computation for callers whose vertex positions live in HOST memory (e.g. a CPU-side
  * optimiser): copies x_host -> device, runs the fused launch, copies energy[3] and grad back,

@@ -314,6 +314,30 @@ int tsb_energy_grad_spheres(tsb_handle_t h, const float *x_dev, const tsb_terms_
                           spheres_out_dev, stream);
 }
 
+int tsb_hvp(tsb_handle_t h, const float *x_dev, const float *v_dev, float c1, float c2, int32_t order, float gradH,
+            const float *gradH_dev, float *hv_out_dev, float *curv_out_dev, void *stream) {
+  if (!h) return TSB_E_INVALID;
+  if (!x_dev || !v_dev || !hv_out_dev) return fail(h, TSB_E_INVALID, "x_dev, v_dev and hv_out_dev must be non-null");
+  if (order != 2 && order != 4) return fail(h, TSB_E_INVALID, "order must be 2 or 4");
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return fail(h, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  tsb::KParams kp = h->kp;
+  kp.x = x_dev; kp.v = v_dev; kp.grad = hv_out_dev; kp.energy_out = curv_out_dev; kp.gradH_dev = gradH_dev;
+  kp.c1 = c1; kp.c2 = c2; kp.c3 = 0.f; kp.gradH = gradH; kp.order = order; kp.energy4 = 0;
+  tsb::LaunchConfig lc = h->lc;
+  lc.amips = 0;
+  lc.det = h->det ? 1 : 0;
+  lc.sph = 0;
+  lc.hvp = 1;
+  cudaError_t e = tsb::launch_energy_grad(kp, lc, static_cast<cudaStream_t>(stream));
+  if (e != cudaSuccess) return fail(h, TSB_E_CUDA, std::string("hvp launch: ") + cudaGetErrorString(e));
+  if (lc.det) {
+    e = tsb::launch_det_gather(h->dp, hv_out_dev, static_cast<cudaStream_t>(stream));
+    if (e != cudaSuccess) return fail(h, TSB_E_CUDA, std::string("deterministic gather launch: ") + cudaGetErrorString(e));
+  }
+  return TSB_OK;
+}
+
 int tsb_energy_grad_host(tsb_handle_t h, const float *x_host, float c1, float c2, int32_t order, float gradH,
                          float *energy_out_host, float *grad_out_host, void *stream) {
   if (!h) return TSB_E_INVALID;

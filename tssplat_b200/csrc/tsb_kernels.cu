@@ -166,7 +166,10 @@ struct WarpStream {
 // SPH (tsb_energy_grad_spheres): at the end of every segment each warp reduces its lanes' energy partials, inverted-tet
 // count and smallest J, and lane 0 stores them as the (segment, warp) record; the running totals move to the warp's
 // red[] slot, so the CTA fold below is unchanged.  sphere_fold_kernel turns the records into per-component statistics.
-template <int NW, int MINB, bool GLOBAL, bool AMIPS, bool DET = false, bool SPH = false>
+// HVP (tsb_hvp; never with AMIPS or SPH): the u slots hold v - v_ref instead of x - X, so the row pass yields M v, an
+// inverted tet adds its H_t v instead of its gradient (through the same scratch or atomics), and the energy partials
+// carry v^T M v and v^T H_t v (DESIGN.md section 5).  x stays in the x slots: the active set is the gradient's.
+template <int NW, int MINB, bool GLOBAL, bool AMIPS, bool DET = false, bool SPH = false, bool HVP = false>
 __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParams p) {
   using F = Fmt<GLOBAL>;
   constexpr int NT = NW * 32;
@@ -215,7 +218,8 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
 #pragma unroll
     for (int k = 0; k < SV; ++k) {
       const int v = tid + k * NT;
-      if (v < h.nv) { X[k] = __ldg(&p.X4[h.x4off + v]); X[k].w = __uint_as_float(uint32_t(__ldg(&p.pos16[h.x4off + v]))); }
+      // HVP: load_x fills xyz with v, and store_staged_ref reads the staging position itself (register budget)
+      if (!HVP && v < h.nv) { X[k] = __ldg(&p.X4[h.x4off + v]); X[k].w = __uint_as_float(uint32_t(__ldg(&p.pos16[h.x4off + v]))); }
     }
   };
 
@@ -261,19 +265,26 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
   if (SPH && lane == 0) { red[3 * warp] = 0.0; red[3 * warp + 1] = 0.0; red[3 * warp + 2] = 0.0; }
 
   // staged u = rel_u(x_i, X_i, c) with c = fp32(x_r - X_r) of the component's local vertex r = 0 (tsb_plan.cpp,
-  // staging_tables): the component's rigid displacement never enters a rounded difference
+  // staging_tables): the component's rigid displacement never enters a rounded difference.  HVP: c = v_r, and the
+  // u slots hold v_i - v_r
   auto load_ref = [&](const SegHdr &h, float (&r)[3]) {
     const size_t gr = gid_of(h, 0);
-    const float4 Xr = __ldg(&p.X4[h.x4off]);
-    r[0] = __ldcg(p.x + 3 * gr) - Xr.x; r[1] = __ldcg(p.x + 3 * gr + 1) - Xr.y; r[2] = __ldcg(p.x + 3 * gr + 2) - Xr.z;
+    if constexpr (HVP) {
+      r[0] = __ldcg(p.v + 3 * gr); r[1] = __ldcg(p.v + 3 * gr + 1); r[2] = __ldcg(p.v + 3 * gr + 2);
+    } else {
+      const float4 Xr = __ldg(&p.X4[h.x4off]);
+      r[0] = __ldcg(p.x + 3 * gr) - Xr.x; r[1] = __ldcg(p.x + 3 * gr + 1) - Xr.y; r[2] = __ldcg(p.x + 3 * gr + 2) - Xr.z;
+    }
   };
-  auto load_x = [&](const SegHdr &h, float (&x)[SV][3]) {      // x of a double-buffered component -> registers
+  // x of a double-buffered component -> registers; HVP: v as well, into X's xyz (its .w, the staging position, stays)
+  auto load_x = [&](const SegHdr &h, float (&x)[SV][3], float4 (&X)[SV]) {
 #pragma unroll
     for (int k = 0; k < SV; ++k) {
       const int v = tid + k * NT;
       if (v < h.nv) {
         const size_t gi = gid_of(h, v);
         x[k][0] = __ldcg(p.x + 3 * gi); x[k][1] = __ldcg(p.x + 3 * gi + 1); x[k][2] = __ldcg(p.x + 3 * gi + 2);
+        if constexpr (HVP) { X[k].x = __ldcg(p.v + 3 * gi); X[k].y = __ldcg(p.v + 3 * gi + 1); X[k].z = __ldcg(p.v + 3 * gi + 2); }
       }
     }
   };
@@ -284,8 +295,9 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
     for (int k = 0; k < SV; ++k) {
       const int v = tid + k * NT;
       if (v < h.nv) {
-        const uint32_t pos = __float_as_uint(X[k].w);
-        ub[pos] = make_float4(rel_u(x[k][0], X[k].x, ref[0]), rel_u(x[k][1], X[k].y, ref[1]), rel_u(x[k][2], X[k].z, ref[2]), 0.f);
+        const uint32_t pos = HVP ? uint32_t(__ldg(&p.pos16[h.x4off + v])) : __float_as_uint(X[k].w);
+        if constexpr (HVP) ub[pos] = make_float4(X[k].x - ref[0], X[k].y - ref[1], X[k].z - ref[2], 0.f);
+        else ub[pos] = make_float4(rel_u(x[k][0], X[k].x, ref[0]), rel_u(x[k][1], X[k].y, ref[1]), rel_u(x[k][2], X[k].z, ref[2]), 0.f);
         xb[pos] = make_float4(x[k][0], x[k][1], x[k][2], 0.f);
       }
     }
@@ -304,7 +316,8 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
       const size_t gi = gid_of(h, v);
       const float x0 = __ldcg(p.x + 3 * gi), x1 = __ldcg(p.x + 3 * gi + 1), x2 = __ldcg(p.x + 3 * gi + 2);
       const uint32_t pos = __ldg(&p.pos16[h.x4off + v]);
-      ub[pos] = make_float4(rel_u(x0, X.x, r[0]), rel_u(x1, X.y, r[1]), rel_u(x2, X.z, r[2]), 0.f);
+      if constexpr (HVP) ub[pos] = make_float4(__ldcg(p.v + 3 * gi) - r[0], __ldcg(p.v + 3 * gi + 1) - r[1], __ldcg(p.v + 3 * gi + 2) - r[2], 0.f);
+      else ub[pos] = make_float4(rel_u(x0, X.x, r[0]), rel_u(x1, X.y, r[1]), rel_u(x2, X.z, r[2]), 0.f);
       xb[pos] = make_float4(x0, x1, x2, 0.f);
     }
   };
@@ -321,7 +334,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
         ws.request_rest();
       } else if (!eager2) {
         float pr[3];
-        load_x(hcur, px); load_ref(hcur, pr);
+        load_x(hcur, px, pX); load_ref(hcur, pr);
         ws.request_rest();
         store_staged_ref(hcur, 0, px, pX, pr);
       } else {
@@ -329,9 +342,9 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
         float qx[SV][3], qr[3], pr[3];
         float4 qX[SV];
         load_rest(h1, qX);
-        load_x(hcur, px);
+        load_x(hcur, px, pX);
         load_ref(h1, qr);
-        load_x(h1, qx);
+        load_x(h1, qx, qX);
         load_ref(hcur, pr);
         ws.request_rest();
         store_staged_ref(hcur, 0, px, pX, pr);
@@ -367,7 +380,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
         pre = !hcur.whole && !hn.whole && !(li == 0 && e2);
         if (pre) {
           load_rest(hn, pX);
-          load_x(hn, px);
+          load_x(hn, px, pX);
         }
       }
     }
@@ -380,6 +393,12 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
     auto gid_x = [&](uint32_t j) -> size_t {
       if (GLOBAL) return size_t(j);
       return size_t(__ldg(&p.pos_gid[hcur.p4off + ((j - uint32_t(xb16)) >> 4)]));
+    };
+    // HVP: staged v - v_ref of the vertex whose x is gathered at j; STAGED: its u slot lies a fixed distance below,
+    // formed here (kept live through the row pass, it would cost a register)
+    auto gatherV = [&](uint32_t j) -> float4 {
+      const uint32_t dv16 = GLOBAL ? 0u : uint32_t(hcur.whole ? hcur.npos : p.vh) * 16u;   // xbase_of - ubase_of
+      return gatherU(j - dv16);
     };
     // reference displacement of the component: sum_i g_i = 0, so 1/2 sum_i (u_i - uref).g_i is the same
     // energy with the rigid translation taken out of the cancellation
@@ -508,7 +527,48 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
           mnK = min(mnK, __reduce_min_sync(0xffffffffu, kJ));
           nneg += __popc(__ballot_sync(0xffffffffu, J < 0.f));
         }
-        if (J < 0.f) {
+        if (HVP && J < 0.f) {
+          // H_t v = phi''(J) dJ g + phi'(J) dg with g_k = dJ/dx_k, dJ = sum_k g_k.f_k and dg_k its derivative along v
+          // (f_k = v_k - v_0); phi = (-J)^p.  v^T H_t v = sum_{k=1..3} f_k.(H_t v)_k
+          const float m = -J, m2 = m * m;
+          const float4 w0 = gatherV(tj[t][0]), w1 = gatherV(tj[t][1]), w2 = gatherV(tj[t][2]), w3 = gatherV(tj[t][3]);
+          const float f1x = w1.x - w0.x, f1y = w1.y - w0.y, f1z = w1.z - w0.z;
+          const float f2x = w2.x - w0.x, f2y = w2.y - w0.y, f2z = w2.z - w0.z;
+          const float f3x = w3.x - w0.x, f3y = w3.y - w0.y, f3z = w3.z - w0.z;
+          // (H_t v)_k = a c_k - b dc_k with c1 = e2 x e3, c2 = e3 x e1, c3 = e1 x e2 and their derivatives along v
+          // dc1 = f2 x e3 + e2 x f3, dc2 = f3 x e1 + e3 x f1, dc3 = f1 x e2 + e1 x f2.  dJ det(Dm) = f1.c1 + f2.c2 + f3.c3
+          // = f1.c1 + e1.dc1, so each k needs only its own c_k, dc_k (fewer live registers)
+          const float d1x = (f2y * e3z - f2z * e3y) + (e2y * f3z - e2z * f3y);
+          const float d1y = (f2z * e3x - f2x * e3z) + (e2z * f3x - e2x * f3z);
+          const float d1z = (f2x * e3y - f2y * e3x) + (e2x * f3y - e2y * f3x);
+          const float dJ = (f1x * c1x + f1y * c1y + f1z * c1z + e1x * d1x + e1y * d1y + e1z * d1z) * idet;
+          const float a = (order2 ? 2.f : 12.f * m2) * dJ * idet;    // p (p-1) (-J)^(p-2) dJ / det(Dm)
+          const float b = (order2 ? 2.f * m : 4.f * m2 * m) * idet;  // p (-J)^(p-1) / det(Dm)
+          // corner k of gradH c2 H_t v leaves as soon as it is formed (register budget): DET into the tet slot's 12 floats
+          // (the layout det_store writes), otherwise added to hv after the component's rows
+          if constexpr (DET) dmask |= 1u << t;
+          else wait_rows();
+          float *dst = reinterpret_cast<float *>(p.det_scratch + 3 * (size_t(tcell0 + tc) * (32 * F::TPL) + lane * F::TPL + t));
+          float g0x = 0.f, g0y = 0.f, g0z = 0.f;
+          float q = 0.f;
+          auto put = [&](int k, float hx, float hy, float hz, float fx, float fy, float fz) {
+            q += fx * hx + fy * hy + fz * hz;
+            const float gx = s2 * hx, gy = s2 * hy, gz = s2 * hz;
+            g0x -= gx; g0y -= gy; g0z -= gz;
+            if constexpr (DET) { dst[3 * k] = gx; dst[3 * k + 1] = gy; dst[3 * k + 2] = gz; }
+            else { const size_t vk = 3 * gid_x(tj[t][k]); atomicAdd(grad + vk, gx); atomicAdd(grad + vk + 1, gy); atomicAdd(grad + vk + 2, gz); }
+          };
+          put(1, a * c1x - b * d1x, a * c1y - b * d1y, a * c1z - b * d1z, f1x, f1y, f1z);
+          put(2, a * (e3y * e1z - e3z * e1y) - b * ((f3y * e1z - f3z * e1y) + (e3y * f1z - e3z * f1y)),
+              a * (e3z * e1x - e3x * e1z) - b * ((f3z * e1x - f3x * e1z) + (e3z * f1x - e3x * f1z)),
+              a * (e3x * e1y - e3y * e1x) - b * ((f3x * e1y - f3y * e1x) + (e3x * f1y - e3y * f1x)), f2x, f2y, f2z);
+          put(3, a * (e1y * e2z - e1z * e2y) - b * ((f1y * e2z - f1z * e2y) + (e1y * f2z - e1z * f2y)),
+              a * (e1z * e2x - e1x * e2z) - b * ((f1z * e2x - f1x * e2z) + (e1z * f2x - e1x * f2z)),
+              a * (e1x * e2y - e1y * e2x) - b * ((f1x * e2y - f1y * e2x) + (e1x * f2y - e1y * f2x)), f3x, f3y, f3z);
+          deb += double(q);   // v^T H_t v
+          if constexpr (DET) { dst[0] = g0x; dst[1] = g0y; dst[2] = g0z; }
+          else { const size_t v0 = 3 * gid_x(tj[t][0]); atomicAdd(grad + v0, g0x); atomicAdd(grad + v0 + 1, g0y); atomicAdd(grad + v0 + 2, g0z); }
+        } else if (!HVP && J < 0.f) {
           const float m = -J, m2 = m * m;
           deb += double(order2 ? m2 : m2 * m2);
           if (grad) {
@@ -655,7 +715,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
   if (tid == 0) {
     double a = 0.0, b = 0.0, c = 0.0;
     for (int w = 0; w < NW; ++w) { a += red[3 * w]; b += red[3 * w + 1]; c += red[3 * w + 2]; }
-    a *= 0.5;
+    if constexpr (!HVP) a *= 0.5;   // HVP: v^T M v itself
     // two 16-byte stores carry the partials; their arrival IS the "this CTA is done" signal (no fence, no ticket)
     unsigned long long ua = (unsigned long long)__double_as_longlong(a), ub = (unsigned long long)__double_as_longlong(b);
     unsigned long long uc = (unsigned long long)__double_as_longlong(c);
@@ -703,7 +763,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
       }
     }
     a = warp_sum(a); b = warp_sum(b); c3sum = warp_sum(c3sum);
-    if (lane == 0) {
+    if (lane == 0 && (!HVP || p.energy_out)) {   // HVP: energy_out is the optional curvature
       p.energy_out[0] = float(double(p.c1) * a + double(p.c2) * b + double(p.c3) * c3sum);
       p.energy_out[1] = float(a);
       p.energy_out[2] = float(b);
@@ -730,6 +790,16 @@ __global__ void prestage_kernel(const float *__restrict__ x, const float4 *__res
     const float c0 = x[3 * r] - Xr.x, c1 = x[3 * r + 1] - Xr.y, c2 = x[3 * r + 2] - Xr.z;
     u4[v] = make_float4(rel_u(a, X.x, c0), rel_u(b, X.y, c1), rel_u(c, X.z, c2), 0.f);
     x4[v] = make_float4(a, b, c, 0.f);
+  }
+}
+
+// The same for the HVP instantiation: u = v - v_r with r = X4[v].w, and x as float4 per vertex.
+__global__ void prestage_hvp_kernel(const float *__restrict__ x, const float *__restrict__ dir, const float4 *__restrict__ X4,
+                                    float4 *__restrict__ u4, float4 *__restrict__ x4, int n) {
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < n; v += gridDim.x * blockDim.x) {
+    const size_t r = size_t(__float_as_uint(X4[v].w));
+    u4[v] = make_float4(dir[3 * size_t(v)] - dir[3 * r], dir[3 * size_t(v) + 1] - dir[3 * r + 1], dir[3 * size_t(v) + 2] - dir[3 * r + 2], 0.f);
+    x4[v] = make_float4(x[3 * size_t(v)], x[3 * size_t(v) + 1], x[3 * size_t(v) + 2], 0.f);
   }
 }
 
@@ -894,19 +964,26 @@ inline int grid_for(int64_t count, int block) {
   return int(g < 1 ? 1 : (g > kMaxGrid ? kMaxGrid : g));
 }
 
-// ---- the energy_grad_kernel instantiations, by flag bits f = AMIPS | DET << 1 | SPH << 2 ---------------------------
+// ---- the energy_grad_kernel instantiations, by flag bits f = AMIPS | DET << 1 | SPH << 2 | HVP << 3 -----------------
 using EnergyKernel = void (*)(KParams);
+
+// HVP is never combined with AMIPS or SPH: those entries are nullptr and never instantiated
+template <int NW, int MINB, bool GLOBAL, int F>
+constexpr EnergyKernel kernel_of() {
+  if constexpr ((F & 8) && (F & 5)) return nullptr;
+  else return energy_grad_kernel<NW, MINB, GLOBAL, bool(F & 1), bool(F & 2), bool(F & 4), bool(F & 8)>;
+}
 
 template <int NW, int MINB, bool GLOBAL, int... F>
 const EnergyKernel *flag_table(std::integer_sequence<int, F...>) {
-  static const EnergyKernel table[] = {energy_grad_kernel<NW, MINB, GLOBAL, bool(F & 1), bool(F & 2), bool(F & 4)>...};
+  static const EnergyKernel table[] = {kernel_of<NW, MINB, GLOBAL, F>()...};
   return table;
 }
 
-// 16 warps run one CTA per SM, 8 warps two; nullptr for any other nw
-EnergyKernel energy_kernel(int nw, bool global, bool amips, bool det, bool sph) {
-  constexpr std::make_integer_sequence<int, 8> flags{};
-  const int f = int(amips) | int(det) << 1 | int(sph) << 2;
+// 16 warps run one CTA per SM, 8 warps two; nullptr for any other nw or a combination that is not instantiated
+EnergyKernel energy_kernel(int nw, bool global, bool amips, bool det, bool sph, bool hvp = false) {
+  constexpr std::make_integer_sequence<int, 16> flags{};
+  const int f = int(amips) | int(det) << 1 | int(sph) << 2 | int(hvp) << 3;
   if (nw == 16) return (global ? flag_table<16, 1, true>(flags) : flag_table<16, 1, false>(flags))[f];
   if (nw == 8) return (global ? flag_table<8, 2, true>(flags) : flag_table<8, 2, false>(flags))[f];
   return nullptr;
@@ -930,11 +1007,13 @@ cudaError_t energy_occupancy(int nw, int smem_bytes, bool global, bool amips, bo
   if (e != cudaSuccess) return e;
   *ctas_per_sm = 0;
   if (smem_bytes > optin) return cudaSuccess;   // does not fit
-  // every instantiation the handle may launch: AMIPS ones when amips, DET ones when det, with and without SPH
+  // every instantiation the handle may launch: AMIPS ones when amips, DET ones when det, with and without SPH, and the
+  // HVP ones (tsb_hvp)
   int ctas = 1 << 30;
-  for (int f = 0; f < 8; ++f) {
+  for (int f = 0; f < 16; ++f) {
     if (((f & 1) && !amips) || ((f & 2) && !det)) continue;
-    const EnergyKernel k = energy_kernel(nw, global, f & 1, f & 2, f & 4);
+    const EnergyKernel k = energy_kernel(nw, global, f & 1, f & 2, f & 4, f & 8);
+    if (!k) continue;   // HVP with AMIPS or SPH
     if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, optin) != cudaSuccess) {
       cudaGetLastError();
       return cudaSuccess;   // does not fit
@@ -949,10 +1028,11 @@ cudaError_t energy_occupancy(int nw, int smem_bytes, bool global, bool amips, bo
 }
 
 cudaError_t launch_energy_grad(const KParams &p, const LaunchConfig &lc, cudaStream_t stream) {
-  const EnergyKernel k = energy_kernel(lc.nw, lc.global, lc.amips, lc.det, lc.sph);
+  const EnergyKernel k = energy_kernel(lc.nw, lc.global, lc.amips, lc.det, lc.sph, lc.hvp);
   if (!k) return cudaErrorInvalidValue;
   if (lc.global) {
-    prestage_kernel<<<grid_for(p.n, 256), 256, 0, stream>>>(p.x, p.X4, p.u4g, p.x4g, p.n);
+    if (lc.hvp) prestage_hvp_kernel<<<grid_for(p.n, 256), 256, 0, stream>>>(p.x, p.v, p.X4, p.u4g, p.x4g, p.n);
+    else prestage_kernel<<<grid_for(p.n, 256), 256, 0, stream>>>(p.x, p.X4, p.u4g, p.x4g, p.n);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
   }

@@ -59,6 +59,9 @@ struct KParams {
   unsigned int *det_flag;       // [n_components] nonzero: a tet of the component contributed (the gather clears it)
   // per-sphere statistics only (the SPH instantiation, tsb_energy_grad_spheres): one record per (segment, warp)
   SphRec *sph_rec;              // [n_segments * nw], rewritten by every SPH launch, read by sphere_fold_kernel
+  // Hessian-vector product only (the HVP instantiation, tsb_hvp): grad receives gradH H(x) v, energy_out (may be
+  // nullptr) v^T H v as (c1 vMv + c2 vHbv, vMv, vHbv)
+  const float *v;               // [3n] direction
 #ifdef TSB_TRACE
   unsigned long long *trace;    // profiling build only: [grid][kTraceSlots] phase stamps
 #endif
@@ -73,6 +76,7 @@ struct LaunchConfig {
   int amips;       // launch the AMIPS-capable instantiation
   int det;         // launch the deterministic instantiation (tets store their corners instead of adding them)
   int sph;         // launch the SPH instantiation (it also writes the per-(segment, warp) sphere records)
+  int hvp;         // launch the HVP instantiation (Hessian-vector product; never with amips or sph)
 };
 
 // sphere_fold_kernel's inputs (HostPlan::comp_*, uploaded, and the records of the SPH launch before it).
@@ -102,8 +106,8 @@ int energy_ring_bytes(int ring_slots, int cells_per_chunk, bool global);
 int energy_smem_bytes(int nw, int ring_slots, int cells_per_chunk, int area_verts, bool global);
 constexpr unsigned long long kEnergySentinel = 0x7FF8F00DBAADC0DEull;   // initial value of cta_energy
 // Max co-resident CTAs per SM for a configuration (0 if it does not fit): the minimum over every instantiation a handle
-// may launch (AMIPS ones when amips, deterministic ones when det, each with and without the sphere records); also opts
-// them in to the smem size.
+// may launch (AMIPS ones when amips, deterministic ones when det, each with and without the sphere records, and the
+// Hessian-vector product ones); also opts them in to the smem size.
 cudaError_t energy_occupancy(int nw, int smem_bytes, bool global, bool amips, bool det, int *ctas_per_sm);
 cudaError_t launch_energy_grad(const KParams &p, const LaunchConfig &lc, cudaStream_t stream);
 // grad[v] += the active corner vectors of v's list, in list order, for every flagged component (after a DET launch).

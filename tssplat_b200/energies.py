@@ -12,10 +12,12 @@ from types import SimpleNamespace
 
 import numpy as np
 import torch
+from torch.autograd.function import once_differentiable
 
 from tet_spheres import tet_spheres_ext
+from . import _capi
 
-__all__ = ["SmoothnessBarrierFunc", "SmoothnessBarrierEnergy"]
+__all__ = ["SmoothnessBarrierFunc", "SmoothnessBarrierFunc2", "SmoothnessBarrierEnergy"]
 
 
 #: route SmoothnessBarrierEnergy through the C++ autograd bridge when it has been built (same launches, same
@@ -44,12 +46,68 @@ class SmoothnessBarrierFunc(torch.autograd.Function):
         return grad, None, None, None, None
 
 
+class _EnergyGrad(torch.autograd.Function):
+    """``s * grad`` for the gradient ``grad`` = dE/dx at ``x`` that a forward launch produced, differentiable once more:
+    given an upstream ``w`` its backward returns ``s * H(x) w`` for ``x`` (one ``tsb_hvp`` launch, gradH = s) and
+    ``sum(grad * w)`` for ``s``.  A third derivative raises (``once_differentiable``)."""
+
+    @staticmethod
+    def forward(ctx, x, s, grad, tet_sp, c1, c2, order):
+        ctx.save_for_backward(x, s, grad)
+        ctx.constants = (tet_sp, c1, c2, order)
+        out = torch.empty_like(grad)
+        gh_val, gh_ptr, keep = tet_sp._gradH_arg(s)
+        rc = _capi.lib.tsb_scale(grad.data_ptr(), grad.numel(), gh_val, gh_ptr, out.data_ptr(),
+                                 tet_spheres_ext._stream_ptr(grad.device))
+        _capi.check(rc, None, "SmoothnessBarrierFunc2.backward")
+        del keep
+        return out.reshape(x.shape)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, w):
+        x, s, grad = ctx.saved_tensors
+        tet_sp, c1, c2, order = ctx.constants
+        gx = gs = None
+        if ctx.needs_input_grad[0]:
+            gx, _ = tet_sp.hvp(x, w, c1, c2, order, gradH=s)
+            gx = gx.reshape(x.shape)
+        if ctx.needs_input_grad[1]:
+            gs = (grad.reshape(-1) * w.reshape(-1)).sum().to(s.dtype).reshape(s.shape)
+        return gx, gs, None, None, None, None, None
+
+
+class SmoothnessBarrierFunc2(torch.autograd.Function):
+    """``SmoothnessBarrierFunc`` made twice differentiable (``FLAGS.twice_differentiable``): its backward returns
+    ``_EnergyGrad(x, grad_output)``, so ``torch.autograd.grad(E, x, create_graph=True)`` yields a gradient whose own
+    backward is a Hessian-vector product of ``c1 * smooth + c2 * barrier``.  One fused launch in forward, as the
+    default route; it does not use the fused-gradient cache."""
+
+    @staticmethod
+    def forward(ctx, x_cur, tet_sp, c1, c2, order):
+        energy, grad = tet_sp.energy_grad(x_cur, c1, c2, order, 1.0, want_grad=bool(ctx.needs_input_grad[0]))
+        ctx.save_for_backward(x_cur, grad)
+        ctx.constants = (tet_sp, c1, c2, order)
+        return energy[0]
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        if grad_output is None:
+            return (None,) * 5
+        x_cur, grad = ctx.saved_tensors
+        tet_sp, c1, c2, order = ctx.constants
+        return _EnergyGrad.apply(x_cur, grad_output, grad, tet_sp, c1, c2, int(order)), None, None, None, None
+
+
 class SmoothnessBarrierEnergy(torch.nn.Module):
     """``SmoothnessBarrierEnergy(tet_v, tet_f, FLAGS)`` (``energies/smooth_barrier.py:34-67``).
 
     ``tet_v``: numpy [n,3] REST positions; ``tet_f``: numpy [nele,4]; ``FLAGS``: mapping or object
     with ``smooth_eng_coeff``, ``barrier_coeff``, ``increase_order_iter`` (``config/gso.yaml:9-11``), and optionally
-    ``deterministic`` (default False): a bitwise repeatable gradient (``TetSpheres(..., deterministic=True)``).
+    ``deterministic`` (default False): a bitwise repeatable gradient (``TetSpheres(..., deterministic=True)``), and
+    ``twice_differentiable`` (default False): ``forward`` goes through ``SmoothnessBarrierFunc2``, whose gradient can be
+    differentiated once more (Hessian-vector products through autograd: ``create_graph=True``,
+    ``torch.autograd.functional.vhp``).  The AMIPS term is not part of either.
     """
 
     def __init__(self, tet_v, tet_f, FLAGS) -> None:
@@ -79,8 +137,17 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         _, _, stats = self.tet_sp.energy_grad_spheres(x.detach(), c1, c2, self.order_at(it), want_grad=False)
         return stats
 
+    def hvp(self, x, v, it):
+        """``H(x) v`` of ``c1 * smooth + c2 * barrier`` with the scheduler's coefficients and the barrier order at ``it``
+        (``tsb_hvp``), outside autograd, in ``x``'s shape."""
+        c1, c2 = self.coeff_scheduler(it)
+        hv, _ = self.tet_sp.hvp(x.detach(), v.detach(), c1, c2, self.order_at(it))
+        return hv.reshape(x.shape)
+
     def forward(self, x, it, c1, c2):
         order = self.order_at(it)
+        if getattr(self.FLAGS, "twice_differentiable", False):
+            return SmoothnessBarrierFunc2.apply(x, self.tet_sp, c1, c2, order)
         if (use_native_autograd and self.smooth_eng_func is SmoothnessBarrierFunc and tet_spheres_ext.fuse_backward_into_forward
                 and not tet_spheres_ext.return_cpu_scalar):
             ns = self.tet_sp.native_state()        # C++ torch::autograd::Function over the same C ABI (csrc/torch_binding.cpp)

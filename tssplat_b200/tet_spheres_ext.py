@@ -32,7 +32,7 @@ import torch
 from . import _capi
 from .mesh import load_veg
 
-__all__ = ["TetSpheres", "SphereStats", "forward", "backward", "random_x", "grad_limit", "energy_grad_host"]
+__all__ = ["TetSpheres", "SphereStats", "forward", "backward", "hvp", "random_x", "grad_limit", "energy_grad_host"]
 
 return_cpu_scalar = False
 _limit_work = {}       # (device, stream) -> float32[4] scratch of grad_limit (caller-owned in the C ABI)
@@ -223,6 +223,24 @@ class TetSpheres:
         stats = SphereStats(f64[:, 0], f64[:, 1], f64[:, 2], f32[:, 0], i32[:, 0], i32[:, 1], i32[:, 2])
         return energy, grad, stats
 
+    def hvp(self, x: torch.Tensor, v: torch.Tensor, c1: float, c2: float, order: int, gradH=1.0,
+            want_curv: bool = False):
+        """Hessian-vector product of ``c1 * smooth + c2 * barrier`` at ``x`` along ``v`` (``tsb_hvp``; the AMIPS term is
+        not part of it).  Returns (``gradH * H(x) v`` as [n,3], curvature or None), both on the device, no host sync.
+        The curvature is ``v^T H v`` as [3] = (c1 vMv + c2 vHbv, vMv, vHbv), not scaled by ``gradH``.  ``gradH`` may be
+        a CUDA tensor (read on the device, like ``energy_grad``)."""
+        xc = self._check_x(x)
+        vc = self._check_x(v)
+        hv = torch.empty((self.n, 3), dtype=torch.float32, device=self.device)
+        curv = torch.empty(3, dtype=torch.float32, device=self.device) if want_curv else None
+        gh_val, gh_ptr, keep = self._gradH_arg(gradH)
+        rc = _capi.lib.tsb_hvp(self._h, xc.data_ptr(), vc.data_ptr(), float(c1), float(c2), int(order), gh_val, gh_ptr,
+                               hv.data_ptr(), curv.data_ptr() if want_curv else None, _stream_ptr(self.device))
+        if rc:
+            _capi.check(rc, self._h, "tet_spheres_ext.hvp")
+        del keep
+        return hv, curv
+
 
 def energy_grad_host(tet_sp: TetSpheres, x_host: torch.Tensor, c1: float, c2: float, order: int, gradH: float,
                      energy_host: torch.Tensor, grad_host: Optional[torch.Tensor]) -> None:
@@ -295,6 +313,13 @@ def backward(gradH, vertexPositions: torch.Tensor, tet_sp: TetSpheres, c1: float
     else:
         _, out = tet_sp.energy_grad(vertexPositions, c1, c2, order, gradH, want_grad=True)
     return out.reshape(shape)
+
+
+def hvp(v: torch.Tensor, vertexPositions: torch.Tensor, tet_sp: TetSpheres, c1: float, c2: float, order: int) -> torch.Tensor:
+    """``H(x) v`` of ``c1 * smooth + c2 * barrier`` as a fresh tensor of ``x``'s shape (argument order of ``backward``,
+    with the direction in place of ``gradH``)."""
+    hv, _ = tet_sp.hvp(vertexPositions, v, c1, c2, order)
+    return hv.reshape(vertexPositions.shape)
 
 
 def random_x(tet_sp: TetSpheres) -> torch.Tensor:
