@@ -20,7 +20,7 @@
 extern "C" {
 #endif
 
-#define TSB_VERSION 3
+#define TSB_VERSION 4
 
 enum {
   TSB_OK = 0,
@@ -162,15 +162,30 @@ int tsb_energy_grad_spheres(tsb_handle_t h, const float *x_dev, const tsb_terms_
  * Hessian of max(-J_t, 0)^order, nonzero only for tets whose fp32 J (the value tsb_energy_grad tests) is negative.
  * vMv = v^T M v and vHbv = sum_t v^T H_t v.  H_t is the exact, indefinite tet Hessian (no SPD projection).
  * The AMIPS term is NOT part of the product: tsb_hvp differentiates c1*smooth + c2*barrier only, also on handles
- * created with enable_amips.  x_dev, v_dev: device float32 [3n], contiguous; order 2 or 4; vertices no tet references
- * get zero rows.  The launch streams the same plan as tsb_energy_grad (one kernel, plus the gather on deterministic
- * handles) and works on every handle: it leaves the handle's scratch as the next tsb_energy_grad expects, so the
- * two may be chained on one stream.  Rows no inverted tet touches are bitwise repeatable on every handle (and equal
- * across default and deterministic handles of the same options); inverted tets add their H_t v with
- * red.global.add.f32 on a default handle, and through the deterministic gather on a deterministic handle, where hv
- * and curv are then bitwise identical across launches, streams and CUDA-graph replays.  DESIGN.md section 5. */
+ * created with enable_amips (tsb_hvp_ex below adds it).  x_dev, v_dev: device float32 [3n], contiguous; order 2 or 4;
+ * vertices no tet references get zero rows.  The launch streams the same plan as tsb_energy_grad (one kernel, plus the
+ * gather on deterministic handles) and works on every handle: it leaves the handle's scratch as the next
+ * tsb_energy_grad expects, so the two may be chained on one stream.  Rows no inverted tet touches are bitwise
+ * repeatable on every handle (and equal across default and deterministic handles of the same options); inverted tets
+ * add their H_t v with red.global.add.f32 on a default handle, and through the deterministic gather on a deterministic
+ * handle, where hv and curv are then bitwise identical across launches, streams and CUDA-graph replays.  DESIGN.md
+ * section 5. */
 int tsb_hvp(tsb_handle_t h, const float *x_dev, const float *v_dev, float c1, float c2, int32_t order,
             float gradH, const float *gradH_dev, float *hv_out_dev, float *curv_out_dev, void *stream);
+
+/* tsb_hvp plus the AMIPS term: the Hessian-vector product of what tsb_energy_grad_ex differentiates.
+ *   hv_out   = gradH * (*gradH_dev) * (c1 M + c2 sum_t H_t + c3 sum_t H_a,t) v      ([n,3] fp32, required)
+ *   curv_out = { c1*vMv + c2*vHbv + c3*vHav, vMv, vHbv, vHav }   (optional device float[4]; NOT scaled by gradH)
+ * with c1, c2, c3, order from *terms (required), and H_a,t the exact (indefinite) Hessian of the tet's AMIPS term
+ * psi = tr(F^T F) / (3 J^(2/3)) - 1, nonzero only for tets whose fp32 J is positive (the tets whose AMIPS gradient
+ * tsb_energy_grad_ex adds); vHav = sum_t v^T H_a,t v.  terms->c3 != 0 needs a handle created with enable_amips = 1
+ * (TSB_E_INVALID otherwise, as tsb_energy_grad_ex).  With terms->c3 == 0 the launch is the very kernel tsb_hvp runs:
+ * hv and curv[0..2] are bitwise tsb_hvp's, and curv[3] = 0.  With c3 != 0 every tet with J > 0 adds its H_a v with
+ * red.global.add.f32 on a default handle (order-dependent rounding) and through the deterministic gather on a
+ * deterministic handle, where hv and curv are bitwise identical across launches, streams and CUDA-graph replays.  Like
+ * tsb_hvp it leaves the handle's scratch re-armed, so it chains with tsb_energy_grad(_ex) on one stream. */
+int tsb_hvp_ex(tsb_handle_t h, const float *x_dev, const float *v_dev, const tsb_terms_t *terms, float gradH,
+               const float *gradH_dev, float *hv_out_dev, float *curv_out_dev, void *stream);
 
 /* Same computation for callers whose vertex positions live in HOST memory (e.g. a CPU-side
  * optimiser): copies x_host -> device, runs the fused launch, copies energy[3] and grad back,

@@ -2,8 +2,12 @@
 SAME handle, timed in one process with CUDA events, alternating.  Each timed unit is a CUDA graph of `--launches`
 launches (replayed `--rounds` times per kind); the median over rounds is reported in us per launch.
 
+The AMIPS rows do the same with the AMIPS term on (c3 != 0, a handle created with enable_amips): tsb_energy_grad_ex
+with the gradient against tsb_hvp_ex, on default and deterministic handles.
+
 Usage: python tools/time_hvp.py [--rounds 30] [--launches 50] [--out DIR]"""
 import argparse
+import ctypes as C
 import json
 import os
 import subprocess
@@ -21,12 +25,42 @@ from tssplat_b200.mesh import make_pack, perturb  # noqa: E402
 TETS = 4096
 # (name, spheres, sigma relative to the edge length h)
 CASES = [("64x4096 benign (0.02 h)", 64, 0.02), ("64x4096 inverted (0.35 h)", 64, 0.35), ("1024x4096 benign (0.02 h)", 1024, 0.02)]
+# AMIPS rows: (name, spheres, sigma, deterministic handle)
+AMIPS_CASES = [("64x4096 AMIPS default", 64, 0.02, False), ("64x4096 AMIPS det", 64, 0.02, True),
+               ("1024x4096 AMIPS default", 1024, 0.02, False), ("1024x4096 AMIPS det", 1024, 0.02, True)]
+C3 = 1e-4
 
 
 def card():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                        capture_output=True, text=True)
     return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
+
+
+def time_kinds(fns, s, rounds, launches):
+    """{kind: [us per launch of each round]}: one CUDA graph of `launches` calls per kind, replayed alternately."""
+    graphs = {}
+    for k, fn in fns.items():
+        with torch.cuda.stream(s):
+            for _ in range(3):                        # warm-up outside the capture
+                assert fn() == 0
+        torch.cuda.synchronize()
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, stream=s):
+            for _ in range(launches):
+                assert fn() == 0
+        graphs[k] = g
+    times = {k: [] for k in graphs}
+    for _ in range(rounds):
+        for k, g in graphs.items():                   # alternating
+            t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            t0.record()
+            g.replay()
+            t1.record()
+            t1.synchronize()
+            times[k].append(t0.elapsed_time(t1) * 1e3 / launches)
+    del graphs
+    return times
 
 
 def main():
@@ -38,49 +72,43 @@ def main():
     dev = card()
     print(f"device: {dev}", flush=True)
     results = []
-    for name, S, sig in CASES:
+    runs = [(name, S, sig, None) for name, S, sig in CASES] + list(AMIPS_CASES)
+    for name, S, sig, det in runs:
+        amips = det is not None
         pack = make_pack(S, TETS, seed=0, unique=8)
-        sp = ext.TetSpheres(pack.verts.reshape(-1), pack.tets.reshape(-1))
+        sp = ext.TetSpheres(pack.verts.reshape(-1), pack.tets.reshape(-1), enable_amips=amips, deterministic=bool(det))
         x = torch.from_numpy(perturb(pack, sigma_rel=sig, seed=0)).cuda()
         v = torch.randn(x.shape, generator=torch.Generator().manual_seed(1)).cuda()
         c1, c2 = 2e-4 / S, 2e-4
+        terms = _capi.tsb_terms_t(c1=c1, c2=c2, order=2, c3=C3)
         energy = torch.empty(4, device="cuda")
         grad = torch.empty_like(x)
         hv = torch.empty_like(x)
-        curv = torch.empty(3, device="cuda")
+        curv = torch.empty(4, device="cuda")
         s = torch.cuda.Stream()
 
-        def gradient():
-            return _capi.lib.tsb_energy_grad(sp._h, x.data_ptr(), c1, c2, 2, 1.0, None, energy.data_ptr(), grad.data_ptr(),
-                                             s.cuda_stream)
+        if amips:
+            def gradient():
+                return _capi.lib.tsb_energy_grad_ex(sp._h, x.data_ptr(), C.byref(terms), 1.0, None, energy.data_ptr(),
+                                                    grad.data_ptr(), s.cuda_stream)
 
-        def hvp():
-            return _capi.lib.tsb_hvp(sp._h, x.data_ptr(), v.data_ptr(), c1, c2, 2, 1.0, None, hv.data_ptr(), curv.data_ptr(),
-                                     s.cuda_stream)
+            def hvp():
+                return _capi.lib.tsb_hvp_ex(sp._h, x.data_ptr(), v.data_ptr(), C.byref(terms), 1.0, None, hv.data_ptr(),
+                                            curv.data_ptr(), s.cuda_stream)
+        else:
+            def gradient():
+                return _capi.lib.tsb_energy_grad(sp._h, x.data_ptr(), c1, c2, 2, 1.0, None, energy.data_ptr(),
+                                                 grad.data_ptr(), s.cuda_stream)
 
-        graphs = {}
-        for k, fn in (("gradient", gradient), ("hvp", hvp)):
-            with torch.cuda.stream(s):
-                for _ in range(3):                        # warm-up outside the capture
-                    assert fn() == 0
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, stream=s):
-                for _ in range(args.launches):
-                    assert fn() == 0
-            graphs[k] = g
-        times = {k: [] for k in graphs}
-        for _ in range(args.rounds):
-            for k, g in graphs.items():                   # alternating
-                t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                t0.record()
-                g.replay()
-                t1.record()
-                t1.synchronize()
-                times[k].append(t0.elapsed_time(t1) * 1e3 / args.launches)
+            def hvp():
+                return _capi.lib.tsb_hvp(sp._h, x.data_ptr(), v.data_ptr(), c1, c2, 2, 1.0, None, hv.data_ptr(),
+                                         curv.data_ptr(), s.cuda_stream)
+
+        times = time_kinds({"gradient": gradient, "hvp": hvp}, s, args.rounds, args.launches)
         _, _, st = sp.energy_grad_spheres(x, c1, c2, 2, want_grad=False)
         n_inv = int(st.n_inverted.sum())
         r = {"case": name, "spheres": S, "tets": S * TETS, "sigma_rel": sig, "grid": sp.info["grid"],
+             "amips_c3": C3 if amips else 0.0, "deterministic": bool(det),
              "inverted_tets": n_inv, "us_per_launch": {k: float(np.median(t)) for k, t in times.items()},
              "us_per_launch_p10_p90": {k: [float(np.percentile(t, 10)), float(np.percentile(t, 90))] for k, t in times.items()},
              "device": dev}
@@ -88,7 +116,7 @@ def main():
         print(f"{name:28s} gradient {us['gradient']:8.2f} us  hvp {us['hvp']:8.2f} us "
               f"({us['hvp'] / us['gradient'] - 1:+.1%})  inverted tets {n_inv}", flush=True)
         results.append(r)
-        del graphs, sp
+        del sp
         torch.cuda.empty_cache()
     if args.out:
         os.makedirs(args.out, exist_ok=True)

@@ -314,18 +314,19 @@ int tsb_energy_grad_spheres(tsb_handle_t h, const float *x_dev, const tsb_terms_
                           spheres_out_dev, stream);
 }
 
-int tsb_hvp(tsb_handle_t h, const float *x_dev, const float *v_dev, float c1, float c2, int32_t order, float gradH,
-            const float *gradH_dev, float *hv_out_dev, float *curv_out_dev, void *stream) {
+static int hvp_impl(tsb_handle_t h, const float *x_dev, const float *v_dev, float c1, float c2, float c3, int32_t order,
+                    float gradH, const float *gradH_dev, float *hv_out_dev, float *curv_out_dev, int curv4, void *stream) {
   if (!h) return TSB_E_INVALID;
   if (!x_dev || !v_dev || !hv_out_dev) return fail(h, TSB_E_INVALID, "x_dev, v_dev and hv_out_dev must be non-null");
   if (order != 2 && order != 4) return fail(h, TSB_E_INVALID, "order must be 2 or 4");
+  if (c3 != 0.f && !h->amips) return fail(h, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
   DeviceGuard guard(h->device);
   if (!guard.ok) return fail(h, TSB_E_CUDA, "cannot select the handle's CUDA device");
   tsb::KParams kp = h->kp;
   kp.x = x_dev; kp.v = v_dev; kp.grad = hv_out_dev; kp.energy_out = curv_out_dev; kp.gradH_dev = gradH_dev;
-  kp.c1 = c1; kp.c2 = c2; kp.c3 = 0.f; kp.gradH = gradH; kp.order = order; kp.energy4 = 0;
+  kp.c1 = c1; kp.c2 = c2; kp.c3 = c3; kp.gradH = gradH; kp.order = order; kp.energy4 = curv4;
   tsb::LaunchConfig lc = h->lc;
-  lc.amips = 0;
+  lc.amips = c3 != 0.f ? 1 : 0;          // c3 == 0: the very instantiation tsb_hvp runs
   lc.det = h->det ? 1 : 0;
   lc.sph = 0;
   lc.hvp = 1;
@@ -336,6 +337,19 @@ int tsb_hvp(tsb_handle_t h, const float *x_dev, const float *v_dev, float c1, fl
     if (e != cudaSuccess) return fail(h, TSB_E_CUDA, std::string("deterministic gather launch: ") + cudaGetErrorString(e));
   }
   return TSB_OK;
+}
+
+int tsb_hvp(tsb_handle_t h, const float *x_dev, const float *v_dev, float c1, float c2, int32_t order, float gradH,
+            const float *gradH_dev, float *hv_out_dev, float *curv_out_dev, void *stream) {
+  return hvp_impl(h, x_dev, v_dev, c1, c2, 0.f, order, gradH, gradH_dev, hv_out_dev, curv_out_dev, 0, stream);
+}
+
+int tsb_hvp_ex(tsb_handle_t h, const float *x_dev, const float *v_dev, const tsb_terms_t *terms, float gradH,
+               const float *gradH_dev, float *hv_out_dev, float *curv_out_dev, void *stream) {
+  if (!h) return TSB_E_INVALID;
+  if (!terms) return fail(h, TSB_E_INVALID, "terms is null");
+  return hvp_impl(h, x_dev, v_dev, terms->c1, terms->c2, terms->c3, terms->order, gradH, gradH_dev, hv_out_dev, curv_out_dev,
+                  1, stream);
 }
 
 int tsb_energy_grad_host(tsb_handle_t h, const float *x_host, float c1, float c2, int32_t order, float gradH,

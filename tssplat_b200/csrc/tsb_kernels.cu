@@ -166,9 +166,10 @@ struct WarpStream {
 // SPH (tsb_energy_grad_spheres): at the end of every segment each warp reduces its lanes' energy partials, inverted-tet
 // count and smallest J, and lane 0 stores them as the (segment, warp) record; the running totals move to the warp's
 // red[] slot, so the CTA fold below is unchanged.  sphere_fold_kernel turns the records into per-component statistics.
-// HVP (tsb_hvp; never with AMIPS or SPH): the u slots hold v - v_ref instead of x - X, so the row pass yields M v, an
+// HVP (tsb_hvp, tsb_hvp_ex; never with SPH): the u slots hold v - v_ref instead of x - X, so the row pass yields M v, an
 // inverted tet adds its H_t v instead of its gradient (through the same scratch or atomics), and the energy partials
-// carry v^T M v and v^T H_t v (DESIGN.md section 5).  x stays in the x slots: the active set is the gradient's.
+// carry v^T M v and v^T H_t v (DESIGN.md section 5).  x stays in the x slots: the active set is the gradient's.  With
+// AMIPS (and c3 != 0) a tet with J > 0 adds its H_a v the same way, and the AMIPS partial carries v^T H_a v.
 template <int NW, int MINB, bool GLOBAL, bool AMIPS, bool DET = false, bool SPH = false, bool HVP = false>
 __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParams p) {
   using F = Fmt<GLOBAL>;
@@ -505,14 +506,21 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
         tj[F::TPL - 1][0] = a.z & 0xFFFFu; tj[F::TPL - 1][1] = a.z >> 16; tj[F::TPL - 1][2] = a.w & 0xFFFFu; tj[F::TPL - 1][3] = a.w >> 16;
         tdet[0] = d.x; tdet[F::TPL - 1] = d.y;
       }
+      // HVP with AMIPS: a lane's later tets gather their corners when they are reached, so that those registers are
+      // free for the AMIPS product (the staging area and x4g stay valid for the whole segment)
+      constexpr bool kLateX = HVP && AMIPS;
       float4 xv[F::TPL][4];
 #pragma unroll
       for (int t = 0; t < int(F::TPL); ++t)
 #pragma unroll
-        for (int k = 0; k < 4; ++k) xv[t][k] = gatherX(tj[t][k]);
+        for (int k = 0; k < 4; ++k)
+          if (!kLateX || t == 0) xv[t][k] = gatherX(tj[t][k]);
       ws.advance(1);
 #pragma unroll
       for (int t = 0; t < int(F::TPL); ++t) {
+        if (kLateX && t > 0)
+#pragma unroll
+          for (int k = 0; k < 4; ++k) xv[t][k] = gatherX(tj[t][k]);
         const float4 x0 = xv[t][0], x1 = xv[t][1], x2 = xv[t][2], x3 = xv[t][3];
         const float idet = tdet[t];
         const float e1x = x1.x - x0.x, e1y = x1.y - x0.y, e1z = x1.z - x0.z;
@@ -589,7 +597,90 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
             atomicAdd(grad + v2, g2x); atomicAdd(grad + v2 + 1, g2y); atomicAdd(grad + v2 + 2, g2z);
             atomicAdd(grad + v3, g3x); atomicAdd(grad + v3 + 1, g3y); atomicAdd(grad + v3 + 2, g3z);
           }
-        } else if (AMIPS && amips_on && J > 0.f) {
+        } else if (HVP && AMIPS && amips_on && J > 0.f) {
+          // H_a v of AMIPS (tsb_hvp_ex): with dF = dDs B (dDs columns f_k = v_k - v_0), a = 2 / (3 J^(2/3)),
+          // beta = tr / (3 J) and C = cof F:  dJ = C:dF,  da = -2/3 a dJ / J,  dbeta = (2 F:dF - tr dJ / J) / (3 J),
+          // dC = cof_pair(F, dF) + cof_pair(dF, F),  dP = da (F - beta C) + a (dF - dbeta C - beta dC).  Corner k + 1
+          // is dP (row k of B)^T, corner 0 minus their sum; v^T H_a v = sum_t dF:dP (DESIGN.md section 5)
+          const int slot = lane * int(F::TPL) + t;
+          const float4 *bp = p.Bt + (size_t(tcell0 + tc) * 3) * (32 * F::TPL) + slot;
+          const float4 b0 = __ldg(bp), b1 = __ldg(bp + 32 * F::TPL), b2 = __ldg(bp + 64 * F::TPL);
+          const float4 w0 = gatherV(tj[t][0]), w1 = gatherV(tj[t][1]), w2 = gatherV(tj[t][2]), w3 = gatherV(tj[t][3]);
+          const float ex[3] = {e1x, e2x, e3x}, ey[3] = {e1y, e2y, e3y}, ez[3] = {e1z, e2z, e3z};
+          const float fx[3] = {w1.x - w0.x, w2.x - w0.x, w3.x - w0.x}, fy[3] = {w1.y - w0.y, w2.y - w0.y, w3.y - w0.y};
+          const float fz[3] = {w1.z - w0.z, w2.z - w0.z, w3.z - w0.z};
+          const float bb[3][3] = {{b0.x, b0.y, b0.z}, {b1.x, b1.y, b1.z}, {b2.x, b2.y, b2.z}};
+          float Fm[3][3], dF[3][3];
+#pragma unroll
+          for (int c = 0; c < 3; ++c) {
+            Fm[0][c] = ex[0] * bb[0][c] + ex[1] * bb[1][c] + ex[2] * bb[2][c];
+            Fm[1][c] = ey[0] * bb[0][c] + ey[1] * bb[1][c] + ey[2] * bb[2][c];
+            Fm[2][c] = ez[0] * bb[0][c] + ez[1] * bb[1][c] + ez[2] * bb[2][c];
+            dF[0][c] = fx[0] * bb[0][c] + fx[1] * bb[1][c] + fx[2] * bb[2][c];
+            dF[1][c] = fy[0] * bb[0][c] + fy[1] * bb[1][c] + fy[2] * bb[2][c];
+            dF[2][c] = fz[0] * bb[0][c] + fz[1] * bb[1][c] + fz[2] * bb[2][c];
+          }
+          // cofactor entries are recomputed where used (register budget): cof_pair(A, B)[r][c] =
+          // A[r+1][c+1] B[r+2][c+2] - A[r+1][c+2] B[r+2][c+1], indices mod 3
+          auto cofp = [](const float (&A)[3][3], const float (&Bm)[3][3], int r, int c) -> float {
+            const int r1 = (r + 1) % 3, r2 = (r + 2) % 3, c1 = (c + 1) % 3, c2 = (c + 2) % 3;
+            return A[r1][c1] * Bm[r2][c2] - A[r1][c2] * Bm[r2][c1];
+          };
+          float tr = 0.f, fdf = 0.f, dJ = 0.f;
+#pragma unroll
+          for (int r = 0; r < 3; ++r)
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+              tr = fmaf(Fm[r][c], Fm[r][c], tr);
+              fdf = fmaf(Fm[r][c], dF[r][c], fdf);
+              dJ = fmaf(cofp(Fm, Fm, r, c), dF[r][c], dJ);
+            }
+          const float cb = cbrtf(J), j23 = cb * cb, iJ = 1.f / J;
+          const float a = 2.f / (3.f * j23), bq = tr * (1.f / 3.f) * iJ;
+          const float da = -(2.f / 3.f) * a * dJ * iJ;
+          const float dbq = (2.f * fdf - tr * dJ * iJ) * (1.f / 3.f) * iJ;
+          float dP[3][3];
+          float q = 0.f;
+#pragma unroll
+          for (int r = 0; r < 3; ++r)
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+              const float C = cofp(Fm, Fm, r, c), dC = cofp(Fm, dF, r, c) + cofp(dF, Fm, r, c);
+              dP[r][c] = da * (Fm[r][c] - bq * C) + a * (dF[r][c] - dbq * C - bq * dC);
+              q = fmaf(dF[r][c], dP[r][c], q);
+            }
+          dea += double(q);   // v^T H_a v
+          // gradH c3 H_a v: DET stores the four corners as the gradient does (three 16-byte stores; every J > 0 tet
+          // contributes, so scalar stores would cost a quarter of the launch), otherwise each corner is added to hv
+          // after the component's rows as soon as it is formed
+          float g0[3] = {0.f, 0.f, 0.f};
+          if constexpr (DET) {
+            float gk[3][3];
+#pragma unroll
+            for (int k = 0; k < 3; ++k)
+#pragma unroll
+              for (int r = 0; r < 3; ++r) {
+                gk[k][r] = s3 * (dP[r][0] * bb[k][0] + dP[r][1] * bb[k][1] + dP[r][2] * bb[k][2]);
+                g0[r] -= gk[k][r];
+              }
+            det_store(tc, t, g0[0], g0[1], g0[2], gk[0][0], gk[0][1], gk[0][2], gk[1][0], gk[1][1], gk[1][2], gk[2][0], gk[2][1], gk[2][2]);
+            dmask |= 1u << t;
+          } else {
+            wait_rows();
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+              const size_t vk = 3 * gid_x(tj[t][k + 1]);
+#pragma unroll
+              for (int r = 0; r < 3; ++r) {
+                const float g = s3 * (dP[r][0] * bb[k][0] + dP[r][1] * bb[k][1] + dP[r][2] * bb[k][2]);
+                g0[r] -= g;
+                atomicAdd(grad + vk + r, g);
+              }
+            }
+            const size_t v0 = 3 * gid_x(tj[t][0]);
+            atomicAdd(grad + v0, g0[0]); atomicAdd(grad + v0 + 1, g0[1]); atomicAdd(grad + v0 + 2, g0[2]);
+          }
+        } else if (!HVP && AMIPS && amips_on && J > 0.f) {
           // AMIPS (default off; no counterpart in the reference -- SURVEY.md F1):  psi = tr(F^T F) / (3 J^(2/3)) - 1,
           // d psi / dF = 2 / (3 J^(2/3)) (F - tr / (3 J) cof F),  F = Ds B with B = Dm^-1 streamed per tet
           const int slot = lane * int(F::TPL) + t;
@@ -967,10 +1058,10 @@ inline int grid_for(int64_t count, int block) {
 // ---- the energy_grad_kernel instantiations, by flag bits f = AMIPS | DET << 1 | SPH << 2 | HVP << 3 -----------------
 using EnergyKernel = void (*)(KParams);
 
-// HVP is never combined with AMIPS or SPH: those entries are nullptr and never instantiated
+// HVP is never combined with SPH: those entries are nullptr and never instantiated
 template <int NW, int MINB, bool GLOBAL, int F>
 constexpr EnergyKernel kernel_of() {
-  if constexpr ((F & 8) && (F & 5)) return nullptr;
+  if constexpr ((F & 8) && (F & 4)) return nullptr;
   else return energy_grad_kernel<NW, MINB, GLOBAL, bool(F & 1), bool(F & 2), bool(F & 4), bool(F & 8)>;
 }
 
@@ -1008,12 +1099,12 @@ cudaError_t energy_occupancy(int nw, int smem_bytes, bool global, bool amips, bo
   *ctas_per_sm = 0;
   if (smem_bytes > optin) return cudaSuccess;   // does not fit
   // every instantiation the handle may launch: AMIPS ones when amips, DET ones when det, with and without SPH, and the
-  // HVP ones (tsb_hvp)
+  // HVP ones (tsb_hvp, and tsb_hvp_ex's AMIPS ones when amips)
   int ctas = 1 << 30;
   for (int f = 0; f < 16; ++f) {
     if (((f & 1) && !amips) || ((f & 2) && !det)) continue;
     const EnergyKernel k = energy_kernel(nw, global, f & 1, f & 2, f & 4, f & 8);
-    if (!k) continue;   // HVP with AMIPS or SPH
+    if (!k) continue;   // HVP with SPH
     if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, optin) != cudaSuccess) {
       cudaGetLastError();
       return cudaSuccess;   // does not fit

@@ -59,8 +59,8 @@ struct KParams {
   unsigned int *det_flag;       // [n_components] nonzero: a tet of the component contributed (the gather clears it)
   // per-sphere statistics only (the SPH instantiation, tsb_energy_grad_spheres): one record per (segment, warp)
   SphRec *sph_rec;              // [n_segments * nw], rewritten by every SPH launch, read by sphere_fold_kernel
-  // Hessian-vector product only (the HVP instantiation, tsb_hvp): grad receives gradH H(x) v, energy_out (may be
-  // nullptr) v^T H v as (c1 vMv + c2 vHbv, vMv, vHbv)
+  // Hessian-vector product only (the HVP instantiations, tsb_hvp / tsb_hvp_ex): grad receives gradH H(x) v, energy_out
+  // (may be nullptr) v^T H v as (c1 vMv + c2 vHbv + c3 vHav, vMv, vHbv[, vHav when energy4])
   const float *v;               // [3n] direction
 #ifdef TSB_TRACE
   unsigned long long *trace;    // profiling build only: [grid][kTraceSlots] phase stamps
@@ -76,7 +76,7 @@ struct LaunchConfig {
   int amips;       // launch the AMIPS-capable instantiation
   int det;         // launch the deterministic instantiation (tets store their corners instead of adding them)
   int sph;         // launch the SPH instantiation (it also writes the per-(segment, warp) sphere records)
-  int hvp;         // launch the HVP instantiation (Hessian-vector product; never with amips or sph)
+  int hvp;         // launch the HVP instantiation (Hessian-vector product; never with sph)
 };
 
 // sphere_fold_kernel's inputs (HostPlan::comp_*, uploaded, and the records of the SPH launch before it).

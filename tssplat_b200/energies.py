@@ -17,7 +17,7 @@ from torch.autograd.function import once_differentiable
 from tet_spheres import tet_spheres_ext
 from . import _capi
 
-__all__ = ["SmoothnessBarrierFunc", "SmoothnessBarrierFunc2", "SmoothnessBarrierEnergy"]
+__all__ = ["SmoothnessBarrierFunc", "SmoothnessBarrierFunc2", "SmoothnessBarrierAmipsFunc", "SmoothnessBarrierEnergy"]
 
 
 #: route SmoothnessBarrierEnergy through the C++ autograd bridge when it has been built (same launches, same
@@ -46,35 +46,41 @@ class SmoothnessBarrierFunc(torch.autograd.Function):
         return grad, None, None, None, None
 
 
+def _scaled_grad(tet_sp, grad, s, shape):
+    """``s * grad`` as a fresh tensor of ``shape`` (``tsb_scale``; ``s`` may be a CUDA tensor, read on the device)."""
+    out = torch.empty_like(grad)
+    gh_val, gh_ptr, keep = tet_sp._gradH_arg(s)
+    rc = _capi.lib.tsb_scale(grad.data_ptr(), grad.numel(), gh_val, gh_ptr, out.data_ptr(),
+                             tet_spheres_ext._stream_ptr(grad.device))
+    _capi.check(rc, None, "SmoothnessBarrierFunc2.backward")
+    del keep
+    return out.reshape(shape)
+
+
 class _EnergyGrad(torch.autograd.Function):
     """``s * grad`` for the gradient ``grad`` = dE/dx at ``x`` that a forward launch produced, differentiable once more:
-    given an upstream ``w`` its backward returns ``s * H(x) w`` for ``x`` (one ``tsb_hvp`` launch, gradH = s) and
-    ``sum(grad * w)`` for ``s``.  A third derivative raises (``once_differentiable``)."""
+    given an upstream ``w`` its backward returns ``s * H(x) w`` for ``x`` (one ``tsb_hvp`` launch, gradH = s, or one
+    ``tsb_hvp_ex`` with ``c3`` when the energy has the AMIPS term) and ``sum(grad * w)`` for ``s``.  A third derivative
+    raises (``once_differentiable``)."""
 
     @staticmethod
-    def forward(ctx, x, s, grad, tet_sp, c1, c2, order):
+    def forward(ctx, x, s, grad, tet_sp, c1, c2, order, c3=0.0):
         ctx.save_for_backward(x, s, grad)
-        ctx.constants = (tet_sp, c1, c2, order)
-        out = torch.empty_like(grad)
-        gh_val, gh_ptr, keep = tet_sp._gradH_arg(s)
-        rc = _capi.lib.tsb_scale(grad.data_ptr(), grad.numel(), gh_val, gh_ptr, out.data_ptr(),
-                                 tet_spheres_ext._stream_ptr(grad.device))
-        _capi.check(rc, None, "SmoothnessBarrierFunc2.backward")
-        del keep
-        return out.reshape(x.shape)
+        ctx.constants = (tet_sp, c1, c2, order, c3)
+        return _scaled_grad(tet_sp, grad, s, x.shape)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, w):
         x, s, grad = ctx.saved_tensors
-        tet_sp, c1, c2, order = ctx.constants
+        tet_sp, c1, c2, order, c3 = ctx.constants
         gx = gs = None
         if ctx.needs_input_grad[0]:
-            gx, _ = tet_sp.hvp(x, w, c1, c2, order, gradH=s)
+            gx, _ = tet_sp.hvp(x, w, c1, c2, order, gradH=s, c3=c3)
             gx = gx.reshape(x.shape)
         if ctx.needs_input_grad[1]:
             gs = (grad.reshape(-1) * w.reshape(-1)).sum().to(s.dtype).reshape(s.shape)
-        return gx, gs, None, None, None, None, None
+        return gx, gs, None, None, None, None, None, None
 
 
 class SmoothnessBarrierFunc2(torch.autograd.Function):
@@ -99,6 +105,33 @@ class SmoothnessBarrierFunc2(torch.autograd.Function):
         return _EnergyGrad.apply(x_cur, grad_output, grad, tet_sp, c1, c2, int(order)), None, None, None, None
 
 
+class SmoothnessBarrierAmipsFunc(torch.autograd.Function):
+    """``c1 * smooth + c2 * barrier + c3 * amips`` (``FLAGS.amips_coeff``; the handle must be created with
+    ``enable_amips=True``).  Forward is one fused launch (``tsb_energy_grad_ex``) that also produces the gradient;
+    backward scales it by ``grad_output`` and does not relaunch.  With ``twice`` the gradient is an ``_EnergyGrad``,
+    whose own backward is one ``tsb_hvp_ex`` with ``c3`` (all three terms); without it, as in ``SmoothnessBarrierFunc``,
+    the gradient carries no graph."""
+
+    @staticmethod
+    def forward(ctx, x_cur, tet_sp, c1, c2, order, c3, twice):
+        energy, grad = tet_sp.energy_grad(x_cur, c1, c2, order, 1.0, want_grad=bool(ctx.needs_input_grad[0]), c3=c3)
+        ctx.save_for_backward(x_cur, grad)
+        ctx.constants = (tet_sp, c1, c2, order, c3, twice)
+        return energy[0]
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        if grad_output is None:
+            return (None,) * 7
+        x_cur, grad = ctx.saved_tensors
+        tet_sp, c1, c2, order, c3, twice = ctx.constants
+        if twice:
+            gx = _EnergyGrad.apply(x_cur, grad_output, grad, tet_sp, c1, c2, int(order), float(c3))
+        else:
+            gx = _scaled_grad(tet_sp, grad, grad_output.detach(), x_cur.shape)
+        return gx, None, None, None, None, None, None
+
+
 class SmoothnessBarrierEnergy(torch.nn.Module):
     """``SmoothnessBarrierEnergy(tet_v, tet_f, FLAGS)`` (``energies/smooth_barrier.py:34-67``).
 
@@ -107,15 +140,28 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
     ``deterministic`` (default False): a bitwise repeatable gradient (``TetSpheres(..., deterministic=True)``), and
     ``twice_differentiable`` (default False): ``forward`` goes through ``SmoothnessBarrierFunc2``, whose gradient can be
     differentiated once more (Hessian-vector products through autograd: ``create_graph=True``,
-    ``torch.autograd.functional.vhp``).  The AMIPS term is not part of either.
+    ``torch.autograd.functional.vhp``), and ``amips_coeff`` (default 0): with a value > 0 the energy gains the AMIPS
+    term, ``c1 * smooth + c2 * barrier + amips_coeff * amips``.  The coefficient is a constant (the scheduler's
+    multiplier applies to the reference's two terms only); ``forward`` then goes through ``SmoothnessBarrierAmipsFunc``
+    (one fused launch, twice differentiable under ``twice_differentiable``), and ``hvp`` and ``sphere_stats`` include
+    the term.  With ``amips_coeff`` absent or 0 nothing changes.
     """
+
+    #: the AMIPS coefficient; a class default, so that a module assembled without ``__init__`` (as ``bench.py`` does)
+    #: keeps the route it had before the term existed
+    amips_coeff = 0.0
 
     def __init__(self, tet_v, tet_f, FLAGS) -> None:
         super().__init__()
         v_flat = np.asarray(tet_v).flatten().astype(np.float32)
         f_flat = np.asarray(tet_f).flatten().astype(np.int32)
         self.FLAGS = SimpleNamespace(**FLAGS) if isinstance(FLAGS, dict) else FLAGS
-        self.tet_sp = tet_spheres_ext.TetSpheres(v_flat, f_flat, deterministic=bool(getattr(self.FLAGS, "deterministic", False)))
+        self.amips_coeff = float(getattr(self.FLAGS, "amips_coeff", 0.0) or 0.0)
+        if not self.amips_coeff >= 0.0:
+            raise ValueError(f"amips_coeff must be >= 0, got {self.amips_coeff}")
+        kw = dict(enable_amips=True) if self.amips_coeff > 0 else {}
+        self.tet_sp = tet_spheres_ext.TetSpheres(v_flat, f_flat, deterministic=bool(getattr(self.FLAGS, "deterministic", False)),
+                                                 **kw)
         self.smooth_eng_func = SmoothnessBarrierFunc          # the reference instantiates it; .apply is static
 
     def coeff_scheduler(self, it):
@@ -130,22 +176,27 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
 
     def sphere_stats(self, x, it):
         """Per-sphere geometry statistics at ``x`` (``tet_spheres_ext.SphereStats`` of device tensors, no host sync):
-        each sphere's smoothness and barrier terms, inverted-tet count and smallest det F, with the barrier order
-        ``forward(x, it, ...)`` uses at ``it``.  An energy-only launch, outside autograd; it leaves the fused-gradient
-        cache alone.  Meant to be logged every N iterations next to the loss."""
+        each sphere's smoothness and barrier terms (and AMIPS term with ``amips_coeff``), inverted-tet count and
+        smallest det F, with the barrier order ``forward(x, it, ...)`` uses at ``it``.  An energy-only launch, outside
+        autograd; it leaves the fused-gradient cache alone.  Meant to be logged every N iterations next to the loss."""
         c1, c2 = self.coeff_scheduler(it)
-        _, _, stats = self.tet_sp.energy_grad_spheres(x.detach(), c1, c2, self.order_at(it), want_grad=False)
+        _, _, stats = self.tet_sp.energy_grad_spheres(x.detach(), c1, c2, self.order_at(it), want_grad=False,
+                                                      c3=self.amips_coeff)
         return stats
 
     def hvp(self, x, v, it):
-        """``H(x) v`` of ``c1 * smooth + c2 * barrier`` with the scheduler's coefficients and the barrier order at ``it``
-        (``tsb_hvp``), outside autograd, in ``x``'s shape."""
+        """``H(x) v`` of ``c1 * smooth + c2 * barrier (+ amips_coeff * amips)`` with the scheduler's coefficients and the
+        barrier order at ``it`` (``tsb_hvp``, or ``tsb_hvp_ex`` with ``amips_coeff``), outside autograd, in ``x``'s
+        shape."""
         c1, c2 = self.coeff_scheduler(it)
-        hv, _ = self.tet_sp.hvp(x.detach(), v.detach(), c1, c2, self.order_at(it))
+        hv, _ = self.tet_sp.hvp(x.detach(), v.detach(), c1, c2, self.order_at(it), c3=self.amips_coeff)
         return hv.reshape(x.shape)
 
     def forward(self, x, it, c1, c2):
         order = self.order_at(it)
+        if self.amips_coeff > 0:
+            return SmoothnessBarrierAmipsFunc.apply(x, self.tet_sp, c1, c2, order, self.amips_coeff,
+                                                    bool(getattr(self.FLAGS, "twice_differentiable", False)))
         if getattr(self.FLAGS, "twice_differentiable", False):
             return SmoothnessBarrierFunc2.apply(x, self.tet_sp, c1, c2, order)
         if (use_native_autograd and self.smooth_eng_func is SmoothnessBarrierFunc and tet_spheres_ext.fuse_backward_into_forward

@@ -224,18 +224,25 @@ class TetSpheres:
         return energy, grad, stats
 
     def hvp(self, x: torch.Tensor, v: torch.Tensor, c1: float, c2: float, order: int, gradH=1.0,
-            want_curv: bool = False):
-        """Hessian-vector product of ``c1 * smooth + c2 * barrier`` at ``x`` along ``v`` (``tsb_hvp``; the AMIPS term is
-        not part of it).  Returns (``gradH * H(x) v`` as [n,3], curvature or None), both on the device, no host sync.
-        The curvature is ``v^T H v`` as [3] = (c1 vMv + c2 vHbv, vMv, vHbv), not scaled by ``gradH``.  ``gradH`` may be
-        a CUDA tensor (read on the device, like ``energy_grad``)."""
+            want_curv: bool = False, c3: float = 0.0):
+        """Hessian-vector product of ``c1 * smooth + c2 * barrier + c3 * amips`` at ``x`` along ``v``.  Returns
+        (``gradH * H(x) v`` as [n,3], curvature or None), both on the device, no host sync.  The curvature is ``v^T H v``
+        as [3] = (c1 vMv + c2 vHbv, vMv, vHbv), not scaled by ``gradH``; with ``c3`` (AMIPS coefficient, handle created
+        with ``enable_amips=True``; ``tsb_hvp_ex``) it has a 4th entry, vHav, and its total includes ``c3 * vHav``, the
+        same 3-vs-4 convention as ``energy_grad``.  ``c3 == 0`` is ``tsb_hvp``.  ``gradH`` may be a CUDA tensor (read
+        on the device, like ``energy_grad``)."""
         xc = self._check_x(x)
         vc = self._check_x(v)
         hv = torch.empty((self.n, 3), dtype=torch.float32, device=self.device)
-        curv = torch.empty(3, dtype=torch.float32, device=self.device) if want_curv else None
+        curv = torch.empty(4 if c3 else 3, dtype=torch.float32, device=self.device) if want_curv else None
         gh_val, gh_ptr, keep = self._gradH_arg(gradH)
-        rc = _capi.lib.tsb_hvp(self._h, xc.data_ptr(), vc.data_ptr(), float(c1), float(c2), int(order), gh_val, gh_ptr,
-                               hv.data_ptr(), curv.data_ptr() if want_curv else None, _stream_ptr(self.device))
+        if c3:
+            terms = _capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
+            rc = _capi.lib.tsb_hvp_ex(self._h, xc.data_ptr(), vc.data_ptr(), C.byref(terms), gh_val, gh_ptr, hv.data_ptr(),
+                                      curv.data_ptr() if want_curv else None, _stream_ptr(self.device))
+        else:
+            rc = _capi.lib.tsb_hvp(self._h, xc.data_ptr(), vc.data_ptr(), float(c1), float(c2), int(order), gh_val,
+                                   gh_ptr, hv.data_ptr(), curv.data_ptr() if want_curv else None, _stream_ptr(self.device))
         if rc:
             _capi.check(rc, self._h, "tet_spheres_ext.hvp")
         del keep
@@ -315,10 +322,11 @@ def backward(gradH, vertexPositions: torch.Tensor, tet_sp: TetSpheres, c1: float
     return out.reshape(shape)
 
 
-def hvp(v: torch.Tensor, vertexPositions: torch.Tensor, tet_sp: TetSpheres, c1: float, c2: float, order: int) -> torch.Tensor:
-    """``H(x) v`` of ``c1 * smooth + c2 * barrier`` as a fresh tensor of ``x``'s shape (argument order of ``backward``,
-    with the direction in place of ``gradH``)."""
-    hv, _ = tet_sp.hvp(vertexPositions, v, c1, c2, order)
+def hvp(v: torch.Tensor, vertexPositions: torch.Tensor, tet_sp: TetSpheres, c1: float, c2: float, order: int,
+        c3: float = 0.0) -> torch.Tensor:
+    """``H(x) v`` of ``c1 * smooth + c2 * barrier (+ c3 * amips)`` as a fresh tensor of ``x``'s shape (argument order of
+    ``backward``, with the direction in place of ``gradH``; ``c3`` as in ``TetSpheres.hvp``)."""
+    hv, _ = tet_sp.hvp(vertexPositions, v, c1, c2, order, c3=c3)
     return hv.reshape(vertexPositions.shape)
 
 
