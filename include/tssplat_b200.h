@@ -20,7 +20,8 @@
 extern "C" {
 #endif
 
-#define TSB_VERSION 4
+#define TSB_VERSION 5
+#define TSB_LINE_MAX_ALPHA 8   /* step sizes one tsb_line_search call may evaluate */
 
 enum {
   TSB_OK = 0,
@@ -186,6 +187,34 @@ int tsb_hvp(tsb_handle_t h, const float *x_dev, const float *v_dev, float c1, fl
  * tsb_hvp it leaves the handle's scratch re-armed, so it chains with tsb_energy_grad(_ex) on one stream. */
 int tsb_hvp_ex(tsb_handle_t h, const float *x_dev, const float *v_dev, const tsb_terms_t *terms, float gradH,
                const float *gradH_dev, float *hv_out_dev, float *curv_out_dev, void *stream);
+
+/* Line search along a direction (no counterpart in the reference): the energy change at up to TSB_LINE_MAX_ALPHA step
+ * sizes and the largest step before a tet inverts, in one pass over the plan.
+ *   delta_out[k]  = { c1*ds + c2*db + c3*da, ds, db, da }      (device float [n_alpha][4], required)
+ * where ds, db, da are the changes E_t(x + alpha_k d) - E_t(x) of the unweighted smoothness, barrier and AMIPS terms of
+ * tsb_energy_grad_ex (da = 0 when terms->c3 == 0), computed as differences, never as two energies subtracted:
+ * ds = alpha u^T M d + 1/2 alpha^2 d^T M d with u = x - X, and per tet from J(alpha) = det F(x + alpha d), a cubic, and
+ * |F + alpha dF|^2, a quadratic.  A tet contributes AMIPS at alpha exactly when its fp32 J(alpha) > 0.
+ *   step_out[0]   = the smallest alpha in (0, alpha_max], alpha_max = max_k alpha_k, at which a real tet whose fp32
+ *                   J(x) > 0 reaches J = 0 (the first root of its cubic, also when the cubic comes back above 0 before
+ *                   alpha_max); +inf if there is none or alpha_max <= 0.  Inverted tets are ignored.  The kernel's own
+ *                   cubic is >= 0 at the returned value.  (optional device float [1])
+ * Per sphere (optional, device memory, component order as tsb_energy_grad_spheres): sphere_delta_out
+ * [n_components][n_alpha][4] and sphere_step_out [n_components], from fp64 per-sphere sums; delta_out is the
+ * fixed-order fp64 sum of those sums rounded once, and step_out their minimum.  Vertices no tet references belong to no
+ * sphere.  x_dev, d_dev: device float32 [3n]; alpha_dev: device float32 [n_alpha], 1 <= n_alpha <= TSB_LINE_MAX_ALPHA,
+ * read on the device (a captured CUDA graph can be replayed with new step sizes).  c1, c2, order, c3 from *terms, with
+ * tsb_energy_grad_ex's rules.  There are no atomics and no per-vertex output: every output is a pure function of (plan,
+ * x, d, alpha, terms), bitwise identical across launches, streams, CUDA-graph replays, and default and deterministic
+ * handles of the same options.  The line search uses no device memory of its own (its records reuse the per-sphere
+ * statistics' scratch) and leaves the handle's scratch as tsb_energy_grad(_ex) and tsb_hvp(_ex) expect, so it chains
+ * with them on one stream.  Three launches: the energy kernel's LINE variant and two small fold kernels.
+ * Argument errors (TSB_E_INVALID, nothing launched): n_alpha outside [1, TSB_LINE_MAX_ALPHA], a null x_dev, d_dev,
+ * alpha_dev, delta_out_dev or terms, an order other than 2 or 4, terms->c3 != 0 on a handle without enable_amips.
+ * DESIGN.md section 5, "Line search". */
+int tsb_line_search(tsb_handle_t h, const float *x_dev, const float *d_dev, const tsb_terms_t *terms,
+                    const float *alpha_dev, int32_t n_alpha, float *delta_out_dev, float *step_out_dev,
+                    float *sphere_delta_out_dev, float *sphere_step_out_dev, void *stream);
 
 /* Same computation for callers whose vertex positions live in HOST memory (e.g. a CPU-side
  * optimiser): copies x_host -> device, runs the fused launch, copies energy[3] and grad back,

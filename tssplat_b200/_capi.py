@@ -14,11 +14,12 @@ from . import build as _build
 LIB_PATH = os.environ.get("TSSPLAT_B200_LIB") or _build.LIB_PATH
 
 TSB_OK, TSB_E_INVALID, TSB_E_MESH, TSB_E_CUDA, TSB_E_NOMEM = 0, -1, -2, -3, -4
+TSB_LINE_MAX_ALPHA = 8
 
 # every symbol include/tssplat_b200.h declares (tests check the library exports each one)
 EXPORTED_SYMBOLS = (
     "tsb_create", "tsb_destroy", "tsb_last_error", "tsb_get_info", "tsb_energy_grad", "tsb_energy_grad_ex", "tsb_energy_grad_spheres", "tsb_hvp", "tsb_hvp_ex",
-    "tsb_energy_grad_host", "tsb_scale",
+    "tsb_line_search", "tsb_energy_grad_host", "tsb_scale",
     "tsb_grad_limit", "tsb_adam_uniform_step",
     "tsb_surface_create", "tsb_surface_destroy", "tsb_surface_last_error", "tsb_surface_forward", "tsb_surface_backward",
     "tsb_surface_extract", "tsb_free_host", "tsb_setup_last_error",
@@ -78,6 +79,8 @@ def _load() -> C.CDLL:
     lib.tsb_hvp.argtypes = [vp, vp, vp, f32, f32, i32, f32, vp, vp, vp, vp]
     lib.tsb_hvp_ex.restype = C.c_int
     lib.tsb_hvp_ex.argtypes = [vp, vp, vp, C.POINTER(tsb_terms_t), f32, vp, vp, vp, vp]
+    lib.tsb_line_search.restype = C.c_int
+    lib.tsb_line_search.argtypes = [vp, vp, vp, C.POINTER(tsb_terms_t), vp, i32, vp, vp, vp, vp, vp]
     lib.tsb_energy_grad_host.restype = C.c_int
     lib.tsb_energy_grad_host.argtypes = [vp, vp, f32, f32, i32, f32, vp, vp, vp]
     lib.tsb_scale.restype = C.c_int

@@ -352,6 +352,39 @@ int tsb_hvp_ex(tsb_handle_t h, const float *x_dev, const float *v_dev, const tsb
                   1, stream);
 }
 
+int tsb_line_search(tsb_handle_t h, const float *x_dev, const float *d_dev, const tsb_terms_t *terms, const float *alpha_dev,
+                    int32_t n_alpha, float *delta_out_dev, float *step_out_dev, float *sphere_delta_out_dev,
+                    float *sphere_step_out_dev, void *stream) {
+  if (!h) return TSB_E_INVALID;
+  if (n_alpha < 1 || n_alpha > TSB_LINE_MAX_ALPHA)
+    return fail(h, TSB_E_INVALID, "n_alpha must be in [1, " + std::to_string(TSB_LINE_MAX_ALPHA) + "]");
+  if (!terms) return fail(h, TSB_E_INVALID, "terms is null");
+  if (!x_dev || !d_dev || !alpha_dev || !delta_out_dev)
+    return fail(h, TSB_E_INVALID, "x_dev, d_dev, alpha_dev and delta_out_dev must be non-null");
+  if (terms->order != 2 && terms->order != 4) return fail(h, TSB_E_INVALID, "order must be 2 or 4");
+  if (terms->c3 != 0.f && !h->amips)
+    return fail(h, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return fail(h, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  tsb::KParams kp = h->kp;
+  kp.x = x_dev; kp.v = d_dev; kp.grad = nullptr; kp.energy_out = nullptr; kp.gradH_dev = nullptr;
+  kp.c1 = terms->c1; kp.c2 = terms->c2; kp.c3 = terms->c3; kp.gradH = 1.f; kp.order = terms->order; kp.energy4 = 0;
+  kp.alpha = alpha_dev; kp.n_alpha = n_alpha;
+  tsb::LaunchConfig lc = h->lc;
+  lc.amips = terms->c3 != 0.f ? 1 : 0;
+  lc.det = 0;              // no per-vertex output: the same launch on default and deterministic handles
+  lc.sph = 0;
+  lc.hvp = 0;
+  lc.line = 1;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaError_t e = tsb::launch_energy_grad(kp, lc, st);
+  if (e != cudaSuccess) return fail(h, TSB_E_CUDA, std::string("line search launch: ") + cudaGetErrorString(e));
+  e = tsb::launch_line_fold(h->sp, alpha_dev, n_alpha, terms->c1, terms->c2, terms->c3, delta_out_dev, step_out_dev,
+                            sphere_delta_out_dev, sphere_step_out_dev, st);
+  if (e != cudaSuccess) return fail(h, TSB_E_CUDA, std::string("line search fold launch: ") + cudaGetErrorString(e));
+  return TSB_OK;
+}
+
 int tsb_energy_grad_host(tsb_handle_t h, const float *x_host, float c1, float c2, int32_t order, float gradH,
                          float *energy_out_host, float *grad_out_host, void *stream) {
   if (!h) return TSB_E_INVALID;

@@ -44,6 +44,16 @@ __device__ __forceinline__ double warp_sum(double v) {
   return v;
 }
 
+// LINE's reduce-scatter of N (8 or 16) per-lane values: the halving with xor offset o = 16, 8, ... leaves the lanes with
+// bit o set the upper half (h = N/2, N/4, ...), so value j ends in the lanes whose bits o are the bits h of j
+template <int N>
+__device__ __forceinline__ int line_lane(int j) {
+  int l = 0;
+#pragma unroll
+  for (int h = N / 2, o = 16; h >= 1; h >>= 1, o >>= 1) l |= (j & h) ? o : 0;
+  return l;
+}
+
 // ---- mbarrier + TMA bulk copy (1-D) ------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return uint32_t(__cvta_generic_to_shared(p)); }
 __device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
@@ -170,9 +180,13 @@ struct WarpStream {
 // inverted tet adds its H_t v instead of its gradient (through the same scratch or atomics), and the energy partials
 // carry v^T M v and v^T H_t v (DESIGN.md section 5).  x stays in the x slots: the active set is the gradient's.  With
 // AMIPS (and c3 != 0) a tet with J > 0 adds its H_a v the same way, and the AMIPS partial carries v^T H_a v.
-template <int NW, int MINB, bool GLOBAL, bool AMIPS, bool DET = false, bool SPH = false, bool HVP = false>
+// LINE (tsb_line_search; with AMIPS only): staged as HVP with v = d, so the row pass yields M d; a row adds d^T M d and
+// u^T M d, every real tet its barrier (and AMIPS) change at each alpha_k and the first root of its det F along d.  No
+// gradient, no energy fold: the CTA's warps combine their sums per segment into one LineRec (DESIGN.md section 5).
+template <int NW, int MINB, bool GLOBAL, bool AMIPS, bool DET = false, bool SPH = false, bool HVP = false, bool LINE = false>
 __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParams p) {
   using F = Fmt<GLOBAL>;
+  constexpr bool VS = HVP || LINE;   // the u slots hold a direction (v, or d) instead of x - X
   constexpr int NT = NW * 32;
   constexpr uint32_t CELL = F::CELL, WOFF = 128 * F::IB;
   constexpr int SV = GLOBAL ? 1 : (1024 + NT - 1) / NT;   // register-prefetch slots per thread (vh <= 1023)
@@ -220,7 +234,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
     for (int k = 0; k < SV; ++k) {
       const int v = tid + k * NT;
       // HVP: load_x fills xyz with v, and store_staged_ref reads the staging position itself (register budget)
-      if (!HVP && v < h.nv) { X[k] = __ldg(&p.X4[h.x4off + v]); X[k].w = __uint_as_float(uint32_t(__ldg(&p.pos16[h.x4off + v]))); }
+      if (!VS && v < h.nv) { X[k] = __ldg(&p.X4[h.x4off + v]); X[k].w = __uint_as_float(uint32_t(__ldg(&p.pos16[h.x4off + v]))); }
     }
   };
 
@@ -264,13 +278,21 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
 
   double des = 0.0, deb = 0.0, dea = 0.0;     // per-lane energy partials (smoothness, barrier, AMIPS)
   if (SPH && lane == 0) { red[3 * warp] = 0.0; red[3 * warp + 1] = 0.0; red[3 * warp + 2] = 0.0; }
+  // LINE: des carries d^T M d and deb u^T M d; lane l keeps the fp64 running sum of tet value line_idx(l) (the warp
+  // reduce-scatter below) in dln, and its smallest first root in rmin
+  constexpr int kLN = AMIPS ? 2 * kLineMaxAlpha : kLineMaxAlpha;   // tet values: barrier changes, then AMIPS changes
+  double dln = 0.0;
+  float rmin = INFINITY, amax = 0.f;
+  const int nal = LINE ? p.n_alpha : 0;
+  if constexpr (LINE)
+    for (int k = 0; k < nal; ++k) amax = fmaxf(amax, __ldg(p.alpha + k));
 
   // staged u = rel_u(x_i, X_i, c) with c = fp32(x_r - X_r) of the component's local vertex r = 0 (tsb_plan.cpp,
   // staging_tables): the component's rigid displacement never enters a rounded difference.  HVP: c = v_r, and the
   // u slots hold v_i - v_r
   auto load_ref = [&](const SegHdr &h, float (&r)[3]) {
     const size_t gr = gid_of(h, 0);
-    if constexpr (HVP) {
+    if constexpr (VS) {
       r[0] = __ldcg(p.v + 3 * gr); r[1] = __ldcg(p.v + 3 * gr + 1); r[2] = __ldcg(p.v + 3 * gr + 2);
     } else {
       const float4 Xr = __ldg(&p.X4[h.x4off]);
@@ -285,7 +307,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
       if (v < h.nv) {
         const size_t gi = gid_of(h, v);
         x[k][0] = __ldcg(p.x + 3 * gi); x[k][1] = __ldcg(p.x + 3 * gi + 1); x[k][2] = __ldcg(p.x + 3 * gi + 2);
-        if constexpr (HVP) { X[k].x = __ldcg(p.v + 3 * gi); X[k].y = __ldcg(p.v + 3 * gi + 1); X[k].z = __ldcg(p.v + 3 * gi + 2); }
+        if constexpr (VS) { X[k].x = __ldcg(p.v + 3 * gi); X[k].y = __ldcg(p.v + 3 * gi + 1); X[k].z = __ldcg(p.v + 3 * gi + 2); }
       }
     }
   };
@@ -296,8 +318,8 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
     for (int k = 0; k < SV; ++k) {
       const int v = tid + k * NT;
       if (v < h.nv) {
-        const uint32_t pos = HVP ? uint32_t(__ldg(&p.pos16[h.x4off + v])) : __float_as_uint(X[k].w);
-        if constexpr (HVP) ub[pos] = make_float4(X[k].x - ref[0], X[k].y - ref[1], X[k].z - ref[2], 0.f);
+        const uint32_t pos = VS ? uint32_t(__ldg(&p.pos16[h.x4off + v])) : __float_as_uint(X[k].w);
+        if constexpr (VS) ub[pos] = make_float4(X[k].x - ref[0], X[k].y - ref[1], X[k].z - ref[2], 0.f);
         else ub[pos] = make_float4(rel_u(x[k][0], X[k].x, ref[0]), rel_u(x[k][1], X[k].y, ref[1]), rel_u(x[k][2], X[k].z, ref[2]), 0.f);
         xb[pos] = make_float4(x[k][0], x[k][1], x[k][2], 0.f);
       }
@@ -317,7 +339,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
       const size_t gi = gid_of(h, v);
       const float x0 = __ldcg(p.x + 3 * gi), x1 = __ldcg(p.x + 3 * gi + 1), x2 = __ldcg(p.x + 3 * gi + 2);
       const uint32_t pos = __ldg(&p.pos16[h.x4off + v]);
-      if constexpr (HVP) ub[pos] = make_float4(__ldcg(p.v + 3 * gi) - r[0], __ldcg(p.v + 3 * gi + 1) - r[1], __ldcg(p.v + 3 * gi + 2) - r[2], 0.f);
+      if constexpr (VS) ub[pos] = make_float4(__ldcg(p.v + 3 * gi) - r[0], __ldcg(p.v + 3 * gi + 1) - r[1], __ldcg(p.v + 3 * gi + 2) - r[2], 0.f);
       else ub[pos] = make_float4(rel_u(x0, X.x, r[0]), rel_u(x1, X.y, r[1]), rel_u(x2, X.z, r[2]), 0.f);
       xb[pos] = make_float4(x0, x1, x2, 0.f);
     }
@@ -405,6 +427,26 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
     // energy with the rigid translation taken out of the cancellation
     const float4 uref = GLOBAL ? __ldg(p.u4g + hcur.x4off) : stage[ubase_of(hcur, li)];
     if (s == cs.x) TSB_STAMP(13);
+    // LINE: u^T M d = sum_i (u_i - c).(M d)_i for any c shared by the component (M has zero row and column sums), here
+    // c = fp32(x_r - X_r) of the component's reference vertex r, with u_i - c formed by rel_u as the energy stages it.
+    // The row's x_i is staged (x slot), its rest position X_i is read by vertex id
+    float lc[3] = {0.f, 0.f, 0.f};
+    if constexpr (LINE) {
+      const size_t gr = GLOBAL ? size_t(hcur.x4off) : gid_of(hcur, 0);
+      const float4 Xr = __ldg(&p.X4[hcur.x4off]);
+      lc[0] = __ldcg(p.x + 3 * gr) - Xr.x; lc[1] = __ldcg(p.x + 3 * gr + 1) - Xr.y; lc[2] = __ldcg(p.x + 3 * gr + 2) - Xr.z;
+    }
+    auto rest_of = [&](uint32_t rid) -> float4 {
+      if (GLOBAL) return __ldg(&p.X4[rid]);
+      if (hcur.vbase >= 0) return __ldg(&p.X4[hcur.x4off + int(rid) - hcur.vbase]);
+      // a component's vertices are staged in ascending id order: binary search of its vlist range
+      int lo = 0, hi = hcur.nv - 1;
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (uint32_t(__ldg(&p.vlist[hcur.x4off + mid])) < rid) lo = mid + 1; else hi = mid;
+      }
+      return __ldg(&p.X4[hcur.x4off + lo]);
+    };
 
     // ---- operator rows: L lanes per vertex row (header in slot 0 of the first quad) ------------------
     for (int rb = 0; rb < int(wseg.x); ++rb) {
@@ -453,6 +495,11 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
       }
       if (active && (lane & ((1u << llog) - 1u)) == 0) {
         des += double(fmaf(ui.x - uref.x, ax, fmaf(ui.y - uref.y, ay, (ui.z - uref.z) * az)));
+        if constexpr (LINE) {
+          const uint32_t dv16 = GLOBAL ? 0u : uint32_t(hcur.whole ? hcur.npos : p.vh) * 16u;   // as gatherV
+          const float4 xi = gatherX(rowj + dv16), Xi = rest_of(rid);
+          deb += double(fmaf(rel_u(xi.x, Xi.x, lc[0]), ax, fmaf(rel_u(xi.y, Xi.y, lc[1]), ay, rel_u(xi.z, Xi.z, lc[2]) * az)));
+        }
         if (grad) {
           const size_t gi = rid;
           grad[3 * gi] = s1 * ax; grad[3 * gi + 1] = s1 * ay; grad[3 * gi + 2] = s1 * az;
@@ -493,6 +540,9 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
     int nneg = 0;
     for (int tc = 0; tc < int(wseg.y); ++tc) {
       uint32_t dmask = 0;   // DET: bit t = this lane's tet t contributed
+      float lv[kLN];        // LINE: this lane's tets' changes per alpha (barrier, then AMIPS), summed over the cell
+#pragma unroll
+      for (int i = 0; i < kLN; ++i) lv[i] = 0.f;
       uint32_t tj[F::TPL][4];
       float tdet[F::TPL];
       if (GLOBAL) {
@@ -535,7 +585,127 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
           mnK = min(mnK, __reduce_min_sync(0xffffffffu, kJ));
           nneg += __popc(__ballot_sync(0xffffffffu, J < 0.f));
         }
-        if (HVP && J < 0.f) {
+        if constexpr (LINE) {
+          // det F(x + alpha d) = J + alpha (J1 + alpha (J2 + alpha J3)): with the edges e_k of x and f_k of d,
+          // J1 = idet f.cof E = idet sum_k f_k.c_k (c1 = e2 x e3, c2 = e3 x e1, c3 = e1 x e2), J2 = idet e.cof(f)
+          // = idet sum_k e_k.g_k (g1 = f2 x f3, ...), J3 = idet f1.g1
+          const float4 w0 = gatherV(tj[t][0]), w1 = gatherV(tj[t][1]), w2 = gatherV(tj[t][2]), w3 = gatherV(tj[t][3]);
+          const float f1x = w1.x - w0.x, f1y = w1.y - w0.y, f1z = w1.z - w0.z;
+          const float f2x = w2.x - w0.x, f2y = w2.y - w0.y, f2z = w2.z - w0.z;
+          const float f3x = w3.x - w0.x, f3y = w3.y - w0.y, f3z = w3.z - w0.z;
+          const float g1x = f2y * f3z - f2z * f3y, g1y = f2z * f3x - f2x * f3z, g1z = f2x * f3y - f2y * f3x;
+          const float J1 = (f1x * c1x + f1y * c1y + f1z * c1z + f2x * (e3y * e1z - e3z * e1y) + f2y * (e3z * e1x - e3x * e1z) +
+                            f2z * (e3x * e1y - e3y * e1x) + f3x * (e1y * e2z - e1z * e2y) + f3y * (e1z * e2x - e1x * e2z) +
+                            f3z * (e1x * e2y - e1y * e2x)) * idet;
+          const float J2 = (e1x * g1x + e1y * g1y + e1z * g1z + e2x * (f3y * f1z - f3z * f1y) + e2y * (f3z * f1x - f3x * f1z) +
+                            e2z * (f3x * f1y - f3y * f1x) + e3x * (f1y * f2z - f1z * f2y) + e3y * (f1z * f2x - f1x * f2z) +
+                            e3z * (f1x * f2y - f1y * f2x)) * idet;
+          const float J3 = (f1x * g1x + f1y * g1y + f1z * g1z) * idet;
+          auto dJ_at = [&](float al) { return al * fmaf(al, fmaf(al, J3, J2), J1); };   // J(al) - J, so J(0) = J
+          // AMIPS: I1(alpha) = |F + alpha dF|^2 = tr + alpha (2 fdf + alpha dd), F = E B, dF = f B
+          float tr = 0.f, fdf = 0.f, dd = 0.f, r0 = 0.f;
+          if (AMIPS && amips_on) {
+            const int slot = lane * int(F::TPL) + t;
+            const float4 *bp = p.Bt + (size_t(tcell0 + tc) * 3) * (32 * F::TPL) + slot;
+            const float4 b0 = __ldg(bp), b1 = __ldg(bp + 32 * F::TPL), b2 = __ldg(bp + 64 * F::TPL);
+            const float bb[3][3] = {{b0.x, b0.y, b0.z}, {b1.x, b1.y, b1.z}, {b2.x, b2.y, b2.z}};
+            const float ex[3] = {e1x, e2x, e3x}, ey[3] = {e1y, e2y, e3y}, ez[3] = {e1z, e2z, e3z};
+            const float fx[3] = {f1x, f2x, f3x}, fy[3] = {f1y, f2y, f3y}, fz[3] = {f1z, f2z, f3z};
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+              const float F0 = ex[0] * bb[0][c] + ex[1] * bb[1][c] + ex[2] * bb[2][c];
+              const float F1 = ey[0] * bb[0][c] + ey[1] * bb[1][c] + ey[2] * bb[2][c];
+              const float F2 = ez[0] * bb[0][c] + ez[1] * bb[1][c] + ez[2] * bb[2][c];
+              const float D0 = fx[0] * bb[0][c] + fx[1] * bb[1][c] + fx[2] * bb[2][c];
+              const float D1 = fy[0] * bb[0][c] + fy[1] * bb[1][c] + fy[2] * bb[2][c];
+              const float D2 = fz[0] * bb[0][c] + fz[1] * bb[1][c] + fz[2] * bb[2][c];
+              tr = fmaf(F0, F0, fmaf(F1, F1, fmaf(F2, F2, tr)));
+              fdf = fmaf(F0, D0, fmaf(F1, D1, fmaf(F2, D2, fdf)));
+              dd = fmaf(D0, D0, fmaf(D1, D1, fmaf(D2, D2, dd)));
+            }
+            if (J > 0.f) r0 = cbrtf(J);
+          }
+#pragma unroll
+          for (int k = 0; k < kLineMaxAlpha; ++k) {
+            if (k < nal) {
+              const float al = __ldg(p.alpha + k);
+              const float dJ = dJ_at(al), Ja = J + dJ;
+              // barrier: with both ends inverted m^p - m0^p = (m - m0)(m + m0)[(m^2 + m0^2)], m - m0 = -dJ
+              const float m0 = fmaxf(-J, 0.f), m = fmaxf(-Ja, 0.f);
+              float db;
+              if (Ja < 0.f && J < 0.f) {
+                const float q = -dJ * (m + m0);
+                db = order2 ? q : q * fmaf(m, m, m0 * m0);
+              } else {
+                const float mm = m * m, mm0 = m0 * m0;   // at most one of them is nonzero
+                db = order2 ? mm - mm0 : mm * mm - mm0 * mm0;
+              }
+              lv[k] += db;
+              if (AMIPS && amips_on) {
+                // psi = I1 / (3 J^(2/3)) - 1 where J > 0.  Both ends active: with r = J(alpha)^(1/3), r0 = J^(1/3),
+                // psi(alpha) - psi(0) = dI1 / (3 r^2) - I1(0) dJ (r0 + r) / (3 r^2 r0^2 (r^2 + r r0 + r0^2)),
+                // free of the cancellation of two psi values near 1
+                float da = 0.f;
+                const float dI = al * fmaf(al, dd, 2.f * fdf);
+                if (Ja > 0.f) {
+                  const float r = cbrtf(Ja), r2 = r * r, q = 1.f / (3.f * r2);
+                  if (J > 0.f) {
+                    const float r02 = r0 * r0;
+                    da = dI * q - tr * dJ * (r0 + r) * q / (r02 * fmaf(r, r + r0, r02));
+                  } else {
+                    da = (tr + dI) * q - 1.f;
+                  }
+                } else if (J > 0.f) {
+                  da = 1.f - tr / (3.f * (r0 * r0));
+                }
+                lv[kLineMaxAlpha + k] += da;
+              }
+            }
+          }
+          // first root of J(alpha) in (0, amax] for a real tet with J > 0 (padding tets have idet = 0, so J = 0): split
+          // [0, amax] at the roots of J' = J1 + 2 J2 a + 3 J3 a^2 into monotone pieces, find the first piece whose end
+          // has J <= 0 (or a critical point where J is within rounding of 0: a double root), then bisect it on the
+          // float's bit pattern (nonnegative floats order as their bits: 32 halvings reach adjacent floats at any scale)
+          float lo = 0.f, hi = -1.f;
+          if (J > 0.f && amax > 0.f) {
+            float q1 = 0.f, q2 = 0.f;    // critical points in (0, amax), ascending; 0 = none
+            if (J3 != 0.f) {
+              const float A = 3.f * J3, Bq = 2.f * J2;
+              const float D = fmaf(Bq, Bq, -4.f * A * J1);
+              if (D > 0.f) {
+                const float qq = -0.5f * (Bq + copysignf(sqrtf(D), Bq));
+                const float ra = qq / A, rb = qq != 0.f ? J1 / qq : ra;
+                q1 = fminf(ra, rb); q2 = fmaxf(ra, rb);
+              }
+            } else if (J2 != 0.f) {
+              q1 = -J1 / (2.f * J2);
+            }
+            q1 = (q1 > 0.f && q1 < amax) ? q1 : 0.f;
+            q2 = (q2 > 0.f && q2 < amax) ? q2 : 0.f;
+            const float ends[3] = {q1, q2, amax};
+#pragma unroll
+            for (int i = 0; i < 3; ++i) {
+              const float e = ends[i];
+              if (hi < 0.f && e > lo) {
+                const float Je = J + dJ_at(e);
+                const float tol = i < 2 ? 4.8e-7f * (fabsf(J) + e * (fabsf(J1) + e * (fabsf(J2) + e * fabsf(J3)))) : 0.f;
+                if (Je <= tol) { hi = e; if (Je > 0.f) lo = e; }
+                else lo = e;
+              }
+            }
+          }
+          if (__any_sync(0xffffffffu, hi >= 0.f)) {
+            uint32_t a = hi >= 0.f ? __float_as_uint(lo) : 0u, b = hi >= 0.f ? __float_as_uint(hi) : 0u;
+#pragma unroll 4
+            for (int it = 0; it < 32; ++it) {
+              const uint32_t mid = a + ((b - a) >> 1);
+              const bool pos = J + dJ_at(__uint_as_float(mid)) > 0.f;
+              a = pos ? mid : a;
+              b = pos ? b : mid;
+            }
+            if (hi >= 0.f) rmin = fminf(rmin, __uint_as_float(a));
+          }
+        } else if (HVP && J < 0.f) {
           // H_t v = phi''(J) dJ g + phi'(J) dg with g_k = dJ/dx_k, dJ = sum_k g_k.f_k and dg_k its derivative along v
           // (f_k = v_k - v_0); phi = (-J)^p.  v^T H_t v = sum_{k=1..3} f_k.(H_t v)_k
           const float m = -J, m2 = m * m;
@@ -744,6 +914,22 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
           }
         }
       }
+      if constexpr (LINE) {
+        // warp reduce-scatter of the cell's kLN sums in fp32 (one halving per xor offset 16, 8, ...; the lanes of a pair
+        // keep the upper or the lower half), then each lane adds value line_idx(lane) to its fp64 running sum
+#pragma unroll
+        for (int h = kLN / 2, o = 16; h >= 1; h >>= 1, o >>= 1) {
+          const bool up = lane & o;
+#pragma unroll
+          for (int i = 0; i < h; ++i) {
+            const float send = up ? lv[i] : lv[i + h], keep = up ? lv[i + h] : lv[i];
+            lv[i] = keep + __shfl_xor_sync(0xffffffffu, send, o);
+          }
+        }
+#pragma unroll
+        for (int o = 16 / kLN; o >= 1; o >>= 1) lv[0] += __shfl_xor_sync(0xffffffffu, lv[0], o);
+        dln += double(lv[0]);
+      }
       if (DET && grad) {   // every launch with a gradient rewrites every cell's ballot: inactive slots are never read
         const unsigned m0 = __ballot_sync(0xffffffffu, dmask & 1u), m1 = F::TPL > 1 ? __ballot_sync(0xffffffffu, dmask & 2u) : 0u;
         if (lane == 0) {
@@ -790,80 +976,105 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
       }
       des = 0.0; deb = 0.0; dea = 0.0;
     }
+    // LINE: the CTA's record of the segment.  The warp's values (tet value j in lane line_lane(j), then u^T M d, d^T M d
+    // and the smallest root) are combined over the warps in fixed order, three per round through red[]
+    if constexpr (LINE) {
+      const double wud = warp_sum(deb), wmd = warp_sum(des);
+      const float wmin = __uint_as_float(__reduce_min_sync(0xffffffffu, __float_as_uint(rmin)));   // roots are >= 0
+      LineRec *rec = line_rec(p.sph_rec, s, NW);
+      constexpr int nv = kLN + 3;
+      for (int q0 = 0; q0 < nv; q0 += 3) {
+        const int j = q0 + min(lane, 2);
+        const double tv = __shfl_sync(0xffffffffu, dln, line_lane<kLN>(j < kLN ? j : 0));
+        const double val = j < kLN ? tv : (j == kLN ? wud : (j == kLN + 1 ? wmd : double(wmin)));
+        if (lane < 3 && j < nv) red[3 * warp + lane] = val;
+        __syncthreads();
+        if (warp == 0 && lane < 3 && j < nv) {
+          double acc = red[lane];
+          for (int w = 1; w < NW; ++w) acc = j == nv - 1 ? fmin(acc, red[3 * w + lane]) : acc + red[3 * w + lane];
+          rec->v[j < kLN ? j : 2 * kLineMaxAlpha + (j - kLN)] = acc;
+        }
+        __syncthreads();
+      }
+      if (!AMIPS && warp == 0 && lane < kLineMaxAlpha) rec->v[kLineMaxAlpha + lane] = 0.0;
+      des = 0.0; deb = 0.0; dln = 0.0;
+      rmin = INFINITY;
+    }
     hcur = hn;
   }
-
-  // ---- energies: lanes -> warp -> CTA partial; CTA 0 folds all partials in fixed order ---------------------
-  TSB_STAMP(7);
-  if constexpr (!SPH) {   // SPH: red[] already holds the warp's sums, segment by segment
-    des = warp_sum(des);
-    deb = warp_sum(deb);
-    if (AMIPS) dea = warp_sum(dea);
-    if (lane == 0) { red[3 * warp] = des; red[3 * warp + 1] = deb; red[3 * warp + 2] = dea; }
-  }
-  __syncthreads();
-  TSB_STAMP(8);
-  if (tid == 0) {
-    double a = 0.0, b = 0.0, c = 0.0;
-    for (int w = 0; w < NW; ++w) { a += red[3 * w]; b += red[3 * w + 1]; c += red[3 * w + 2]; }
-    if constexpr (!HVP) a *= 0.5;   // HVP: v^T M v itself
-    // two 16-byte stores carry the partials; their arrival IS the "this CTA is done" signal (no fence, no ticket)
-    unsigned long long ua = (unsigned long long)__double_as_longlong(a), ub = (unsigned long long)__double_as_longlong(b);
-    unsigned long long uc = (unsigned long long)__double_as_longlong(c);
-    if (ua == kSentinel) ua = 0x7FF8000000000000ull;
-    if (ub == kSentinel) ub = 0x7FF8000000000000ull;
-    if (uc == kSentinel) uc = 0x7FF8000000000000ull;
-    asm volatile("st.global.v2.u64 [%0], {%1, %2};" ::"l"(p.cta_energy + 4 * blockIdx.x), "l"(ua), "l"(ub) : "memory");
-    asm volatile("st.global.v2.u64 [%0], {%1, %2};" ::"l"(p.cta_energy + 4 * blockIdx.x + 2), "l"(uc), "l"(0ull) : "memory");
-  }
-  TSB_STAMP(9);
-  if (blockIdx.x == 0 && warp == 0) {
-    __syncwarp();
-    double a = 0.0, b = 0.0, c3sum = 0.0;
-    // Each lane owns slots lane, lane + 32, ...; the loads of a batch of kPollBatch slots are issued together, so one
-    // L2 round trip after the last partial has landed finishes the fold (polling them one after the other cost five
-    // dependent round trips, ~2 us per launch).  The summation order stays fixed: slot order per lane, then the shuffle tree.
-    constexpr int kPollBatch = 5;
-    for (int c0 = lane; c0 < int(gridDim.x); c0 += 32 * kPollBatch) {
-      unsigned long long ua[kPollBatch], ub[kPollBatch], uc[kPollBatch], ud[kPollBatch];
-      bool pending = true;
-      while (pending) {
-        pending = false;
+  if constexpr (!LINE) {   // LINE: no energy fold, the records are the output
+    // ---- energies: lanes -> warp -> CTA partial; CTA 0 folds all partials in fixed order ---------------------
+    TSB_STAMP(7);
+    if constexpr (!SPH) {   // SPH: red[] already holds the warp's sums, segment by segment
+      des = warp_sum(des);
+      deb = warp_sum(deb);
+      if (AMIPS) dea = warp_sum(dea);
+      if (lane == 0) { red[3 * warp] = des; red[3 * warp + 1] = deb; red[3 * warp + 2] = dea; }
+    }
+    __syncthreads();
+    TSB_STAMP(8);
+    if (tid == 0) {
+      double a = 0.0, b = 0.0, c = 0.0;
+      for (int w = 0; w < NW; ++w) { a += red[3 * w]; b += red[3 * w + 1]; c += red[3 * w + 2]; }
+      if constexpr (!HVP) a *= 0.5;   // HVP: v^T M v itself
+      // two 16-byte stores carry the partials; their arrival IS the "this CTA is done" signal (no fence, no ticket)
+      unsigned long long ua = (unsigned long long)__double_as_longlong(a), ub = (unsigned long long)__double_as_longlong(b);
+      unsigned long long uc = (unsigned long long)__double_as_longlong(c);
+      if (ua == kSentinel) ua = 0x7FF8000000000000ull;
+      if (ub == kSentinel) ub = 0x7FF8000000000000ull;
+      if (uc == kSentinel) uc = 0x7FF8000000000000ull;
+      asm volatile("st.global.v2.u64 [%0], {%1, %2};" ::"l"(p.cta_energy + 4 * blockIdx.x), "l"(ua), "l"(ub) : "memory");
+      asm volatile("st.global.v2.u64 [%0], {%1, %2};" ::"l"(p.cta_energy + 4 * blockIdx.x + 2), "l"(uc), "l"(0ull) : "memory");
+    }
+    TSB_STAMP(9);
+    if (blockIdx.x == 0 && warp == 0) {
+      __syncwarp();
+      double a = 0.0, b = 0.0, c3sum = 0.0;
+      // Each lane owns slots lane, lane + 32, ...; the loads of a batch of kPollBatch slots are issued together, so one
+      // L2 round trip after the last partial has landed finishes the fold (polling them one after the other cost five
+      // dependent round trips, ~2 us per launch).  The summation order stays fixed: slot order per lane, then the shuffle tree.
+      constexpr int kPollBatch = 5;
+      for (int c0 = lane; c0 < int(gridDim.x); c0 += 32 * kPollBatch) {
+        unsigned long long ua[kPollBatch], ub[kPollBatch], uc[kPollBatch], ud[kPollBatch];
+        bool pending = true;
+        while (pending) {
+          pending = false;
+#pragma unroll
+          for (int k = 0; k < kPollBatch; ++k) {
+            const int c = c0 + 32 * k;
+            if (c < int(gridDim.x)) {
+              asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(ua[k]), "=l"(ub[k]) : "l"(p.cta_energy + 4 * c) : "memory");
+              asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(uc[k]), "=l"(ud[k]) : "l"(p.cta_energy + 4 * c + 2) : "memory");
+            }
+          }
+#pragma unroll
+          for (int k = 0; k < kPollBatch; ++k)
+            if (c0 + 32 * k < int(gridDim.x)) pending |= ua[k] == kSentinel || ub[k] == kSentinel || uc[k] == kSentinel || ud[k] == kSentinel;
+        }
 #pragma unroll
         for (int k = 0; k < kPollBatch; ++k) {
           const int c = c0 + 32 * k;
           if (c < int(gridDim.x)) {
-            asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(ua[k]), "=l"(ub[k]) : "l"(p.cta_energy + 4 * c) : "memory");
-            asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(uc[k]), "=l"(ud[k]) : "l"(p.cta_energy + 4 * c + 2) : "memory");
+            asm volatile("st.global.v2.u64 [%0], {%1, %2};" ::"l"(p.cta_energy + 4 * c), "l"(kSentinel), "l"(kSentinel) : "memory");   // re-arm
+            asm volatile("st.global.v2.u64 [%0], {%1, %2};" ::"l"(p.cta_energy + 4 * c + 2), "l"(kSentinel), "l"(kSentinel) : "memory");
+            a += __longlong_as_double((long long)ua[k]);
+            b += __longlong_as_double((long long)ub[k]);
+            c3sum += __longlong_as_double((long long)uc[k]);
           }
         }
-#pragma unroll
-        for (int k = 0; k < kPollBatch; ++k)
-          if (c0 + 32 * k < int(gridDim.x)) pending |= ua[k] == kSentinel || ub[k] == kSentinel || uc[k] == kSentinel || ud[k] == kSentinel;
       }
-#pragma unroll
-      for (int k = 0; k < kPollBatch; ++k) {
-        const int c = c0 + 32 * k;
-        if (c < int(gridDim.x)) {
-          asm volatile("st.global.v2.u64 [%0], {%1, %2};" ::"l"(p.cta_energy + 4 * c), "l"(kSentinel), "l"(kSentinel) : "memory");   // re-arm
-          asm volatile("st.global.v2.u64 [%0], {%1, %2};" ::"l"(p.cta_energy + 4 * c + 2), "l"(kSentinel), "l"(kSentinel) : "memory");
-          a += __longlong_as_double((long long)ua[k]);
-          b += __longlong_as_double((long long)ub[k]);
-          c3sum += __longlong_as_double((long long)uc[k]);
-        }
+      a = warp_sum(a); b = warp_sum(b); c3sum = warp_sum(c3sum);
+      if (lane == 0 && (!HVP || p.energy_out)) {   // HVP: energy_out is the optional curvature
+        p.energy_out[0] = float(double(p.c1) * a + double(p.c2) * b + double(p.c3) * c3sum);
+        p.energy_out[1] = float(a);
+        p.energy_out[2] = float(b);
+        if (p.energy4) p.energy_out[3] = float(c3sum);
       }
+      if (!DET)
+        for (int c = lane; c < p.n_components; c += 32) p.done[c] = 0u;   // every CTA has finished: safe to re-arm
     }
-    a = warp_sum(a); b = warp_sum(b); c3sum = warp_sum(c3sum);
-    if (lane == 0 && (!HVP || p.energy_out)) {   // HVP: energy_out is the optional curvature
-      p.energy_out[0] = float(double(p.c1) * a + double(p.c2) * b + double(p.c3) * c3sum);
-      p.energy_out[1] = float(a);
-      p.energy_out[2] = float(b);
-      if (p.energy4) p.energy_out[3] = float(c3sum);
-    }
-    if (!DET)
-      for (int c = lane; c < p.n_components; c += 32) p.done[c] = 0u;   // every CTA has finished: safe to re-arm
+    TSB_STAMP(10);
   }
-  TSB_STAMP(10);
 #ifdef TSB_TRACE
   if (tid == 0 && p.trace) p.trace[blockIdx.x * kTraceSlots + 11] = gtime();
 #endif
@@ -972,6 +1183,79 @@ __global__ void __launch_bounds__(kFoldWarps * 32) sphere_fold_kernel(const SphP
   }
 }
 
+// Line search, after a LINE launch on the same stream.  Every sum below runs in a fixed order over the records alone.
+struct LineArgs {
+  const float *alpha;
+  int32_t n_alpha;
+  float c1, c2, c3;
+};
+
+// (c1 ds + c2 db + c3 da, ds, db, da) at alpha_k from a (component or total) value set held one value per lane (lane j:
+// value j of LineRec), written by lane k < n_alpha to out[4k..4k+3]; ds = alpha u^T M d + 1/2 alpha^2 d^T M d
+__device__ __forceinline__ void line_write_delta(double v, int lane, const LineArgs &la, float *out) {
+  const double ud = __shfl_sync(0xffffffffu, v, 2 * kLineMaxAlpha), dd = __shfl_sync(0xffffffffu, v, 2 * kLineMaxAlpha + 1);
+  const double db = __shfl_sync(0xffffffffu, v, lane & (kLineMaxAlpha - 1));
+  const double da = __shfl_sync(0xffffffffu, v, kLineMaxAlpha + (lane & (kLineMaxAlpha - 1)));
+  if (out && lane < la.n_alpha) {
+    const double al = double(__ldg(la.alpha + lane));
+    const double ds = al * ud + 0.5 * (al * al) * dd;
+    out[4 * lane] = float(double(la.c1) * ds + double(la.c2) * db + double(la.c3) * da);
+    out[4 * lane + 1] = float(ds);
+    out[4 * lane + 2] = float(db);
+    out[4 * lane + 3] = float(da);
+  }
+}
+
+// One warp per component: lane j < kLineVals folds value j of the component's segment records in segment order (the
+// root: their minimum) and stores it over the record of the component's first segment (each lane reads and writes its
+// own slot only), then the optional per-sphere outputs.
+__global__ void __launch_bounds__(kFoldWarps * 32) line_fold_kernel(const SphParams sp, const LineArgs la, float *__restrict__ sd,
+                                                                    float *__restrict__ ss) {
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  const int c = blockIdx.x * kFoldWarps + int(threadIdx.x >> 5), lane = int(threadIdx.x & 31);
+  if (c >= sp.n_components) return;
+  SphRec *rec = const_cast<SphRec *>(sp.rec);
+  const int s0 = __ldg(&sp.comp_seg[c]), s1 = __ldg(&sp.comp_seg[c + 1]);
+  double v = 0.0;
+  if (lane < kLineVals) {
+    v = line_rec(rec, s0, sp.nw)->v[lane];
+    for (int s = s0 + 1; s < s1; ++s) {
+      const double e = line_rec(rec, s, sp.nw)->v[lane];
+      v = lane == kLineVals - 1 ? fmin(v, e) : v + e;
+    }
+    line_rec(rec, s0, sp.nw)->v[lane] = v;
+  }
+  line_write_delta(v, lane, la, sd ? sd + size_t(c) * la.n_alpha * 4 : nullptr);
+  if (ss && lane == kLineVals - 1) ss[c] = float(v);
+}
+
+// One CTA: warp w folds the components w, w + kFoldWarps, ... in order (lane j: value j), warp 0 the warps' partials in
+// order; then delta_out and step_out.
+__global__ void __launch_bounds__(kFoldWarps * 32) line_total_kernel(const SphParams sp, const LineArgs la, float *__restrict__ delta,
+                                                                     float *__restrict__ step) {
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  __shared__ double part[kFoldWarps][kLineVals];
+  const int w = int(threadIdx.x >> 5), lane = int(threadIdx.x & 31);
+  const SphRec *rec = sp.rec;
+  if (lane < kLineVals) {
+    double v = lane == kLineVals - 1 ? double(INFINITY) : 0.0;
+    for (int c = w; c < sp.n_components; c += kFoldWarps) {
+      const double e = line_rec(const_cast<SphRec *>(rec), __ldg(&sp.comp_seg[c]), sp.nw)->v[lane];
+      v = lane == kLineVals - 1 ? fmin(v, e) : v + e;
+    }
+    part[w][lane] = v;
+  }
+  __syncthreads();
+  if (w != 0) return;
+  double v = 0.0;
+  if (lane < kLineVals) {
+    v = part[0][lane];
+    for (int k = 1; k < kFoldWarps; ++k) v = lane == kLineVals - 1 ? fmin(v, part[k][lane]) : v + part[k][lane];
+  }
+  line_write_delta(v, lane, la, delta);
+  if (step && lane == kLineVals - 1) step[0] = float(v);
+}
+
 // ---- level-1 helpers -------------------------------------------------------------------------------
 __global__ void scale_kernel(const float *__restrict__ g, int64_t count, float gradH, const float *gradH_dev,
                              float *__restrict__ out) {
@@ -1055,13 +1339,15 @@ inline int grid_for(int64_t count, int block) {
   return int(g < 1 ? 1 : (g > kMaxGrid ? kMaxGrid : g));
 }
 
-// ---- the energy_grad_kernel instantiations, by flag bits f = AMIPS | DET << 1 | SPH << 2 | HVP << 3 -----------------
+// ---- the energy_grad_kernel instantiations, by flag bits f = AMIPS | DET << 1 | SPH << 2 | HVP << 3 | LINE << 4 ------
 using EnergyKernel = void (*)(KParams);
 
-// HVP is never combined with SPH: those entries are nullptr and never instantiated
+// HVP is never combined with SPH, LINE with nothing but AMIPS: those entries are nullptr and never instantiated
 template <int NW, int MINB, bool GLOBAL, int F>
 constexpr EnergyKernel kernel_of() {
   if constexpr ((F & 8) && (F & 4)) return nullptr;
+  else if constexpr ((F & 16) && (F & 14)) return nullptr;
+  else if constexpr (F & 16) return energy_grad_kernel<NW, MINB, GLOBAL, bool(F & 1), false, false, false, true>;
   else return energy_grad_kernel<NW, MINB, GLOBAL, bool(F & 1), bool(F & 2), bool(F & 4), bool(F & 8)>;
 }
 
@@ -1072,9 +1358,9 @@ const EnergyKernel *flag_table(std::integer_sequence<int, F...>) {
 }
 
 // 16 warps run one CTA per SM, 8 warps two; nullptr for any other nw or a combination that is not instantiated
-EnergyKernel energy_kernel(int nw, bool global, bool amips, bool det, bool sph, bool hvp = false) {
-  constexpr std::make_integer_sequence<int, 16> flags{};
-  const int f = int(amips) | int(det) << 1 | int(sph) << 2 | int(hvp) << 3;
+EnergyKernel energy_kernel(int nw, bool global, bool amips, bool det, bool sph, bool hvp = false, bool line = false) {
+  constexpr std::make_integer_sequence<int, 32> flags{};
+  const int f = int(amips) | int(det) << 1 | int(sph) << 2 | int(hvp) << 3 | int(line) << 4;
   if (nw == 16) return (global ? flag_table<16, 1, true>(flags) : flag_table<16, 1, false>(flags))[f];
   if (nw == 8) return (global ? flag_table<8, 2, true>(flags) : flag_table<8, 2, false>(flags))[f];
   return nullptr;
@@ -1099,12 +1385,12 @@ cudaError_t energy_occupancy(int nw, int smem_bytes, bool global, bool amips, bo
   *ctas_per_sm = 0;
   if (smem_bytes > optin) return cudaSuccess;   // does not fit
   // every instantiation the handle may launch: AMIPS ones when amips, DET ones when det, with and without SPH, and the
-  // HVP ones (tsb_hvp, and tsb_hvp_ex's AMIPS ones when amips)
+  // HVP ones (tsb_hvp, and tsb_hvp_ex's AMIPS ones when amips), and the LINE ones (tsb_line_search)
   int ctas = 1 << 30;
-  for (int f = 0; f < 16; ++f) {
+  for (int f = 0; f < 32; ++f) {
     if (((f & 1) && !amips) || ((f & 2) && !det)) continue;
-    const EnergyKernel k = energy_kernel(nw, global, f & 1, f & 2, f & 4, f & 8);
-    if (!k) continue;   // HVP with SPH
+    const EnergyKernel k = energy_kernel(nw, global, f & 1, f & 2, f & 4, f & 8, f & 16);
+    if (!k) continue;   // HVP with SPH, LINE with anything but AMIPS
     if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, optin) != cudaSuccess) {
       cudaGetLastError();
       return cudaSuccess;   // does not fit
@@ -1119,10 +1405,10 @@ cudaError_t energy_occupancy(int nw, int smem_bytes, bool global, bool amips, bo
 }
 
 cudaError_t launch_energy_grad(const KParams &p, const LaunchConfig &lc, cudaStream_t stream) {
-  const EnergyKernel k = energy_kernel(lc.nw, lc.global, lc.amips, lc.det, lc.sph, lc.hvp);
+  const EnergyKernel k = energy_kernel(lc.nw, lc.global, lc.amips, lc.det, lc.sph, lc.hvp, lc.line);
   if (!k) return cudaErrorInvalidValue;
   if (lc.global) {
-    if (lc.hvp) prestage_hvp_kernel<<<grid_for(p.n, 256), 256, 0, stream>>>(p.x, p.v, p.X4, p.u4g, p.x4g, p.n);
+    if (lc.hvp || lc.line) prestage_hvp_kernel<<<grid_for(p.n, 256), 256, 0, stream>>>(p.x, p.v, p.X4, p.u4g, p.x4g, p.n);
     else prestage_kernel<<<grid_for(p.n, 256), 256, 0, stream>>>(p.x, p.X4, p.u4g, p.x4g, p.n);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
@@ -1150,6 +1436,17 @@ cudaError_t launch_det_gather(const DetParams &d, float *grad, cudaStream_t stre
 
 cudaError_t launch_sphere_fold(const SphParams &sp, tsb_sphere_stats_t *out, cudaStream_t stream) {
   sphere_fold_kernel<<<unsigned((sp.n_components + kFoldWarps - 1) / kFoldWarps), kFoldWarps * 32, 0, stream>>>(sp, out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_line_fold(const SphParams &sp, const float *alpha, int n_alpha, float c1, float c2, float c3,
+                             float *delta_out, float *step_out, float *sphere_delta_out, float *sphere_step_out,
+                             cudaStream_t stream) {
+  const LineArgs la{alpha, n_alpha, c1, c2, c3};
+  if (sp.n_components > 0)
+    line_fold_kernel<<<unsigned((sp.n_components + kFoldWarps - 1) / kFoldWarps), kFoldWarps * 32, 0, stream>>>(
+        sp, la, sphere_delta_out, sphere_step_out);
+  line_total_kernel<<<1, kFoldWarps * 32, 0, stream>>>(sp, la, delta_out, step_out);
   return cudaGetLastError();
 }
 

@@ -18,6 +18,21 @@ struct __align__(16) SphRec {
 };
 static_assert(sizeof(SphRec) == 32, "SphRec must be 32 bytes");
 
+// What one CTA saw of one segment in a line search (LINE instantiation), in fp64: v[k] = barrier change at alpha_k,
+// v[8 + k] = AMIPS change, v[16] = u^T M d and v[17] = d^T M d over the segment's rows, v[18] = the smallest first
+// root of a tet's det F along d (+inf: none).  Segment s's record lies at byte s * nw * 32 of the sph_rec array (nw
+// SphRec slots per segment, >= 256 bytes), so the line search needs no device memory of its own.  line_fold_kernel
+// overwrites the record of a component's first segment with the component's sums.
+constexpr int kLineMaxAlpha = TSB_LINE_MAX_ALPHA;
+constexpr int kLineVals = 2 * kLineMaxAlpha + 3;
+struct LineRec {
+  double v[kLineVals];
+};
+static_assert(sizeof(LineRec) <= 8 * sizeof(SphRec), "a LineRec must fit the SphRec slots of one segment");
+__host__ __device__ inline LineRec *line_rec(SphRec *base, int s, int nw) {
+  return reinterpret_cast<LineRec *>(reinterpret_cast<unsigned char *>(base) + size_t(s) * size_t(nw) * sizeof(SphRec));
+}
+
 struct KParams {
   // plan (read-only, built once by tsb_create)
   const unsigned char *stream;  // per-warp byte streams (operator rows + tet blocks)
@@ -62,6 +77,10 @@ struct KParams {
   // Hessian-vector product only (the HVP instantiations, tsb_hvp / tsb_hvp_ex): grad receives gradH H(x) v, energy_out
   // (may be nullptr) v^T H v as (c1 vMv + c2 vHbv + c3 vHav, vMv, vHbv[, vHav when energy4])
   const float *v;               // [3n] direction
+  // line search only (the LINE instantiations, tsb_line_search): v is the direction d, grad and energy_out are nullptr,
+  // and the per-segment records (LineRec) are written over sph_rec
+  const float *alpha;           // [n_alpha] step sizes, read on the device
+  int32_t n_alpha;              // 1..kLineMaxAlpha
 #ifdef TSB_TRACE
   unsigned long long *trace;    // profiling build only: [grid][kTraceSlots] phase stamps
 #endif
@@ -77,6 +96,7 @@ struct LaunchConfig {
   int det;         // launch the deterministic instantiation (tets store their corners instead of adding them)
   int sph;         // launch the SPH instantiation (it also writes the per-(segment, warp) sphere records)
   int hvp;         // launch the HVP instantiation (Hessian-vector product; never with sph)
+  int line;        // launch the LINE instantiation (line search; combines with amips only)
 };
 
 // sphere_fold_kernel's inputs (HostPlan::comp_*, uploaded, and the records of the SPH launch before it).
@@ -114,6 +134,11 @@ cudaError_t launch_energy_grad(const KParams &p, const LaunchConfig &lc, cudaStr
 cudaError_t launch_det_gather(const DetParams &d, float *grad, cudaStream_t stream);
 // One tsb_sphere_stats_t per component from the records of the SPH launch before it on the same stream.
 cudaError_t launch_sphere_fold(const SphParams &sp, tsb_sphere_stats_t *out, cudaStream_t stream);
+// After a LINE launch on the same stream: per-component sums of its records (in place, and to the optional per-sphere
+// outputs), then their fixed-order total to delta_out [n_alpha][4] and the optional step_out [1].
+cudaError_t launch_line_fold(const SphParams &sp, const float *alpha, int n_alpha, float c1, float c2, float c3,
+                             float *delta_out, float *step_out, float *sphere_delta_out, float *sphere_step_out,
+                             cudaStream_t stream);
 
 cudaError_t launch_scale(const float *g, int64_t count, float gradH, const float *gradH_dev, float *out, cudaStream_t s);
 cudaError_t launch_grad_limit(float *g, int64_t count, float thr, float s, float *work4, cudaStream_t st);

@@ -192,6 +192,14 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         hv, _ = self.tet_sp.hvp(x.detach(), v.detach(), c1, c2, self.order_at(it), c3=self.amips_coeff)
         return hv.reshape(x.shape)
 
+    def line_search(self, x, d, it, alphas, per_sphere=False):
+        """``E(x + alpha_k d) - E(x)`` of ``c1 * smooth + c2 * barrier (+ amips_coeff * amips)`` at the step sizes
+        ``alphas`` and the largest inversion-free step along ``d`` (``tet_spheres_ext.LineSearch``), with the scheduler's
+        coefficients and the barrier order at ``it``; outside autograd, no host sync."""
+        c1, c2 = self.coeff_scheduler(it)
+        return self.tet_sp.line_search(x.detach(), d.detach(), alphas, c1, c2, self.order_at(it), c3=self.amips_coeff,
+                                       per_sphere=per_sphere)
+
     def forward(self, x, it, c1, c2):
         order = self.order_at(it)
         if self.amips_coeff > 0:

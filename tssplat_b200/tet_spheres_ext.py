@@ -32,7 +32,8 @@ import torch
 from . import _capi
 from .mesh import load_veg
 
-__all__ = ["TetSpheres", "SphereStats", "forward", "backward", "hvp", "random_x", "grad_limit", "energy_grad_host"]
+__all__ = ["TetSpheres", "SphereStats", "LineSearch", "forward", "backward", "hvp", "line_search", "random_x", "grad_limit",
+           "energy_grad_host"]
 
 return_cpu_scalar = False
 _limit_work = {}       # (device, stream) -> float32[4] scratch of grad_limit (caller-owned in the C ABI)
@@ -64,6 +65,15 @@ class SphereStats(NamedTuple):
 
 
 _STATS_BYTES = C.sizeof(_capi.tsb_sphere_stats_t)     # 40
+
+
+class LineSearch(NamedTuple):
+    """What ``TetSpheres.line_search`` returns, device tensors (``tsb_line_search`` in ``include/tssplat_b200.h``).
+    K = number of step sizes, S = number of components (spheres, in the order of their lowest vertex ids)."""
+    delta: torch.Tensor                        # f32 [K, 4]: (c1 ds + c2 db + c3 da, ds, db, da) = E(x + alpha_k d) - E(x)
+    max_step: torch.Tensor                     # f32 []: first alpha in (0, max alphas] at which a tet inverts (+inf: none)
+    sphere_delta: Optional[torch.Tensor]       # f32 [S, K, 4] per sphere, or None
+    sphere_max_step: Optional[torch.Tensor]    # f32 [S] per sphere, or None
 
 
 class TetSpheres:
@@ -248,6 +258,35 @@ class TetSpheres:
         del keep
         return hv, curv
 
+    def line_search(self, x: torch.Tensor, d: torch.Tensor, alphas, c1: float, c2: float, order: int, c3: float = 0.0,
+                    per_sphere: bool = False) -> LineSearch:
+        """Energy changes ``E(x + alpha_k d) - E(x)`` of ``c1 * smooth + c2 * barrier (+ c3 * amips)`` at up to 8 step
+        sizes, per term, and the largest inversion-free step along ``d`` (``tsb_line_search``), in one pass over the plan
+        and without a host sync.  ``alphas``: a sequence of floats, or a CUDA float32 tensor that is read on the device
+        when the launch runs (so a captured CUDA graph can be replayed with new values written into it).  ``c3`` needs a
+        handle created with ``enable_amips=True``.  ``per_sphere`` also returns each sphere's changes and step."""
+        xc = self._check_x(x)
+        dc = self._check_x(d)
+        if isinstance(alphas, torch.Tensor):
+            if not alphas.is_cuda or alphas.dtype != torch.float32 or alphas.device != self.device or not alphas.is_contiguous():
+                raise RuntimeError("alphas must be a contiguous float32 tensor on the handle's device, or a sequence of floats")
+            a = alphas.reshape(-1)
+        else:
+            a = torch.tensor([float(v) for v in alphas], dtype=torch.float32).to(self.device, non_blocking=True)
+        K = int(a.numel())
+        delta = torch.empty((K, 4), dtype=torch.float32, device=self.device)
+        step = torch.empty((), dtype=torch.float32, device=self.device)
+        S = int(self.info["n_components"])
+        sd = torch.empty((S, K, 4), dtype=torch.float32, device=self.device) if per_sphere else None
+        ss = torch.empty((S,), dtype=torch.float32, device=self.device) if per_sphere else None
+        terms = _capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
+        rc = _capi.lib.tsb_line_search(self._h, xc.data_ptr(), dc.data_ptr(), C.byref(terms), a.data_ptr(), K,
+                                       delta.data_ptr(), step.data_ptr(), sd.data_ptr() if per_sphere else None,
+                                       ss.data_ptr() if per_sphere else None, _stream_ptr(self.device))
+        if rc:
+            _capi.check(rc, self._h, "tet_spheres_ext.line_search")
+        return LineSearch(delta, step, sd, ss)
+
 
 def energy_grad_host(tet_sp: TetSpheres, x_host: torch.Tensor, c1: float, c2: float, order: int, gradH: float,
                      energy_host: torch.Tensor, grad_host: Optional[torch.Tensor]) -> None:
@@ -328,6 +367,13 @@ def hvp(v: torch.Tensor, vertexPositions: torch.Tensor, tet_sp: TetSpheres, c1: 
     ``backward``, with the direction in place of ``gradH``; ``c3`` as in ``TetSpheres.hvp``)."""
     hv, _ = tet_sp.hvp(vertexPositions, v, c1, c2, order, c3=c3)
     return hv.reshape(vertexPositions.shape)
+
+
+def line_search(d: torch.Tensor, vertexPositions: torch.Tensor, tet_sp: TetSpheres, alphas, c1: float, c2: float,
+                order: int, c3: float = 0.0, per_sphere: bool = False) -> LineSearch:
+    """``TetSpheres.line_search`` in the argument order of ``hvp`` (direction first): the energy changes at ``alphas``
+    along ``d`` and the largest inversion-free step."""
+    return tet_sp.line_search(vertexPositions, d, alphas, c1, c2, order, c3=c3, per_sphere=per_sphere)
 
 
 def random_x(tet_sp: TetSpheres) -> torch.Tensor:
