@@ -20,7 +20,7 @@
 extern "C" {
 #endif
 
-#define TSB_VERSION 5
+#define TSB_VERSION 6
 #define TSB_LINE_MAX_ALPHA 8   /* step sizes one tsb_line_search call may evaluate */
 
 enum {
@@ -215,6 +215,25 @@ int tsb_hvp_ex(tsb_handle_t h, const float *x_dev, const float *v_dev, const tsb
 int tsb_line_search(tsb_handle_t h, const float *x_dev, const float *d_dev, const tsb_terms_t *terms,
                     const float *alpha_dev, int32_t n_alpha, float *delta_out_dev, float *step_out_dev,
                     float *sphere_delta_out_dev, float *sphere_step_out_dev, void *stream);
+
+/* Per-vertex 3x3 diagonal blocks of the Hessian of what tsb_hvp_ex differentiates (no counterpart in the reference),
+ * for block-Jacobi preconditioning:
+ *   diag_out = gradH * (*gradH_dev) * D      (device float32 [2][n][3], fully overwritten, required)
+ * where D_i is the 3x3 block of H(x) = c1 M + c2 sum_t H_t + c3 sum_t H_a,t at vertex i (the H of tsb_hvp_ex):
+ * plane 0 holds (H_xx, H_yy, H_zz) of each vertex, plane 1 (H_yz, H_xz, H_xy).  The smoothness part is c1 M_ii I
+ * (M = M1 (x) I3).  A tet with fp32 J < 0 adds, at each corner k, the rank-1 block p (p-1) (-J)^(p-2) g_k g_k^T
+ * (g_k = dJ/dx_k); with c3 != 0 a tet with fp32 J > 0 adds the exact AMIPS block of its corner, which may be indefinite
+ * far from rest.  Vertices no tet references get zero rows in both planes.  c1, c2, order, c3 from *terms with
+ * tsb_hvp_ex's rules.  Default handle: one launch; the rows are stored, then active tets add their six entries per
+ * corner with red.global.add.f32 (order-dependent rounding in their vertices).  Deterministic handle: one launch and
+ * one deterministic gather per plane; the output is then bitwise identical across launches, streams, CUDA-graph replays
+ * and handles with the same options, and rows no active tet touches are bitwise those of a default handle.  Uses no
+ * device memory of its own and leaves the handle's scratch re-armed, so it chains with tsb_energy_grad(_ex),
+ * tsb_hvp(_ex) and tsb_line_search on one stream.  Argument errors (TSB_E_INVALID, nothing launched): a null terms,
+ * x_dev or diag_out_dev, an order other than 2 or 4, terms->c3 != 0 on a handle without enable_amips.
+ * DESIGN.md section 5, "Hessian diagonal". */
+int tsb_hess_diag(tsb_handle_t h, const float *x_dev, const tsb_terms_t *terms, float gradH, const float *gradH_dev,
+                  float *diag_out_dev, void *stream);
 
 /* Same computation for callers whose vertex positions live in HOST memory (e.g. a CPU-side
  * optimiser): copies x_host -> device, runs the fused launch, copies energy[3] and grad back,

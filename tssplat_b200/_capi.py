@@ -19,7 +19,7 @@ TSB_LINE_MAX_ALPHA = 8
 # every symbol include/tssplat_b200.h declares (tests check the library exports each one)
 EXPORTED_SYMBOLS = (
     "tsb_create", "tsb_destroy", "tsb_last_error", "tsb_get_info", "tsb_energy_grad", "tsb_energy_grad_ex", "tsb_energy_grad_spheres", "tsb_hvp", "tsb_hvp_ex",
-    "tsb_line_search", "tsb_energy_grad_host", "tsb_scale",
+    "tsb_line_search", "tsb_hess_diag", "tsb_energy_grad_host", "tsb_scale",
     "tsb_grad_limit", "tsb_adam_uniform_step",
     "tsb_surface_create", "tsb_surface_destroy", "tsb_surface_last_error", "tsb_surface_forward", "tsb_surface_backward",
     "tsb_surface_extract", "tsb_free_host", "tsb_setup_last_error",
@@ -81,6 +81,8 @@ def _load() -> C.CDLL:
     lib.tsb_hvp_ex.argtypes = [vp, vp, vp, C.POINTER(tsb_terms_t), f32, vp, vp, vp, vp]
     lib.tsb_line_search.restype = C.c_int
     lib.tsb_line_search.argtypes = [vp, vp, vp, C.POINTER(tsb_terms_t), vp, i32, vp, vp, vp, vp, vp]
+    lib.tsb_hess_diag.restype = C.c_int
+    lib.tsb_hess_diag.argtypes = [vp, vp, C.POINTER(tsb_terms_t), f32, vp, vp, vp]
     lib.tsb_energy_grad_host.restype = C.c_int
     lib.tsb_energy_grad_host.argtypes = [vp, vp, f32, f32, i32, f32, vp, vp, vp]
     lib.tsb_scale.restype = C.c_int

@@ -385,6 +385,43 @@ int tsb_line_search(tsb_handle_t h, const float *x_dev, const float *d_dev, cons
   return TSB_OK;
 }
 
+int tsb_hess_diag(tsb_handle_t h, const float *x_dev, const tsb_terms_t *terms, float gradH, const float *gradH_dev,
+                  float *diag_out_dev, void *stream) {
+  if (!h) return TSB_E_INVALID;
+  if (!terms) return fail(h, TSB_E_INVALID, "terms is null");
+  if (!x_dev || !diag_out_dev) return fail(h, TSB_E_INVALID, "x_dev and diag_out_dev must be non-null");
+  if (terms->order != 2 && terms->order != 4) return fail(h, TSB_E_INVALID, "order must be 2 or 4");
+  if (terms->c3 != 0.f && !h->amips)
+    return fail(h, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return fail(h, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  tsb::KParams kp = h->kp;
+  kp.x = x_dev; kp.v = nullptr; kp.grad = diag_out_dev; kp.energy_out = nullptr; kp.gradH_dev = gradH_dev;
+  kp.c1 = terms->c1; kp.c2 = terms->c2; kp.c3 = terms->c3; kp.gradH = gradH; kp.order = terms->order; kp.energy4 = 0;
+  kp.diag_plane = 0;
+  tsb::LaunchConfig lc = h->lc;
+  lc.amips = terms->c3 != 0.f ? 1 : 0;
+  lc.det = h->det ? 1 : 0;
+  lc.sph = 0;
+  lc.hvp = 0;
+  lc.line = 0;
+  lc.diag = 1;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // default handle: one launch writes both planes; deterministic handle: a tet slot holds one plane of its corners, so
+  // one launch and one gather per plane
+  for (int plane = 0; plane < (lc.det ? 2 : 1); ++plane) {
+    kp.diag_plane = plane;
+    kp.grad = diag_out_dev + size_t(plane) * 3 * size_t(h->info.n);
+    cudaError_t e = tsb::launch_energy_grad(kp, lc, st);
+    if (e != cudaSuccess) return fail(h, TSB_E_CUDA, std::string("hess_diag launch: ") + cudaGetErrorString(e));
+    if (lc.det) {
+      e = tsb::launch_det_gather(h->dp, kp.grad, st);
+      if (e != cudaSuccess) return fail(h, TSB_E_CUDA, std::string("deterministic gather launch: ") + cudaGetErrorString(e));
+    }
+  }
+  return TSB_OK;
+}
+
 int tsb_energy_grad_host(tsb_handle_t h, const float *x_host, float c1, float c2, int32_t order, float gradH,
                          float *energy_out_host, float *grad_out_host, void *stream) {
   if (!h) return TSB_E_INVALID;

@@ -183,7 +183,11 @@ struct WarpStream {
 // LINE (tsb_line_search; with AMIPS only): staged as HVP with v = d, so the row pass yields M d; a row adds d^T M d and
 // u^T M d, every real tet its barrier (and AMIPS) change at each alpha_k and the first root of its det F along d.  No
 // gradient, no energy fold: the CTA's warps combine their sums per segment into one LineRec (DESIGN.md section 5).
-template <int NW, int MINB, bool GLOBAL, bool AMIPS, bool DET = false, bool SPH = false, bool HVP = false, bool LINE = false>
+// DIAG (tsb_hess_diag; with AMIPS and DET only): staged as the gradient.  A row stores s1 M_ii = -s1 sum_j M_ij (its
+// streamed weights, no gather), an inverted tet (and with AMIPS a tet with J > 0) the diagonal 3x3 blocks of its Hessian
+// at its four corners, through the same scratch or atomics as the gradient (DESIGN.md section 5, "Hessian diagonal").
+template <int NW, int MINB, bool GLOBAL, bool AMIPS, bool DET = false, bool SPH = false, bool HVP = false, bool LINE = false,
+          bool DIAG = false>
 __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParams p) {
   using F = Fmt<GLOBAL>;
   constexpr bool VS = HVP || LINE;   // the u slots hold a direction (v, or d) instead of x - X
@@ -273,6 +277,10 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
     for (int i = blockIdx.x * NT + tid; i < p.n_orphans; i += gridDim.x * NT) {
       const int v = __ldg(&p.orphans[i]);
       grad[3 * size_t(v)] = 0.f; grad[3 * size_t(v) + 1] = 0.f; grad[3 * size_t(v) + 2] = 0.f;
+      if constexpr (DIAG && !DET) {   // both planes in one launch
+        float *g2 = grad + 3 * size_t(p.n);
+        g2[3 * size_t(v)] = 0.f; g2[3 * size_t(v) + 1] = 0.f; g2[3 * size_t(v) + 2] = 0.f;
+      }
     }
   }
 
@@ -455,7 +463,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
       const bool active = rid != 0xFFFFFFu;
       const uint32_t rowj = GLOBAL ? *reinterpret_cast<const uint32_t *>(ws.cell + lane * 16)
                                    : uint32_t(*reinterpret_cast<const uint16_t *>(ws.cell + lane * 8));
-      const float4 ui = gatherU(rowj);
+      const float4 ui = DIAG ? make_float4(0.f, 0.f, 0.f, 0.f) : gatherU(rowj);
       f32x2 AX{0.f, 0.f}, AY{0.f, 0.f}, AZ{0.f, 0.f};     // (even-entry, odd-entry) partial sums
       uint32_t left = len4;
       while (left) {
@@ -472,6 +480,13 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
             j[0] = qi.x & 0xFFFFu; j[1] = qi.x >> 16; j[2] = qi.y & 0xFFFFu; j[3] = qi.y >> 16;
           }
           const float4 qw = *reinterpret_cast<const float4 *>(cp + WOFF + lane * (16 - 4 * F::IB));
+          if constexpr (DIAG) {
+            // the row's off-diagonal weights M_ij; an entry whose column is the row itself is the lane's header slot
+            // (its weight is the header's bit pattern) and adds nothing, as it adds nothing to M u
+            AX.lo += j[0] != rowj ? qw.x : 0.f; AX.hi += j[1] != rowj ? qw.y : 0.f;
+            AX.lo += j[2] != rowj ? qw.z : 0.f; AX.hi += j[3] != rowj ? qw.w : 0.f;
+            continue;
+          }
           const float4 u0 = gatherU(j[0]), u1 = gatherU(j[1]), u2 = gatherU(j[2]), u3 = gatherU(j[3]);
           const f32x2 W01 = pk2(qw.x, qw.y), W23 = pk2(qw.z, qw.w);
           fma2_acc(AX, W01, pk2(u0.x - ui.x, u1.x - ui.x));
@@ -490,10 +505,22 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
       float ax = sum2(AX), ay = sum2(AY), az = sum2(AZ);
       for (uint32_t o = 1; o < (1u << llog); o <<= 1) {   // the L lanes of a row are adjacent
         ax += __shfl_xor_sync(0xffffffffu, ax, o);
-        ay += __shfl_xor_sync(0xffffffffu, ay, o);
-        az += __shfl_xor_sync(0xffffffffu, az, o);
+        if constexpr (!DIAG) {
+          ay += __shfl_xor_sync(0xffffffffu, ay, o);
+          az += __shfl_xor_sync(0xffffffffu, az, o);
+        }
       }
-      if (active && (lane & ((1u << llog) - 1u)) == 0) {
+      if (DIAG && active && (lane & ((1u << llog) - 1u)) == 0) {
+        // plane 0: s1 M_ii (1, 1, 1) with M_ii = -sum_{j != i} M_ij (M has zero row sums); plane 1: 0.  DET: the plane
+        // of this launch
+        const size_t gi = rid;
+        const float d = (DET && p.diag_plane) ? 0.f : -(s1 * ax);
+        grad[3 * gi] = d; grad[3 * gi + 1] = d; grad[3 * gi + 2] = d;
+        if constexpr (!DET) {
+          float *g2 = grad + 3 * size_t(p.n);
+          g2[3 * gi] = 0.f; g2[3 * gi + 1] = 0.f; g2[3 * gi + 2] = 0.f;
+        }
+      } else if (!DIAG && active && (lane & ((1u << llog) - 1u)) == 0) {
         des += double(fmaf(ui.x - uref.x, ax, fmaf(ui.y - uref.y, ay, (ui.z - uref.z) * az)));
         if constexpr (LINE) {
           const uint32_t dv16 = GLOBAL ? 0u : uint32_t(hcur.whole ? hcur.npos : p.vh) * 16u;   // as gatherV
@@ -556,9 +583,9 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
         tj[F::TPL - 1][0] = a.z & 0xFFFFu; tj[F::TPL - 1][1] = a.z >> 16; tj[F::TPL - 1][2] = a.w & 0xFFFFu; tj[F::TPL - 1][3] = a.w >> 16;
         tdet[0] = d.x; tdet[F::TPL - 1] = d.y;
       }
-      // HVP with AMIPS: a lane's later tets gather their corners when they are reached, so that those registers are
-      // free for the AMIPS product (the staging area and x4g stay valid for the whole segment)
-      constexpr bool kLateX = HVP && AMIPS;
+      // HVP or DIAG with AMIPS: a lane's later tets gather their corners when they are reached, so that those registers
+      // are free for the AMIPS product or blocks (the staging area and x4g stay valid for the whole segment)
+      constexpr bool kLateX = (HVP || DIAG) && AMIPS;
       float4 xv[F::TPL][4];
 #pragma unroll
       for (int t = 0; t < int(F::TPL); ++t)
@@ -585,7 +612,88 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
           mnK = min(mnK, __reduce_min_sync(0xffffffffu, kJ));
           nneg += __popc(__ballot_sync(0xffffffffu, J < 0.f));
         }
-        if constexpr (LINE) {
+        if constexpr (DIAG) {
+          // Diagonal block of corner k: D_k = al |b_k|^2 I + be (g f^T + f g^T) + ga g g^T, g = dJ/dx_k = idet c_k (the
+          // gradient's corner vector; g_0 = -(g_1 + g_2 + g_3)).  Barrier (J < 0, m = -J): J is multilinear in the
+          // corners, so d2J/dx_k^2 = 0 and al = be = 0, ga = s2 p (p-1) m^(p-2).  AMIPS (J > 0): moving corner k gives
+          // dF = delta b_k^T (b_k: row k of B = Dm^-1, b_0 = -sum), f = F b_k, a = 2 / (3 J^(2/3)): al = s3 a,
+          // be = -2 al / (3 J), ga = 5 al I1 / (9 J^2)   (DESIGN.md section 5, "Hessian diagonal")
+          if (J < 0.f || (AMIPS && amips_on && J > 0.f)) {
+            float al = 0.f, be = 0.f, ga;
+            float Fm[3][3] = {}, bb[3][3] = {};
+            if (J < 0.f) {
+              const float m = -J;
+              ga = s2 * (order2 ? 2.f : 12.f * m * m);
+            } else {
+              const int slot = lane * int(F::TPL) + t;
+              const float4 *bp = p.Bt + (size_t(tcell0 + tc) * 3) * (32 * F::TPL) + slot;
+              const float4 b0 = __ldg(bp), b1 = __ldg(bp + 32 * F::TPL), b2 = __ldg(bp + 64 * F::TPL);
+              bb[0][0] = b0.x; bb[0][1] = b0.y; bb[0][2] = b0.z;
+              bb[1][0] = b1.x; bb[1][1] = b1.y; bb[1][2] = b1.z;
+              bb[2][0] = b2.x; bb[2][1] = b2.y; bb[2][2] = b2.z;
+              const float ex[3] = {e1x, e2x, e3x}, ey[3] = {e1y, e2y, e3y}, ez[3] = {e1z, e2z, e3z};
+              float tr = 0.f;
+#pragma unroll
+              for (int c = 0; c < 3; ++c) {
+                Fm[0][c] = ex[0] * bb[0][c] + ex[1] * bb[1][c] + ex[2] * bb[2][c];
+                Fm[1][c] = ey[0] * bb[0][c] + ey[1] * bb[1][c] + ey[2] * bb[2][c];
+                Fm[2][c] = ez[0] * bb[0][c] + ez[1] * bb[1][c] + ez[2] * bb[2][c];
+                tr = fmaf(Fm[0][c], Fm[0][c], fmaf(Fm[1][c], Fm[1][c], fmaf(Fm[2][c], Fm[2][c], tr)));
+              }
+              const float cb = cbrtf(J), iJ = 1.f / J;
+              al = s3 * (2.f / (3.f * (cb * cb)));
+              be = -(2.f / 3.f) * al * iJ;
+              ga = (5.f / 9.f) * al * tr * (iJ * iJ);
+            }
+            // the six entries of D_k: (xx, yy, zz) for plane 0, (yz, xz, xy) for plane 1
+            auto block = [&](const float (&g)[3], const float (&f)[3], float b2, float (&o)[6]) {
+#pragma unroll
+              for (int r = 0; r < 3; ++r) o[r] = fmaf(al, b2, fmaf(2.f * be * g[r], f[r], ga * g[r] * g[r]));
+              o[3] = fmaf(be, fmaf(g[1], f[2], f[1] * g[2]), ga * g[1] * g[2]);
+              o[4] = fmaf(be, fmaf(g[0], f[2], f[0] * g[2]), ga * g[0] * g[2]);
+              o[5] = fmaf(be, fmaf(g[0], f[1], f[0] * g[1]), ga * g[0] * g[1]);
+            };
+            const bool pl = DET && p.diag_plane;
+            float keep[4][3];   // DET: this launch's plane of every corner
+            auto emit = [&](int k, const float (&o)[6]) {
+              if constexpr (DET) {
+#pragma unroll
+                for (int r = 0; r < 3; ++r) keep[k][r] = pl ? o[3 + r] : o[r];
+              } else {
+                const size_t vk = 3 * gid_x(tj[t][k]);
+                float *g2 = grad + 3 * size_t(p.n);
+#pragma unroll
+                for (int r = 0; r < 3; ++r) { atomicAdd(grad + vk + r, o[r]); atomicAdd(g2 + vk + r, o[3 + r]); }
+              }
+            };
+            if constexpr (DET) dmask |= 1u << t;
+            else wait_rows();
+            // corner k = 0..3: the edge pair (a, b) of c_k = a x b, with c_0 = -(c1 + c2 + c3) = (e3 - e1) x (e2 - e1)
+            // (c1 = e2 x e3, c2 = e3 x e1, c3 = e1 x e2), and b_k (b_0 = -(b_1 + b_2 + b_3))
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const float ax = k == 0 ? e3x - e1x : (k == 1 ? e2x : (k == 2 ? e3x : e1x));
+              const float ay = k == 0 ? e3y - e1y : (k == 1 ? e2y : (k == 2 ? e3y : e1y));
+              const float az = k == 0 ? e3z - e1z : (k == 1 ? e2z : (k == 2 ? e3z : e1z));
+              const float bx = k == 0 ? e2x - e1x : (k == 1 ? e3x : (k == 2 ? e1x : e2x));
+              const float by = k == 0 ? e2y - e1y : (k == 1 ? e3y : (k == 2 ? e1y : e2y));
+              const float bz = k == 0 ? e2z - e1z : (k == 1 ? e3z : (k == 2 ? e1z : e2z));
+              const float g[3] = {idet * (ay * bz - az * by), idet * (az * bx - ax * bz), idet * (ax * by - ay * bx)};
+              float bk[3];
+#pragma unroll
+              for (int c = 0; c < 3; ++c) bk[c] = k == 0 ? -(bb[0][c] + bb[1][c] + bb[2][c]) : bb[k - 1][c];
+              float f[3];
+#pragma unroll
+              for (int r = 0; r < 3; ++r) f[r] = Fm[r][0] * bk[0] + Fm[r][1] * bk[1] + Fm[r][2] * bk[2];
+              float o[6];
+              block(g, f, bk[0] * bk[0] + bk[1] * bk[1] + bk[2] * bk[2], o);
+              emit(k, o);
+            }
+            if constexpr (DET)
+              det_store(tc, t, keep[0][0], keep[0][1], keep[0][2], keep[1][0], keep[1][1], keep[1][2], keep[2][0], keep[2][1],
+                        keep[2][2], keep[3][0], keep[3][1], keep[3][2]);
+          }
+        } else if constexpr (LINE) {
           // det F(x + alpha d) = J + alpha (J1 + alpha (J2 + alpha J3)): with the edges e_k of x and f_k of d,
           // J1 = idet f.cof E = idet sum_k f_k.c_k (c1 = e2 x e3, c2 = e3 x e1, c3 = e1 x e2), J2 = idet e.cof(f)
           // = idet sum_k e_k.g_k (g1 = f2 x f3, ...), J3 = idet f1.g1
@@ -1064,7 +1172,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
         }
       }
       a = warp_sum(a); b = warp_sum(b); c3sum = warp_sum(c3sum);
-      if (lane == 0 && (!HVP || p.energy_out)) {   // HVP: energy_out is the optional curvature
+      if (lane == 0 && (!(HVP || DIAG) || p.energy_out)) {   // HVP: energy_out is the optional curvature; DIAG: nullptr
         p.energy_out[0] = float(double(p.c1) * a + double(p.c2) * b + double(p.c3) * c3sum);
         p.energy_out[1] = float(a);
         p.energy_out[2] = float(b);
@@ -1339,14 +1447,18 @@ inline int grid_for(int64_t count, int block) {
   return int(g < 1 ? 1 : (g > kMaxGrid ? kMaxGrid : g));
 }
 
-// ---- the energy_grad_kernel instantiations, by flag bits f = AMIPS | DET << 1 | SPH << 2 | HVP << 3 | LINE << 4 ------
+// ---- the energy_grad_kernel instantiations, by flag bits f = AMIPS | DET << 1 | SPH << 2 | HVP << 3 | LINE << 4 |
+// DIAG << 5 ------------------------------------------------------------------------------------------------------------
 using EnergyKernel = void (*)(KParams);
 
-// HVP is never combined with SPH, LINE with nothing but AMIPS: those entries are nullptr and never instantiated
+// HVP is never combined with SPH, LINE with nothing but AMIPS, DIAG with nothing but AMIPS and DET: those entries are
+// nullptr and never instantiated
 template <int NW, int MINB, bool GLOBAL, int F>
 constexpr EnergyKernel kernel_of() {
   if constexpr ((F & 8) && (F & 4)) return nullptr;
   else if constexpr ((F & 16) && (F & 14)) return nullptr;
+  else if constexpr ((F & 32) && (F & 28)) return nullptr;
+  else if constexpr (F & 32) return energy_grad_kernel<NW, MINB, GLOBAL, bool(F & 1), bool(F & 2), false, false, false, true>;
   else if constexpr (F & 16) return energy_grad_kernel<NW, MINB, GLOBAL, bool(F & 1), false, false, false, true>;
   else return energy_grad_kernel<NW, MINB, GLOBAL, bool(F & 1), bool(F & 2), bool(F & 4), bool(F & 8)>;
 }
@@ -1358,9 +1470,10 @@ const EnergyKernel *flag_table(std::integer_sequence<int, F...>) {
 }
 
 // 16 warps run one CTA per SM, 8 warps two; nullptr for any other nw or a combination that is not instantiated
-EnergyKernel energy_kernel(int nw, bool global, bool amips, bool det, bool sph, bool hvp = false, bool line = false) {
-  constexpr std::make_integer_sequence<int, 32> flags{};
-  const int f = int(amips) | int(det) << 1 | int(sph) << 2 | int(hvp) << 3 | int(line) << 4;
+EnergyKernel energy_kernel(int nw, bool global, bool amips, bool det, bool sph, bool hvp = false, bool line = false,
+                           bool diag = false) {
+  constexpr std::make_integer_sequence<int, 64> flags{};
+  const int f = int(amips) | int(det) << 1 | int(sph) << 2 | int(hvp) << 3 | int(line) << 4 | int(diag) << 5;
   if (nw == 16) return (global ? flag_table<16, 1, true>(flags) : flag_table<16, 1, false>(flags))[f];
   if (nw == 8) return (global ? flag_table<8, 2, true>(flags) : flag_table<8, 2, false>(flags))[f];
   return nullptr;
@@ -1385,12 +1498,13 @@ cudaError_t energy_occupancy(int nw, int smem_bytes, bool global, bool amips, bo
   *ctas_per_sm = 0;
   if (smem_bytes > optin) return cudaSuccess;   // does not fit
   // every instantiation the handle may launch: AMIPS ones when amips, DET ones when det, with and without SPH, and the
-  // HVP ones (tsb_hvp, and tsb_hvp_ex's AMIPS ones when amips), and the LINE ones (tsb_line_search)
+  // HVP ones (tsb_hvp, and tsb_hvp_ex's AMIPS ones when amips), the LINE ones (tsb_line_search) and the DIAG ones
+  // (tsb_hess_diag)
   int ctas = 1 << 30;
-  for (int f = 0; f < 32; ++f) {
+  for (int f = 0; f < 64; ++f) {
     if (((f & 1) && !amips) || ((f & 2) && !det)) continue;
-    const EnergyKernel k = energy_kernel(nw, global, f & 1, f & 2, f & 4, f & 8, f & 16);
-    if (!k) continue;   // HVP with SPH, LINE with anything but AMIPS
+    const EnergyKernel k = energy_kernel(nw, global, f & 1, f & 2, f & 4, f & 8, f & 16, f & 32);
+    if (!k) continue;   // HVP with SPH, LINE with anything but AMIPS, DIAG with anything but AMIPS and DET
     if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, optin) != cudaSuccess) {
       cudaGetLastError();
       return cudaSuccess;   // does not fit
@@ -1405,7 +1519,7 @@ cudaError_t energy_occupancy(int nw, int smem_bytes, bool global, bool amips, bo
 }
 
 cudaError_t launch_energy_grad(const KParams &p, const LaunchConfig &lc, cudaStream_t stream) {
-  const EnergyKernel k = energy_kernel(lc.nw, lc.global, lc.amips, lc.det, lc.sph, lc.hvp, lc.line);
+  const EnergyKernel k = energy_kernel(lc.nw, lc.global, lc.amips, lc.det, lc.sph, lc.hvp, lc.line, lc.diag);
   if (!k) return cudaErrorInvalidValue;
   if (lc.global) {
     if (lc.hvp || lc.line) prestage_hvp_kernel<<<grid_for(p.n, 256), 256, 0, stream>>>(p.x, p.v, p.X4, p.u4g, p.x4g, p.n);

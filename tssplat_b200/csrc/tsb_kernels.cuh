@@ -81,6 +81,10 @@ struct KParams {
   // and the per-segment records (LineRec) are written over sph_rec
   const float *alpha;           // [n_alpha] step sizes, read on the device
   int32_t n_alpha;              // 1..kLineMaxAlpha
+  // Hessian diagonal only (the DIAG instantiations, tsb_hess_diag): grad receives the per-vertex 3x3 diagonal blocks,
+  // (H_xx, H_yy, H_zz) in plane 0 and (H_yz, H_xz, H_xy) in plane 1 (grad + 3n).  DET: one launch per plane, grad points
+  // at that plane and diag_plane selects it (a tet slot holds one plane of its four corners)
+  int32_t diag_plane;
 #ifdef TSB_TRACE
   unsigned long long *trace;    // profiling build only: [grid][kTraceSlots] phase stamps
 #endif
@@ -97,6 +101,7 @@ struct LaunchConfig {
   int sph;         // launch the SPH instantiation (it also writes the per-(segment, warp) sphere records)
   int hvp;         // launch the HVP instantiation (Hessian-vector product; never with sph)
   int line;        // launch the LINE instantiation (line search; combines with amips only)
+  int diag;        // launch the DIAG instantiation (Hessian diagonal blocks; combines with amips and det only)
 };
 
 // sphere_fold_kernel's inputs (HostPlan::comp_*, uploaded, and the records of the SPH launch before it).
@@ -127,7 +132,7 @@ int energy_smem_bytes(int nw, int ring_slots, int cells_per_chunk, int area_vert
 constexpr unsigned long long kEnergySentinel = 0x7FF8F00DBAADC0DEull;   // initial value of cta_energy
 // Max co-resident CTAs per SM for a configuration (0 if it does not fit): the minimum over every instantiation a handle
 // may launch (AMIPS ones when amips, deterministic ones when det, each with and without the sphere records, and the
-// Hessian-vector product ones); also opts them in to the smem size.
+// Hessian-vector product, line search and Hessian diagonal ones); also opts them in to the smem size.
 cudaError_t energy_occupancy(int nw, int smem_bytes, bool global, bool amips, bool det, int *ctas_per_sm);
 cudaError_t launch_energy_grad(const KParams &p, const LaunchConfig &lc, cudaStream_t stream);
 // grad[v] += the active corner vectors of v's list, in list order, for every flagged component (after a DET launch).

@@ -200,6 +200,14 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         return self.tet_sp.line_search(x.detach(), d.detach(), alphas, c1, c2, self.order_at(it), c3=self.amips_coeff,
                                        per_sphere=per_sphere)
 
+    def hess_diag(self, x, it):
+        """Per-vertex 3x3 diagonal blocks of the Hessian of ``c1 * smooth + c2 * barrier (+ amips_coeff * amips)`` with
+        the scheduler's coefficients and the barrier order at ``it`` (``tsb_hess_diag``), as [2, n, 3] (see
+        ``TetSpheres.hess_diag``); outside autograd, no host sync.  ``tssplat_b200.newton.block_jacobi`` makes a
+        preconditioner of them."""
+        c1, c2 = self.coeff_scheduler(it)
+        return self.tet_sp.hess_diag(x.detach(), c1, c2, self.order_at(it), c3=self.amips_coeff)
+
     def forward(self, x, it, c1, c2):
         order = self.order_at(it)
         if self.amips_coeff > 0:

@@ -32,8 +32,8 @@ import torch
 from . import _capi
 from .mesh import load_veg
 
-__all__ = ["TetSpheres", "SphereStats", "LineSearch", "forward", "backward", "hvp", "line_search", "random_x", "grad_limit",
-           "energy_grad_host"]
+__all__ = ["TetSpheres", "SphereStats", "LineSearch", "forward", "backward", "hvp", "line_search", "hess_diag", "random_x",
+           "grad_limit", "energy_grad_host"]
 
 return_cpu_scalar = False
 _limit_work = {}       # (device, stream) -> float32[4] scratch of grad_limit (caller-owned in the C ABI)
@@ -287,6 +287,28 @@ class TetSpheres:
             _capi.check(rc, self._h, "tet_spheres_ext.line_search")
         return LineSearch(delta, step, sd, ss)
 
+    def hess_diag(self, x: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0, gradH=1.0,
+                  out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Per-vertex 3x3 diagonal blocks of the Hessian of ``c1 * smooth + c2 * barrier (+ c3 * amips)`` at ``x``
+        (``tsb_hess_diag``), scaled by ``gradH``, as [2, n, 3] on the device without a host sync: ``[0]`` holds
+        (H_xx, H_yy, H_zz) of each vertex, ``[1]`` (H_yz, H_xz, H_xy).  ``tssplat_b200.newton.hess_blocks`` turns them into
+        [n, 3, 3] blocks.  ``c3`` needs a handle created with ``enable_amips=True``; ``gradH`` may be a CUDA tensor (read
+        on the device).  ``out``: an optional contiguous float32 [2, n, 3] tensor on the handle's device to write into."""
+        xc = self._check_x(x)
+        if out is None:
+            out = torch.empty((2, self.n, 3), dtype=torch.float32, device=self.device)
+        elif (not isinstance(out, torch.Tensor) or out.dtype != torch.float32 or out.device != self.device
+              or not out.is_contiguous() or out.numel() != 2 * self.n3):
+            raise RuntimeError("out must be a contiguous float32 tensor of 2 * 3n entries on the handle's device")
+        gh_val, gh_ptr, keep = self._gradH_arg(gradH)
+        terms = _capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
+        rc = _capi.lib.tsb_hess_diag(self._h, xc.data_ptr(), C.byref(terms), gh_val, gh_ptr, out.data_ptr(),
+                                     _stream_ptr(self.device))
+        if rc:
+            _capi.check(rc, self._h, "tet_spheres_ext.hess_diag")
+        del keep
+        return out
+
 
 def energy_grad_host(tet_sp: TetSpheres, x_host: torch.Tensor, c1: float, c2: float, order: int, gradH: float,
                      energy_host: torch.Tensor, grad_host: Optional[torch.Tensor]) -> None:
@@ -374,6 +396,13 @@ def line_search(d: torch.Tensor, vertexPositions: torch.Tensor, tet_sp: TetSpher
     """``TetSpheres.line_search`` in the argument order of ``hvp`` (direction first): the energy changes at ``alphas``
     along ``d`` and the largest inversion-free step."""
     return tet_sp.line_search(vertexPositions, d, alphas, c1, c2, order, c3=c3, per_sphere=per_sphere)
+
+
+def hess_diag(vertexPositions: torch.Tensor, tet_sp: TetSpheres, c1: float, c2: float, order: int,
+              c3: float = 0.0) -> torch.Tensor:
+    """``TetSpheres.hess_diag`` in the argument order of ``forward``: the per-vertex 3x3 diagonal blocks of the Hessian
+    as [2, n, 3] (diagonal entries, then (yz, xz, xy))."""
+    return tet_sp.hess_diag(vertexPositions, c1, c2, order, c3=c3)
 
 
 def random_x(tet_sp: TetSpheres) -> torch.Tensor:
