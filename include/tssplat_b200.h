@@ -20,7 +20,7 @@
 extern "C" {
 #endif
 
-#define TSB_VERSION 6
+#define TSB_VERSION 7
 #define TSB_LINE_MAX_ALPHA 8   /* step sizes one tsb_line_search call may evaluate */
 
 enum {
@@ -234,6 +234,89 @@ int tsb_line_search(tsb_handle_t h, const float *x_dev, const float *d_dev, cons
  * DESIGN.md section 5, "Hessian diagonal". */
 int tsb_hess_diag(tsb_handle_t h, const float *x_dev, const tsb_terms_t *terms, float gradH, const float *gradH_dev,
                   float *diag_out_dev, void *stream);
+
+/* ---- Newton-CG solve: per-sphere preconditioned CG on the device (no counterpart in the reference) --------------
+ * Spheres share no vertices, so the Hessian H(x) of tsb_hvp_ex is block diagonal by connected component.  tsb_pcg_solve
+ * runs block-Jacobi preconditioned, truncated (Steihaug) conjugate gradients on every block independently -- each
+ * sphere its own alpha, beta, residual test and negative-curvature test -- with all spheres batched in the same
+ * launches and every scalar in device memory: no device-to-host read inside an iteration.  DESIGN.md section 5,
+ * "Newton-CG solve".
+ *
+ * A workspace is a separate object sized from a handle (which must outlive it); creating one changes nothing about the
+ * handle (tsb_get_info and the plan stay as they are).  It owns the component vertex lists (the non-orphan vertex ids
+ * grouped by component, ascending inside a component, components in the order of tsb_energy_grad_spheres), a chunk
+ * table of <= 256 vertices per chunk, the vectors r, z, p, Hp, the inverse preconditioner blocks, per-chunk fp64
+ * partial sums and the per-component state.  Device memory, reported by tsb_pcg_device_bytes:
+ *   72 n + 4 rows + 36 chunks + 64 n_components + 4 (n_components + 1) + 4   bytes
+ * (rows = vertices some tet references, chunks = sum over components of ceil(vertices / 256)).  Like a handle, a
+ * workspace serves one stream at a time. */
+typedef struct tsb_pcg_s *tsb_pcg_t;
+int tsb_pcg_create(tsb_handle_t h, tsb_pcg_t *out);
+void tsb_pcg_destroy(tsb_pcg_t s);
+const char *tsb_pcg_last_error(tsb_pcg_t s);   /* s may be NULL: last tsb_pcg_create failure */
+int64_t tsb_pcg_device_bytes(tsb_pcg_t s);
+
+/* Sets the preconditioner from the diagonal blocks of tsb_hess_diag (diag_dev: device float32 [2][n][3]; NULL = the
+ * identity, which is also what a new workspace holds).  One kernel, one thread per vertex: the symmetric 3x3 block is
+ * diagonalised in fp64 registers (cyclic Jacobi), its eigenvalues are clamped from below to rel_floor * lambda_max and
+ * the block is inverted; a block with lambda_max <= 0 (a vertex no tet references, or one with only negative curvature)
+ * becomes the zero block, so that vertex does not move.  inv_out_dev (optional, device float32 [n][6]) receives the
+ * inverse blocks as (xx, yy, zz, yz, xz, xy) per vertex.  No host sync. */
+int tsb_pcg_set_blocks(tsb_pcg_t s, const float *diag_dev, float rel_floor, float *inv_out_dev, void *stream);
+
+enum {
+  TSB_PCG_MAXITER = 0,        /* max_iter products used, residual test not met                         */
+  TSB_PCG_CONVERGED = 1,      /* |r_c| <= rtol |b_c|                                                    */
+  TSB_PCG_NEGCURV = 2,        /* p^T H p <= 0 at a later direction: d_c is the iterate reached before it */
+  TSB_PCG_NEGCURV_FIRST = 3,  /* p^T H p <= 0 at the first direction: d_c = P b_c                        */
+  TSB_PCG_ZERO_RHS = 4        /* |b_c| = 0: d_c = 0                                                      */
+};
+
+typedef struct {
+  int32_t max_iter;         /* >= 1: Hessian-vector products at most                                                 */
+  float rtol;               /* >= 0: a sphere stops at |r_c| <= rtol |b_c|                                           */
+  int32_t check_every;      /* 0: enqueue exactly max_iter iterations, never touch the host (capturable in a CUDA graph;
+                               stopped spheres idle); k > 0: enqueue k iterations at a time, then read one int32, the
+                               number of spheres still active, and stop when it is 0                                  */
+  int32_t reserved[5];
+} tsb_pcg_options_t;
+
+typedef struct {            /* one per component, in the component order of tsb_energy_grad_spheres; 32 bytes        */
+  float rel_residual;       /* |r_c| / |b_c| of the returned d_c from the recurrence's residual (1 at NEGCURV_FIRST,
+                               0 at ZERO_RHS)                                                                         */
+  float b_dot_d;            /* b_c . d_c: with b = -grad, minus the directional derivative of a per-sphere Armijo test */
+  float d_H_d;              /* sum of alpha^2 p^T H p = d_c^T H d_c up to CG rounding; 0 if no step was accumulated   */
+  int32_t n_hvp;            /* products in which this component was still active                                      */
+  int32_t status;           /* TSB_PCG_*                                                                              */
+  int32_t first_vertex;     /* its lowest vertex id                                                                   */
+  int32_t n_vertices;
+  int32_t reserved;
+} tsb_pcg_sphere_t;
+
+/* Solves H(x) d = b on every component, H exactly what tsb_hvp_ex multiplies by with *terms (c3 != 0 needs a handle
+ * created with enable_amips = 1).  x_dev, b_dev: device float32 [3n]; d_out_dev: device float32 [3n], fully overwritten
+ * (zero on vertices no tet references); spheres_out_dev: optional device array [info.n_components]; iters_run_out:
+ * optional host int32, the iterations enqueued.  Per component c, independently: r = b_c, z = P r, p = z; each
+ * iteration forms alpha = r.z / p^T H p, stops at p^T H p <= 0 (returning the iterate so far, or P b_c at the first
+ * direction), else d += alpha p, r -= alpha H p, stops at |r| <= rtol |b_c|, else z = P r, p = z + beta p.  A stopped
+ * component's p is 0, so later products leave it untouched and its d_c is final.
+ * Per iteration the stream sees the launches of tsb_hvp_ex on p (the gather follows on deterministic handles) and
+ * three small kernels over the chunk table.  Dot products are accumulated in fp64 in a fixed order and there are no
+ * floating-point atomics, so on a deterministic handle d and the records are bitwise identical across calls, streams
+ * and CUDA-graph replays, and a component's result does not depend on the other components' right-hand sides.  (On a
+ * default handle the products add active tets' contributions with red.global.add.f32, as tsb_hvp_ex does.)
+ * Chains with every other call of the handle on one stream.
+ * Argument errors (TSB_E_INVALID, nothing launched): a null x_dev, b_dev, d_out_dev, terms or opt, max_iter < 1,
+ * rtol < 0 or NaN, check_every < 0, check_every > 0 on a stream that is being captured, an order other than 2 or 4,
+ * terms->c3 != 0 on a handle without enable_amips. */
+int tsb_pcg_solve(tsb_pcg_t s, const float *x_dev, const float *b_dev, const tsb_terms_t *terms,
+                  const tsb_pcg_options_t *opt, float *d_out_dev, tsb_pcg_sphere_t *spheres_out_dev,
+                  int32_t *iters_run_out, void *stream);
+
+/* Per-sphere step: out_v = x_v + a[component of v] * d_v, vertices no tet references copied.  a_sphere_dev: device
+ * float32 [info.n_components]; out_dev may alias x_dev.  One launch, no host sync. */
+int tsb_sphere_axpy(tsb_pcg_t s, const float *x_dev, const float *a_sphere_dev, const float *d_dev, float *out_dev,
+                    void *stream);
 
 /* Same computation for callers whose vertex positions live in HOST memory (e.g. a CPU-side
  * optimiser): copies x_host -> device, runs the fused launch, copies energy[3] and grad back,

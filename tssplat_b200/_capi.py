@@ -15,11 +15,13 @@ LIB_PATH = os.environ.get("TSSPLAT_B200_LIB") or _build.LIB_PATH
 
 TSB_OK, TSB_E_INVALID, TSB_E_MESH, TSB_E_CUDA, TSB_E_NOMEM = 0, -1, -2, -3, -4
 TSB_LINE_MAX_ALPHA = 8
+TSB_PCG_MAXITER, TSB_PCG_CONVERGED, TSB_PCG_NEGCURV, TSB_PCG_NEGCURV_FIRST, TSB_PCG_ZERO_RHS = 0, 1, 2, 3, 4
 
 # every symbol include/tssplat_b200.h declares (tests check the library exports each one)
 EXPORTED_SYMBOLS = (
     "tsb_create", "tsb_destroy", "tsb_last_error", "tsb_get_info", "tsb_energy_grad", "tsb_energy_grad_ex", "tsb_energy_grad_spheres", "tsb_hvp", "tsb_hvp_ex",
-    "tsb_line_search", "tsb_hess_diag", "tsb_energy_grad_host", "tsb_scale",
+    "tsb_line_search", "tsb_hess_diag", "tsb_pcg_create", "tsb_pcg_destroy", "tsb_pcg_last_error", "tsb_pcg_device_bytes",
+    "tsb_pcg_set_blocks", "tsb_pcg_solve", "tsb_sphere_axpy", "tsb_energy_grad_host", "tsb_scale",
     "tsb_grad_limit", "tsb_adam_uniform_step",
     "tsb_surface_create", "tsb_surface_destroy", "tsb_surface_last_error", "tsb_surface_forward", "tsb_surface_backward",
     "tsb_surface_extract", "tsb_free_host", "tsb_setup_last_error",
@@ -39,6 +41,15 @@ class tsb_terms_t(C.Structure):
 class tsb_sphere_stats_t(C.Structure):
     _fields_ = [("smooth", C.c_double), ("barrier", C.c_double), ("amips", C.c_double), ("min_J", C.c_float),
                 ("n_inverted", C.c_int32), ("n_tets", C.c_int32), ("first_vertex", C.c_int32)]
+
+
+class tsb_pcg_options_t(C.Structure):
+    _fields_ = [("max_iter", C.c_int32), ("rtol", C.c_float), ("check_every", C.c_int32), ("reserved", C.c_int32 * 5)]
+
+
+class tsb_pcg_sphere_t(C.Structure):
+    _fields_ = [("rel_residual", C.c_float), ("b_dot_d", C.c_float), ("d_H_d", C.c_float), ("n_hvp", C.c_int32),
+                ("status", C.c_int32), ("first_vertex", C.c_int32), ("n_vertices", C.c_int32), ("reserved", C.c_int32)]
 
 
 class tsb_info_t(C.Structure):
@@ -83,6 +94,21 @@ def _load() -> C.CDLL:
     lib.tsb_line_search.argtypes = [vp, vp, vp, C.POINTER(tsb_terms_t), vp, i32, vp, vp, vp, vp, vp]
     lib.tsb_hess_diag.restype = C.c_int
     lib.tsb_hess_diag.argtypes = [vp, vp, C.POINTER(tsb_terms_t), f32, vp, vp, vp]
+    lib.tsb_pcg_create.restype = C.c_int
+    lib.tsb_pcg_create.argtypes = [vp, C.POINTER(vp)]
+    lib.tsb_pcg_destroy.restype = None
+    lib.tsb_pcg_destroy.argtypes = [vp]
+    lib.tsb_pcg_last_error.restype = C.c_char_p
+    lib.tsb_pcg_last_error.argtypes = [vp]
+    lib.tsb_pcg_device_bytes.restype = i64
+    lib.tsb_pcg_device_bytes.argtypes = [vp]
+    lib.tsb_pcg_set_blocks.restype = C.c_int
+    lib.tsb_pcg_set_blocks.argtypes = [vp, vp, f32, vp, vp]
+    lib.tsb_pcg_solve.restype = C.c_int
+    lib.tsb_pcg_solve.argtypes = [vp, vp, vp, C.POINTER(tsb_terms_t), C.POINTER(tsb_pcg_options_t), vp, vp,
+                                  C.POINTER(C.c_int32), vp]
+    lib.tsb_sphere_axpy.restype = C.c_int
+    lib.tsb_sphere_axpy.argtypes = [vp, vp, vp, vp, vp, vp]
     lib.tsb_energy_grad_host.restype = C.c_int
     lib.tsb_energy_grad_host.argtypes = [vp, vp, f32, f32, i32, f32, vp, vp, vp]
     lib.tsb_scale.restype = C.c_int

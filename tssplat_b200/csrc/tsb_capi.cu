@@ -9,8 +9,10 @@
 #include "../../include/tssplat_b200.h"
 #include "tsb_kernels.cuh"
 #include "tsb_plan.h"
+#include "tsb_solver.cuh"
 
 static_assert(sizeof(tsb_sphere_stats_t) == 40, "tsb_sphere_stats_t must be 40 bytes");
+static_assert(sizeof(tsb_pcg_sphere_t) == 32, "tsb_pcg_sphere_t must be 32 bytes");
 
 struct tsb_handle_s {
   int device = 0;
@@ -29,6 +31,17 @@ struct tsb_handle_s {
   tsb::DetParams dp{};
   tsb::SphParams sp{};          // per-sphere statistics: the fold's tables (records: kp.sph_rec)
   tsb_info_t info{};
+  std::vector<int32_t> comp_label;   // host only: component of every vertex (-1: no tet), for tsb_pcg_create
+  std::vector<void *> allocs;
+  std::string err;
+};
+
+struct tsb_pcg_s {
+  tsb_handle_t h = nullptr;
+  tsb::PcgParams P{};
+  int64_t device_bytes = 0;
+  int32_t *active_host = nullptr;    // pinned: the "components still active" count of check_every > 0
+  cudaEvent_t ev = nullptr;
   std::vector<void *> allocs;
   std::string err;
 };
@@ -91,6 +104,28 @@ int alloc_zero(tsb_handle_t h, size_t elems, T **out) {
   h->info.device_bytes += int64_t(bytes);
   e = cudaMemset(d, 0, bytes);
   if (e != cudaSuccess) return fail(h, TSB_E_CUDA, std::string("cudaMemset: ") + cudaGetErrorString(e));
+  *out = static_cast<T *>(d);
+  return TSB_OK;
+}
+
+// the same for a solver workspace (tsb_pcg_t)
+thread_local std::string g_pcg_create_err;
+
+int pcg_fail(tsb_pcg_t s, int code, const std::string &msg) {
+  if (s) s->err = msg; else g_pcg_create_err = msg;
+  return code;
+}
+
+template <class T>
+int pcg_alloc(tsb_pcg_t s, size_t elems, const T *src, T **out) {
+  const size_t bytes = elems * sizeof(T);
+  void *d = nullptr;
+  cudaError_t e = cudaMalloc(&d, bytes);
+  if (e != cudaSuccess) return pcg_fail(s, TSB_E_NOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e));
+  s->allocs.push_back(d);
+  s->device_bytes += int64_t(bytes);
+  e = src ? cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice) : cudaMemset(d, 0, bytes);
+  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("workspace initialisation: ") + cudaGetErrorString(e));
   *out = static_cast<T *>(d);
   return TSB_OK;
 }
@@ -227,6 +262,7 @@ int tsb_create(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t ne
   h->lc = tsb::LaunchConfig{nw, plan.grid, smem, plan.mode_global, 0, 0, 0};
   h->amips = pc.enable_amips != 0;
   h->det = pc.deterministic != 0;
+  h->comp_label = std::move(plan.comp_label);
 
   tsb_info_t &I = h->info;
   I.n = plan.n; I.nele = plan.nele; I.n_components = plan.n_components; I.grid = plan.grid;
@@ -419,6 +455,133 @@ int tsb_hess_diag(tsb_handle_t h, const float *x_dev, const tsb_terms_t *terms, 
       if (e != cudaSuccess) return fail(h, TSB_E_CUDA, std::string("deterministic gather launch: ") + cudaGetErrorString(e));
     }
   }
+  return TSB_OK;
+}
+
+/* ---- Newton-CG solve (tsb_solver.cu) ---- */
+
+int tsb_pcg_create(tsb_handle_t h, tsb_pcg_t *out) {
+  if (!out) return pcg_fail(nullptr, TSB_E_INVALID, "out is null");
+  *out = nullptr;
+  if (!h) return pcg_fail(nullptr, TSB_E_INVALID, "handle is null");
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return pcg_fail(nullptr, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  tsb::PcgLists L;
+  tsb::build_pcg_lists(h->comp_label, h->info.n_components, L);
+  tsb_pcg_t s = new tsb_pcg_s();
+  s->h = h;
+  tsb::PcgParams &P = s->P;
+  const size_t n = size_t(h->info.n), n3 = 3 * n;
+  int32_t *vert = nullptr, *comp_chunk = nullptr, *chunk = nullptr;
+  int rc = TSB_OK;
+#define TSB_TRY(expr) do { rc = (expr); if (rc != TSB_OK) { g_pcg_create_err = s->err; tsb_pcg_destroy(s); return rc; } } while (0)
+  TSB_TRY(pcg_alloc(s, L.vert.size(), L.vert.data(), &vert));
+  TSB_TRY(pcg_alloc(s, L.comp_chunk.size(), L.comp_chunk.data(), &comp_chunk));
+  TSB_TRY(pcg_alloc(s, L.chunk.size(), L.chunk.data(), &chunk));
+  TSB_TRY(pcg_alloc<float>(s, n3, nullptr, &P.r));
+  TSB_TRY(pcg_alloc<float>(s, n3, nullptr, &P.z));
+  TSB_TRY(pcg_alloc<float>(s, n3, nullptr, &P.p));     // zero on vertices no tet references, and stays so
+  TSB_TRY(pcg_alloc<float>(s, n3, nullptr, &P.Hp));
+  TSB_TRY(pcg_alloc<float>(s, 2 * n3, nullptr, &P.pinv));
+  TSB_TRY(pcg_alloc<double>(s, 3 * (L.chunk.size() / 3), nullptr, &P.part));
+  TSB_TRY(pcg_alloc<tsb::PcgComp>(s, size_t(h->info.n_components), nullptr, &P.comp));
+  TSB_TRY(pcg_alloc<int32_t>(s, 1, nullptr, &P.active));
+#undef TSB_TRY
+  P.vert = vert; P.comp_chunk = comp_chunk; P.chunk = chunk;
+  P.orphans = h->kp.orphans; P.n_orphans = h->kp.n_orphans;
+  P.n_chunks = int32_t(L.chunk.size() / 3); P.n_components = h->info.n_components; P.n = h->info.n;
+  cudaError_t e = cudaMallocHost(reinterpret_cast<void **>(&s->active_host), sizeof(int32_t));
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->ev, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = tsb::launch_pcg_blocks(P, nullptr, 0.f, nullptr, nullptr);     // identity preconditioner
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) {
+    pcg_fail(nullptr, TSB_E_CUDA, std::string("tsb_pcg_create: ") + cudaGetErrorString(e));
+    tsb_pcg_destroy(s);
+    return TSB_E_CUDA;
+  }
+  *out = s;
+  return TSB_OK;
+}
+
+void tsb_pcg_destroy(tsb_pcg_t s) {
+  if (!s) return;
+  DeviceGuard guard(s->h->device);
+  if (s->ev) cudaEventDestroy(s->ev);
+  if (s->active_host) cudaFreeHost(s->active_host);
+  for (void *p : s->allocs) cudaFree(p);
+  delete s;
+}
+
+const char *tsb_pcg_last_error(tsb_pcg_t s) { return s ? s->err.c_str() : g_pcg_create_err.c_str(); }
+
+int64_t tsb_pcg_device_bytes(tsb_pcg_t s) { return s ? s->device_bytes : 0; }
+
+int tsb_pcg_set_blocks(tsb_pcg_t s, const float *diag_dev, float rel_floor, float *inv_out_dev, void *stream) {
+  if (!s) return TSB_E_INVALID;
+  if (!(rel_floor >= 0.f)) return pcg_fail(s, TSB_E_INVALID, "rel_floor must be >= 0");
+  DeviceGuard guard(s->h->device);
+  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  const cudaError_t e = tsb::launch_pcg_blocks(s->P, diag_dev, rel_floor, inv_out_dev, static_cast<cudaStream_t>(stream));
+  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("preconditioner launch: ") + cudaGetErrorString(e));
+  return TSB_OK;
+}
+
+int tsb_pcg_solve(tsb_pcg_t s, const float *x_dev, const float *b_dev, const tsb_terms_t *terms, const tsb_pcg_options_t *opt,
+                  float *d_out_dev, tsb_pcg_sphere_t *spheres_out_dev, int32_t *iters_run_out, void *stream) {
+  if (!s) return TSB_E_INVALID;
+  if (!x_dev || !b_dev || !d_out_dev || !terms || !opt)
+    return pcg_fail(s, TSB_E_INVALID, "x_dev, b_dev, d_out_dev, terms and opt must be non-null");
+  if (opt->max_iter < 1) return pcg_fail(s, TSB_E_INVALID, "max_iter must be >= 1");
+  if (!(opt->rtol >= 0.f)) return pcg_fail(s, TSB_E_INVALID, "rtol must be >= 0");
+  if (opt->check_every < 0) return pcg_fail(s, TSB_E_INVALID, "check_every must be >= 0");
+  if (terms->order != 2 && terms->order != 4) return pcg_fail(s, TSB_E_INVALID, "order must be 2 or 4");
+  if (terms->c3 != 0.f && !s->h->amips)
+    return pcg_fail(s, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
+  DeviceGuard guard(s->h->device);
+  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (opt->check_every > 0) {          // the termination check waits on the host: not possible inside a stream capture
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    if (cudaStreamIsCapturing(st, &cap) != cudaSuccess) { cudaGetLastError(); return pcg_fail(s, TSB_E_CUDA, "cannot query the stream"); }
+    if (cap != cudaStreamCaptureStatusNone)
+      return pcg_fail(s, TSB_E_INVALID, "check_every > 0 reads the host and cannot be captured in a CUDA graph: use check_every = 0");
+  }
+  const tsb::PcgParams &P = s->P;
+  cudaError_t e = tsb::launch_pcg_begin(P, b_dev, d_out_dev, st);
+  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver launch: ") + cudaGetErrorString(e));
+  int32_t it = 0;
+  while (it < opt->max_iter) {
+    const int rc = hvp_impl(s->h, x_dev, P.p, terms->c1, terms->c2, terms->c3, terms->order, 1.f, nullptr, P.Hp, nullptr, 1, st);
+    if (rc != TSB_OK) return pcg_fail(s, rc, s->h->err);
+    e = tsb::launch_pcg_step(P, d_out_dev, it, opt->rtol, st);
+    if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver launch: ") + cudaGetErrorString(e));
+    ++it;
+    if (opt->check_every > 0 && it % opt->check_every == 0 && it < opt->max_iter) {
+      e = tsb::launch_pcg_count(P, st);
+      if (e == cudaSuccess) e = cudaMemcpyAsync(s->active_host, P.active, sizeof(int32_t), cudaMemcpyDeviceToHost, st);
+      if (e == cudaSuccess) e = cudaEventRecord(s->ev, st);
+      if (e == cudaSuccess) e = cudaEventSynchronize(s->ev);
+      if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver termination check: ") + cudaGetErrorString(e));
+      if (*s->active_host == 0) break;
+    }
+  }
+  if (iters_run_out) *iters_run_out = it;
+  if (spheres_out_dev) {
+    e = tsb::launch_pcg_records(P, b_dev, d_out_dev, spheres_out_dev, st);
+    if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver record launch: ") + cudaGetErrorString(e));
+  }
+  return TSB_OK;
+}
+
+int tsb_sphere_axpy(tsb_pcg_t s, const float *x_dev, const float *a_sphere_dev, const float *d_dev, float *out_dev,
+                    void *stream) {
+  if (!s) return TSB_E_INVALID;
+  if (!x_dev || !a_sphere_dev || !d_dev || !out_dev)
+    return pcg_fail(s, TSB_E_INVALID, "x_dev, a_sphere_dev, d_dev and out_dev must be non-null");
+  DeviceGuard guard(s->h->device);
+  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  const cudaError_t e = tsb::launch_sphere_axpy(s->P, x_dev, a_sphere_dev, d_dev, out_dev, static_cast<cudaStream_t>(stream));
+  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("sphere axpy launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 

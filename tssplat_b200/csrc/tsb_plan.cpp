@@ -640,10 +640,12 @@ std::vector<Comp> find_components(Mesh &M, HostPlan &P) {
   }
   std::vector<Comp> comps;
   std::vector<int32_t> label(M.n, -1);
+  P.comp_label.assign(size_t(M.n), -1);
   for (int v = 0; v < M.n; ++v) {
     if (!used[v]) { P.orphans.push_back(v); continue; }
     const int r = uf.find(v);
     if (label[r] < 0) { label[r] = int32_t(comps.size()); comps.emplace_back(); }
+    P.comp_label[v] = label[r];
     Comp &C = comps[label[r]];
     M.local_of[v] = int32_t(C.verts.size());
     C.verts.push_back(v);
@@ -1104,6 +1106,27 @@ int det_lists(const std::vector<Comp> &comps, const std::vector<std::vector<int3
 }
 
 }  // namespace
+
+void build_pcg_lists(const std::vector<int32_t> &comp_label, int32_t n_components, PcgLists &out) {
+  out.comp_off.assign(size_t(n_components) + 1, 0);
+  for (const int32_t c : comp_label)
+    if (c >= 0) ++out.comp_off[size_t(c) + 1];
+  for (int32_t c = 0; c < n_components; ++c) out.comp_off[size_t(c) + 1] += out.comp_off[c];
+  out.vert.assign(size_t(out.comp_off[n_components]), 0);
+  std::vector<int32_t> cur(out.comp_off.begin(), out.comp_off.end() - 1);
+  for (size_t v = 0; v < comp_label.size(); ++v)      // ascending v: every component's list comes out sorted
+    if (comp_label[v] >= 0) out.vert[size_t(cur[comp_label[v]]++)] = int32_t(v);
+  out.chunk.clear();
+  out.comp_chunk.assign(size_t(n_components) + 1, 0);
+  for (int32_t c = 0; c < n_components; ++c) {
+    for (int32_t b = out.comp_off[c]; b < out.comp_off[c + 1]; b += kPcgChunkVerts) {
+      out.chunk.push_back(c);
+      out.chunk.push_back(b);
+      out.chunk.push_back(std::min(b + kPcgChunkVerts, out.comp_off[c + 1]));
+    }
+    out.comp_chunk[size_t(c) + 1] = int32_t(out.chunk.size() / 3);
+  }
+}
 
 int build_plan(const float *rest, const int32_t *tets, int32_t n, int32_t nele, const PlanConfig &cfg,
                HostPlan &P, std::string &err) {

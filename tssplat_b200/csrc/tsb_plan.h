@@ -134,6 +134,7 @@ struct HostPlan {
   std::vector<int32_t> comp_seg;          // [n_components + 1]
   std::vector<int32_t> comp_first_vertex; // [n_components] lowest vertex id (components are numbered by it)
   std::vector<int32_t> comp_ntets;        // [n_components]
+  std::vector<int32_t> comp_label;        // [n] component of every vertex, -1 = no tet references it (host only)
   // AMIPS only: rest inverses B = Dm^-1 of every streamed tet (in its streamed vertex order), one block of
   // 3 rows x (tets per cell) float4 per tet cell, and the first tet cell of every (segment, warp)
   std::vector<float> Bt;
@@ -147,6 +148,19 @@ struct HostPlan {
   std::vector<int32_t> det_comp_row;   // [n_components + 1] first row of every component
   std::vector<int32_t> det_chunk;   // [2 * chunks] (component, first row) of every run of <= kDetChunkRows rows
 };
+
+// The Newton-CG solver's view of the components (tsb_pcg_create): vert lists the non-orphan vertices grouped by
+// component (components in order, vertices ascending), comp_off[c] is the first entry of component c, chunk holds
+// (component, begin, end) for every run of <= kPcgChunkVerts entries of one component, components in order, and
+// comp_chunk[c] is the first chunk of component c.
+constexpr int kPcgChunkVerts = 256;
+struct PcgLists {
+  std::vector<int32_t> vert;        // [non-orphan vertices]
+  std::vector<int32_t> comp_off;    // [n_components + 1]
+  std::vector<int32_t> chunk;       // [3 * chunks]
+  std::vector<int32_t> comp_chunk;  // [n_components + 1]
+};
+void build_pcg_lists(const std::vector<int32_t> &comp_label, int32_t n_components, PcgLists &out);
 
 // Returns 0 on success, TSB_E_* otherwise (message in err).
 int build_plan(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele,

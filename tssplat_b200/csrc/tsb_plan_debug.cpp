@@ -9,7 +9,7 @@
 #include "../../include/tssplat_b200.h"
 #include "tsb_plan.h"
 
-struct tsbdbg_plan { tsb::HostPlan plan; };
+struct tsbdbg_plan { tsb::HostPlan plan; tsb::PcgLists pcg; };
 static thread_local std::string g_err;
 
 extern "C" {
@@ -35,6 +35,7 @@ int tsbdbg_build_det(const float *rest_xyz, const int32_t *tets, int32_t n, int3
   tsbdbg_plan *d = new tsbdbg_plan();
   const int rc = tsb::build_plan(rest_xyz, tets, n, nele, pc, d->plan, g_err);
   if (rc != TSB_OK) { delete d; return rc; }
+  tsb::build_pcg_lists(d->plan.comp_label, d->plan.n_components, d->pcg);   // what tsb_pcg_create uploads
   *out = d;
   return TSB_OK;
 }
@@ -60,6 +61,8 @@ int tsbdbg_array(tsbdbg_plan *d, const char *name, const void **ptr, int64_t *co
   ARR("det_rowptr", P.det_rowptr, 4) ARR("det_vert", P.det_vert, 4) ARR("det_ent", P.det_ent, 4)
   ARR("det_comp_row", P.det_comp_row, 4) ARR("det_chunk", P.det_chunk, 4)
   ARR("comp_seg", P.comp_seg, 4) ARR("comp_first_vertex", P.comp_first_vertex, 4) ARR("comp_ntets", P.comp_ntets, 4)
+  ARR("comp_label", P.comp_label, 4) ARR("pcg_vert", d->pcg.vert, 4) ARR("pcg_comp_off", d->pcg.comp_off, 4)
+  ARR("pcg_chunk", d->pcg.chunk, 4) ARR("pcg_comp_chunk", d->pcg.comp_chunk, 4)
 #undef ARR
   return TSB_E_INVALID;
 }

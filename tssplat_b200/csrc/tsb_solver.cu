@@ -1,0 +1,333 @@
+// Per-component (per tet-sphere) block-Jacobi preconditioned truncated CG on the device: the small kernels that run
+// between two Hessian-vector products of tsb_pcg_solve (include/tssplat_b200.h; DESIGN.md section 5, "Newton-CG solve").
+//
+// Spheres share no vertices, so H is block diagonal by component and CG runs independently on every block, all blocks
+// in the same launches.  A CTA owns one chunk: <= kPcgChunkVerts consecutive entries of one component's vertex list
+// (thread = vertex).  A dot product over a component is two steps: every chunk stores its fp64 partial (a shuffle tree
+// and a fixed-order sum over the CTA's warps), and in the next kernel every chunk of the component folds the
+// component's partials itself, in chunk order, from a column of the partial table that no CTA of that kernel writes.
+// The fold is redundant across the chunks of a component, but it needs no ticket, no atomic and no fence, and every
+// chunk gets bitwise the same scalar.  All scalars stay in device memory.
+#include "tsb_solver.cuh"
+
+namespace tsb {
+namespace {
+
+constexpr int kT = kPcgChunkVerts;   // threads per CTA
+
+// Sum of v over the CTA in a fixed order; the result is valid in thread 0.
+__device__ __forceinline__ double block_sum(double v, double *sh) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, o);
+  __syncthreads();                                  // sh may still be read from the previous sum
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double s = 0.0;
+  if (threadIdx.x == 0)
+#pragma unroll
+    for (int w = 0; w < kT / 32; ++w) s += sh[w];
+  return s;
+}
+
+// The partial table has three columns per chunk, each with one writing kernel per iteration and read only by the kernel
+// after it, so no launch folds a column it also writes: kPHp (pcg_curv_kernel -> pcg_update_kernel; pcg_bdotd_kernel ->
+// pcg_record_kernel), kRz and kRr (pcg_init_kernel / pcg_update_kernel -> pcg_dir_kernel).
+constexpr int kPartCols = 3, kPHp = 0, kRz = 1, kRr = 2;
+
+// Sum of one column of the partials of chunks [c0, c1) in a fixed order, valid in every thread: lane l of warp 0 adds
+// chunks c0 + l, c0 + l + 32, ..., a shuffle tree combines the lanes.
+__device__ __forceinline__ double fold(const double *part, int col, int c0, int c1, double *sh) {
+  if (threadIdx.x < 32) {
+    double a = 0.0;
+    for (int k = c0 + int(threadIdx.x); k < c1; k += 32) a += part[kPartCols * size_t(k) + col];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xFFFFFFFFu, a, o);
+    if (threadIdx.x == 0) sh[0] = a;
+  }
+  __syncthreads();
+  const double out = sh[0];
+  __syncthreads();                                  // sh is reused by the next fold and by block_sum
+  return out;
+}
+
+struct F3 { float x, y, z; };
+__device__ __forceinline__ F3 ld3(const float *a, int v) { return F3{a[3 * size_t(v)], a[3 * size_t(v) + 1], a[3 * size_t(v) + 2]}; }
+__device__ __forceinline__ void st3(float *a, int v, F3 q) { a[3 * size_t(v)] = q.x; a[3 * size_t(v) + 1] = q.y; a[3 * size_t(v) + 2] = q.z; }
+__device__ __forceinline__ double dot3(F3 a, F3 b) { return double(a.x) * double(b.x) + double(a.y) * double(b.y) + double(a.z) * double(b.z); }
+// z = P r with the symmetric block stored as xx yy zz yz xz xy
+__device__ __forceinline__ F3 apply_block(const float *pinv, int v, F3 r) {
+  const float *q = pinv + 6 * size_t(v);
+  const float xx = q[0], yy = q[1], zz = q[2], yz = q[3], xz = q[4], xy = q[5];
+  return F3{xx * r.x + xy * r.y + xz * r.z, xy * r.x + yy * r.y + yz * r.z, xz * r.x + yz * r.y + zz * r.z};
+}
+
+// One Jacobi rotation of a symmetric 3x3 matrix that zeroes a_pq; r is the third index, (v?p, v?q) are columns p and q
+// of the eigenvector matrix.
+__device__ __forceinline__ void jacobi_rot(double &app, double &aqq, double &apq, double &apr, double &aqr, double &v0p,
+                                           double &v0q, double &v1p, double &v1q, double &v2p, double &v2q) {
+  if (apq == 0.0) return;
+  const double theta = (aqq - app) / (2.0 * apq);
+  const double t = copysign(1.0, theta) / (fabs(theta) + sqrt(theta * theta + 1.0));
+  const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+  app -= t * apq; aqq += t * apq; apq = 0.0;
+  double a = c * apr - s * aqr; aqr = s * apr + c * aqr; apr = a;
+  a = c * v0p - s * v0q; v0q = s * v0p + c * v0q; v0p = a;
+  a = c * v1p - s * v1q; v1q = s * v1p + c * v1q; v1p = a;
+  a = c * v2p - s * v2q; v2q = s * v2p + c * v2q; v2p = a;
+}
+
+constexpr int kJacobiSweeps = 8;
+
+// Inverse preconditioner block of every vertex (thread = vertex): cyclic Jacobi eigen-decomposition in fp64 registers,
+// eigenvalues clamped from below to rel_floor * lambda_max, block inverted; lambda_max <= 0 gives the zero block.
+// diag == nullptr: the identity.
+__global__ void __launch_bounds__(kT) pcg_blocks_kernel(const float *__restrict__ diag, int n, float rel_floor,
+                                                        float *__restrict__ pinv, float *__restrict__ inv_out) {
+  const int v = blockIdx.x * kT + int(threadIdx.x);
+  if (v >= n) return;
+  float o[6] = {1.f, 1.f, 1.f, 0.f, 0.f, 0.f};
+  if (diag) {
+    const float *d0 = diag + 3 * size_t(v), *d1 = diag + 3 * (size_t(n) + size_t(v));
+    double a00 = d0[0], a11 = d0[1], a22 = d0[2], a12 = d1[0], a02 = d1[1], a01 = d1[2];
+    double v00 = 1, v01 = 0, v02 = 0, v10 = 0, v11 = 1, v12 = 0, v20 = 0, v21 = 0, v22 = 1;
+#pragma unroll 1
+    for (int sweep = 0; sweep < kJacobiSweeps; ++sweep) {
+      if (a01 == 0.0 && a02 == 0.0 && a12 == 0.0) break;
+      jacobi_rot(a00, a11, a01, a02, a12, v00, v01, v10, v11, v20, v21);
+      jacobi_rot(a00, a22, a02, a01, a12, v00, v02, v10, v12, v20, v22);
+      jacobi_rot(a11, a22, a12, a01, a02, v01, v02, v11, v12, v21, v22);
+    }
+    const double lmax = fmax(a00, fmax(a11, a22));
+    if (lmax > 0.0) {
+      const double fl = double(rel_floor) * lmax;
+      const double i0 = 1.0 / fmax(a00, fl), i1 = 1.0 / fmax(a11, fl), i2 = 1.0 / fmax(a22, fl);
+      o[0] = float(i0 * v00 * v00 + i1 * v01 * v01 + i2 * v02 * v02);
+      o[1] = float(i0 * v10 * v10 + i1 * v11 * v11 + i2 * v12 * v12);
+      o[2] = float(i0 * v20 * v20 + i1 * v21 * v21 + i2 * v22 * v22);
+      o[3] = float(i0 * v10 * v20 + i1 * v11 * v21 + i2 * v12 * v22);
+      o[4] = float(i0 * v00 * v20 + i1 * v01 * v21 + i2 * v02 * v22);
+      o[5] = float(i0 * v00 * v10 + i1 * v01 * v11 + i2 * v02 * v12);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 6; ++k) o[k] = 0.f;
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 6; ++k) {
+    pinv[6 * size_t(v) + k] = o[k];
+    if (inv_out) inv_out[6 * size_t(v) + k] = o[k];
+  }
+}
+
+// r = b, z = P r, d = 0, partials of r.z and r.r.  CTAs past the chunk table zero d on the orphan vertices.
+__global__ void __launch_bounds__(kT) pcg_init_kernel(const PcgParams s, const float *__restrict__ b, float *__restrict__ d) {
+  __shared__ double sh[kT / 32];
+  if (int(blockIdx.x) >= s.n_chunks) {
+    const int k = (int(blockIdx.x) - s.n_chunks) * kT + int(threadIdx.x);
+    if (k < s.n_orphans) st3(d, s.orphans[k], F3{0.f, 0.f, 0.f});
+    return;
+  }
+  const int begin = s.chunk[3 * blockIdx.x + 1], end = s.chunk[3 * blockIdx.x + 2];
+  const int e = begin + int(threadIdx.x);
+  double rz = 0.0, rr = 0.0;
+  if (e < end) {
+    const int v = s.vert[e];
+    const F3 r = ld3(b, v), z = apply_block(s.pinv, v, r);
+    st3(s.r, v, r); st3(s.z, v, z); st3(d, v, F3{0.f, 0.f, 0.f});
+    rz = dot3(r, z); rr = dot3(r, r);
+  }
+  rz = block_sum(rz, sh);
+  rr = block_sum(rr, sh);
+  if (threadIdx.x == 0) { s.part[kPartCols * size_t(blockIdx.x) + kRz] = rz; s.part[kPartCols * size_t(blockIdx.x) + kRr] = rr; }
+}
+
+// Partial of p.Hp of every chunk of an active component.
+__global__ void __launch_bounds__(kT) pcg_curv_kernel(const PcgParams s) {
+  __shared__ double sh[kT / 32];
+  const int c = s.chunk[3 * blockIdx.x];
+  if (s.comp[c].st_dir != kPcgActive) return;
+  const int begin = s.chunk[3 * blockIdx.x + 1], end = s.chunk[3 * blockIdx.x + 2];
+  const int e = begin + int(threadIdx.x);
+  double q = 0.0;
+  if (e < end) { const int v = s.vert[e]; q = dot3(ld3(s.p, v), ld3(s.Hp, v)); }
+  q = block_sum(q, sh);
+  if (threadIdx.x == 0) s.part[kPartCols * size_t(blockIdx.x) + kPHp] = q;
+}
+
+// alpha = r.z / p.Hp per component; p.Hp <= 0 stops the component (at the first direction d = z = P b), otherwise
+// d += alpha p, r -= alpha Hp, z = P r and the partials of the new r.z and r.r.
+__global__ void __launch_bounds__(kT) pcg_update_kernel(const PcgParams s, float *__restrict__ d, int iter) {
+  __shared__ double sh[kT / 32];
+  const int c = s.chunk[3 * blockIdx.x];
+  const bool lead = int(blockIdx.x) == s.comp_chunk[c] && threadIdx.x == 0;
+  PcgComp &C = s.comp[c];
+  const int st = C.st_dir;
+  if (st != kPcgActive) {
+    if (lead) { C.st_upd = st; C.idle = 1; }
+    return;
+  }
+  const double pHp = fold(s.part, kPHp, s.comp_chunk[c], s.comp_chunk[c + 1], sh);
+  const double rz = C.rz;
+  const int begin = s.chunk[3 * blockIdx.x + 1], end = s.chunk[3 * blockIdx.x + 2];
+  const int e = begin + int(threadIdx.x);
+  if (!(pHp > 0.0)) {
+    if (iter == 0 && e < end) { const int v = s.vert[e]; st3(d, v, ld3(s.z, v)); }
+    if (lead) { C.st_upd = iter == 0 ? TSB_PCG_NEGCURV_FIRST : TSB_PCG_NEGCURV; C.idle = 0; C.n_hvp = iter + 1; }
+    return;
+  }
+  const double alpha = rz / pHp;
+  const float a = float(alpha);
+  double nrz = 0.0, nrr = 0.0;
+  if (e < end) {
+    const int v = s.vert[e];
+    const F3 p = ld3(s.p, v), hp = ld3(s.Hp, v);
+    F3 x = ld3(d, v), r = ld3(s.r, v);
+    x.x += a * p.x; x.y += a * p.y; x.z += a * p.z;
+    r.x -= a * hp.x; r.y -= a * hp.y; r.z -= a * hp.z;
+    const F3 z = apply_block(s.pinv, v, r);
+    st3(d, v, x); st3(s.r, v, r); st3(s.z, v, z);
+    nrz = dot3(r, z); nrr = dot3(r, r);
+  }
+  nrz = block_sum(nrz, sh);
+  nrr = block_sum(nrr, sh);
+  if (threadIdx.x == 0) { s.part[kPartCols * size_t(blockIdx.x) + kRz] = nrz; s.part[kPartCols * size_t(blockIdx.x) + kRr] = nrr; }
+  if (lead) { C.st_upd = kPcgActive; C.idle = 0; C.n_hvp = iter + 1; C.rz_prev = rz; C.dHd += alpha * alpha * pHp; }
+}
+
+// Folds r.z and r.r, tests convergence and sets the next direction p = z + beta p; a stopped component gets p = 0, so
+// later products leave it untouched.  FIRST: the direction of iteration 0 (p = z), which also initialises the state.
+template <bool FIRST>
+__global__ void __launch_bounds__(kT) pcg_dir_kernel(const PcgParams s, float rtol) {
+  __shared__ double sh[kT / 32];
+  const int c = s.chunk[3 * blockIdx.x];
+  const bool lead = int(blockIdx.x) == s.comp_chunk[c] && threadIdx.x == 0;
+  PcgComp &C = s.comp[c];
+  if (!FIRST && C.idle) return;
+  int st = FIRST ? kPcgActive : C.st_upd;
+  float beta = 0.f;
+  if (st == kPcgActive) {
+    const double2 f = make_double2(fold(s.part, kRz, s.comp_chunk[c], s.comp_chunk[c + 1], sh),
+                                   fold(s.part, kRr, s.comp_chunk[c], s.comp_chunk[c + 1], sh));   // (r.z, r.r)
+    if (FIRST) {
+      if (f.y == 0.0) st = TSB_PCG_ZERO_RHS;
+      if (lead) { C.rz = f.x; C.rz_prev = f.x; C.bb = f.y; C.rr = f.y; C.dHd = 0.0; C.st_upd = st; C.idle = 0; C.n_hvp = 0; }
+    } else {
+      if (sqrt(f.y) <= double(rtol) * sqrt(C.bb)) st = TSB_PCG_CONVERGED;
+      beta = float(f.x / C.rz_prev);
+      if (lead) { C.rz = f.x; C.rr = f.y; }
+    }
+  }
+  if (lead) C.st_dir = st;
+  const int begin = s.chunk[3 * blockIdx.x + 1], end = s.chunk[3 * blockIdx.x + 2];
+  const int e = begin + int(threadIdx.x);
+  if (e < end) {
+    const int v = s.vert[e];
+    F3 p{0.f, 0.f, 0.f};
+    if (st == kPcgActive) {
+      p = ld3(s.z, v);
+      if (!FIRST) { const F3 q = ld3(s.p, v); p.x += beta * q.x; p.y += beta * q.y; p.z += beta * q.z; }
+    }
+    st3(s.p, v, p);
+  }
+}
+
+// Components still active, for the host's termination test every check_every iterations.
+__global__ void __launch_bounds__(kT) pcg_count_kernel(const PcgParams s) {
+  __shared__ int cnt;
+  if (threadIdx.x == 0) cnt = 0;
+  __syncthreads();
+  int k = 0;
+  for (int c = int(threadIdx.x); c < s.n_components; c += kT) k += s.comp[c].st_dir == kPcgActive;
+  if (k) atomicAdd(&cnt, k);
+  __syncthreads();
+  if (threadIdx.x == 0) *s.active = cnt;
+}
+
+// Partial of b.d of every chunk.
+__global__ void __launch_bounds__(kT) pcg_bdotd_kernel(const PcgParams s, const float *__restrict__ b, const float *__restrict__ d) {
+  __shared__ double sh[kT / 32];
+  const int begin = s.chunk[3 * blockIdx.x + 1], end = s.chunk[3 * blockIdx.x + 2];
+  const int e = begin + int(threadIdx.x);
+  double q = 0.0;
+  if (e < end) { const int v = s.vert[e]; q = dot3(ld3(b, v), ld3(d, v)); }
+  q = block_sum(q, sh);
+  if (threadIdx.x == 0) s.part[kPartCols * size_t(blockIdx.x) + kPHp] = q;
+}
+
+// One tsb_pcg_sphere_t per component (thread = component).
+__global__ void __launch_bounds__(kT) pcg_record_kernel(const PcgParams s, tsb_pcg_sphere_t *__restrict__ out) {
+  const int c = blockIdx.x * kT + int(threadIdx.x);
+  if (c >= s.n_components) return;
+  const PcgComp C = s.comp[c];
+  const int k0 = s.comp_chunk[c], k1 = s.comp_chunk[c + 1];
+  double bd = 0.0;
+  for (int k = k0; k < k1; ++k) bd += s.part[kPartCols * size_t(k) + kPHp];
+  tsb_pcg_sphere_t o;
+  o.status = C.st_dir == kPcgActive ? TSB_PCG_MAXITER : C.st_dir;
+  o.rel_residual = o.status == TSB_PCG_ZERO_RHS ? 0.f : o.status == TSB_PCG_NEGCURV_FIRST ? 1.f : float(sqrt(C.rr / C.bb));
+  o.b_dot_d = float(bd);
+  o.d_H_d = float(C.dHd);
+  o.n_hvp = C.n_hvp;
+  o.first_vertex = s.vert[s.chunk[3 * size_t(k0) + 1]];
+  o.n_vertices = s.chunk[3 * size_t(k1 - 1) + 2] - s.chunk[3 * size_t(k0) + 1];
+  o.reserved = 0;
+  out[c] = o;
+}
+
+// out = x + a[component] d; CTAs past the chunk table copy the orphan vertices.  out may alias x.
+__global__ void __launch_bounds__(kT) sphere_axpy_kernel(const PcgParams s, const float *x, const float *__restrict__ a,
+                                                         const float *__restrict__ d, float *out) {
+  if (int(blockIdx.x) >= s.n_chunks) {
+    const int k = (int(blockIdx.x) - s.n_chunks) * kT + int(threadIdx.x);
+    if (k < s.n_orphans) { const int v = s.orphans[k]; st3(out, v, ld3(x, v)); }
+    return;
+  }
+  const int e = s.chunk[3 * blockIdx.x + 1] + int(threadIdx.x);
+  if (e >= s.chunk[3 * blockIdx.x + 2]) return;
+  const int v = s.vert[e];
+  const float al = a[s.chunk[3 * blockIdx.x]];
+  const F3 q = ld3(d, v);
+  F3 y = ld3(x, v);
+  y.x += al * q.x; y.y += al * q.y; y.z += al * q.z;
+  st3(out, v, y);
+}
+
+unsigned with_orphans(const PcgParams &s) { return unsigned(s.n_chunks + (s.n_orphans + kT - 1) / kT); }
+
+}  // namespace
+
+cudaError_t launch_pcg_blocks(const PcgParams &s, const float *diag, float rel_floor, float *inv_out, cudaStream_t st) {
+  pcg_blocks_kernel<<<unsigned((s.n + kT - 1) / kT), kT, 0, st>>>(diag, s.n, rel_floor, s.pinv, inv_out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_pcg_begin(const PcgParams &s, const float *b, float *d, cudaStream_t st) {
+  pcg_init_kernel<<<with_orphans(s), kT, 0, st>>>(s, b, d);
+  pcg_dir_kernel<true><<<unsigned(s.n_chunks), kT, 0, st>>>(s, 0.f);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, cudaStream_t st) {
+  pcg_curv_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s);
+  pcg_update_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, d, iter);
+  pcg_dir_kernel<false><<<unsigned(s.n_chunks), kT, 0, st>>>(s, rtol);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_pcg_count(const PcgParams &s, cudaStream_t st) {
+  pcg_count_kernel<<<1, kT, 0, st>>>(s);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_pcg_records(const PcgParams &s, const float *b, const float *d, tsb_pcg_sphere_t *out, cudaStream_t st) {
+  pcg_bdotd_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, b, d);
+  pcg_record_kernel<<<unsigned((s.n_components + kT - 1) / kT), kT, 0, st>>>(s, out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_sphere_axpy(const PcgParams &s, const float *x, const float *a, const float *d, float *out, cudaStream_t st) {
+  sphere_axpy_kernel<<<with_orphans(s), kT, 0, st>>>(s, x, a, d, out);
+  return cudaGetLastError();
+}
+
+}  // namespace tsb

@@ -208,6 +208,25 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         c1, c2 = self.coeff_scheduler(it)
         return self.tet_sp.hess_diag(x.detach(), c1, c2, self.order_at(it), c3=self.amips_coeff)
 
+    def newton_direction(self, x, it, b=None, **solve_kw):
+        """A Newton direction per sphere, on the device without a host sync: ``hess_diag`` -> block-Jacobi preconditioner
+        -> ``tssplat_b200.newton.DevicePCG.solve`` of ``H(x) d = b`` with the scheduler's coefficients, the barrier order
+        at ``it`` and ``amips_coeff``.  ``b=None`` takes ``b = -grad`` from one gradient launch.  ``solve_kw``:
+        ``max_iter``, ``rtol``, ``check_every``.  Returns a ``DevicePCGResult`` (its ``b_dot_d`` is what a per-sphere
+        Armijo test needs); the workspace, ``self.device_pcg`` (its ``axpy`` takes the per-sphere step), is created on
+        first use."""
+        from .newton import DevicePCG
+        pcg = getattr(self, "device_pcg", None)
+        if pcg is None:
+            pcg = self.device_pcg = DevicePCG(self.tet_sp)
+        c1, c2 = self.coeff_scheduler(it)
+        order, xd = self.order_at(it), x.detach()
+        if b is None:
+            _, g = self.tet_sp.energy_grad(xd, c1, c2, order, -1.0, c3=self.amips_coeff)
+            b = g.reshape(x.shape)
+        pcg.set_blocks(self.tet_sp.hess_diag(xd, c1, c2, order, c3=self.amips_coeff))
+        return pcg.solve(xd, b.detach(), c1, c2, order, c3=self.amips_coeff, **solve_kw)
+
     def forward(self, x, it, c1, c2):
         order = self.order_at(it)
         if self.amips_coeff > 0:

@@ -5,14 +5,19 @@
 Hessian-vector product (``TetSpheres.hvp``), stopping at negative curvature.  Plain torch on the planes' device; the
 Hessian itself is only ever touched through the CUDA library's launches.  INTEGRATION.md shows one Newton step built
 from these and ``TetSpheres.line_search``.
+
+``DevicePCG`` is the device-resident solver (``tsb_pcg_solve``): the same truncated PCG, but run independently on every
+tet-sphere (the Hessian is block diagonal by sphere) with all scalars in device memory, so there is no host read inside
+an iteration and the solve can be captured in a CUDA graph.  ``pcg`` below stays as the reference implementation.
 """
 from __future__ import annotations
 
+import ctypes as C
 from typing import Callable, NamedTuple, Optional, Union
 
 import torch
 
-__all__ = ["hess_blocks", "block_jacobi", "apply_blocks", "pcg", "PCGResult"]
+__all__ = ["hess_blocks", "block_jacobi", "apply_blocks", "pcg", "PCGResult", "DevicePCG", "DevicePCGResult"]
 
 
 def hess_blocks(planes: torch.Tensor) -> torch.Tensor:
@@ -101,3 +106,103 @@ def pcg(hvp_fn: Callable[[torch.Tensor], torch.Tensor], b: torch.Tensor,
         p = z + (rz_new / rz) * p
         rz = rz_new
     return PCGResult(x, n, False, False, float(r.double().norm()) / bnorm)
+
+
+class DevicePCGResult(NamedTuple):
+    """What ``DevicePCG.solve`` returns: device tensors, S = number of spheres in the order of their lowest vertex ids
+    (``tsb_pcg_sphere_t`` in ``include/tssplat_b200.h``)."""
+    d: torch.Tensor                 # f32 [n, 3]: the step of every sphere; 0 on vertices no tet references
+    status: torch.Tensor            # i32 [S]: 0 max_iter, 1 converged, 2 negative curvature, 3 the same at the first
+                                    # direction (d_c = P b_c), 4 zero right-hand side
+    n_hvp: torch.Tensor             # i32 [S]: products in which the sphere was still active
+    rel_residual: torch.Tensor      # f32 [S]: |r_c| / |b_c| of the returned step
+    b_dot_d: torch.Tensor           # f32 [S]: b_c . d_c
+    d_H_d: torch.Tensor             # f32 [S]: d_c^T H d_c as accumulated by CG
+    iters_run: int                  # iterations enqueued (= max_iter with check_every = 0)
+
+
+class DevicePCG:
+    """Per-sphere block-Jacobi PCG workspace of one ``TetSpheres`` handle (``tsb_pcg_create``), which it keeps alive.
+    Serves one stream at a time, like the handle."""
+
+    def __init__(self, tet_sp):
+        from . import _capi
+        from .tet_spheres_ext import _stream_ptr
+        self._capi, self._stream_ptr = _capi, _stream_ptr
+        self._s = None
+        self.tet_sp = tet_sp
+        s = C.c_void_p()
+        rc = _capi.lib.tsb_pcg_create(tet_sp._h, C.byref(s))
+        if rc:
+            raise RuntimeError(f"DevicePCG: {self._error(None)} (code {rc})")
+        self._s = s
+        self.n_spheres = int(tet_sp.info["n_components"])
+        self.device_bytes = int(_capi.lib.tsb_pcg_device_bytes(s))
+
+    def __del__(self):
+        s, self._s = getattr(self, "_s", None), None
+        if s:
+            try:
+                self._capi.lib.tsb_pcg_destroy(s)
+            except Exception:  # interpreter shutdown
+                pass
+
+    def _error(self, s) -> str:
+        msg = self._capi.lib.tsb_pcg_last_error(s)
+        return msg.decode("utf-8", "replace") if msg else ""
+
+    def _check(self, rc: int, what: str) -> None:
+        if rc:
+            raise RuntimeError(f"DevicePCG.{what}: {self._error(self._s)} (code {rc})")
+
+    def _f32(self, t: torch.Tensor, numel: int, name: str) -> torch.Tensor:
+        if (not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or t.device != self.tet_sp.device
+                or t.numel() != numel):
+            raise RuntimeError(f"{name} must be a float32 tensor of {numel} entries on {self.tet_sp.device}")
+        return t if t.is_contiguous() else t.contiguous()
+
+    def set_blocks(self, planes: Optional[torch.Tensor] = None, rel_floor: float = 1e-6,
+                   want_inverse: bool = False) -> Optional[torch.Tensor]:
+        """Preconditioner from the [2, n, 3] planes of ``hess_diag`` with ``block_jacobi``'s semantics, computed on the
+        device (``tsb_pcg_set_blocks``); ``None`` is the identity.  ``want_inverse`` returns the inverse blocks as
+        [n, 6] = (xx, yy, zz, yz, xz, xy)."""
+        n = self.tet_sp.n
+        pc = None if planes is None else self._f32(planes, 6 * n, "planes")
+        inv = torch.empty((n, 6), dtype=torch.float32, device=self.tet_sp.device) if want_inverse else None
+        rc = self._capi.lib.tsb_pcg_set_blocks(self._s, pc.data_ptr() if pc is not None else None, float(rel_floor),
+                                               inv.data_ptr() if want_inverse else None, self._stream_ptr(self.tet_sp.device))
+        self._check(rc, "set_blocks")
+        return inv
+
+    def solve(self, x: torch.Tensor, b: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0,
+              max_iter: int = 100, rtol: float = 1e-3, check_every: int = 0) -> DevicePCGResult:
+        """``H(x) d = b`` on every sphere by truncated PCG (``tsb_pcg_solve``), ``H`` the Hessian ``TetSpheres.hvp``
+        multiplies by.  ``check_every = 0`` enqueues ``max_iter`` iterations without touching the host (and can be
+        captured in a CUDA graph); ``k > 0`` reads the number of active spheres every ``k`` iterations and stops
+        early."""
+        n3, dev = self.tet_sp.n3, self.tet_sp.device
+        xc, bc = self._f32(x, n3, "x"), self._f32(b, n3, "b")
+        d = torch.empty((self.tet_sp.n, 3), dtype=torch.float32, device=dev)
+        raw = torch.empty((self.n_spheres, 8), dtype=torch.int32, device=dev)
+        terms = self._capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
+        opt = self._capi.tsb_pcg_options_t(max_iter=int(max_iter), rtol=float(rtol), check_every=int(check_every))
+        iters = C.c_int32(0)
+        rc = self._capi.lib.tsb_pcg_solve(self._s, xc.data_ptr(), bc.data_ptr(), C.byref(terms), C.byref(opt), d.data_ptr(),
+                                          raw.data_ptr(), C.byref(iters), self._stream_ptr(dev))
+        self._check(rc, "solve")
+        f = raw.view(torch.float32)
+        return DevicePCGResult(d, raw[:, 4], raw[:, 3], f[:, 0], f[:, 1], f[:, 2], int(iters.value))
+
+    def axpy(self, x: torch.Tensor, a_sphere: torch.Tensor, d: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``x + a_sphere[sphere of v] * d`` per vertex (``tsb_sphere_axpy``), in ``x``'s shape; vertices no tet
+        references are copied.  ``out`` may be ``x`` (in place)."""
+        n3 = self.tet_sp.n3
+        xc, dc, ac = self._f32(x, n3, "x"), self._f32(d, n3, "d"), self._f32(a_sphere, self.n_spheres, "a_sphere")
+        if out is None:
+            out = torch.empty_like(xc)
+        elif self._f32(out, n3, "out") is not out:
+            raise RuntimeError("out must be contiguous")
+        rc = self._capi.lib.tsb_sphere_axpy(self._s, xc.data_ptr(), ac.data_ptr(), dc.data_ptr(), out.data_ptr(),
+                                            self._stream_ptr(self.tet_sp.device))
+        self._check(rc, "axpy")
+        return out
