@@ -20,7 +20,7 @@
 extern "C" {
 #endif
 
-#define TSB_VERSION 7
+#define TSB_VERSION 8
 #define TSB_LINE_MAX_ALPHA 8   /* step sizes one tsb_line_search call may evaluate */
 
 enum {
@@ -317,6 +317,101 @@ int tsb_pcg_solve(tsb_pcg_t s, const float *x_dev, const float *b_dev, const tsb
  * float32 [info.n_components]; out_dev may alias x_dev.  One launch, no host sync. */
 int tsb_sphere_axpy(tsb_pcg_t s, const float *x_dev, const float *a_sphere_dev, const float *d_dev, float *out_dev,
                     void *stream);
+
+/* ---- Damped (Levenberg-Marquardt) solve: H + mu_c I per sphere --------------------------------------------------
+ * shift_dev: device float32 [info.n_components], mu_c >= 0 per component in component order, read on the device (a
+ * captured graph can be replayed with new shifts).  With shift_dev == NULL both calls are exactly tsb_pcg_set_blocks and
+ * tsb_pcg_solve.
+ *
+ * tsb_pcg_set_blocks_ex: every vertex of component c gets the block D_v + mu_c I before the eigen-clamp-invert of
+ * tsb_pcg_set_blocks (vertices no tet references keep the zero block; diag_dev == NULL gives the identity, unshifted).
+ * One launch over the component chunk table.
+ *
+ * tsb_pcg_solve_ex: solves (H(x) + mu_c I) d = b_c on every component with tsb_pcg_solve's algorithm, rules and records.
+ * The shift enters as p.(Hp + mu p) in the curvature and r -= alpha (Hp + mu p) in the residual update, both in fp32
+ * with the same rounding; the Hessian-vector product launches are tsb_pcg_solve's.  H + mu_c I is positive definite
+ * once mu_c exceeds minus the smallest eigenvalue of the component's H, and the solve then converges where the unshifted
+ * one stops at negative curvature.  In the records d_H_d is d^T (H + mu_c I) d. */
+int tsb_pcg_set_blocks_ex(tsb_pcg_t s, const float *diag_dev, float rel_floor, const float *shift_dev, float *inv_out_dev,
+                          void *stream);
+int tsb_pcg_solve_ex(tsb_pcg_t s, const float *x_dev, const float *b_dev, const tsb_terms_t *terms,
+                     const tsb_pcg_options_t *opt, const float *shift_dev, float *d_out_dev,
+                     tsb_pcg_sphere_t *spheres_out_dev, int32_t *iters_run_out, void *stream);
+
+/* ---- Damped Newton step: one Levenberg-Marquardt iteration per sphere on the device (no counterpart in the reference)
+ * A Newton workspace sits beside a solver workspace (which must outlive it; creating one changes nothing about the
+ * handle or the solver workspace) and holds b, d and the two diagonal planes (12 floats per vertex), the per-sphere line
+ * search outputs, the step-size table alpha_k = 2^-k (k < TSB_LINE_MAX_ALPHA), the per-sphere state (mu, nu, status,
+ * whether mu is initialised), three fp64 partials per chunk and the per-sphere step sizes.  Device memory, reported by
+ * tsb_newton_device_bytes:
+ *   48 n + 24 chunks + 172 n_components + 176   bytes
+ * (chunks as for tsb_pcg_device_bytes).  A new workspace is reset (every sphere ACTIVE, mu not initialised).  Like the
+ * handle and the solver workspace it serves one stream at a time, and it shares the solver workspace's scratch. */
+typedef struct tsb_newton_s *tsb_newton_t;
+int tsb_newton_create(tsb_pcg_t s, tsb_newton_t *out);
+void tsb_newton_destroy(tsb_newton_t nw);
+const char *tsb_newton_last_error(tsb_newton_t nw);   /* nw may be NULL: last tsb_newton_create failure */
+int64_t tsb_newton_device_bytes(tsb_newton_t nw);
+
+/* Marks every sphere ACTIVE with mu not initialised (one memset on the stream; capturable). */
+int tsb_newton_reset(tsb_newton_t nw, void *stream);
+
+enum {
+  TSB_NEWTON_ACTIVE = 0,      /* still iterating                                                             */
+  TSB_NEWTON_CONVERGED = 1,   /* |grad_c| <= gtol: frozen                                                     */
+  TSB_NEWTON_STALLED = 2      /* no acceptable step with mu_c at mu_max: frozen                                */
+};
+
+typedef struct {            /* 64 bytes */
+  int32_t max_iter;         /* >= 1: the damped solve enqueues exactly max_iter iterations (check_every = 0)        */
+  float rtol;               /* >= 0: the solve's residual test                                                       */
+  float rel_floor;          /* >= 0: the preconditioner's eigenvalue floor (tsb_pcg_set_blocks)                      */
+  float tau;                /* > 0: initial mu_c = tau * max over the sphere's vertices of the diagonal entries D_ii  */
+  float mu_min, mu_max;     /* 0 < mu_min <= mu_max, finite: bounds on mu_c                                          */
+  float gtol;               /* >= 0: a sphere with |grad_c| <= gtol is CONVERGED                                     */
+  float sigma;              /* in (0, 1): Armijo constant (1e-4 is the usual choice)                                 */
+  float eta;                /* in (0, 1]: a step must lie below eta times the sphere's inversion-free step (0.9)      */
+  int32_t n_alpha;          /* 1..TSB_LINE_MAX_ALPHA: step sizes 1, 1/2, ..., 2^-(n_alpha - 1)                       */
+  int32_t reserved[6];      /* must be 0                                                                             */
+} tsb_newton_options_t;
+
+typedef struct {            /* one per component, component order of tsb_energy_grad_spheres; 64 bytes               */
+  double mu;                /* mu_c after this step's update                                                         */
+  double rho;               /* gain ratio of the full step, -dE_c(1) / pred (1 when pred <= 0); 0 when no decision ran */
+  float grad_norm;          /* |grad_c| at x before the step (0 on a sphere already frozen: its right-hand side is 0) */
+  float alpha;              /* the step taken (0: none)                                                              */
+  float delta;              /* E_c(x + alpha d) - E_c(x) from the line search (0 if no step)                          */
+  float b_dot_d;            /* b_c . d_c, b = -grad                                                                   */
+  int32_t k;                /* index of the step size taken, -1 when none                                            */
+  int32_t pcg_status;       /* TSB_PCG_* of the damped solve                                                         */
+  int32_t n_hvp;            /* products in which the sphere was active in the solve                                  */
+  int32_t status;           /* TSB_NEWTON_* after the step                                                           */
+  int32_t first_vertex;     /* its lowest vertex id                                                                  */
+  int32_t reserved[3];
+} tsb_newton_sphere_t;
+
+/* One damped Newton iteration on every sphere; x_dev (device float32 [3n]) is updated in place.  c1, c2, order, c3 from
+ * *terms with tsb_hvp_ex's rules.  On one stream, without any host read (capturable in a CUDA graph), in this order:
+ *   1. b = -grad E(x) (one gradient launch, gradH = -1); b_c = 0 on spheres already frozen, so their solve is ZERO_RHS;
+ *   2. tsb_hess_diag;  3. on a sphere's first step, mu_c = tau * max_v max_i (D_v)_ii clamped to [mu_min, mu_max];
+ *   4. tsb_pcg_set_blocks_ex and tsb_pcg_solve_ex with shift mu_c (fp32);  5. per sphere b.d and |d|^2 (fp64, fixed order);
+ *   6. tsb_line_search at alpha_k = 2^-k, k < n_alpha, per sphere;  7. the decision below;  8. tsb_sphere_axpy in place.
+ * Decision per sphere c, with g = |b_c| (from the solve's fp64 |b_c|^2), bd and dHd the solve's b.d and d^T (H + mu I) d
+ * rounded to fp32 as tsb_pcg_sphere_t reports them, dd = |d_c|^2, dE_k = E_c(x + alpha_k d) - E_c(x) and alpha^ the
+ * sphere's inversion-free step over (0, 1] (both from the line search):
+ *   frozen: alpha = 0.  g <= gtol: CONVERGED, frozen, alpha = 0.
+ *   k* = the smallest k with alpha_k < eta alpha^ and dE_k <= -sigma alpha_k bd; none (or bd <= 0): alpha = 0, k = -1.
+ *   pred = bd - (dHd - mu' dd) / 2, mu' = the fp32 shift the solve used;  rho = -dE_0 / pred if pred > 0, else 1.
+ *   k* = 0: mu = max(mu_min, mu max(1/3, 1 - (2 rho - 1)^3)), nu = 2;  otherwise mu = min(mu_max, mu nu), nu = 2 nu.
+ *   no step and mu = mu_max: STALLED, frozen.      (mu, nu and rho in fp64)
+ * records_out_dev (optional, device [info.n_components]) receives one tsb_newton_sphere_t per sphere.  No floating-point
+ * atomics in the new kernels and every fold in a fixed order: on a deterministic handle x and the records are bitwise
+ * identical across calls, streams and graph replays, and a sphere's trajectory does not depend on the other spheres.
+ * Vertices no tet references never move.  Argument errors (TSB_E_INVALID, nothing launched): a null nw, x_dev, terms or
+ * opt, an option outside its range above (NaN included), nonzero reserved words, an order other than 2 or 4,
+ * terms->c3 != 0 on a handle without enable_amips.  DESIGN.md section 5, "Damped Newton step". */
+int tsb_newton_step(tsb_newton_t nw, float *x_dev, const tsb_terms_t *terms, const tsb_newton_options_t *opt,
+                    tsb_newton_sphere_t *records_out_dev, void *stream);
 
 /* Same computation for callers whose vertex positions live in HOST memory (e.g. a CPU-side
  * optimiser): copies x_host -> device, runs the fused launch, copies energy[3] and grad back,

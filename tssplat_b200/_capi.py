@@ -16,12 +16,15 @@ LIB_PATH = os.environ.get("TSSPLAT_B200_LIB") or _build.LIB_PATH
 TSB_OK, TSB_E_INVALID, TSB_E_MESH, TSB_E_CUDA, TSB_E_NOMEM = 0, -1, -2, -3, -4
 TSB_LINE_MAX_ALPHA = 8
 TSB_PCG_MAXITER, TSB_PCG_CONVERGED, TSB_PCG_NEGCURV, TSB_PCG_NEGCURV_FIRST, TSB_PCG_ZERO_RHS = 0, 1, 2, 3, 4
+TSB_NEWTON_ACTIVE, TSB_NEWTON_CONVERGED, TSB_NEWTON_STALLED = 0, 1, 2
 
 # every symbol include/tssplat_b200.h declares (tests check the library exports each one)
 EXPORTED_SYMBOLS = (
     "tsb_create", "tsb_destroy", "tsb_last_error", "tsb_get_info", "tsb_energy_grad", "tsb_energy_grad_ex", "tsb_energy_grad_spheres", "tsb_hvp", "tsb_hvp_ex",
     "tsb_line_search", "tsb_hess_diag", "tsb_pcg_create", "tsb_pcg_destroy", "tsb_pcg_last_error", "tsb_pcg_device_bytes",
-    "tsb_pcg_set_blocks", "tsb_pcg_solve", "tsb_sphere_axpy", "tsb_energy_grad_host", "tsb_scale",
+    "tsb_pcg_set_blocks", "tsb_pcg_solve", "tsb_sphere_axpy", "tsb_pcg_set_blocks_ex", "tsb_pcg_solve_ex",
+    "tsb_newton_create", "tsb_newton_destroy", "tsb_newton_last_error", "tsb_newton_device_bytes", "tsb_newton_reset",
+    "tsb_newton_step", "tsb_energy_grad_host", "tsb_scale",
     "tsb_grad_limit", "tsb_adam_uniform_step",
     "tsb_surface_create", "tsb_surface_destroy", "tsb_surface_last_error", "tsb_surface_forward", "tsb_surface_backward",
     "tsb_surface_extract", "tsb_free_host", "tsb_setup_last_error",
@@ -50,6 +53,18 @@ class tsb_pcg_options_t(C.Structure):
 class tsb_pcg_sphere_t(C.Structure):
     _fields_ = [("rel_residual", C.c_float), ("b_dot_d", C.c_float), ("d_H_d", C.c_float), ("n_hvp", C.c_int32),
                 ("status", C.c_int32), ("first_vertex", C.c_int32), ("n_vertices", C.c_int32), ("reserved", C.c_int32)]
+
+
+class tsb_newton_options_t(C.Structure):
+    _fields_ = [("max_iter", C.c_int32), ("rtol", C.c_float), ("rel_floor", C.c_float), ("tau", C.c_float),
+                ("mu_min", C.c_float), ("mu_max", C.c_float), ("gtol", C.c_float), ("sigma", C.c_float), ("eta", C.c_float),
+                ("n_alpha", C.c_int32), ("reserved", C.c_int32 * 6)]
+
+
+class tsb_newton_sphere_t(C.Structure):
+    _fields_ = [("mu", C.c_double), ("rho", C.c_double), ("grad_norm", C.c_float), ("alpha", C.c_float), ("delta", C.c_float),
+                ("b_dot_d", C.c_float), ("k", C.c_int32), ("pcg_status", C.c_int32), ("n_hvp", C.c_int32),
+                ("status", C.c_int32), ("first_vertex", C.c_int32), ("reserved", C.c_int32 * 3)]
 
 
 class tsb_info_t(C.Structure):
@@ -109,6 +124,23 @@ def _load() -> C.CDLL:
                                   C.POINTER(C.c_int32), vp]
     lib.tsb_sphere_axpy.restype = C.c_int
     lib.tsb_sphere_axpy.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.tsb_pcg_set_blocks_ex.restype = C.c_int
+    lib.tsb_pcg_set_blocks_ex.argtypes = [vp, vp, f32, vp, vp, vp]
+    lib.tsb_pcg_solve_ex.restype = C.c_int
+    lib.tsb_pcg_solve_ex.argtypes = [vp, vp, vp, C.POINTER(tsb_terms_t), C.POINTER(tsb_pcg_options_t), vp, vp, vp,
+                                     C.POINTER(C.c_int32), vp]
+    lib.tsb_newton_create.restype = C.c_int
+    lib.tsb_newton_create.argtypes = [vp, C.POINTER(vp)]
+    lib.tsb_newton_destroy.restype = None
+    lib.tsb_newton_destroy.argtypes = [vp]
+    lib.tsb_newton_last_error.restype = C.c_char_p
+    lib.tsb_newton_last_error.argtypes = [vp]
+    lib.tsb_newton_device_bytes.restype = i64
+    lib.tsb_newton_device_bytes.argtypes = [vp]
+    lib.tsb_newton_reset.restype = C.c_int
+    lib.tsb_newton_reset.argtypes = [vp, vp]
+    lib.tsb_newton_step.restype = C.c_int
+    lib.tsb_newton_step.argtypes = [vp, vp, C.POINTER(tsb_terms_t), C.POINTER(tsb_newton_options_t), vp, vp]
     lib.tsb_energy_grad_host.restype = C.c_int
     lib.tsb_energy_grad_host.argtypes = [vp, vp, f32, f32, i32, f32, vp, vp, vp]
     lib.tsb_scale.restype = C.c_int

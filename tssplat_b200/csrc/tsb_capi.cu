@@ -1,6 +1,7 @@
 // C ABI (include/tssplat_b200.h) over the plan builder and the sm_90a kernels.
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <string>
@@ -13,6 +14,8 @@
 
 static_assert(sizeof(tsb_sphere_stats_t) == 40, "tsb_sphere_stats_t must be 40 bytes");
 static_assert(sizeof(tsb_pcg_sphere_t) == 32, "tsb_pcg_sphere_t must be 32 bytes");
+static_assert(sizeof(tsb_newton_options_t) == 64, "tsb_newton_options_t must be 64 bytes");
+static_assert(sizeof(tsb_newton_sphere_t) == 64, "tsb_newton_sphere_t must be 64 bytes");
 
 struct tsb_handle_s {
   int device = 0;
@@ -38,10 +41,23 @@ struct tsb_handle_s {
 
 struct tsb_pcg_s {
   tsb_handle_t h = nullptr;
+  int device = 0;                    // the handle's device, kept so that destroying never reads the handle
   tsb::PcgParams P{};
   int64_t device_bytes = 0;
   int32_t *active_host = nullptr;    // pinned: the "components still active" count of check_every > 0
   cudaEvent_t ev = nullptr;
+  std::vector<void *> allocs;
+  std::string err;
+};
+
+struct tsb_newton_s {
+  tsb_pcg_t s = nullptr;
+  int device = 0;                    // the handle's device, kept so that destroying never reads the solver workspace
+                                     // (a garbage collector may free the handle and workspaces in any order)
+  tsb::NewtonParams W{};
+  float *energy = nullptr;           // [4] energies of the gradient launch (not reported)
+  float *delta = nullptr;            // [TSB_LINE_MAX_ALPHA][4] the line search's totals (not reported)
+  int64_t device_bytes = 0;
   std::vector<void *> allocs;
   std::string err;
 };
@@ -108,7 +124,7 @@ int alloc_zero(tsb_handle_t h, size_t elems, T **out) {
   return TSB_OK;
 }
 
-// the same for a solver workspace (tsb_pcg_t)
+// the same for a solver workspace (tsb_pcg_t) ...
 thread_local std::string g_pcg_create_err;
 
 int pcg_fail(tsb_pcg_t s, int code, const std::string &msg) {
@@ -116,16 +132,25 @@ int pcg_fail(tsb_pcg_t s, int code, const std::string &msg) {
   return code;
 }
 
-template <class T>
-int pcg_alloc(tsb_pcg_t s, size_t elems, const T *src, T **out) {
+// ... and a Newton workspace (tsb_newton_t)
+thread_local std::string g_newton_create_err;
+
+int newton_fail(tsb_newton_t nw, int code, const std::string &msg) {
+  if (nw) nw->err = msg; else g_newton_create_err = msg;
+  return code;
+}
+
+// Device array of a workspace (tsb_pcg_t or tsb_newton_t): copied from src, or zeroed
+template <class T, class W>
+int ws_alloc(W *s, size_t elems, const T *src, T **out) {
   const size_t bytes = elems * sizeof(T);
   void *d = nullptr;
   cudaError_t e = cudaMalloc(&d, bytes);
-  if (e != cudaSuccess) return pcg_fail(s, TSB_E_NOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) { s->err = std::string("cudaMalloc: ") + cudaGetErrorString(e); return TSB_E_NOMEM; }
   s->allocs.push_back(d);
   s->device_bytes += int64_t(bytes);
   e = src ? cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice) : cudaMemset(d, 0, bytes);
-  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("workspace initialisation: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) { s->err = std::string("workspace initialisation: ") + cudaGetErrorString(e); return TSB_E_CUDA; }
   *out = static_cast<T *>(d);
   return TSB_OK;
 }
@@ -470,22 +495,23 @@ int tsb_pcg_create(tsb_handle_t h, tsb_pcg_t *out) {
   tsb::build_pcg_lists(h->comp_label, h->info.n_components, L);
   tsb_pcg_t s = new tsb_pcg_s();
   s->h = h;
+  s->device = h->device;
   tsb::PcgParams &P = s->P;
   const size_t n = size_t(h->info.n), n3 = 3 * n;
   int32_t *vert = nullptr, *comp_chunk = nullptr, *chunk = nullptr;
   int rc = TSB_OK;
 #define TSB_TRY(expr) do { rc = (expr); if (rc != TSB_OK) { g_pcg_create_err = s->err; tsb_pcg_destroy(s); return rc; } } while (0)
-  TSB_TRY(pcg_alloc(s, L.vert.size(), L.vert.data(), &vert));
-  TSB_TRY(pcg_alloc(s, L.comp_chunk.size(), L.comp_chunk.data(), &comp_chunk));
-  TSB_TRY(pcg_alloc(s, L.chunk.size(), L.chunk.data(), &chunk));
-  TSB_TRY(pcg_alloc<float>(s, n3, nullptr, &P.r));
-  TSB_TRY(pcg_alloc<float>(s, n3, nullptr, &P.z));
-  TSB_TRY(pcg_alloc<float>(s, n3, nullptr, &P.p));     // zero on vertices no tet references, and stays so
-  TSB_TRY(pcg_alloc<float>(s, n3, nullptr, &P.Hp));
-  TSB_TRY(pcg_alloc<float>(s, 2 * n3, nullptr, &P.pinv));
-  TSB_TRY(pcg_alloc<double>(s, 3 * (L.chunk.size() / 3), nullptr, &P.part));
-  TSB_TRY(pcg_alloc<tsb::PcgComp>(s, size_t(h->info.n_components), nullptr, &P.comp));
-  TSB_TRY(pcg_alloc<int32_t>(s, 1, nullptr, &P.active));
+  TSB_TRY(ws_alloc(s, L.vert.size(), L.vert.data(), &vert));
+  TSB_TRY(ws_alloc(s, L.comp_chunk.size(), L.comp_chunk.data(), &comp_chunk));
+  TSB_TRY(ws_alloc(s, L.chunk.size(), L.chunk.data(), &chunk));
+  TSB_TRY(ws_alloc<float>(s, n3, nullptr, &P.r));
+  TSB_TRY(ws_alloc<float>(s, n3, nullptr, &P.z));
+  TSB_TRY(ws_alloc<float>(s, n3, nullptr, &P.p));     // zero on vertices no tet references, and stays so
+  TSB_TRY(ws_alloc<float>(s, n3, nullptr, &P.Hp));
+  TSB_TRY(ws_alloc<float>(s, 2 * n3, nullptr, &P.pinv));
+  TSB_TRY(ws_alloc<double>(s, 3 * (L.chunk.size() / 3), nullptr, &P.part));
+  TSB_TRY(ws_alloc<tsb::PcgComp>(s, size_t(h->info.n_components), nullptr, &P.comp));
+  TSB_TRY(ws_alloc<int32_t>(s, 1, nullptr, &P.active));
 #undef TSB_TRY
   P.vert = vert; P.comp_chunk = comp_chunk; P.chunk = chunk;
   P.orphans = h->kp.orphans; P.n_orphans = h->kp.n_orphans;
@@ -505,7 +531,7 @@ int tsb_pcg_create(tsb_handle_t h, tsb_pcg_t *out) {
 
 void tsb_pcg_destroy(tsb_pcg_t s) {
   if (!s) return;
-  DeviceGuard guard(s->h->device);
+  DeviceGuard guard(s->device);
   if (s->ev) cudaEventDestroy(s->ev);
   if (s->active_host) cudaFreeHost(s->active_host);
   for (void *p : s->allocs) cudaFree(p);
@@ -517,17 +543,30 @@ const char *tsb_pcg_last_error(tsb_pcg_t s) { return s ? s->err.c_str() : g_pcg_
 int64_t tsb_pcg_device_bytes(tsb_pcg_t s) { return s ? s->device_bytes : 0; }
 
 int tsb_pcg_set_blocks(tsb_pcg_t s, const float *diag_dev, float rel_floor, float *inv_out_dev, void *stream) {
+  return tsb_pcg_set_blocks_ex(s, diag_dev, rel_floor, nullptr, inv_out_dev, stream);
+}
+
+int tsb_pcg_set_blocks_ex(tsb_pcg_t s, const float *diag_dev, float rel_floor, const float *shift_dev, float *inv_out_dev,
+                          void *stream) {
   if (!s) return TSB_E_INVALID;
   if (!(rel_floor >= 0.f)) return pcg_fail(s, TSB_E_INVALID, "rel_floor must be >= 0");
   DeviceGuard guard(s->h->device);
   if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
-  const cudaError_t e = tsb::launch_pcg_blocks(s->P, diag_dev, rel_floor, inv_out_dev, static_cast<cudaStream_t>(stream));
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const cudaError_t e = diag_dev && shift_dev ? tsb::launch_pcg_blocks_shift(s->P, diag_dev, rel_floor, shift_dev, inv_out_dev, st)
+                                              : tsb::launch_pcg_blocks(s->P, diag_dev, rel_floor, inv_out_dev, st);
   if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("preconditioner launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 
 int tsb_pcg_solve(tsb_pcg_t s, const float *x_dev, const float *b_dev, const tsb_terms_t *terms, const tsb_pcg_options_t *opt,
                   float *d_out_dev, tsb_pcg_sphere_t *spheres_out_dev, int32_t *iters_run_out, void *stream) {
+  return tsb_pcg_solve_ex(s, x_dev, b_dev, terms, opt, nullptr, d_out_dev, spheres_out_dev, iters_run_out, stream);
+}
+
+int tsb_pcg_solve_ex(tsb_pcg_t s, const float *x_dev, const float *b_dev, const tsb_terms_t *terms, const tsb_pcg_options_t *opt,
+                     const float *shift_dev, float *d_out_dev, tsb_pcg_sphere_t *spheres_out_dev, int32_t *iters_run_out,
+                     void *stream) {
   if (!s) return TSB_E_INVALID;
   if (!x_dev || !b_dev || !d_out_dev || !terms || !opt)
     return pcg_fail(s, TSB_E_INVALID, "x_dev, b_dev, d_out_dev, terms and opt must be non-null");
@@ -553,7 +592,7 @@ int tsb_pcg_solve(tsb_pcg_t s, const float *x_dev, const float *b_dev, const tsb
   while (it < opt->max_iter) {
     const int rc = hvp_impl(s->h, x_dev, P.p, terms->c1, terms->c2, terms->c3, terms->order, 1.f, nullptr, P.Hp, nullptr, 1, st);
     if (rc != TSB_OK) return pcg_fail(s, rc, s->h->err);
-    e = tsb::launch_pcg_step(P, d_out_dev, it, opt->rtol, st);
+    e = tsb::launch_pcg_step(P, d_out_dev, it, opt->rtol, shift_dev, st);
     if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver launch: ") + cudaGetErrorString(e));
     ++it;
     if (opt->check_every > 0 && it % opt->check_every == 0 && it < opt->max_iter) {
@@ -582,6 +621,116 @@ int tsb_sphere_axpy(tsb_pcg_t s, const float *x_dev, const float *a_sphere_dev, 
   if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
   const cudaError_t e = tsb::launch_sphere_axpy(s->P, x_dev, a_sphere_dev, d_dev, out_dev, static_cast<cudaStream_t>(stream));
   if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("sphere axpy launch: ") + cudaGetErrorString(e));
+  return TSB_OK;
+}
+
+/* ---- Damped Newton step (tsb_solver.cu) ---- */
+
+int tsb_newton_create(tsb_pcg_t s, tsb_newton_t *out) {
+  if (!out) return newton_fail(nullptr, TSB_E_INVALID, "out is null");
+  *out = nullptr;
+  if (!s) return newton_fail(nullptr, TSB_E_INVALID, "solver workspace is null");
+  DeviceGuard guard(s->h->device);
+  if (!guard.ok) return newton_fail(nullptr, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  tsb_newton_t nw = new tsb_newton_s();
+  nw->s = s;
+  nw->device = s->h->device;
+  tsb::NewtonParams &W = nw->W;
+  const size_t n3 = 3 * size_t(s->P.n), S = size_t(s->P.n_components), K = TSB_LINE_MAX_ALPHA;
+  std::vector<float> alphas(K);
+  for (size_t k = 0; k < K; ++k) alphas[k] = std::ldexp(1.f, -int(k));
+  float *alphas_dev = nullptr;
+  int rc = TSB_OK;
+#define TSB_TRY(expr) do { rc = (expr); if (rc != TSB_OK) { g_newton_create_err = nw->err; tsb_newton_destroy(nw); return rc; } } while (0)
+  TSB_TRY(ws_alloc<float>(nw, n3, nullptr, &W.b));
+  TSB_TRY(ws_alloc<float>(nw, n3, nullptr, &W.d));
+  TSB_TRY(ws_alloc<float>(nw, 2 * n3, nullptr, &W.diag));
+  TSB_TRY(ws_alloc<float>(nw, S, nullptr, &W.shift));
+  TSB_TRY(ws_alloc<float>(nw, S, nullptr, &W.alpha_sphere));
+  TSB_TRY(ws_alloc<float>(nw, K, alphas.data(), &alphas_dev));
+  TSB_TRY(ws_alloc<float>(nw, S * K * 4, nullptr, &W.sphere_delta));
+  TSB_TRY(ws_alloc<float>(nw, S, nullptr, &W.sphere_step));
+  TSB_TRY(ws_alloc<double>(nw, 3 * size_t(s->P.n_chunks), nullptr, &W.part));
+  TSB_TRY(ws_alloc<tsb::NewtonComp>(nw, S, nullptr, &W.comp));     // zero: ACTIVE, mu not initialised
+  TSB_TRY(ws_alloc<float>(nw, 4, nullptr, &nw->energy));
+  TSB_TRY(ws_alloc<float>(nw, K * 4, nullptr, &nw->delta));
+#undef TSB_TRY
+  W.alphas = alphas_dev;
+  *out = nw;
+  return TSB_OK;
+}
+
+void tsb_newton_destroy(tsb_newton_t nw) {
+  if (!nw) return;
+  DeviceGuard guard(nw->device);
+  for (void *p : nw->allocs) cudaFree(p);
+  delete nw;
+}
+
+const char *tsb_newton_last_error(tsb_newton_t nw) { return nw ? nw->err.c_str() : g_newton_create_err.c_str(); }
+
+int64_t tsb_newton_device_bytes(tsb_newton_t nw) { return nw ? nw->device_bytes : 0; }
+
+int tsb_newton_reset(tsb_newton_t nw, void *stream) {
+  if (!nw) return TSB_E_INVALID;
+  DeviceGuard guard(nw->s->h->device);
+  if (!guard.ok) return newton_fail(nw, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  const cudaError_t e = cudaMemsetAsync(nw->W.comp, 0, size_t(nw->s->P.n_components) * sizeof(tsb::NewtonComp),
+                                        static_cast<cudaStream_t>(stream));
+  if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("reset: ") + cudaGetErrorString(e));
+  return TSB_OK;
+}
+
+int tsb_newton_step(tsb_newton_t nw, float *x_dev, const tsb_terms_t *terms, const tsb_newton_options_t *opt,
+                    tsb_newton_sphere_t *records_out_dev, void *stream) {
+  if (!nw) return TSB_E_INVALID;
+  if (!x_dev || !terms || !opt) return newton_fail(nw, TSB_E_INVALID, "x_dev, terms and opt must be non-null");
+  const tsb_newton_options_t &o = *opt;
+  if (o.max_iter < 1) return newton_fail(nw, TSB_E_INVALID, "max_iter must be >= 1");
+  if (!(o.rtol >= 0.f)) return newton_fail(nw, TSB_E_INVALID, "rtol must be >= 0");
+  if (!(o.rel_floor >= 0.f)) return newton_fail(nw, TSB_E_INVALID, "rel_floor must be >= 0");
+  if (!(o.tau > 0.f) || !std::isfinite(o.tau)) return newton_fail(nw, TSB_E_INVALID, "tau must be finite and > 0");
+  if (!(o.mu_min > 0.f) || !(o.mu_min <= o.mu_max) || !std::isfinite(o.mu_max))
+    return newton_fail(nw, TSB_E_INVALID, "mu_min and mu_max must satisfy 0 < mu_min <= mu_max < inf");
+  if (!(o.gtol >= 0.f)) return newton_fail(nw, TSB_E_INVALID, "gtol must be >= 0");
+  if (!(o.sigma > 0.f && o.sigma < 1.f)) return newton_fail(nw, TSB_E_INVALID, "sigma must be in (0, 1)");
+  if (!(o.eta > 0.f && o.eta <= 1.f)) return newton_fail(nw, TSB_E_INVALID, "eta must be in (0, 1]");
+  if (o.n_alpha < 1 || o.n_alpha > TSB_LINE_MAX_ALPHA)
+    return newton_fail(nw, TSB_E_INVALID, "n_alpha must be in [1, " + std::to_string(TSB_LINE_MAX_ALPHA) + "]");
+  for (int32_t r : o.reserved)
+    if (r != 0) return newton_fail(nw, TSB_E_INVALID, "reserved fields must be 0");
+  tsb_pcg_t s = nw->s;
+  tsb_handle_t h = s->h;
+  if (terms->order != 2 && terms->order != 4) return newton_fail(nw, TSB_E_INVALID, "order must be 2 or 4");
+  if (terms->c3 != 0.f && !h->amips)
+    return newton_fail(nw, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return newton_fail(nw, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const tsb::NewtonParams &W = nw->W;
+  const tsb::NewtonRule R{o.tau, o.mu_min, o.mu_max, o.gtol, o.sigma, o.eta, o.n_alpha};
+  const tsb_pcg_options_t po{o.max_iter, o.rtol, 0, {0, 0, 0, 0, 0}};
+  // 1-2: b = -grad, the diagonal blocks
+  int rc = energy_grad_impl(h, x_dev, terms->c1, terms->c2, terms->c3, terms->order, -1.f, nullptr, nw->energy, 1, W.b, nullptr, st);
+  if (rc == TSB_OK) rc = tsb_hess_diag(h, x_dev, terms, 1.f, nullptr, W.diag, st);
+  if (rc != TSB_OK) return newton_fail(nw, rc, h->err);
+  // 3: frozen spheres' b = 0, mu on a first step
+  cudaError_t e = tsb::launch_newton_prep(s->P, W, R, st);
+  if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
+  // 4: the damped solve
+  rc = tsb_pcg_set_blocks_ex(s, W.diag, o.rel_floor, W.shift, nullptr, st);
+  if (rc == TSB_OK) rc = tsb_pcg_solve_ex(s, x_dev, W.b, terms, &po, W.shift, W.d, nullptr, nullptr, st);
+  if (rc != TSB_OK) return newton_fail(nw, rc, s->err);
+  // 5: b.d and |d|^2 per chunk
+  e = tsb::launch_newton_dots(s->P, W, st);
+  if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
+  // 6: line search at 2^-k, per sphere
+  rc = tsb_line_search(h, x_dev, W.d, terms, W.alphas, o.n_alpha, nw->delta, nullptr, W.sphere_delta, W.sphere_step, st);
+  if (rc != TSB_OK) return newton_fail(nw, rc, h->err);
+  // 7-8: decision, step
+  e = tsb::launch_newton_decide(s->P, W, R, records_out_dev, st);
+  if (e == cudaSuccess) e = tsb::launch_sphere_axpy(s->P, x_dev, W.alpha_sphere, W.d, x_dev, st);
+  if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 

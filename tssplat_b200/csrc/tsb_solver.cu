@@ -78,17 +78,17 @@ __device__ __forceinline__ void jacobi_rot(double &app, double &aqq, double &apq
 
 constexpr int kJacobiSweeps = 8;
 
-// Inverse preconditioner block of every vertex (thread = vertex): cyclic Jacobi eigen-decomposition in fp64 registers,
-// eigenvalues clamped from below to rel_floor * lambda_max, block inverted; lambda_max <= 0 gives the zero block.
-// diag == nullptr: the identity.
-__global__ void __launch_bounds__(kT) pcg_blocks_kernel(const float *__restrict__ diag, int n, float rel_floor,
-                                                        float *__restrict__ pinv, float *__restrict__ inv_out) {
-  const int v = blockIdx.x * kT + int(threadIdx.x);
-  if (v >= n) return;
+// Inverse preconditioner block of vertex v: cyclic Jacobi eigen-decomposition in fp64 registers, eigenvalues clamped
+// from below to rel_floor * lambda_max, block inverted; lambda_max <= 0 gives the zero block.  diag == nullptr: the
+// identity.  SHIFT: the block is D_v + mu I.
+template <bool SHIFT>
+__device__ __forceinline__ void block_inverse(const float *__restrict__ diag, int n, int v, float rel_floor, double mu,
+                                              float *__restrict__ pinv, float *__restrict__ inv_out) {
   float o[6] = {1.f, 1.f, 1.f, 0.f, 0.f, 0.f};
   if (diag) {
     const float *d0 = diag + 3 * size_t(v), *d1 = diag + 3 * (size_t(n) + size_t(v));
     double a00 = d0[0], a11 = d0[1], a22 = d0[2], a12 = d1[0], a02 = d1[1], a01 = d1[2];
+    if (SHIFT) { a00 += mu; a11 += mu; a22 += mu; }
     double v00 = 1, v01 = 0, v02 = 0, v10 = 0, v11 = 1, v12 = 0, v20 = 0, v21 = 0, v22 = 1;
 #pragma unroll 1
     for (int sweep = 0; sweep < kJacobiSweeps; ++sweep) {
@@ -119,6 +119,33 @@ __global__ void __launch_bounds__(kT) pcg_blocks_kernel(const float *__restrict_
   }
 }
 
+// Inverse preconditioner block of every vertex (thread = vertex).
+__global__ void __launch_bounds__(kT) pcg_blocks_kernel(const float *__restrict__ diag, int n, float rel_floor,
+                                                        float *__restrict__ pinv, float *__restrict__ inv_out) {
+  const int v = blockIdx.x * kT + int(threadIdx.x);
+  if (v >= n) return;
+  block_inverse<false>(diag, n, v, rel_floor, 0.0, pinv, inv_out);
+}
+
+// The same with the blocks D_v + mu_c I, over the chunk table (thread = vertex of a component, which gives its mu_c);
+// CTAs past the chunk table take the orphan vertices, unshifted (their rows of diag are zero: the zero block).
+__global__ void __launch_bounds__(kT) pcg_blocks_shift_kernel(const PcgParams s, const float *__restrict__ diag, float rel_floor,
+                                                              const float *__restrict__ shift, float *__restrict__ inv_out) {
+  int v;
+  double mu = 0.0;
+  if (int(blockIdx.x) >= s.n_chunks) {
+    const int k = (int(blockIdx.x) - s.n_chunks) * kT + int(threadIdx.x);
+    if (k >= s.n_orphans) return;
+    v = s.orphans[k];
+  } else {
+    const int e = s.chunk[3 * blockIdx.x + 1] + int(threadIdx.x);
+    if (e >= s.chunk[3 * blockIdx.x + 2]) return;
+    v = s.vert[e];
+    mu = double(shift[s.chunk[3 * blockIdx.x]]);
+  }
+  block_inverse<true>(diag, s.n, v, rel_floor, mu, s.pinv, inv_out);
+}
+
 // r = b, z = P r, d = 0, partials of r.z and r.r.  CTAs past the chunk table zero d on the orphan vertices.
 __global__ void __launch_bounds__(kT) pcg_init_kernel(const PcgParams s, const float *__restrict__ b, float *__restrict__ d) {
   __shared__ double sh[kT / 32];
@@ -141,23 +168,43 @@ __global__ void __launch_bounds__(kT) pcg_init_kernel(const PcgParams s, const f
   if (threadIdx.x == 0) { s.part[kPartCols * size_t(blockIdx.x) + kRz] = rz; s.part[kPartCols * size_t(blockIdx.x) + kRr] = rr; }
 }
 
-// Partial of p.Hp of every chunk of an active component.
-__global__ void __launch_bounds__(kT) pcg_curv_kernel(const PcgParams s) {
-  __shared__ double sh[kT / 32];
+// Hp + mu p with one rounding per entry, in curvature and update alike
+__device__ __forceinline__ F3 shifted(F3 hp, F3 p, float mu) {
+  return F3{fmaf(mu, p.x, hp.x), fmaf(mu, p.y, hp.y), fmaf(mu, p.z, hp.z)};
+}
+
+// Partial of p.Hp (SHIFT: p.(Hp + mu_c p)) of every chunk of an active component.
+template <bool SHIFT>
+__device__ __forceinline__ void curv_body(const PcgParams &s, const float *__restrict__ shift, double *sh) {
   const int c = s.chunk[3 * blockIdx.x];
   if (s.comp[c].st_dir != kPcgActive) return;
   const int begin = s.chunk[3 * blockIdx.x + 1], end = s.chunk[3 * blockIdx.x + 2];
   const int e = begin + int(threadIdx.x);
   double q = 0.0;
-  if (e < end) { const int v = s.vert[e]; q = dot3(ld3(s.p, v), ld3(s.Hp, v)); }
+  if (e < end) {
+    const int v = s.vert[e];
+    const F3 p = ld3(s.p, v);
+    q = dot3(p, SHIFT ? shifted(ld3(s.Hp, v), p, shift[c]) : ld3(s.Hp, v));
+  }
   q = block_sum(q, sh);
   if (threadIdx.x == 0) s.part[kPartCols * size_t(blockIdx.x) + kPHp] = q;
 }
 
-// alpha = r.z / p.Hp per component; p.Hp <= 0 stops the component (at the first direction d = z = P b), otherwise
-// d += alpha p, r -= alpha Hp, z = P r and the partials of the new r.z and r.r.
-__global__ void __launch_bounds__(kT) pcg_update_kernel(const PcgParams s, float *__restrict__ d, int iter) {
+__global__ void __launch_bounds__(kT) pcg_curv_kernel(const PcgParams s) {
   __shared__ double sh[kT / 32];
+  curv_body<false>(s, nullptr, sh);
+}
+
+__global__ void __launch_bounds__(kT) pcg_curv_shift_kernel(const PcgParams s, const float *__restrict__ shift) {
+  __shared__ double sh[kT / 32];
+  curv_body<true>(s, shift, sh);
+}
+
+// alpha = r.z / p.Hp per component; p.Hp <= 0 stops the component (at the first direction d = z = P b), otherwise
+// d += alpha p, r -= alpha Hp, z = P r and the partials of the new r.z and r.r.  SHIFT: Hp + mu_c p in place of Hp.
+template <bool SHIFT>
+__device__ __forceinline__ void update_body(const PcgParams &s, float *__restrict__ d, int iter, const float *__restrict__ shift,
+                                            double *sh) {
   const int c = s.chunk[3 * blockIdx.x];
   const bool lead = int(blockIdx.x) == s.comp_chunk[c] && threadIdx.x == 0;
   PcgComp &C = s.comp[c];
@@ -180,7 +227,7 @@ __global__ void __launch_bounds__(kT) pcg_update_kernel(const PcgParams s, float
   double nrz = 0.0, nrr = 0.0;
   if (e < end) {
     const int v = s.vert[e];
-    const F3 p = ld3(s.p, v), hp = ld3(s.Hp, v);
+    const F3 p = ld3(s.p, v), hp = SHIFT ? shifted(ld3(s.Hp, v), p, shift[c]) : ld3(s.Hp, v);
     F3 x = ld3(d, v), r = ld3(s.r, v);
     x.x += a * p.x; x.y += a * p.y; x.z += a * p.z;
     r.x -= a * hp.x; r.y -= a * hp.y; r.z -= a * hp.z;
@@ -192,6 +239,17 @@ __global__ void __launch_bounds__(kT) pcg_update_kernel(const PcgParams s, float
   nrr = block_sum(nrr, sh);
   if (threadIdx.x == 0) { s.part[kPartCols * size_t(blockIdx.x) + kRz] = nrz; s.part[kPartCols * size_t(blockIdx.x) + kRr] = nrr; }
   if (lead) { C.st_upd = kPcgActive; C.idle = 0; C.n_hvp = iter + 1; C.rz_prev = rz; C.dHd += alpha * alpha * pHp; }
+}
+
+__global__ void __launch_bounds__(kT) pcg_update_kernel(const PcgParams s, float *__restrict__ d, int iter) {
+  __shared__ double sh[kT / 32];
+  update_body<false>(s, d, iter, nullptr, sh);
+}
+
+__global__ void __launch_bounds__(kT) pcg_update_shift_kernel(const PcgParams s, float *__restrict__ d, int iter,
+                                                              const float *__restrict__ shift) {
+  __shared__ double sh[kT / 32];
+  update_body<true>(s, d, iter, shift, sh);
 }
 
 // Folds r.z and r.r, tests convergence and sets the next direction p = z + beta p; a stopped component gets p = 0, so
@@ -292,6 +350,132 @@ __global__ void __launch_bounds__(kT) sphere_axpy_kernel(const PcgParams s, cons
   st3(out, v, y);
 }
 
+// ---- Damped Newton step (tsb_newton_step): the small kernels around the solve and the line search -------------------
+// Newton partial table: three columns per chunk, each written by one kernel and folded only by a later one.
+constexpr int kNwCols = 3, kNwMaxD = 0, kNwBd = 1, kNwDd = 2;
+
+// Maximum of v over the CTA; valid in thread 0 (a max does not depend on the order).
+__device__ __forceinline__ double block_max(double v, double *sh) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xFFFFFFFFu, v, o));
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double m = -INFINITY;
+  if (threadIdx.x == 0)
+#pragma unroll
+    for (int w = 0; w < kT / 32; ++w) m = fmax(m, sh[w]);
+  return m;
+}
+
+// b_c = 0 on the components already frozen; per-chunk maximum of the diagonal entries (D_v)_ii.
+__global__ void __launch_bounds__(kT) newton_prep_kernel(const PcgParams s, const NewtonParams w) {
+  __shared__ double sh[kT / 32];
+  const int c = s.chunk[3 * blockIdx.x];
+  const int e = s.chunk[3 * blockIdx.x + 1] + int(threadIdx.x);
+  double m = -INFINITY;
+  if (e < s.chunk[3 * blockIdx.x + 2]) {
+    const int v = s.vert[e];
+    if (w.comp[c].status != TSB_NEWTON_ACTIVE) st3(w.b, v, F3{0.f, 0.f, 0.f});
+    const F3 q = ld3(w.diag, v);
+    m = fmax(double(q.x), fmax(double(q.y), double(q.z)));
+  }
+  m = block_max(m, sh);
+  if (threadIdx.x == 0) w.part[kNwCols * size_t(blockIdx.x) + kNwMaxD] = m;
+}
+
+// mu_c = tau * max (D_v)_ii on a component's first step (clamped to [mu_min, mu_max]), nu_c = 2; the fp32 shift of the
+// solve (thread = component).
+__global__ void __launch_bounds__(kT) newton_shift_kernel(const PcgParams s, const NewtonParams w, NewtonRule r) {
+  const int c = blockIdx.x * kT + int(threadIdx.x);
+  if (c >= s.n_components) return;
+  NewtonComp &N = w.comp[c];
+  if (!N.init) {
+    double m = -INFINITY;
+    for (int k = s.comp_chunk[c]; k < s.comp_chunk[c + 1]; ++k) m = fmax(m, w.part[kNwCols * size_t(k) + kNwMaxD]);
+    N.mu = fmin(double(r.mu_max), fmax(double(r.mu_min), double(r.tau) * m));
+    N.nu = 2.0;
+    N.init = 1;
+  }
+  w.shift[c] = float(N.mu);
+}
+
+// Per-chunk partials of b.d and d.d (b.d exactly as pcg_bdotd_kernel forms it).
+__global__ void __launch_bounds__(kT) newton_dots_kernel(const PcgParams s, const NewtonParams w) {
+  __shared__ double sh[kT / 32];
+  const int e = s.chunk[3 * blockIdx.x + 1] + int(threadIdx.x);
+  double bd = 0.0, dd = 0.0;
+  if (e < s.chunk[3 * blockIdx.x + 2]) {
+    const int v = s.vert[e];
+    const F3 d = ld3(w.d, v);
+    bd = dot3(ld3(w.b, v), d);
+    dd = dot3(d, d);
+  }
+  bd = block_sum(bd, sh);
+  dd = block_sum(dd, sh);
+  if (threadIdx.x == 0) { w.part[kNwCols * size_t(blockIdx.x) + kNwBd] = bd; w.part[kNwCols * size_t(blockIdx.x) + kNwDd] = dd; }
+}
+
+// The step choice and the damping update of every component (thread = component); see tsb_newton_step in the header.
+__global__ void __launch_bounds__(kT) newton_decide_kernel(const PcgParams s, const NewtonParams w, NewtonRule r,
+                                                           tsb_newton_sphere_t *__restrict__ out) {
+  const int c = blockIdx.x * kT + int(threadIdx.x);
+  if (c >= s.n_components) return;
+  const PcgComp C = s.comp[c];
+  NewtonComp N = w.comp[c];
+  const int k0 = s.comp_chunk[c], k1 = s.comp_chunk[c + 1];
+  double bd = 0.0, dd = 0.0;
+  for (int k = k0; k < k1; ++k) bd += w.part[kNwCols * size_t(k) + kNwBd];
+  for (int k = k0; k < k1; ++k) dd += w.part[kNwCols * size_t(k) + kNwDd];
+  const double bdf = double(float(bd)), dHd = double(float(C.dHd));   // the values the solve's records report
+  const double g = sqrt(C.bb);
+  int ks = -1;
+  float alpha = 0.f, delta = 0.f;
+  double rho = 0.0;
+  if (N.status == TSB_NEWTON_ACTIVE) {
+    if (g <= double(r.gtol)) {
+      N.status = TSB_NEWTON_CONVERGED;
+    } else {
+      const float *dl = w.sphere_delta + size_t(c) * size_t(r.n_alpha) * 4;
+      const double lim = double(r.eta) * double(w.sphere_step[c]);
+      if (bdf > 0.0)
+        for (int k = 0; k < r.n_alpha; ++k) {
+          const double a = double(w.alphas[k]);
+          if (a < lim && double(dl[4 * k]) <= -double(r.sigma) * a * bdf) { ks = k; break; }
+        }
+      const double pred = bdf - 0.5 * (dHd - double(w.shift[c]) * dd);
+      rho = pred > 0.0 ? -double(dl[0]) / pred : 1.0;
+      if (ks == 0) {
+        const double t = 2.0 * rho - 1.0;
+        N.mu = fmax(double(r.mu_min), N.mu * fmax(1.0 / 3.0, 1.0 - t * t * t));
+        N.nu = 2.0;
+      } else {
+        N.mu = fmin(double(r.mu_max), N.mu * N.nu);
+        N.nu *= 2.0;
+      }
+      if (ks < 0 && N.mu == double(r.mu_max)) N.status = TSB_NEWTON_STALLED;
+      if (ks >= 0) { alpha = w.alphas[ks]; delta = dl[4 * ks]; }
+    }
+  }
+  w.alpha_sphere[c] = alpha;
+  w.comp[c] = N;
+  if (!out) return;
+  tsb_newton_sphere_t o;
+  o.mu = N.mu;
+  o.rho = rho;
+  o.grad_norm = float(g);
+  o.alpha = alpha;
+  o.delta = delta;
+  o.b_dot_d = float(bd);
+  o.k = ks;
+  o.pcg_status = C.st_dir == kPcgActive ? TSB_PCG_MAXITER : C.st_dir;
+  o.n_hvp = C.n_hvp;
+  o.status = N.status;
+  o.first_vertex = s.vert[s.chunk[3 * size_t(k0) + 1]];
+  o.reserved[0] = o.reserved[1] = o.reserved[2] = 0;
+  out[c] = o;
+}
+
 unsigned with_orphans(const PcgParams &s) { return unsigned(s.n_chunks + (s.n_orphans + kT - 1) / kT); }
 
 }  // namespace
@@ -307,9 +491,20 @@ cudaError_t launch_pcg_begin(const PcgParams &s, const float *b, float *d, cudaS
   return cudaGetLastError();
 }
 
-cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, cudaStream_t st) {
-  pcg_curv_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s);
-  pcg_update_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, d, iter);
+cudaError_t launch_pcg_blocks_shift(const PcgParams &s, const float *diag, float rel_floor, const float *shift, float *inv_out,
+                                    cudaStream_t st) {
+  pcg_blocks_shift_kernel<<<with_orphans(s), kT, 0, st>>>(s, diag, rel_floor, shift, inv_out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, const float *shift, cudaStream_t st) {
+  if (shift) {
+    pcg_curv_shift_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, shift);
+    pcg_update_shift_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, d, iter, shift);
+  } else {
+    pcg_curv_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s);
+    pcg_update_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, d, iter);
+  }
   pcg_dir_kernel<false><<<unsigned(s.n_chunks), kT, 0, st>>>(s, rtol);
   return cudaGetLastError();
 }
@@ -327,6 +522,23 @@ cudaError_t launch_pcg_records(const PcgParams &s, const float *b, const float *
 
 cudaError_t launch_sphere_axpy(const PcgParams &s, const float *x, const float *a, const float *d, float *out, cudaStream_t st) {
   sphere_axpy_kernel<<<with_orphans(s), kT, 0, st>>>(s, x, a, d, out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_newton_prep(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, cudaStream_t st) {
+  newton_prep_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w);
+  newton_shift_kernel<<<unsigned((s.n_components + kT - 1) / kT), kT, 0, st>>>(s, w, r);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_newton_dots(const PcgParams &s, const NewtonParams &w, cudaStream_t st) {
+  newton_dots_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_newton_decide(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, tsb_newton_sphere_t *out,
+                                 cudaStream_t st) {
+  newton_decide_kernel<<<unsigned((s.n_components + kT - 1) / kT), kT, 0, st>>>(s, w, r, out);
   return cudaGetLastError();
 }
 

@@ -41,13 +41,51 @@ struct PcgParams {
   int32_t *active;             // [1] components still active (pcg_count_kernel)
 };
 
+// State of one component of the damped Newton step (tsb_newton_step).  The shift kernel writes mu, nu and init on a
+// component's first step, the decision kernel mu, nu and status; the other kernels only read it.  32 bytes.
+struct NewtonComp {
+  double mu, nu;
+  int32_t status;   // TSB_NEWTON_*
+  int32_t init;     // mu initialised
+  int32_t pad[2];
+};
+static_assert(sizeof(NewtonComp) == 32, "NewtonComp must be 32 bytes");
+
+struct NewtonParams {
+  float *b, *d;              // [n, 3]: -grad (zeroed on frozen components), the damped Newton direction
+  float *diag;               // [2, n, 3]: tsb_hess_diag's planes
+  float *shift;              // [n_components] fp32 mu_c handed to the solve
+  float *alpha_sphere;       // [n_components] step taken
+  const float *alphas;       // [TSB_LINE_MAX_ALPHA] 2^-k
+  float *sphere_delta;       // [n_components][n_alpha][4] line search
+  float *sphere_step;        // [n_components] inversion-free step over (0, 1]
+  double *part;              // [n_chunks, 3] per-chunk partials: max (D_v)_ii, b.d, d.d
+  NewtonComp *comp;          // [n_components]
+};
+
+struct NewtonRule {           // the options the kernels read
+  float tau, mu_min, mu_max, gtol, sigma, eta;
+  int32_t n_alpha;
+};
+
 cudaError_t launch_pcg_blocks(const PcgParams &s, const float *diag, float rel_floor, float *inv_out, cudaStream_t st);
+// blocks D_v + shift[c] I (over the chunk table; orphan vertices unshifted)
+cudaError_t launch_pcg_blocks_shift(const PcgParams &s, const float *diag, float rel_floor, const float *shift, float *inv_out,
+                                    cudaStream_t st);
 // r = b, z = P r, d = 0 and the first direction; leaves every component ACTIVE or ZERO_RHS
 cudaError_t launch_pcg_begin(const PcgParams &s, const float *b, float *d, cudaStream_t st);
-// after Hp = H p of iteration `iter` (0-based) is complete on the stream: curvature, update and next direction
-cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, cudaStream_t st);
+// after Hp = H p of iteration `iter` (0-based) is complete on the stream: curvature, update and next direction; with
+// shift != nullptr the operator is H + shift[c] I
+cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, const float *shift, cudaStream_t st);
 cudaError_t launch_pcg_count(const PcgParams &s, cudaStream_t st);
 cudaError_t launch_pcg_records(const PcgParams &s, const float *b, const float *d, tsb_pcg_sphere_t *out, cudaStream_t st);
 cudaError_t launch_sphere_axpy(const PcgParams &s, const float *x, const float *a, const float *d, float *out, cudaStream_t st);
+// b_c = 0 on frozen components, per-chunk max (D_v)_ii, then mu_c on a first step and the fp32 shift
+cudaError_t launch_newton_prep(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, cudaStream_t st);
+// per-chunk b.d and d.d
+cudaError_t launch_newton_dots(const PcgParams &s, const NewtonParams &w, cudaStream_t st);
+// step choice, damping update, records (out may be null)
+cudaError_t launch_newton_decide(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, tsb_newton_sphere_t *out,
+                                 cudaStream_t st);
 
 }  // namespace tsb

@@ -227,6 +227,22 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         pcg.set_blocks(self.tet_sp.hess_diag(xd, c1, c2, order, c3=self.amips_coeff))
         return pcg.solve(xd, b.detach(), c1, c2, order, c3=self.amips_coeff, **solve_kw)
 
+    def newton_step(self, x, it, **opts):
+        """One damped (Levenberg-Marquardt) Newton step per sphere of ``c1 * smooth + c2 * barrier (+ amips_coeff *
+        amips)`` with the scheduler's coefficients and the barrier order at ``it``: ``tssplat_b200.newton.DeviceNewton``
+        (``tsb_newton_step``), which updates ``x.data`` in place without a host read.  ``opts``: the fields of
+        ``newton.NEWTON_DEFAULTS``.  The workspace, ``self.device_newton``, is created on first use (sharing
+        ``self.device_pcg``); its ``reset()`` restarts every sphere.  Returns the ``NewtonStepResult``."""
+        from .newton import DeviceNewton, DevicePCG
+        nw = getattr(self, "device_newton", None)
+        if nw is None:
+            pcg = getattr(self, "device_pcg", None)
+            if pcg is None:
+                pcg = self.device_pcg = DevicePCG(self.tet_sp)
+            nw = self.device_newton = DeviceNewton(self.tet_sp, pcg)
+        c1, c2 = self.coeff_scheduler(it)
+        return nw.step(x.data, c1, c2, self.order_at(it), c3=self.amips_coeff, **opts)
+
     def forward(self, x, it, c1, c2):
         order = self.order_at(it)
         if self.amips_coeff > 0:

@@ -9,6 +9,11 @@ from these and ``TetSpheres.line_search``.
 ``DevicePCG`` is the device-resident solver (``tsb_pcg_solve``): the same truncated PCG, but run independently on every
 tet-sphere (the Hessian is block diagonal by sphere) with all scalars in device memory, so there is no host read inside
 an iteration and the solve can be captured in a CUDA graph.  ``pcg`` below stays as the reference implementation.
+With a per-sphere ``shift`` it solves ``(H + mu_c I) d = b`` (``tsb_pcg_solve_ex``).
+
+``DeviceNewton`` joins the pieces into a minimiser (``tsb_newton_step``): one damped (Levenberg-Marquardt) Newton step per
+sphere per call -- gradient, diagonal blocks, shifted solve, line search, step choice and damping update -- on one
+stream without a host read.
 """
 from __future__ import annotations
 
@@ -17,7 +22,8 @@ from typing import Callable, NamedTuple, Optional, Union
 
 import torch
 
-__all__ = ["hess_blocks", "block_jacobi", "apply_blocks", "pcg", "PCGResult", "DevicePCG", "DevicePCGResult"]
+__all__ = ["hess_blocks", "block_jacobi", "apply_blocks", "pcg", "PCGResult", "DevicePCG", "DevicePCGResult", "DeviceNewton",
+           "NewtonStepResult", "NEWTON_DEFAULTS"]
 
 
 def hess_blocks(planes: torch.Tensor) -> torch.Tensor:
@@ -161,34 +167,48 @@ class DevicePCG:
             raise RuntimeError(f"{name} must be a float32 tensor of {numel} entries on {self.tet_sp.device}")
         return t if t.is_contiguous() else t.contiguous()
 
+    def _shift(self, shift) -> Optional[torch.Tensor]:
+        """None, a Python float (every sphere), or a float32 CUDA tensor of one entry per sphere."""
+        if shift is None:
+            return None
+        if isinstance(shift, torch.Tensor):
+            return self._f32(shift, self.n_spheres, "shift")
+        return torch.full((self.n_spheres,), float(shift), dtype=torch.float32, device=self.tet_sp.device)
+
     def set_blocks(self, planes: Optional[torch.Tensor] = None, rel_floor: float = 1e-6,
-                   want_inverse: bool = False) -> Optional[torch.Tensor]:
+                   want_inverse: bool = False, shift=None) -> Optional[torch.Tensor]:
         """Preconditioner from the [2, n, 3] planes of ``hess_diag`` with ``block_jacobi``'s semantics, computed on the
         device (``tsb_pcg_set_blocks``); ``None`` is the identity.  ``want_inverse`` returns the inverse blocks as
-        [n, 6] = (xx, yy, zz, yz, xz, xy)."""
+        [n, 6] = (xx, yy, zz, yz, xz, xy).  ``shift``: per-sphere ``mu_c`` (a float32 CUDA tensor [S], or a float for
+        every sphere); the blocks are then ``D_v + mu_c I`` (``tsb_pcg_set_blocks_ex``)."""
         n = self.tet_sp.n
         pc = None if planes is None else self._f32(planes, 6 * n, "planes")
+        sh = self._shift(shift)
         inv = torch.empty((n, 6), dtype=torch.float32, device=self.tet_sp.device) if want_inverse else None
-        rc = self._capi.lib.tsb_pcg_set_blocks(self._s, pc.data_ptr() if pc is not None else None, float(rel_floor),
-                                               inv.data_ptr() if want_inverse else None, self._stream_ptr(self.tet_sp.device))
+        rc = self._capi.lib.tsb_pcg_set_blocks_ex(self._s, pc.data_ptr() if pc is not None else None, float(rel_floor),
+                                                  sh.data_ptr() if sh is not None else None,
+                                                  inv.data_ptr() if want_inverse else None, self._stream_ptr(self.tet_sp.device))
         self._check(rc, "set_blocks")
         return inv
 
     def solve(self, x: torch.Tensor, b: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0,
-              max_iter: int = 100, rtol: float = 1e-3, check_every: int = 0) -> DevicePCGResult:
+              max_iter: int = 100, rtol: float = 1e-3, check_every: int = 0, shift=None) -> DevicePCGResult:
         """``H(x) d = b`` on every sphere by truncated PCG (``tsb_pcg_solve``), ``H`` the Hessian ``TetSpheres.hvp``
         multiplies by.  ``check_every = 0`` enqueues ``max_iter`` iterations without touching the host (and can be
         captured in a CUDA graph); ``k > 0`` reads the number of active spheres every ``k`` iterations and stops
-        early."""
+        early.  ``shift`` (as in ``set_blocks``) solves ``(H + mu_c I) d = b`` instead (``tsb_pcg_solve_ex``); ``d_H_d``
+        is then ``d^T (H + mu_c I) d``."""
         n3, dev = self.tet_sp.n3, self.tet_sp.device
         xc, bc = self._f32(x, n3, "x"), self._f32(b, n3, "b")
+        sh = self._shift(shift)
         d = torch.empty((self.tet_sp.n, 3), dtype=torch.float32, device=dev)
         raw = torch.empty((self.n_spheres, 8), dtype=torch.int32, device=dev)
         terms = self._capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
         opt = self._capi.tsb_pcg_options_t(max_iter=int(max_iter), rtol=float(rtol), check_every=int(check_every))
         iters = C.c_int32(0)
-        rc = self._capi.lib.tsb_pcg_solve(self._s, xc.data_ptr(), bc.data_ptr(), C.byref(terms), C.byref(opt), d.data_ptr(),
-                                          raw.data_ptr(), C.byref(iters), self._stream_ptr(dev))
+        rc = self._capi.lib.tsb_pcg_solve_ex(self._s, xc.data_ptr(), bc.data_ptr(), C.byref(terms), C.byref(opt),
+                                             sh.data_ptr() if sh is not None else None, d.data_ptr(), raw.data_ptr(),
+                                             C.byref(iters), self._stream_ptr(dev))
         self._check(rc, "solve")
         f = raw.view(torch.float32)
         return DevicePCGResult(d, raw[:, 4], raw[:, 3], f[:, 0], f[:, 1], f[:, 2], int(iters.value))
@@ -206,3 +226,110 @@ class DevicePCG:
                                             self._stream_ptr(self.tet_sp.device))
         self._check(rc, "axpy")
         return out
+
+
+#: options of ``DeviceNewton.step`` (``tsb_newton_options_t``)
+NEWTON_DEFAULTS = dict(max_iter=20, rtol=1e-2, rel_floor=1e-6, tau=1e-3, mu_min=1e-12, mu_max=1e12, gtol=0.0, sigma=1e-4,
+                       eta=0.9, n_alpha=8)
+
+
+class NewtonStepResult(NamedTuple):
+    """What ``DeviceNewton.step`` returns: device tensors [S], spheres in the order of their lowest vertex ids
+    (``tsb_newton_sphere_t`` in ``include/tssplat_b200.h``)."""
+    grad_norm: torch.Tensor         # f32: |grad_c| before the step (0 once the sphere is frozen)
+    alpha: torch.Tensor             # f32: step taken (0: none)
+    k: torch.Tensor                 # i32: index of the step size 2^-k taken, -1 when none
+    delta: torch.Tensor             # f32: E_c(x + alpha d) - E_c(x) of the step taken (0 if none)
+    mu: torch.Tensor                # f64: damping after the update
+    rho: torch.Tensor               # f64: gain ratio of the full step (0 when no decision ran)
+    pcg_status: torch.Tensor        # i32: TSB_PCG_* of the damped solve
+    n_hvp: torch.Tensor             # i32: products in which the sphere was active
+    b_dot_d: torch.Tensor           # f32: b_c . d_c, b = -grad
+    status: torch.Tensor            # i32: 0 active, 1 converged, 2 stalled (both frozen)
+    first_vertex: torch.Tensor      # i32: lowest vertex id of the sphere
+
+
+class DeviceNewton:
+    """Damped Newton workspace (``tsb_newton_create``) of one ``TetSpheres`` handle: reuses ``pcg`` (a ``DevicePCG`` of
+    the same handle) or creates one, and keeps it alive.  Every sphere runs its own Levenberg-Marquardt iteration;
+    ``reset`` starts them all again.  Serves one stream at a time, like the handle."""
+
+    def __init__(self, tet_sp, pcg: Optional[DevicePCG] = None):
+        from . import _capi
+        from .tet_spheres_ext import _stream_ptr
+        self._capi, self._stream_ptr = _capi, _stream_ptr
+        self._nw = None
+        if pcg is None:
+            pcg = DevicePCG(tet_sp)
+        elif pcg.tet_sp is not tet_sp:
+            raise RuntimeError("DeviceNewton: pcg belongs to another handle")
+        self.tet_sp, self.pcg, self.n_spheres = tet_sp, pcg, pcg.n_spheres
+        nw = C.c_void_p()
+        rc = _capi.lib.tsb_newton_create(pcg._s, C.byref(nw))
+        if rc:
+            raise RuntimeError(f"DeviceNewton: {self._error(None)} (code {rc})")
+        self._nw = nw
+        self.device_bytes = int(_capi.lib.tsb_newton_device_bytes(nw))
+
+    def __del__(self):
+        nw, self._nw = getattr(self, "_nw", None), None
+        if nw:
+            try:
+                self._capi.lib.tsb_newton_destroy(nw)
+            except Exception:  # interpreter shutdown
+                pass
+
+    def _error(self, nw) -> str:
+        msg = self._capi.lib.tsb_newton_last_error(nw)
+        return msg.decode("utf-8", "replace") if msg else ""
+
+    def _check(self, rc: int, what: str) -> None:
+        if rc:
+            raise RuntimeError(f"DeviceNewton.{what}: {self._error(self._nw)} (code {rc})")
+
+    def reset(self) -> None:
+        """Every sphere ACTIVE again, its damping re-initialised at the next step."""
+        self._check(self._capi.lib.tsb_newton_reset(self._nw, self._stream_ptr(self.tet_sp.device)), "reset")
+
+    def options(self, **opts):
+        """``tsb_newton_options_t`` from ``NEWTON_DEFAULTS`` updated with ``opts``."""
+        bad = set(opts) - set(NEWTON_DEFAULTS)
+        if bad:
+            raise TypeError(f"unknown Newton options: {sorted(bad)}")
+        o = {**NEWTON_DEFAULTS, **opts}
+        return self._capi.tsb_newton_options_t(**{k: (int(v) if k in ("max_iter", "n_alpha") else float(v)) for k, v in o.items()})
+
+    def step(self, x: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0, **opts) -> NewtonStepResult:
+        """One damped Newton step of ``c1 * smooth + c2 * barrier (+ c3 * amips)`` on every sphere, updating ``x`` (a
+        contiguous float32 CUDA tensor of 3n entries) in place, without a host read (capturable in a CUDA graph).
+        ``opts``: the fields of ``NEWTON_DEFAULTS``."""
+        xc = self.pcg._f32(x, self.tet_sp.n3, "x")
+        if xc is not x:
+            raise RuntimeError("x must be contiguous (it is updated in place)")
+        raw = torch.empty((self.n_spheres, 16), dtype=torch.int32, device=self.tet_sp.device)
+        terms = self._capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
+        opt = self.options(**opts)
+        rc = self._capi.lib.tsb_newton_step(self._nw, x.data_ptr(), C.byref(terms), C.byref(opt), raw.data_ptr(),
+                                            self._stream_ptr(self.tet_sp.device))
+        self._check(rc, "step")
+        f64, f32 = raw[:, 0:4].view(torch.float64), raw[:, 4:8].view(torch.float32)
+        return NewtonStepResult(f32[:, 0], f32[:, 1], raw[:, 8], f32[:, 2], f64[:, 0], f64[:, 1], raw[:, 9], raw[:, 10],
+                                f32[:, 3], raw[:, 11], raw[:, 12])
+
+    def minimize(self, x: torch.Tensor, n_steps: int, c1: float, c2: float, order: int, c3: float = 0.0,
+                 check_every: int = 0, **opts):
+        """Up to ``n_steps`` calls of ``step``; returns (steps run, the last ``NewtonStepResult``).  ``check_every = 0``
+        never touches the host (capturable); ``k > 0`` reads one integer, the number of spheres still active, every
+        ``k`` steps and stops when it is 0 (refused while the stream is being captured)."""
+        if check_every < 0 or n_steps < 0:
+            raise ValueError("n_steps and check_every must be >= 0")
+        if check_every > 0 and torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("DeviceNewton.minimize: check_every > 0 reads the host and cannot be captured in a CUDA "
+                               "graph: use check_every = 0")
+        res = None
+        for i in range(n_steps):
+            res = self.step(x, c1, c2, order, c3=c3, **opts)
+            if check_every > 0 and (i + 1) % check_every == 0 and i + 1 < n_steps:
+                if int((res.status == 0).sum()) == 0:
+                    return i + 1, res
+        return n_steps, res

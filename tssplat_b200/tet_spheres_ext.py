@@ -32,7 +32,8 @@ import torch
 from . import _capi
 from .mesh import load_veg
 
-__all__ = ["TetSpheres", "SphereStats", "LineSearch", "forward", "backward", "hvp", "line_search", "hess_diag", "random_x",
+__all__ = ["TetSpheres", "SphereStats", "LineSearch", "forward", "backward", "hvp", "line_search", "hess_diag", "newton_step",
+           "random_x",
            "grad_limit", "energy_grad_host"]
 
 return_cpu_scalar = False
@@ -403,6 +404,13 @@ def hess_diag(vertexPositions: torch.Tensor, tet_sp: TetSpheres, c1: float, c2: 
     """``TetSpheres.hess_diag`` in the argument order of ``forward``: the per-vertex 3x3 diagonal blocks of the Hessian
     as [2, n, 3] (diagonal entries, then (yz, xz, xy))."""
     return tet_sp.hess_diag(vertexPositions, c1, c2, order, c3=c3)
+
+
+def newton_step(vertexPositions: torch.Tensor, newton, c1: float, c2: float, order: int, c3: float = 0.0, **opts):
+    """``tssplat_b200.newton.DeviceNewton.step`` in the argument order of ``forward``, with the Newton workspace (created
+    with ``DeviceNewton(tet_sp)``) in place of the handle: one damped Newton step per sphere, updating
+    ``vertexPositions`` in place (``tsb_newton_step``)."""
+    return newton.step(vertexPositions, c1, c2, order, c3=c3, **opts)
 
 
 def random_x(tet_sp: TetSpheres) -> torch.Tensor:
