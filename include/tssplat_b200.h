@@ -20,7 +20,7 @@
 extern "C" {
 #endif
 
-#define TSB_VERSION 8
+#define TSB_VERSION 9
 #define TSB_LINE_MAX_ALPHA 8   /* step sizes one tsb_line_search call may evaluate */
 
 enum {
@@ -345,8 +345,9 @@ int tsb_pcg_solve_ex(tsb_pcg_t s, const float *x_dev, const float *b_dev, const 
  * whether mu is initialised), three fp64 partials per chunk and the per-sphere step sizes.  Device memory, reported by
  * tsb_newton_device_bytes:
  *   48 n + 24 chunks + 172 n_components + 176   bytes
- * (chunks as for tsb_pcg_device_bytes).  A new workspace is reset (every sphere ACTIVE, mu not initialised).  Like the
- * handle and the solver workspace it serves one stream at a time, and it shares the solver workspace's scratch. */
+ * (chunks as for tsb_pcg_device_bytes), plus 8 max(chunks, 1) bytes once a tsb_newton_prox_step has been made.  A
+ * new workspace is reset (every sphere ACTIVE, mu not initialised).  Like the handle and the solver workspace it serves
+ * one stream at a time, and it shares the solver workspace's scratch. */
 typedef struct tsb_newton_s *tsb_newton_t;
 int tsb_newton_create(tsb_pcg_t s, tsb_newton_t *out);
 void tsb_newton_destroy(tsb_newton_t nw);
@@ -412,6 +413,44 @@ typedef struct {            /* one per component, component order of tsb_energy_
  * terms->c3 != 0 on a handle without enable_amips.  DESIGN.md section 5, "Damped Newton step". */
 int tsb_newton_step(tsb_newton_t nw, float *x_dev, const tsb_terms_t *terms, const tsb_newton_options_t *opt,
                     tsb_newton_sphere_t *records_out_dev, void *stream);
+
+/* ---- Proximal Newton step: the geometry energy plus a per-sphere pull toward an anchor --------------------------
+ * One damped Newton iteration, on every sphere c, of the proximal objective
+ *   Phi_c(x) = E_c(x) + (w_c / 2) |x_c - y_c|^2        (summed over the vertices of c)
+ * with E = c1 smooth + c2 barrier (+ c3 amips) from *terms as in tsb_newton_step.  anchor_dev: device float32 [3n], the
+ * anchor y; weight_dev: device float32 [info.n_components], w_c in the component order of tsb_energy_grad_spheres.  Both
+ * are read on the device, so a captured graph can be replayed after new anchor data and new weights are copied into the
+ * same buffers.  The use: a first-order optimiser takes its step on the data term alone, giving y, and this call then
+ * pulls the geometry energy down without moving far from y (the Hessian H + w_c I stays block diagonal by sphere).  A
+ * linear term needs no separate support: q.x + (w/2)|x - x0|^2 = (w/2)|x - (x0 - q/w)|^2 + const, so a caller with a
+ * linearised data gradient q passes the anchor x0 - q/w.
+ *
+ * tsb_newton_step's eight phases, options, records and invariants, with these changes:
+ *   1. after the gradient launch, b_v += (-w_c)(x_v - y_v) on active spheres, each operation rounded on its own (no
+ *      contraction), so that eager torch's b + (-w) * (x - y) gives the same bits; g = |b_c| = |grad Phi_c|, tested
+ *      against gtol;
+ *   3. on a sphere's first step mu_c = tau (max_v max_i (D_v)_ii + w_c), clamped as before; the solve's fp32 shift is
+ *      fp32(mu_c + w_c), in tsb_pcg_set_blocks_ex and tsb_pcg_solve_ex alike (the record's mu is the damping alone);
+ *   5. also d.(x - y) per sphere (fp64 partials per chunk, folded in a fixed order);
+ *   7. the decision uses dPhi_k = dE_k + w_c (alpha_k d.(x - y) + alpha_k^2 |d|^2 / 2) (fp64) wherever the plain rule uses
+ *      dE_k: in the Armijo test and in rho; pred = bd - (dHd - mu' dd) / 2 with mu' = double(shift) - double(w_c), since
+ *      the solve's dHd is d^T (H + shift I) d; the inversion bound eta alpha^ is unchanged.
+ * Records: the same layout; grad_norm is |grad Phi_c|, delta the dPhi of the step taken, b_dot_d uses b = -grad Phi.
+ * A sphere whose w_c is NaN, infinite or negative gets b_c = 0 and alpha = 0 and is marked STALLED (frozen until
+ * tsb_newton_reset): its vertices do not move.  With every w_c = 0 the call gives bitwise the x and records of
+ * tsb_newton_step.  The new kernels use no floating-point atomics and fold in a fixed order, so the determinism and
+ * independence statements of tsb_newton_step hold here too (a sphere's trajectory depends on its own anchor and weight
+ * only).
+ * The first call on a workspace allocates 8 max(chunks, 1) bytes for the d.(x - y) partials with cudaMalloc;
+ * tsb_newton_device_bytes includes them from then on.  Make that first call outside any stream capture: on a stream
+ * being captured it returns TSB_E_INVALID, and a cudaMalloc while another stream of the process is being captured in
+ * global mode invalidates that capture.
+ * Argument errors (TSB_E_INVALID, nothing launched): everything tsb_newton_step rejects, a null anchor_dev or
+ * weight_dev, and anchor_dev == x_dev (x is updated in place while the anchor is read).  DESIGN.md section 5, "Proximal
+ * Newton step". */
+int tsb_newton_prox_step(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const float *weight_dev,
+                         const tsb_terms_t *terms, const tsb_newton_options_t *opt,
+                         tsb_newton_sphere_t *records_out_dev, void *stream);
 
 /* Same computation for callers whose vertex positions live in HOST memory (e.g. a CPU-side
  * optimiser): copies x_host -> device, runs the fused launch, copies energy[3] and grad back,

@@ -52,4 +52,21 @@ if not big:
     sv2, sf2 = surface_vf_gpu(pack.tets, pack.n)
     assert np.array_equal(sv, sv2) and np.array_equal(sf, sf2)
     print("surface extraction ok", len(sv2), len(sf2))
+    # one proximal Newton step runs the whole Newton stack: gradient, diagonal blocks, the shifted block-Jacobi PCG,
+    # the line search, the step's own kernels and the axpy, first in their proximal variants (one sphere with a NaN
+    # weight), then the plain ones
+    from tssplat_b200.newton import DeviceNewton
+    pack = make_pack(3, 1024, seed=3, unique=4)
+    sp = ext.TetSpheres(pack.verts.reshape(-1), pack.tets.reshape(-1), enable_amips=True, deterministic=True)
+    nw = DeviceNewton(sp)
+    x = torch.from_numpy(perturb(pack, sigma_rel=0.35, seed=1)).cuda()
+    y = x.clone()
+    w = torch.tensor([1e-3, 1.0, float("nan")], device="cuda")
+    r = nw.step(x, 2e-4, 3e-4, 2, c3=1e-4, anchor=y, weight=w, max_iter=5)
+    torch.cuda.synchronize()
+    print("prox step ok", r.status.tolist(), r.alpha.tolist())
+    nw.reset()                                         # and the plain step's kernels
+    r = nw.step(x, 2e-4, 3e-4, 2, c3=1e-4, max_iter=5)
+    torch.cuda.synchronize()
+    print("newton step ok", r.status.tolist(), r.alpha.tolist())
 print("DONE")

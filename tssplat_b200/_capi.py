@@ -24,7 +24,7 @@ EXPORTED_SYMBOLS = (
     "tsb_line_search", "tsb_hess_diag", "tsb_pcg_create", "tsb_pcg_destroy", "tsb_pcg_last_error", "tsb_pcg_device_bytes",
     "tsb_pcg_set_blocks", "tsb_pcg_solve", "tsb_sphere_axpy", "tsb_pcg_set_blocks_ex", "tsb_pcg_solve_ex",
     "tsb_newton_create", "tsb_newton_destroy", "tsb_newton_last_error", "tsb_newton_device_bytes", "tsb_newton_reset",
-    "tsb_newton_step", "tsb_energy_grad_host", "tsb_scale",
+    "tsb_newton_step", "tsb_newton_prox_step", "tsb_energy_grad_host", "tsb_scale",
     "tsb_grad_limit", "tsb_adam_uniform_step",
     "tsb_surface_create", "tsb_surface_destroy", "tsb_surface_last_error", "tsb_surface_forward", "tsb_surface_backward",
     "tsb_surface_extract", "tsb_free_host", "tsb_setup_last_error",
@@ -141,6 +141,8 @@ def _load() -> C.CDLL:
     lib.tsb_newton_reset.argtypes = [vp, vp]
     lib.tsb_newton_step.restype = C.c_int
     lib.tsb_newton_step.argtypes = [vp, vp, C.POINTER(tsb_terms_t), C.POINTER(tsb_newton_options_t), vp, vp]
+    lib.tsb_newton_prox_step.restype = C.c_int
+    lib.tsb_newton_prox_step.argtypes = [vp, vp, vp, vp, C.POINTER(tsb_terms_t), C.POINTER(tsb_newton_options_t), vp, vp]
     lib.tsb_energy_grad_host.restype = C.c_int
     lib.tsb_energy_grad_host.argtypes = [vp, vp, f32, f32, i32, f32, vp, vp, vp]
     lib.tsb_scale.restype = C.c_int

@@ -57,6 +57,7 @@ struct tsb_newton_s {
   tsb::NewtonParams W{};
   float *energy = nullptr;           // [4] energies of the gradient launch (not reported)
   float *delta = nullptr;            // [TSB_LINE_MAX_ALPHA][4] the line search's totals (not reported)
+  double *prox_part = nullptr;       // [chunks] d.(x - y) partials of tsb_newton_prox_step (allocated by its first call)
   int64_t device_bytes = 0;
   std::vector<void *> allocs;
   std::string err;
@@ -681,9 +682,12 @@ int tsb_newton_reset(tsb_newton_t nw, void *stream) {
   return TSB_OK;
 }
 
-int tsb_newton_step(tsb_newton_t nw, float *x_dev, const tsb_terms_t *terms, const tsb_newton_options_t *opt,
-                    tsb_newton_sphere_t *records_out_dev, void *stream) {
-  if (!nw) return TSB_E_INVALID;
+}  // extern "C"
+
+namespace {
+
+// tsb_newton_step's argument rules, shared by tsb_newton_prox_step
+int newton_check(tsb_newton_t nw, const float *x_dev, const tsb_terms_t *terms, const tsb_newton_options_t *opt) {
   if (!x_dev || !terms || !opt) return newton_fail(nw, TSB_E_INVALID, "x_dev, terms and opt must be non-null");
   const tsb_newton_options_t &o = *opt;
   if (o.max_iter < 1) return newton_fail(nw, TSB_E_INVALID, "max_iter must be >= 1");
@@ -699,14 +703,17 @@ int tsb_newton_step(tsb_newton_t nw, float *x_dev, const tsb_terms_t *terms, con
     return newton_fail(nw, TSB_E_INVALID, "n_alpha must be in [1, " + std::to_string(TSB_LINE_MAX_ALPHA) + "]");
   for (int32_t r : o.reserved)
     if (r != 0) return newton_fail(nw, TSB_E_INVALID, "reserved fields must be 0");
+  if (terms->order != 2 && terms->order != 4) return newton_fail(nw, TSB_E_INVALID, "order must be 2 or 4");
+  if (terms->c3 != 0.f && !nw->s->h->amips)
+    return newton_fail(nw, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
+  return TSB_OK;
+}
+
+// The eight phases of tsb_newton_step; prox != nullptr: those of tsb_newton_prox_step (the PROX kernel variants).
+int newton_run(tsb_newton_t nw, float *x_dev, const tsb::ProxParams *prox, const tsb_terms_t *terms,
+               const tsb_newton_options_t &o, tsb_newton_sphere_t *records_out_dev, cudaStream_t st) {
   tsb_pcg_t s = nw->s;
   tsb_handle_t h = s->h;
-  if (terms->order != 2 && terms->order != 4) return newton_fail(nw, TSB_E_INVALID, "order must be 2 or 4");
-  if (terms->c3 != 0.f && !h->amips)
-    return newton_fail(nw, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
-  DeviceGuard guard(h->device);
-  if (!guard.ok) return newton_fail(nw, TSB_E_CUDA, "cannot select the handle's CUDA device");
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   const tsb::NewtonParams &W = nw->W;
   const tsb::NewtonRule R{o.tau, o.mu_min, o.mu_max, o.gtol, o.sigma, o.eta, o.n_alpha};
   const tsb_pcg_options_t po{o.max_iter, o.rtol, 0, {0, 0, 0, 0, 0}};
@@ -714,24 +721,68 @@ int tsb_newton_step(tsb_newton_t nw, float *x_dev, const tsb_terms_t *terms, con
   int rc = energy_grad_impl(h, x_dev, terms->c1, terms->c2, terms->c3, terms->order, -1.f, nullptr, nw->energy, 1, W.b, nullptr, st);
   if (rc == TSB_OK) rc = tsb_hess_diag(h, x_dev, terms, 1.f, nullptr, W.diag, st);
   if (rc != TSB_OK) return newton_fail(nw, rc, h->err);
-  // 3: frozen spheres' b = 0, mu on a first step
-  cudaError_t e = tsb::launch_newton_prep(s->P, W, R, st);
+  // 3: frozen spheres' b = 0 (prox: b -= w (x - y)), mu on a first step
+  cudaError_t e = tsb::launch_newton_prep(s->P, W, R, prox, st);
   if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
   // 4: the damped solve
   rc = tsb_pcg_set_blocks_ex(s, W.diag, o.rel_floor, W.shift, nullptr, st);
   if (rc == TSB_OK) rc = tsb_pcg_solve_ex(s, x_dev, W.b, terms, &po, W.shift, W.d, nullptr, nullptr, st);
   if (rc != TSB_OK) return newton_fail(nw, rc, s->err);
-  // 5: b.d and |d|^2 per chunk
-  e = tsb::launch_newton_dots(s->P, W, st);
+  // 5: b.d and |d|^2 (prox: and d.(x - y)) per chunk
+  e = tsb::launch_newton_dots(s->P, W, prox, st);
   if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
   // 6: line search at 2^-k, per sphere
   rc = tsb_line_search(h, x_dev, W.d, terms, W.alphas, o.n_alpha, nw->delta, nullptr, W.sphere_delta, W.sphere_step, st);
   if (rc != TSB_OK) return newton_fail(nw, rc, h->err);
   // 7-8: decision, step
-  e = tsb::launch_newton_decide(s->P, W, R, records_out_dev, st);
+  e = tsb::launch_newton_decide(s->P, W, R, prox, records_out_dev, st);
   if (e == cudaSuccess) e = tsb::launch_sphere_axpy(s->P, x_dev, W.alpha_sphere, W.d, x_dev, st);
   if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
   return TSB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int tsb_newton_step(tsb_newton_t nw, float *x_dev, const tsb_terms_t *terms, const tsb_newton_options_t *opt,
+                    tsb_newton_sphere_t *records_out_dev, void *stream) {
+  if (!nw) return TSB_E_INVALID;
+  int rc = newton_check(nw, x_dev, terms, opt);
+  if (rc != TSB_OK) return rc;
+  DeviceGuard guard(nw->s->h->device);
+  if (!guard.ok) return newton_fail(nw, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  return newton_run(nw, x_dev, nullptr, terms, *opt, records_out_dev, static_cast<cudaStream_t>(stream));
+}
+
+int tsb_newton_prox_step(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const float *weight_dev,
+                         const tsb_terms_t *terms, const tsb_newton_options_t *opt, tsb_newton_sphere_t *records_out_dev,
+                         void *stream) {
+  if (!nw) return TSB_E_INVALID;
+  int rc = newton_check(nw, x_dev, terms, opt);
+  if (rc != TSB_OK) return rc;
+  if (!anchor_dev || !weight_dev) return newton_fail(nw, TSB_E_INVALID, "anchor_dev and weight_dev must be non-null");
+  if (anchor_dev == x_dev)
+    return newton_fail(nw, TSB_E_INVALID, "anchor_dev must not be x_dev: x is updated in place while the anchor is read");
+  DeviceGuard guard(nw->s->h->device);
+  if (!guard.ok) return newton_fail(nw, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!nw->prox_part) {        // the d.(x - y) partials: allocated by the first proximal step, never read before written
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    if (cudaStreamIsCapturing(st, &cap) != cudaSuccess) { cudaGetLastError(); return newton_fail(nw, TSB_E_CUDA, "cannot query the stream"); }
+    if (cap != cudaStreamCaptureStatusNone)
+      return newton_fail(nw, TSB_E_INVALID, "the first tsb_newton_prox_step of a workspace allocates device memory and cannot be "
+                                            "captured in a CUDA graph: make one call outside any capture first");
+    const size_t bytes = std::max<size_t>(size_t(nw->s->P.n_chunks), 1) * sizeof(double);
+    void *d = nullptr;
+    const cudaError_t e = cudaMalloc(&d, bytes);
+    if (e != cudaSuccess) return newton_fail(nw, TSB_E_NOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e));
+    nw->allocs.push_back(d);
+    nw->device_bytes += int64_t(bytes);
+    nw->prox_part = static_cast<double *>(d);
+  }
+  const tsb::ProxParams prox{x_dev, anchor_dev, weight_dev, nw->prox_part};
+  return newton_run(nw, x_dev, &prox, terms, *opt, records_out_dev, st);
 }
 
 int tsb_energy_grad_host(tsb_handle_t h, const float *x_host, float c1, float c2, int32_t order, float gradH,

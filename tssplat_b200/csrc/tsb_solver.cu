@@ -368,15 +368,31 @@ __device__ __forceinline__ double block_max(double v, double *sh) {
   return m;
 }
 
-// b_c = 0 on the components already frozen; per-chunk maximum of the diagonal entries (D_v)_ii.
-__global__ void __launch_bounds__(kT) newton_prep_kernel(const PcgParams s, const NewtonParams w) {
-  __shared__ double sh[kT / 32];
+// The proximal weight of a component is usable when it is finite and >= 0 (NaN fails both tests).
+__device__ __forceinline__ bool prox_weight_ok(float wc) { return wc >= 0.f && wc < INFINITY; }
+
+// b_c = 0 on the components already frozen; per-chunk maximum of the diagonal entries (D_v)_ii.  PROX: b_c = 0 also where
+// w_c is unusable, and elsewhere b_v += (-w_c)(x_v - y_v), each operation rounded on its own (no contraction), as eager
+// torch rounds b + (-w) * (x - y); w_c = 0 leaves b as it is.
+template <bool PROX>
+__device__ __forceinline__ void prep_body(const PcgParams &s, const NewtonParams &w, const ProxParams &p, double *sh) {
   const int c = s.chunk[3 * blockIdx.x];
   const int e = s.chunk[3 * blockIdx.x + 1] + int(threadIdx.x);
   double m = -INFINITY;
   if (e < s.chunk[3 * blockIdx.x + 2]) {
     const int v = s.vert[e];
-    if (w.comp[c].status != TSB_NEWTON_ACTIVE) st3(w.b, v, F3{0.f, 0.f, 0.f});
+    if (PROX) {
+      const float wc = p.weight[c];
+      if (w.comp[c].status != TSB_NEWTON_ACTIVE || !prox_weight_ok(wc)) {
+        st3(w.b, v, F3{0.f, 0.f, 0.f});
+      } else if (wc != 0.f) {
+        const F3 b = ld3(w.b, v), x = ld3(p.x, v), y = ld3(p.anchor, v);
+        st3(w.b, v, F3{__fadd_rn(b.x, __fmul_rn(-wc, __fsub_rn(x.x, y.x))), __fadd_rn(b.y, __fmul_rn(-wc, __fsub_rn(x.y, y.y))),
+                       __fadd_rn(b.z, __fmul_rn(-wc, __fsub_rn(x.z, y.z)))});
+      }
+    } else if (w.comp[c].status != TSB_NEWTON_ACTIVE) {
+      st3(w.b, v, F3{0.f, 0.f, 0.f});
+    }
     const F3 q = ld3(w.diag, v);
     m = fmax(double(q.x), fmax(double(q.y), double(q.z)));
   }
@@ -384,56 +400,118 @@ __global__ void __launch_bounds__(kT) newton_prep_kernel(const PcgParams s, cons
   if (threadIdx.x == 0) w.part[kNwCols * size_t(blockIdx.x) + kNwMaxD] = m;
 }
 
+__global__ void __launch_bounds__(kT) newton_prep_kernel(const PcgParams s, const NewtonParams w) {
+  __shared__ double sh[kT / 32];
+  prep_body<false>(s, w, ProxParams{}, sh);
+}
+
+__global__ void __launch_bounds__(kT) newton_prep_prox_kernel(const PcgParams s, const NewtonParams w, const ProxParams p) {
+  __shared__ double sh[kT / 32];
+  prep_body<true>(s, w, p, sh);
+}
+
 // mu_c = tau * max (D_v)_ii on a component's first step (clamped to [mu_min, mu_max]), nu_c = 2; the fp32 shift of the
-// solve (thread = component).
-__global__ void __launch_bounds__(kT) newton_shift_kernel(const PcgParams s, const NewtonParams w, NewtonRule r) {
+// solve (thread = component).  PROX: mu_c = tau * (max (D_v)_ii + w_c) and the shift is mu_c + w_c (w_c read as 0 where
+// it is unusable: that component's right-hand side is 0).
+template <bool PROX>
+__device__ __forceinline__ void shift_body(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, const ProxParams &p) {
   const int c = blockIdx.x * kT + int(threadIdx.x);
   if (c >= s.n_components) return;
   NewtonComp &N = w.comp[c];
+  double wc = 0.0;
+  if (PROX) { const float q = p.weight[c]; wc = prox_weight_ok(q) ? double(q) : 0.0; }
   if (!N.init) {
     double m = -INFINITY;
     for (int k = s.comp_chunk[c]; k < s.comp_chunk[c + 1]; ++k) m = fmax(m, w.part[kNwCols * size_t(k) + kNwMaxD]);
-    N.mu = fmin(double(r.mu_max), fmax(double(r.mu_min), double(r.tau) * m));
+    N.mu = fmin(double(r.mu_max), fmax(double(r.mu_min), double(r.tau) * (PROX ? m + wc : m)));
     N.nu = 2.0;
     N.init = 1;
   }
-  w.shift[c] = float(N.mu);
+  w.shift[c] = float(PROX ? N.mu + wc : N.mu);
 }
 
-// Per-chunk partials of b.d and d.d (b.d exactly as pcg_bdotd_kernel forms it).
-__global__ void __launch_bounds__(kT) newton_dots_kernel(const PcgParams s, const NewtonParams w) {
-  __shared__ double sh[kT / 32];
+__global__ void __launch_bounds__(kT) newton_shift_kernel(const PcgParams s, const NewtonParams w, NewtonRule r) {
+  shift_body<false>(s, w, r, ProxParams{});
+}
+
+__global__ void __launch_bounds__(kT) newton_shift_prox_kernel(const PcgParams s, const NewtonParams w, NewtonRule r,
+                                                               const ProxParams p) {
+  shift_body<true>(s, w, r, p);
+}
+
+// Per-chunk partials of b.d and d.d (b.d exactly as pcg_bdotd_kernel forms it).  PROX: also d.(x - y), in its own array.
+template <bool PROX>
+__device__ __forceinline__ void dots_body(const PcgParams &s, const NewtonParams &w, const ProxParams &p, double *sh) {
   const int e = s.chunk[3 * blockIdx.x + 1] + int(threadIdx.x);
-  double bd = 0.0, dd = 0.0;
+  double bd = 0.0, dd = 0.0, dx = 0.0;
   if (e < s.chunk[3 * blockIdx.x + 2]) {
     const int v = s.vert[e];
     const F3 d = ld3(w.d, v);
     bd = dot3(ld3(w.b, v), d);
     dd = dot3(d, d);
+    if (PROX) {
+      const F3 x = ld3(p.x, v), y = ld3(p.anchor, v);
+      dx = double(d.x) * (double(x.x) - double(y.x)) + double(d.y) * (double(x.y) - double(y.y)) +
+           double(d.z) * (double(x.z) - double(y.z));
+    }
   }
   bd = block_sum(bd, sh);
   dd = block_sum(dd, sh);
-  if (threadIdx.x == 0) { w.part[kNwCols * size_t(blockIdx.x) + kNwBd] = bd; w.part[kNwCols * size_t(blockIdx.x) + kNwDd] = dd; }
+  if (PROX) dx = block_sum(dx, sh);
+  if (threadIdx.x == 0) {
+    w.part[kNwCols * size_t(blockIdx.x) + kNwBd] = bd;
+    w.part[kNwCols * size_t(blockIdx.x) + kNwDd] = dd;
+    if (PROX) p.part[blockIdx.x] = dx;
+  }
 }
 
-// The step choice and the damping update of every component (thread = component); see tsb_newton_step in the header.
-__global__ void __launch_bounds__(kT) newton_decide_kernel(const PcgParams s, const NewtonParams w, NewtonRule r,
-                                                           tsb_newton_sphere_t *__restrict__ out) {
+__global__ void __launch_bounds__(kT) newton_dots_kernel(const PcgParams s, const NewtonParams w) {
+  __shared__ double sh[kT / 32];
+  dots_body<false>(s, w, ProxParams{}, sh);
+}
+
+__global__ void __launch_bounds__(kT) newton_dots_prox_kernel(const PcgParams s, const NewtonParams w, const ProxParams p) {
+  __shared__ double sh[kT / 32];
+  dots_body<true>(s, w, p, sh);
+}
+
+// Phi_c(x + a d) - Phi_c(x) from the line search's dE = E_c(x + a d) - E_c(x): dE + w_c (a d.(x - y) + a^2 |d|^2 / 2).
+// Without PROX, or with w_c = 0, it is dE itself.
+template <bool PROX>
+__device__ __forceinline__ double step_change(float dE, double wc, double a, double dx, double dd) {
+  return PROX && wc > 0.0 ? double(dE) + wc * (a * dx + 0.5 * a * a * dd) : double(dE);
+}
+
+// The step choice and the damping update of every component (thread = component); see tsb_newton_step and
+// tsb_newton_prox_step in the header.
+template <bool PROX>
+__device__ __forceinline__ void decide_body(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, const ProxParams &p,
+                                            tsb_newton_sphere_t *__restrict__ out) {
   const int c = blockIdx.x * kT + int(threadIdx.x);
   if (c >= s.n_components) return;
   const PcgComp C = s.comp[c];
   NewtonComp N = w.comp[c];
   const int k0 = s.comp_chunk[c], k1 = s.comp_chunk[c + 1];
-  double bd = 0.0, dd = 0.0;
+  double bd = 0.0, dd = 0.0, dx = 0.0;
   for (int k = k0; k < k1; ++k) bd += w.part[kNwCols * size_t(k) + kNwBd];
   for (int k = k0; k < k1; ++k) dd += w.part[kNwCols * size_t(k) + kNwDd];
+  double wc = 0.0;
+  bool bad_w = false;
+  if (PROX) {
+    for (int k = k0; k < k1; ++k) dx += p.part[k];
+    const float q = p.weight[c];
+    bad_w = !prox_weight_ok(q);
+    wc = bad_w ? 0.0 : double(q);
+  }
   const double bdf = double(float(bd)), dHd = double(float(C.dHd));   // the values the solve's records report
   const double g = sqrt(C.bb);
   int ks = -1;
   float alpha = 0.f, delta = 0.f;
   double rho = 0.0;
   if (N.status == TSB_NEWTON_ACTIVE) {
-    if (g <= double(r.gtol)) {
+    if (PROX && bad_w) {
+      N.status = TSB_NEWTON_STALLED;
+    } else if (g <= double(r.gtol)) {
       N.status = TSB_NEWTON_CONVERGED;
     } else {
       const float *dl = w.sphere_delta + size_t(c) * size_t(r.n_alpha) * 4;
@@ -441,10 +519,10 @@ __global__ void __launch_bounds__(kT) newton_decide_kernel(const PcgParams s, co
       if (bdf > 0.0)
         for (int k = 0; k < r.n_alpha; ++k) {
           const double a = double(w.alphas[k]);
-          if (a < lim && double(dl[4 * k]) <= -double(r.sigma) * a * bdf) { ks = k; break; }
+          if (a < lim && step_change<PROX>(dl[4 * k], wc, a, dx, dd) <= -double(r.sigma) * a * bdf) { ks = k; break; }
         }
-      const double pred = bdf - 0.5 * (dHd - double(w.shift[c]) * dd);
-      rho = pred > 0.0 ? -double(dl[0]) / pred : 1.0;
+      const double pred = bdf - 0.5 * (dHd - (PROX ? double(w.shift[c]) - wc : double(w.shift[c])) * dd);
+      rho = pred > 0.0 ? -step_change<PROX>(dl[0], wc, double(w.alphas[0]), dx, dd) / pred : 1.0;
       if (ks == 0) {
         const double t = 2.0 * rho - 1.0;
         N.mu = fmax(double(r.mu_min), N.mu * fmax(1.0 / 3.0, 1.0 - t * t * t));
@@ -454,7 +532,10 @@ __global__ void __launch_bounds__(kT) newton_decide_kernel(const PcgParams s, co
         N.nu *= 2.0;
       }
       if (ks < 0 && N.mu == double(r.mu_max)) N.status = TSB_NEWTON_STALLED;
-      if (ks >= 0) { alpha = w.alphas[ks]; delta = dl[4 * ks]; }
+      if (ks >= 0) {
+        alpha = w.alphas[ks];
+        delta = PROX ? float(step_change<PROX>(dl[4 * ks], wc, double(alpha), dx, dd)) : dl[4 * ks];
+      }
     }
   }
   w.alpha_sphere[c] = alpha;
@@ -474,6 +555,16 @@ __global__ void __launch_bounds__(kT) newton_decide_kernel(const PcgParams s, co
   o.first_vertex = s.vert[s.chunk[3 * size_t(k0) + 1]];
   o.reserved[0] = o.reserved[1] = o.reserved[2] = 0;
   out[c] = o;
+}
+
+__global__ void __launch_bounds__(kT) newton_decide_kernel(const PcgParams s, const NewtonParams w, NewtonRule r,
+                                                           tsb_newton_sphere_t *__restrict__ out) {
+  decide_body<false>(s, w, r, ProxParams{}, out);
+}
+
+__global__ void __launch_bounds__(kT) newton_decide_prox_kernel(const PcgParams s, const NewtonParams w, NewtonRule r,
+                                                                tsb_newton_sphere_t *__restrict__ out, const ProxParams p) {
+  decide_body<true>(s, w, r, p, out);
 }
 
 unsigned with_orphans(const PcgParams &s) { return unsigned(s.n_chunks + (s.n_orphans + kT - 1) / kT); }
@@ -525,20 +616,30 @@ cudaError_t launch_sphere_axpy(const PcgParams &s, const float *x, const float *
   return cudaGetLastError();
 }
 
-cudaError_t launch_newton_prep(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, cudaStream_t st) {
-  newton_prep_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w);
-  newton_shift_kernel<<<unsigned((s.n_components + kT - 1) / kT), kT, 0, st>>>(s, w, r);
+cudaError_t launch_newton_prep(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, const ProxParams *p,
+                               cudaStream_t st) {
+  const unsigned comp_blocks = unsigned((s.n_components + kT - 1) / kT);
+  if (p) {
+    newton_prep_prox_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w, *p);
+    newton_shift_prox_kernel<<<comp_blocks, kT, 0, st>>>(s, w, r, *p);
+  } else {
+    newton_prep_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w);
+    newton_shift_kernel<<<comp_blocks, kT, 0, st>>>(s, w, r);
+  }
   return cudaGetLastError();
 }
 
-cudaError_t launch_newton_dots(const PcgParams &s, const NewtonParams &w, cudaStream_t st) {
-  newton_dots_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w);
+cudaError_t launch_newton_dots(const PcgParams &s, const NewtonParams &w, const ProxParams *p, cudaStream_t st) {
+  if (p) newton_dots_prox_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w, *p);
+  else newton_dots_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w);
   return cudaGetLastError();
 }
 
-cudaError_t launch_newton_decide(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, tsb_newton_sphere_t *out,
-                                 cudaStream_t st) {
-  newton_decide_kernel<<<unsigned((s.n_components + kT - 1) / kT), kT, 0, st>>>(s, w, r, out);
+cudaError_t launch_newton_decide(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, const ProxParams *p,
+                                 tsb_newton_sphere_t *out, cudaStream_t st) {
+  const unsigned comp_blocks = unsigned((s.n_components + kT - 1) / kT);
+  if (p) newton_decide_prox_kernel<<<comp_blocks, kT, 0, st>>>(s, w, r, out, *p);
+  else newton_decide_kernel<<<comp_blocks, kT, 0, st>>>(s, w, r, out);
   return cudaGetLastError();
 }
 

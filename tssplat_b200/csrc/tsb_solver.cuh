@@ -63,6 +63,13 @@ struct NewtonParams {
   NewtonComp *comp;          // [n_components]
 };
 
+// The proximal step's extra inputs (tsb_newton_prox_step), read by the PROX variants of the Newton kernels only.
+struct ProxParams {
+  const float *x, *anchor;   // [n, 3]: the point of the step and the anchor y
+  const float *weight;       // [n_components] w_c
+  double *part;              // [n_chunks] per-chunk partials of d.(x - y)
+};
+
 struct NewtonRule {           // the options the kernels read
   float tau, mu_min, mu_max, gtol, sigma, eta;
   int32_t n_alpha;
@@ -80,12 +87,14 @@ cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, 
 cudaError_t launch_pcg_count(const PcgParams &s, cudaStream_t st);
 cudaError_t launch_pcg_records(const PcgParams &s, const float *b, const float *d, tsb_pcg_sphere_t *out, cudaStream_t st);
 cudaError_t launch_sphere_axpy(const PcgParams &s, const float *x, const float *a, const float *d, float *out, cudaStream_t st);
+// The three launchers below run the proximal variants when p != nullptr.
 // b_c = 0 on frozen components, per-chunk max (D_v)_ii, then mu_c on a first step and the fp32 shift
-cudaError_t launch_newton_prep(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, cudaStream_t st);
-// per-chunk b.d and d.d
-cudaError_t launch_newton_dots(const PcgParams &s, const NewtonParams &w, cudaStream_t st);
+cudaError_t launch_newton_prep(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, const ProxParams *p,
+                               cudaStream_t st);
+// per-chunk b.d and d.d (and d.(x - y))
+cudaError_t launch_newton_dots(const PcgParams &s, const NewtonParams &w, const ProxParams *p, cudaStream_t st);
 // step choice, damping update, records (out may be null)
-cudaError_t launch_newton_decide(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, tsb_newton_sphere_t *out,
-                                 cudaStream_t st);
+cudaError_t launch_newton_decide(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, const ProxParams *p,
+                                 tsb_newton_sphere_t *out, cudaStream_t st);
 
 }  // namespace tsb

@@ -227,12 +227,7 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         pcg.set_blocks(self.tet_sp.hess_diag(xd, c1, c2, order, c3=self.amips_coeff))
         return pcg.solve(xd, b.detach(), c1, c2, order, c3=self.amips_coeff, **solve_kw)
 
-    def newton_step(self, x, it, **opts):
-        """One damped (Levenberg-Marquardt) Newton step per sphere of ``c1 * smooth + c2 * barrier (+ amips_coeff *
-        amips)`` with the scheduler's coefficients and the barrier order at ``it``: ``tssplat_b200.newton.DeviceNewton``
-        (``tsb_newton_step``), which updates ``x.data`` in place without a host read.  ``opts``: the fields of
-        ``newton.NEWTON_DEFAULTS``.  The workspace, ``self.device_newton``, is created on first use (sharing
-        ``self.device_pcg``); its ``reset()`` restarts every sphere.  Returns the ``NewtonStepResult``."""
+    def _device_newton(self):
         from .newton import DeviceNewton, DevicePCG
         nw = getattr(self, "device_newton", None)
         if nw is None:
@@ -240,8 +235,35 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
             if pcg is None:
                 pcg = self.device_pcg = DevicePCG(self.tet_sp)
             nw = self.device_newton = DeviceNewton(self.tet_sp, pcg)
+        return nw
+
+    def newton_step(self, x, it, **opts):
+        """One damped (Levenberg-Marquardt) Newton step per sphere of ``c1 * smooth + c2 * barrier (+ amips_coeff *
+        amips)`` with the scheduler's coefficients and the barrier order at ``it``: ``tssplat_b200.newton.DeviceNewton``
+        (``tsb_newton_step``), which updates ``x.data`` in place without a host read.  ``opts``: the fields of
+        ``newton.NEWTON_DEFAULTS``.  The workspace, ``self.device_newton``, is created on first use (sharing
+        ``self.device_pcg``); its ``reset()`` restarts every sphere.  Returns the ``NewtonStepResult``."""
+        nw = self._device_newton()
         c1, c2 = self.coeff_scheduler(it)
         return nw.step(x.data, c1, c2, self.order_at(it), c3=self.amips_coeff, **opts)
+
+    def prox_step(self, x, y, it, weight, n_steps=1, restart=True, **opts):
+        """The regulariser half of a split step: ``n_steps`` proximal Newton steps per sphere of
+        ``E(x) + (w_c / 2) |x_c - y_c|^2``, ``E`` the energy of ``newton_step`` at ``it`` (scheduler coefficients,
+        barrier order, ``amips_coeff``), anchored at ``y`` (typically ``x`` right after the optimiser's step on the data
+        term, copied: ``y`` must not be ``x``).  ``weight``: a float for every sphere or a float32 CUDA tensor [S].
+        Updates ``x.data`` in place with no host read (``tsb_newton_prox_step``) and returns the last
+        ``NewtonStepResult``.  ``restart`` resets the workspace first: a new anchor is a new problem, and a sphere frozen
+        on the old one must not stay frozen.  ``opts``: the fields of ``newton.NEWTON_DEFAULTS``."""
+        if n_steps < 1:
+            raise ValueError("n_steps must be >= 1")
+        nw = self._device_newton()
+        if restart:
+            nw.reset()
+        c1, c2 = self.coeff_scheduler(it)
+        _, res = nw.minimize(x.data, n_steps, c1, c2, self.order_at(it), c3=self.amips_coeff, anchor=y.detach(),
+                             weight=weight, **opts)
+        return res
 
     def forward(self, x, it, c1, c2):
         order = self.order_at(it)

@@ -13,7 +13,9 @@ With a per-sphere ``shift`` it solves ``(H + mu_c I) d = b`` (``tsb_pcg_solve_ex
 
 ``DeviceNewton`` joins the pieces into a minimiser (``tsb_newton_step``): one damped (Levenberg-Marquardt) Newton step per
 sphere per call -- gradient, diagonal blocks, shifted solve, line search, step choice and damping update -- on one
-stream without a host read.
+stream without a host read.  Given an ``anchor`` y and per-sphere weights w, the step minimises the proximal objective
+``E(x) + (w_c / 2) |x_c - y_c|^2`` instead (``tsb_newton_prox_step``): the regulariser half of a split training loop whose
+data term keeps its first-order optimiser.
 """
 from __future__ import annotations
 
@@ -167,12 +169,12 @@ class DevicePCG:
             raise RuntimeError(f"{name} must be a float32 tensor of {numel} entries on {self.tet_sp.device}")
         return t if t.is_contiguous() else t.contiguous()
 
-    def _shift(self, shift) -> Optional[torch.Tensor]:
+    def _shift(self, shift, name: str = "shift") -> Optional[torch.Tensor]:
         """None, a Python float (every sphere), or a float32 CUDA tensor of one entry per sphere."""
         if shift is None:
             return None
         if isinstance(shift, torch.Tensor):
-            return self._f32(shift, self.n_spheres, "shift")
+            return self._f32(shift, self.n_spheres, name)
         return torch.full((self.n_spheres,), float(shift), dtype=torch.float32, device=self.tet_sp.device)
 
     def set_blocks(self, planes: Optional[torch.Tensor] = None, rel_floor: float = 1e-6,
@@ -269,7 +271,11 @@ class DeviceNewton:
         if rc:
             raise RuntimeError(f"DeviceNewton: {self._error(None)} (code {rc})")
         self._nw = nw
-        self.device_bytes = int(_capi.lib.tsb_newton_device_bytes(nw))
+
+    @property
+    def device_bytes(self) -> int:
+        """``tsb_newton_device_bytes``: grows by 8 bytes per chunk at the first proximal step."""
+        return int(self._capi.lib.tsb_newton_device_bytes(self._nw))
 
     def __del__(self):
         nw, self._nw = getattr(self, "_nw", None), None
@@ -299,36 +305,61 @@ class DeviceNewton:
         o = {**NEWTON_DEFAULTS, **opts}
         return self._capi.tsb_newton_options_t(**{k: (int(v) if k in ("max_iter", "n_alpha") else float(v)) for k, v in o.items()})
 
-    def step(self, x: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0, **opts) -> NewtonStepResult:
+    def step(self, x: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0, anchor: Optional[torch.Tensor] = None,
+             weight=None, **opts) -> NewtonStepResult:
         """One damped Newton step of ``c1 * smooth + c2 * barrier (+ c3 * amips)`` on every sphere, updating ``x`` (a
         contiguous float32 CUDA tensor of 3n entries) in place, without a host read (capturable in a CUDA graph).
-        ``opts``: the fields of ``NEWTON_DEFAULTS``."""
+        ``opts``: the fields of ``NEWTON_DEFAULTS``.
+
+        With an ``anchor`` y (a contiguous float32 tensor of 3n entries on the handle's device, not ``x`` itself) the
+        step is one of the proximal objective ``E(x) + (w_c / 2) |x_c - y_c|^2`` per sphere (``tsb_newton_prox_step``);
+        ``weight`` is then required: a float for every sphere, or a float32 CUDA tensor [S] read on the device.  The
+        records' ``grad_norm``, ``delta`` and ``b_dot_d`` are then those of the proximal objective, and a sphere whose
+        weight is NaN, infinite or negative is frozen (STALLED) without moving.  A linear term ``q . x`` folds into the
+        anchor: pass ``y = x0 - q / w``."""
         xc = self.pcg._f32(x, self.tet_sp.n3, "x")
         if xc is not x:
             raise RuntimeError("x must be contiguous (it is updated in place)")
+        if anchor is None and weight is not None:
+            raise RuntimeError("weight needs an anchor")
+        if anchor is not None:
+            if weight is None:
+                raise RuntimeError("an anchor needs a weight (a float or a float32 CUDA tensor of one entry per sphere)")
+            if self.pcg._f32(anchor, self.tet_sp.n3, "anchor") is not anchor:
+                raise RuntimeError("anchor must be contiguous")
+            if anchor.data_ptr() == x.data_ptr():
+                raise RuntimeError("anchor must not be x (x is updated in place while the anchor is read)")
+            w = self.pcg._shift(weight, "weight")
         raw = torch.empty((self.n_spheres, 16), dtype=torch.int32, device=self.tet_sp.device)
         terms = self._capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
         opt = self.options(**opts)
-        rc = self._capi.lib.tsb_newton_step(self._nw, x.data_ptr(), C.byref(terms), C.byref(opt), raw.data_ptr(),
-                                            self._stream_ptr(self.tet_sp.device))
+        st = self._stream_ptr(self.tet_sp.device)
+        if anchor is None:
+            rc = self._capi.lib.tsb_newton_step(self._nw, x.data_ptr(), C.byref(terms), C.byref(opt), raw.data_ptr(), st)
+        else:
+            rc = self._capi.lib.tsb_newton_prox_step(self._nw, x.data_ptr(), anchor.data_ptr(), w.data_ptr(), C.byref(terms),
+                                                     C.byref(opt), raw.data_ptr(), st)
         self._check(rc, "step")
         f64, f32 = raw[:, 0:4].view(torch.float64), raw[:, 4:8].view(torch.float32)
         return NewtonStepResult(f32[:, 0], f32[:, 1], raw[:, 8], f32[:, 2], f64[:, 0], f64[:, 1], raw[:, 9], raw[:, 10],
                                 f32[:, 3], raw[:, 11], raw[:, 12])
 
     def minimize(self, x: torch.Tensor, n_steps: int, c1: float, c2: float, order: int, c3: float = 0.0,
-                 check_every: int = 0, **opts):
+                 check_every: int = 0, anchor: Optional[torch.Tensor] = None, weight=None, **opts):
         """Up to ``n_steps`` calls of ``step``; returns (steps run, the last ``NewtonStepResult``).  ``check_every = 0``
         never touches the host (capturable); ``k > 0`` reads one integer, the number of spheres still active, every
-        ``k`` steps and stops when it is 0 (refused while the stream is being captured)."""
+        ``k`` steps and stops when it is 0 (refused while the stream is being captured).  ``anchor`` and ``weight``: the
+        proximal step of ``step``."""
         if check_every < 0 or n_steps < 0:
             raise ValueError("n_steps and check_every must be >= 0")
         if check_every > 0 and torch.cuda.is_current_stream_capturing():
             raise RuntimeError("DeviceNewton.minimize: check_every > 0 reads the host and cannot be captured in a CUDA "
                                "graph: use check_every = 0")
+        if anchor is not None and weight is not None and not isinstance(weight, torch.Tensor):
+            weight = self.pcg._shift(weight, "weight")         # one tensor for every step
         res = None
         for i in range(n_steps):
-            res = self.step(x, c1, c2, order, c3=c3, **opts)
+            res = self.step(x, c1, c2, order, c3=c3, anchor=anchor, weight=weight, **opts)
             if check_every > 0 and (i + 1) % check_every == 0 and i + 1 < n_steps:
                 if int((res.status == 0).sum()) == 0:
                     return i + 1, res
