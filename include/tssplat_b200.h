@@ -20,7 +20,7 @@
 extern "C" {
 #endif
 
-#define TSB_VERSION 9
+#define TSB_VERSION 10
 #define TSB_LINE_MAX_ALPHA 8   /* step sizes one tsb_line_search call may evaluate */
 
 enum {
@@ -161,7 +161,8 @@ int tsb_energy_grad_spheres(tsb_handle_t h, const float *x_dev, const tsb_terms_
  *   curv_out = v^T H v as { c1*vMv + c2*vHbv, vMv, vHbv }   (optional device float[3]; NOT scaled by gradH)
  * with H(x) = c1 M + c2 sum_t H_t(x): M = G^T L^T L G (the smoothness Hessian: 1/2 x^T M x has Hessian M), and H_t the
  * Hessian of max(-J_t, 0)^order, nonzero only for tets whose fp32 J (the value tsb_energy_grad tests) is negative.
- * vMv = v^T M v and vHbv = sum_t v^T H_t v.  H_t is the exact, indefinite tet Hessian (no SPD projection).
+ * vMv = v^T M v and vHbv = sum_t v^T H_t v.  H_t is the exact, indefinite tet Hessian (tsb_pcg_hvp_psd multiplies by its
+ * PSD projection).
  * The AMIPS term is NOT part of the product: tsb_hvp differentiates c1*smooth + c2*barrier only, also on handles
  * created with enable_amips (tsb_hvp_ex below adds it).  x_dev, v_dev: device float32 [3n], contiguous; order 2 or 4;
  * vertices no tet references get zero rows.  The launch streams the same plan as tsb_energy_grad (one kernel, plus the
@@ -337,6 +338,54 @@ int tsb_pcg_set_blocks_ex(tsb_pcg_t s, const float *diag_dev, float rel_floor, c
 int tsb_pcg_solve_ex(tsb_pcg_t s, const float *x_dev, const float *b_dev, const tsb_terms_t *terms,
                      const tsb_pcg_options_t *opt, const float *shift_dev, float *d_out_dev,
                      tsb_pcg_sphere_t *spheres_out_dev, int32_t *iters_run_out, void *stream);
+
+/* ---- Projected Hessian (projected Newton) ---------------------------------------------------------------------------
+ * Opt-in on a solver workspace: every tet's Hessian in deformation-gradient space is replaced by its positive
+ * semidefinite projection (same eigenvectors, negative eigenvalues clamped to 0), so the solve multiplies by
+ *   H+(x) = c1 M + c2 sum_t K_t^T P(H_b,t) K_t + c3 sum_t K_t^T P(H_a,t) K_t       (K_t: dx -> dF = dDs Dm^-1)
+ * which is PSD on every sphere: CG on it never stops at negative curvature from the tet terms, and a Levenberg-Marquardt
+ * shift only has to regularise.  A tet is barrier-active where its det F < 0 and AMIPS-active where det F > 0 and
+ * c3 != 0 (det F in fp64 from the fp32 positions: its sign can differ from the energy kernel's fp32 J only for |J| within
+ * rounding of 0).  The projection uses the closed form of isotropic energies (signed SVD F = U diag(s) V^T, U and V proper
+ * rotations; DESIGN.md section 5, "Projected Hessian").  This is a different model, not another implementation of the
+ * exact one: iterates differ from the exact mode's, and the exact-mode calls are unchanged.
+ *
+ * tsb_pcg_enable_psd: rest_xyz (host float32 [3n]) and tets (host int32 [4 nele]) must be the mesh the workspace's handle
+ * was created from.  Checks nele against the handle (TSB_E_INVALID), and every vertex id against [0, n) and every tet's
+ * four vertices against the handle's components (TSB_E_MESH); computes Dm^-1 per tet in fp64 (stored as fp32; a zero-volume
+ * rest tet is TSB_E_MESH), builds the per-vertex incidence lists of (tet, corner) ascending on the host, and allocates the
+ * per-tet operators and the corner scratch.  After it, tsb_pcg_device_bytes has grown by
+ *   237 nele + 4 (n + 1) + 16 ceil(nele / 256) + 16   bytes
+ * (tet ids 16, Dm^-1 36, operator 120, activity 1, corner vectors 48 and incidence entries 16 per tet); the handle's
+ * info.device_bytes is unchanged, and a workspace that never enables the mode keeps its size.  A second call is
+ * TSB_E_INVALID.  After a failure the workspace is as before.
+ * CAPTURE: the call is synchronous and allocates with cudaMalloc; it takes no stream, so it can only see a capture on the
+ * legacy default stream (then TSB_E_INVALID).  A capture on any other stream is NOT detected: cudaMalloc then fails
+ * (TSB_E_NOMEM with the CUDA message) and, in global capture mode, invalidates that capture.  Make the call before any
+ * capture starts (DevicePCG(hessian="psd") refuses to run while torch's current stream is capturing).
+ *
+ * tsb_pcg_hvp_psd: projects at x, then hv_out = H+(x) v (device float32 [3n], fully overwritten, required) and
+ *   curv_out = { c1 vMv + c2 vHb+v + c3 vHa+v, vMv, vHb+v, vHa+v }     (optional device float[4])
+ * with vHb+v and vHa+v unweighted sums over the active tets.  c1, c2, order, c3 from *terms with tsb_hvp_ex's rules, and
+ * c1, c2, c3 >= 0 (a negative or NaN coefficient is TSB_E_INVALID: the projection does not commute with a negative
+ * weight).  Launches: the projection (one thread per tet), tsb_hvp_ex with c2 = c3 = 0 for c1 M v (its tet pass then adds
+ * exact zeros), the tet kernel that writes each active tet's weighted corner vectors to the scratch, the vertex gather
+ * that adds each vertex's active corners in incidence-list order (and, with curv_out, one fold kernel).
+ *
+ * With the mode enabled, tsb_pcg_solve(_ex) runs one projection launch before its loop and the projected product in place
+ * of tsb_hvp_ex; the records' d_H_d is then d^T (H+ + mu I) d.  tsb_newton_step and tsb_newton_prox_step on a Newton
+ * workspace over this solver workspace follow with no change of signature (their pred then models H+), and reject
+ * negative coefficients.  The preconditioner stays the exact tsb_hess_diag blocks, clamped by tsb_pcg_set_blocks(_ex).
+ * Invariants: no host read and no allocation after enable (everything is capturable in a CUDA graph); no floating-point
+ * atomics in the new kernels and every per-vertex sum in incidence-list order, so hv, curv, d and the records are bitwise
+ * identical across calls, streams and graph replays, on default and deterministic handles alike (the two give the same
+ * bits for the same options), and a sphere's rows do not depend on another sphere's x or v.
+ * Argument errors (nothing launched): a null workspace, x_dev, v_dev, terms or hv_out_dev, hv_out_dev equal to x_dev or
+ * v_dev (hv is written before x and v are read for the last time; partial overlaps are the caller's to avoid), the mode not
+ * enabled, an order other than 2 or 4, terms->c3 != 0 on a handle without enable_amips, a negative coefficient. */
+int tsb_pcg_enable_psd(tsb_pcg_t s, const float *rest_xyz, const int32_t *tets, int32_t nele);
+int tsb_pcg_hvp_psd(tsb_pcg_t s, const float *x_dev, const float *v_dev, const tsb_terms_t *terms, float *hv_out_dev,
+                    float *curv_out_dev, void *stream);
 
 /* ---- Damped Newton step: one Levenberg-Marquardt iteration per sphere on the device (no counterpart in the reference)
  * A Newton workspace sits beside a solver workspace (which must outlive it; creating one changes nothing about the

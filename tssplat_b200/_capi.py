@@ -23,6 +23,7 @@ EXPORTED_SYMBOLS = (
     "tsb_create", "tsb_destroy", "tsb_last_error", "tsb_get_info", "tsb_energy_grad", "tsb_energy_grad_ex", "tsb_energy_grad_spheres", "tsb_hvp", "tsb_hvp_ex",
     "tsb_line_search", "tsb_hess_diag", "tsb_pcg_create", "tsb_pcg_destroy", "tsb_pcg_last_error", "tsb_pcg_device_bytes",
     "tsb_pcg_set_blocks", "tsb_pcg_solve", "tsb_sphere_axpy", "tsb_pcg_set_blocks_ex", "tsb_pcg_solve_ex",
+    "tsb_pcg_enable_psd", "tsb_pcg_hvp_psd",
     "tsb_newton_create", "tsb_newton_destroy", "tsb_newton_last_error", "tsb_newton_device_bytes", "tsb_newton_reset",
     "tsb_newton_step", "tsb_newton_prox_step", "tsb_energy_grad_host", "tsb_scale",
     "tsb_grad_limit", "tsb_adam_uniform_step",
@@ -129,6 +130,10 @@ def _load() -> C.CDLL:
     lib.tsb_pcg_solve_ex.restype = C.c_int
     lib.tsb_pcg_solve_ex.argtypes = [vp, vp, vp, C.POINTER(tsb_terms_t), C.POINTER(tsb_pcg_options_t), vp, vp, vp,
                                      C.POINTER(C.c_int32), vp]
+    lib.tsb_pcg_enable_psd.restype = C.c_int
+    lib.tsb_pcg_enable_psd.argtypes = [vp, vp, vp, i32]
+    lib.tsb_pcg_hvp_psd.restype = C.c_int
+    lib.tsb_pcg_hvp_psd.argtypes = [vp, vp, vp, C.POINTER(tsb_terms_t), vp, vp, vp]
     lib.tsb_newton_create.restype = C.c_int
     lib.tsb_newton_create.argtypes = [vp, C.POINTER(vp)]
     lib.tsb_newton_destroy.restype = None

@@ -10,6 +10,7 @@
 #include "../../include/tssplat_b200.h"
 #include "tsb_kernels.cuh"
 #include "tsb_plan.h"
+#include "tsb_psd.cuh"
 #include "tsb_solver.cuh"
 
 static_assert(sizeof(tsb_sphere_stats_t) == 40, "tsb_sphere_stats_t must be 40 bytes");
@@ -46,6 +47,8 @@ struct tsb_pcg_s {
   int64_t device_bytes = 0;
   int32_t *active_host = nullptr;    // pinned: the "components still active" count of check_every > 0
   cudaEvent_t ev = nullptr;
+  bool psd = false;                  // tsb_pcg_enable_psd: the solve multiplies by the projected Hessian
+  tsb::PsdParams Q{};
   std::vector<void *> allocs;
   std::string err;
 };
@@ -560,6 +563,135 @@ int tsb_pcg_set_blocks_ex(tsb_pcg_t s, const float *diag_dev, float rel_floor, c
   return TSB_OK;
 }
 
+}  // extern "C"
+
+namespace {
+
+// The projection multiplies by c2 and c3, so it is only the projection of the weighted sum for weights >= 0
+int psd_check_terms(tsb_pcg_t s, const tsb_terms_t &t) {
+  if (!(t.c1 >= 0.f && t.c2 >= 0.f && t.c3 >= 0.f))
+    return pcg_fail(s, TSB_E_INVALID, "the projected Hessian needs c1, c2 and c3 >= 0 (projection does not commute with a negative weight)");
+  return TSB_OK;
+}
+
+// hv = c1 M v (the exact product with c2 = c3 = 0: its tet pass adds exact zeros) + c2 P(H_b) v + c3 P(H_a) v at the
+// workspace's last projection; curv (optional, device float[4]) as tsb_pcg_hvp_psd reports it
+int psd_product(tsb_pcg_t s, const float *x_dev, const float *v_dev, const tsb_terms_t &t, float *hv, float *curv,
+                cudaStream_t st) {
+  const int rc = hvp_impl(s->h, x_dev, v_dev, t.c1, 0.f, 0.f, t.order, 1.f, nullptr, hv, curv ? s->Q.curv_m : nullptr, 1, st);
+  if (rc != TSB_OK) return pcg_fail(s, rc, s->h->err);
+  cudaError_t e = tsb::launch_psd_apply(s->Q, v_dev, t.c2, t.c3, curv != nullptr, hv, st);
+  if (e == cudaSuccess && curv) e = tsb::launch_psd_curv(s->Q, t.c1, t.c2, t.c3, curv, st);
+  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("projected product launch: ") + cudaGetErrorString(e));
+  return TSB_OK;
+}
+
+int psd_project(tsb_pcg_t s, const float *x_dev, const tsb_terms_t &t, cudaStream_t st) {
+  const cudaError_t e = tsb::launch_psd_project(s->Q, x_dev, t.order, t.c3 != 0.f ? 1 : 0, st);
+  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("projection launch: ") + cudaGetErrorString(e));
+  return TSB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int tsb_pcg_enable_psd(tsb_pcg_t s, const float *rest_xyz, const int32_t *tets, int32_t nele) {
+  if (!s) return TSB_E_INVALID;
+  if (s->psd) return pcg_fail(s, TSB_E_INVALID, "the projected Hessian is already enabled on this workspace");
+  if (!rest_xyz || !tets) return pcg_fail(s, TSB_E_INVALID, "rest_xyz and tets must be non-null");
+  const tsb_handle_t h = s->h;
+  if (nele != h->info.nele)
+    return pcg_fail(s, TSB_E_INVALID, "nele = " + std::to_string(nele) + " but the handle has " + std::to_string(h->info.nele) + " tets");
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(cudaStreamLegacy, &cap) != cudaSuccess || cap != cudaStreamCaptureStatusNone) {
+    cudaGetLastError();
+    return pcg_fail(s, TSB_E_INVALID, "tsb_pcg_enable_psd allocates device memory and cannot run while a stream is being captured");
+  }
+  const int32_t n = h->info.n;
+  const size_t ne = size_t(nele);
+  // the mesh: every vertex in range, every tet inside one component, B = Dm^-1 in fp64 stored as fp32 (row-major, one
+  // array per entry)
+  std::vector<float> B(9 * ne);
+  std::vector<int32_t> cnt(size_t(n) + 1, 0);
+  for (size_t t = 0; t < ne; ++t) {
+    const int32_t *q = tets + 4 * t;
+    for (int k = 0; k < 4; ++k)
+      if (q[k] < 0 || q[k] >= n)
+        return pcg_fail(s, TSB_E_MESH, "tet " + std::to_string(t) + " has vertex " + std::to_string(q[k]) + " outside [0, " + std::to_string(n) + ")");
+    const int32_t c = h->comp_label[size_t(q[0])];
+    if (c < 0 || h->comp_label[size_t(q[1])] != c || h->comp_label[size_t(q[2])] != c || h->comp_label[size_t(q[3])] != c)
+      return pcg_fail(s, TSB_E_MESH, "tet " + std::to_string(t) + " spans two components of the handle: not the mesh it was created from");
+    double D[3][3];
+    for (int k = 0; k < 3; ++k)
+      for (int r = 0; r < 3; ++r)
+        D[r][k] = double(rest_xyz[3 * size_t(q[k + 1]) + r]) - double(rest_xyz[3 * size_t(q[0]) + r]);
+    const double c00 = D[1][1] * D[2][2] - D[1][2] * D[2][1], c01 = D[1][2] * D[2][0] - D[1][0] * D[2][2],
+                 c02 = D[1][0] * D[2][1] - D[1][1] * D[2][0];
+    const double det = D[0][0] * c00 + D[0][1] * c01 + D[0][2] * c02;
+    if (!(std::fabs(det) > 0.0) || !std::isfinite(det))
+      return pcg_fail(s, TSB_E_MESH, "tet " + std::to_string(t) + " has a zero-volume or non-finite rest shape");
+    const double inv[3][3] = {
+        {c00 / det, (D[0][2] * D[2][1] - D[0][1] * D[2][2]) / det, (D[0][1] * D[1][2] - D[0][2] * D[1][1]) / det},
+        {c01 / det, (D[0][0] * D[2][2] - D[0][2] * D[2][0]) / det, (D[0][2] * D[1][0] - D[0][0] * D[1][2]) / det},
+        {c02 / det, (D[0][1] * D[2][0] - D[0][0] * D[2][1]) / det, (D[0][0] * D[1][1] - D[0][1] * D[1][0]) / det}};
+    for (int k = 0; k < 9; ++k) B[size_t(k) * ne + t] = float(inv[k / 3][k % 3]);
+    for (int k = 0; k < 4; ++k) ++cnt[size_t(q[k]) + 1];
+  }
+  // per-vertex incidence lists of 4 tet + corner, ascending (a counting sort over ascending entries keeps the order)
+  for (size_t v = 0; v < size_t(n); ++v) cnt[v + 1] += cnt[v];
+  std::vector<int32_t> inc(4 * ne), fill(cnt.begin(), cnt.end() - 1);
+  for (size_t t = 0; t < ne; ++t)
+    for (int k = 0; k < 4; ++k) inc[size_t(fill[size_t(tets[4 * t + k])]++)] = int32_t(4 * t + k);
+  tsb::PsdParams Q{};
+  Q.nele = nele; Q.n = n; Q.n_blocks = int32_t((ne + tsb::kPsdT - 1) / tsb::kPsdT);
+  const size_t allocs0 = s->allocs.size();
+  const int64_t bytes0 = s->device_bytes;
+  int32_t *tets_dev = nullptr, *inc_ptr = nullptr, *inc_dev = nullptr;
+  float *B_dev = nullptr;
+  int rc = ws_alloc(s, 4 * ne, tets, &tets_dev);
+  if (rc == TSB_OK) rc = ws_alloc(s, 9 * ne, B.data(), &B_dev);
+  if (rc == TSB_OK) rc = ws_alloc<float>(s, tsb::kPsdOpFloats * ne, nullptr, &Q.op);
+  if (rc == TSB_OK) rc = ws_alloc<uint8_t>(s, ne, nullptr, &Q.kind);
+  if (rc == TSB_OK) rc = ws_alloc<float>(s, 12 * ne, nullptr, &Q.corner);
+  if (rc == TSB_OK) rc = ws_alloc(s, cnt.size(), cnt.data(), &inc_ptr);
+  if (rc == TSB_OK) rc = ws_alloc(s, inc.size(), inc.data(), &inc_dev);
+  if (rc == TSB_OK) rc = ws_alloc<double>(s, 2 * size_t(Q.n_blocks), nullptr, &Q.part);
+  if (rc == TSB_OK) rc = ws_alloc<float>(s, 4, nullptr, &Q.curv_m);
+  if (rc != TSB_OK) {            // leave the workspace as it was
+    for (size_t k = allocs0; k < s->allocs.size(); ++k) cudaFree(s->allocs[k]);
+    s->allocs.resize(allocs0);
+    s->device_bytes = bytes0;
+    return rc;
+  }
+  Q.tets = reinterpret_cast<const int4 *>(tets_dev); Q.B = B_dev; Q.inc_ptr = inc_ptr; Q.inc = inc_dev;
+  s->Q = Q;
+  s->psd = true;
+  return TSB_OK;
+}
+
+int tsb_pcg_hvp_psd(tsb_pcg_t s, const float *x_dev, const float *v_dev, const tsb_terms_t *terms, float *hv_out_dev,
+                    float *curv_out_dev, void *stream) {
+  if (!s) return TSB_E_INVALID;
+  if (!s->psd) return pcg_fail(s, TSB_E_INVALID, "tsb_pcg_hvp_psd needs a workspace after tsb_pcg_enable_psd");
+  if (!x_dev || !v_dev || !terms || !hv_out_dev) return pcg_fail(s, TSB_E_INVALID, "x_dev, v_dev, terms and hv_out_dev must be non-null");
+  if (hv_out_dev == v_dev || hv_out_dev == x_dev)
+    return pcg_fail(s, TSB_E_INVALID, "hv_out_dev must not be x_dev or v_dev: hv is written before v and x are read for the last time");
+  if (terms->order != 2 && terms->order != 4) return pcg_fail(s, TSB_E_INVALID, "order must be 2 or 4");
+  if (terms->c3 != 0.f && !s->h->amips)
+    return pcg_fail(s, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
+  int rc = psd_check_terms(s, *terms);
+  if (rc != TSB_OK) return rc;
+  DeviceGuard guard(s->h->device);
+  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  rc = psd_project(s, x_dev, *terms, st);
+  if (rc == TSB_OK) rc = psd_product(s, x_dev, v_dev, *terms, hv_out_dev, curv_out_dev, st);
+  return rc;
+}
+
 int tsb_pcg_solve(tsb_pcg_t s, const float *x_dev, const float *b_dev, const tsb_terms_t *terms, const tsb_pcg_options_t *opt,
                   float *d_out_dev, tsb_pcg_sphere_t *spheres_out_dev, int32_t *iters_run_out, void *stream) {
   return tsb_pcg_solve_ex(s, x_dev, b_dev, terms, opt, nullptr, d_out_dev, spheres_out_dev, iters_run_out, stream);
@@ -577,6 +709,10 @@ int tsb_pcg_solve_ex(tsb_pcg_t s, const float *x_dev, const float *b_dev, const 
   if (terms->order != 2 && terms->order != 4) return pcg_fail(s, TSB_E_INVALID, "order must be 2 or 4");
   if (terms->c3 != 0.f && !s->h->amips)
     return pcg_fail(s, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
+  if (s->psd) {
+    const int rc = psd_check_terms(s, *terms);
+    if (rc != TSB_OK) return rc;
+  }
   DeviceGuard guard(s->h->device);
   if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -587,12 +723,21 @@ int tsb_pcg_solve_ex(tsb_pcg_t s, const float *x_dev, const float *b_dev, const 
       return pcg_fail(s, TSB_E_INVALID, "check_every > 0 reads the host and cannot be captured in a CUDA graph: use check_every = 0");
   }
   const tsb::PcgParams &P = s->P;
+  if (s->psd) {                        // x does not change during the solve: one projection
+    const int rc = psd_project(s, x_dev, *terms, st);
+    if (rc != TSB_OK) return rc;
+  }
   cudaError_t e = tsb::launch_pcg_begin(P, b_dev, d_out_dev, st);
   if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver launch: ") + cudaGetErrorString(e));
   int32_t it = 0;
   while (it < opt->max_iter) {
-    const int rc = hvp_impl(s->h, x_dev, P.p, terms->c1, terms->c2, terms->c3, terms->order, 1.f, nullptr, P.Hp, nullptr, 1, st);
-    if (rc != TSB_OK) return pcg_fail(s, rc, s->h->err);
+    if (s->psd) {
+      const int rc = psd_product(s, x_dev, P.p, *terms, P.Hp, nullptr, st);
+      if (rc != TSB_OK) return rc;
+    } else {
+      const int rc = hvp_impl(s->h, x_dev, P.p, terms->c1, terms->c2, terms->c3, terms->order, 1.f, nullptr, P.Hp, nullptr, 1, st);
+      if (rc != TSB_OK) return pcg_fail(s, rc, s->h->err);
+    }
     e = tsb::launch_pcg_step(P, d_out_dev, it, opt->rtol, shift_dev, st);
     if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver launch: ") + cudaGetErrorString(e));
     ++it;
@@ -706,6 +851,8 @@ int newton_check(tsb_newton_t nw, const float *x_dev, const tsb_terms_t *terms, 
   if (terms->order != 2 && terms->order != 4) return newton_fail(nw, TSB_E_INVALID, "order must be 2 or 4");
   if (terms->c3 != 0.f && !nw->s->h->amips)
     return newton_fail(nw, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
+  if (nw->s->psd && !(terms->c1 >= 0.f && terms->c2 >= 0.f && terms->c3 >= 0.f))
+    return newton_fail(nw, TSB_E_INVALID, "the projected Hessian needs c1, c2 and c3 >= 0 (projection does not commute with a negative weight)");
   return TSB_OK;
 }
 

@@ -8,6 +8,7 @@
 // component's partials itself, in chunk order, from a column of the partial table that no CTA of that kernel writes.
 // The fold is redundant across the chunks of a component, but it needs no ticket, no atomic and no fence, and every
 // chunk gets bitwise the same scalar.  All scalars stay in device memory.
+#include "tsb_jacobi.cuh"
 #include "tsb_solver.cuh"
 
 namespace tsb {
@@ -60,23 +61,6 @@ __device__ __forceinline__ F3 apply_block(const float *pinv, int v, F3 r) {
   const float xx = q[0], yy = q[1], zz = q[2], yz = q[3], xz = q[4], xy = q[5];
   return F3{xx * r.x + xy * r.y + xz * r.z, xy * r.x + yy * r.y + yz * r.z, xz * r.x + yz * r.y + zz * r.z};
 }
-
-// One Jacobi rotation of a symmetric 3x3 matrix that zeroes a_pq; r is the third index, (v?p, v?q) are columns p and q
-// of the eigenvector matrix.
-__device__ __forceinline__ void jacobi_rot(double &app, double &aqq, double &apq, double &apr, double &aqr, double &v0p,
-                                           double &v0q, double &v1p, double &v1q, double &v2p, double &v2q) {
-  if (apq == 0.0) return;
-  const double theta = (aqq - app) / (2.0 * apq);
-  const double t = copysign(1.0, theta) / (fabs(theta) + sqrt(theta * theta + 1.0));
-  const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
-  app -= t * apq; aqq += t * apq; apq = 0.0;
-  double a = c * apr - s * aqr; aqr = s * apr + c * aqr; apr = a;
-  a = c * v0p - s * v0q; v0q = s * v0p + c * v0q; v0p = a;
-  a = c * v1p - s * v1q; v1q = s * v1p + c * v1q; v1p = a;
-  a = c * v2p - s * v2q; v2q = s * v2p + c * v2q; v2p = a;
-}
-
-constexpr int kJacobiSweeps = 8;
 
 // Inverse preconditioner block of vertex v: cyclic Jacobi eigen-decomposition in fp64 registers, eigenvalues clamped
 // from below to rel_floor * lambda_max, block inverted; lambda_max <= 0 gives the zero block.  diag == nullptr: the

@@ -144,7 +144,9 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
     term, ``c1 * smooth + c2 * barrier + amips_coeff * amips``.  The coefficient is a constant (the scheduler's
     multiplier applies to the reference's two terms only); ``forward`` then goes through ``SmoothnessBarrierAmipsFunc``
     (one fused launch, twice differentiable under ``twice_differentiable``), and ``hvp`` and ``sphere_stats`` include
-    the term.  With ``amips_coeff`` absent or 0 nothing changes.
+    the term.  With ``amips_coeff`` absent or 0 nothing changes.  ``newton_hessian`` (default ``"exact"``) selects the
+    model of ``device_pcg``, which ``newton_direction``, ``newton_step`` and ``prox_step`` solve with: ``"psd"`` is the
+    projected Hessian (``newton.DevicePCG``).
     """
 
     #: the AMIPS coefficient; a class default, so that a module assembled without ``__init__`` (as ``bench.py`` does)
@@ -208,6 +210,13 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         c1, c2 = self.coeff_scheduler(it)
         return self.tet_sp.hess_diag(x.detach(), c1, c2, self.order_at(it), c3=self.amips_coeff)
 
+    def _device_pcg(self):
+        from .newton import DevicePCG
+        pcg = getattr(self, "device_pcg", None)
+        if pcg is None:
+            pcg = self.device_pcg = DevicePCG(self.tet_sp, hessian=getattr(self.FLAGS, "newton_hessian", "exact") or "exact")
+        return pcg
+
     def newton_direction(self, x, it, b=None, **solve_kw):
         """A Newton direction per sphere, on the device without a host sync: ``hess_diag`` -> block-Jacobi preconditioner
         -> ``tssplat_b200.newton.DevicePCG.solve`` of ``H(x) d = b`` with the scheduler's coefficients, the barrier order
@@ -215,10 +224,7 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         ``max_iter``, ``rtol``, ``check_every``.  Returns a ``DevicePCGResult`` (its ``b_dot_d`` is what a per-sphere
         Armijo test needs); the workspace, ``self.device_pcg`` (its ``axpy`` takes the per-sphere step), is created on
         first use."""
-        from .newton import DevicePCG
-        pcg = getattr(self, "device_pcg", None)
-        if pcg is None:
-            pcg = self.device_pcg = DevicePCG(self.tet_sp)
+        pcg = self._device_pcg()
         c1, c2 = self.coeff_scheduler(it)
         order, xd = self.order_at(it), x.detach()
         if b is None:
@@ -228,13 +234,10 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         return pcg.solve(xd, b.detach(), c1, c2, order, c3=self.amips_coeff, **solve_kw)
 
     def _device_newton(self):
-        from .newton import DeviceNewton, DevicePCG
+        from .newton import DeviceNewton
         nw = getattr(self, "device_newton", None)
         if nw is None:
-            pcg = getattr(self, "device_pcg", None)
-            if pcg is None:
-                pcg = self.device_pcg = DevicePCG(self.tet_sp)
-            nw = self.device_newton = DeviceNewton(self.tet_sp, pcg)
+            nw = self.device_newton = DeviceNewton(self.tet_sp, self._device_pcg())
         return nw
 
     def newton_step(self, x, it, **opts):

@@ -9,7 +9,9 @@ from these and ``TetSpheres.line_search``.
 ``DevicePCG`` is the device-resident solver (``tsb_pcg_solve``): the same truncated PCG, but run independently on every
 tet-sphere (the Hessian is block diagonal by sphere) with all scalars in device memory, so there is no host read inside
 an iteration and the solve can be captured in a CUDA graph.  ``pcg`` below stays as the reference implementation.
-With a per-sphere ``shift`` it solves ``(H + mu_c I) d = b`` (``tsb_pcg_solve_ex``).
+With a per-sphere ``shift`` it solves ``(H + mu_c I) d = b`` (``tsb_pcg_solve_ex``).  ``DevicePCG(tet_sp, hessian="psd")``
+multiplies by the projected Hessian instead (``tsb_pcg_enable_psd``): every tet's Hessian replaced by its positive
+semidefinite projection, so the solve never stops at negative curvature from the tet terms.
 
 ``DeviceNewton`` joins the pieces into a minimiser (``tsb_newton_step``): one damped (Levenberg-Marquardt) Newton step per
 sphere per call -- gradient, diagonal blocks, shifted solve, line search, step choice and damping update -- on one
@@ -25,7 +27,7 @@ from typing import Callable, NamedTuple, Optional, Union
 import torch
 
 __all__ = ["hess_blocks", "block_jacobi", "apply_blocks", "pcg", "PCGResult", "DevicePCG", "DevicePCGResult", "DeviceNewton",
-           "NewtonStepResult", "NEWTON_DEFAULTS"]
+           "NewtonStepResult", "NEWTON_DEFAULTS", "HESSIANS"]
 
 
 def hess_blocks(planes: torch.Tensor) -> torch.Tensor:
@@ -129,22 +131,34 @@ class DevicePCGResult(NamedTuple):
     iters_run: int                  # iterations enqueued (= max_iter with check_every = 0)
 
 
+HESSIANS = ("exact", "psd")
+
+
 class DevicePCG:
     """Per-sphere block-Jacobi PCG workspace of one ``TetSpheres`` handle (``tsb_pcg_create``), which it keeps alive.
-    Serves one stream at a time, like the handle."""
+    Serves one stream at a time, like the handle.  ``hessian="psd"`` enables the projected Hessian on it
+    (``tsb_pcg_enable_psd``, from the mesh the handle keeps): ``solve`` and every ``DeviceNewton`` step over this workspace
+    then multiply by ``H+``, and ``hvp_psd`` is available.  Creating it allocates, so not inside a CUDA graph capture."""
 
-    def __init__(self, tet_sp):
+    def __init__(self, tet_sp, hessian: str = "exact"):
         from . import _capi
         from .tet_spheres_ext import _stream_ptr
         self._capi, self._stream_ptr = _capi, _stream_ptr
         self._s = None
-        self.tet_sp = tet_sp
+        if hessian not in HESSIANS:
+            raise ValueError(f"hessian must be one of {HESSIANS}, got {hessian!r}")
+        if hessian == "psd" and torch.cuda.is_current_stream_capturing():
+            raise RuntimeError('DevicePCG(hessian="psd") allocates device memory and cannot be created during a CUDA graph capture')
+        self.tet_sp, self.hessian = tet_sp, hessian
         s = C.c_void_p()
         rc = _capi.lib.tsb_pcg_create(tet_sp._h, C.byref(s))
         if rc:
             raise RuntimeError(f"DevicePCG: {self._error(None)} (code {rc})")
         self._s = s
         self.n_spheres = int(tet_sp.info["n_components"])
+        if hessian == "psd":
+            rc = _capi.lib.tsb_pcg_enable_psd(s, tet_sp.vertices.ctypes.data, tet_sp.elements.ctypes.data, int(tet_sp.nele))
+            self._check(rc, "__init__")
         self.device_bytes = int(_capi.lib.tsb_pcg_device_bytes(s))
 
     def __del__(self):
@@ -215,6 +229,22 @@ class DevicePCG:
         f = raw.view(torch.float32)
         return DevicePCGResult(d, raw[:, 4], raw[:, 3], f[:, 0], f[:, 1], f[:, 2], int(iters.value))
 
+    def hvp_psd(self, x: torch.Tensor, v: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0):
+        """``H+(x) v`` of ``c1 * smooth + c2 * barrier (+ c3 * amips)`` with every tet's Hessian projected to PSD at ``x``
+        (``tsb_pcg_hvp_psd``; needs ``hessian="psd"``), in ``v``'s shape, and the curvature record, a float32 CUDA
+        tensor ``[c1 vMv + c2 vHb+v + c3 vHa+v, vMv, vHb+v, vHa+v]``.  Coefficients must be >= 0.  No host sync."""
+        if self.hessian != "psd":
+            raise RuntimeError('DevicePCG.hvp_psd needs a workspace created with hessian="psd"')
+        n3, dev = self.tet_sp.n3, self.tet_sp.device
+        xc, vc = self._f32(x, n3, "x"), self._f32(v, n3, "v")
+        hv = torch.empty_like(vc)
+        curv = torch.empty(4, dtype=torch.float32, device=dev)
+        terms = self._capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
+        rc = self._capi.lib.tsb_pcg_hvp_psd(self._s, xc.data_ptr(), vc.data_ptr(), C.byref(terms), hv.data_ptr(), curv.data_ptr(),
+                                            self._stream_ptr(dev))
+        self._check(rc, "hvp_psd")
+        return hv.reshape(v.shape), curv
+
     def axpy(self, x: torch.Tensor, a_sphere: torch.Tensor, d: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``x + a_sphere[sphere of v] * d`` per vertex (``tsb_sphere_axpy``), in ``x``'s shape; vertices no tet
         references are copied.  ``out`` may be ``x`` (in place)."""
@@ -254,17 +284,24 @@ class NewtonStepResult(NamedTuple):
 class DeviceNewton:
     """Damped Newton workspace (``tsb_newton_create``) of one ``TetSpheres`` handle: reuses ``pcg`` (a ``DevicePCG`` of
     the same handle) or creates one, and keeps it alive.  Every sphere runs its own Levenberg-Marquardt iteration;
-    ``reset`` starts them all again.  Serves one stream at a time, like the handle."""
+    ``reset`` starts them all again.  Serves one stream at a time, like the handle.  ``hessian``: the solve's model,
+    ``"exact"`` or ``"psd"`` (the projected Hessian, see ``DevicePCG``); ``None`` takes ``pcg``'s, or ``"exact"`` when a
+    workspace is created.  A given ``pcg`` of another mode is an error."""
 
-    def __init__(self, tet_sp, pcg: Optional[DevicePCG] = None):
+    def __init__(self, tet_sp, pcg: Optional[DevicePCG] = None, hessian: Optional[str] = None):
         from . import _capi
         from .tet_spheres_ext import _stream_ptr
         self._capi, self._stream_ptr = _capi, _stream_ptr
         self._nw = None
+        if hessian is not None and hessian not in HESSIANS:
+            raise ValueError(f"hessian must be one of {HESSIANS}, got {hessian!r}")
         if pcg is None:
-            pcg = DevicePCG(tet_sp)
+            pcg = DevicePCG(tet_sp, hessian=hessian or "exact")
         elif pcg.tet_sp is not tet_sp:
             raise RuntimeError("DeviceNewton: pcg belongs to another handle")
+        elif hessian is not None and pcg.hessian != hessian:
+            raise RuntimeError(f"DeviceNewton: hessian={hessian!r} but pcg was created with hessian={pcg.hessian!r}")
+        self.hessian = pcg.hessian
         self.tet_sp, self.pcg, self.n_spheres = tet_sp, pcg, pcg.n_spheres
         nw = C.c_void_p()
         rc = _capi.lib.tsb_newton_create(pcg._s, C.byref(nw))

@@ -125,6 +125,9 @@ class TetSpheres:
                                   elements.size // 4, C.byref(opt), self.device.index, C.byref(h))
         _capi.check(rc, None, "TetSpheres")
         self._h = h
+        # copies of the mesh the handle was built from (flat float32 rest positions, flat int32 tets), so that a caller
+        # changing its arrays later does not change what DevicePCG(hessian="psd") hands to tsb_pcg_enable_psd
+        self.vertices, self.elements = vertices.copy(), elements.copy()
         info = _capi.tsb_info_t()
         _capi.check(_capi.lib.tsb_get_info(self._h, C.byref(info)), self._h, "TetSpheres")
         self.info = {k: getattr(info, k) for k, _ in _capi.tsb_info_t._fields_}
