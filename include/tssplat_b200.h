@@ -20,7 +20,7 @@
 extern "C" {
 #endif
 
-#define TSB_VERSION 10
+#define TSB_VERSION 11
 #define TSB_LINE_MAX_ALPHA 8   /* step sizes one tsb_line_search call may evaluate */
 
 enum {
@@ -270,7 +270,10 @@ enum {
   TSB_PCG_CONVERGED = 1,      /* |r_c| <= rtol |b_c|                                                    */
   TSB_PCG_NEGCURV = 2,        /* p^T H p <= 0 at a later direction: d_c is the iterate reached before it */
   TSB_PCG_NEGCURV_FIRST = 3,  /* p^T H p <= 0 at the first direction: d_c = P b_c                        */
-  TSB_PCG_ZERO_RHS = 4        /* |b_c| = 0: d_c = 0                                                      */
+  TSB_PCG_ZERO_RHS = 4,       /* |b_c| = 0: d_c = 0                                                      */
+  TSB_PCG_BOUNDARY = 5,       /* tsb_pcg_solve_tr only: the next iterate would leave the radius; d_c on the boundary */
+  TSB_PCG_NEGCURV_BOUNDARY = 6 /* tsb_pcg_solve_tr only: p^T H p <= 0, followed to the boundary (tau P b_c at the first
+                                 direction)                                                                         */
 };
 
 typedef struct {
@@ -339,6 +342,32 @@ int tsb_pcg_solve_ex(tsb_pcg_t s, const float *x_dev, const float *b_dev, const 
                      const tsb_pcg_options_t *opt, const float *shift_dev, float *d_out_dev,
                      tsb_pcg_sphere_t *spheres_out_dev, int32_t *iters_run_out, void *stream);
 
+/* ---- Trust-region solve (Steihaug-Toint CG) ------------------------------------------------------------------------
+ * Solves (H(x) + shift_c I) d = b_c on every component with tsb_pcg_solve_ex's algorithm, options, preconditioner, rules
+ * and records (shift_dev may be NULL), inside a per-component radius: |d_c|_M <= Delta_c in the preconditioner norm
+ * |v|_M^2 = v^T P^-1 v, P the clamped inverse blocks of tsb_pcg_set_blocks(_ex) (the norm in which the CG iterates'
+ * length grows monotonically, so the first crossing is the one to stop at).  radius_dev: device float32
+ * [info.n_components], Delta_c in component order, read on the device (+inf: no radius; NaN or <= 0: radius 0, d_c = 0).
+ * Per component, in fp64 and without an extra vector pass, the lead CTA keeps
+ *   pMp_0 = r.z,  dMp_0 = dMd_0 = 0;  after a step s along p: dMd += 2 s dMp + s^2 pMp, and then
+ *   dMp = beta (dMp + s pMp),  pMp = r.z + beta^2 pMp
+ * and with tau >= 0 solving |d + tau p|_M = Delta, formed as (Delta^2 - dMd) / (dMp + sqrt(dMp^2 + pMp (Delta^2 - dMd))):
+ *   p^T (H + shift) p <= 0:                    d += tau p, NEGCURV_BOUNDARY (tau P b_c at the first direction);
+ *   else dMd + 2 alpha dMp + alpha^2 pMp >= Delta^2:  d += tau p, BOUNDARY;
+ * d_H_d then gains tau^2 p^T (H + shift) p (d^T H p = 0 by conjugacy) and rel_residual is that of the iterate before the
+ * boundary step.  With Delta_c = +inf every component's d and record is bitwise that of tsb_pcg_solve_ex, negative
+ * curvature included (NEGCURV, NEGCURV_FIRST).  The solve's invariants hold: one writing kernel per field, no launch reads
+ * what another CTA of it writes, no floating-point atomics, folds in a fixed order; check_every and the projected Hessian
+ * (tsb_pcg_enable_psd) work as in tsb_pcg_solve_ex.
+ * The first call on a workspace allocates the recurrence state, 32 bytes per component, with cudaMalloc;
+ * tsb_pcg_device_bytes includes it from then on, and a workspace that never takes a trust-region solve keeps its size.
+ * Make that first call outside any stream capture: on a stream being captured it returns TSB_E_INVALID, and a cudaMalloc
+ * while another stream of the process is being captured in global mode invalidates that capture.
+ * Argument errors (TSB_E_INVALID, nothing launched): those of tsb_pcg_solve_ex and a null radius_dev. */
+int tsb_pcg_solve_tr(tsb_pcg_t s, const float *x_dev, const float *b_dev, const tsb_terms_t *terms,
+                     const tsb_pcg_options_t *opt, const float *shift_dev, const float *radius_dev, float *d_out_dev,
+                     tsb_pcg_sphere_t *spheres_out_dev, int32_t *iters_run_out, void *stream);
+
 /* ---- Projected Hessian (projected Newton) ---------------------------------------------------------------------------
  * Opt-in on a solver workspace: every tet's Hessian in deformation-gradient space is replaced by its positive
  * semidefinite projection (same eigenvectors, negative eigenvalues clamped to 0), so the solve multiplies by
@@ -394,7 +423,8 @@ int tsb_pcg_hvp_psd(tsb_pcg_t s, const float *x_dev, const float *v_dev, const t
  * whether mu is initialised), three fp64 partials per chunk and the per-sphere step sizes.  Device memory, reported by
  * tsb_newton_device_bytes:
  *   48 n + 24 chunks + 172 n_components + 176   bytes
- * (chunks as for tsb_pcg_device_bytes), plus 8 max(chunks, 1) bytes once a tsb_newton_prox_step has been made.  A
+ * (chunks as for tsb_pcg_device_bytes), plus 8 max(chunks, 1) bytes once a tsb_newton_prox_step (or a proximal
+ * tsb_newton_tr_step) has been made and 20 n_components bytes once a tsb_newton_tr_step has been made.  A
  * new workspace is reset (every sphere ACTIVE, mu not initialised).  Like the handle and the solver workspace it serves
  * one stream at a time, and it shares the solver workspace's scratch. */
 typedef struct tsb_newton_s *tsb_newton_t;
@@ -403,7 +433,8 @@ void tsb_newton_destroy(tsb_newton_t nw);
 const char *tsb_newton_last_error(tsb_newton_t nw);   /* nw may be NULL: last tsb_newton_create failure */
 int64_t tsb_newton_device_bytes(tsb_newton_t nw);
 
-/* Marks every sphere ACTIVE with mu not initialised (one memset on the stream; capturable). */
+/* Marks every sphere ACTIVE with mu not initialised (one memset on the stream; capturable); after a tsb_newton_tr_step
+ * also the trust-region radius (a second memset). */
 int tsb_newton_reset(tsb_newton_t nw, void *stream);
 
 enum {
@@ -500,6 +531,72 @@ int tsb_newton_step(tsb_newton_t nw, float *x_dev, const tsb_terms_t *terms, con
 int tsb_newton_prox_step(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const float *weight_dev,
                          const tsb_terms_t *terms, const tsb_newton_options_t *opt,
                          tsb_newton_sphere_t *records_out_dev, void *stream);
+
+/* ---- Trust-region Newton step: one per-sphere trust-region iteration on the device ---------------------------------
+ * Minimises E (anchor_dev = weight_dev = NULL) or the proximal objective Phi_c = E_c + (w_c / 2)|x_c - y_c|^2 (both set,
+ * with tsb_newton_prox_step's semantics for the right-hand side, the d.(x - y) partials and an unusable weight) by a
+ * trust-region step per sphere: no damping shift, but a radius Delta_c in the preconditioner norm inside which
+ * tsb_pcg_solve_tr follows negative curvature to the boundary instead of stopping.  On one stream, without any host read
+ * (capturable in a CUDA graph after the first call):
+ *   1. b = -grad (prox: b -= w (x - y)); b_c = 0 on frozen spheres;  2. tsb_hess_diag;
+ *   3. tsb_pcg_set_blocks_ex with shift w_c (prox) or none;
+ *   4. on a sphere's first step after a reset, Delta_c = clamp(radius_init sqrt(b_c^T P b_c), radius_min, radius_max) (fp64);
+ *   5. tsb_pcg_solve_tr with fp32(Delta_c) and shift w_c (prox) or none;  6. per sphere b.d and |d|^2 (and d.(x - y));
+ *   7. tsb_line_search at the single step alpha = 1, per sphere;  8. the decision below;  9. tsb_sphere_axpy in place.
+ * Decision per sphere c, in fp64, with g = |b_c|, bd and dHd the solve's b.d and d^T (H + w_c I) d rounded to fp32 as
+ * tsb_pcg_sphere_t reports them, dMd = |d_c|_M^2 from the solve's recurrences, dPhi = Phi_c(x + d) - Phi_c(x) (dE for the
+ * plain objective) and alpha^ the inversion-free step over (0, 1] from the line search:
+ *   frozen: alpha = 0.  g <= gtol: CONVERGED, frozen.
+ *   pred = bd - dHd / 2;  rho = -dPhi / pred if pred > 0, else 0 (the step is rejected).
+ *   1 >= eta alpha^ (the full step would invert a tet): rejected, Delta = min(Delta / 4, eta alpha^ sqrt(dMd));
+ *   else rho < 1/4 (or NaN): Delta = sqrt(dMd) / 4;  else rho > 3/4 on a BOUNDARY or NEGCURV_BOUNDARY solve:
+ *   Delta = min(2 Delta, radius_max).
+ *   accepted (alpha = 1) iff pred > 0, rho > accept and no tet inverts; rejected with Delta < radius_min: STALLED, frozen.
+ * records_out_dev (optional, device [info.n_components]) receives one tsb_newton_tr_sphere_t per sphere.  No floating-point
+ * atomics in the new kernels and every fold in a fixed order: on a deterministic handle x and the records are bitwise
+ * identical across calls, streams and graph replays, and a sphere's trajectory depends on its own start, anchor and
+ * weight only.  Vertices no tet references never move.
+ * State: the radius and its init flag, 16 bytes per sphere, plus the fp32 radius, 4 bytes per sphere, allocated with the
+ * solve's recurrence state (tsb_pcg_solve_tr) and, for the proximal objective, tsb_newton_prox_step's partials, by the
+ * first call; tsb_newton_device_bytes grows by 20 n_components (+ 8 max(chunks, 1) if no proximal step was made yet) and
+ * tsb_newton_reset re-arms the radius.  Make the first call outside any stream capture: on a stream being captured it
+ * returns TSB_E_INVALID.
+ * Argument errors (TSB_E_INVALID, nothing launched): a null nw, x_dev, terms or opt, exactly one of anchor_dev and
+ * weight_dev null, anchor_dev == x_dev, an option outside its range (NaN included), nonzero reserved words, an order other
+ * than 2 or 4, terms->c3 != 0 on a handle without enable_amips, a negative coefficient on a projected-Hessian workspace.
+ * DESIGN.md section 5, "Trust-region Newton step". */
+typedef struct {            /* 64 bytes */
+  int32_t max_iter;         /* >= 1: the solve enqueues exactly max_iter iterations (check_every = 0)                   */
+  float rtol;               /* >= 0: the solve's residual test                                                       */
+  float rel_floor;          /* >= 0: the preconditioner's eigenvalue floor (tsb_pcg_set_blocks)                      */
+  float gtol;               /* >= 0: a sphere with |grad_c| <= gtol is CONVERGED                                     */
+  float radius_init;        /* > 0, finite: Delta_c = radius_init |b_c|_P on a first step, clamped                   */
+  float radius_min;         /* 0 < radius_min <= radius_max < inf: a rejected step with Delta_c < radius_min STALLS  */
+  float radius_max;
+  float accept;             /* in [0, 1/4): a step is accepted when rho > accept (1e-4 is the usual choice)           */
+  float eta;                /* in (0, 1]: the full step must lie below eta times the sphere's inversion-free step    */
+  int32_t reserved[7];      /* must be 0                                                                             */
+} tsb_newton_tr_options_t;
+
+typedef struct {            /* one per component, component order of tsb_energy_grad_spheres; 64 bytes               */
+  double radius;            /* Delta_c after this step's update                                                      */
+  double rho;               /* -dPhi / pred (0 when pred <= 0 or no decision ran)                                    */
+  float grad_norm;          /* |grad_c| at x before the step (0 on a sphere already frozen)                          */
+  float alpha;              /* 1: the step was taken, 0: not                                                          */
+  float delta;              /* Phi_c(x + d) - Phi_c(x) of the step taken (0 if none)                                 */
+  float b_dot_d;            /* b_c . d_c, b = -grad                                                                   */
+  float pred;               /* bd - dHd / 2, the model decrease (0 when no decision ran)                               */
+  float d_norm;             /* |d_c|_M = sqrt(dMd)                                                                    */
+  int32_t pcg_status;       /* TSB_PCG_* of the trust-region solve                                                    */
+  int32_t n_hvp;            /* products in which the sphere was active in the solve                                  */
+  int32_t status;           /* TSB_NEWTON_* after the step                                                           */
+  int32_t first_vertex;     /* its lowest vertex id                                                                  */
+  int32_t reserved[2];
+} tsb_newton_tr_sphere_t;
+
+int tsb_newton_tr_step(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const float *weight_dev,
+                       const tsb_terms_t *terms, const tsb_newton_tr_options_t *opt,
+                       tsb_newton_tr_sphere_t *records_out_dev, void *stream);
 
 /* Same computation for callers whose vertex positions live in HOST memory (e.g. a CPU-side
  * optimiser): copies x_host -> device, runs the fused launch, copies energy[3] and grad back,

@@ -69,4 +69,13 @@ if not big:
     r = nw.step(x, 2e-4, 3e-4, 2, c3=1e-4, max_iter=5)
     torch.cuda.synchronize()
     print("newton step ok", r.status.tolist(), r.alpha.tolist())
+    # one trust-region step, proximal then plain: the radius kernels, the trust-region solve's update and direction
+    # kernels (shifted, then unshifted) and the decision kernels
+    nw.reset()
+    r = nw.tr_step(x, 2e-4, 3e-4, 2, c3=1e-4, anchor=y, weight=w, max_iter=5)
+    torch.cuda.synchronize()
+    print("prox tr step ok", r.status.tolist(), r.alpha.tolist(), r.pcg_status.tolist())
+    r = nw.tr_step(x, 2e-4, 3e-4, 2, c3=1e-4, max_iter=5)
+    torch.cuda.synchronize()
+    print("tr step ok", r.status.tolist(), r.alpha.tolist(), r.pcg_status.tolist())
 print("DONE")

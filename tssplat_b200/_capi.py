@@ -16,6 +16,7 @@ LIB_PATH = os.environ.get("TSSPLAT_B200_LIB") or _build.LIB_PATH
 TSB_OK, TSB_E_INVALID, TSB_E_MESH, TSB_E_CUDA, TSB_E_NOMEM = 0, -1, -2, -3, -4
 TSB_LINE_MAX_ALPHA = 8
 TSB_PCG_MAXITER, TSB_PCG_CONVERGED, TSB_PCG_NEGCURV, TSB_PCG_NEGCURV_FIRST, TSB_PCG_ZERO_RHS = 0, 1, 2, 3, 4
+TSB_PCG_BOUNDARY, TSB_PCG_NEGCURV_BOUNDARY = 5, 6
 TSB_NEWTON_ACTIVE, TSB_NEWTON_CONVERGED, TSB_NEWTON_STALLED = 0, 1, 2
 
 # every symbol include/tssplat_b200.h declares (tests check the library exports each one)
@@ -23,9 +24,9 @@ EXPORTED_SYMBOLS = (
     "tsb_create", "tsb_destroy", "tsb_last_error", "tsb_get_info", "tsb_energy_grad", "tsb_energy_grad_ex", "tsb_energy_grad_spheres", "tsb_hvp", "tsb_hvp_ex",
     "tsb_line_search", "tsb_hess_diag", "tsb_pcg_create", "tsb_pcg_destroy", "tsb_pcg_last_error", "tsb_pcg_device_bytes",
     "tsb_pcg_set_blocks", "tsb_pcg_solve", "tsb_sphere_axpy", "tsb_pcg_set_blocks_ex", "tsb_pcg_solve_ex",
-    "tsb_pcg_enable_psd", "tsb_pcg_hvp_psd",
+    "tsb_pcg_enable_psd", "tsb_pcg_hvp_psd", "tsb_pcg_solve_tr",
     "tsb_newton_create", "tsb_newton_destroy", "tsb_newton_last_error", "tsb_newton_device_bytes", "tsb_newton_reset",
-    "tsb_newton_step", "tsb_newton_prox_step", "tsb_energy_grad_host", "tsb_scale",
+    "tsb_newton_step", "tsb_newton_prox_step", "tsb_newton_tr_step", "tsb_energy_grad_host", "tsb_scale",
     "tsb_grad_limit", "tsb_adam_uniform_step",
     "tsb_surface_create", "tsb_surface_destroy", "tsb_surface_last_error", "tsb_surface_forward", "tsb_surface_backward",
     "tsb_surface_extract", "tsb_free_host", "tsb_setup_last_error",
@@ -66,6 +67,19 @@ class tsb_newton_sphere_t(C.Structure):
     _fields_ = [("mu", C.c_double), ("rho", C.c_double), ("grad_norm", C.c_float), ("alpha", C.c_float), ("delta", C.c_float),
                 ("b_dot_d", C.c_float), ("k", C.c_int32), ("pcg_status", C.c_int32), ("n_hvp", C.c_int32),
                 ("status", C.c_int32), ("first_vertex", C.c_int32), ("reserved", C.c_int32 * 3)]
+
+
+class tsb_newton_tr_options_t(C.Structure):
+    _fields_ = [("max_iter", C.c_int32), ("rtol", C.c_float), ("rel_floor", C.c_float), ("gtol", C.c_float),
+                ("radius_init", C.c_float), ("radius_min", C.c_float), ("radius_max", C.c_float), ("accept", C.c_float),
+                ("eta", C.c_float), ("reserved", C.c_int32 * 7)]
+
+
+class tsb_newton_tr_sphere_t(C.Structure):
+    _fields_ = [("radius", C.c_double), ("rho", C.c_double), ("grad_norm", C.c_float), ("alpha", C.c_float),
+                ("delta", C.c_float), ("b_dot_d", C.c_float), ("pred", C.c_float), ("d_norm", C.c_float),
+                ("pcg_status", C.c_int32), ("n_hvp", C.c_int32), ("status", C.c_int32), ("first_vertex", C.c_int32),
+                ("reserved", C.c_int32 * 2)]
 
 
 class tsb_info_t(C.Structure):
@@ -134,6 +148,9 @@ def _load() -> C.CDLL:
     lib.tsb_pcg_enable_psd.argtypes = [vp, vp, vp, i32]
     lib.tsb_pcg_hvp_psd.restype = C.c_int
     lib.tsb_pcg_hvp_psd.argtypes = [vp, vp, vp, C.POINTER(tsb_terms_t), vp, vp, vp]
+    lib.tsb_pcg_solve_tr.restype = C.c_int
+    lib.tsb_pcg_solve_tr.argtypes = [vp, vp, vp, C.POINTER(tsb_terms_t), C.POINTER(tsb_pcg_options_t), vp, vp, vp, vp,
+                                     C.POINTER(C.c_int32), vp]
     lib.tsb_newton_create.restype = C.c_int
     lib.tsb_newton_create.argtypes = [vp, C.POINTER(vp)]
     lib.tsb_newton_destroy.restype = None
@@ -148,6 +165,8 @@ def _load() -> C.CDLL:
     lib.tsb_newton_step.argtypes = [vp, vp, C.POINTER(tsb_terms_t), C.POINTER(tsb_newton_options_t), vp, vp]
     lib.tsb_newton_prox_step.restype = C.c_int
     lib.tsb_newton_prox_step.argtypes = [vp, vp, vp, vp, C.POINTER(tsb_terms_t), C.POINTER(tsb_newton_options_t), vp, vp]
+    lib.tsb_newton_tr_step.restype = C.c_int
+    lib.tsb_newton_tr_step.argtypes = [vp, vp, vp, vp, C.POINTER(tsb_terms_t), C.POINTER(tsb_newton_tr_options_t), vp, vp]
     lib.tsb_energy_grad_host.restype = C.c_int
     lib.tsb_energy_grad_host.argtypes = [vp, vp, f32, f32, i32, f32, vp, vp, vp]
     lib.tsb_scale.restype = C.c_int

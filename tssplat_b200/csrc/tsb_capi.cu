@@ -17,6 +17,8 @@ static_assert(sizeof(tsb_sphere_stats_t) == 40, "tsb_sphere_stats_t must be 40 b
 static_assert(sizeof(tsb_pcg_sphere_t) == 32, "tsb_pcg_sphere_t must be 32 bytes");
 static_assert(sizeof(tsb_newton_options_t) == 64, "tsb_newton_options_t must be 64 bytes");
 static_assert(sizeof(tsb_newton_sphere_t) == 64, "tsb_newton_sphere_t must be 64 bytes");
+static_assert(sizeof(tsb_newton_tr_options_t) == 64, "tsb_newton_tr_options_t must be 64 bytes");
+static_assert(sizeof(tsb_newton_tr_sphere_t) == 64, "tsb_newton_tr_sphere_t must be 64 bytes");
 
 struct tsb_handle_s {
   int device = 0;
@@ -49,6 +51,7 @@ struct tsb_pcg_s {
   cudaEvent_t ev = nullptr;
   bool psd = false;                  // tsb_pcg_enable_psd: the solve multiplies by the projected Hessian
   tsb::PsdParams Q{};
+  tsb::TrComp *tr = nullptr;         // [n_components] trust-region recurrences (allocated by the first tsb_pcg_solve_tr)
   std::vector<void *> allocs;
   std::string err;
 };
@@ -61,6 +64,8 @@ struct tsb_newton_s {
   float *energy = nullptr;           // [4] energies of the gradient launch (not reported)
   float *delta = nullptr;            // [TSB_LINE_MAX_ALPHA][4] the line search's totals (not reported)
   double *prox_part = nullptr;       // [chunks] d.(x - y) partials of tsb_newton_prox_step (allocated by its first call)
+  tsb::TrState *tr_state = nullptr;  // [n_components] trust-region radius state (allocated by the first tsb_newton_tr_step)
+  float *tr_radius = nullptr;        // [n_components] its fp32 radius, handed to tsb_pcg_solve_tr
   int64_t device_bytes = 0;
   std::vector<void *> allocs;
   std::string err;
@@ -157,6 +162,14 @@ int ws_alloc(W *s, size_t elems, const T *src, T **out) {
   if (e != cudaSuccess) { s->err = std::string("workspace initialisation: ") + cudaGetErrorString(e); return TSB_E_CUDA; }
   *out = static_cast<T *>(d);
   return TSB_OK;
+}
+
+// For the calls whose first use allocates: TSB_OK when st is not being captured, TSB_E_INVALID when it is, TSB_E_CUDA when
+// the query fails.
+int not_capturing(cudaStream_t st) {
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(st, &cap) != cudaSuccess) { cudaGetLastError(); return TSB_E_CUDA; }
+  return cap == cudaStreamCaptureStatusNone ? TSB_OK : TSB_E_INVALID;
 }
 
 }  // namespace
@@ -697,10 +710,33 @@ int tsb_pcg_solve(tsb_pcg_t s, const float *x_dev, const float *b_dev, const tsb
   return tsb_pcg_solve_ex(s, x_dev, b_dev, terms, opt, nullptr, d_out_dev, spheres_out_dev, iters_run_out, stream);
 }
 
-int tsb_pcg_solve_ex(tsb_pcg_t s, const float *x_dev, const float *b_dev, const tsb_terms_t *terms, const tsb_pcg_options_t *opt,
-                     const float *shift_dev, float *d_out_dev, tsb_pcg_sphere_t *spheres_out_dev, int32_t *iters_run_out,
-                     void *stream) {
-  if (!s) return TSB_E_INVALID;
+}  // extern "C"
+
+namespace {
+
+// The trust-region recurrence state of a workspace: allocated once, outside any stream capture (the dir kernel of iteration
+// 0 writes it before any kernel reads it).
+int pcg_tr_alloc(tsb_pcg_t s, cudaStream_t st) {
+  if (s->tr) return TSB_OK;
+  const int rc = not_capturing(st);
+  if (rc == TSB_E_CUDA) return pcg_fail(s, rc, "cannot query the stream");
+  if (rc != TSB_OK)
+    return pcg_fail(s, rc, "the first tsb_pcg_solve_tr of a workspace allocates device memory and cannot be captured in a "
+                           "CUDA graph: make one call outside any capture first");
+  void *d = nullptr;
+  const size_t bytes = std::max<size_t>(size_t(s->P.n_components), 1) * sizeof(tsb::TrComp);
+  const cudaError_t e = cudaMalloc(&d, bytes);
+  if (e != cudaSuccess) return pcg_fail(s, TSB_E_NOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e));
+  s->allocs.push_back(d);
+  s->device_bytes += int64_t(bytes);
+  s->tr = static_cast<tsb::TrComp *>(d);
+  return TSB_OK;
+}
+
+// tsb_pcg_solve_ex, and tsb_pcg_solve_tr when radius_dev != nullptr
+int pcg_solve_impl(tsb_pcg_t s, const float *x_dev, const float *b_dev, const tsb_terms_t *terms, const tsb_pcg_options_t *opt,
+                   const float *shift_dev, const float *radius_dev, float *d_out_dev, tsb_pcg_sphere_t *spheres_out_dev,
+                   int32_t *iters_run_out, void *stream) {
   if (!x_dev || !b_dev || !d_out_dev || !terms || !opt)
     return pcg_fail(s, TSB_E_INVALID, "x_dev, b_dev, d_out_dev, terms and opt must be non-null");
   if (opt->max_iter < 1) return pcg_fail(s, TSB_E_INVALID, "max_iter must be >= 1");
@@ -722,12 +758,18 @@ int tsb_pcg_solve_ex(tsb_pcg_t s, const float *x_dev, const float *b_dev, const 
     if (cap != cudaStreamCaptureStatusNone)
       return pcg_fail(s, TSB_E_INVALID, "check_every > 0 reads the host and cannot be captured in a CUDA graph: use check_every = 0");
   }
+  if (radius_dev) {
+    const int rc = pcg_tr_alloc(s, st);
+    if (rc != TSB_OK) return rc;
+  }
+  const tsb::TrParams tp{radius_dev, s->tr};
+  const tsb::TrParams *tr = radius_dev ? &tp : nullptr;
   const tsb::PcgParams &P = s->P;
   if (s->psd) {                        // x does not change during the solve: one projection
     const int rc = psd_project(s, x_dev, *terms, st);
     if (rc != TSB_OK) return rc;
   }
-  cudaError_t e = tsb::launch_pcg_begin(P, b_dev, d_out_dev, st);
+  cudaError_t e = tsb::launch_pcg_begin(P, b_dev, d_out_dev, st, tr);
   if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver launch: ") + cudaGetErrorString(e));
   int32_t it = 0;
   while (it < opt->max_iter) {
@@ -738,7 +780,7 @@ int tsb_pcg_solve_ex(tsb_pcg_t s, const float *x_dev, const float *b_dev, const 
       const int rc = hvp_impl(s->h, x_dev, P.p, terms->c1, terms->c2, terms->c3, terms->order, 1.f, nullptr, P.Hp, nullptr, 1, st);
       if (rc != TSB_OK) return pcg_fail(s, rc, s->h->err);
     }
-    e = tsb::launch_pcg_step(P, d_out_dev, it, opt->rtol, shift_dev, st);
+    e = tsb::launch_pcg_step(P, d_out_dev, it, opt->rtol, shift_dev, st, tr);
     if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver launch: ") + cudaGetErrorString(e));
     ++it;
     if (opt->check_every > 0 && it % opt->check_every == 0 && it < opt->max_iter) {
@@ -756,6 +798,25 @@ int tsb_pcg_solve_ex(tsb_pcg_t s, const float *x_dev, const float *b_dev, const 
     if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver record launch: ") + cudaGetErrorString(e));
   }
   return TSB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int tsb_pcg_solve_ex(tsb_pcg_t s, const float *x_dev, const float *b_dev, const tsb_terms_t *terms, const tsb_pcg_options_t *opt,
+                     const float *shift_dev, float *d_out_dev, tsb_pcg_sphere_t *spheres_out_dev, int32_t *iters_run_out,
+                     void *stream) {
+  if (!s) return TSB_E_INVALID;
+  return pcg_solve_impl(s, x_dev, b_dev, terms, opt, shift_dev, nullptr, d_out_dev, spheres_out_dev, iters_run_out, stream);
+}
+
+int tsb_pcg_solve_tr(tsb_pcg_t s, const float *x_dev, const float *b_dev, const tsb_terms_t *terms, const tsb_pcg_options_t *opt,
+                     const float *shift_dev, const float *radius_dev, float *d_out_dev, tsb_pcg_sphere_t *spheres_out_dev,
+                     int32_t *iters_run_out, void *stream) {
+  if (!s) return TSB_E_INVALID;
+  if (!radius_dev) return pcg_fail(s, TSB_E_INVALID, "radius_dev must be non-null");
+  return pcg_solve_impl(s, x_dev, b_dev, terms, opt, shift_dev, radius_dev, d_out_dev, spheres_out_dev, iters_run_out, stream);
 }
 
 int tsb_sphere_axpy(tsb_pcg_t s, const float *x_dev, const float *a_sphere_dev, const float *d_dev, float *out_dev,
@@ -821,8 +882,9 @@ int tsb_newton_reset(tsb_newton_t nw, void *stream) {
   if (!nw) return TSB_E_INVALID;
   DeviceGuard guard(nw->s->h->device);
   if (!guard.ok) return newton_fail(nw, TSB_E_CUDA, "cannot select the handle's CUDA device");
-  const cudaError_t e = cudaMemsetAsync(nw->W.comp, 0, size_t(nw->s->P.n_components) * sizeof(tsb::NewtonComp),
-                                        static_cast<cudaStream_t>(stream));
+  const size_t S = size_t(nw->s->P.n_components);
+  cudaError_t e = cudaMemsetAsync(nw->W.comp, 0, S * sizeof(tsb::NewtonComp), static_cast<cudaStream_t>(stream));
+  if (e == cudaSuccess && nw->tr_state) e = cudaMemsetAsync(nw->tr_state, 0, S * sizeof(tsb::TrState), static_cast<cudaStream_t>(stream));
   if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("reset: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
@@ -930,6 +992,127 @@ int tsb_newton_prox_step(tsb_newton_t nw, float *x_dev, const float *anchor_dev,
   }
   const tsb::ProxParams prox{x_dev, anchor_dev, weight_dev, nw->prox_part};
   return newton_run(nw, x_dev, &prox, terms, *opt, records_out_dev, st);
+}
+
+}  // extern "C"
+
+namespace {
+
+int newton_tr_check(tsb_newton_t nw, const float *x_dev, const float *anchor_dev, const float *weight_dev,
+                    const tsb_terms_t *terms, const tsb_newton_tr_options_t *opt) {
+  if (!x_dev || !terms || !opt) return newton_fail(nw, TSB_E_INVALID, "x_dev, terms and opt must be non-null");
+  if (!anchor_dev != !weight_dev)
+    return newton_fail(nw, TSB_E_INVALID, "anchor_dev and weight_dev must be both null (objective E) or both set (proximal objective)");
+  if (anchor_dev && anchor_dev == x_dev)
+    return newton_fail(nw, TSB_E_INVALID, "anchor_dev must not be x_dev: x is updated in place while the anchor is read");
+  const tsb_newton_tr_options_t &o = *opt;
+  if (o.max_iter < 1) return newton_fail(nw, TSB_E_INVALID, "max_iter must be >= 1");
+  if (!(o.rtol >= 0.f)) return newton_fail(nw, TSB_E_INVALID, "rtol must be >= 0");
+  if (!(o.rel_floor >= 0.f)) return newton_fail(nw, TSB_E_INVALID, "rel_floor must be >= 0");
+  if (!(o.gtol >= 0.f)) return newton_fail(nw, TSB_E_INVALID, "gtol must be >= 0");
+  if (!(o.radius_init > 0.f) || !std::isfinite(o.radius_init))
+    return newton_fail(nw, TSB_E_INVALID, "radius_init must be finite and > 0");
+  if (!(o.radius_min > 0.f) || !(o.radius_min <= o.radius_max) || !std::isfinite(o.radius_max))
+    return newton_fail(nw, TSB_E_INVALID, "radius_min and radius_max must satisfy 0 < radius_min <= radius_max < inf");
+  if (!(o.accept >= 0.f && o.accept < 0.25f)) return newton_fail(nw, TSB_E_INVALID, "accept must be in [0, 1/4)");
+  if (!(o.eta > 0.f && o.eta <= 1.f)) return newton_fail(nw, TSB_E_INVALID, "eta must be in (0, 1]");
+  for (int32_t r : o.reserved)
+    if (r != 0) return newton_fail(nw, TSB_E_INVALID, "reserved fields must be 0");
+  if (terms->order != 2 && terms->order != 4) return newton_fail(nw, TSB_E_INVALID, "order must be 2 or 4");
+  if (terms->c3 != 0.f && !nw->s->h->amips)
+    return newton_fail(nw, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
+  if (nw->s->psd && !(terms->c1 >= 0.f && terms->c2 >= 0.f && terms->c3 >= 0.f))
+    return newton_fail(nw, TSB_E_INVALID, "the projected Hessian needs c1, c2 and c3 >= 0 (projection does not commute with a negative weight)");
+  return TSB_OK;
+}
+
+// The first trust-region step's allocations: the radius state, the d.(x - y) partials of a proximal step, and (through a
+// first tsb_pcg_solve_tr) the solve's recurrence state.  Nothing is allocated on a stream being captured.
+int newton_tr_alloc(tsb_newton_t nw, bool prox, cudaStream_t st) {
+  const bool need = !nw->tr_state || !nw->s->tr || (prox && !nw->prox_part);
+  if (!need) return TSB_OK;
+  const int rc = not_capturing(st);
+  if (rc == TSB_E_CUDA) return newton_fail(nw, rc, "cannot query the stream");
+  if (rc != TSB_OK)
+    return newton_fail(nw, rc, "the first tsb_newton_tr_step of a workspace (and the first proximal one) allocates device memory "
+                               "and cannot be captured in a CUDA graph: make one call outside any capture first");
+  const size_t S = std::max<size_t>(size_t(nw->s->P.n_components), 1);
+  auto alloc = [&](size_t bytes, void **out) -> int {
+    const cudaError_t e = cudaMalloc(out, bytes);
+    if (e != cudaSuccess) return newton_fail(nw, TSB_E_NOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e));
+    nw->allocs.push_back(*out);
+    nw->device_bytes += int64_t(bytes);
+    return TSB_OK;
+  };
+  if (!nw->tr_state) {
+    void *a = nullptr, *b = nullptr;
+    int r = alloc(S * sizeof(tsb::TrState), &a);
+    if (r == TSB_OK) r = alloc(S * sizeof(float), &b);
+    if (r != TSB_OK) return r;
+    const cudaError_t e = cudaMemsetAsync(a, 0, S * sizeof(tsb::TrState), st);    // every radius to be initialised
+    if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("cudaMemsetAsync: ") + cudaGetErrorString(e));
+    nw->tr_state = static_cast<tsb::TrState *>(a);
+    nw->tr_radius = static_cast<float *>(b);
+  }
+  if (prox && !nw->prox_part) {
+    void *a = nullptr;
+    const int r = alloc(std::max<size_t>(size_t(nw->s->P.n_chunks), 1) * sizeof(double), &a);
+    if (r != TSB_OK) return r;
+    nw->prox_part = static_cast<double *>(a);
+  }
+  const int r = pcg_tr_alloc(nw->s, st);
+  return r == TSB_OK ? TSB_OK : newton_fail(nw, r, nw->s->err);
+}
+
+}  // namespace
+
+extern "C" {
+
+int tsb_newton_tr_step(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const float *weight_dev, const tsb_terms_t *terms,
+                       const tsb_newton_tr_options_t *opt, tsb_newton_tr_sphere_t *records_out_dev, void *stream) {
+  if (!nw) return TSB_E_INVALID;
+  int rc = newton_tr_check(nw, x_dev, anchor_dev, weight_dev, terms, opt);
+  if (rc != TSB_OK) return rc;
+  tsb_pcg_t s = nw->s;
+  tsb_handle_t h = s->h;
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return newton_fail(nw, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool prox = anchor_dev != nullptr;
+  rc = newton_tr_alloc(nw, prox, st);
+  if (rc != TSB_OK) return rc;
+  const tsb_newton_tr_options_t &o = *opt;
+  const tsb::NewtonParams &W = nw->W;
+  const tsb::ProxParams pp{x_dev, anchor_dev, weight_dev, nw->prox_part};
+  const tsb::ProxParams *p = prox ? &pp : nullptr;
+  const tsb::NewtonTrRule R{o.gtol, o.radius_init, o.radius_min, o.radius_max, o.accept, o.eta};
+  const tsb_pcg_options_t po{o.max_iter, o.rtol, 0, {0, 0, 0, 0, 0}};
+  const float *shift = prox ? weight_dev : nullptr;     // an unusable w_c only reaches a sphere whose b_c is 0
+  // 1-2: b = -grad, the diagonal blocks; frozen spheres' b = 0 (prox: b -= w (x - y))
+  rc = energy_grad_impl(h, x_dev, terms->c1, terms->c2, terms->c3, terms->order, -1.f, nullptr, nw->energy, 1, W.b, nullptr, st);
+  if (rc == TSB_OK) rc = tsb_hess_diag(h, x_dev, terms, 1.f, nullptr, W.diag, st);
+  if (rc != TSB_OK) return newton_fail(nw, rc, h->err);
+  cudaError_t e = tsb::launch_newton_tr_prep(s->P, W, p, st);
+  if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
+  // 3: the preconditioner (shift w_c);  4: the radius on a first step
+  rc = tsb_pcg_set_blocks_ex(s, W.diag, o.rel_floor, shift, nullptr, st);
+  if (rc != TSB_OK) return newton_fail(nw, rc, s->err);
+  const tsb::NewtonTrParams T{nw->tr_state, nw->tr_radius, s->tr};
+  e = tsb::launch_newton_tr_radius(s->P, W, T, R, st);
+  if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
+  // 5: the trust-region solve
+  rc = tsb_pcg_solve_tr(s, x_dev, W.b, terms, &po, shift, nw->tr_radius, W.d, nullptr, nullptr, st);
+  if (rc != TSB_OK) return newton_fail(nw, rc, s->err);
+  // 6: b.d and |d|^2 (prox: and d.(x - y)) per chunk;  7: the line search at alpha = 1
+  e = tsb::launch_newton_dots(s->P, W, p, st);
+  if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
+  rc = tsb_line_search(h, x_dev, W.d, terms, W.alphas, 1, nw->delta, nullptr, W.sphere_delta, W.sphere_step, st);
+  if (rc != TSB_OK) return newton_fail(nw, rc, h->err);
+  // 8-9: decision, step
+  e = tsb::launch_newton_tr_decide(s->P, W, T, R, p, records_out_dev, st);
+  if (e == cudaSuccess) e = tsb::launch_sphere_axpy(s->P, x_dev, W.alpha_sphere, W.d, x_dev, st);
+  if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
+  return TSB_OK;
 }
 
 int tsb_energy_grad_host(tsb_handle_t h, const float *x_host, float c1, float c2, int32_t order, float gradH,

@@ -184,11 +184,22 @@ __global__ void __launch_bounds__(kT) pcg_curv_shift_kernel(const PcgParams s, c
   curv_body<true>(s, shift, sh);
 }
 
+// tau >= 0 with |d + tau p|_M = Delta from the recurrences, in the form without cancellation (Delta2 = Delta^2); 0 when
+// d is already on or outside the boundary or p has no length
+__device__ __forceinline__ double boundary_tau(double pMp, double dMp, double dMd, double Delta2) {
+  const double num = Delta2 - dMd;
+  const double den = dMp + sqrt(dMp * dMp + pMp * num);
+  return num > 0.0 && den > 0.0 ? num / den : 0.0;
+}
+
 // alpha = r.z / p.Hp per component; p.Hp <= 0 stops the component (at the first direction d = z = P b), otherwise
 // d += alpha p, r -= alpha Hp, z = P r and the partials of the new r.z and r.r.  SHIFT: Hp + mu_c p in place of Hp.
-template <bool SHIFT>
+// TR, with a finite radius Delta_c: p.Hp <= 0, or a step that would end at |d + alpha p|_M >= Delta_c, stops the component
+// on the boundary instead, d += tau p (NEGCURV_BOUNDARY, BOUNDARY); r and z are then left as they were.  With Delta_c =
+// +inf every value written is the one the plain body writes.
+template <bool SHIFT, bool TR>
 __device__ __forceinline__ void update_body(const PcgParams &s, float *__restrict__ d, int iter, const float *__restrict__ shift,
-                                            double *sh) {
+                                            const TrParams &t, double *sh) {
   const int c = s.chunk[3 * blockIdx.x];
   const bool lead = int(blockIdx.x) == s.comp_chunk[c] && threadIdx.x == 0;
   PcgComp &C = s.comp[c];
@@ -201,9 +212,38 @@ __device__ __forceinline__ void update_body(const PcgParams &s, float *__restric
   const double rz = C.rz;
   const int begin = s.chunk[3 * blockIdx.x + 1], end = s.chunk[3 * blockIdx.x + 2];
   const int e = begin + int(threadIdx.x);
+  if (TR) {
+    const float rf = t.radius[c];
+    const double D = rf > 0.f ? double(rf) : 0.0;     // NaN and <= 0: radius 0
+    if (D < INFINITY) {
+      const double pMp = t.comp[c].pMp, dMp = t.comp[c].dMp, dMd = t.comp[c].dMd;   // not .step: the lead writes it
+      const double D2 = D * D;
+      int bst = kPcgActive;                              // stays so for a step inside the radius
+      if (!(pHp > 0.0)) {
+        bst = TSB_PCG_NEGCURV_BOUNDARY;
+      } else {
+        const double a = rz / pHp;
+        if (dMd + 2.0 * a * dMp + a * a * pMp >= D2) bst = TSB_PCG_BOUNDARY;
+      }
+      if (bst != kPcgActive) {
+        const double tau = boundary_tau(pMp, dMp, dMd, D2);
+        const float a = float(tau);
+        if (e < end) {
+          const int v = s.vert[e];
+          const F3 p = ld3(s.p, v);
+          F3 x = ld3(d, v);
+          x.x += a * p.x; x.y += a * p.y; x.z += a * p.z;
+          st3(d, v, x);
+        }
+        if (lead) { C.st_upd = bst; C.idle = 0; C.n_hvp = iter + 1; C.dHd += tau * tau * pHp; t.comp[c].step = tau; }
+        return;
+      }
+    }
+  }
   if (!(pHp > 0.0)) {
     if (iter == 0 && e < end) { const int v = s.vert[e]; st3(d, v, ld3(s.z, v)); }
     if (lead) { C.st_upd = iter == 0 ? TSB_PCG_NEGCURV_FIRST : TSB_PCG_NEGCURV; C.idle = 0; C.n_hvp = iter + 1; }
+    if (TR && lead) t.comp[c].step = iter == 0 ? 1.0 : 0.0;
     return;
   }
   const double alpha = rz / pHp;
@@ -223,17 +263,29 @@ __device__ __forceinline__ void update_body(const PcgParams &s, float *__restric
   nrr = block_sum(nrr, sh);
   if (threadIdx.x == 0) { s.part[kPartCols * size_t(blockIdx.x) + kRz] = nrz; s.part[kPartCols * size_t(blockIdx.x) + kRr] = nrr; }
   if (lead) { C.st_upd = kPcgActive; C.idle = 0; C.n_hvp = iter + 1; C.rz_prev = rz; C.dHd += alpha * alpha * pHp; }
+  if (TR && lead) t.comp[c].step = alpha;
 }
 
 __global__ void __launch_bounds__(kT) pcg_update_kernel(const PcgParams s, float *__restrict__ d, int iter) {
   __shared__ double sh[kT / 32];
-  update_body<false>(s, d, iter, nullptr, sh);
+  update_body<false, false>(s, d, iter, nullptr, TrParams{}, sh);
 }
 
 __global__ void __launch_bounds__(kT) pcg_update_shift_kernel(const PcgParams s, float *__restrict__ d, int iter,
                                                               const float *__restrict__ shift) {
   __shared__ double sh[kT / 32];
-  update_body<true>(s, d, iter, shift, sh);
+  update_body<true, false>(s, d, iter, shift, TrParams{}, sh);
+}
+
+__global__ void __launch_bounds__(kT) pcg_update_tr_kernel(const PcgParams s, float *__restrict__ d, int iter, const TrParams t) {
+  __shared__ double sh[kT / 32];
+  update_body<false, true>(s, d, iter, nullptr, t, sh);
+}
+
+__global__ void __launch_bounds__(kT) pcg_update_shift_tr_kernel(const PcgParams s, float *__restrict__ d, int iter,
+                                                                 const float *__restrict__ shift, const TrParams t) {
+  __shared__ double sh[kT / 32];
+  update_body<true, true>(s, d, iter, shift, t, sh);
 }
 
 // Folds r.z and r.r, tests convergence and sets the next direction p = z + beta p; a stopped component gets p = 0, so
@@ -258,6 +310,58 @@ __global__ void __launch_bounds__(kT) pcg_dir_kernel(const PcgParams s, float rt
       beta = float(f.x / C.rz_prev);
       if (lead) { C.rz = f.x; C.rr = f.y; }
     }
+  }
+  if (lead) C.st_dir = st;
+  const int begin = s.chunk[3 * blockIdx.x + 1], end = s.chunk[3 * blockIdx.x + 2];
+  const int e = begin + int(threadIdx.x);
+  if (e < end) {
+    const int v = s.vert[e];
+    F3 p{0.f, 0.f, 0.f};
+    if (st == kPcgActive) {
+      p = ld3(s.z, v);
+      if (!FIRST) { const F3 q = ld3(s.p, v); p.x += beta * q.x; p.y += beta * q.y; p.z += beta * q.z; }
+    }
+    st3(s.p, v, p);
+  }
+}
+
+// pcg_dir_kernel with the trust-region recurrences: the lead also advances them (Steihaug; r^T p_k = 0 and
+// d_k^T M z_{k+1} = r_{k+1}^T d_k = 0):
+//   FIRST: pMp = r.z, dMp = dMd = 0;  after a step s along p:  dMd += 2 s dMp + s^2 pMp, and, if still active,
+//   dMp = beta (dMp + s pMp), pMp = r.z + beta^2 pMp (beta the fp32 value p is formed with, old pMp on the right).
+// A kernel of its own rather than a flag on pcg_dir_kernel's body: that keeps pcg_dir_kernel's machine code as it was.
+__device__ __forceinline__ void tr_advance(TrComp &T, bool active, double beta, double rz) {
+  const double a = T.step, pMp = T.pMp, dMp = T.dMp;
+  T.dMd = T.dMd + 2.0 * a * dMp + a * a * pMp;
+  if (active) {
+    T.dMp = beta * (dMp + a * pMp);
+    T.pMp = rz + beta * beta * pMp;
+  }
+}
+
+template <bool FIRST>
+__global__ void __launch_bounds__(kT) pcg_dir_tr_kernel(const PcgParams s, float rtol, const TrParams t) {
+  __shared__ double sh[kT / 32];
+  const int c = s.chunk[3 * blockIdx.x];
+  const bool lead = int(blockIdx.x) == s.comp_chunk[c] && threadIdx.x == 0;
+  PcgComp &C = s.comp[c];
+  if (!FIRST && C.idle) return;
+  int st = FIRST ? kPcgActive : C.st_upd;
+  float beta = 0.f;
+  if (st == kPcgActive) {
+    const double2 f = make_double2(fold(s.part, kRz, s.comp_chunk[c], s.comp_chunk[c + 1], sh),
+                                   fold(s.part, kRr, s.comp_chunk[c], s.comp_chunk[c + 1], sh));   // (r.z, r.r)
+    if (FIRST) {
+      if (f.y == 0.0) st = TSB_PCG_ZERO_RHS;
+      if (lead) { C.rz = f.x; C.rz_prev = f.x; C.bb = f.y; C.rr = f.y; C.dHd = 0.0; C.st_upd = st; C.idle = 0; C.n_hvp = 0; }
+      if (lead) { t.comp[c].pMp = f.x; t.comp[c].dMp = 0.0; t.comp[c].dMd = 0.0; }
+    } else {
+      if (sqrt(f.y) <= double(rtol) * sqrt(C.bb)) st = TSB_PCG_CONVERGED;
+      beta = float(f.x / C.rz_prev);
+      if (lead) { C.rz = f.x; C.rr = f.y; tr_advance(t.comp[c], st == kPcgActive, double(beta), f.x); }
+    }
+  } else if (!FIRST && lead) {     // stopped by the update (boundary, negative curvature): its last step still counts
+    tr_advance(t.comp[c], false, 0.0, 0.0);
   }
   if (lead) C.st_dir = st;
   const int begin = s.chunk[3 * blockIdx.x + 1], end = s.chunk[3 * blockIdx.x + 2];
@@ -551,6 +655,124 @@ __global__ void __launch_bounds__(kT) newton_decide_prox_kernel(const PcgParams 
   decide_body<true>(s, w, r, p, out);
 }
 
+// ---- Trust-region Newton step (tsb_newton_tr_step) -------------------------------------------------------------------
+// It reuses the prep kernels above (their max (D_v)_ii column is not read in this step) and puts the per-chunk partials
+// of b^T P b in that column instead: written by newton_tr_bpb_kernel, folded by newton_tr_radius_kernel.
+
+// Partial of b^T P b of every chunk of a component whose radius is not yet initialised (P: the blocks just set).
+__global__ void __launch_bounds__(kT) newton_tr_bpb_kernel(const PcgParams s, const NewtonParams w, const NewtonTrParams t) {
+  __shared__ double sh[kT / 32];
+  if (t.state[s.chunk[3 * blockIdx.x]].init) return;
+  const int e = s.chunk[3 * blockIdx.x + 1] + int(threadIdx.x);
+  double q = 0.0;
+  if (e < s.chunk[3 * blockIdx.x + 2]) {
+    const int v = s.vert[e];
+    const F3 b = ld3(w.b, v);
+    q = dot3(b, apply_block(s.pinv, v, b));
+  }
+  q = block_sum(q, sh);
+  if (threadIdx.x == 0) w.part[kNwCols * size_t(blockIdx.x) + kNwMaxD] = q;
+}
+
+// Delta_c = clamp(radius_init sqrt(b^T P b), radius_min, radius_max) on a component's first step after a reset, and the
+// fp32 radius of the solve (thread = component).
+__global__ void __launch_bounds__(kT) newton_tr_radius_kernel(const PcgParams s, const NewtonParams w, const NewtonTrParams t,
+                                                              const NewtonTrRule r) {
+  const int c = blockIdx.x * kT + int(threadIdx.x);
+  if (c >= s.n_components) return;
+  TrState S = t.state[c];
+  if (!S.init) {
+    double bpb = 0.0;
+    for (int k = s.comp_chunk[c]; k < s.comp_chunk[c + 1]; ++k) bpb += w.part[kNwCols * size_t(k) + kNwMaxD];
+    S.radius = fmin(double(r.radius_max), fmax(double(r.radius_min), double(r.radius_init) * sqrt(bpb)));
+    S.init = 1;
+    t.state[c] = S;
+  }
+  t.radius[c] = float(S.radius);
+}
+
+// Acceptance and radius update of every component (thread = component); see tsb_newton_tr_step in the header.
+template <bool PROX>
+__device__ __forceinline__ void decide_tr_body(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t,
+                                               const NewtonTrRule &r, const ProxParams &p, tsb_newton_tr_sphere_t *__restrict__ out) {
+  const int c = blockIdx.x * kT + int(threadIdx.x);
+  if (c >= s.n_components) return;
+  const PcgComp C = s.comp[c];
+  NewtonComp N = w.comp[c];
+  TrState S = t.state[c];
+  const double dMd = t.tr[c].dMd;
+  const int k0 = s.comp_chunk[c], k1 = s.comp_chunk[c + 1];
+  double bd = 0.0, dd = 0.0, dx = 0.0;
+  for (int k = k0; k < k1; ++k) bd += w.part[kNwCols * size_t(k) + kNwBd];
+  for (int k = k0; k < k1; ++k) dd += w.part[kNwCols * size_t(k) + kNwDd];
+  double wc = 0.0;
+  bool bad_w = false;
+  if (PROX) {
+    for (int k = k0; k < k1; ++k) dx += p.part[k];
+    const float q = p.weight[c];
+    bad_w = !prox_weight_ok(q);
+    wc = bad_w ? 0.0 : double(q);
+  }
+  const double bdf = double(float(bd)), dHd = double(float(C.dHd));   // the values the solve's records report
+  const double g = sqrt(C.bb), dn = sqrt(dMd);
+  const int pst = C.st_dir == kPcgActive ? TSB_PCG_MAXITER : C.st_dir;
+  float alpha = 0.f, delta = 0.f;
+  double rho = 0.0, pred = 0.0;
+  if (N.status == TSB_NEWTON_ACTIVE) {
+    if (PROX && bad_w) {
+      N.status = TSB_NEWTON_STALLED;
+    } else if (g <= double(r.gtol)) {
+      N.status = TSB_NEWTON_CONVERGED;
+    } else {
+      pred = bdf - 0.5 * dHd;
+      const double dphi = step_change<PROX>(w.sphere_delta[4 * size_t(c)], wc, 1.0, dx, dd);
+      if (pred > 0.0) rho = -dphi / pred;
+      const double lim = double(r.eta) * double(w.sphere_step[c]);
+      const bool flips = !(1.0 < lim);
+      if (flips) S.radius = fmin(0.25 * S.radius, lim * dn);
+      else if (!(rho >= 0.25)) S.radius = 0.25 * dn;
+      else if (rho > 0.75 && (pst == TSB_PCG_BOUNDARY || pst == TSB_PCG_NEGCURV_BOUNDARY))
+        S.radius = fmin(2.0 * S.radius, double(r.radius_max));
+      if (!flips && pred > 0.0 && rho > double(r.accept)) {
+        alpha = 1.f;
+        delta = float(dphi);
+      } else if (S.radius < double(r.radius_min)) {
+        N.status = TSB_NEWTON_STALLED;
+      }
+    }
+  }
+  w.alpha_sphere[c] = alpha;
+  w.comp[c] = N;
+  t.state[c] = S;
+  if (!out) return;
+  tsb_newton_tr_sphere_t o;
+  o.radius = S.radius;
+  o.rho = rho;
+  o.grad_norm = float(g);
+  o.alpha = alpha;
+  o.delta = delta;
+  o.b_dot_d = float(bd);
+  o.pred = float(pred);
+  o.d_norm = float(dn);
+  o.pcg_status = pst;
+  o.n_hvp = C.n_hvp;
+  o.status = N.status;
+  o.first_vertex = s.vert[s.chunk[3 * size_t(k0) + 1]];
+  o.reserved[0] = o.reserved[1] = 0;
+  out[c] = o;
+}
+
+__global__ void __launch_bounds__(kT) newton_decide_tr_kernel(const PcgParams s, const NewtonParams w, const NewtonTrParams t,
+                                                              const NewtonTrRule r, tsb_newton_tr_sphere_t *__restrict__ out) {
+  decide_tr_body<false>(s, w, t, r, ProxParams{}, out);
+}
+
+__global__ void __launch_bounds__(kT) newton_decide_tr_prox_kernel(const PcgParams s, const NewtonParams w, const NewtonTrParams t,
+                                                                   const NewtonTrRule r, tsb_newton_tr_sphere_t *__restrict__ out,
+                                                                   const ProxParams p) {
+  decide_tr_body<true>(s, w, t, r, p, out);
+}
+
 unsigned with_orphans(const PcgParams &s) { return unsigned(s.n_chunks + (s.n_orphans + kT - 1) / kT); }
 
 }  // namespace
@@ -560,9 +782,10 @@ cudaError_t launch_pcg_blocks(const PcgParams &s, const float *diag, float rel_f
   return cudaGetLastError();
 }
 
-cudaError_t launch_pcg_begin(const PcgParams &s, const float *b, float *d, cudaStream_t st) {
+cudaError_t launch_pcg_begin(const PcgParams &s, const float *b, float *d, cudaStream_t st, const TrParams *tr) {
   pcg_init_kernel<<<with_orphans(s), kT, 0, st>>>(s, b, d);
-  pcg_dir_kernel<true><<<unsigned(s.n_chunks), kT, 0, st>>>(s, 0.f);
+  if (!tr) pcg_dir_kernel<true><<<unsigned(s.n_chunks), kT, 0, st>>>(s, 0.f);
+  else pcg_dir_tr_kernel<true><<<unsigned(s.n_chunks), kT, 0, st>>>(s, 0.f, *tr);
   return cudaGetLastError();
 }
 
@@ -572,7 +795,19 @@ cudaError_t launch_pcg_blocks_shift(const PcgParams &s, const float *diag, float
   return cudaGetLastError();
 }
 
-cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, const float *shift, cudaStream_t st) {
+cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, const float *shift, cudaStream_t st,
+                            const TrParams *tr) {
+  if (tr) {
+    if (shift) {
+      pcg_curv_shift_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, shift);
+      pcg_update_shift_tr_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, d, iter, shift, *tr);
+    } else {
+      pcg_curv_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s);
+      pcg_update_tr_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, d, iter, *tr);
+    }
+    pcg_dir_tr_kernel<false><<<unsigned(s.n_chunks), kT, 0, st>>>(s, rtol, *tr);
+    return cudaGetLastError();
+  }
   if (shift) {
     pcg_curv_shift_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, shift);
     pcg_update_shift_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, d, iter, shift);
@@ -624,6 +859,27 @@ cudaError_t launch_newton_decide(const PcgParams &s, const NewtonParams &w, cons
   const unsigned comp_blocks = unsigned((s.n_components + kT - 1) / kT);
   if (p) newton_decide_prox_kernel<<<comp_blocks, kT, 0, st>>>(s, w, r, out, *p);
   else newton_decide_kernel<<<comp_blocks, kT, 0, st>>>(s, w, r, out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_newton_tr_prep(const PcgParams &s, const NewtonParams &w, const ProxParams *p, cudaStream_t st) {
+  if (p) newton_prep_prox_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w, *p);
+  else newton_prep_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_newton_tr_radius(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t, const NewtonTrRule &r,
+                                    cudaStream_t st) {
+  newton_tr_bpb_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w, t);
+  newton_tr_radius_kernel<<<unsigned((s.n_components + kT - 1) / kT), kT, 0, st>>>(s, w, t, r);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_newton_tr_decide(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t, const NewtonTrRule &r,
+                                    const ProxParams *p, tsb_newton_tr_sphere_t *out, cudaStream_t st) {
+  const unsigned comp_blocks = unsigned((s.n_components + kT - 1) / kT);
+  if (p) newton_decide_tr_prox_kernel<<<comp_blocks, kT, 0, st>>>(s, w, t, r, out, *p);
+  else newton_decide_tr_kernel<<<comp_blocks, kT, 0, st>>>(s, w, t, r, out);
   return cudaGetLastError();
 }
 

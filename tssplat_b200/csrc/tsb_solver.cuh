@@ -43,6 +43,23 @@ struct PcgParams {
 
 // State of one component of the damped Newton step (tsb_newton_step).  The shift kernel writes mu, nu and init on a
 // component's first step, the decision kernel mu, nu and status; the other kernels only read it.  32 bytes.
+// Trust-region recurrences of one component (tsb_pcg_solve_tr), in preconditioner norm |v|_M^2 = v^T P^-1 v.  A separate
+// array, allocated by a workspace's first trust-region solve, so PcgComp and the plain solves are unchanged.  The lead
+// thread of the component's first chunk in the dir kernel writes pMp, dMp and dMd (the update kernel reads them in every
+// chunk); the update kernel's lead writes step (the dir kernel's lead reads it).  32 bytes.
+struct TrComp {
+  double pMp;    // |p|_M^2 of the current direction
+  double dMp;    // d^T M p
+  double dMd;    // |d|_M^2 of the current iterate
+  double step;   // the step the last update took along p: alpha, the boundary tau, or 0 when d did not move
+};
+static_assert(sizeof(TrComp) == 32, "TrComp must be 32 bytes");
+
+struct TrParams {
+  const float *radius;   // [n_components] Delta_c (+inf: no radius; NaN or <= 0: radius 0)
+  TrComp *comp;          // [n_components]
+};
+
 struct NewtonComp {
   double mu, nu;
   int32_t status;   // TSB_NEWTON_*
@@ -75,15 +92,36 @@ struct NewtonRule {           // the options the kernels read
   int32_t n_alpha;
 };
 
+// Radius state of one component of the trust-region step (tsb_newton_tr_step), allocated by the first such step.  The
+// radius kernel writes it on a component's first step after a reset, the decision kernel afterwards.  16 bytes.
+struct TrState {
+  double radius;    // Delta_c
+  int32_t init;     // radius initialised
+  int32_t pad;
+};
+static_assert(sizeof(TrState) == 16, "TrState must be 16 bytes");
+
+struct NewtonTrParams {
+  TrState *state;            // [n_components]
+  float *radius;             // [n_components] fp32 Delta_c handed to the solve
+  const TrComp *tr;          // [n_components] the solve's recurrences (|d|_M^2)
+};
+
+struct NewtonTrRule {         // the options the trust-region kernels read
+  float gtol, radius_init, radius_min, radius_max, accept, eta;
+};
+
 cudaError_t launch_pcg_blocks(const PcgParams &s, const float *diag, float rel_floor, float *inv_out, cudaStream_t st);
 // blocks D_v + shift[c] I (over the chunk table; orphan vertices unshifted)
 cudaError_t launch_pcg_blocks_shift(const PcgParams &s, const float *diag, float rel_floor, const float *shift, float *inv_out,
                                     cudaStream_t st);
 // r = b, z = P r, d = 0 and the first direction; leaves every component ACTIVE or ZERO_RHS
-cudaError_t launch_pcg_begin(const PcgParams &s, const float *b, float *d, cudaStream_t st);
+// (tr != nullptr: also initialises the trust-region recurrences)
+cudaError_t launch_pcg_begin(const PcgParams &s, const float *b, float *d, cudaStream_t st, const TrParams *tr = nullptr);
 // after Hp = H p of iteration `iter` (0-based) is complete on the stream: curvature, update and next direction; with
-// shift != nullptr the operator is H + shift[c] I
-cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, const float *shift, cudaStream_t st);
+// shift != nullptr the operator is H + shift[c] I; with tr != nullptr every component stays inside its radius
+cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, const float *shift, cudaStream_t st,
+                            const TrParams *tr = nullptr);
 cudaError_t launch_pcg_count(const PcgParams &s, cudaStream_t st);
 cudaError_t launch_pcg_records(const PcgParams &s, const float *b, const float *d, tsb_pcg_sphere_t *out, cudaStream_t st);
 cudaError_t launch_sphere_axpy(const PcgParams &s, const float *x, const float *a, const float *d, float *out, cudaStream_t st);
@@ -96,5 +134,14 @@ cudaError_t launch_newton_dots(const PcgParams &s, const NewtonParams &w, const 
 // step choice, damping update, records (out may be null)
 cudaError_t launch_newton_decide(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, const ProxParams *p,
                                  tsb_newton_sphere_t *out, cudaStream_t st);
+// Trust-region step (p != nullptr: the proximal objective).  b_c = 0 on frozen components (prox: b -= w (x - y)), without
+// the damping of launch_newton_prep
+cudaError_t launch_newton_tr_prep(const PcgParams &s, const NewtonParams &w, const ProxParams *p, cudaStream_t st);
+// after the preconditioner is set: b^T P b per component, Delta_c on a first step, the fp32 radius
+cudaError_t launch_newton_tr_radius(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t, const NewtonTrRule &r,
+                                    cudaStream_t st);
+// acceptance, radius update, records (out may be null)
+cudaError_t launch_newton_tr_decide(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t, const NewtonTrRule &r,
+                                    const ProxParams *p, tsb_newton_tr_sphere_t *out, cudaStream_t st);
 
 }  // namespace tsb

@@ -245,10 +245,20 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         amips)`` with the scheduler's coefficients and the barrier order at ``it``: ``tssplat_b200.newton.DeviceNewton``
         (``tsb_newton_step``), which updates ``x.data`` in place without a host read.  ``opts``: the fields of
         ``newton.NEWTON_DEFAULTS``.  The workspace, ``self.device_newton``, is created on first use (sharing
-        ``self.device_pcg``); its ``reset()`` restarts every sphere.  Returns the ``NewtonStepResult``."""
+        ``self.device_pcg``); its ``reset()`` restarts every sphere.  Returns the ``NewtonStepResult``.
+        ``FLAGS.newton_method = "tr"`` takes the trust-region step instead (``DeviceNewton.tr_step``; ``opts`` then the
+        fields of ``newton.NEWTON_TR_DEFAULTS``; returns a ``NewtonTRStepResult``)."""
         nw = self._device_newton()
         c1, c2 = self.coeff_scheduler(it)
-        return nw.step(x.data, c1, c2, self.order_at(it), c3=self.amips_coeff, **opts)
+        run = nw.tr_step if self._newton_method() == "tr" else nw.step
+        return run(x.data, c1, c2, self.order_at(it), c3=self.amips_coeff, **opts)
+
+    def _newton_method(self) -> str:
+        from .newton import METHODS
+        m = getattr(self.FLAGS, "newton_method", "lm") or "lm"
+        if m not in METHODS:
+            raise ValueError(f"FLAGS.newton_method must be one of {METHODS}, got {m!r}")
+        return m
 
     def prox_step(self, x, y, it, weight, n_steps=1, restart=True, **opts):
         """The regulariser half of a split step: ``n_steps`` proximal Newton steps per sphere of
@@ -257,7 +267,8 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         term, copied: ``y`` must not be ``x``).  ``weight``: a float for every sphere or a float32 CUDA tensor [S].
         Updates ``x.data`` in place with no host read (``tsb_newton_prox_step``) and returns the last
         ``NewtonStepResult``.  ``restart`` resets the workspace first: a new anchor is a new problem, and a sphere frozen
-        on the old one must not stay frozen.  ``opts``: the fields of ``newton.NEWTON_DEFAULTS``."""
+        on the old one must not stay frozen.  ``opts``: the fields of ``newton.NEWTON_DEFAULTS`` (of
+        ``newton.NEWTON_TR_DEFAULTS`` with ``FLAGS.newton_method = "tr"``, which takes trust-region steps)."""
         if n_steps < 1:
             raise ValueError("n_steps must be >= 1")
         nw = self._device_newton()
@@ -265,7 +276,7 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
             nw.reset()
         c1, c2 = self.coeff_scheduler(it)
         _, res = nw.minimize(x.data, n_steps, c1, c2, self.order_at(it), c3=self.amips_coeff, anchor=y.detach(),
-                             weight=weight, **opts)
+                             weight=weight, method=self._newton_method(), **opts)
         return res
 
     def forward(self, x, it, c1, c2):

@@ -17,7 +17,9 @@ semidefinite projection, so the solve never stops at negative curvature from the
 sphere per call -- gradient, diagonal blocks, shifted solve, line search, step choice and damping update -- on one
 stream without a host read.  Given an ``anchor`` y and per-sphere weights w, the step minimises the proximal objective
 ``E(x) + (w_c / 2) |x_c - y_c|^2`` instead (``tsb_newton_prox_step``): the regulariser half of a split training loop whose
-data term keeps its first-order optimiser.
+data term keeps its first-order optimiser.  ``DeviceNewton.tr_step`` is the trust-region alternative
+(``tsb_newton_tr_step``): no damping shift, a per-sphere radius in the preconditioner norm inside which the solve
+(``DevicePCG.solve(..., radius=)``, ``tsb_pcg_solve_tr``) follows negative curvature to the boundary.
 """
 from __future__ import annotations
 
@@ -27,7 +29,7 @@ from typing import Callable, NamedTuple, Optional, Union
 import torch
 
 __all__ = ["hess_blocks", "block_jacobi", "apply_blocks", "pcg", "PCGResult", "DevicePCG", "DevicePCGResult", "DeviceNewton",
-           "NewtonStepResult", "NEWTON_DEFAULTS", "HESSIANS"]
+           "NewtonStepResult", "NEWTON_DEFAULTS", "HESSIANS", "NewtonTRStepResult", "NEWTON_TR_DEFAULTS", "METHODS"]
 
 
 def hess_blocks(planes: torch.Tensor) -> torch.Tensor:
@@ -123,7 +125,8 @@ class DevicePCGResult(NamedTuple):
     (``tsb_pcg_sphere_t`` in ``include/tssplat_b200.h``)."""
     d: torch.Tensor                 # f32 [n, 3]: the step of every sphere; 0 on vertices no tet references
     status: torch.Tensor            # i32 [S]: 0 max_iter, 1 converged, 2 negative curvature, 3 the same at the first
-                                    # direction (d_c = P b_c), 4 zero right-hand side
+                                    # direction (d_c = P b_c), 4 zero right-hand side; with a radius also 5 stopped on
+                                    # the boundary, 6 negative curvature followed to the boundary
     n_hvp: torch.Tensor             # i32 [S]: products in which the sphere was still active
     rel_residual: torch.Tensor      # f32 [S]: |r_c| / |b_c| of the returned step
     b_dot_d: torch.Tensor           # f32 [S]: b_c . d_c
@@ -208,23 +211,33 @@ class DevicePCG:
         return inv
 
     def solve(self, x: torch.Tensor, b: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0,
-              max_iter: int = 100, rtol: float = 1e-3, check_every: int = 0, shift=None) -> DevicePCGResult:
+              max_iter: int = 100, rtol: float = 1e-3, check_every: int = 0, shift=None, radius=None) -> DevicePCGResult:
         """``H(x) d = b`` on every sphere by truncated PCG (``tsb_pcg_solve``), ``H`` the Hessian ``TetSpheres.hvp``
         multiplies by.  ``check_every = 0`` enqueues ``max_iter`` iterations without touching the host (and can be
         captured in a CUDA graph); ``k > 0`` reads the number of active spheres every ``k`` iterations and stops
         early.  ``shift`` (as in ``set_blocks``) solves ``(H + mu_c I) d = b`` instead (``tsb_pcg_solve_ex``); ``d_H_d``
-        is then ``d^T (H + mu_c I) d``."""
+        is then ``d^T (H + mu_c I) d``.  ``radius`` (a float for every sphere, or a float32 CUDA tensor [S] read on the
+        device) keeps every sphere's step inside ``|d_c|_M <= radius_c`` in the preconditioner norm (``tsb_pcg_solve_tr``,
+        Steihaug-Toint): negative curvature and a step that would leave the radius end on the boundary (status 6 and 5).
+        ``radius=inf`` gives the bits of the call without it; the first call with a radius allocates, so it cannot be
+        captured."""
         n3, dev = self.tet_sp.n3, self.tet_sp.device
         xc, bc = self._f32(x, n3, "x"), self._f32(b, n3, "b")
         sh = self._shift(shift)
+        rad = self._shift(radius, "radius")
         d = torch.empty((self.tet_sp.n, 3), dtype=torch.float32, device=dev)
         raw = torch.empty((self.n_spheres, 8), dtype=torch.int32, device=dev)
         terms = self._capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
         opt = self._capi.tsb_pcg_options_t(max_iter=int(max_iter), rtol=float(rtol), check_every=int(check_every))
         iters = C.c_int32(0)
-        rc = self._capi.lib.tsb_pcg_solve_ex(self._s, xc.data_ptr(), bc.data_ptr(), C.byref(terms), C.byref(opt),
-                                             sh.data_ptr() if sh is not None else None, d.data_ptr(), raw.data_ptr(),
-                                             C.byref(iters), self._stream_ptr(dev))
+        if rad is None:
+            rc = self._capi.lib.tsb_pcg_solve_ex(self._s, xc.data_ptr(), bc.data_ptr(), C.byref(terms), C.byref(opt),
+                                                 sh.data_ptr() if sh is not None else None, d.data_ptr(), raw.data_ptr(),
+                                                 C.byref(iters), self._stream_ptr(dev))
+        else:
+            rc = self._capi.lib.tsb_pcg_solve_tr(self._s, xc.data_ptr(), bc.data_ptr(), C.byref(terms), C.byref(opt),
+                                                 sh.data_ptr() if sh is not None else None, rad.data_ptr(), d.data_ptr(),
+                                                 raw.data_ptr(), C.byref(iters), self._stream_ptr(dev))
         self._check(rc, "solve")
         f = raw.view(torch.float32)
         return DevicePCGResult(d, raw[:, 4], raw[:, 3], f[:, 0], f[:, 1], f[:, 2], int(iters.value))
@@ -281,6 +294,31 @@ class NewtonStepResult(NamedTuple):
     first_vertex: torch.Tensor      # i32: lowest vertex id of the sphere
 
 
+#: options of ``DeviceNewton.tr_step`` (``tsb_newton_tr_options_t``)
+NEWTON_TR_DEFAULTS = dict(max_iter=20, rtol=1e-2, rel_floor=1e-6, gtol=0.0, radius_init=1.0, radius_min=1e-12,
+                          radius_max=1e12, accept=1e-4, eta=0.9)
+
+#: the steps of ``DeviceNewton.minimize``: Levenberg-Marquardt (``step``) or trust region (``tr_step``)
+METHODS = ("lm", "tr")
+
+
+class NewtonTRStepResult(NamedTuple):
+    """What ``DeviceNewton.tr_step`` returns: device tensors [S], spheres in the order of their lowest vertex ids
+    (``tsb_newton_tr_sphere_t`` in ``include/tssplat_b200.h``)."""
+    grad_norm: torch.Tensor         # f32: |grad_c| before the step (0 once the sphere is frozen)
+    alpha: torch.Tensor             # f32: 1 when the step was taken, else 0
+    delta: torch.Tensor             # f32: objective change of the step taken (0 if none)
+    radius: torch.Tensor            # f64: trust radius after the update (preconditioner norm)
+    rho: torch.Tensor               # f64: gain ratio -delta(1) / pred (0 when pred <= 0 or no decision ran)
+    pred: torch.Tensor              # f32: model decrease b.d - d^T H d / 2
+    d_norm: torch.Tensor            # f32: |d_c|_M of the solve's step
+    pcg_status: torch.Tensor        # i32: TSB_PCG_* of the trust-region solve
+    n_hvp: torch.Tensor             # i32: products in which the sphere was active
+    b_dot_d: torch.Tensor           # f32: b_c . d_c, b = -grad
+    status: torch.Tensor            # i32: 0 active, 1 converged, 2 stalled (both frozen)
+    first_vertex: torch.Tensor      # i32: lowest vertex id of the sphere
+
+
 class DeviceNewton:
     """Damped Newton workspace (``tsb_newton_create``) of one ``TetSpheres`` handle: reuses ``pcg`` (a ``DevicePCG`` of
     the same handle) or creates one, and keeps it alive.  Every sphere runs its own Levenberg-Marquardt iteration;
@@ -311,7 +349,8 @@ class DeviceNewton:
 
     @property
     def device_bytes(self) -> int:
-        """``tsb_newton_device_bytes``: grows by 8 bytes per chunk at the first proximal step."""
+        """``tsb_newton_device_bytes``: grows by 8 bytes per chunk at the first proximal step and by 20 bytes per sphere
+        at the first trust-region step."""
         return int(self._capi.lib.tsb_newton_device_bytes(self._nw))
 
     def __del__(self):
@@ -331,7 +370,7 @@ class DeviceNewton:
             raise RuntimeError(f"DeviceNewton.{what}: {self._error(self._nw)} (code {rc})")
 
     def reset(self) -> None:
-        """Every sphere ACTIVE again, its damping re-initialised at the next step."""
+        """Every sphere ACTIVE again, its damping (and trust radius) re-initialised at the next step."""
         self._check(self._capi.lib.tsb_newton_reset(self._nw, self._stream_ptr(self.tet_sp.device)), "reset")
 
     def options(self, **opts):
@@ -341,6 +380,51 @@ class DeviceNewton:
             raise TypeError(f"unknown Newton options: {sorted(bad)}")
         o = {**NEWTON_DEFAULTS, **opts}
         return self._capi.tsb_newton_options_t(**{k: (int(v) if k in ("max_iter", "n_alpha") else float(v)) for k, v in o.items()})
+
+    def _x_anchor(self, x, anchor, weight):
+        """Checks x (updated in place) and the proximal pair; returns the weight tensor or None."""
+        xc = self.pcg._f32(x, self.tet_sp.n3, "x")
+        if xc is not x:
+            raise RuntimeError("x must be contiguous (it is updated in place)")
+        if anchor is None and weight is not None:
+            raise RuntimeError("weight needs an anchor")
+        if anchor is None:
+            return None
+        if weight is None:
+            raise RuntimeError("an anchor needs a weight (a float or a float32 CUDA tensor of one entry per sphere)")
+        if self.pcg._f32(anchor, self.tet_sp.n3, "anchor") is not anchor:
+            raise RuntimeError("anchor must be contiguous")
+        if anchor.data_ptr() == x.data_ptr():
+            raise RuntimeError("anchor must not be x (x is updated in place while the anchor is read)")
+        return self.pcg._shift(weight, "weight")
+
+    def tr_options(self, **opts):
+        """``tsb_newton_tr_options_t`` from ``NEWTON_TR_DEFAULTS`` updated with ``opts``."""
+        bad = set(opts) - set(NEWTON_TR_DEFAULTS)
+        if bad:
+            raise TypeError(f"unknown trust-region options: {sorted(bad)}")
+        o = {**NEWTON_TR_DEFAULTS, **opts}
+        return self._capi.tsb_newton_tr_options_t(**{k: (int(v) if k == "max_iter" else float(v)) for k, v in o.items()})
+
+    def tr_step(self, x: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0,
+                anchor: Optional[torch.Tensor] = None, weight=None, **opts) -> NewtonTRStepResult:
+        """One trust-region Newton step (``tsb_newton_tr_step``) of ``c1 * smooth + c2 * barrier (+ c3 * amips)`` on every
+        sphere, or of the proximal objective with ``anchor`` and ``weight`` as in ``step``; ``x`` is updated in place
+        without a host read.  Each sphere keeps a radius in the preconditioner norm: the solve stays inside it (following
+        negative curvature to its boundary), the step is taken whole or not at all, and the gain ratio grows or shrinks
+        the radius.  ``opts``: the fields of ``NEWTON_TR_DEFAULTS``.  The first call on a workspace allocates, so it
+        cannot be captured in a CUDA graph; later ones can."""
+        w = self._x_anchor(x, anchor, weight)
+        raw = torch.empty((self.n_spheres, 16), dtype=torch.int32, device=self.tet_sp.device)
+        terms = self._capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
+        opt = self.tr_options(**opts)
+        rc = self._capi.lib.tsb_newton_tr_step(self._nw, x.data_ptr(), anchor.data_ptr() if anchor is not None else None,
+                                               w.data_ptr() if w is not None else None, C.byref(terms), C.byref(opt),
+                                               raw.data_ptr(), self._stream_ptr(self.tet_sp.device))
+        self._check(rc, "tr_step")
+        f64, f32 = raw[:, 0:4].view(torch.float64), raw[:, 4:10].view(torch.float32)
+        return NewtonTRStepResult(f32[:, 0], f32[:, 1], f32[:, 2], f64[:, 0], f64[:, 1], f32[:, 4], f32[:, 5], raw[:, 10],
+                                  raw[:, 11], f32[:, 3], raw[:, 12], raw[:, 13])
 
     def step(self, x: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0, anchor: Optional[torch.Tensor] = None,
              weight=None, **opts) -> NewtonStepResult:
@@ -354,19 +438,7 @@ class DeviceNewton:
         records' ``grad_norm``, ``delta`` and ``b_dot_d`` are then those of the proximal objective, and a sphere whose
         weight is NaN, infinite or negative is frozen (STALLED) without moving.  A linear term ``q . x`` folds into the
         anchor: pass ``y = x0 - q / w``."""
-        xc = self.pcg._f32(x, self.tet_sp.n3, "x")
-        if xc is not x:
-            raise RuntimeError("x must be contiguous (it is updated in place)")
-        if anchor is None and weight is not None:
-            raise RuntimeError("weight needs an anchor")
-        if anchor is not None:
-            if weight is None:
-                raise RuntimeError("an anchor needs a weight (a float or a float32 CUDA tensor of one entry per sphere)")
-            if self.pcg._f32(anchor, self.tet_sp.n3, "anchor") is not anchor:
-                raise RuntimeError("anchor must be contiguous")
-            if anchor.data_ptr() == x.data_ptr():
-                raise RuntimeError("anchor must not be x (x is updated in place while the anchor is read)")
-            w = self.pcg._shift(weight, "weight")
+        w = self._x_anchor(x, anchor, weight)
         raw = torch.empty((self.n_spheres, 16), dtype=torch.int32, device=self.tet_sp.device)
         terms = self._capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
         opt = self.options(**opts)
@@ -382,11 +454,14 @@ class DeviceNewton:
                                 f32[:, 3], raw[:, 11], raw[:, 12])
 
     def minimize(self, x: torch.Tensor, n_steps: int, c1: float, c2: float, order: int, c3: float = 0.0,
-                 check_every: int = 0, anchor: Optional[torch.Tensor] = None, weight=None, **opts):
-        """Up to ``n_steps`` calls of ``step``; returns (steps run, the last ``NewtonStepResult``).  ``check_every = 0``
-        never touches the host (capturable); ``k > 0`` reads one integer, the number of spheres still active, every
-        ``k`` steps and stops when it is 0 (refused while the stream is being captured).  ``anchor`` and ``weight``: the
-        proximal step of ``step``."""
+                 check_every: int = 0, anchor: Optional[torch.Tensor] = None, weight=None, method: str = "lm", **opts):
+        """Up to ``n_steps`` calls of ``step`` (``method="lm"``) or ``tr_step`` (``method="tr"``, ``opts`` then the fields
+        of ``NEWTON_TR_DEFAULTS``); returns (steps run, the last result).  ``check_every = 0`` never touches the host
+        (capturable); ``k > 0`` reads one integer, the number of spheres still active, every ``k`` steps and stops when
+        it is 0 (refused while the stream is being captured).  ``anchor`` and ``weight``: the proximal step of
+        ``step``."""
+        if method not in METHODS:
+            raise ValueError(f"method must be one of {METHODS}, got {method!r}")
         if check_every < 0 or n_steps < 0:
             raise ValueError("n_steps and check_every must be >= 0")
         if check_every > 0 and torch.cuda.is_current_stream_capturing():
@@ -396,7 +471,8 @@ class DeviceNewton:
             weight = self.pcg._shift(weight, "weight")         # one tensor for every step
         res = None
         for i in range(n_steps):
-            res = self.step(x, c1, c2, order, c3=c3, anchor=anchor, weight=weight, **opts)
+            run = self.tr_step if method == "tr" else self.step
+            res = run(x, c1, c2, order, c3=c3, anchor=anchor, weight=weight, **opts)
             if check_every > 0 and (i + 1) % check_every == 0 and i + 1 < n_steps:
                 if int((res.status == 0).sum()) == 0:
                     return i + 1, res
