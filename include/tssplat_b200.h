@@ -598,6 +598,35 @@ int tsb_newton_tr_step(tsb_newton_t nw, float *x_dev, const float *anchor_dev, c
                        const tsb_terms_t *terms, const tsb_newton_tr_options_t *opt,
                        tsb_newton_tr_sphere_t *records_out_dev, void *stream);
 
+/* ---- Backtracking trust-region Newton step: the trust-region step that takes a fraction of a rejected step ----------
+ * tsb_newton_tr_step with bt == NULL (the same launches, the same bits).  With bt set, the same nine phases with two
+ * changes: phase 7 runs tsb_line_search at the bt->n_alpha step sizes alpha_k = 2^-k of the workspace's table (as
+ * tsb_newton_step does), and phase 8 is the rule below.  Per sphere, in fp64, with tsb_newton_tr_step's quantities
+ * (pred, rho from dPhi_0 = dPhi at alpha = 1, eta alpha^, |d|_M) and dPhi_k = Phi_c(x + alpha_k d) - Phi_c(x):
+ *   frozen, an unusable weight, g <= gtol: as tsb_newton_tr_step.
+ *   the full step is accepted (no tet inverts, pred > 0, rho > accept): as tsb_newton_tr_step, radius update included.
+ *   otherwise, if bd > 0, k* = the smallest k in [1, n_alpha) with alpha_k < eta alpha^ and
+ *   dPhi_k <= -sigma alpha_k bd (the Armijo test of tsb_newton_step).  Found: the step alpha_{k*} d is taken and
+ *   Delta = clamp(max(alpha_{k*} |d|_M, Delta / 4), radius_min, radius_max) (Delta before this step), so a step limited
+ *   by the inversion bound alone shrinks the radius by at most the quarter of a poor model instead of down to
+ *   eta alpha^ |d|_M.  Not found: rejected with tsb_newton_tr_step's radius update; then Delta < radius_min: STALLED.
+ * Records: tsb_newton_tr_sphere_t; alpha is the fraction taken (1, 2^-k* or 0) and delta its dPhi.  No floating-point
+ * atomics and every fold in a fixed order: the determinism and independence statements of tsb_newton_tr_step hold.  No
+ * device memory beyond tsb_newton_tr_step's (the line search's per-sphere outputs are sized for TSB_LINE_MAX_ALPHA
+ * steps from tsb_newton_create on); the first call allocates exactly as that one does and cannot be captured.
+ * Argument errors (TSB_E_INVALID, nothing launched): everything tsb_newton_tr_step rejects, n_alpha outside
+ * [2, TSB_LINE_MAX_ALPHA], sigma outside (0, 1/2) (NaN included), nonzero reserved words.  DESIGN.md section 5,
+ * "Backtracking trust-region step". */
+typedef struct {            /* 32 bytes */
+  int32_t n_alpha;          /* 2..TSB_LINE_MAX_ALPHA: step sizes alpha_k = 2^-k, k < n_alpha                          */
+  float sigma;              /* in (0, 1/2): the Armijo constant                                                        */
+  int32_t reserved[6];      /* must be 0                                                                               */
+} tsb_newton_backtrack_t;
+
+int tsb_newton_tr_step_ex(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const float *weight_dev,
+                          const tsb_terms_t *terms, const tsb_newton_tr_options_t *opt, const tsb_newton_backtrack_t *bt,
+                          tsb_newton_tr_sphere_t *records_out_dev, void *stream);
+
 /* Same computation for callers whose vertex positions live in HOST memory (e.g. a CPU-side
  * optimiser): copies x_host -> device, runs the fused launch, copies energy[3] and grad back,
  * asynchronously; the outputs are valid once `stream` has been synchronised and the host buffers

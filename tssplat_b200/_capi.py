@@ -26,7 +26,7 @@ EXPORTED_SYMBOLS = (
     "tsb_pcg_set_blocks", "tsb_pcg_solve", "tsb_sphere_axpy", "tsb_pcg_set_blocks_ex", "tsb_pcg_solve_ex",
     "tsb_pcg_enable_psd", "tsb_pcg_hvp_psd", "tsb_pcg_solve_tr",
     "tsb_newton_create", "tsb_newton_destroy", "tsb_newton_last_error", "tsb_newton_device_bytes", "tsb_newton_reset",
-    "tsb_newton_step", "tsb_newton_prox_step", "tsb_newton_tr_step", "tsb_energy_grad_host", "tsb_scale",
+    "tsb_newton_step", "tsb_newton_prox_step", "tsb_newton_tr_step", "tsb_newton_tr_step_ex", "tsb_energy_grad_host", "tsb_scale",
     "tsb_grad_limit", "tsb_adam_uniform_step",
     "tsb_surface_create", "tsb_surface_destroy", "tsb_surface_last_error", "tsb_surface_forward", "tsb_surface_backward",
     "tsb_surface_extract", "tsb_free_host", "tsb_setup_last_error",
@@ -80,6 +80,10 @@ class tsb_newton_tr_sphere_t(C.Structure):
                 ("delta", C.c_float), ("b_dot_d", C.c_float), ("pred", C.c_float), ("d_norm", C.c_float),
                 ("pcg_status", C.c_int32), ("n_hvp", C.c_int32), ("status", C.c_int32), ("first_vertex", C.c_int32),
                 ("reserved", C.c_int32 * 2)]
+
+
+class tsb_newton_backtrack_t(C.Structure):
+    _fields_ = [("n_alpha", C.c_int32), ("sigma", C.c_float), ("reserved", C.c_int32 * 6)]
 
 
 class tsb_info_t(C.Structure):
@@ -167,6 +171,9 @@ def _load() -> C.CDLL:
     lib.tsb_newton_prox_step.argtypes = [vp, vp, vp, vp, C.POINTER(tsb_terms_t), C.POINTER(tsb_newton_options_t), vp, vp]
     lib.tsb_newton_tr_step.restype = C.c_int
     lib.tsb_newton_tr_step.argtypes = [vp, vp, vp, vp, C.POINTER(tsb_terms_t), C.POINTER(tsb_newton_tr_options_t), vp, vp]
+    lib.tsb_newton_tr_step_ex.restype = C.c_int
+    lib.tsb_newton_tr_step_ex.argtypes = [vp, vp, vp, vp, C.POINTER(tsb_terms_t), C.POINTER(tsb_newton_tr_options_t),
+                                          C.POINTER(tsb_newton_backtrack_t), vp, vp]
     lib.tsb_energy_grad_host.restype = C.c_int
     lib.tsb_energy_grad_host.argtypes = [vp, vp, f32, f32, i32, f32, vp, vp, vp]
     lib.tsb_scale.restype = C.c_int

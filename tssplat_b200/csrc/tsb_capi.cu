@@ -19,6 +19,7 @@ static_assert(sizeof(tsb_newton_options_t) == 64, "tsb_newton_options_t must be 
 static_assert(sizeof(tsb_newton_sphere_t) == 64, "tsb_newton_sphere_t must be 64 bytes");
 static_assert(sizeof(tsb_newton_tr_options_t) == 64, "tsb_newton_tr_options_t must be 64 bytes");
 static_assert(sizeof(tsb_newton_tr_sphere_t) == 64, "tsb_newton_tr_sphere_t must be 64 bytes");
+static_assert(sizeof(tsb_newton_backtrack_t) == 32, "tsb_newton_backtrack_t must be 32 bytes");
 
 struct tsb_handle_s {
   int device = 0;
@@ -1070,9 +1071,22 @@ extern "C" {
 
 int tsb_newton_tr_step(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const float *weight_dev, const tsb_terms_t *terms,
                        const tsb_newton_tr_options_t *opt, tsb_newton_tr_sphere_t *records_out_dev, void *stream) {
+  return tsb_newton_tr_step_ex(nw, x_dev, anchor_dev, weight_dev, terms, opt, nullptr, records_out_dev, stream);
+}
+
+int tsb_newton_tr_step_ex(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const float *weight_dev, const tsb_terms_t *terms,
+                          const tsb_newton_tr_options_t *opt, const tsb_newton_backtrack_t *bt,
+                          tsb_newton_tr_sphere_t *records_out_dev, void *stream) {
   if (!nw) return TSB_E_INVALID;
   int rc = newton_tr_check(nw, x_dev, anchor_dev, weight_dev, terms, opt);
   if (rc != TSB_OK) return rc;
+  if (bt) {
+    if (bt->n_alpha < 2 || bt->n_alpha > TSB_LINE_MAX_ALPHA)
+      return newton_fail(nw, TSB_E_INVALID, "n_alpha must be in [2, " + std::to_string(TSB_LINE_MAX_ALPHA) + "]");
+    if (!(bt->sigma > 0.f && bt->sigma < 0.5f)) return newton_fail(nw, TSB_E_INVALID, "sigma must be in (0, 1/2)");
+    for (int32_t r : bt->reserved)
+      if (r != 0) return newton_fail(nw, TSB_E_INVALID, "reserved fields must be 0");
+  }
   tsb_pcg_t s = nw->s;
   tsb_handle_t h = s->h;
   DeviceGuard guard(h->device);
@@ -1103,13 +1117,14 @@ int tsb_newton_tr_step(tsb_newton_t nw, float *x_dev, const float *anchor_dev, c
   // 5: the trust-region solve
   rc = tsb_pcg_solve_tr(s, x_dev, W.b, terms, &po, shift, nw->tr_radius, W.d, nullptr, nullptr, st);
   if (rc != TSB_OK) return newton_fail(nw, rc, s->err);
-  // 6: b.d and |d|^2 (prox: and d.(x - y)) per chunk;  7: the line search at alpha = 1
+  // 6: b.d and |d|^2 (prox: and d.(x - y)) per chunk;  7: the line search at alpha = 1 (bt: at 2^-k, k < n_alpha)
   e = tsb::launch_newton_dots(s->P, W, p, st);
   if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
-  rc = tsb_line_search(h, x_dev, W.d, terms, W.alphas, 1, nw->delta, nullptr, W.sphere_delta, W.sphere_step, st);
+  rc = tsb_line_search(h, x_dev, W.d, terms, W.alphas, bt ? bt->n_alpha : 1, nw->delta, nullptr, W.sphere_delta, W.sphere_step, st);
   if (rc != TSB_OK) return newton_fail(nw, rc, h->err);
-  // 8-9: decision, step
-  e = tsb::launch_newton_tr_decide(s->P, W, T, R, p, records_out_dev, st);
+  // 8-9: decision (bt: with backtracking), step
+  const tsb::NewtonBacktrack B{bt ? bt->sigma : 0.f, bt ? bt->n_alpha : 1};
+  e = tsb::launch_newton_tr_decide(s->P, W, T, R, p, records_out_dev, st, bt ? &B : nullptr);
   if (e == cudaSuccess) e = tsb::launch_sphere_axpy(s->P, x_dev, W.alpha_sphere, W.d, x_dev, st);
   if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
   return TSB_OK;

@@ -691,10 +691,13 @@ __global__ void __launch_bounds__(kT) newton_tr_radius_kernel(const PcgParams s,
   t.radius[c] = float(S.radius);
 }
 
-// Acceptance and radius update of every component (thread = component); see tsb_newton_tr_step in the header.
-template <bool PROX>
+// Acceptance and radius update of every component (thread = component); see tsb_newton_tr_step in the header.  LS: a
+// step the trust-region rule rejects is backtracked to the largest 2^-k (k >= 1) of the line search with the Armijo
+// decrease below the inversion bound (tsb_newton_tr_step_ex); the backtracking options b are read only then.
+template <bool PROX, bool LS = false>
 __device__ __forceinline__ void decide_tr_body(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t,
-                                               const NewtonTrRule &r, const ProxParams &p, tsb_newton_tr_sphere_t *__restrict__ out) {
+                                               const NewtonTrRule &r, const ProxParams &p, tsb_newton_tr_sphere_t *__restrict__ out,
+                                               const NewtonBacktrack &b = NewtonBacktrack{}) {
   const int c = blockIdx.x * kT + int(threadIdx.x);
   if (c >= s.n_components) return;
   const PcgComp C = s.comp[c];
@@ -725,19 +728,33 @@ __device__ __forceinline__ void decide_tr_body(const PcgParams &s, const NewtonP
       N.status = TSB_NEWTON_CONVERGED;
     } else {
       pred = bdf - 0.5 * dHd;
-      const double dphi = step_change<PROX>(w.sphere_delta[4 * size_t(c)], wc, 1.0, dx, dd);
+      const float *dl = w.sphere_delta + (LS ? size_t(c) * size_t(b.n_alpha) * 4 : 4 * size_t(c));   // [n_alpha][4]
+      const double dphi = step_change<PROX>(dl[0], wc, 1.0, dx, dd);
       if (pred > 0.0) rho = -dphi / pred;
       const double lim = double(r.eta) * double(w.sphere_step[c]);
       const bool flips = !(1.0 < lim);
+      const double r0 = S.radius;
       if (flips) S.radius = fmin(0.25 * S.radius, lim * dn);
       else if (!(rho >= 0.25)) S.radius = 0.25 * dn;
       else if (rho > 0.75 && (pst == TSB_PCG_BOUNDARY || pst == TSB_PCG_NEGCURV_BOUNDARY))
         S.radius = fmin(2.0 * S.radius, double(r.radius_max));
+      int ks = -1;
       if (!flips && pred > 0.0 && rho > double(r.accept)) {
         alpha = 1.f;
         delta = float(dphi);
-      } else if (S.radius < double(r.radius_min)) {
-        N.status = TSB_NEWTON_STALLED;
+      } else {
+        if (LS && bdf > 0.0)
+          for (int k = 1; k < b.n_alpha; ++k) {
+            const double a = double(w.alphas[k]);
+            if (a < lim && step_change<PROX>(dl[4 * k], wc, a, dx, dd) <= -double(b.sigma) * a * bdf) { ks = k; break; }
+          }
+        if (LS && ks > 0) {       // the radius shrinks by at most the quarter of a poor model, to no less than the step
+          alpha = w.alphas[ks];
+          delta = float(step_change<PROX>(dl[4 * ks], wc, double(alpha), dx, dd));
+          S.radius = fmin(double(r.radius_max), fmax(double(r.radius_min), fmax(double(alpha) * dn, 0.25 * r0)));
+        } else if (S.radius < double(r.radius_min)) {
+          N.status = TSB_NEWTON_STALLED;
+        }
       }
     }
   }
@@ -771,6 +788,18 @@ __global__ void __launch_bounds__(kT) newton_decide_tr_prox_kernel(const PcgPara
                                                                    const NewtonTrRule r, tsb_newton_tr_sphere_t *__restrict__ out,
                                                                    const ProxParams p) {
   decide_tr_body<true>(s, w, t, r, p, out);
+}
+
+__global__ void __launch_bounds__(kT) newton_decide_trls_kernel(const PcgParams s, const NewtonParams w, const NewtonTrParams t,
+                                                                const NewtonTrRule r, const NewtonBacktrack b,
+                                                                tsb_newton_tr_sphere_t *__restrict__ out) {
+  decide_tr_body<false, true>(s, w, t, r, ProxParams{}, out, b);
+}
+
+__global__ void __launch_bounds__(kT) newton_decide_trls_prox_kernel(const PcgParams s, const NewtonParams w, const NewtonTrParams t,
+                                                                     const NewtonTrRule r, const NewtonBacktrack b,
+                                                                     tsb_newton_tr_sphere_t *__restrict__ out, const ProxParams p) {
+  decide_tr_body<true, true>(s, w, t, r, p, out, b);
 }
 
 unsigned with_orphans(const PcgParams &s) { return unsigned(s.n_chunks + (s.n_orphans + kT - 1) / kT); }
@@ -876,9 +905,11 @@ cudaError_t launch_newton_tr_radius(const PcgParams &s, const NewtonParams &w, c
 }
 
 cudaError_t launch_newton_tr_decide(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t, const NewtonTrRule &r,
-                                    const ProxParams *p, tsb_newton_tr_sphere_t *out, cudaStream_t st) {
+                                    const ProxParams *p, tsb_newton_tr_sphere_t *out, cudaStream_t st, const NewtonBacktrack *bt) {
   const unsigned comp_blocks = unsigned((s.n_components + kT - 1) / kT);
-  if (p) newton_decide_tr_prox_kernel<<<comp_blocks, kT, 0, st>>>(s, w, t, r, out, *p);
+  if (bt && p) newton_decide_trls_prox_kernel<<<comp_blocks, kT, 0, st>>>(s, w, t, r, *bt, out, *p);
+  else if (bt) newton_decide_trls_kernel<<<comp_blocks, kT, 0, st>>>(s, w, t, r, *bt, out);
+  else if (p) newton_decide_tr_prox_kernel<<<comp_blocks, kT, 0, st>>>(s, w, t, r, out, *p);
   else newton_decide_tr_kernel<<<comp_blocks, kT, 0, st>>>(s, w, t, r, out);
   return cudaGetLastError();
 }

@@ -111,6 +111,11 @@ struct NewtonTrRule {         // the options the trust-region kernels read
   float gtol, radius_init, radius_min, radius_max, accept, eta;
 };
 
+struct NewtonBacktrack {      // the backtracking options of tsb_newton_tr_step_ex (tsb_newton_backtrack_t)
+  float sigma;
+  int32_t n_alpha;
+};
+
 cudaError_t launch_pcg_blocks(const PcgParams &s, const float *diag, float rel_floor, float *inv_out, cudaStream_t st);
 // blocks D_v + shift[c] I (over the chunk table; orphan vertices unshifted)
 cudaError_t launch_pcg_blocks_shift(const PcgParams &s, const float *diag, float rel_floor, const float *shift, float *inv_out,
@@ -140,8 +145,10 @@ cudaError_t launch_newton_tr_prep(const PcgParams &s, const NewtonParams &w, con
 // after the preconditioner is set: b^T P b per component, Delta_c on a first step, the fp32 radius
 cudaError_t launch_newton_tr_radius(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t, const NewtonTrRule &r,
                                     cudaStream_t st);
-// acceptance, radius update, records (out may be null)
+// acceptance, radius update, records (out may be null); bt != nullptr: a rejected step is backtracked along the line
+// search's n_alpha step sizes (tsb_newton_tr_step_ex)
 cudaError_t launch_newton_tr_decide(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t, const NewtonTrRule &r,
-                                    const ProxParams *p, tsb_newton_tr_sphere_t *out, cudaStream_t st);
+                                    const ProxParams *p, tsb_newton_tr_sphere_t *out, cudaStream_t st,
+                                    const NewtonBacktrack *bt = nullptr);
 
 }  // namespace tsb

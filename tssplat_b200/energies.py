@@ -247,10 +247,11 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         ``newton.NEWTON_DEFAULTS``.  The workspace, ``self.device_newton``, is created on first use (sharing
         ``self.device_pcg``); its ``reset()`` restarts every sphere.  Returns the ``NewtonStepResult``.
         ``FLAGS.newton_method = "tr"`` takes the trust-region step instead (``DeviceNewton.tr_step``; ``opts`` then the
-        fields of ``newton.NEWTON_TR_DEFAULTS``; returns a ``NewtonTRStepResult``)."""
+        fields of ``newton.NEWTON_TR_DEFAULTS``; returns a ``NewtonTRStepResult``), and ``"trls"`` the backtracking
+        trust-region step (``DeviceNewton.trls_step``; the fields of ``newton.NEWTON_TRLS_DEFAULTS``)."""
         nw = self._device_newton()
         c1, c2 = self.coeff_scheduler(it)
-        run = nw.tr_step if self._newton_method() == "tr" else nw.step
+        run = {"lm": nw.step, "tr": nw.tr_step, "trls": nw.trls_step}[self._newton_method()]
         return run(x.data, c1, c2, self.order_at(it), c3=self.amips_coeff, **opts)
 
     def _newton_method(self) -> str:
@@ -268,7 +269,8 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         Updates ``x.data`` in place with no host read (``tsb_newton_prox_step``) and returns the last
         ``NewtonStepResult``.  ``restart`` resets the workspace first: a new anchor is a new problem, and a sphere frozen
         on the old one must not stay frozen.  ``opts``: the fields of ``newton.NEWTON_DEFAULTS`` (of
-        ``newton.NEWTON_TR_DEFAULTS`` with ``FLAGS.newton_method = "tr"``, which takes trust-region steps)."""
+        ``newton.NEWTON_TR_DEFAULTS`` with ``FLAGS.newton_method = "tr"``, which takes trust-region steps, and of
+        ``newton.NEWTON_TRLS_DEFAULTS`` with ``"trls"``, which takes backtracking trust-region steps)."""
         if n_steps < 1:
             raise ValueError("n_steps must be >= 1")
         nw = self._device_newton()

@@ -20,6 +20,8 @@ stream without a host read.  Given an ``anchor`` y and per-sphere weights w, the
 data term keeps its first-order optimiser.  ``DeviceNewton.tr_step`` is the trust-region alternative
 (``tsb_newton_tr_step``): no damping shift, a per-sphere radius in the preconditioner norm inside which the solve
 (``DevicePCG.solve(..., radius=)``, ``tsb_pcg_solve_tr``) follows negative curvature to the boundary.
+``DeviceNewton.trls_step`` (``tsb_newton_tr_step_ex``) is the same step, but one the trust-region rule rejects is
+backtracked along ``2^-k`` with the Armijo test instead of being dropped whole.
 """
 from __future__ import annotations
 
@@ -29,7 +31,8 @@ from typing import Callable, NamedTuple, Optional, Union
 import torch
 
 __all__ = ["hess_blocks", "block_jacobi", "apply_blocks", "pcg", "PCGResult", "DevicePCG", "DevicePCGResult", "DeviceNewton",
-           "NewtonStepResult", "NEWTON_DEFAULTS", "HESSIANS", "NewtonTRStepResult", "NEWTON_TR_DEFAULTS", "METHODS"]
+           "NewtonStepResult", "NEWTON_DEFAULTS", "HESSIANS", "NewtonTRStepResult", "NEWTON_TR_DEFAULTS", "NEWTON_TRLS_DEFAULTS",
+           "METHODS"]
 
 
 def hess_blocks(planes: torch.Tensor) -> torch.Tensor:
@@ -298,15 +301,19 @@ class NewtonStepResult(NamedTuple):
 NEWTON_TR_DEFAULTS = dict(max_iter=20, rtol=1e-2, rel_floor=1e-6, gtol=0.0, radius_init=1.0, radius_min=1e-12,
                           radius_max=1e12, accept=1e-4, eta=0.9)
 
-#: the steps of ``DeviceNewton.minimize``: Levenberg-Marquardt (``step``) or trust region (``tr_step``)
-METHODS = ("lm", "tr")
+#: options of ``DeviceNewton.trls_step``: ``NEWTON_TR_DEFAULTS`` and the backtracking (``tsb_newton_backtrack_t``)
+NEWTON_TRLS_DEFAULTS = dict(NEWTON_TR_DEFAULTS, n_alpha=8, sigma=1e-4)
+
+#: the steps of ``DeviceNewton.minimize``: Levenberg-Marquardt (``step``), trust region (``tr_step``) or backtracking
+#: trust region (``trls_step``)
+METHODS = ("lm", "tr", "trls")
 
 
 class NewtonTRStepResult(NamedTuple):
     """What ``DeviceNewton.tr_step`` returns: device tensors [S], spheres in the order of their lowest vertex ids
     (``tsb_newton_tr_sphere_t`` in ``include/tssplat_b200.h``)."""
     grad_norm: torch.Tensor         # f32: |grad_c| before the step (0 once the sphere is frozen)
-    alpha: torch.Tensor             # f32: 1 when the step was taken, else 0
+    alpha: torch.Tensor             # f32: 1 when the step was taken, else 0 (trls_step: the fraction 2^-k taken, or 0)
     delta: torch.Tensor             # f32: objective change of the step taken (0 if none)
     radius: torch.Tensor            # f64: trust radius after the update (preconditioner norm)
     rho: torch.Tensor               # f64: gain ratio -delta(1) / pred (0 when pred <= 0 or no decision ran)
@@ -406,6 +413,42 @@ class DeviceNewton:
         o = {**NEWTON_TR_DEFAULTS, **opts}
         return self._capi.tsb_newton_tr_options_t(**{k: (int(v) if k == "max_iter" else float(v)) for k, v in o.items()})
 
+    def trls_options(self, **opts):
+        """(``tsb_newton_tr_options_t``, ``tsb_newton_backtrack_t``) from ``NEWTON_TRLS_DEFAULTS`` updated with ``opts``."""
+        bad = set(opts) - set(NEWTON_TRLS_DEFAULTS)
+        if bad:
+            raise TypeError(f"unknown backtracking trust-region options: {sorted(bad)}")
+        o = {**NEWTON_TRLS_DEFAULTS, **opts}
+        bt = self._capi.tsb_newton_backtrack_t(n_alpha=int(o.pop("n_alpha")), sigma=float(o.pop("sigma")))
+        return self.tr_options(**o), bt
+
+    def _tr_run(self, x, c1, c2, order, c3, anchor, weight, opt, bt, what) -> NewtonTRStepResult:
+        w = self._x_anchor(x, anchor, weight)
+        raw = torch.empty((self.n_spheres, 16), dtype=torch.int32, device=self.tet_sp.device)
+        terms = self._capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
+        args = (self._nw, x.data_ptr(), anchor.data_ptr() if anchor is not None else None, w.data_ptr() if w is not None else None,
+                C.byref(terms), C.byref(opt))
+        st = self._stream_ptr(self.tet_sp.device)
+        if bt is None:
+            rc = self._capi.lib.tsb_newton_tr_step(*args, raw.data_ptr(), st)
+        else:
+            rc = self._capi.lib.tsb_newton_tr_step_ex(*args, C.byref(bt), raw.data_ptr(), st)
+        self._check(rc, what)
+        f64, f32 = raw[:, 0:4].view(torch.float64), raw[:, 4:10].view(torch.float32)
+        return NewtonTRStepResult(f32[:, 0], f32[:, 1], f32[:, 2], f64[:, 0], f64[:, 1], f32[:, 4], f32[:, 5], raw[:, 10],
+                                  raw[:, 11], f32[:, 3], raw[:, 12], raw[:, 13])
+
+    def trls_step(self, x: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0,
+                  anchor: Optional[torch.Tensor] = None, weight=None, **opts) -> NewtonTRStepResult:
+        """One backtracking trust-region Newton step (``tsb_newton_tr_step_ex``): ``tr_step``, except that a step the
+        trust-region rule rejects (it would invert a tet, or the model predicted the change poorly) is backtracked to the
+        largest ``2^-k``, ``1 <= k < n_alpha``, below the inversion bound with the Armijo decrease
+        ``dPhi <= -sigma 2^-k b.d``; the radius then becomes ``max(2^-k |d|_M, radius / 4)``, clamped.  The result's
+        ``alpha`` is the fraction taken (1, ``2^-k`` or 0).  ``opts``: the fields of ``NEWTON_TRLS_DEFAULTS``.  The first
+        call on a workspace allocates (as ``tr_step``'s), so it cannot be captured in a CUDA graph; later ones can."""
+        opt, bt = self.trls_options(**opts)
+        return self._tr_run(x, c1, c2, order, c3, anchor, weight, opt, bt, "trls_step")
+
     def tr_step(self, x: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0,
                 anchor: Optional[torch.Tensor] = None, weight=None, **opts) -> NewtonTRStepResult:
         """One trust-region Newton step (``tsb_newton_tr_step``) of ``c1 * smooth + c2 * barrier (+ c3 * amips)`` on every
@@ -414,17 +457,7 @@ class DeviceNewton:
         negative curvature to its boundary), the step is taken whole or not at all, and the gain ratio grows or shrinks
         the radius.  ``opts``: the fields of ``NEWTON_TR_DEFAULTS``.  The first call on a workspace allocates, so it
         cannot be captured in a CUDA graph; later ones can."""
-        w = self._x_anchor(x, anchor, weight)
-        raw = torch.empty((self.n_spheres, 16), dtype=torch.int32, device=self.tet_sp.device)
-        terms = self._capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
-        opt = self.tr_options(**opts)
-        rc = self._capi.lib.tsb_newton_tr_step(self._nw, x.data_ptr(), anchor.data_ptr() if anchor is not None else None,
-                                               w.data_ptr() if w is not None else None, C.byref(terms), C.byref(opt),
-                                               raw.data_ptr(), self._stream_ptr(self.tet_sp.device))
-        self._check(rc, "tr_step")
-        f64, f32 = raw[:, 0:4].view(torch.float64), raw[:, 4:10].view(torch.float32)
-        return NewtonTRStepResult(f32[:, 0], f32[:, 1], f32[:, 2], f64[:, 0], f64[:, 1], f32[:, 4], f32[:, 5], raw[:, 10],
-                                  raw[:, 11], f32[:, 3], raw[:, 12], raw[:, 13])
+        return self._tr_run(x, c1, c2, order, c3, anchor, weight, self.tr_options(**opts), None, "tr_step")
 
     def step(self, x: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0, anchor: Optional[torch.Tensor] = None,
              weight=None, **opts) -> NewtonStepResult:
@@ -455,8 +488,9 @@ class DeviceNewton:
 
     def minimize(self, x: torch.Tensor, n_steps: int, c1: float, c2: float, order: int, c3: float = 0.0,
                  check_every: int = 0, anchor: Optional[torch.Tensor] = None, weight=None, method: str = "lm", **opts):
-        """Up to ``n_steps`` calls of ``step`` (``method="lm"``) or ``tr_step`` (``method="tr"``, ``opts`` then the fields
-        of ``NEWTON_TR_DEFAULTS``); returns (steps run, the last result).  ``check_every = 0`` never touches the host
+        """Up to ``n_steps`` calls of ``step`` (``method="lm"``), ``tr_step`` (``method="tr"``, ``opts`` then the fields
+        of ``NEWTON_TR_DEFAULTS``) or ``trls_step`` (``method="trls"``, the fields of ``NEWTON_TRLS_DEFAULTS``); returns
+        (steps run, the last result).  ``check_every = 0`` never touches the host
         (capturable); ``k > 0`` reads one integer, the number of spheres still active, every ``k`` steps and stops when
         it is 0 (refused while the stream is being captured).  ``anchor`` and ``weight``: the proximal step of
         ``step``."""
@@ -471,7 +505,7 @@ class DeviceNewton:
             weight = self.pcg._shift(weight, "weight")         # one tensor for every step
         res = None
         for i in range(n_steps):
-            run = self.tr_step if method == "tr" else self.step
+            run = {"lm": self.step, "tr": self.tr_step, "trls": self.trls_step}[method]
             res = run(x, c1, c2, order, c3=c3, anchor=anchor, weight=weight, **opts)
             if check_every > 0 and (i + 1) % check_every == 0 and i + 1 < n_steps:
                 if int((res.status == 0).sum()) == 0:
