@@ -42,6 +42,24 @@ __device__ __forceinline__ void swap_col(double (&ev)[3], double (&Q)[3][3], int
   for (int r = 0; r < 3; ++r) { t = Q[r][a]; Q[r][a] = Q[r][b]; Q[r][b] = t; }
 }
 
+// One-sided (Hestenes) Jacobi rotation of columns p and q of W = F V, and of V with them, that makes w_p and w_q
+// orthogonal.  Its angle comes from the columns' own dot products, accurate relative to |w_p| |w_q|; the entries of F^T F
+// carry an error of eps s_1^2, which loses the directions of every s_i^2 below that.
+__device__ __forceinline__ void hestenes_rot(double (&W)[3][3], double (&V)[3][3], int p, int q) {
+  const double al = W[0][p] * W[0][p] + W[1][p] * W[1][p] + W[2][p] * W[2][p];
+  const double be = W[0][q] * W[0][q] + W[1][q] * W[1][q] + W[2][q] * W[2][q];
+  const double ga = W[0][p] * W[0][q] + W[1][p] * W[1][q] + W[2][p] * W[2][q];
+  if (ga == 0.0) return;
+  const double theta = (be - al) / (2.0 * ga);
+  const double t = copysign(1.0, theta) / (fabs(theta) + sqrt(theta * theta + 1.0));
+  const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    double a = c * W[r][p] - s * W[r][q]; W[r][q] = s * W[r][p] + c * W[r][q]; W[r][p] = a;
+    a = c * V[r][p] - s * V[r][q]; V[r][q] = s * V[r][p] + c * V[r][q]; V[r][p] = a;
+  }
+}
+
 __device__ __forceinline__ void normalize(double (&u)[3]) {
   const double s = 1.0 / sqrt(u[0] * u[0] + u[1] * u[1] + u[2] * u[2]);
   u[0] *= s; u[1] *= s; u[2] *= s;
@@ -51,7 +69,7 @@ __device__ __forceinline__ void normalize(double (&u)[3]) {
 __device__ constexpr int kPi[3] = {0, 0, 1}, kPj[3] = {1, 2, 2}, kPk[3] = {2, 1, 0};
 
 // One thread per tet: F in fp64 from the fp32 edges and B, activity from the sign of det F, signed SVD from the Jacobi
-// eigen-decomposition of F^T F, then the clamped eigen-system.
+// eigen-decomposition of F^T F refined by one one-sided Jacobi sweep on F V, then the clamped eigen-system.
 __global__ void __launch_bounds__(kPsdProjectT) psd_project_kernel(const PsdParams p, const float *__restrict__ x, int order,
                                                                    int amips) {
   const int t = blockIdx.x * kPsdProjectT + int(threadIdx.x);
@@ -95,6 +113,32 @@ __global__ void __launch_bounds__(kPsdProjectT) psd_project_kernel(const PsdPara
   if (det3(V) < 0.0)
 #pragma unroll
     for (int r = 0; r < 3; ++r) V[r][2] = -V[r][2];
+  // one one-sided Jacobi sweep on the columns of W = F V refines V where F^T F cannot resolve it (s_2 or s_3 below
+  // ~ sqrt(eps) s_1: needles, collapsing planes); then descending column norms and V proper again
+  double W[3][3];
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+#pragma unroll
+    for (int i = 0; i < 3; ++i) W[r][i] = F[r][0] * V[0][i] + F[r][1] * V[1][i] + F[r][2] * V[2][i];
+  hestenes_rot(W, V, 0, 1);
+  hestenes_rot(W, V, 0, 2);
+  hestenes_rot(W, V, 1, 2);
+  {
+    double n2[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) n2[i] = W[0][i] * W[0][i] + W[1][i] * W[1][i] + W[2][i] * W[2][i];
+    auto swap_wv = [&](int a, int b) {
+      swap_col(n2, V, a, b);
+#pragma unroll
+      for (int r = 0; r < 3; ++r) { const double t = W[r][a]; W[r][a] = W[r][b]; W[r][b] = t; }
+    };
+    if (n2[0] < n2[1]) swap_wv(0, 1);
+    if (n2[1] < n2[2]) swap_wv(1, 2);
+    if (n2[0] < n2[1]) swap_wv(0, 1);
+  }
+  if (det3(V) < 0.0)
+#pragma unroll
+    for (int r = 0; r < 3; ++r) { V[r][2] = -V[r][2]; W[r][2] = -W[r][2]; }
   // u_1 = F v_1 / s_1, u_2 = the part of F v_2 orthogonal to u_1, u_3 = u_1 x u_2; s_3 = det F / (s_1 s_2) carries the
   // sign (reflections land in s_3, never in U or V) and stays accurate as s_3 -> 0
   double u[3][3], sg[3];
@@ -102,7 +146,7 @@ __global__ void __launch_bounds__(kPsdProjectT) psd_project_kernel(const PsdPara
 #pragma unroll
   for (int i = 0; i < 3; ++i)
 #pragma unroll
-    for (int r = 0; r < 3; ++r) w[i][r] = F[r][0] * V[0][i] + F[r][1] * V[1][i] + F[r][2] * V[2][i];
+    for (int r = 0; r < 3; ++r) w[i][r] = W[r][i];
   sg[0] = sqrt(w[0][0] * w[0][0] + w[0][1] * w[0][1] + w[0][2] * w[0][2]);
 #pragma unroll
   for (int r = 0; r < 3; ++r) u[0][r] = w[0][r] / sg[0];     // sg[0] > 0: det F != 0
