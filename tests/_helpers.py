@@ -232,13 +232,38 @@ def _rel_u(x, X, xr, Xr):
     return (s - c) + e
 
 
-def emulate_kernel(plan, x, c1, c2, order, gradH=1.0, dtype=np.float64, c3=None):
+def amips_psi(F, tr, j23):
+    """The kernel's per-tet AMIPS energy psi = tr / (3 J^(2/3)) - 1 in its deviatoric form, in F's dtype: with C = F^T
+    F, m = tr / 3 and D = C - m I (diagonal from differences of C's diagonal, tr D = 0), psi = (m/2 |D|^2 - det D) /
+    (l (m^2 + m l + l^2)), l = j23 = J^(2/3).  F [t, 3, 3], tr and j23 [t]."""
+    dt = F.dtype.type
+    C = np.einsum("tri,trj->tij", F, F)
+    a01, a02, a12 = C[:, 0, 0] - C[:, 1, 1], C[:, 0, 0] - C[:, 2, 2], C[:, 1, 1] - C[:, 2, 2]
+    third = dt(1.0) / dt(3.0)
+    d0, d1 = (a01 + a02) * third, (a12 - a01) * third
+    d2 = -(d0 + d1)
+    o01, o02, o12 = C[:, 0, 1], C[:, 0, 2], C[:, 1, 2]
+    dd = (d0 * d0 + d1 * d1 + d2 * d2) + dt(2.0) * (o01 * o01 + o02 * o02 + o12 * o12)
+    detD = d0 * (d1 * d2 - o12 * o12) - o01 * (o01 * d2 - o12 * o02) + o02 * (o01 * o12 - d1 * o02)
+    m = tr * third
+    return (dt(0.5) * m * dd - detD) / (j23 * (m * (m + j23) + j23 * j23))
+
+
+def emulate_kernel(plan, x, c1, c2, order, gradH=1.0, dtype=np.float64, c3=None, stats=None):
     """numpy re-enactment of energy_grad_kernel (tsb_kernels.cu) on the host plan: every CTA, every
     warp walks its cell stream exactly as the kernel does (row blocks, then tet cells, segment by
     segment), with the same formulas.  Returns (energy_total, smooth, barrier, grad[n,3]); with c3
     (the AMIPS coefficient; the plan must be built with enable_amips) it also evaluates the AMIPS term of
     every J > 0 tet from the plan's per-cell rest inverses (Bt, wtc0) and returns
-    (energy_total, smooth, barrier, amips, grad[n,3])."""
+    (energy_total, smooth, barrier, amips, grad[n,3]).
+
+    stats: a dict, filled with the per-sphere records of tsb_energy_grad_spheres folded per component (the plan's
+    component order): "smooth", "barrier", "amips" (fp64 sums of the per-row and per-tet values), "n_inverted" (tets
+    with J < 0) and "min_J" (smallest J of the component's real tets; padding tets have 1/det(Dm) = 0)."""
+    if stats is not None:
+        nc = plan["n_components"]
+        stats.update(smooth=np.zeros(nc), barrier=np.zeros(nc), amips=np.zeros(nc),
+                     n_inverted=np.zeros(nc, np.int64), min_J=np.full(nc, np.inf))
     G, NW, glob = plan["grid"], plan["nw"], bool(plan["mode_global"])
     IB = 4 if glob else 2
     idt = np.uint32 if glob else np.uint16
@@ -337,7 +362,10 @@ def emulate_kernel(plan, x, c1, c2, order, gradH=1.0, dtype=np.float64, c3=None)
                     assert np.isnan(grad[gids[ra]]).all(), "a vertex row has two writers"
                     grad[gids[ra]] = gradH * c1 * tot[lead[::L]]
                     uref = U[h["x4off"]] if glob else U[0]
-                    es += 0.5 * np.einsum("lr,lr->", ui[lead] - uref, tot[lead[::L]])
+                    de = 0.5 * np.einsum("lr,lr->", ui[lead] - uref, tot[lead[::L]])
+                    es += de
+                    if stats is not None:
+                        stats["smooth"][h["comp"]] += float(de)
                     rows_seen += int(lead.sum())
                 assert ntc == 0 or w < NW - 1 or NW == 1, "the signalling warp must own no tets"
                 for tc in range(ntc):
@@ -352,6 +380,13 @@ def emulate_kernel(plan, x, c1, c2, order, gradH=1.0, dtype=np.float64, c3=None)
                     inv = J < 0
                     m = np.where(inv, -J, 0.0)
                     eb += (m ** order).sum()
+                    if stats is not None:
+                        cp = h["comp"]
+                        stats["barrier"][cp] += float((m ** order).astype(np.float64).sum())
+                        stats["n_inverted"][cp] += int(inv.sum())
+                        real = idet != 0                                                # padding: 1/det(Dm) = 0
+                        if real.any():
+                            stats["min_J"][cp] = min(stats["min_J"][cp], float(J[real].min()))
                     coef = order * m ** (order - 1)
                     k = (-coef * idet * c2 * gradH)[:, None]
                     g1, g2, g3 = k * c23, k * np.cross(e3, e1), k * np.cross(e1, e2)
@@ -365,7 +400,10 @@ def emulate_kernel(plan, x, c1, c2, order, gradH=1.0, dtype=np.float64, c3=None)
                         Jp = J[ok]
                         tr = (F * F).sum(axis=(1, 2))
                         j23 = np.cbrt(Jp) ** 2
-                        ea += (tr / (3 * j23) - 1).sum()
+                        psi = amips_psi(F, tr, j23)
+                        ea += psi.sum()
+                        if stats is not None:
+                            stats["amips"][h["comp"]] += float(psi.astype(np.float64).sum())
                         cof = np.linalg.det(F)[:, None, None] * np.linalg.inv(F).transpose(0, 2, 1)
                         P = (2 / (3 * j23) * c3 * gradH)[:, None, None] * (F - (tr / (3 * Jp))[:, None, None] * cof)
                         gk = P @ B.transpose(0, 2, 1)                                             # [tet][r][k]: vertex k+1

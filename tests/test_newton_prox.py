@@ -386,7 +386,6 @@ def test_prox_convergence_mixed_pack(ext, amips):
     wn = w.double().cpu().numpy()
     e0, q0, g0, _ = _oracle_phi(P, x.detach(), yn, wn, grad=True)
     phi_start = e0 + wn * q0
-    n_tets = np.bincount(P.tsid, minlength=S).astype(float)
     quiet = np.arange(S) % 4 != 0
     gtol = 1e-3 * float(g0[quiet].min())
     acc = np.zeros(S)
@@ -397,7 +396,7 @@ def test_prox_convergence_mixed_pack(ext, amips):
         assert (d <= 0).all(), t
         acc += d
         e, q = _oracle_phi(P, x.detach(), yn, wn)
-        tol = 1e-4 * np.abs(phi_start) + E.amips_coeff * n_tets * 2.0 ** -21
+        tol = 1e-4 * np.abs(phi_start)
         err = np.abs(e + wn * q - phi_start - acc)
         checked = quiet if amips else np.ones(S, bool)
         assert (err[checked] <= tol[checked]).all(), (t, float((err / tol)[checked].max()))

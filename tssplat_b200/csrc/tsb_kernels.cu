@@ -979,7 +979,25 @@ __global__ void __launch_bounds__(NW * 32, MINB) energy_grad_kernel(const KParam
 #pragma unroll
             for (int c = 0; c < 3; ++c) tr = fmaf(Fm[r][c], Fm[r][c], tr);
           const float cb = cbrtf(J), j23 = cb * cb;
-          dea += double(tr / (3.f * j23) - 1.f);
+          {
+            // psi = (m - l) / l with m = tr / 3 and l = J^(2/3), formed without that difference of two values near 1 (it
+            // costs about an ulp of 1 per tet, where psi is O(sigma^2) near a rotation and uniform scaling): with C = F^T F
+            // and its deviator D = C - m I (tr D = 0), m^3 - l^3 = m^3 - det C = m/2 |D|^2 - det D, so psi = (m/2 |D|^2 -
+            // det D) / (l (m^2 + m l + l^2)).  D's diagonal is formed from differences of C's (exact when they are close,
+            // Sterbenz), so only the rounding of C enters it (DESIGN.md section 5, "Per-sphere statistics")
+            float Cm[3][3];
+#pragma unroll
+            for (int i = 0; i < 3; ++i)
+#pragma unroll
+              for (int j = i; j < 3; ++j) Cm[i][j] = Fm[0][i] * Fm[0][j] + Fm[1][i] * Fm[1][j] + Fm[2][i] * Fm[2][j];
+            const float a01 = Cm[0][0] - Cm[1][1], a02 = Cm[0][0] - Cm[2][2], a12 = Cm[1][1] - Cm[2][2];
+            const float d0 = (a01 + a02) * (1.f / 3.f), d1 = (a12 - a01) * (1.f / 3.f), d2 = -(d0 + d1);
+            const float o01 = Cm[0][1], o02 = Cm[0][2], o12 = Cm[1][2];
+            const float dd = fmaf(d0, d0, fmaf(d1, d1, d2 * d2)) + 2.f * fmaf(o01, o01, fmaf(o02, o02, o12 * o12));
+            const float detD = d0 * (d1 * d2 - o12 * o12) - o01 * (o01 * d2 - o12 * o02) + o02 * (o01 * o12 - d1 * o02);
+            const float m = tr * (1.f / 3.f);
+            dea += double(fmaf(0.5f * m, dd, -detD) / (j23 * fmaf(m, m + j23, j23 * j23)));
+          }
           if (grad) {
             const float a = 2.f / (3.f * j23) * s3, bq = tr / (3.f * J);
             float Pm[3][3];   // a (F - bq cof F)
