@@ -416,6 +416,46 @@ int tsb_pcg_enable_psd(tsb_pcg_t s, const float *rest_xyz, const int32_t *tets, 
 int tsb_pcg_hvp_psd(tsb_pcg_t s, const float *x_dev, const float *v_dev, const tsb_terms_t *terms, float *hv_out_dev,
                     float *curv_out_dev, void *stream);
 
+/* ---- Assembled Hessian: the matrix a solver workspace multiplies by, as 3x3 block-CSR ------------------------------
+ * A Hessian workspace sits beside a solver workspace (which must outlive it) and follows its mode at creation:
+ *   exact:  H(x)  = c1 M + c2 sum_t K_t^T H_b,t K_t + c3 sum_t K_t^T H_a,t K_t
+ *   PSD:    H+(x) with every tet block replaced by the projection tsb_pcg_hvp_psd applies (tsb_pcg_enable_psd first)
+ * Layout: block rows over all n vertices, crow int32 [n + 1], col int32 [nnzb] (global vertex ids, ascending inside a
+ * row), values float32 [nnzb][3][3] row-major, both triangles stored: torch.sparse_bsr_tensor(crow, col, values) and
+ * scipy.sparse.bsr_matrix((values, col, crow)) take them as they are.  The pattern is M's off-diagonal pattern plus the
+ * diagonal: every vertex some tet references has its diagonal block, an orphan vertex's row is empty, no block couples
+ * two components.  Activity as in the PSD mode: barrier where det F < 0, AMIPS where det F > 0 and c3 != 0, det F in fp64
+ * from the fp32 positions (its sign can differ from the energy kernel's fp32 J only for |J| within rounding of 0).
+ *
+ * tsb_hessian_create: rest_xyz (host float32 [3n]) and tets (host int32 [4 nele]) must be the mesh the handle was created
+ * from (TSB_E_INVALID for another nele, TSB_E_MESH for a bad tet or other components).  Builds the block pattern on the
+ * host (a mesh with 2^31 or more blocks is TSB_E_INVALID: shard it) and allocates, reported by tsb_hessian_device_bytes:
+ *   8 (n + 1) + 8 nnzb + 493 nele   bytes (exact)          8 (n + 1) + 8 nnzb + 561 nele   bytes (PSD)
+ * (row offsets and incidence offsets 4 (n + 1) each; columns and M weights 4 each per block; per tet: the 16 corner-pair
+ * block indices 64, incidence entries 16, activity 1, the 10 weighted 3x3 blocks of its Hessian 360, and tet ids 16 plus
+ * Dm^-1 36 (exact) or a private projection operator 120 (PSD, tet ids and Dm^-1 are the solver workspace's)).  Creating
+ * one changes nothing about the handle or the solver workspace.  Synchronous, allocates: not during a stream capture
+ * (detected on the legacy default stream only, as for tsb_pcg_enable_psd).
+ *
+ * tsb_hessian_pattern: *nnzb (optional) and, when non-null, copies crow (device int32 [n + 1]) and col (device int32
+ * [nnzb]) on the stream.
+ *
+ * tsb_hessian_assemble: values_dev (device float32 [9 nnzb], fully overwritten) at x_dev (device float32 [3n]).  c1, c2,
+ * order, c3 from *terms with tsb_hvp_ex's rules; in PSD mode c1, c2, c3 >= 0.  Launches: (PSD) the projection, the
+ * per-tet block kernel, the row gather (c1 M_ij I plus the active tets' blocks of the row in incidence-list order).  No
+ * host read, no allocation, no floating-point atomics: capturable in a CUDA graph, bitwise repeatable, equal on default,
+ * deterministic and force_global handles of one mesh; blocks (i, j) and (j, i)^T are bitwise equal; a sphere's blocks do
+ * not depend on another sphere's x.  Like the solver workspace it serves one stream at a time.
+ * Argument errors (TSB_E_INVALID, nothing launched): a null workspace, x_dev, terms or values_dev, an order other than 2
+ * or 4, terms->c3 != 0 on a handle without enable_amips, a negative coefficient in PSD mode. */
+typedef struct tsb_hessian_s *tsb_hessian_t;
+int tsb_hessian_create(tsb_pcg_t s, const float *rest_xyz, const int32_t *tets, int32_t nele, tsb_hessian_t *out);
+void tsb_hessian_destroy(tsb_hessian_t hs);
+const char *tsb_hessian_last_error(tsb_hessian_t hs);   /* hs may be NULL: last tsb_hessian_create failure */
+int64_t tsb_hessian_device_bytes(tsb_hessian_t hs);
+int tsb_hessian_pattern(tsb_hessian_t hs, int64_t *nnzb, int32_t *crow_dev_out, int32_t *col_dev_out, void *stream);
+int tsb_hessian_assemble(tsb_hessian_t hs, const float *x_dev, const tsb_terms_t *terms, float *values_dev, void *stream);
+
 /* ---- Damped Newton step: one Levenberg-Marquardt iteration per sphere on the device (no counterpart in the reference)
  * A Newton workspace sits beside a solver workspace (which must outlive it; creating one changes nothing about the
  * handle or the solver workspace) and holds b, d and the two diagonal planes (12 floats per vertex), the per-sphere line

@@ -25,6 +25,8 @@ EXPORTED_SYMBOLS = (
     "tsb_line_search", "tsb_hess_diag", "tsb_pcg_create", "tsb_pcg_destroy", "tsb_pcg_last_error", "tsb_pcg_device_bytes",
     "tsb_pcg_set_blocks", "tsb_pcg_solve", "tsb_sphere_axpy", "tsb_pcg_set_blocks_ex", "tsb_pcg_solve_ex",
     "tsb_pcg_enable_psd", "tsb_pcg_hvp_psd", "tsb_pcg_solve_tr",
+    "tsb_hessian_create", "tsb_hessian_destroy", "tsb_hessian_last_error", "tsb_hessian_device_bytes", "tsb_hessian_pattern",
+    "tsb_hessian_assemble",
     "tsb_newton_create", "tsb_newton_destroy", "tsb_newton_last_error", "tsb_newton_device_bytes", "tsb_newton_reset",
     "tsb_newton_step", "tsb_newton_prox_step", "tsb_newton_tr_step", "tsb_newton_tr_step_ex", "tsb_energy_grad_host", "tsb_scale",
     "tsb_grad_limit", "tsb_adam_uniform_step",
@@ -155,6 +157,18 @@ def _load() -> C.CDLL:
     lib.tsb_pcg_solve_tr.restype = C.c_int
     lib.tsb_pcg_solve_tr.argtypes = [vp, vp, vp, C.POINTER(tsb_terms_t), C.POINTER(tsb_pcg_options_t), vp, vp, vp, vp,
                                      C.POINTER(C.c_int32), vp]
+    lib.tsb_hessian_create.restype = C.c_int
+    lib.tsb_hessian_create.argtypes = [vp, vp, vp, i32, C.POINTER(vp)]
+    lib.tsb_hessian_destroy.restype = None
+    lib.tsb_hessian_destroy.argtypes = [vp]
+    lib.tsb_hessian_last_error.restype = C.c_char_p
+    lib.tsb_hessian_last_error.argtypes = [vp]
+    lib.tsb_hessian_device_bytes.restype = i64
+    lib.tsb_hessian_device_bytes.argtypes = [vp]
+    lib.tsb_hessian_pattern.restype = C.c_int
+    lib.tsb_hessian_pattern.argtypes = [vp, C.POINTER(i64), vp, vp, vp]
+    lib.tsb_hessian_assemble.restype = C.c_int
+    lib.tsb_hessian_assemble.argtypes = [vp, vp, C.POINTER(tsb_terms_t), vp, vp]
     lib.tsb_newton_create.restype = C.c_int
     lib.tsb_newton_create.argtypes = [vp, C.POINTER(vp)]
     lib.tsb_newton_destroy.restype = None

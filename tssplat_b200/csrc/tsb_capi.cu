@@ -8,6 +8,7 @@
 #include <vector>
 
 #include "../../include/tssplat_b200.h"
+#include "tsb_hessian.cuh"
 #include "tsb_kernels.cuh"
 #include "tsb_plan.h"
 #include "tsb_psd.cuh"
@@ -35,6 +36,7 @@ struct tsb_handle_s {
   unsigned host_calls = 0;
   bool amips = false;
   bool det = false;             // deterministic gradient: DET energy kernel + det_gather_kernel
+  int32_t lap_scale = 0;        // tsb_options_t.laplacian_scale (tsb_hessian_create rebuilds the operator rows)
   tsb::DetParams dp{};
   tsb::SphParams sp{};          // per-sphere statistics: the fold's tables (records: kp.sph_rec)
   tsb_info_t info{};
@@ -67,6 +69,18 @@ struct tsb_newton_s {
   double *prox_part = nullptr;       // [chunks] d.(x - y) partials of tsb_newton_prox_step (allocated by its first call)
   tsb::TrState *tr_state = nullptr;  // [n_components] trust-region radius state (allocated by the first tsb_newton_tr_step)
   float *tr_radius = nullptr;        // [n_components] its fp32 radius, handed to tsb_pcg_solve_tr
+  int64_t device_bytes = 0;
+  std::vector<void *> allocs;
+  std::string err;
+};
+
+struct tsb_hessian_s {
+  tsb_pcg_t s = nullptr;
+  int device = 0;                    // the handle's device, kept so that destroying never reads the solver workspace
+  bool psd = false;                  // the solver workspace's mode at creation
+  tsb::HessParams P{};
+  int32_t *crow = nullptr, *col = nullptr;
+  int64_t nnzb = 0;
   int64_t device_bytes = 0;
   std::vector<void *> allocs;
   std::string err;
@@ -150,7 +164,15 @@ int newton_fail(tsb_newton_t nw, int code, const std::string &msg) {
   return code;
 }
 
-// Device array of a workspace (tsb_pcg_t or tsb_newton_t): copied from src, or zeroed
+// ... and a Hessian workspace (tsb_hessian_t)
+thread_local std::string g_hessian_create_err;
+
+int hessian_fail(tsb_hessian_t hs, int code, const std::string &msg) {
+  if (hs) hs->err = msg; else g_hessian_create_err = msg;
+  return code;
+}
+
+// Device array of a workspace (tsb_pcg_t, tsb_newton_t or tsb_hessian_t): copied from src, or zeroed
 template <class T, class W>
 int ws_alloc(W *s, size_t elems, const T *src, T **out) {
   const size_t bytes = elems * sizeof(T);
@@ -305,6 +327,7 @@ int tsb_create(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t ne
   h->lc = tsb::LaunchConfig{nw, plan.grid, smem, plan.mode_global, 0, 0, 0};
   h->amips = pc.enable_amips != 0;
   h->det = pc.deterministic != 0;
+  h->lap_scale = pc.laplacian_scale;
   h->comp_label = std::move(plan.comp_label);
 
   tsb_info_t &I = h->info;
@@ -1127,6 +1150,119 @@ int tsb_newton_tr_step_ex(tsb_newton_t nw, float *x_dev, const float *anchor_dev
   e = tsb::launch_newton_tr_decide(s->P, W, T, R, p, records_out_dev, st, bt ? &B : nullptr);
   if (e == cudaSuccess) e = tsb::launch_sphere_axpy(s->P, x_dev, W.alpha_sphere, W.d, x_dev, st);
   if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
+  return TSB_OK;
+}
+
+/* ---- Assembled Hessian (tsb_hessian.cu) ---- */
+
+int tsb_hessian_create(tsb_pcg_t s, const float *rest_xyz, const int32_t *tets, int32_t nele, tsb_hessian_t *out) {
+  if (!out) return hessian_fail(nullptr, TSB_E_INVALID, "out is null");
+  *out = nullptr;
+  if (!s) return hessian_fail(nullptr, TSB_E_INVALID, "solver workspace is null");
+  if (!rest_xyz || !tets) return hessian_fail(nullptr, TSB_E_INVALID, "rest_xyz and tets must be non-null");
+  const tsb_handle_t h = s->h;
+  if (nele != h->info.nele)
+    return hessian_fail(nullptr, TSB_E_INVALID, "nele = " + std::to_string(nele) + " but the handle has " + std::to_string(h->info.nele) + " tets");
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return hessian_fail(nullptr, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(cudaStreamLegacy, &cap) != cudaSuccess || cap != cudaStreamCaptureStatusNone) {
+    cudaGetLastError();
+    return hessian_fail(nullptr, TSB_E_INVALID, "tsb_hessian_create allocates device memory and cannot run while a stream is being captured");
+  }
+  tsb::HessPattern H;
+  std::string err;
+  int rc = tsb::build_hessian_pattern(rest_xyz, tets, h->info.n, nele, h->lap_scale, H, err);
+  if (rc != TSB_OK) return hessian_fail(nullptr, rc, err);
+  if (H.comp_label != h->comp_label || H.nnz != h->info.nnz)
+    return hessian_fail(nullptr, TSB_E_MESH, "the mesh's components or operator differ from the handle's: not the mesh it was created from");
+  tsb_hessian_t hs = new tsb_hessian_s();
+  hs->s = s;
+  hs->device = h->device;
+  hs->psd = s->psd;
+  hs->nnzb = H.nnzb;
+  tsb::HessParams &P = hs->P;
+  const size_t ne = size_t(nele);
+  int32_t *crow = nullptr, *tblk = nullptr, *inc_ptr = nullptr, *inc = nullptr;
+  float *w = nullptr;
+#define TSB_TRY(expr) do { rc = (expr); if (rc != TSB_OK) { g_hessian_create_err = hs->err; tsb_hessian_destroy(hs); return rc; } } while (0)
+  TSB_TRY(ws_alloc(hs, H.crow.size(), H.crow.data(), &crow));
+  TSB_TRY(ws_alloc(hs, H.col.size(), H.col.data(), &hs->col));
+  TSB_TRY(ws_alloc(hs, H.w.size(), H.w.data(), &w));
+  TSB_TRY(ws_alloc(hs, H.tblk.size(), H.tblk.data(), &tblk));
+  TSB_TRY(ws_alloc(hs, H.inc_ptr.size(), H.inc_ptr.data(), &inc_ptr));
+  TSB_TRY(ws_alloc(hs, H.inc.size(), H.inc.data(), &inc));
+  TSB_TRY(ws_alloc<uint8_t>(hs, ne, nullptr, &P.kind));
+  TSB_TRY(ws_alloc<float>(hs, ne * tsb::kHessTetFloats, nullptr, &P.blk));
+  if (hs->psd) {                     // the projection's tets and rest inverses, a private operator
+    float *op = nullptr;
+    TSB_TRY(ws_alloc<float>(hs, ne * tsb::kPsdOpFloats, nullptr, &op));
+    P.op = op;
+    P.tets = s->Q.tets;
+    P.B = s->Q.B;
+  } else {
+    int32_t *tets_dev = nullptr;
+    float *B = nullptr;
+    TSB_TRY(ws_alloc(hs, 4 * ne, tets, &tets_dev));
+    TSB_TRY(ws_alloc(hs, H.B.size(), H.B.data(), &B));
+    P.tets = reinterpret_cast<const int4 *>(tets_dev);
+    P.B = B;
+  }
+#undef TSB_TRY
+  hs->crow = crow;
+  P.crow = crow; P.w = w; P.tblk = tblk; P.inc_ptr = inc_ptr; P.inc = inc;
+  P.n = h->info.n; P.nele = nele;
+  *out = hs;
+  return TSB_OK;
+}
+
+void tsb_hessian_destroy(tsb_hessian_t hs) {
+  if (!hs) return;
+  DeviceGuard guard(hs->device);
+  for (void *p : hs->allocs) cudaFree(p);
+  delete hs;
+}
+
+const char *tsb_hessian_last_error(tsb_hessian_t hs) { return hs ? hs->err.c_str() : g_hessian_create_err.c_str(); }
+
+int64_t tsb_hessian_device_bytes(tsb_hessian_t hs) { return hs ? hs->device_bytes : 0; }
+
+int tsb_hessian_pattern(tsb_hessian_t hs, int64_t *nnzb, int32_t *crow_dev_out, int32_t *col_dev_out, void *stream) {
+  if (!hs) return TSB_E_INVALID;
+  if (nnzb) *nnzb = hs->nnzb;
+  DeviceGuard guard(hs->device);
+  if (!guard.ok) return hessian_fail(hs, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaError_t e = cudaSuccess;
+  if (crow_dev_out) e = cudaMemcpyAsync(crow_dev_out, hs->crow, (size_t(hs->P.n) + 1) * sizeof(int32_t), cudaMemcpyDeviceToDevice, st);
+  if (e == cudaSuccess && col_dev_out)
+    e = cudaMemcpyAsync(col_dev_out, hs->col, size_t(hs->nnzb) * sizeof(int32_t), cudaMemcpyDeviceToDevice, st);
+  if (e != cudaSuccess) return hessian_fail(hs, TSB_E_CUDA, std::string("pattern copy: ") + cudaGetErrorString(e));
+  return TSB_OK;
+}
+
+int tsb_hessian_assemble(tsb_hessian_t hs, const float *x_dev, const tsb_terms_t *terms, float *values_dev, void *stream) {
+  if (!hs) return TSB_E_INVALID;
+  if (!x_dev || !terms || !values_dev) return hessian_fail(hs, TSB_E_INVALID, "x_dev, terms and values_dev must be non-null");
+  if (terms->order != 2 && terms->order != 4) return hessian_fail(hs, TSB_E_INVALID, "order must be 2 or 4");
+  const tsb_handle_t h = hs->s->h;
+  if (terms->c3 != 0.f && !h->amips)
+    return hessian_fail(hs, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
+  if (hs->psd && !(terms->c1 >= 0.f && terms->c2 >= 0.f && terms->c3 >= 0.f))
+    return hessian_fail(hs, TSB_E_INVALID, "the projected Hessian needs c1, c2 and c3 >= 0 (projection does not commute with a negative weight)");
+  DeviceGuard guard(hs->device);
+  if (!guard.ok) return hessian_fail(hs, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaError_t e = cudaSuccess;
+  if (hs->psd) {                     // the workspace's projection kernel, into this workspace's operator and activity
+    tsb::PsdParams Q = hs->s->Q;
+    Q.op = const_cast<float *>(hs->P.op);
+    Q.kind = hs->P.kind;
+    e = tsb::launch_psd_project(Q, x_dev, terms->order, terms->c3 != 0.f ? 1 : 0, st);
+  }
+  if (e == cudaSuccess) e = tsb::launch_hessian_blocks(hs->P, x_dev, terms->order, terms->c2, terms->c3, hs->psd, st);
+  if (e == cudaSuccess) e = tsb::launch_hessian_gather(hs->P, terms->c1, values_dev, st);
+  if (e != cudaSuccess) return hessian_fail(hs, TSB_E_CUDA, std::string("hessian launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 

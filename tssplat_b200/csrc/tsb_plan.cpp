@@ -1128,6 +1128,98 @@ void build_pcg_lists(const std::vector<int32_t> &comp_label, int32_t n_component
   }
 }
 
+int build_hessian_pattern(const float *rest, const int32_t *tets, int32_t n, int32_t nele, int32_t laplacian_scale,
+                          HessPattern &H, std::string &err) {
+  if (!rest || !tets || n <= 0 || nele <= 0) { err = "null input or non-positive size"; return TSB_E_INVALID; }
+  H = HessPattern();
+  const int nth = std::clamp(int(std::thread::hardware_concurrency()), 1, kMaxHostThreads);
+  int rc = validate(rest, tets, n, nele, nth, err);
+  if (rc != TSB_OK) return rc;
+  HostPlan P;          // find_components fills its orphans and component labels
+  Mesh M{rest, tets, n, nele, std::vector<int32_t>(size_t(nele) * 4, -1), std::vector<int32_t>(size_t(n), -1), laplacian_scale ? 1 : 0};
+  std::vector<Comp> comps = find_components(M, P);
+  std::atomic<bool> bad{false};
+  parallel_for(comps.size(), 1, nth, [&](size_t c0, size_t c1) {
+    for (size_t c = c0; c < c1; ++c) {
+      if (build_adjacency(M, comps[c]) < 0) { bad = true; continue; }
+      build_rows(M, comps[c]);
+    }
+  });
+  if (bad) { err = "non-manifold mesh: a face is shared by more than two tets"; return TSB_E_MESH; }
+  // rows in vertex order: the component's off-diagonal entries plus the diagonal; orphans empty
+  H.crow.assign(size_t(n) + 1, 0);
+  for (const Comp &C : comps) {
+    H.nnz += int64_t(C.col.size());
+    for (size_t l = 0; l < C.verts.size(); ++l) H.crow[size_t(C.verts[l]) + 1] = C.rptr[l + 1] - C.rptr[l] + 1;
+  }
+  int64_t total = 0;
+  for (int32_t v = 0; v < n; ++v) {
+    total += H.crow[size_t(v) + 1];
+    if (total >= (int64_t(1) << 31)) { err = "the assembled Hessian has 2^31 or more 3x3 blocks (int32 block offsets): shard the mesh"; return TSB_E_INVALID; }
+    H.crow[size_t(v) + 1] = int32_t(total);
+  }
+  H.nnzb = total;
+  H.col.resize(size_t(total));
+  H.w.resize(size_t(total));
+  H.tblk.resize(size_t(nele) * 16);
+  std::atomic<int> missing{nele};
+  parallel_for(comps.size(), 1, nth, [&](size_t c0, size_t c1) {
+    for (size_t c = c0; c < c1; ++c) {
+      const Comp &C = comps[c];
+      for (size_t l = 0; l < C.verts.size(); ++l) {
+        int32_t o = H.crow[size_t(C.verts[l])];
+        double diag = 0.0;
+        for (int32_t p = C.rptr[l]; p < C.rptr[l + 1]; ++p) diag += double(C.val[size_t(p)]);
+        bool placed = false;
+        for (int32_t p = C.rptr[l]; p <= C.rptr[l + 1]; ++p) {
+          if (!placed && (p == C.rptr[l + 1] || C.col[size_t(p)] > int32_t(l))) {
+            H.col[size_t(o)] = C.verts[l];
+            H.w[size_t(o++)] = float(-diag);
+            placed = true;
+          }
+          if (p == C.rptr[l + 1]) break;
+          H.col[size_t(o)] = C.verts[size_t(C.col[size_t(p)])];
+          H.w[size_t(o++)] = C.val[size_t(p)];
+        }
+      }
+      for (const int32_t t : C.tets)
+        for (int k = 0; k < 4; ++k) {
+          const int32_t i = tets[4 * size_t(t) + k];
+          const int32_t *r0 = H.col.data() + H.crow[size_t(i)], *r1 = H.col.data() + H.crow[size_t(i) + 1];
+          for (int l = 0; l < 4; ++l) {
+            const int32_t *q = std::lower_bound(r0, r1, tets[4 * size_t(t) + l]);
+            if (q == r1 || *q != tets[4 * size_t(t) + l]) {
+              int cur = missing.load();
+              while (t < cur && !missing.compare_exchange_weak(cur, t)) {}
+            }
+            H.tblk[16 * size_t(t) + 4 * k + l] = int32_t(q - H.col.data());
+          }
+        }
+    }
+  });
+  if (missing.load() != nele) {
+    err = "internal: tet " + std::to_string(missing.load()) + " has a corner pair that is not an entry of the operator";
+    return TSB_E_MESH;
+  }
+  // incidence lists (a counting sort over ascending entries keeps them ascending) and the rest inverses
+  H.inc_ptr.assign(size_t(n) + 1, 0);
+  for (size_t e = 0; e < 4 * size_t(nele); ++e) ++H.inc_ptr[size_t(tets[e]) + 1];
+  for (int32_t v = 0; v < n; ++v) H.inc_ptr[size_t(v) + 1] += H.inc_ptr[size_t(v)];
+  H.inc.resize(4 * size_t(nele));
+  std::vector<int32_t> fill(H.inc_ptr.begin(), H.inc_ptr.end() - 1);
+  for (size_t e = 0; e < 4 * size_t(nele); ++e) H.inc[size_t(fill[size_t(tets[e])]++)] = int32_t(e);
+  H.B.resize(9 * size_t(nele));
+  parallel_for(size_t(nele), 8192, nth, [&](size_t b, size_t e) {
+    for (size_t t = b; t < e; ++t) {
+      double Bi[9], det;
+      rest_inverse(rest, tets + 4 * t, Bi, &det);     // validated above
+      for (int k = 0; k < 9; ++k) H.B[size_t(k) * size_t(nele) + t] = float(Bi[k]);
+    }
+  });
+  H.comp_label = std::move(P.comp_label);
+  return TSB_OK;
+}
+
 int build_plan(const float *rest, const int32_t *tets, int32_t n, int32_t nele, const PlanConfig &cfg,
                HostPlan &P, std::string &err) {
   if (!rest || !tets || n <= 0 || nele <= 0) { err = "null input or non-positive size"; return TSB_E_INVALID; }

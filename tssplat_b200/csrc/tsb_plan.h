@@ -162,6 +162,27 @@ struct PcgLists {
 };
 void build_pcg_lists(const std::vector<int32_t> &comp_label, int32_t n_components, PcgLists &out);
 
+// Block pattern of the assembled Hessian (tsb_hessian_create): 3 x 3 block-CSR over all n vertex rows, the off-diagonal
+// pattern of M plus the diagonal, columns ascending, no block between two components, orphan rows empty.  Every pair of
+// vertices sharing a tet is a structural entry of M (build_rows keeps every column a tet stencil touches), which the
+// builder checks while it fills tblk.
+struct HessPattern {
+  int64_t nnzb = 0;
+  int64_t nnz = 0;                  // off-diagonal operator entries (= HostPlan::nnz of the same mesh)
+  std::vector<int32_t> crow;        // [n + 1]
+  std::vector<int32_t> col;         // [nnzb] global vertex ids
+  std::vector<float> w;             // [nnzb] fp32 M_ij as the plan streams it; diagonal -sum_j M_ij (fp64, column order)
+  std::vector<int32_t> tblk;        // [16 nele] block of corner pair (k, l) of tet t at 16 t + 4 k + l
+  std::vector<int32_t> inc_ptr;     // [n + 1]
+  std::vector<int32_t> inc;         // [4 nele] 4 tet + corner, ascending within a vertex row
+  std::vector<float> B;             // [9][nele] rest inverse Dm^-1 (fp64, rounded), row-major entries
+  std::vector<int32_t> comp_label;  // [n] component of every vertex, -1 = orphan
+};
+
+// Returns 0 on success, TSB_E_* otherwise (message in err).
+int build_hessian_pattern(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele, int32_t laplacian_scale,
+                          HessPattern &out, std::string &err);
+
 // Returns 0 on success, TSB_E_* otherwise (message in err).
 int build_plan(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele,
                const PlanConfig &cfg, HostPlan &plan, std::string &err);

@@ -210,6 +210,18 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         c1, c2 = self.coeff_scheduler(it)
         return self.tet_sp.hess_diag(x.detach(), c1, c2, self.order_at(it), c3=self.amips_coeff)
 
+    def hessian(self, x, it):
+        """Block values [nnzb, 3, 3] of the Hessian of ``c1 * smooth + c2 * barrier (+ amips_coeff * amips)`` at ``x``,
+        with the scheduler's coefficients and the barrier order at ``it``, in the model of ``device_pcg``
+        (``FLAGS.newton_hessian``: exact or projected); the pattern is ``self.device_hessian``'s ``crow`` and ``col``
+        (``tssplat_b200.hessian.DeviceHessian``, created on first use).  Outside autograd, no host sync."""
+        from .hessian import DeviceHessian
+        hs = getattr(self, "device_hessian", None)
+        if hs is None:
+            hs = self.device_hessian = DeviceHessian(self._device_pcg())
+        c1, c2 = self.coeff_scheduler(it)
+        return hs.assemble(x.detach(), c1, c2, self.order_at(it), c3=self.amips_coeff)
+
     def _device_pcg(self):
         from .newton import DevicePCG
         pcg = getattr(self, "device_pcg", None)
