@@ -49,7 +49,7 @@ def init_mu_prox(st, maxD, w, o):
 
 
 def decide_prox(s, g, bd, dHd, mu_f, dd, dE, ahat, o, w, dx, alphas=ALPHAS):
-    """decide of test_newton_lm with the proximal terms (newton_decide_prox_kernel in fp64): dPhi_k = dE_k + w (a_k dx +
+    """decide of test_newton_lm with the proximal terms (newton_decide_kernel<true> in fp64): dPhi_k = dE_k + w (a_k dx +
     a_k^2 dd / 2) in place of dE_k, pred with mu' = mu_f - w; an unusable w freezes the sphere as STALLED.  dx = d.(x - y).
     Returns (alpha, k, dPhi of the step, rho)."""
     if s["status"] != ACTIVE:

@@ -98,6 +98,21 @@ class tsb_info_t(C.Structure):
     ]
 
 
+_RECORD_DTYPES = {C.c_float: "float32", C.c_double: "float64", C.c_int32: "int32"}
+
+
+def record_fields(raw, struct) -> dict:
+    """Views of the scalar fields of ``struct`` (a ctypes Structure above) in ``raw``, a [S, sizeof(struct)] uint8 tensor
+    of S such records: field name -> [S] tensor of the field's type (array fields such as ``reserved`` are left out)."""
+    import torch
+    out = {}
+    for name, ctype in struct._fields_:
+        if ctype in _RECORD_DTYPES:
+            off = getattr(struct, name).offset
+            out[name] = raw[:, off:off + C.sizeof(ctype)].view(getattr(torch, _RECORD_DTYPES[ctype]))[:, 0]
+    return out
+
+
 def _load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise ImportError(

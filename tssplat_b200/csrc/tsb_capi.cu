@@ -187,12 +187,37 @@ int ws_alloc(W *s, size_t elems, const T *src, T **out) {
   return TSB_OK;
 }
 
-// For the calls whose first use allocates: TSB_OK when st is not being captured, TSB_E_INVALID when it is, TSB_E_CUDA when
-// the query fails.
-int not_capturing(cudaStream_t st) {
+// Device array of a workspace that a call allocates on its first use, of max(elems, 1) elements (zero: cleared on st).
+// Nothing happens once *out is set; on a stream being captured nothing is allocated and the call is refused with `refusal`.
+template <class T, class W>
+int alloc_once(W *s, size_t elems, T **out, cudaStream_t st, const char *refusal, bool zero = false) {
+  if (*out) return TSB_OK;
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  if (cudaStreamIsCapturing(st, &cap) != cudaSuccess) { cudaGetLastError(); return TSB_E_CUDA; }
-  return cap == cudaStreamCaptureStatusNone ? TSB_OK : TSB_E_INVALID;
+  if (cudaStreamIsCapturing(st, &cap) != cudaSuccess) { cudaGetLastError(); s->err = "cannot query the stream"; return TSB_E_CUDA; }
+  if (cap != cudaStreamCaptureStatusNone) { s->err = refusal; return TSB_E_INVALID; }
+  const size_t bytes = std::max<size_t>(elems, 1) * sizeof(T);
+  void *d = nullptr;
+  cudaError_t e = cudaMalloc(&d, bytes);
+  if (e != cudaSuccess) { s->err = std::string("cudaMalloc: ") + cudaGetErrorString(e); return TSB_E_NOMEM; }
+  s->allocs.push_back(d);
+  s->device_bytes += int64_t(bytes);
+  if (zero && (e = cudaMemsetAsync(d, 0, bytes, st)) != cudaSuccess) {
+    s->err = std::string("cudaMemsetAsync: ") + cudaGetErrorString(e);
+    return TSB_E_CUDA;
+  }
+  *out = static_cast<T *>(d);
+  return TSB_OK;
+}
+
+// The rules of a tsb_terms_t: the barrier order, AMIPS only on a handle created with it, and for the projected Hessian
+// (psd) weights >= 0 (the projection multiplies by c2 and c3, so it is only the projection of the weighted sum for
+// weights >= 0).  Returns the message of the first rule broken, or null.
+const char *check_terms(tsb_handle_t h, bool psd, const tsb_terms_t &t) {
+  if (t.order != 2 && t.order != 4) return "order must be 2 or 4";
+  if (t.c3 != 0.f && !h->amips) return "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1";
+  if (psd && !(t.c1 >= 0.f && t.c2 >= 0.f && t.c3 >= 0.f))
+    return "the projected Hessian needs c1, c2 and c3 >= 0 (projection does not commute with a negative weight)";
+  return nullptr;
 }
 
 }  // namespace
@@ -463,9 +488,7 @@ int tsb_line_search(tsb_handle_t h, const float *x_dev, const float *d_dev, cons
   if (!terms) return fail(h, TSB_E_INVALID, "terms is null");
   if (!x_dev || !d_dev || !alpha_dev || !delta_out_dev)
     return fail(h, TSB_E_INVALID, "x_dev, d_dev, alpha_dev and delta_out_dev must be non-null");
-  if (terms->order != 2 && terms->order != 4) return fail(h, TSB_E_INVALID, "order must be 2 or 4");
-  if (terms->c3 != 0.f && !h->amips)
-    return fail(h, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
+  if (const char *m = check_terms(h, false, *terms)) return fail(h, TSB_E_INVALID, m);
   DeviceGuard guard(h->device);
   if (!guard.ok) return fail(h, TSB_E_CUDA, "cannot select the handle's CUDA device");
   tsb::KParams kp = h->kp;
@@ -492,9 +515,7 @@ int tsb_hess_diag(tsb_handle_t h, const float *x_dev, const tsb_terms_t *terms, 
   if (!h) return TSB_E_INVALID;
   if (!terms) return fail(h, TSB_E_INVALID, "terms is null");
   if (!x_dev || !diag_out_dev) return fail(h, TSB_E_INVALID, "x_dev and diag_out_dev must be non-null");
-  if (terms->order != 2 && terms->order != 4) return fail(h, TSB_E_INVALID, "order must be 2 or 4");
-  if (terms->c3 != 0.f && !h->amips)
-    return fail(h, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
+  if (const char *m = check_terms(h, false, *terms)) return fail(h, TSB_E_INVALID, m);
   DeviceGuard guard(h->device);
   if (!guard.ok) return fail(h, TSB_E_CUDA, "cannot select the handle's CUDA device");
   tsb::KParams kp = h->kp;
@@ -604,13 +625,6 @@ int tsb_pcg_set_blocks_ex(tsb_pcg_t s, const float *diag_dev, float rel_floor, c
 
 namespace {
 
-// The projection multiplies by c2 and c3, so it is only the projection of the weighted sum for weights >= 0
-int psd_check_terms(tsb_pcg_t s, const tsb_terms_t &t) {
-  if (!(t.c1 >= 0.f && t.c2 >= 0.f && t.c3 >= 0.f))
-    return pcg_fail(s, TSB_E_INVALID, "the projected Hessian needs c1, c2 and c3 >= 0 (projection does not commute with a negative weight)");
-  return TSB_OK;
-}
-
 // hv = c1 M v (the exact product with c2 = c3 = 0: its tet pass adds exact zeros) + c2 P(H_b) v + c3 P(H_a) v at the
 // workspace's last projection; curv (optional, device float[4]) as tsb_pcg_hvp_psd reports it
 int psd_product(tsb_pcg_t s, const float *x_dev, const float *v_dev, const tsb_terms_t &t, float *hv, float *curv,
@@ -716,15 +730,11 @@ int tsb_pcg_hvp_psd(tsb_pcg_t s, const float *x_dev, const float *v_dev, const t
   if (!x_dev || !v_dev || !terms || !hv_out_dev) return pcg_fail(s, TSB_E_INVALID, "x_dev, v_dev, terms and hv_out_dev must be non-null");
   if (hv_out_dev == v_dev || hv_out_dev == x_dev)
     return pcg_fail(s, TSB_E_INVALID, "hv_out_dev must not be x_dev or v_dev: hv is written before v and x are read for the last time");
-  if (terms->order != 2 && terms->order != 4) return pcg_fail(s, TSB_E_INVALID, "order must be 2 or 4");
-  if (terms->c3 != 0.f && !s->h->amips)
-    return pcg_fail(s, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
-  int rc = psd_check_terms(s, *terms);
-  if (rc != TSB_OK) return rc;
+  if (const char *m = check_terms(s->h, true, *terms)) return pcg_fail(s, TSB_E_INVALID, m);
   DeviceGuard guard(s->h->device);
   if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  rc = psd_project(s, x_dev, *terms, st);
+  int rc = psd_project(s, x_dev, *terms, st);
   if (rc == TSB_OK) rc = psd_product(s, x_dev, v_dev, *terms, hv_out_dev, curv_out_dev, st);
   return rc;
 }
@@ -738,25 +748,6 @@ int tsb_pcg_solve(tsb_pcg_t s, const float *x_dev, const float *b_dev, const tsb
 
 namespace {
 
-// The trust-region recurrence state of a workspace: allocated once, outside any stream capture (the dir kernel of iteration
-// 0 writes it before any kernel reads it).
-int pcg_tr_alloc(tsb_pcg_t s, cudaStream_t st) {
-  if (s->tr) return TSB_OK;
-  const int rc = not_capturing(st);
-  if (rc == TSB_E_CUDA) return pcg_fail(s, rc, "cannot query the stream");
-  if (rc != TSB_OK)
-    return pcg_fail(s, rc, "the first tsb_pcg_solve_tr of a workspace allocates device memory and cannot be captured in a "
-                           "CUDA graph: make one call outside any capture first");
-  void *d = nullptr;
-  const size_t bytes = std::max<size_t>(size_t(s->P.n_components), 1) * sizeof(tsb::TrComp);
-  const cudaError_t e = cudaMalloc(&d, bytes);
-  if (e != cudaSuccess) return pcg_fail(s, TSB_E_NOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e));
-  s->allocs.push_back(d);
-  s->device_bytes += int64_t(bytes);
-  s->tr = static_cast<tsb::TrComp *>(d);
-  return TSB_OK;
-}
-
 // tsb_pcg_solve_ex, and tsb_pcg_solve_tr when radius_dev != nullptr
 int pcg_solve_impl(tsb_pcg_t s, const float *x_dev, const float *b_dev, const tsb_terms_t *terms, const tsb_pcg_options_t *opt,
                    const float *shift_dev, const float *radius_dev, float *d_out_dev, tsb_pcg_sphere_t *spheres_out_dev,
@@ -766,13 +757,7 @@ int pcg_solve_impl(tsb_pcg_t s, const float *x_dev, const float *b_dev, const ts
   if (opt->max_iter < 1) return pcg_fail(s, TSB_E_INVALID, "max_iter must be >= 1");
   if (!(opt->rtol >= 0.f)) return pcg_fail(s, TSB_E_INVALID, "rtol must be >= 0");
   if (opt->check_every < 0) return pcg_fail(s, TSB_E_INVALID, "check_every must be >= 0");
-  if (terms->order != 2 && terms->order != 4) return pcg_fail(s, TSB_E_INVALID, "order must be 2 or 4");
-  if (terms->c3 != 0.f && !s->h->amips)
-    return pcg_fail(s, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
-  if (s->psd) {
-    const int rc = psd_check_terms(s, *terms);
-    if (rc != TSB_OK) return rc;
-  }
+  if (const char *m = check_terms(s->h, s->psd, *terms)) return pcg_fail(s, TSB_E_INVALID, m);
   DeviceGuard guard(s->h->device);
   if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -782,8 +767,10 @@ int pcg_solve_impl(tsb_pcg_t s, const float *x_dev, const float *b_dev, const ts
     if (cap != cudaStreamCaptureStatusNone)
       return pcg_fail(s, TSB_E_INVALID, "check_every > 0 reads the host and cannot be captured in a CUDA graph: use check_every = 0");
   }
-  if (radius_dev) {
-    const int rc = pcg_tr_alloc(s, st);
+  if (radius_dev) {     // the recurrence state: the dir kernel of iteration 0 writes it before any kernel reads it
+    const int rc = alloc_once(s, size_t(s->P.n_components), &s->tr, st,
+                              "the first tsb_pcg_solve_tr of a workspace allocates device memory and cannot be captured in a "
+                              "CUDA graph: make one call outside any capture first");
     if (rc != TSB_OK) return rc;
   }
   const tsb::TrParams tp{radius_dev, s->tr};
@@ -793,7 +780,7 @@ int pcg_solve_impl(tsb_pcg_t s, const float *x_dev, const float *b_dev, const ts
     const int rc = psd_project(s, x_dev, *terms, st);
     if (rc != TSB_OK) return rc;
   }
-  cudaError_t e = tsb::launch_pcg_begin(P, b_dev, d_out_dev, st, tr);
+  cudaError_t e = tsb::launch_pcg_begin(P, b_dev, d_out_dev, tr, st);
   if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver launch: ") + cudaGetErrorString(e));
   int32_t it = 0;
   while (it < opt->max_iter) {
@@ -804,7 +791,7 @@ int pcg_solve_impl(tsb_pcg_t s, const float *x_dev, const float *b_dev, const ts
       const int rc = hvp_impl(s->h, x_dev, P.p, terms->c1, terms->c2, terms->c3, terms->order, 1.f, nullptr, P.Hp, nullptr, 1, st);
       if (rc != TSB_OK) return pcg_fail(s, rc, s->h->err);
     }
-    e = tsb::launch_pcg_step(P, d_out_dev, it, opt->rtol, shift_dev, st, tr);
+    e = tsb::launch_pcg_step(P, d_out_dev, it, opt->rtol, shift_dev, tr, st);
     if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver launch: ") + cudaGetErrorString(e));
     ++it;
     if (opt->check_every > 0 && it % opt->check_every == 0 && it < opt->max_iter) {
@@ -917,58 +904,131 @@ int tsb_newton_reset(tsb_newton_t nw, void *stream) {
 
 namespace {
 
-// tsb_newton_step's argument rules, shared by tsb_newton_prox_step
-int newton_check(tsb_newton_t nw, const float *x_dev, const tsb_terms_t *terms, const tsb_newton_options_t *opt) {
+// The options a kind of Newton step adds to those every step has: "" when they hold, or the message of the first broken
+std::string rule_error(const tsb_newton_options_t &o) {
+  if (!(o.tau > 0.f) || !std::isfinite(o.tau)) return "tau must be finite and > 0";
+  if (!(o.mu_min > 0.f) || !(o.mu_min <= o.mu_max) || !std::isfinite(o.mu_max))
+    return "mu_min and mu_max must satisfy 0 < mu_min <= mu_max < inf";
+  if (!(o.sigma > 0.f && o.sigma < 1.f)) return "sigma must be in (0, 1)";
+  if (o.n_alpha < 1 || o.n_alpha > TSB_LINE_MAX_ALPHA) return "n_alpha must be in [1, " + std::to_string(TSB_LINE_MAX_ALPHA) + "]";
+  return "";
+}
+
+std::string rule_error(const tsb_newton_tr_options_t &o) {
+  if (!(o.radius_init > 0.f) || !std::isfinite(o.radius_init)) return "radius_init must be finite and > 0";
+  if (!(o.radius_min > 0.f) || !(o.radius_min <= o.radius_max) || !std::isfinite(o.radius_max))
+    return "radius_min and radius_max must satisfy 0 < radius_min <= radius_max < inf";
+  if (!(o.accept >= 0.f && o.accept < 0.25f)) return "accept must be in [0, 1/4)";
+  return "";
+}
+
+// The argument rules of every Newton step: the pointers, the proximal pair (anchor_dev and weight_dev both null: objective
+// E, or both set, the anchor not x), the options all steps have, those of the step's kind (O), and the terms.
+template <class O>
+int newton_check(tsb_newton_t nw, const float *x_dev, const float *anchor_dev, const float *weight_dev, const tsb_terms_t *terms,
+                 const O *opt) {
   if (!x_dev || !terms || !opt) return newton_fail(nw, TSB_E_INVALID, "x_dev, terms and opt must be non-null");
-  const tsb_newton_options_t &o = *opt;
+  if (!anchor_dev != !weight_dev)
+    return newton_fail(nw, TSB_E_INVALID, "anchor_dev and weight_dev must be both null (objective E) or both set (proximal objective)");
+  if (anchor_dev && anchor_dev == x_dev)
+    return newton_fail(nw, TSB_E_INVALID, "anchor_dev must not be x_dev: x is updated in place while the anchor is read");
+  const O &o = *opt;
   if (o.max_iter < 1) return newton_fail(nw, TSB_E_INVALID, "max_iter must be >= 1");
   if (!(o.rtol >= 0.f)) return newton_fail(nw, TSB_E_INVALID, "rtol must be >= 0");
   if (!(o.rel_floor >= 0.f)) return newton_fail(nw, TSB_E_INVALID, "rel_floor must be >= 0");
-  if (!(o.tau > 0.f) || !std::isfinite(o.tau)) return newton_fail(nw, TSB_E_INVALID, "tau must be finite and > 0");
-  if (!(o.mu_min > 0.f) || !(o.mu_min <= o.mu_max) || !std::isfinite(o.mu_max))
-    return newton_fail(nw, TSB_E_INVALID, "mu_min and mu_max must satisfy 0 < mu_min <= mu_max < inf");
   if (!(o.gtol >= 0.f)) return newton_fail(nw, TSB_E_INVALID, "gtol must be >= 0");
-  if (!(o.sigma > 0.f && o.sigma < 1.f)) return newton_fail(nw, TSB_E_INVALID, "sigma must be in (0, 1)");
   if (!(o.eta > 0.f && o.eta <= 1.f)) return newton_fail(nw, TSB_E_INVALID, "eta must be in (0, 1]");
-  if (o.n_alpha < 1 || o.n_alpha > TSB_LINE_MAX_ALPHA)
-    return newton_fail(nw, TSB_E_INVALID, "n_alpha must be in [1, " + std::to_string(TSB_LINE_MAX_ALPHA) + "]");
   for (int32_t r : o.reserved)
     if (r != 0) return newton_fail(nw, TSB_E_INVALID, "reserved fields must be 0");
-  if (terms->order != 2 && terms->order != 4) return newton_fail(nw, TSB_E_INVALID, "order must be 2 or 4");
-  if (terms->c3 != 0.f && !nw->s->h->amips)
-    return newton_fail(nw, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
-  if (nw->s->psd && !(terms->c1 >= 0.f && terms->c2 >= 0.f && terms->c3 >= 0.f))
-    return newton_fail(nw, TSB_E_INVALID, "the projected Hessian needs c1, c2 and c3 >= 0 (projection does not commute with a negative weight)");
+  const std::string rule = rule_error(o);
+  if (!rule.empty()) return newton_fail(nw, TSB_E_INVALID, rule);
+  if (const char *m = check_terms(nw->s->h, nw->s->psd, *terms)) return newton_fail(nw, TSB_E_INVALID, m);
   return TSB_OK;
 }
 
-// The eight phases of tsb_newton_step; prox != nullptr: those of tsb_newton_prox_step (the PROX kernel variants).
-int newton_run(tsb_newton_t nw, float *x_dev, const tsb::ProxParams *prox, const tsb_terms_t *terms,
-               const tsb_newton_options_t &o, tsb_newton_sphere_t *records_out_dev, cudaStream_t st) {
+// What tells the Newton steps apart.  The damped step (tsb_newton_step, tsb_newton_prox_step) solves with the shift mu_c
+// (+ w_c) and no radius, line-searches n_alpha step sizes and decides by the damping rule; the trust-region step
+// (tsb_newton_tr_step, _ex) solves with the shift w_c of a proximal step (none otherwise) inside the radius, line-searches
+// alpha = 1 (with backtracking: bt.n_alpha step sizes) and decides by the trust-region rule.
+struct NewtonStep {
+  bool damped;
+  tsb::NewtonRule lm{};
+  tsb_newton_sphere_t *lm_out = nullptr;
+  tsb::NewtonTrRule tr{};
+  bool backtrack = false;
+  tsb::NewtonBacktrack bt{};
+  tsb_newton_tr_sphere_t *tr_out = nullptr;
+  tsb_pcg_options_t po;
+  float rel_floor;
+  int32_t n_alpha;
+
+  NewtonStep(const tsb_newton_options_t &o, tsb_newton_sphere_t *out)
+      : damped(true), lm{o.tau, o.mu_min, o.mu_max, o.gtol, o.sigma, o.eta, o.n_alpha}, lm_out(out),
+        po{o.max_iter, o.rtol, 0, {0, 0, 0, 0, 0}}, rel_floor(o.rel_floor), n_alpha(o.n_alpha) {}
+  NewtonStep(const tsb_newton_tr_options_t &o, const tsb_newton_backtrack_t *b, tsb_newton_tr_sphere_t *out)
+      : damped(false), tr{o.gtol, o.radius_init, o.radius_min, o.radius_max, o.accept, o.eta}, backtrack(b != nullptr),
+        bt{b ? b->sigma : 0.f, b ? b->n_alpha : 1}, tr_out(out), po{o.max_iter, o.rtol, 0, {0, 0, 0, 0, 0}},
+        rel_floor(o.rel_floor), n_alpha(b ? b->n_alpha : 1) {}
+};
+
+// One Newton step of every sphere after its arguments are checked: the first call's allocations, then gradient, diagonal
+// blocks, prep (damped: and the shift), preconditioner, (trust region: the radius), solve, dots, line search, decision and
+// the step itself.
+int newton_run(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const float *weight_dev, const tsb_terms_t *terms,
+               const NewtonStep &k, void *stream) {
   tsb_pcg_t s = nw->s;
   tsb_handle_t h = s->h;
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return newton_fail(nw, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const char *refusal = k.damped ? "the first tsb_newton_prox_step of a workspace allocates device memory and cannot be "
+                                   "captured in a CUDA graph: make one call outside any capture first"
+                                 : "the first tsb_newton_tr_step of a workspace (and the first proximal one) allocates device memory "
+                                   "and cannot be captured in a CUDA graph: make one call outside any capture first";
+  const size_t S = size_t(s->P.n_components);
+  int rc = TSB_OK;
+  if (!k.damped) {      // the radius state (every radius to be initialised) and its fp32 radius
+    rc = alloc_once(nw, S, &nw->tr_state, st, refusal, true);
+    if (rc == TSB_OK) rc = alloc_once(nw, S, &nw->tr_radius, st, refusal);
+  }
+  // the d.(x - y) partials, never read before written
+  if (rc == TSB_OK && anchor_dev) rc = alloc_once(nw, size_t(s->P.n_chunks), &nw->prox_part, st, refusal);
+  if (rc != TSB_OK) return rc;
+  if (!k.damped) {      // the solve's recurrence state, as a first tsb_pcg_solve_tr allocates it
+    rc = alloc_once(s, S, &s->tr, st, refusal);
+    if (rc != TSB_OK) return newton_fail(nw, rc, s->err);
+  }
   const tsb::NewtonParams &W = nw->W;
-  const tsb::NewtonRule R{o.tau, o.mu_min, o.mu_max, o.gtol, o.sigma, o.eta, o.n_alpha};
-  const tsb_pcg_options_t po{o.max_iter, o.rtol, 0, {0, 0, 0, 0, 0}};
-  // 1-2: b = -grad, the diagonal blocks
-  int rc = energy_grad_impl(h, x_dev, terms->c1, terms->c2, terms->c3, terms->order, -1.f, nullptr, nw->energy, 1, W.b, nullptr, st);
+  const tsb::ProxParams pp{x_dev, anchor_dev, weight_dev, nw->prox_part};
+  const tsb::ProxParams *prox = anchor_dev ? &pp : nullptr;
+  const tsb::NewtonTrParams T{nw->tr_state, nw->tr_radius, s->tr};
+  // the trust-region step's shift w_c: an unusable w_c only reaches a sphere whose b_c is 0
+  const float *shift = k.damped ? W.shift : weight_dev;
+  // b = -grad, the diagonal blocks; frozen spheres' b = 0 (prox: b -= w (x - y)); damped: mu on a first step
+  rc = energy_grad_impl(h, x_dev, terms->c1, terms->c2, terms->c3, terms->order, -1.f, nullptr, nw->energy, 1, W.b, nullptr, st);
   if (rc == TSB_OK) rc = tsb_hess_diag(h, x_dev, terms, 1.f, nullptr, W.diag, st);
   if (rc != TSB_OK) return newton_fail(nw, rc, h->err);
-  // 3: frozen spheres' b = 0 (prox: b -= w (x - y)), mu on a first step
-  cudaError_t e = tsb::launch_newton_prep(s->P, W, R, prox, st);
+  cudaError_t e = tsb::launch_newton_prep(s->P, W, prox, st);
+  if (e == cudaSuccess && k.damped) e = tsb::launch_newton_shift(s->P, W, k.lm, prox, st);
   if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
-  // 4: the damped solve
-  rc = tsb_pcg_set_blocks_ex(s, W.diag, o.rel_floor, W.shift, nullptr, st);
-  if (rc == TSB_OK) rc = tsb_pcg_solve_ex(s, x_dev, W.b, terms, &po, W.shift, W.d, nullptr, nullptr, st);
+  // the preconditioner; trust region: the radius on a first step
+  rc = tsb_pcg_set_blocks_ex(s, W.diag, k.rel_floor, shift, nullptr, st);
   if (rc != TSB_OK) return newton_fail(nw, rc, s->err);
-  // 5: b.d and |d|^2 (prox: and d.(x - y)) per chunk
+  if (!k.damped) {
+    e = tsb::launch_newton_tr_radius(s->P, W, T, k.tr, st);
+    if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
+  }
+  // the solve
+  rc = pcg_solve_impl(s, x_dev, W.b, terms, &k.po, shift, k.damped ? nullptr : nw->tr_radius, W.d, nullptr, nullptr, st);
+  if (rc != TSB_OK) return newton_fail(nw, rc, s->err);
+  // b.d and |d|^2 (prox: and d.(x - y)) per chunk; the line search at 2^-k, k < n_alpha, per sphere
   e = tsb::launch_newton_dots(s->P, W, prox, st);
   if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
-  // 6: line search at 2^-k, per sphere
-  rc = tsb_line_search(h, x_dev, W.d, terms, W.alphas, o.n_alpha, nw->delta, nullptr, W.sphere_delta, W.sphere_step, st);
+  rc = tsb_line_search(h, x_dev, W.d, terms, W.alphas, k.n_alpha, nw->delta, nullptr, W.sphere_delta, W.sphere_step, st);
   if (rc != TSB_OK) return newton_fail(nw, rc, h->err);
-  // 7-8: decision, step
-  e = tsb::launch_newton_decide(s->P, W, R, prox, records_out_dev, st);
+  // decision, step
+  e = k.damped ? tsb::launch_newton_decide(s->P, W, k.lm, prox, k.lm_out, st)
+               : tsb::launch_newton_tr_decide(s->P, W, T, k.tr, prox, k.backtrack ? &k.bt : nullptr, k.tr_out, st);
   if (e == cudaSuccess) e = tsb::launch_sphere_axpy(s->P, x_dev, W.alpha_sphere, W.d, x_dev, st);
   if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
   return TSB_OK;
@@ -981,116 +1041,20 @@ extern "C" {
 int tsb_newton_step(tsb_newton_t nw, float *x_dev, const tsb_terms_t *terms, const tsb_newton_options_t *opt,
                     tsb_newton_sphere_t *records_out_dev, void *stream) {
   if (!nw) return TSB_E_INVALID;
-  int rc = newton_check(nw, x_dev, terms, opt);
+  const int rc = newton_check(nw, x_dev, nullptr, nullptr, terms, opt);
   if (rc != TSB_OK) return rc;
-  DeviceGuard guard(nw->s->h->device);
-  if (!guard.ok) return newton_fail(nw, TSB_E_CUDA, "cannot select the handle's CUDA device");
-  return newton_run(nw, x_dev, nullptr, terms, *opt, records_out_dev, static_cast<cudaStream_t>(stream));
+  return newton_run(nw, x_dev, nullptr, nullptr, terms, NewtonStep(*opt, records_out_dev), stream);
 }
 
 int tsb_newton_prox_step(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const float *weight_dev,
                          const tsb_terms_t *terms, const tsb_newton_options_t *opt, tsb_newton_sphere_t *records_out_dev,
                          void *stream) {
   if (!nw) return TSB_E_INVALID;
-  int rc = newton_check(nw, x_dev, terms, opt);
-  if (rc != TSB_OK) return rc;
   if (!anchor_dev || !weight_dev) return newton_fail(nw, TSB_E_INVALID, "anchor_dev and weight_dev must be non-null");
-  if (anchor_dev == x_dev)
-    return newton_fail(nw, TSB_E_INVALID, "anchor_dev must not be x_dev: x is updated in place while the anchor is read");
-  DeviceGuard guard(nw->s->h->device);
-  if (!guard.ok) return newton_fail(nw, TSB_E_CUDA, "cannot select the handle's CUDA device");
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (!nw->prox_part) {        // the d.(x - y) partials: allocated by the first proximal step, never read before written
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    if (cudaStreamIsCapturing(st, &cap) != cudaSuccess) { cudaGetLastError(); return newton_fail(nw, TSB_E_CUDA, "cannot query the stream"); }
-    if (cap != cudaStreamCaptureStatusNone)
-      return newton_fail(nw, TSB_E_INVALID, "the first tsb_newton_prox_step of a workspace allocates device memory and cannot be "
-                                            "captured in a CUDA graph: make one call outside any capture first");
-    const size_t bytes = std::max<size_t>(size_t(nw->s->P.n_chunks), 1) * sizeof(double);
-    void *d = nullptr;
-    const cudaError_t e = cudaMalloc(&d, bytes);
-    if (e != cudaSuccess) return newton_fail(nw, TSB_E_NOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e));
-    nw->allocs.push_back(d);
-    nw->device_bytes += int64_t(bytes);
-    nw->prox_part = static_cast<double *>(d);
-  }
-  const tsb::ProxParams prox{x_dev, anchor_dev, weight_dev, nw->prox_part};
-  return newton_run(nw, x_dev, &prox, terms, *opt, records_out_dev, st);
+  const int rc = newton_check(nw, x_dev, anchor_dev, weight_dev, terms, opt);
+  if (rc != TSB_OK) return rc;
+  return newton_run(nw, x_dev, anchor_dev, weight_dev, terms, NewtonStep(*opt, records_out_dev), stream);
 }
-
-}  // extern "C"
-
-namespace {
-
-int newton_tr_check(tsb_newton_t nw, const float *x_dev, const float *anchor_dev, const float *weight_dev,
-                    const tsb_terms_t *terms, const tsb_newton_tr_options_t *opt) {
-  if (!x_dev || !terms || !opt) return newton_fail(nw, TSB_E_INVALID, "x_dev, terms and opt must be non-null");
-  if (!anchor_dev != !weight_dev)
-    return newton_fail(nw, TSB_E_INVALID, "anchor_dev and weight_dev must be both null (objective E) or both set (proximal objective)");
-  if (anchor_dev && anchor_dev == x_dev)
-    return newton_fail(nw, TSB_E_INVALID, "anchor_dev must not be x_dev: x is updated in place while the anchor is read");
-  const tsb_newton_tr_options_t &o = *opt;
-  if (o.max_iter < 1) return newton_fail(nw, TSB_E_INVALID, "max_iter must be >= 1");
-  if (!(o.rtol >= 0.f)) return newton_fail(nw, TSB_E_INVALID, "rtol must be >= 0");
-  if (!(o.rel_floor >= 0.f)) return newton_fail(nw, TSB_E_INVALID, "rel_floor must be >= 0");
-  if (!(o.gtol >= 0.f)) return newton_fail(nw, TSB_E_INVALID, "gtol must be >= 0");
-  if (!(o.radius_init > 0.f) || !std::isfinite(o.radius_init))
-    return newton_fail(nw, TSB_E_INVALID, "radius_init must be finite and > 0");
-  if (!(o.radius_min > 0.f) || !(o.radius_min <= o.radius_max) || !std::isfinite(o.radius_max))
-    return newton_fail(nw, TSB_E_INVALID, "radius_min and radius_max must satisfy 0 < radius_min <= radius_max < inf");
-  if (!(o.accept >= 0.f && o.accept < 0.25f)) return newton_fail(nw, TSB_E_INVALID, "accept must be in [0, 1/4)");
-  if (!(o.eta > 0.f && o.eta <= 1.f)) return newton_fail(nw, TSB_E_INVALID, "eta must be in (0, 1]");
-  for (int32_t r : o.reserved)
-    if (r != 0) return newton_fail(nw, TSB_E_INVALID, "reserved fields must be 0");
-  if (terms->order != 2 && terms->order != 4) return newton_fail(nw, TSB_E_INVALID, "order must be 2 or 4");
-  if (terms->c3 != 0.f && !nw->s->h->amips)
-    return newton_fail(nw, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
-  if (nw->s->psd && !(terms->c1 >= 0.f && terms->c2 >= 0.f && terms->c3 >= 0.f))
-    return newton_fail(nw, TSB_E_INVALID, "the projected Hessian needs c1, c2 and c3 >= 0 (projection does not commute with a negative weight)");
-  return TSB_OK;
-}
-
-// The first trust-region step's allocations: the radius state, the d.(x - y) partials of a proximal step, and (through a
-// first tsb_pcg_solve_tr) the solve's recurrence state.  Nothing is allocated on a stream being captured.
-int newton_tr_alloc(tsb_newton_t nw, bool prox, cudaStream_t st) {
-  const bool need = !nw->tr_state || !nw->s->tr || (prox && !nw->prox_part);
-  if (!need) return TSB_OK;
-  const int rc = not_capturing(st);
-  if (rc == TSB_E_CUDA) return newton_fail(nw, rc, "cannot query the stream");
-  if (rc != TSB_OK)
-    return newton_fail(nw, rc, "the first tsb_newton_tr_step of a workspace (and the first proximal one) allocates device memory "
-                               "and cannot be captured in a CUDA graph: make one call outside any capture first");
-  const size_t S = std::max<size_t>(size_t(nw->s->P.n_components), 1);
-  auto alloc = [&](size_t bytes, void **out) -> int {
-    const cudaError_t e = cudaMalloc(out, bytes);
-    if (e != cudaSuccess) return newton_fail(nw, TSB_E_NOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e));
-    nw->allocs.push_back(*out);
-    nw->device_bytes += int64_t(bytes);
-    return TSB_OK;
-  };
-  if (!nw->tr_state) {
-    void *a = nullptr, *b = nullptr;
-    int r = alloc(S * sizeof(tsb::TrState), &a);
-    if (r == TSB_OK) r = alloc(S * sizeof(float), &b);
-    if (r != TSB_OK) return r;
-    const cudaError_t e = cudaMemsetAsync(a, 0, S * sizeof(tsb::TrState), st);    // every radius to be initialised
-    if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("cudaMemsetAsync: ") + cudaGetErrorString(e));
-    nw->tr_state = static_cast<tsb::TrState *>(a);
-    nw->tr_radius = static_cast<float *>(b);
-  }
-  if (prox && !nw->prox_part) {
-    void *a = nullptr;
-    const int r = alloc(std::max<size_t>(size_t(nw->s->P.n_chunks), 1) * sizeof(double), &a);
-    if (r != TSB_OK) return r;
-    nw->prox_part = static_cast<double *>(a);
-  }
-  const int r = pcg_tr_alloc(nw->s, st);
-  return r == TSB_OK ? TSB_OK : newton_fail(nw, r, nw->s->err);
-}
-
-}  // namespace
-
-extern "C" {
 
 int tsb_newton_tr_step(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const float *weight_dev, const tsb_terms_t *terms,
                        const tsb_newton_tr_options_t *opt, tsb_newton_tr_sphere_t *records_out_dev, void *stream) {
@@ -1101,7 +1065,7 @@ int tsb_newton_tr_step_ex(tsb_newton_t nw, float *x_dev, const float *anchor_dev
                           const tsb_newton_tr_options_t *opt, const tsb_newton_backtrack_t *bt,
                           tsb_newton_tr_sphere_t *records_out_dev, void *stream) {
   if (!nw) return TSB_E_INVALID;
-  int rc = newton_tr_check(nw, x_dev, anchor_dev, weight_dev, terms, opt);
+  const int rc = newton_check(nw, x_dev, anchor_dev, weight_dev, terms, opt);
   if (rc != TSB_OK) return rc;
   if (bt) {
     if (bt->n_alpha < 2 || bt->n_alpha > TSB_LINE_MAX_ALPHA)
@@ -1110,47 +1074,7 @@ int tsb_newton_tr_step_ex(tsb_newton_t nw, float *x_dev, const float *anchor_dev
     for (int32_t r : bt->reserved)
       if (r != 0) return newton_fail(nw, TSB_E_INVALID, "reserved fields must be 0");
   }
-  tsb_pcg_t s = nw->s;
-  tsb_handle_t h = s->h;
-  DeviceGuard guard(h->device);
-  if (!guard.ok) return newton_fail(nw, TSB_E_CUDA, "cannot select the handle's CUDA device");
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const bool prox = anchor_dev != nullptr;
-  rc = newton_tr_alloc(nw, prox, st);
-  if (rc != TSB_OK) return rc;
-  const tsb_newton_tr_options_t &o = *opt;
-  const tsb::NewtonParams &W = nw->W;
-  const tsb::ProxParams pp{x_dev, anchor_dev, weight_dev, nw->prox_part};
-  const tsb::ProxParams *p = prox ? &pp : nullptr;
-  const tsb::NewtonTrRule R{o.gtol, o.radius_init, o.radius_min, o.radius_max, o.accept, o.eta};
-  const tsb_pcg_options_t po{o.max_iter, o.rtol, 0, {0, 0, 0, 0, 0}};
-  const float *shift = prox ? weight_dev : nullptr;     // an unusable w_c only reaches a sphere whose b_c is 0
-  // 1-2: b = -grad, the diagonal blocks; frozen spheres' b = 0 (prox: b -= w (x - y))
-  rc = energy_grad_impl(h, x_dev, terms->c1, terms->c2, terms->c3, terms->order, -1.f, nullptr, nw->energy, 1, W.b, nullptr, st);
-  if (rc == TSB_OK) rc = tsb_hess_diag(h, x_dev, terms, 1.f, nullptr, W.diag, st);
-  if (rc != TSB_OK) return newton_fail(nw, rc, h->err);
-  cudaError_t e = tsb::launch_newton_tr_prep(s->P, W, p, st);
-  if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
-  // 3: the preconditioner (shift w_c);  4: the radius on a first step
-  rc = tsb_pcg_set_blocks_ex(s, W.diag, o.rel_floor, shift, nullptr, st);
-  if (rc != TSB_OK) return newton_fail(nw, rc, s->err);
-  const tsb::NewtonTrParams T{nw->tr_state, nw->tr_radius, s->tr};
-  e = tsb::launch_newton_tr_radius(s->P, W, T, R, st);
-  if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
-  // 5: the trust-region solve
-  rc = tsb_pcg_solve_tr(s, x_dev, W.b, terms, &po, shift, nw->tr_radius, W.d, nullptr, nullptr, st);
-  if (rc != TSB_OK) return newton_fail(nw, rc, s->err);
-  // 6: b.d and |d|^2 (prox: and d.(x - y)) per chunk;  7: the line search at alpha = 1 (bt: at 2^-k, k < n_alpha)
-  e = tsb::launch_newton_dots(s->P, W, p, st);
-  if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
-  rc = tsb_line_search(h, x_dev, W.d, terms, W.alphas, bt ? bt->n_alpha : 1, nw->delta, nullptr, W.sphere_delta, W.sphere_step, st);
-  if (rc != TSB_OK) return newton_fail(nw, rc, h->err);
-  // 8-9: decision (bt: with backtracking), step
-  const tsb::NewtonBacktrack B{bt ? bt->sigma : 0.f, bt ? bt->n_alpha : 1};
-  e = tsb::launch_newton_tr_decide(s->P, W, T, R, p, records_out_dev, st, bt ? &B : nullptr);
-  if (e == cudaSuccess) e = tsb::launch_sphere_axpy(s->P, x_dev, W.alpha_sphere, W.d, x_dev, st);
-  if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
-  return TSB_OK;
+  return newton_run(nw, x_dev, anchor_dev, weight_dev, terms, NewtonStep(*opt, bt, records_out_dev), stream);
 }
 
 /* ---- Assembled Hessian (tsb_hessian.cu) ---- */
@@ -1244,12 +1168,7 @@ int tsb_hessian_pattern(tsb_hessian_t hs, int64_t *nnzb, int32_t *crow_dev_out, 
 int tsb_hessian_assemble(tsb_hessian_t hs, const float *x_dev, const tsb_terms_t *terms, float *values_dev, void *stream) {
   if (!hs) return TSB_E_INVALID;
   if (!x_dev || !terms || !values_dev) return hessian_fail(hs, TSB_E_INVALID, "x_dev, terms and values_dev must be non-null");
-  if (terms->order != 2 && terms->order != 4) return hessian_fail(hs, TSB_E_INVALID, "order must be 2 or 4");
-  const tsb_handle_t h = hs->s->h;
-  if (terms->c3 != 0.f && !h->amips)
-    return hessian_fail(hs, TSB_E_INVALID, "c3 != 0 needs a handle created with tsb_options_t.enable_amips = 1");
-  if (hs->psd && !(terms->c1 >= 0.f && terms->c2 >= 0.f && terms->c3 >= 0.f))
-    return hessian_fail(hs, TSB_E_INVALID, "the projected Hessian needs c1, c2 and c3 >= 0 (projection does not commute with a negative weight)");
+  if (const char *m = check_terms(hs->s->h, hs->psd, *terms)) return hessian_fail(hs, TSB_E_INVALID, m);
   DeviceGuard guard(hs->device);
   if (!guard.ok) return hessian_fail(hs, TSB_E_CUDA, "cannot select the handle's CUDA device");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);

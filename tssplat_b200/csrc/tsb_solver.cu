@@ -159,7 +159,8 @@ __device__ __forceinline__ F3 shifted(F3 hp, F3 p, float mu) {
 
 // Partial of p.Hp (SHIFT: p.(Hp + mu_c p)) of every chunk of an active component.
 template <bool SHIFT>
-__device__ __forceinline__ void curv_body(const PcgParams &s, const float *__restrict__ shift, double *sh) {
+__global__ void __launch_bounds__(kT) pcg_curv_kernel(const PcgParams s, const float *__restrict__ shift) {
+  __shared__ double sh[kT / 32];
   const int c = s.chunk[3 * blockIdx.x];
   if (s.comp[c].st_dir != kPcgActive) return;
   const int begin = s.chunk[3 * blockIdx.x + 1], end = s.chunk[3 * blockIdx.x + 2];
@@ -174,16 +175,6 @@ __device__ __forceinline__ void curv_body(const PcgParams &s, const float *__res
   if (threadIdx.x == 0) s.part[kPartCols * size_t(blockIdx.x) + kPHp] = q;
 }
 
-__global__ void __launch_bounds__(kT) pcg_curv_kernel(const PcgParams s) {
-  __shared__ double sh[kT / 32];
-  curv_body<false>(s, nullptr, sh);
-}
-
-__global__ void __launch_bounds__(kT) pcg_curv_shift_kernel(const PcgParams s, const float *__restrict__ shift) {
-  __shared__ double sh[kT / 32];
-  curv_body<true>(s, shift, sh);
-}
-
 // tau >= 0 with |d + tau p|_M = Delta from the recurrences, in the form without cancellation (Delta2 = Delta^2); 0 when
 // d is already on or outside the boundary or p has no length
 __device__ __forceinline__ double boundary_tau(double pMp, double dMp, double dMd, double Delta2) {
@@ -196,10 +187,11 @@ __device__ __forceinline__ double boundary_tau(double pMp, double dMp, double dM
 // d += alpha p, r -= alpha Hp, z = P r and the partials of the new r.z and r.r.  SHIFT: Hp + mu_c p in place of Hp.
 // TR, with a finite radius Delta_c: p.Hp <= 0, or a step that would end at |d + alpha p|_M >= Delta_c, stops the component
 // on the boundary instead, d += tau p (NEGCURV_BOUNDARY, BOUNDARY); r and z are then left as they were.  With Delta_c =
-// +inf every value written is the one the plain body writes.
+// +inf every value written is the one TR = false writes.
 template <bool SHIFT, bool TR>
-__device__ __forceinline__ void update_body(const PcgParams &s, float *__restrict__ d, int iter, const float *__restrict__ shift,
-                                            const TrParams &t, double *sh) {
+__global__ void __launch_bounds__(kT) pcg_update_kernel(const PcgParams s, float *__restrict__ d, int iter,
+                                                        const float *__restrict__ shift, const TrParams t) {
+  __shared__ double sh[kT / 32];
   const int c = s.chunk[3 * blockIdx.x];
   const bool lead = int(blockIdx.x) == s.comp_chunk[c] && threadIdx.x == 0;
   PcgComp &C = s.comp[c];
@@ -266,70 +258,9 @@ __device__ __forceinline__ void update_body(const PcgParams &s, float *__restric
   if (TR && lead) t.comp[c].step = alpha;
 }
 
-__global__ void __launch_bounds__(kT) pcg_update_kernel(const PcgParams s, float *__restrict__ d, int iter) {
-  __shared__ double sh[kT / 32];
-  update_body<false, false>(s, d, iter, nullptr, TrParams{}, sh);
-}
-
-__global__ void __launch_bounds__(kT) pcg_update_shift_kernel(const PcgParams s, float *__restrict__ d, int iter,
-                                                              const float *__restrict__ shift) {
-  __shared__ double sh[kT / 32];
-  update_body<true, false>(s, d, iter, shift, TrParams{}, sh);
-}
-
-__global__ void __launch_bounds__(kT) pcg_update_tr_kernel(const PcgParams s, float *__restrict__ d, int iter, const TrParams t) {
-  __shared__ double sh[kT / 32];
-  update_body<false, true>(s, d, iter, nullptr, t, sh);
-}
-
-__global__ void __launch_bounds__(kT) pcg_update_shift_tr_kernel(const PcgParams s, float *__restrict__ d, int iter,
-                                                                 const float *__restrict__ shift, const TrParams t) {
-  __shared__ double sh[kT / 32];
-  update_body<true, true>(s, d, iter, shift, t, sh);
-}
-
-// Folds r.z and r.r, tests convergence and sets the next direction p = z + beta p; a stopped component gets p = 0, so
-// later products leave it untouched.  FIRST: the direction of iteration 0 (p = z), which also initialises the state.
-template <bool FIRST>
-__global__ void __launch_bounds__(kT) pcg_dir_kernel(const PcgParams s, float rtol) {
-  __shared__ double sh[kT / 32];
-  const int c = s.chunk[3 * blockIdx.x];
-  const bool lead = int(blockIdx.x) == s.comp_chunk[c] && threadIdx.x == 0;
-  PcgComp &C = s.comp[c];
-  if (!FIRST && C.idle) return;
-  int st = FIRST ? kPcgActive : C.st_upd;
-  float beta = 0.f;
-  if (st == kPcgActive) {
-    const double2 f = make_double2(fold(s.part, kRz, s.comp_chunk[c], s.comp_chunk[c + 1], sh),
-                                   fold(s.part, kRr, s.comp_chunk[c], s.comp_chunk[c + 1], sh));   // (r.z, r.r)
-    if (FIRST) {
-      if (f.y == 0.0) st = TSB_PCG_ZERO_RHS;
-      if (lead) { C.rz = f.x; C.rz_prev = f.x; C.bb = f.y; C.rr = f.y; C.dHd = 0.0; C.st_upd = st; C.idle = 0; C.n_hvp = 0; }
-    } else {
-      if (sqrt(f.y) <= double(rtol) * sqrt(C.bb)) st = TSB_PCG_CONVERGED;
-      beta = float(f.x / C.rz_prev);
-      if (lead) { C.rz = f.x; C.rr = f.y; }
-    }
-  }
-  if (lead) C.st_dir = st;
-  const int begin = s.chunk[3 * blockIdx.x + 1], end = s.chunk[3 * blockIdx.x + 2];
-  const int e = begin + int(threadIdx.x);
-  if (e < end) {
-    const int v = s.vert[e];
-    F3 p{0.f, 0.f, 0.f};
-    if (st == kPcgActive) {
-      p = ld3(s.z, v);
-      if (!FIRST) { const F3 q = ld3(s.p, v); p.x += beta * q.x; p.y += beta * q.y; p.z += beta * q.z; }
-    }
-    st3(s.p, v, p);
-  }
-}
-
-// pcg_dir_kernel with the trust-region recurrences: the lead also advances them (Steihaug; r^T p_k = 0 and
-// d_k^T M z_{k+1} = r_{k+1}^T d_k = 0):
+// The trust-region recurrences (TR), advanced by the lead (Steihaug; r^T p_k = 0 and d_k^T M z_{k+1} = r_{k+1}^T d_k = 0):
 //   FIRST: pMp = r.z, dMp = dMd = 0;  after a step s along p:  dMd += 2 s dMp + s^2 pMp, and, if still active,
 //   dMp = beta (dMp + s pMp), pMp = r.z + beta^2 pMp (beta the fp32 value p is formed with, old pMp on the right).
-// A kernel of its own rather than a flag on pcg_dir_kernel's body: that keeps pcg_dir_kernel's machine code as it was.
 __device__ __forceinline__ void tr_advance(TrComp &T, bool active, double beta, double rz) {
   const double a = T.step, pMp = T.pMp, dMp = T.dMp;
   T.dMd = T.dMd + 2.0 * a * dMp + a * a * pMp;
@@ -339,8 +270,11 @@ __device__ __forceinline__ void tr_advance(TrComp &T, bool active, double beta, 
   }
 }
 
-template <bool FIRST>
-__global__ void __launch_bounds__(kT) pcg_dir_tr_kernel(const PcgParams s, float rtol, const TrParams t) {
+// Folds r.z and r.r, tests convergence and sets the next direction p = z + beta p; a stopped component gets p = 0, so
+// later products leave it untouched.  FIRST: the direction of iteration 0 (p = z), which also initialises the state.
+// TR: the lead also advances the trust-region recurrences.
+template <bool FIRST, bool TR>
+__global__ void __launch_bounds__(kT) pcg_dir_kernel(const PcgParams s, float rtol, const TrParams t) {
   __shared__ double sh[kT / 32];
   const int c = s.chunk[3 * blockIdx.x];
   const bool lead = int(blockIdx.x) == s.comp_chunk[c] && threadIdx.x == 0;
@@ -354,13 +288,13 @@ __global__ void __launch_bounds__(kT) pcg_dir_tr_kernel(const PcgParams s, float
     if (FIRST) {
       if (f.y == 0.0) st = TSB_PCG_ZERO_RHS;
       if (lead) { C.rz = f.x; C.rz_prev = f.x; C.bb = f.y; C.rr = f.y; C.dHd = 0.0; C.st_upd = st; C.idle = 0; C.n_hvp = 0; }
-      if (lead) { t.comp[c].pMp = f.x; t.comp[c].dMp = 0.0; t.comp[c].dMd = 0.0; }
+      if (TR && lead) { t.comp[c].pMp = f.x; t.comp[c].dMp = 0.0; t.comp[c].dMd = 0.0; }
     } else {
       if (sqrt(f.y) <= double(rtol) * sqrt(C.bb)) st = TSB_PCG_CONVERGED;
       beta = float(f.x / C.rz_prev);
-      if (lead) { C.rz = f.x; C.rr = f.y; tr_advance(t.comp[c], st == kPcgActive, double(beta), f.x); }
+      if (lead) { C.rz = f.x; C.rr = f.y; if (TR) tr_advance(t.comp[c], st == kPcgActive, double(beta), f.x); }
     }
-  } else if (!FIRST && lead) {     // stopped by the update (boundary, negative curvature): its last step still counts
+  } else if (TR && !FIRST && lead) {     // stopped by the update (boundary, negative curvature): its last step still counts
     tr_advance(t.comp[c], false, 0.0, 0.0);
   }
   if (lead) C.st_dir = st;
@@ -463,7 +397,8 @@ __device__ __forceinline__ bool prox_weight_ok(float wc) { return wc >= 0.f && w
 // w_c is unusable, and elsewhere b_v += (-w_c)(x_v - y_v), each operation rounded on its own (no contraction), as eager
 // torch rounds b + (-w) * (x - y); w_c = 0 leaves b as it is.
 template <bool PROX>
-__device__ __forceinline__ void prep_body(const PcgParams &s, const NewtonParams &w, const ProxParams &p, double *sh) {
+__global__ void __launch_bounds__(kT) newton_prep_kernel(const PcgParams s, const NewtonParams w, const ProxParams p) {
+  __shared__ double sh[kT / 32];
   const int c = s.chunk[3 * blockIdx.x];
   const int e = s.chunk[3 * blockIdx.x + 1] + int(threadIdx.x);
   double m = -INFINITY;
@@ -488,21 +423,11 @@ __device__ __forceinline__ void prep_body(const PcgParams &s, const NewtonParams
   if (threadIdx.x == 0) w.part[kNwCols * size_t(blockIdx.x) + kNwMaxD] = m;
 }
 
-__global__ void __launch_bounds__(kT) newton_prep_kernel(const PcgParams s, const NewtonParams w) {
-  __shared__ double sh[kT / 32];
-  prep_body<false>(s, w, ProxParams{}, sh);
-}
-
-__global__ void __launch_bounds__(kT) newton_prep_prox_kernel(const PcgParams s, const NewtonParams w, const ProxParams p) {
-  __shared__ double sh[kT / 32];
-  prep_body<true>(s, w, p, sh);
-}
-
 // mu_c = tau * max (D_v)_ii on a component's first step (clamped to [mu_min, mu_max]), nu_c = 2; the fp32 shift of the
 // solve (thread = component).  PROX: mu_c = tau * (max (D_v)_ii + w_c) and the shift is mu_c + w_c (w_c read as 0 where
 // it is unusable: that component's right-hand side is 0).
 template <bool PROX>
-__device__ __forceinline__ void shift_body(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, const ProxParams &p) {
+__global__ void __launch_bounds__(kT) newton_shift_kernel(const PcgParams s, const NewtonParams w, NewtonRule r, const ProxParams p) {
   const int c = blockIdx.x * kT + int(threadIdx.x);
   if (c >= s.n_components) return;
   NewtonComp &N = w.comp[c];
@@ -518,20 +443,12 @@ __device__ __forceinline__ void shift_body(const PcgParams &s, const NewtonParam
   w.shift[c] = float(PROX ? N.mu + wc : N.mu);
 }
 
-__global__ void __launch_bounds__(kT) newton_shift_kernel(const PcgParams s, const NewtonParams w, NewtonRule r) {
-  shift_body<false>(s, w, r, ProxParams{});
-}
-
-__global__ void __launch_bounds__(kT) newton_shift_prox_kernel(const PcgParams s, const NewtonParams w, NewtonRule r,
-                                                               const ProxParams p) {
-  shift_body<true>(s, w, r, p);
-}
-
 // Per-chunk partials of b.d and d.d (b.d exactly as pcg_bdotd_kernel forms it).  PROX: also d.(x - y), in its own array.
 template <bool PROX>
-__device__ __forceinline__ void dots_body(const PcgParams &s, const NewtonParams &w, const ProxParams &p, double *sh) {
+__global__ void __launch_bounds__(kT) newton_dots_kernel(const PcgParams s, const NewtonParams w, const ProxParams p) {
+  __shared__ double sh[kT / 32];
   const int e = s.chunk[3 * blockIdx.x + 1] + int(threadIdx.x);
-  double bd = 0.0, dd = 0.0, dx = 0.0;
+  double dd = 0.0, bd = 0.0, dx = 0.0;
   if (e < s.chunk[3 * blockIdx.x + 2]) {
     const int v = s.vert[e];
     const F3 d = ld3(w.d, v);
@@ -553,16 +470,6 @@ __device__ __forceinline__ void dots_body(const PcgParams &s, const NewtonParams
   }
 }
 
-__global__ void __launch_bounds__(kT) newton_dots_kernel(const PcgParams s, const NewtonParams w) {
-  __shared__ double sh[kT / 32];
-  dots_body<false>(s, w, ProxParams{}, sh);
-}
-
-__global__ void __launch_bounds__(kT) newton_dots_prox_kernel(const PcgParams s, const NewtonParams w, const ProxParams p) {
-  __shared__ double sh[kT / 32];
-  dots_body<true>(s, w, p, sh);
-}
-
 // Phi_c(x + a d) - Phi_c(x) from the line search's dE = E_c(x + a d) - E_c(x): dE + w_c (a d.(x - y) + a^2 |d|^2 / 2).
 // Without PROX, or with w_c = 0, it is dE itself.
 template <bool PROX>
@@ -573,8 +480,8 @@ __device__ __forceinline__ double step_change(float dE, double wc, double a, dou
 // The step choice and the damping update of every component (thread = component); see tsb_newton_step and
 // tsb_newton_prox_step in the header.
 template <bool PROX>
-__device__ __forceinline__ void decide_body(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, const ProxParams &p,
-                                            tsb_newton_sphere_t *__restrict__ out) {
+__global__ void __launch_bounds__(kT) newton_decide_kernel(const PcgParams s, const NewtonParams w, NewtonRule r,
+                                                           tsb_newton_sphere_t *__restrict__ out, const ProxParams p) {
   const int c = blockIdx.x * kT + int(threadIdx.x);
   if (c >= s.n_components) return;
   const PcgComp C = s.comp[c];
@@ -645,16 +552,6 @@ __device__ __forceinline__ void decide_body(const PcgParams &s, const NewtonPara
   out[c] = o;
 }
 
-__global__ void __launch_bounds__(kT) newton_decide_kernel(const PcgParams s, const NewtonParams w, NewtonRule r,
-                                                           tsb_newton_sphere_t *__restrict__ out) {
-  decide_body<false>(s, w, r, ProxParams{}, out);
-}
-
-__global__ void __launch_bounds__(kT) newton_decide_prox_kernel(const PcgParams s, const NewtonParams w, NewtonRule r,
-                                                                tsb_newton_sphere_t *__restrict__ out, const ProxParams p) {
-  decide_body<true>(s, w, r, p, out);
-}
-
 // ---- Trust-region Newton step (tsb_newton_tr_step) -------------------------------------------------------------------
 // It reuses the prep kernels above (their max (D_v)_ii column is not read in this step) and puts the per-chunk partials
 // of b^T P b in that column instead: written by newton_tr_bpb_kernel, folded by newton_tr_radius_kernel.
@@ -694,10 +591,10 @@ __global__ void __launch_bounds__(kT) newton_tr_radius_kernel(const PcgParams s,
 // Acceptance and radius update of every component (thread = component); see tsb_newton_tr_step in the header.  LS: a
 // step the trust-region rule rejects is backtracked to the largest 2^-k (k >= 1) of the line search with the Armijo
 // decrease below the inversion bound (tsb_newton_tr_step_ex); the backtracking options b are read only then.
-template <bool PROX, bool LS = false>
-__device__ __forceinline__ void decide_tr_body(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t,
-                                               const NewtonTrRule &r, const ProxParams &p, tsb_newton_tr_sphere_t *__restrict__ out,
-                                               const NewtonBacktrack &b = NewtonBacktrack{}) {
+template <bool PROX, bool LS>
+__global__ void __launch_bounds__(kT) newton_decide_tr_kernel(const PcgParams s, const NewtonParams w, const NewtonTrParams t,
+                                                              const NewtonTrRule r, tsb_newton_tr_sphere_t *__restrict__ out,
+                                                              const ProxParams p, const NewtonBacktrack b) {
   const int c = blockIdx.x * kT + int(threadIdx.x);
   if (c >= s.n_components) return;
   const PcgComp C = s.comp[c];
@@ -779,42 +676,13 @@ __device__ __forceinline__ void decide_tr_body(const PcgParams &s, const NewtonP
   out[c] = o;
 }
 
-__global__ void __launch_bounds__(kT) newton_decide_tr_kernel(const PcgParams s, const NewtonParams w, const NewtonTrParams t,
-                                                              const NewtonTrRule r, tsb_newton_tr_sphere_t *__restrict__ out) {
-  decide_tr_body<false>(s, w, t, r, ProxParams{}, out);
-}
-
-__global__ void __launch_bounds__(kT) newton_decide_tr_prox_kernel(const PcgParams s, const NewtonParams w, const NewtonTrParams t,
-                                                                   const NewtonTrRule r, tsb_newton_tr_sphere_t *__restrict__ out,
-                                                                   const ProxParams p) {
-  decide_tr_body<true>(s, w, t, r, p, out);
-}
-
-__global__ void __launch_bounds__(kT) newton_decide_trls_kernel(const PcgParams s, const NewtonParams w, const NewtonTrParams t,
-                                                                const NewtonTrRule r, const NewtonBacktrack b,
-                                                                tsb_newton_tr_sphere_t *__restrict__ out) {
-  decide_tr_body<false, true>(s, w, t, r, ProxParams{}, out, b);
-}
-
-__global__ void __launch_bounds__(kT) newton_decide_trls_prox_kernel(const PcgParams s, const NewtonParams w, const NewtonTrParams t,
-                                                                     const NewtonTrRule r, const NewtonBacktrack b,
-                                                                     tsb_newton_tr_sphere_t *__restrict__ out, const ProxParams p) {
-  decide_tr_body<true, true>(s, w, t, r, p, out, b);
-}
-
 unsigned with_orphans(const PcgParams &s) { return unsigned(s.n_chunks + (s.n_orphans + kT - 1) / kT); }
+unsigned comp_blocks(const PcgParams &s) { return unsigned((s.n_components + kT - 1) / kT); }   // thread = component
 
 }  // namespace
 
 cudaError_t launch_pcg_blocks(const PcgParams &s, const float *diag, float rel_floor, float *inv_out, cudaStream_t st) {
   pcg_blocks_kernel<<<unsigned((s.n + kT - 1) / kT), kT, 0, st>>>(diag, s.n, rel_floor, s.pinv, inv_out);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_pcg_begin(const PcgParams &s, const float *b, float *d, cudaStream_t st, const TrParams *tr) {
-  pcg_init_kernel<<<with_orphans(s), kT, 0, st>>>(s, b, d);
-  if (!tr) pcg_dir_kernel<true><<<unsigned(s.n_chunks), kT, 0, st>>>(s, 0.f);
-  else pcg_dir_tr_kernel<true><<<unsigned(s.n_chunks), kT, 0, st>>>(s, 0.f, *tr);
   return cudaGetLastError();
 }
 
@@ -824,27 +692,20 @@ cudaError_t launch_pcg_blocks_shift(const PcgParams &s, const float *diag, float
   return cudaGetLastError();
 }
 
-cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, const float *shift, cudaStream_t st,
-                            const TrParams *tr) {
-  if (tr) {
-    if (shift) {
-      pcg_curv_shift_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, shift);
-      pcg_update_shift_tr_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, d, iter, shift, *tr);
-    } else {
-      pcg_curv_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s);
-      pcg_update_tr_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, d, iter, *tr);
-    }
-    pcg_dir_tr_kernel<false><<<unsigned(s.n_chunks), kT, 0, st>>>(s, rtol, *tr);
-    return cudaGetLastError();
-  }
-  if (shift) {
-    pcg_curv_shift_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, shift);
-    pcg_update_shift_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, d, iter, shift);
-  } else {
-    pcg_curv_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s);
-    pcg_update_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, d, iter);
-  }
-  pcg_dir_kernel<false><<<unsigned(s.n_chunks), kT, 0, st>>>(s, rtol);
+cudaError_t launch_pcg_begin(const PcgParams &s, const float *b, float *d, const TrParams *tr, cudaStream_t st) {
+  pcg_init_kernel<<<with_orphans(s), kT, 0, st>>>(s, b, d);
+  (tr ? pcg_dir_kernel<true, true> : pcg_dir_kernel<true, false>)<<<unsigned(s.n_chunks), kT, 0, st>>>(s, 0.f, tr ? *tr : TrParams{});
+  return cudaGetLastError();
+}
+
+cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, const float *shift, const TrParams *tr,
+                            cudaStream_t st) {
+  const TrParams t = tr ? *tr : TrParams{};
+  (shift ? pcg_curv_kernel<true> : pcg_curv_kernel<false>)<<<unsigned(s.n_chunks), kT, 0, st>>>(s, shift);
+  (shift ? (tr ? pcg_update_kernel<true, true> : pcg_update_kernel<true, false>)
+         : (tr ? pcg_update_kernel<false, true> : pcg_update_kernel<false, false>))<<<unsigned(s.n_chunks), kT, 0, st>>>(
+      s, d, iter, shift, t);
+  (tr ? pcg_dir_kernel<false, true> : pcg_dir_kernel<false, false>)<<<unsigned(s.n_chunks), kT, 0, st>>>(s, rtol, t);
   return cudaGetLastError();
 }
 
@@ -855,7 +716,7 @@ cudaError_t launch_pcg_count(const PcgParams &s, cudaStream_t st) {
 
 cudaError_t launch_pcg_records(const PcgParams &s, const float *b, const float *d, tsb_pcg_sphere_t *out, cudaStream_t st) {
   pcg_bdotd_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, b, d);
-  pcg_record_kernel<<<unsigned((s.n_components + kT - 1) / kT), kT, 0, st>>>(s, out);
+  pcg_record_kernel<<<comp_blocks(s), kT, 0, st>>>(s, out);
   return cudaGetLastError();
 }
 
@@ -864,53 +725,41 @@ cudaError_t launch_sphere_axpy(const PcgParams &s, const float *x, const float *
   return cudaGetLastError();
 }
 
-cudaError_t launch_newton_prep(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, const ProxParams *p,
-                               cudaStream_t st) {
-  const unsigned comp_blocks = unsigned((s.n_components + kT - 1) / kT);
-  if (p) {
-    newton_prep_prox_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w, *p);
-    newton_shift_prox_kernel<<<comp_blocks, kT, 0, st>>>(s, w, r, *p);
-  } else {
-    newton_prep_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w);
-    newton_shift_kernel<<<comp_blocks, kT, 0, st>>>(s, w, r);
-  }
+cudaError_t launch_newton_prep(const PcgParams &s, const NewtonParams &w, const ProxParams *p, cudaStream_t st) {
+  (p ? newton_prep_kernel<true> : newton_prep_kernel<false>)<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w, p ? *p : ProxParams{});
+  return cudaGetLastError();
+}
+
+cudaError_t launch_newton_shift(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, const ProxParams *p,
+                                cudaStream_t st) {
+  (p ? newton_shift_kernel<true> : newton_shift_kernel<false>)<<<comp_blocks(s), kT, 0, st>>>(s, w, r, p ? *p : ProxParams{});
   return cudaGetLastError();
 }
 
 cudaError_t launch_newton_dots(const PcgParams &s, const NewtonParams &w, const ProxParams *p, cudaStream_t st) {
-  if (p) newton_dots_prox_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w, *p);
-  else newton_dots_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w);
+  (p ? newton_dots_kernel<true> : newton_dots_kernel<false>)<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w, p ? *p : ProxParams{});
   return cudaGetLastError();
 }
 
 cudaError_t launch_newton_decide(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, const ProxParams *p,
                                  tsb_newton_sphere_t *out, cudaStream_t st) {
-  const unsigned comp_blocks = unsigned((s.n_components + kT - 1) / kT);
-  if (p) newton_decide_prox_kernel<<<comp_blocks, kT, 0, st>>>(s, w, r, out, *p);
-  else newton_decide_kernel<<<comp_blocks, kT, 0, st>>>(s, w, r, out);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_newton_tr_prep(const PcgParams &s, const NewtonParams &w, const ProxParams *p, cudaStream_t st) {
-  if (p) newton_prep_prox_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w, *p);
-  else newton_prep_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w);
+  (p ? newton_decide_kernel<true> : newton_decide_kernel<false>)<<<comp_blocks(s), kT, 0, st>>>(s, w, r, out,
+                                                                                                 p ? *p : ProxParams{});
   return cudaGetLastError();
 }
 
 cudaError_t launch_newton_tr_radius(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t, const NewtonTrRule &r,
                                     cudaStream_t st) {
   newton_tr_bpb_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w, t);
-  newton_tr_radius_kernel<<<unsigned((s.n_components + kT - 1) / kT), kT, 0, st>>>(s, w, t, r);
+  newton_tr_radius_kernel<<<comp_blocks(s), kT, 0, st>>>(s, w, t, r);
   return cudaGetLastError();
 }
 
 cudaError_t launch_newton_tr_decide(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t, const NewtonTrRule &r,
-                                    const ProxParams *p, tsb_newton_tr_sphere_t *out, cudaStream_t st, const NewtonBacktrack *bt) {
-  const unsigned comp_blocks = unsigned((s.n_components + kT - 1) / kT);
-  if (bt && p) newton_decide_trls_prox_kernel<<<comp_blocks, kT, 0, st>>>(s, w, t, r, *bt, out, *p);
-  else if (bt) newton_decide_trls_kernel<<<comp_blocks, kT, 0, st>>>(s, w, t, r, *bt, out);
-  else if (p) newton_decide_tr_prox_kernel<<<comp_blocks, kT, 0, st>>>(s, w, t, r, out, *p);
-  else newton_decide_tr_kernel<<<comp_blocks, kT, 0, st>>>(s, w, t, r, out);
+                                    const ProxParams *p, const NewtonBacktrack *bt, tsb_newton_tr_sphere_t *out, cudaStream_t st) {
+  (p ? (bt ? newton_decide_tr_kernel<true, true> : newton_decide_tr_kernel<true, false>)
+     : (bt ? newton_decide_tr_kernel<false, true> : newton_decide_tr_kernel<false, false>))<<<comp_blocks(s), kT, 0, st>>>(
+      s, w, t, r, out, p ? *p : ProxParams{}, bt ? *bt : NewtonBacktrack{});
   return cudaGetLastError();
 }
 

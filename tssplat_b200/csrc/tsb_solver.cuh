@@ -41,8 +41,6 @@ struct PcgParams {
   int32_t *active;             // [1] components still active (pcg_count_kernel)
 };
 
-// State of one component of the damped Newton step (tsb_newton_step).  The shift kernel writes mu, nu and init on a
-// component's first step, the decision kernel mu, nu and status; the other kernels only read it.  32 bytes.
 // Trust-region recurrences of one component (tsb_pcg_solve_tr), in preconditioner norm |v|_M^2 = v^T P^-1 v.  A separate
 // array, allocated by a workspace's first trust-region solve, so PcgComp and the plain solves are unchanged.  The lead
 // thread of the component's first chunk in the dir kernel writes pMp, dMp and dMd (the update kernel reads them in every
@@ -60,6 +58,8 @@ struct TrParams {
   TrComp *comp;          // [n_components]
 };
 
+// State of one component of the damped Newton step (tsb_newton_step).  The shift kernel writes mu, nu and init on a
+// component's first step, the decision kernel mu, nu and status; the other kernels only read it.  32 bytes.
 struct NewtonComp {
   double mu, nu;
   int32_t status;   // TSB_NEWTON_*
@@ -122,33 +122,31 @@ cudaError_t launch_pcg_blocks_shift(const PcgParams &s, const float *diag, float
                                     cudaStream_t st);
 // r = b, z = P r, d = 0 and the first direction; leaves every component ACTIVE or ZERO_RHS
 // (tr != nullptr: also initialises the trust-region recurrences)
-cudaError_t launch_pcg_begin(const PcgParams &s, const float *b, float *d, cudaStream_t st, const TrParams *tr = nullptr);
+cudaError_t launch_pcg_begin(const PcgParams &s, const float *b, float *d, const TrParams *tr, cudaStream_t st);
 // after Hp = H p of iteration `iter` (0-based) is complete on the stream: curvature, update and next direction; with
 // shift != nullptr the operator is H + shift[c] I; with tr != nullptr every component stays inside its radius
-cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, const float *shift, cudaStream_t st,
-                            const TrParams *tr = nullptr);
+cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, const float *shift, const TrParams *tr,
+                            cudaStream_t st);
 cudaError_t launch_pcg_count(const PcgParams &s, cudaStream_t st);
 cudaError_t launch_pcg_records(const PcgParams &s, const float *b, const float *d, tsb_pcg_sphere_t *out, cudaStream_t st);
 cudaError_t launch_sphere_axpy(const PcgParams &s, const float *x, const float *a, const float *d, float *out, cudaStream_t st);
-// The three launchers below run the proximal variants when p != nullptr.
-// b_c = 0 on frozen components, per-chunk max (D_v)_ii, then mu_c on a first step and the fp32 shift
-cudaError_t launch_newton_prep(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, const ProxParams *p,
-                               cudaStream_t st);
+// The Newton launchers below run the proximal variants when p != nullptr.
+// b_c = 0 on frozen components (prox: b -= w (x - y)), per-chunk max (D_v)_ii
+cudaError_t launch_newton_prep(const PcgParams &s, const NewtonParams &w, const ProxParams *p, cudaStream_t st);
+// damped step: mu_c on a first step and the fp32 shift
+cudaError_t launch_newton_shift(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, const ProxParams *p,
+                                cudaStream_t st);
 // per-chunk b.d and d.d (and d.(x - y))
 cudaError_t launch_newton_dots(const PcgParams &s, const NewtonParams &w, const ProxParams *p, cudaStream_t st);
-// step choice, damping update, records (out may be null)
+// damped step: step choice, damping update, records (out may be null)
 cudaError_t launch_newton_decide(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, const ProxParams *p,
                                  tsb_newton_sphere_t *out, cudaStream_t st);
-// Trust-region step (p != nullptr: the proximal objective).  b_c = 0 on frozen components (prox: b -= w (x - y)), without
-// the damping of launch_newton_prep
-cudaError_t launch_newton_tr_prep(const PcgParams &s, const NewtonParams &w, const ProxParams *p, cudaStream_t st);
-// after the preconditioner is set: b^T P b per component, Delta_c on a first step, the fp32 radius
+// trust-region step, after the preconditioner is set: b^T P b per component, Delta_c on a first step, the fp32 radius
 cudaError_t launch_newton_tr_radius(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t, const NewtonTrRule &r,
                                     cudaStream_t st);
-// acceptance, radius update, records (out may be null); bt != nullptr: a rejected step is backtracked along the line
-// search's n_alpha step sizes (tsb_newton_tr_step_ex)
+// trust-region step: acceptance, radius update, records (out may be null); bt != nullptr: a rejected step is backtracked
+// along the line search's n_alpha step sizes (tsb_newton_tr_step_ex)
 cudaError_t launch_newton_tr_decide(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t, const NewtonTrRule &r,
-                                    const ProxParams *p, tsb_newton_tr_sphere_t *out, cudaStream_t st,
-                                    const NewtonBacktrack *bt = nullptr);
+                                    const ProxParams *p, const NewtonBacktrack *bt, tsb_newton_tr_sphere_t *out, cudaStream_t st);
 
 }  // namespace tsb

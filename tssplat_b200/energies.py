@@ -263,8 +263,7 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         trust-region step (``DeviceNewton.trls_step``; the fields of ``newton.NEWTON_TRLS_DEFAULTS``)."""
         nw = self._device_newton()
         c1, c2 = self.coeff_scheduler(it)
-        run = {"lm": nw.step, "tr": nw.tr_step, "trls": nw.trls_step}[self._newton_method()]
-        return run(x.data, c1, c2, self.order_at(it), c3=self.amips_coeff, **opts)
+        return nw._step(self._newton_method(), x.data, c1, c2, self.order_at(it), self.amips_coeff, None, None, opts)
 
     def _newton_method(self) -> str:
         from .newton import METHODS

@@ -229,7 +229,7 @@ class DevicePCG:
         sh = self._shift(shift)
         rad = self._shift(radius, "radius")
         d = torch.empty((self.tet_sp.n, 3), dtype=torch.float32, device=dev)
-        raw = torch.empty((self.n_spheres, 8), dtype=torch.int32, device=dev)
+        raw = torch.empty((self.n_spheres, C.sizeof(self._capi.tsb_pcg_sphere_t)), dtype=torch.uint8, device=dev)
         terms = self._capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
         opt = self._capi.tsb_pcg_options_t(max_iter=int(max_iter), rtol=float(rtol), check_every=int(check_every))
         iters = C.c_int32(0)
@@ -242,8 +242,8 @@ class DevicePCG:
                                                  sh.data_ptr() if sh is not None else None, rad.data_ptr(), d.data_ptr(),
                                                  raw.data_ptr(), C.byref(iters), self._stream_ptr(dev))
         self._check(rc, "solve")
-        f = raw.view(torch.float32)
-        return DevicePCGResult(d, raw[:, 4], raw[:, 3], f[:, 0], f[:, 1], f[:, 2], int(iters.value))
+        f = self._capi.record_fields(raw, self._capi.tsb_pcg_sphere_t)
+        return DevicePCGResult(d=d, iters_run=int(iters.value), **{k: f[k] for k in DevicePCGResult._fields if k in f})
 
     def hvp_psd(self, x: torch.Tensor, v: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0):
         """``H+(x) v`` of ``c1 * smooth + c2 * barrier (+ c3 * amips)`` with every tet's Hessian projected to PSD at ``x``
@@ -304,10 +304,6 @@ NEWTON_TR_DEFAULTS = dict(max_iter=20, rtol=1e-2, rel_floor=1e-6, gtol=0.0, radi
 #: options of ``DeviceNewton.trls_step``: ``NEWTON_TR_DEFAULTS`` and the backtracking (``tsb_newton_backtrack_t``)
 NEWTON_TRLS_DEFAULTS = dict(NEWTON_TR_DEFAULTS, n_alpha=8, sigma=1e-4)
 
-#: the steps of ``DeviceNewton.minimize``: Levenberg-Marquardt (``step``), trust region (``tr_step``) or backtracking
-#: trust region (``trls_step``)
-METHODS = ("lm", "tr", "trls")
-
 
 class NewtonTRStepResult(NamedTuple):
     """What ``DeviceNewton.tr_step`` returns: device tensors [S], spheres in the order of their lowest vertex ids
@@ -324,6 +320,31 @@ class NewtonTRStepResult(NamedTuple):
     b_dot_d: torch.Tensor           # f32: b_c . d_c, b = -grad
     status: torch.Tensor            # i32: 0 active, 1 converged, 2 stalled (both frozen)
     first_vertex: torch.Tensor      # i32: lowest vertex id of the sphere
+
+
+class _Method(NamedTuple):
+    defaults: dict                  # the options and their defaults
+    what: str                       # what an unknown option's error calls them
+    structs: tuple                  # the C entry's option structs (names in _capi), filled by field name from the options
+    entry: str                      # the C entry (anchor and weight may be null unless ``plain`` takes that case)
+    plain: Optional[str]            # the C entry without anchor and weight, if another
+    record: str                     # the record struct
+    result: type
+    name: str                       # the DeviceNewton method
+
+
+_STEPS = {
+    "lm": _Method(NEWTON_DEFAULTS, "Newton", ("tsb_newton_options_t",), "tsb_newton_prox_step", "tsb_newton_step",
+                  "tsb_newton_sphere_t", NewtonStepResult, "step"),
+    "tr": _Method(NEWTON_TR_DEFAULTS, "trust-region", ("tsb_newton_tr_options_t",), "tsb_newton_tr_step", None,
+                  "tsb_newton_tr_sphere_t", NewtonTRStepResult, "tr_step"),
+    "trls": _Method(NEWTON_TRLS_DEFAULTS, "backtracking trust-region", ("tsb_newton_tr_options_t", "tsb_newton_backtrack_t"),
+                    "tsb_newton_tr_step_ex", None, "tsb_newton_tr_sphere_t", NewtonTRStepResult, "trls_step"),
+}
+
+#: the steps of ``DeviceNewton.minimize``: Levenberg-Marquardt (``step``), trust region (``tr_step``) or backtracking
+#: trust region (``trls_step``)
+METHODS = tuple(_STEPS)
 
 
 class DeviceNewton:
@@ -380,13 +401,27 @@ class DeviceNewton:
         """Every sphere ACTIVE again, its damping (and trust radius) re-initialised at the next step."""
         self._check(self._capi.lib.tsb_newton_reset(self._nw, self._stream_ptr(self.tet_sp.device)), "reset")
 
+    def _options(self, method: str, opts: dict) -> list:
+        """The option structs of ``method``'s C entry from its defaults updated with ``opts``."""
+        m = _STEPS[method]
+        bad = set(opts) - set(m.defaults)
+        if bad:
+            raise TypeError(f"unknown {m.what} options: {sorted(bad)}")
+        o = {**m.defaults, **opts}
+        structs = [getattr(self._capi, name) for name in m.structs]
+        return [S(**{k: (int(o[k]) if t is C.c_int32 else float(o[k])) for k, t in S._fields_ if k in o}) for S in structs]
+
     def options(self, **opts):
         """``tsb_newton_options_t`` from ``NEWTON_DEFAULTS`` updated with ``opts``."""
-        bad = set(opts) - set(NEWTON_DEFAULTS)
-        if bad:
-            raise TypeError(f"unknown Newton options: {sorted(bad)}")
-        o = {**NEWTON_DEFAULTS, **opts}
-        return self._capi.tsb_newton_options_t(**{k: (int(v) if k in ("max_iter", "n_alpha") else float(v)) for k, v in o.items()})
+        return self._options("lm", opts)[0]
+
+    def tr_options(self, **opts):
+        """``tsb_newton_tr_options_t`` from ``NEWTON_TR_DEFAULTS`` updated with ``opts``."""
+        return self._options("tr", opts)[0]
+
+    def trls_options(self, **opts):
+        """(``tsb_newton_tr_options_t``, ``tsb_newton_backtrack_t``) from ``NEWTON_TRLS_DEFAULTS`` updated with ``opts``."""
+        return tuple(self._options("trls", opts))
 
     def _x_anchor(self, x, anchor, weight):
         """Checks x (updated in place) and the proximal pair; returns the weight tensor or None."""
@@ -405,38 +440,23 @@ class DeviceNewton:
             raise RuntimeError("anchor must not be x (x is updated in place while the anchor is read)")
         return self.pcg._shift(weight, "weight")
 
-    def tr_options(self, **opts):
-        """``tsb_newton_tr_options_t`` from ``NEWTON_TR_DEFAULTS`` updated with ``opts``."""
-        bad = set(opts) - set(NEWTON_TR_DEFAULTS)
-        if bad:
-            raise TypeError(f"unknown trust-region options: {sorted(bad)}")
-        o = {**NEWTON_TR_DEFAULTS, **opts}
-        return self._capi.tsb_newton_tr_options_t(**{k: (int(v) if k == "max_iter" else float(v)) for k, v in o.items()})
-
-    def trls_options(self, **opts):
-        """(``tsb_newton_tr_options_t``, ``tsb_newton_backtrack_t``) from ``NEWTON_TRLS_DEFAULTS`` updated with ``opts``."""
-        bad = set(opts) - set(NEWTON_TRLS_DEFAULTS)
-        if bad:
-            raise TypeError(f"unknown backtracking trust-region options: {sorted(bad)}")
-        o = {**NEWTON_TRLS_DEFAULTS, **opts}
-        bt = self._capi.tsb_newton_backtrack_t(n_alpha=int(o.pop("n_alpha")), sigma=float(o.pop("sigma")))
-        return self.tr_options(**o), bt
-
-    def _tr_run(self, x, c1, c2, order, c3, anchor, weight, opt, bt, what) -> NewtonTRStepResult:
+    def _step(self, method: str, x, c1, c2, order, c3, anchor, weight, opts: dict):
+        """One step of ``method`` (a key of ``_STEPS``): the runner of ``step``, ``tr_step`` and ``trls_step``."""
+        m = _STEPS[method]
+        opt = self._options(method, opts)
         w = self._x_anchor(x, anchor, weight)
-        raw = torch.empty((self.n_spheres, 16), dtype=torch.int32, device=self.tet_sp.device)
+        rec = getattr(self._capi, m.record)
+        raw = torch.empty((self.n_spheres, C.sizeof(rec)), dtype=torch.uint8, device=self.tet_sp.device)
         terms = self._capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
-        args = (self._nw, x.data_ptr(), anchor.data_ptr() if anchor is not None else None, w.data_ptr() if w is not None else None,
-                C.byref(terms), C.byref(opt))
-        st = self._stream_ptr(self.tet_sp.device)
-        if bt is None:
-            rc = self._capi.lib.tsb_newton_tr_step(*args, raw.data_ptr(), st)
+        args = (C.byref(terms), *(C.byref(o) for o in opt), raw.data_ptr(), self._stream_ptr(self.tet_sp.device))
+        if anchor is None and m.plain:
+            rc = getattr(self._capi.lib, m.plain)(self._nw, x.data_ptr(), *args)
         else:
-            rc = self._capi.lib.tsb_newton_tr_step_ex(*args, C.byref(bt), raw.data_ptr(), st)
-        self._check(rc, what)
-        f64, f32 = raw[:, 0:4].view(torch.float64), raw[:, 4:10].view(torch.float32)
-        return NewtonTRStepResult(f32[:, 0], f32[:, 1], f32[:, 2], f64[:, 0], f64[:, 1], f32[:, 4], f32[:, 5], raw[:, 10],
-                                  raw[:, 11], f32[:, 3], raw[:, 12], raw[:, 13])
+            rc = getattr(self._capi.lib, m.entry)(self._nw, x.data_ptr(), anchor.data_ptr() if anchor is not None else None,
+                                                  w.data_ptr() if w is not None else None, *args)
+        self._check(rc, m.name)
+        f = self._capi.record_fields(raw, rec)
+        return m.result(*(f[k] for k in m.result._fields))
 
     def trls_step(self, x: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0,
                   anchor: Optional[torch.Tensor] = None, weight=None, **opts) -> NewtonTRStepResult:
@@ -446,8 +466,7 @@ class DeviceNewton:
         ``dPhi <= -sigma 2^-k b.d``; the radius then becomes ``max(2^-k |d|_M, radius / 4)``, clamped.  The result's
         ``alpha`` is the fraction taken (1, ``2^-k`` or 0).  ``opts``: the fields of ``NEWTON_TRLS_DEFAULTS``.  The first
         call on a workspace allocates (as ``tr_step``'s), so it cannot be captured in a CUDA graph; later ones can."""
-        opt, bt = self.trls_options(**opts)
-        return self._tr_run(x, c1, c2, order, c3, anchor, weight, opt, bt, "trls_step")
+        return self._step("trls", x, c1, c2, order, c3, anchor, weight, opts)
 
     def tr_step(self, x: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0,
                 anchor: Optional[torch.Tensor] = None, weight=None, **opts) -> NewtonTRStepResult:
@@ -457,7 +476,7 @@ class DeviceNewton:
         negative curvature to its boundary), the step is taken whole or not at all, and the gain ratio grows or shrinks
         the radius.  ``opts``: the fields of ``NEWTON_TR_DEFAULTS``.  The first call on a workspace allocates, so it
         cannot be captured in a CUDA graph; later ones can."""
-        return self._tr_run(x, c1, c2, order, c3, anchor, weight, self.tr_options(**opts), None, "tr_step")
+        return self._step("tr", x, c1, c2, order, c3, anchor, weight, opts)
 
     def step(self, x: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0, anchor: Optional[torch.Tensor] = None,
              weight=None, **opts) -> NewtonStepResult:
@@ -471,20 +490,7 @@ class DeviceNewton:
         records' ``grad_norm``, ``delta`` and ``b_dot_d`` are then those of the proximal objective, and a sphere whose
         weight is NaN, infinite or negative is frozen (STALLED) without moving.  A linear term ``q . x`` folds into the
         anchor: pass ``y = x0 - q / w``."""
-        w = self._x_anchor(x, anchor, weight)
-        raw = torch.empty((self.n_spheres, 16), dtype=torch.int32, device=self.tet_sp.device)
-        terms = self._capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
-        opt = self.options(**opts)
-        st = self._stream_ptr(self.tet_sp.device)
-        if anchor is None:
-            rc = self._capi.lib.tsb_newton_step(self._nw, x.data_ptr(), C.byref(terms), C.byref(opt), raw.data_ptr(), st)
-        else:
-            rc = self._capi.lib.tsb_newton_prox_step(self._nw, x.data_ptr(), anchor.data_ptr(), w.data_ptr(), C.byref(terms),
-                                                     C.byref(opt), raw.data_ptr(), st)
-        self._check(rc, "step")
-        f64, f32 = raw[:, 0:4].view(torch.float64), raw[:, 4:8].view(torch.float32)
-        return NewtonStepResult(f32[:, 0], f32[:, 1], raw[:, 8], f32[:, 2], f64[:, 0], f64[:, 1], raw[:, 9], raw[:, 10],
-                                f32[:, 3], raw[:, 11], raw[:, 12])
+        return self._step("lm", x, c1, c2, order, c3, anchor, weight, opts)
 
     def minimize(self, x: torch.Tensor, n_steps: int, c1: float, c2: float, order: int, c3: float = 0.0,
                  check_every: int = 0, anchor: Optional[torch.Tensor] = None, weight=None, method: str = "lm", **opts):
@@ -505,8 +511,7 @@ class DeviceNewton:
             weight = self.pcg._shift(weight, "weight")         # one tensor for every step
         res = None
         for i in range(n_steps):
-            run = {"lm": self.step, "tr": self.tr_step, "trls": self.trls_step}[method]
-            res = run(x, c1, c2, order, c3=c3, anchor=anchor, weight=weight, **opts)
+            res = self._step(method, x, c1, c2, order, c3, anchor, weight, opts)
             if check_every > 0 and (i + 1) % check_every == 0 and i + 1 < n_steps:
                 if int((res.status == 0).sum()) == 0:
                     return i + 1, res

@@ -233,9 +233,8 @@ class TetSpheres:
         if rc:
             _capi.check(rc, self._h, "tet_spheres_ext.energy_grad_spheres")
         del keep
-        f64, f32, i32 = (raw[:, 0:24].view(torch.float64), raw[:, 24:28].view(torch.float32), raw[:, 28:40].view(torch.int32))
-        stats = SphereStats(f64[:, 0], f64[:, 1], f64[:, 2], f32[:, 0], i32[:, 0], i32[:, 1], i32[:, 2])
-        return energy, grad, stats
+        f = _capi.record_fields(raw, _capi.tsb_sphere_stats_t)
+        return energy, grad, SphereStats(*(f[k] for k in SphereStats._fields))
 
     def hvp(self, x: torch.Tensor, v: torch.Tensor, c1: float, c2: float, order: int, gradH=1.0,
             want_curv: bool = False, c3: float = 0.0):
