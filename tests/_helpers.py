@@ -122,6 +122,122 @@ def pole_mesh(m):
     return verts, tets.astype(np.int32)
 
 
+def whole_area_meshes():
+    """Components staged in the whole staging area (1024..2047 positions): one alone; two mixed with 600 double-buffered
+    twelve-tet spheres so that CTAs hold both kinds of segment; one of 2041 vertices that bank colouring pads past
+    2047 staging positions, which sends the mesh to the global-gather mode."""
+    from tssplat_b200.mesh import concat_spheres, make_pack, make_tet_sphere
+    tiny = make_pack(600, 12, seed=3, unique=6)
+    a, b = tiny.slice_spheres(0, 300), tiny.slice_spheres(300, 600)
+    mixed = concat_spheres([(a.verts, a.tets), make_tet_sphere(1500, 7000), (b.verts, b.tets), make_tet_sphere(1501, 7700)])
+    alone, near_cap = make_tet_sphere(1502, 7000), make_tet_sphere(1510, 10000)
+    return {"alone": (alone[0].astype(np.float32), alone[1]), "mixed": (mixed.verts, mixed.tets),
+            "near_cap": (near_cap[0].astype(np.float32), near_cap[1])}
+
+
+# The meshes whose plans have shapes only they produce (assert_plan_shape says which): the 988-neighbour pole, the
+# whole-area meshes and 2600 twelve-tet spheres (more segments per CTA than the shared-memory segment table holds).
+PLAN_SHAPE_MESHES = ("pole", "alone", "mixed", "near_cap", "tiny2600")
+_PLAN_SHAPE_CACHE = {}
+
+
+def plan_shape_mesh(name):
+    """(fp32 rest [n, 3], int32 tets [t, 4]) of a PLAN_SHAPE_MESHES mesh, built once."""
+    if name not in _PLAN_SHAPE_CACHE:
+        if name == "pole":
+            V, T = pole_mesh(988)
+        elif name == "tiny2600":
+            from tssplat_b200.mesh import make_pack
+            pk = make_pack(2600, 12, seed=3, unique=6)
+            V, T = pk.verts, pk.tets
+        else:
+            V, T = whole_area_meshes()[name]
+        _PLAN_SHAPE_CACHE[name] = (np.ascontiguousarray(V, np.float32).reshape(-1, 3),
+                                   np.ascontiguousarray(T, np.int32).reshape(-1, 4))
+    return _PLAN_SHAPE_CACHE[name]
+
+
+def cpu_plan(sp, verts, tets, ring_slots=0, force_global=False, enable_amips=False, deterministic=False):
+    """The host plan of handle sp, rebuilt on the CPU with the handle's warps and grid (and the ring it requested: row
+    splitting depends on it); it must agree with the handle, so what it shows is what the kernel ran."""
+    info = sp.info
+    plan = build_host_plan(verts, tets, nw=info["warps_per_cta"], grid=info["grid"], force_global=int(force_global),
+                           ring_slots=ring_slots, enable_amips=int(enable_amips), deterministic=int(deterministic))
+    assert plan["mode_global"] == info["mode_global"] and len(plan["segs"]) == info["n_segments"]
+    assert plan["nnz_padded"] == info["nnz_padded"]
+    return plan
+
+
+def row_blocks(plan):
+    """(len4, lanes per row) of every row block in the plan's streams."""
+    return [((int(h[0]) >> 24) & 63, 1 << (int(h[0]) >> 30)) for _, h in walk_streams(plan)[0]]
+
+
+def segment_patterns(plan):
+    """The set of per-CTA segment sequences, each segment 'whole' (whole staging area) or 'half' (double-buffered)."""
+    cs = plan["cta_seg"].reshape(-1, 2)
+    return {tuple("whole" if plan["segs"][s]["whole"] else "half" for s in range(a, b)) for a, b in cs if b > a}
+
+
+def assert_plan_shape(name, plan, kw):
+    """Fail unless the plan of a PLAN_SHAPE_MESHES mesh, built for handle options kw, has the shape that mesh is in the
+    suites for: the pole's (62, 4) row block (a 62-cell row block of 4 lanes, wrapping the ring); whole-area segments
+    (and for mixed a CTA with whole and double-buffered segments); near_cap in GLOBAL mode without forcing; tiny2600 at 16
+    warps with more segments in one CTA than the shared-memory segment table (16) holds."""
+    forced = bool(kw.get("force_global"))
+    if name == "pole":
+        assert (62, 4) in row_blocks(plan), "the pole's row is no longer one 62-cell row block of 4 lanes"
+    elif name in ("alone", "mixed"):
+        pats = segment_patterns(plan)
+        assert plan["mode_global"] == 0 and any("whole" in p for p in pats), pats
+        if name == "mixed":
+            assert any("whole" in p and "half" in p for p in pats), pats
+    elif name == "near_cap":
+        assert not forced and plan["mode_global"] == 1 and plan["max_comp_verts"] <= 2047
+    elif name == "tiny2600":
+        cs = plan["cta_seg"].reshape(-1, 2)
+        if plan["nw"] == 16:
+            assert (cs[:, 1] - cs[:, 0]).max() > 16, "no CTA reads segment headers past the shared-memory table"
+    else:
+        raise KeyError(name)
+    if forced:
+        assert plan["mode_global"] == 1
+
+
+# Handle options per PLAN_SHAPE_MESHES mesh, chosen to reach each shape's own paths (ring wraps of the pole's row block,
+# both gather modes, both CTA widths, the register prefetch past the segment table, the deterministic gather)
+PLAN_SHAPE_VARIANTS = {
+    "pole": [dict(), dict(warps_per_cta=8), dict(force_global=True), dict(warps_per_cta=8, ring_slots=4),
+             dict(warps_per_cta=8, force_global=True, ring_slots=4), dict(deterministic=True)],
+    "alone": [dict(), dict(warps_per_cta=8), dict(deterministic=True)],
+    "mixed": [dict(), dict(warps_per_cta=8), dict(deterministic=True)],
+    "near_cap": [dict(), dict(warps_per_cta=8)],
+    "tiny2600": [dict(), dict(warps_per_cta=8), dict(force_global=True), dict(ring_slots=3), dict(deterministic=True)],
+}
+
+
+def variant_id(kw):
+    return "-".join(f"{a}{b}" for a, b in kw.items()) or "default"
+
+
+def plan_shape_cases(deterministic=True):
+    """pytest parameters (mesh, kw) over PLAN_SHAPE_VARIANTS, without the deterministic handles if not deterministic."""
+    import pytest
+    return [pytest.param(m, kw, id=f"{m}-{variant_id(kw)}") for m, kws in PLAN_SHAPE_VARIANTS.items() for kw in kws
+            if deterministic or not kw.get("deterministic")]
+
+
+def check_handle_plan_shape(name, sp, kw, enable_amips=False):
+    """The CPU-rebuilt plan of handle sp (mesh name, created with options kw), checked by assert_plan_shape."""
+    V, T = plan_shape_mesh(name)
+    if kw.get("ring_slots"):
+        assert sp.info["ring_slots"] == kw["ring_slots"], "the ring was shrunk: this variant would not test its depth"
+    plan = cpu_plan(sp, V, T, ring_slots=kw.get("ring_slots", 0), force_global=kw.get("force_global", False),
+                    enable_amips=enable_amips, deterministic=kw.get("deterministic", False))
+    assert_plan_shape(name, plan, kw)
+    return plan
+
+
 PLAN_DEBUG_SO = os.path.join(ROOT, "tests", "native", "libtsb_plan_debug.so")
 CELLS_PER_CHUNK = 6      # tsb_plan.h kCellsPerChunk: cells per ring slot
 # Stream cells (tsb_plan.h): (cell bytes, bytes per index, tets per lane) of the STAGED (16-bit smem offsets) and

@@ -257,8 +257,9 @@ def test_det_parity(ext, kw):
 
 @pytest.mark.gpu
 def test_det_parity_whole_area_staging(ext):
-    from test_gpu_parity import _check, _check_amips, _whole_area_meshes
-    for name, (V, T) in _whole_area_meshes().items():
+    from _helpers import whole_area_meshes
+    from test_gpu_parity import _check, _check_amips
+    for name, (V, T) in whole_area_meshes().items():
         x_amips = perturb(V, T, 0.05, 4)
         if name == "mixed":
             x_amips = mirror_components(x_amips, T)

@@ -30,9 +30,9 @@ import scipy.sparse as sps
 from scipy.sparse.csgraph import connected_components
 
 import _helpers as H
-from _helpers import RIGID_MOTIONS, COracle, build_host_plan, emulate_kernel, mirror_components, rigid_motion
+from _helpers import RIGID_MOTIONS, COracle, build_host_plan, emulate_kernel, mirror_components, plan_shape_mesh, rigid_motion
 from oracle.tet_energy_oracle import ReferenceEnergyOracle
-from tssplat_b200.mesh import concat_spheres, make_pack, make_tet_sphere
+from tssplat_b200.mesh import make_pack
 
 U = 2.0 ** -24                  # fp32 unit roundoff
 # |E_gpu - E64| <= KAPPA u A + u |E64| per term, per sphere and in total (test_kappa_calibration: the fp32 re-enactment
@@ -286,16 +286,6 @@ def _shuffled():
     V = rng.normal(size=(n, 3)).astype(f32)
     V[ids] = pk.verts
     return V, ids[pk.tets].astype(np.int32)
-
-
-def _whole_area():
-    """Components staged in the whole staging area (test_gpu_parity's whole-area meshes): one alone, two mixed with 600
-    twelve-tet spheres, and one that bank colouring pads past 2047 staging positions (GLOBAL)."""
-    tiny = make_pack(600, 12, seed=3, unique=6)
-    a, b = tiny.slice_spheres(0, 300), tiny.slice_spheres(300, 600)
-    mixed = concat_spheres([(a.verts, a.tets), make_tet_sphere(1500, 7000), (b.verts, b.tets), make_tet_sphere(1501, 7700)])
-    near_cap = make_tet_sphere(1510, 10000)
-    return {"whole_mixed": (mixed.verts, mixed.tets), "whole_near_cap": (near_cap[0].astype(f32), near_cap[1])}
 
 
 MESHES = {
@@ -603,9 +593,7 @@ def gpu_geo(name):
             if name in MESHES:
                 V, T = MESHES[name]()
             else:
-                if "whole" not in _GEO:
-                    _GEO["whole"] = _whole_area()
-                V, T = _GEO["whole"][name]
+                V, T = plan_shape_mesh(name[len("whole_"):])
             g = Geo(V, T)
             _GEO[name] = (g, inputs(g))
     return _GEO[name]

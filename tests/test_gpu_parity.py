@@ -11,9 +11,9 @@ import numpy as np
 import pytest
 import torch
 
-from _helpers import (GOLDEN, RIGID_MOTIONS, COracle, build_host_plan, min_abs_J, mirror_components, pole_mesh,
-                      rigid_motion)
-from tssplat_b200.mesh import concat_spheres, make_pack, make_tet_sphere, perturb
+from _helpers import (GOLDEN, RIGID_MOTIONS, COracle, assert_plan_shape, build_host_plan, cpu_plan as _cpu_plan, min_abs_J,
+                      mirror_components, pole_mesh, rigid_motion, row_blocks, whole_area_meshes)
+from tssplat_b200.mesh import make_pack, make_tet_sphere, perturb
 
 pytestmark = pytest.mark.gpu
 REL = 1e-5
@@ -50,23 +50,6 @@ def _check(ext, verts, tets, x_np, c1, c2, order, gradH=1.0, scale=0, rel=REL, *
 VARIANTS = [dict(), dict(warps_per_cta=8), dict(force_global=True), dict(warps_per_cta=8, force_global=True),
             dict(warps_per_cta=8, ring_slots=3), dict(warps_per_cta=8, ring_slots=4),
             dict(warps_per_cta=8, force_global=True, ring_slots=3), dict(warps_per_cta=8, force_global=True, ring_slots=4)]
-
-
-def _cpu_plan(sp, verts, tets, ring_slots=0, force_global=False, enable_amips=False):
-    """The host plan of handle sp, rebuilt on the CPU with the handle's warps and grid (and the ring it requested: row
-    splitting depends on it); it must agree with the handle, so what it shows is what the kernel ran."""
-    I = sp.info
-    plan = build_host_plan(verts, tets, nw=I["warps_per_cta"], grid=I["grid"], force_global=int(force_global),
-                           ring_slots=ring_slots, enable_amips=int(enable_amips))
-    assert plan["mode_global"] == I["mode_global"] and len(plan["segs"]) == I["n_segments"]
-    assert plan["nnz_padded"] == I["nnz_padded"]
-    return plan
-
-
-def _segment_patterns(plan):
-    """The set of per-CTA segment sequences, each segment 'whole' (whole staging area) or 'half' (double-buffered)."""
-    cs = plan["cta_seg"].reshape(-1, 2)
-    return {tuple("whole" if plan["segs"][s]["whole"] else "half" for s in range(a, b)) for a, b in cs if b > a}
 
 
 def _check_amips(sp, verts, tets, x_np, order, c=(2e-4, 3e-4, 1e-4), gradH=0.8, rel=2e-5):
@@ -113,33 +96,16 @@ def test_displacement_precision_far_from_rest(ext, kw):
     assert float(e[0]) == 0.0 and float(g.abs().max()) == 0.0
 
 
-def _whole_area_meshes():
-    """Components staged in the whole staging area (1024..2047 positions): one alone; two mixed with 600 double-buffered
-    twelve-tet spheres so that CTAs hold both kinds of segment; one of 2041 vertices that bank colouring pads past
-    2047 staging positions, which sends the mesh to the global-gather mode."""
-    tiny = make_pack(600, 12, seed=3, unique=6)
-    a, b = tiny.slice_spheres(0, 300), tiny.slice_spheres(300, 600)
-    mixed = concat_spheres([(a.verts, a.tets), make_tet_sphere(1500, 7000), (b.verts, b.tets), make_tet_sphere(1501, 7700)])
-    alone, near_cap = make_tet_sphere(1502, 7000), make_tet_sphere(1510, 10000)
-    return {"alone": (alone[0].astype(np.float32), alone[1]), "mixed": (mixed.verts, mixed.tets),
-            "near_cap": (near_cap[0].astype(np.float32), near_cap[1])}
-
-
 @pytest.mark.parametrize("nw", [16, 8])
 def test_whole_area_staging(ext, nw):
     """Whole-area staging (its own staging pass, u / x bases, hand-overs and gradient-id base) against the oracle, at
     orders 2 and 4, benign and inverted, with and without AMIPS.  The handle's plan, rebuilt on the CPU, proves the
     path: whole segments, CTAs that mix whole and double-buffered segments, and the padded near-cap mesh in GLOBAL."""
-    for name, (v, t) in _whole_area_meshes().items():
+    for name, (v, t) in whole_area_meshes().items():
         sp = ext.TetSpheres(v.reshape(-1), t.reshape(-1), warps_per_cta=nw, enable_amips=True)
-        plan = _cpu_plan(sp, v, t, enable_amips=True)
-        pats = _segment_patterns(plan)
+        assert_plan_shape(name, _cpu_plan(sp, v, t, enable_amips=True), {})
         if name == "near_cap":
             assert sp.info["max_component_vertices"] <= 2047 and sp.info["mode_global"] == 1
-        else:
-            assert sp.info["mode_global"] == 0 and any("whole" in p for p in pats), pats
-        if name == "mixed":
-            assert any("whole" in p and "half" in p for p in pats), pats
         orc = COracle(v, t)
         for sig, order in ((0.02, 2), (0.35, 2), (0.35, 4)):
             x_np = perturb(v, t, sig, 4)
@@ -167,8 +133,7 @@ def test_high_valence_row(ext, kw):
     x_np = perturb(v, t, 0.3, 2)
     sp, e, g = _check(ext, v, t, x_np, 1e-3, 2e-3, 2, gradH=0.6, **kw)
     plan = _cpu_plan(sp, v, t, ring_slots=kw.get("ring_slots", 0), force_global=kw.get("force_global", False))
-    from test_host_logic import _block_headers
-    assert (62, 4) in _block_headers(plan)
+    assert (62, 4) in row_blocks(plan)
     assert e[2] > 0
     _check(ext, v, t, perturb(v, t, 0.05, 2), 1e-3, 2e-3, 4, **kw)
 

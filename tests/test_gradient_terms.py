@@ -21,7 +21,7 @@ import numpy as np
 import pytest
 import scipy.sparse as sps
 
-from _helpers import COracle, build_host_plan, emulate_kernel, mirror_components, walk_streams
+from _helpers import COracle, build_host_plan, emulate_kernel, mirror_components, plan_shape_mesh, walk_streams
 from oracle.tet_energy_oracle import build_G, rest_inverse, tet_laplacian
 from tssplat_b200.mesh import connected_components, make_pack, perturb
 
@@ -253,14 +253,10 @@ def _inputs(name):
         pk = make_pack(16, 4096, seed=0, unique=4)
         return pk.verts, pk.tets, [(f"sig{sig}-o{order}", perturb(pk, sigma_rel=sig, seed=1), (2e-4 / 16, 2e-4, 0.0), order)
                                    for sig, order in ((0.02, 2), (0.35, 4))]
-    if name == "tiny2600":
-        pk = make_pack(2600, 12, seed=3, unique=6)
-        return pk.verts, pk.tets, _mesh_inputs(pk.verts, pk.tets, True)
     if name.startswith("ragged"):
         return _ragged_inputs(int(name[len("ragged"):]))
-    from test_gpu_parity import _whole_area_meshes
-    V, T = _whole_area_meshes()[name]
-    return V, T, _mesh_inputs(V, T, name == "mixed")
+    V, T = plan_shape_mesh(name)
+    return V, T, _mesh_inputs(V, T, name in ("mixed", "tiny2600"))
 
 
 _CACHE = {}

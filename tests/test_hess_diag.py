@@ -14,7 +14,8 @@ import numpy as np
 import pytest
 import scipy.sparse as sp
 
-from _helpers import CELL_FORMAT, build_host_plan, min_abs_J, mirror_components, walk_streams
+from _helpers import (CELL_FORMAT, build_host_plan, check_handle_plan_shape, min_abs_J, mirror_components, plan_shape_cases,
+                      walk_streams)
 from oracle.tet_energy_oracle import ReferenceEnergyOracle, _cof3, _det3, rest_inverse
 from test_hvp import _cof_pair
 from tssplat_b200.mesh import make_pack, perturb
@@ -76,6 +77,42 @@ def psi_hessians(F, order=None, amips=False):
             dP[~inv] = 0
         H[:, :, q] = dP.reshape(T, 9)
     return H
+
+
+def tet_hessians(V, T, x, c2, c3, order, project=False, rest64=False):
+    """[T, 12, 12] per tet: K_t^T (c2 H_b + c3 H_a) K_t and its magnitude c2 |K_t^T H_b K_t| + c3 |K_t^T H_a K_t|
+    (corner-major, three coordinates per corner), on the kernels' inputs: F = E B with B = fp32 Dm^-1 (fp64 with
+    rest64) and corner vectors from B, E the exact edges of the fp32 x, or with project the fp32-rounded edges the
+    projection forms and each term's 9 x 9 Hessian projected to PSD.  An AMIPS tet's Hessian grows like I1 / J^2, so a
+    relative rounding of an edge moves it by far more than u A_ij on a near-flat tet: the kernels' own roundings of their
+    inputs are not what the checks built on this measure."""
+    T = np.asarray(T, np.int64).reshape(-1, 4)
+    B = rest_inverse(V, T)
+    if not rest64:
+        B = B.astype(np.float32).astype(np.float64)
+    x32 = np.asarray(x, np.float32).reshape(-1, 3)
+    if project:
+        E = np.stack([(x32[T[:, k]] - x32[T[:, 0]]).astype(np.float64) for k in (1, 2, 3)], 1)
+    else:
+        E = np.stack([x32[T[:, k]].astype(np.float64) - x32[T[:, 0]].astype(np.float64) for k in (1, 2, 3)], 1)
+    F = np.einsum("tkr,tkc->trc", E, B)
+    a = np.concatenate([-B.sum(axis=1, keepdims=True), B], axis=1)            # [T, 4, 3]
+    Km = np.zeros((len(T), 9, 12))
+    for k in range(4):
+        for r in range(3):
+            Km[:, 3 * r:3 * r + 3, 3 * k + r] = a[:, k]
+    H, A = np.zeros((len(T), 12, 12)), np.zeros((len(T), 12, 12))
+    for wgt, kind in ((c2, dict(order=order)), (c3, dict(amips=True))):
+        if not wgt:
+            continue
+        Hm = psi_hessians(F, **kind)
+        if project:
+            w, Q = np.linalg.eigh(0.5 * (Hm + Hm.transpose(0, 2, 1)))
+            Hm = np.einsum("tij,tj,tkj->tik", Q, np.maximum(w, 0), Q)
+        Kt = wgt * np.einsum("tma,tmn,tnb->tab", Km, Hm, Km, optimize=True)
+        H += Kt
+        A += np.abs(Kt)
+    return H, A
 
 
 def corner_blocks(orc, x, order=None, amips=False):
@@ -511,6 +548,17 @@ def test_cross_check_against_hvp(ext, det):
                 hv = hv.cpu().numpy().astype(np.float64)
                 err = np.abs(hv[S] - P[S, :, a]).max(axis=1)
                 assert (err <= 2 * KAPPA * U * A[S]).all(), (case, a, (err / (U * A[S])).max())
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("mesh,kw", plan_shape_cases())
+def test_hess_diag_plan_shapes(ext, mesh, kw):
+    """The diagonal blocks per row on the plans only these meshes produce (assert_plan_shape): the pole's row 0 sums its
+    988 weights in one ring-wrapping row block and its 1972 tets' blocks."""
+    V, T, *_ = _refs(mesh)
+    sp = _handle(ext, V, T, enable_amips=True, **kw)
+    check_handle_plan_shape(mesh, sp, kw, enable_amips=True)
+    _check_against_fp64(sp, mesh, str(kw))
 
 
 def _call(sp, x, terms, out, stream, gradH=1.0, gradH_dev=None):

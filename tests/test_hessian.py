@@ -14,7 +14,7 @@ import numpy as np
 import pytest
 
 from _helpers import CELL_FORMAT, PLAN_DEBUG_SO, build_host_plan, walk_streams
-from test_hess_diag import psi_hessians
+from test_hess_diag import psi_hessians, tet_hessians
 from test_newton_lm import C3, COEF, _cuda, _handle, _pack, _torch, ext  # noqa: F401
 from test_newton_psd import _psd_pack, _small_mixed
 from tssplat_b200.mesh import make_pack
@@ -230,32 +230,9 @@ def _bsr_hv(torch, hs, values, v):
 
 def kernel_input_dense(orc, pk, x, c1, c2, c3, order, project, nsph):
     """Per-sphere dense fp64 c1 M + sum_t K_t^T (c2 H_b + c3 H_a) K_t and the magnitude sums c1 |M| + sum_t |K_t^T H K_t|,
-    with the tet terms evaluated on the kernel's inputs: F = E B32 with B32 = fp32 Dm^-1 and corner vectors from B32, E the
-    exact edges (exact mode) or the fp32-rounded edges the projection forms (PSD).  An AMIPS tet's Hessian grows like
-    I1 / J^2, so a relative rounding of an edge moves it by far more than u A_ij on a near-flat tet: the kernels' own
-    roundings of their inputs are not what this test measures."""
-    from oracle.tet_energy_oracle import rest_inverse
+    with the tet terms of tet_hessians (on the kernels' inputs)."""
     T = np.asarray(pk.tets, np.int64)
-    B = rest_inverse(pk.verts, T).astype(np.float32).astype(np.float64)
-    x32 = np.asarray(x, np.float32)
-    if project:
-        E = np.stack([(x32[T[:, k]] - x32[T[:, 0]]).astype(np.float64) for k in (1, 2, 3)], 1)
-    else:
-        E = np.stack([x32[T[:, k]].astype(np.float64) - x32[T[:, 0]].astype(np.float64) for k in (1, 2, 3)], 1)
-    F = np.einsum("tkr,tkc->trc", E, B)
-    Hs = []
-    for H in ((psi_hessians(F, order=order), c2), (psi_hessians(F, amips=True) if c3 else np.zeros((len(T), 9, 9)), c3)):
-        Hm, wgt = H
-        if project:
-            w, Q = np.linalg.eigh(0.5 * (Hm + Hm.transpose(0, 2, 1)))
-            Hm = np.einsum("tij,tj,tkj->tik", Q, np.maximum(w, 0), Q)
-        Hs.append(wgt * Hm)
-    a = np.concatenate([-B.sum(axis=1, keepdims=True), B], axis=1)            # [T, 4, 3]
-    Km = np.zeros((len(T), 9, 12))
-    for k in range(4):
-        for r in range(3):
-            Km[:, 3 * r:3 * r + 3, 3 * k + r] = a[:, k]
-    Kb, Ka = (np.einsum("tma,tmn,tnb->tab", Km, H, Km) for H in Hs)
+    Ht, At = tet_hessians(pk.verts, T, x, c2, c3, order, project=project)
     M = orc.M.toarray()
     rowsum = np.abs(c1) * (np.abs(M).sum(axis=1) - np.abs(np.diag(M)))     # M_ii = -sum_j M_ij cancels: its error scales so
     refs, mags = [], []
@@ -265,8 +242,8 @@ def kernel_input_dense(orc, pk, x, c1, c2, c3, order, project, nsph):
         A = np.abs(H) + np.diag(rowsum[3 * v0:3 * v1])
         for t in np.nonzero((T[:, 0] >= v0) & (T[:, 0] < v1))[0]:
             idx = np.concatenate([3 * (T[t, k] - v0) + np.arange(3) for k in range(4)])
-            H[np.ix_(idx, idx)] += Kb[t] + Ka[t]
-            A[np.ix_(idx, idx)] += np.abs(Kb[t]) + np.abs(Ka[t])
+            H[np.ix_(idx, idx)] += Ht[t]
+            A[np.ix_(idx, idx)] += At[t]
         refs.append(H)
         mags.append(A)
     return refs, mags
@@ -513,3 +490,113 @@ def test_errors_memory_and_module(ext):
         cc1, cc2 = E.coeff_scheduler(it)
         ref = E.device_hessian.assemble(x, cc1, cc2, E.order_at(it), c3=C3)
         assert torch.equal(got, ref) and E.device_hessian.hessian == "psd" and E.device_hessian.pcg is E.device_pcg
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the plan-shape meshes: a sparse fp64 reference on the block pattern (a dense one would need 11 GB for mixed, 125 GB
+# for tiny2600)
+
+
+def sparse_reference(V, T, x, c1, c2, c3, order, project, pattern, rest64=False):
+    """fp64 blocks [nnzb, 3, 3] of c1 M_ij I plus the tet blocks of tet_hessians scattered to their (crow, col) blocks,
+    the magnitudes as kernel_input_dense forms them (|c1 M_ij| I, c1 sum_{j != i} |M_ij| on the diagonal, sum_t |K_t^T H
+    K_t|), and each block's number of fp32 addends n_ij: its active tets + 1 (c1 M_ij I)."""
+    from oracle.tet_energy_oracle import ReferenceEnergyOracle
+    T = np.asarray(T, np.int64).reshape(-1, 4)
+    crow, col, tblk = pattern["crow"], pattern["col"], pattern["tblk"].reshape(-1)
+    n, nnzb = len(crow) - 1, len(col)
+    rows = np.repeat(np.arange(n), np.diff(crow))
+    M1 = ReferenceEnergyOracle(V, T).M[0::3, 0::3].tocsr()
+    Mij = np.asarray(M1[rows, col]).ravel()
+    rowsum = np.abs(c1) * (np.asarray(abs(M1).sum(axis=1)).ravel() - np.abs(M1.diagonal()))
+    eye = np.eye(3)
+    ref = (c1 * Mij)[:, None, None] * eye
+    mag = (np.abs(c1 * Mij) + np.where(rows == col, rowsum[rows], 0.0))[:, None, None] * eye
+    Ht, At = tet_hessians(V, T, x, c2, c3, order, project=project, rest64=rest64)
+    blk = lambda H: H.reshape(-1, 4, 3, 4, 3).transpose(0, 1, 3, 2, 4).reshape(-1, 3, 3)      # [t, k, l] blocks
+    np.add.at(ref, tblk, blk(Ht))
+    np.add.at(mag, tblk, blk(At))
+    active = np.repeat(At.reshape(len(T), -1).max(axis=1) > 0, 16)
+    return ref, mag, np.bincount(tblk[active], minlength=nnzb) + 1
+
+
+def _bsr_mul(pattern, blocks, v):
+    crow, col = pattern["crow"], pattern["col"]
+    rows = np.repeat(np.arange(len(crow) - 1), np.diff(crow))
+    y = np.zeros((len(crow) - 1, 3))
+    np.add.at(y, rows, np.einsum("bij,bj->bi", blocks, np.asarray(v, np.float64).reshape(-1, 3)[col]))
+    return y
+
+
+@pytest.mark.parametrize("name", ["pole", "near_cap"])
+def test_sparse_reference_is_the_products(name):
+    """With fp64 rest inverses, sparse_reference times v is c1 M v + c2 H_b v + c3 H_a v of the fp64 matrix-form
+    products (test_hvp, test_hvp_amips) on every input of the suites: the scatter puts every tet block where it belongs."""
+    from test_hvp import hvp_terms
+    from test_hvp_amips import _mesh, amips_hvp_terms
+    V, T, orc, inputs, v = _mesh(name)
+    pattern = hess_pattern(V, T)
+    vv = v.astype(np.float64)
+    c1, c2, c3 = 2e-3, 0.8, 0.5
+    for case, (x, _) in inputs.items():
+        Hav, _ = amips_hvp_terms(orc, x.astype(np.float64), vv)
+        for order in (2, 4):
+            Mv, Hbv, _, _ = hvp_terms(orc, x.astype(np.float64), vv, order)
+            ref = (c1 * Mv + c2 * Hbv + c3 * Hav).reshape(-1, 3)
+            blocks, _, _ = sparse_reference(V, T, x, c1, c2, c3, order, False, pattern, rest64=True)
+            y = _bsr_mul(pattern, blocks, v)
+            assert np.linalg.norm(y - ref) <= 1e-12 * np.linalg.norm(ref), (case, order, np.linalg.norm(y - ref) / np.linalg.norm(ref))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("hessian", ["exact", "psd"])
+@pytest.mark.parametrize("mesh", ["pole", "near_cap", "tiny2600", "mixed"])
+def test_blocks_plan_shapes(ext, mesh, hessian):
+    """The assembled blocks of the plan-shape meshes against sparse_reference, block by block, within (KAPPA_BLOCK +
+    n_ij) u A_ij (KAPPA_PSD projected): the pole's row 0 has 989 blocks (31 passes of the row gather) and block (0, 0)
+    is a recursive fp32 sum of 1973 addends; near_cap's and the pole's last block-kernel CTA is partial; tiny2600 has 2600
+    spheres (also checked through hs.sphere on a sample) and mixed whole-area and twelve-tet spheres side by side."""
+    from _helpers import assert_plan_shape, cpu_plan
+    from test_hvp_amips import _mesh
+    V, T, _, inputs, _ = _mesh(mesh)
+    sp = _handle(ext, V, T, enable_amips=True)
+    assert_plan_shape(mesh, cpu_plan(sp, V, T, enable_amips=True), {})
+    hs = _dev_hessian(sp, hessian)
+    pattern = hess_pattern(V, T)
+    crow = hs.crow.cpu().numpy()
+    assert (crow == pattern["crow"]).all() and (hs.col.cpu().numpy() == pattern["col"]).all()
+    if mesh == "pole":
+        assert crow[1] - crow[0] == 989 and pattern["inc_ptr"][1] - pattern["inc_ptr"][0] == 1972
+    assert len(T) % 128 != 0                                        # the block kernel's last CTA (kHessT tets) is partial
+    mirror = _torch().from_numpy(_mirror_index(hs)).long().cuda() if mesh == "pole" else None
+    rows = np.repeat(np.arange(len(V)), np.diff(crow))
+    c1, c2 = COEF
+    kappa = KAPPA_PSD if hessian == "psd" else KAPPA_BLOCK
+    worst, worst_frac = 0.0, 0.0
+    for case, c3 in (("inverted_o2", 0.0), ("inverted_o2", C3), ("stretched_o2", C3)):
+        x_np = inputs[case][0]
+        x = _cuda(x_np)
+        for order in (2, 4):
+            vals = hs.assemble(x, c1, c2, order, c3=c3)
+            if mirror is not None:                               # row 0 in 31 passes, its mirrors from 988 short rows
+                assert _torch().equal(vals, vals[mirror].transpose(1, 2))
+            got = vals.double().cpu().numpy()
+            ref, mag, nadd = sparse_reference(V, T, x_np, c1, c2, c3, order, hessian == "psd", pattern)
+            r = np.abs(got - ref).max(axis=(1, 2)) / (U * np.maximum(np.abs(mag).max(axis=(1, 2)), 1e-300))
+            key = (mesh, hessian, case, order, c3)
+            assert (r <= kappa + nadd).all(), (key, r.max(), int(np.argmax(r / (kappa + nadd))))
+            worst, worst_frac = max(worst, r.max()), max(worst_frac, (r / (kappa + nadd)).max())
+            if mesh == "tiny2600":
+                for s in np.random.default_rng(order).choice(sp.info["n_components"], 12, replace=False):
+                    vs = hs.sphere_vertices(int(s))
+                    loc = np.full(len(V), -1)
+                    loc[vs] = np.arange(len(vs))
+                    inside = np.isin(rows, vs)
+                    dense = np.zeros((3 * len(vs), 3 * len(vs)))
+                    for b in np.nonzero(inside)[0]:
+                        i, j = loc[rows[b]], loc[pattern["col"][b]]
+                        dense[3 * i:3 * i + 3, 3 * j:3 * j + 3] = ref[b]
+                    gs = hs.sphere(vals, int(s)).toarray().astype(np.float64)
+                    bound = (kappa + nadd[inside].max()) * U * np.abs(mag[inside]).max()
+                    assert np.abs(gs - dense).max() <= bound, (key, int(s))
+    print(f"{mesh} {hessian}: worst |H - H64| / (u A_ij) = {worst:.3g}, of the bound (KAPPA + n_ij): {worst_frac:.3g}")

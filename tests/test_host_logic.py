@@ -8,8 +8,8 @@ import re
 import numpy as np
 import pytest
 
-from _helpers import (GOLDEN, RIGID_MOTIONS, ROOT, COracle, build_host_plan, emulate_kernel, min_abs_J, pole_mesh,
-                      rigid_motion, walk_streams)
+from _helpers import (GOLDEN, RIGID_MOTIONS, ROOT, COracle, assert_plan_shape, build_host_plan, emulate_kernel, min_abs_J,
+                      plan_shape_cases, plan_shape_mesh, pole_mesh, rigid_motion, row_blocks, walk_streams)
 from tssplat_b200 import _capi
 from tssplat_b200.mesh import (concat_spheres, connected_components, load_veg, make_pack, make_tet_sphere, perturb,
                                save_veg)
@@ -90,7 +90,7 @@ def test_high_valence_rows():
     x = perturb(v, t, 0.3, 2)
     for kw in (dict(nw=16, grid=132), dict(nw=8, grid=264), dict(nw=16, grid=132, force_global=1)):
         plan = build_host_plan(v, t, **kw)
-        hdr = _block_headers(plan)
+        hdr = row_blocks(plan)
         assert any(len4 == 62 and L == 4 for len4, L in hdr), "the pole row must be one 4-lane, 62-cell block"
         E, es, eb, g = emulate_kernel(plan, x, 1e-3, 2e-3, 2)
         Eo, terms, go = orc.energy_grad(x, 1e-3, 2e-3, 2)
@@ -98,11 +98,6 @@ def test_high_valence_rows():
         assert np.linalg.norm(g - go) <= 2e-6 * np.linalg.norm(go)
     with pytest.raises(RuntimeError, match="more than 988 operator neighbours"):
         build_host_plan(*pole_mesh(989))
-
-
-def _block_headers(plan):
-    """(len4, lanes per row) of every row block in the plan's streams."""
-    return [((int(h[0]) >> 24) & 63, 1 << (int(h[0]) >> 30)) for _, h in walk_streams(plan)[0]]
 
 
 def test_plan_operator_is_the_reference_matrix():
@@ -405,3 +400,14 @@ def test_plan_thousands_of_tiny_components():
     E, _, _, g = emulate_kernel(plan, x, 2e-4, 3e-4, 2)
     Eo, _, go = COracle(pk.verts, pk.tets).energy_grad(x, 2e-4, 3e-4, 2)
     assert E == pytest.approx(Eo, rel=2e-6) and np.linalg.norm(g - go) <= 2e-6 * np.linalg.norm(go)
+
+
+@pytest.mark.parametrize("mesh,kw", plan_shape_cases())
+def test_plan_shape_meshes_keep_their_shapes(mesh, kw):
+    """The plans an H100 builds for the plan-shape meshes (132 SMs: 132 CTAs of 16 warps or 264 of 8) have the shapes
+    the second-order suites run them for; a plan-builder change that loses one fails here before any GPU run."""
+    V, T = plan_shape_mesh(mesh)
+    nw = kw.get("warps_per_cta", 16)
+    plan = build_host_plan(V, T, nw=nw, grid=132 * 16 // nw, force_global=int(kw.get("force_global", False)),
+                           ring_slots=kw.get("ring_slots", 0), enable_amips=1, deterministic=int(kw.get("deterministic", False)))
+    assert_plan_shape(mesh, plan, kw)

@@ -11,13 +11,20 @@ from types import SimpleNamespace
 import numpy as np
 import pytest
 
-from _helpers import GOLDEN, min_abs_J, mirror_components
+from _helpers import (CELL_FORMAT, GOLDEN, PLAN_SHAPE_MESHES, build_host_plan, check_handle_plan_shape, min_abs_J,
+                      mirror_components, plan_shape_cases, plan_shape_mesh, walk_streams)
 from oracle.tet_energy_oracle import ReferenceEnergyOracle, _cof3, _det3
 from tssplat_b200.mesh import make_pack, perturb
 
 REL = 1e-5                  # kernel vs the fp64 oracle
 GH = 0.7                    # gradH of the GPU runs
 TERMS = [(1.0, 0.0), (0.0, 1.0), (2e-3, 0.8)]
+U = 2.0 ** -24              # fp32 unit roundoff
+# plan-shape meshes: per sphere |err_s| <= max(REL |ref_s|, KAPPA_SPHERE u |A_s|) (A: the row magnitudes |c1 M| |v| +
+# |c2 H_b| |v| + |c3 H_a| |v|), and on the pole's row 0 (988 streamed entries, 1972 tets) |err_0| <= KAPPA_ROW u A_0
+# per coordinate (test_pole_row_kappa: an fp32 re-enactment of the row stays within KAPPA_ROW / 4)
+KAPPA_SPHERE = 64
+KAPPA_ROW = 16
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -154,6 +161,61 @@ def test_oracle_known_answers(small):
     assert np.abs(hv).max() <= 1e-12 * scale
 
 
+def _pole_row_fp32(v, c1, tet_rows, seed):
+    """Row 0 of c1 M v + the tet products on the pole, re-enacted in fp32: the smoothness row pass over the GLOBAL plan's
+    row block in lane order (each lane a sequence of fp32 fused multiply-adds w (v_j - v_0), then the pairwise lane
+    reduction), plus the tets' fp64 contributions rounded to fp32 and added in a random order (the atomics' order)."""
+    V, T = plan_shape_mesh("pole")
+    plan = build_host_plan(V, T, force_global=1)
+    CELL, IB, _ = CELL_FORMAT[True]
+    st, f32 = plan["stream"], np.float32
+    v32 = np.asarray(v, f32)
+    blocks = [(p, hdr) for p, hdr in walk_streams(plan)[0] if (hdr & 0xFFFFFF == 0).any()]
+    assert len(blocks) == 1
+    p, hdr = blocks[0]
+    len4, L = int((hdr[0] >> 24) & 63), 1 << int(hdr[0] >> 30)
+    lanes = np.arange(L) + np.flatnonzero((hdr & 0xFFFFFF) == 0)[0]
+    acc = np.zeros((L, 3), f32)
+    for q in range(len4):
+        j = st[p + q * CELL:p + q * CELL + 128 * IB].view(np.uint32).reshape(32, 4)[lanes].astype(np.int64)
+        w = st[p + q * CELL + 128 * IB:p + q * CELL + 128 * IB + 512].view(f32).reshape(32, 4)[lanes]
+        for c in range(4):
+            d = (v32[j[:, c]] - v32[0]).astype(f32)
+            acc = (w[:, c, None].astype(np.float64) * d + acc).astype(f32)
+    while len(acc) > 1:
+        acc = (acc[:len(acc) // 2] + acc[len(acc) // 2:]).astype(f32)
+    out = (f32(c1) * acc[0]).astype(f32)
+    for t in np.random.default_rng(seed).permutation(len(tet_rows)):
+        out = (out + tet_rows[t].astype(f32)).astype(f32)
+    return out.astype(np.float64)
+
+
+def test_pole_row_kappa():
+    """KAPPA_ROW holds with a factor 4 to spare for the fp32 re-enactment of the pole's row 0 (_pole_row_fp32) on every
+    input and term combination of the GPU checks, with and without AMIPS."""
+    from test_hess_diag import tet_hessians
+    from test_hvp_amips import _mesh as amips_mesh
+    V, T, orc, inputs, v = amips_mesh("pole")
+    T64 = np.asarray(T, np.int64)
+    vv = v.astype(np.float64)
+    assert (T64[:, 0] == 0).all()                              # every tet has the pole as corner 0
+    worst = 0.0
+    for case, (x, order) in inputs.items():
+        sc = row_scales("pole", case, x, order)
+        for c1, c2, c3 in ((1.0, 0.0, 0.0), (0.0, 1.0, 0.0), (2e-3, 0.8, 0.0), (0.0, 0.0, 1.0), (2e-3, 0.8, 0.5)):
+            Ht, _ = tet_hessians(V, T64, x, c2, c3, order)
+            tet_rows = np.einsum("tab,tb->ta", Ht[:, :3], vv[T64].reshape(-1, 12))
+            Mv = (orc.M @ vv.reshape(-1)).reshape(-1, 3)
+            ref = c1 * Mv[0] + tet_rows.sum(axis=0)
+            A = c1 * sc[0][0] + c2 * sc[1][0] + c3 * sc[2][0]
+            for seed in range(3):
+                err = np.abs(_pole_row_fp32(v, c1, tet_rows, seed) - ref)
+                assert (err[A == 0] == 0).all()                # e.g. the barrier alone with no inverted tet
+                worst = max(worst, (err[A > 0] / (U * A[A > 0])).max(initial=0.0))
+    print(f"pole row 0, fp32 re-enactment: max |err_0| / (u A_0) = {worst:.3g} (KAPPA_ROW {KAPPA_ROW})")
+    assert worst <= KAPPA_ROW / 4
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # GPU
 
@@ -210,6 +272,16 @@ def _mesh(name):
             xi = V.copy()
             xi[ids] = _inverted(pk, seed=2)
             inputs = {"benign_o2": (xb, 2), "inverted_o2": (xi, 2), "inverted_o4": (xi, 4)}
+        elif name in PLAN_SHAPE_MESHES:
+            V, T = plan_shape_mesh(name)
+            T64 = T.astype(np.int64)
+            P = V[T64].astype(np.float64)              # h: the tets' shortest edge (the pole's are 1 long, 0.1 wide)
+            h = np.min([np.linalg.norm(P[:, a] - P[:, b], axis=1) for a in range(4) for b in range(a)], axis=0).mean()
+            used = np.unique(T64)
+            xb = V.copy()
+            xb[used] += np.random.default_rng(6).normal(scale=0.02 * h, size=(len(used), 3)).astype(np.float32)
+            xi = mirror_components(xb, T)
+            inputs = {"benign_o2": (xb, 2), "inverted_o2": (xi, 2), "inverted_o4": (xi, 4)}
         else:
             raise KeyError(name)
         for key, (x, order) in inputs.items():
@@ -219,6 +291,60 @@ def _mesh(name):
         v = np.random.default_rng(9).normal(size=(len(V), 3)).astype(np.float32)
         _MESHES[name] = (V, T, orc, inputs, v)
     return _MESHES[name]
+
+
+_SCALES = {}
+
+
+def row_scales(mesh, case, x, order):
+    """[3, n, 3]: |M| |v|, sum_t |H_b,t| |v| and sum_t |H_a,t| |v| at input `case` (x, order) of a plan-shape mesh, the
+    terms of the row magnitude A of the per-sphere and pole-row bounds."""
+    if (mesh, case) not in _SCALES:
+        from test_hess_diag import tet_hessians
+        V, T, orc, _, v = _mesh(mesh)
+        av = np.abs(v.astype(np.float64))
+        out = [(abs(orc.M) @ av.reshape(-1)).reshape(-1, 3)]
+        for c2, c3 in ((1.0, 0.0), (0.0, 1.0)):
+            At = tet_hessians(V, T, x, c2, c3, order)[1]
+            y = np.einsum("tab,tb->ta", At, av[T].reshape(-1, 12)).reshape(-1, 4, 3)
+            s = np.zeros_like(av)
+            np.add.at(s, np.asarray(T, np.int64), y)
+            out.append(s)
+        _SCALES[(mesh, case)] = np.stack(out)
+    return _SCALES[(mesh, case)]
+
+
+def check_spheres_and_pole_row(mesh, key, err, parts, A):
+    """Per sphere |err_s| <= max(sum_k rel_k |part_k,s|, KAPPA_SPHERE u |A_s|) for parts = [(rel_k, part_k [n, 3])] (the
+    suite's own whole-mesh bound, taken per sphere), and on the pole |err_0| <= KAPPA_ROW u A_0.  Returns the worst ratio
+    of each."""
+    from tssplat_b200.mesh import connected_components
+    V, T, *_ = _mesh(mesh)
+    lab = connected_components(len(V), np.asarray(T).reshape(-1, 4))
+    nrm = lambda a: np.sqrt(np.bincount(lab, weights=(a * a).sum(axis=1)))
+    bound = np.maximum(sum(rel * nrm(p) for rel, p in parts), KAPPA_SPHERE * U * nrm(A))
+    e = nrm(err)
+    assert (e <= bound).all(), (key, int(np.argmax(e / bound)), (e / bound).max())
+    worst = {"sphere": (e / np.maximum(bound, 1e-300)).max()}
+    if mesh == "pole":
+        a0, e0 = A[0], np.abs(err[0])
+        assert (e0[a0 == 0] == 0).all(), (key, e0)          # e.g. the barrier alone with no inverted tet
+        r = e0[a0 > 0] / (U * a0[a0 > 0])
+        assert (r <= KAPPA_ROW).all(), (key, r)
+        worst["row 0"] = r.max(initial=0.0)
+    return worst
+
+
+WORST = {}
+
+
+@pytest.fixture(scope="module", autouse=True)
+def _report():
+    yield
+    if WORST:
+        print("\nhvp on the plan-shape meshes: worst |err_s| / bound per sphere, |err_0| / (u A_0) on the pole row:")
+        for k, v in sorted(WORST.items()):
+            print(f"  {k}: {v:.3g}")
 
 
 def _hvp(sp, x, v, c1, c2, order, gradH=GH):
@@ -244,6 +370,11 @@ def _check_against_oracle(sp, mesh, key_prefix, orphans=None):
                 assert _rel(hv, ref) <= REL, (key, _rel(hv, ref))
             if orphans is not None:
                 assert not hv[orphans].any(), key
+            if mesh in PLAN_SHAPE_MESHES:
+                sc = row_scales(mesh, case, x, order)
+                parts = [(REL, ref)]
+                for name, w in check_spheres_and_pole_row(mesh, key, hv - ref, parts, GH * (c1 * sc[0] + c2 * sc[1])).items():
+                    WORST[(mesh, name)] = max(WORST.get((mesh, name), 0.0), w)
             scale = c1 * abs(vMv) + c2 * np.abs(q).sum()
             assert abs(curv[0] - (c1 * vMv + c2 * q.sum())) <= REL * scale, (key, curv, vMv, q.sum())
             assert abs(curv[1] - vMv) <= REL * abs(vMv), (key, curv[1], vMv)
@@ -283,6 +414,17 @@ def test_hvp_shuffled_ids_with_orphans(ext, kw):
     orphans[np.unique(T)] = False
     assert orphans.sum() == 500
     _check_against_oracle(sp, "shuffled", str(kw), orphans=orphans)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("mesh,kw", plan_shape_cases())
+def test_hvp_plan_shapes(ext, mesh, kw):
+    """The products on the plans only these meshes produce (assert_plan_shape): the pole's ring-wrapping row block, whole-
+    area staging, GLOBAL by size, segment headers past the shared-memory table."""
+    V, T, *_ = _mesh(mesh)
+    sp = _handle(ext, V, T, **kw)
+    check_handle_plan_shape(mesh, sp, kw)
+    _check_against_oracle(sp, mesh, str(kw))
 
 
 def _inverted_touched(T, x):

@@ -12,9 +12,9 @@ from types import SimpleNamespace
 import numpy as np
 import pytest
 
-from _helpers import min_abs_J, mirror_components
+from _helpers import PLAN_SHAPE_MESHES, check_handle_plan_shape, min_abs_J, mirror_components, plan_shape_cases
 from oracle.tet_energy_oracle import ReferenceEnergyOracle, _cof3, _det3, rest_inverse
-from test_hvp import _cof_pair, _mesh as _hvp_mesh, hvp_terms
+from test_hvp import _cof_pair, _mesh as _hvp_mesh, check_spheres_and_pole_row, hvp_terms, row_scales
 from tssplat_b200.mesh import make_pack, perturb
 
 REL = 1e-5                  # smoothness and barrier terms, as tests/test_hvp.py
@@ -286,6 +286,12 @@ def _check_against_fp64(sp, mesh, key_prefix, orphans=None):
             assert np.linalg.norm(hv - ref) <= bound, (key, np.linalg.norm(hv - ref) / bound)
             if orphans is not None:
                 assert not hv[orphans].any(), key
+            if mesh in PLAN_SHAPE_MESHES:
+                sc = row_scales(mesh, case, x, order)
+                prts = [(GH * REL, parts[0].reshape(-1, 3)), (GH * REL, parts[1].reshape(-1, 3)), (GH * REL_A, parts[2].reshape(-1, 3))]
+                A = GH * (c1 * sc[0] + c2 * sc[1] + c3 * sc[2])
+                for name, w in check_spheres_and_pole_row(mesh, key, hv - ref, prts, A).items():
+                    WORST[(mesh, name)] = max(WORST.get((mesh, name), 0.0), w)
             total = c1 * vMv + c2 * q.sum() + c3 * qa.sum()
             scale = REL * (c1 * abs(vMv) + c2 * np.abs(q).sum()) + REL_A * c3 * np.abs(qa).sum()
             assert abs(curv[0] - total) <= scale, (key, curv, total)
@@ -326,6 +332,28 @@ def test_amips_hvp_shuffled_ids_with_orphans(ext, kw):
     orphans[np.unique(T)] = False
     assert orphans.sum() == 500
     _check_against_fp64(sp, "shuffled", str(kw), orphans=orphans)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("mesh,kw", plan_shape_cases())
+def test_amips_hvp_plan_shapes(ext, mesh, kw):
+    """The AMIPS products on the plans only these meshes produce (assert_plan_shape)."""
+    V, T, *_ = _mesh(mesh)
+    sp = _handle(ext, V, T, enable_amips=True, **kw)
+    check_handle_plan_shape(mesh, sp, kw, enable_amips=True)
+    _check_against_fp64(sp, mesh, str(kw))
+
+
+WORST = {}
+
+
+@pytest.fixture(scope="module", autouse=True)
+def _report():
+    yield
+    if WORST:
+        print("\nAMIPS hvp on the plan-shape meshes: worst |err_s| / bound per sphere, |err_0| / (u A_0) on the pole row:")
+        for k, v in sorted(WORST.items()):
+            print(f"  {k}: {v:.3g}")
 
 
 def _lib():

@@ -13,7 +13,7 @@ import pytest
 import scipy.sparse as sps
 from scipy.sparse.csgraph import connected_components
 
-from _helpers import min_abs_J
+from _helpers import PLAN_SHAPE_MESHES, min_abs_J
 from oracle.tet_energy_oracle import ReferenceEnergyOracle, _cof3, _det3
 from tssplat_b200.mesh import make_pack, perturb
 
@@ -374,7 +374,8 @@ _MESHES = {}
 
 
 def _mesh(name):
-    """(V, T, oracle, {case: x}, d) with a benign (sigma 0.02 h) and an inverted (sigma 0.35 h) input."""
+    """(V, T, oracle, {case: x}, d) with a benign (sigma 0.02 h) and an inverted (sigma 0.35 h) input; the plan-shape
+    meshes take test_hvp_amips's benign, mirrored and stretched inputs instead."""
     if name not in _MESHES:
         from test_hvp import _mesh as hvp_mesh
         V, T, _, _, _ = hvp_mesh(name)
@@ -384,10 +385,14 @@ def _mesh(name):
         rng = np.random.default_rng(21)
         used = np.unique(T64)
         xs = {}
+        if name in PLAN_SHAPE_MESHES:         # the inputs of the products' suites: benign, mirrored, stretched
+            from test_hvp_amips import _mesh as amips_mesh
+            ins = amips_mesh(name)[3]
+            xs = {"benign": ins["benign_o2"][0], "inverted": ins["inverted_o2"][0], "stretched": ins["stretched_o2"][0]}
         for case, s in (("benign", 0.02), ("inverted", 0.35)):
             x = V.copy()
             x[used] += rng.normal(scale=s * h, size=(len(used), 3)).astype(np.float32)
-            xs[case] = x
+            xs.setdefault(case, x)
         assert min_abs_J(V, T, xs["benign"]) > 1e-3
         d = np.zeros_like(V)
         d[used] = rng.normal(scale=0.1 * h, size=(len(used), 3)).astype(np.float32)

@@ -21,7 +21,7 @@ import numpy as np
 import pytest
 import scipy.sparse as sps
 
-from _helpers import rigid_motion
+from _helpers import check_handle_plan_shape, plan_shape_cases, rigid_motion
 from test_line_search import REL, components, line_terms, make_oracle
 from test_psd_edges import single_tet_mesh
 from tssplat_b200.mesh import make_pack, perturb
@@ -746,7 +746,10 @@ def gpu_mesh(name):
             from test_line_search import _mesh
             V, T, _, xs, d = _mesh(name)
             g = Geo(V, T)
-            _GPU[name] = (g, inputs(g, xs["benign"], xs["inverted"], d, 40), None)
+            ins = inputs(g, xs["benign"], xs["inverted"], d, 40)
+            if "stretched" in xs:
+                ins["stretched"] = (np.ascontiguousarray(xs["stretched"], f32), d)
+            _GPU[name] = (g, ins, None)
     return _GPU[name]
 
 
@@ -849,6 +852,15 @@ def test_shuffled_ids_with_orphans(ext):
     g = gpu_mesh("shuffled")[0]
     assert (~g.used).sum() == 500
     run_mesh(ext, "shuffled", dict())
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("mesh,kw", plan_shape_cases(deterministic=False))
+def test_line_search_plan_shapes(ext, mesh, kw):
+    """The changes on the plans only these meshes produce (assert_plan_shape): the staged direction of whole-area
+    segments, the direction prefetched past the segment table, the pole's ring-wrapping row block."""
+    sp = run_mesh(ext, mesh, kw)
+    check_handle_plan_shape(mesh, sp, kw, enable_amips=True)
 
 
 @pytest.mark.gpu
