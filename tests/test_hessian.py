@@ -14,9 +14,8 @@ import numpy as np
 import pytest
 
 from _helpers import CELL_FORMAT, PLAN_DEBUG_SO, build_host_plan, walk_streams
+from _newton_model import C3, COEF, _cuda, _handle, _pack, _psd_pack, _small_mixed, _torch, ext  # noqa: F401
 from test_hess_diag import psi_hessians, tet_hessians
-from test_newton_lm import C3, COEF, _cuda, _handle, _pack, _torch, ext  # noqa: F401
-from test_newton_psd import _psd_pack, _small_mixed
 from tssplat_b200.mesh import make_pack
 
 U = 2.0 ** -24

@@ -6,15 +6,20 @@ rule in the rotated frame) against numpy.linalg.eigh of the 9 x 9 F-space Hessia
 of test_hess_diag, on random, rotated, degenerate, near-rest and inverted F; known answers; the dense per-sphere projected
 Hessian of the small mixed pack is PSD where the exact one is not.  GPU: tsb_pcg_hvp_psd against the fp64 projected
 oracle on handle variants; agreement with tsb_hvp_ex where every active tet is already PSD; per-sphere curvature;
-bitwise repeatability and independence; the PSD solve and Newton steps; argument errors and memory; the module route."""
+bitwise repeatability and independence; the PSD solve and Newton steps, and the steps within the fp64 projected
+reference's count; argument errors and memory; the module route.  The projected reference itself and the steps against
+their composition run through the shared checks of _newton_checks."""
 import ctypes as C
 
 import numpy as np
 import pytest
 
-from test_hess_diag import corner_G, psi_hessians
-from test_newton_lm import C3, COEF, OPTS, _cuda, _handle, _pack, _torch, ext  # noqa: F401
-from tssplat_b200.mesh import make_pack, perturb
+from _newton_checks import check_composition, check_reference
+from _newton_model import (C3, COEF, GPU_SLACK, PSD_MUST, PSD_REF_STEPS, _cases, _cuda, _handle, _pack, _psd_pack,  # noqa: F401
+                           _records, _rot, _small_mixed, _torch, dense_sphere_hessians, ext, reference_problem,
+                           reference_run, tet_hessians)
+from test_hess_diag import psi_hessians
+from tssplat_b200.mesh import make_pack
 
 REL = 1e-4          # GPU projected product against the fp64 oracle, relative L2 per sphere
 
@@ -95,30 +100,6 @@ def eigh_projection(H):
     return (Q * np.maximum(w, 0)) @ Q.T, w
 
 
-def _rot(rng):
-    Q, R = np.linalg.qr(rng.standard_normal((3, 3)))
-    Q = Q * np.sign(np.diag(R))
-    return Q if np.linalg.det(Q) > 0 else -Q
-
-
-def _cases(rng):
-    """(name, F): random, rotations and identity, two equal s, near rest, s_3 -> 0-, s_3 ~ -s_2, reflections."""
-    out = []
-    for k in range(4):
-        F = rng.standard_normal((3, 3))
-        out.append((f"random{k}", F))
-    R = _rot(rng)
-    out += [("identity", np.eye(3)), ("rotation", R), ("scaled rotation", 1.7 * R),
-            ("two equal", _rot(rng) @ np.diag([1.3, 0.8, 0.8]) @ _rot(rng).T),
-            ("near rest", np.eye(3) + 1e-4 * rng.standard_normal((3, 3))),
-            ("near rest rotated", R @ (np.eye(3) + 1e-4 * rng.standard_normal((3, 3))))]
-    refl = np.diag([1.0, 1.0, -1.0])
-    out += [("s3 -> 0-", _rot(rng) @ np.diag([1.2, 0.9, -1e-6]) @ _rot(rng).T),
-            ("s3 ~ -s2", _rot(rng) @ np.diag([1.1, 0.7, -0.7 + 1e-9]) @ _rot(rng).T),
-            ("reflection", R @ refl), ("reflected stretch", _rot(rng) @ np.diag([1.4, 0.75, -1.0]) @ _rot(rng).T)]
-    return out
-
-
 @pytest.mark.parametrize("term", ["barrier2", "barrier4", "amips"])
 def test_closed_form_against_eigh(term):
     rng = np.random.default_rng(7)
@@ -162,47 +143,6 @@ def test_known_answers():
             assert np.isclose(abs(ls[P]), abs(d1 * s[k])) and ((ls[P] > 0) != (la[P] > 0))
 
 
-def _small_mixed():
-    """test_newton_prox's small mixed pack: 3 x 256, sphere 0 at 0.35 h (with inverted tets)."""
-    pk = make_pack(3, 256, seed=4)
-    x = perturb(pk, sigma_rel=0.02, seed=1).astype(np.float64)
-    rough = perturb(pk, sigma_rel=0.35, seed=3)
-    x[pk.vert_offsets[0]:pk.vert_offsets[1]] = rough[pk.vert_offsets[0]:pk.vert_offsets[1]]
-    return pk, x.astype(np.float32).astype(np.float64)
-
-
-def tet_hessians(orc, x, order, c3, project):
-    """[T, 9, 9] weighted F-space Hessians c2-free: barrier on J < 0 tets, c3 AMIPS on J > 0 ones (projected or not)."""
-    F = (orc.G @ np.asarray(x, np.float64).reshape(-1)).reshape(-1, 3, 3)
-    Hb = psi_hessians(F, order=order)
-    Ha = psi_hessians(F, amips=True) if c3 else np.zeros_like(Hb)
-    if project:
-        w, Q = np.linalg.eigh(0.5 * (Hb + Hb.transpose(0, 2, 1)))
-        Hb = np.einsum("tij,tj,tkj->tik", Q, np.maximum(w, 0), Q)
-        if c3:
-            w, Q = np.linalg.eigh(0.5 * (Ha + Ha.transpose(0, 2, 1)))
-            Ha = np.einsum("tij,tj,tkj->tik", Q, np.maximum(w, 0), Q)
-    return Hb, Ha
-
-
-def dense_sphere_hessians(orc, pk, x, c1, c2, c3, order, project):
-    """Dense per-sphere c1 M + c2 sum K^T H_b K + c3 sum K^T H_a K (exact or projected tet blocks)."""
-    Hb, Ha = tet_hessians(orc, x, order, c3, project)
-    Ht = c2 * Hb + c3 * Ha
-    Gk = corner_G(orc).transpose(0, 2, 1, 3).reshape(orc.nele, 9, 12)          # [T, 9, 4 corners x 3]
-    K = np.einsum("tma,tmn,tnb->tab", Gk, Ht, Gk)
-    M = orc.M.toarray()
-    out = []
-    for s in range(pk.num_spheres):
-        v0, v1 = pk.vert_offsets[s], pk.vert_offsets[s + 1]
-        H = c1 * M[3 * v0:3 * v1, 3 * v0:3 * v1]
-        for t in np.nonzero((orc.tets[:, 0] >= v0) & (orc.tets[:, 0] < v1))[0]:
-            idx = np.concatenate([3 * (orc.tets[t, k] - v0) + np.arange(3) for k in range(4)])
-            H[np.ix_(idx, idx)] += K[t]
-        out.append(H)
-    return out
-
-
 @pytest.mark.parametrize("amips", [False, True], ids=["amips-off", "amips-on"])
 def test_dense_projected_hessian_is_psd_on_the_small_mixed_pack(amips):
     from oracle.tet_energy_oracle import ReferenceEnergyOracle
@@ -233,18 +173,6 @@ def projected_hvp_oracle(orc, x, v, c1, c2, c3, order):
     hv = c1 * Mv + orc.G.T @ (c2 * yb + c3 * ya).reshape(-1)
     mag = np.abs(c1) * np.abs(orc.M) @ np.abs(v) + np.abs(orc.G.T) @ np.abs(c2 * yb + c3 * ya).reshape(-1)
     return hv, mag, (float(v @ Mv), float((dF * yb).sum()), float((dF * ya).sum()))
-
-
-def _psd_pack(name):
-    """(pack, x): "mixed8" = 8 x 1024 with spheres 0 and 4 at 0.35 h; "mixed64" = test_newton_lm's mixed 64 x 4096."""
-    if name == "mixed64":
-        return _pack("mixed")
-    pk = make_pack(8, 1024, seed=2)
-    x = perturb(pk, sigma_rel=0.02, seed=1)
-    rough = perturb(pk, sigma_rel=0.35, seed=3)
-    for s in (0, 4):
-        x[pk.vert_offsets[s]:pk.vert_offsets[s + 1]] = rough[pk.vert_offsets[s]:pk.vert_offsets[s + 1]]
-    return pk, x
 
 
 def _sphere_rel(pk, got, ref, mag, spheres):
@@ -420,11 +348,6 @@ def test_psd_solve_never_stops_at_negative_curvature(ext, amips):
     assert (out["psd"].d_H_d >= 0).all()
 
 
-def _newton_run(torch, nw, x, n, c1, c2, c3, **o):
-    recs = [nw.step(x, c1, c2, 2, c3=c3, **o) for _ in range(n)]
-    return torch.cat([torch.cat([f.reshape(-1).contiguous().view(torch.int32) for f in r]) for r in recs])
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("amips", [False, True], ids=["amips-off", "amips-on"])
 def test_psd_newton_steps(ext, amips):
@@ -461,9 +384,9 @@ def test_psd_newton_steps(ext, amips):
     # bitwise: two runs and a graph of 5 steps
     xa, xb, xg = _cuda(x_np), _cuda(x_np), _cuda(x_np)
     nw.reset()
-    ra = _newton_run(torch, nw, xa, 5, c1, c2, c3, max_iter=10)
+    ra = _records(torch, [nw.step(xa, c1, c2, 2, c3=c3, max_iter=10) for _ in range(5)])
     nw.reset()
-    rb = _newton_run(torch, nw, xb, 5, c1, c2, c3, max_iter=10)
+    rb = _records(torch, [nw.step(xb, c1, c2, 2, c3=c3, max_iter=10) for _ in range(5)])
     assert torch.equal(xa, xb) and torch.equal(ra, rb)
     s = torch.cuda.Stream()
     torch.cuda.synchronize()
@@ -473,7 +396,7 @@ def test_psd_newton_steps(ext, amips):
     graph = torch.cuda.CUDAGraph()
     with torch.cuda.graph(graph):
         nw.reset()
-        rg = _newton_run(torch, nw, xg, 5, c1, c2, c3, max_iter=10)
+        rg = _records(torch, [nw.step(xg, c1, c2, 2, c3=c3, max_iter=10) for _ in range(5)])
     for _ in range(2):
         xg.copy_(_cuda(x_np))
         graph.replay()
@@ -578,190 +501,18 @@ def test_module_route(ext):
     assert (r.delta <= 0).all()
 
 
-# ---------------------------------------------------------------------------------------------------------------------
-# fp64 projected LM reference (CPU) and the Newton steps it pins (GPU)
-
-# steps the fp64 projected reference needs on the small mixed pack until the spheres it must converge are CONVERGED: with
-# w = 0 ("plain") every sphere, the rough one included (the exact reference needs 12, test_newton_lm.REF_STEPS); with
-# test_newton_prox's small weight the two quiet spheres.  There the rough sphere takes the full step every time and Phi
-# falls at every step, but the projected model drops the negative curvature of its remaining inverted tets, so the
-# iteration is only linearly convergent and does not reach gtol within 20 steps (the exact reference needs 12).  The GPU
-# runs on the same pack may take GPU_SLACK more.
-PSD_REF_STEPS = {"plain": 7, "small": 2}
-PSD_MUST = {"plain": (0, 1, 2), "small": (1, 2)}
-
-
-def psd_lm_reference(P, x0, y, w, n_steps, o):
-    """prox_lm_reference of test_newton_prox with the solve's H replaced by the projected H+ (dense, per sphere); the
-    preconditioner keeps the exact diagonal blocks, as tsb_newton_step does in PSD mode.  w = 0 is tsb_newton_step (the
-    proximal rule with w = 0 is the plain one)."""
-    from test_newton_lm import new_state
-    from test_newton_prox import ACTIVE, ALPHAS, decide_prox, init_mu_prox, weight_ok
-    from test_pcg_device import batched_pcg_reference, jacobi_inverse_blocks
-    x = np.asarray(x0, np.float64).reshape(-1).copy()
-    y = np.asarray(y, np.float64).reshape(-1)
-    st = new_state(P.S)
-    sl = [slice(3 * P.vo[s], 3 * P.vo[s + 1]) for s in range(P.S)]
-    hist = []
-    for _ in range(n_steps):
-        b = -P.grad(x)
-        for s in range(P.S):
-            if st[s]["status"] != ACTIVE or not weight_ok(w[s]):
-                b[sl[s]] = 0.0
-            elif w[s]:
-                b[sl[s]] -= w[s] * (x[sl[s]] - y[sl[s]])
-        He = dense_sphere_hessians(P.orc, P.pk, x, P.c1, P.c2, P.c3, P.order, False)
-        Hp = dense_sphere_hessians(P.orc, P.pk, x, P.c1, P.c2, P.c3, P.order, True)
-        D = [np.stack([Hc[3 * i:3 * i + 3, 3 * i:3 * i + 3] for i in range(len(Hc) // 3)]) for Hc in He]
-        shift = init_mu_prox(st, [Dc[:, [0, 1, 2], [0, 1, 2]].max() for Dc in D], w, o)
-        Pc = []
-        for Dc, m in zip(D, shift):
-            inv = jacobi_inverse_blocks(Dc + float(m) * np.eye(3), o["rel_floor"])
-            B = np.zeros((3 * len(Dc), 3 * len(Dc)))
-            for i, q in enumerate(inv):
-                B[3 * i:3 * i + 3, 3 * i:3 * i + 3] = [[q[0], q[5], q[4]], [q[5], q[1], q[3]], [q[4], q[3], q[2]]]
-            Pc.append(B)
-        bs = [b[sl[s]] for s in range(P.S)]
-        sol = batched_pcg_reference([Hc + float(m) * np.eye(len(Hc)) for Hc, m in zip(Hp, shift)], bs, Pc, o["max_iter"], o["rtol"])
-        d = np.concatenate([r["d"] for r in sol])
-        E0, inv0 = P.sphere_energy(x)
-        dE = np.stack([P.sphere_energy(x + a * d)[0] - E0 for a in ALPHAS[:o["n_alpha"]]], axis=1)
-        ahat = P.inversion_bound(x, d)
-        step = []
-        for s, r in enumerate(sol):
-            ds = r["d"]
-            out = decide_prox(st[s], float(np.linalg.norm(bs[s])), r["b_dot_d"], r["d_H_d"], shift[s], float(ds @ ds), dE[s],
-                              ahat[s], o, w[s], float(ds @ (x[sl[s]] - y[sl[s]])))
-            step.append(dict(zip(("alpha", "k", "delta", "rho"), out), status=st[s]["status"], inv0=inv0[s], pcg=r["status"],
-                             phi0=E0[s] + 0.5 * w[s] * float((x[sl[s]] - y[sl[s]]) @ (x[sl[s]] - y[sl[s]]))))
-        for s in range(P.S):
-            x[sl[s]] += step[s]["alpha"] * sol[s]["d"]
-        hist.append(step)
-    return x, hist
-
-
-_PSD_REF = {}
-
-
-def _psd_ref(kind):
-    """The reference pack of test_newton_prox (_prox_ref: 3 x 256, sphere 0 at 0.35 h, AMIPS off, started at x = y, gtol
-    1e-3 times the smallest starting |g_c|), w = 0 ("plain") or the small weight ("small")."""
-    if kind not in _PSD_REF:
-        from test_newton_prox import _prox_ref
-        P, x, w, o, _ = _prox_ref("small")
-        w = np.zeros_like(w) if kind == "plain" else w
-        _PSD_REF[kind] = (P, x, w, o, psd_lm_reference(P, x, x, w, 20, o))
-    return _PSD_REF[kind]
-
-
-def _converged_at(hist, S):
-    from test_newton_prox import N_CONVERGED
-    return [next((t for t, step in enumerate(hist) if step[s]["status"] == N_CONVERGED), None) for s in range(S)]
-
-
-@pytest.mark.parametrize("kind", ["plain", "small"])
-def test_psd_reference_mixed_pack(kind):
-    """The projected reference: Phi never increases and its change is the record's; no solve ends at negative
-    curvature; the spheres of PSD_MUST CONVERGED within PSD_REF_STEPS (with w = 0 all three); with the small weight the
-    rough sphere's Phi falls at every step, and the converged spheres' fixed point is the exact mode's (test_newton_prox's
-    fp64 reference) and scipy's trust-region Newton-CG's on Phi, within the stationarity bound
-    (|grad Phi_c(x)| + |grad Phi_c(x*)|) / w_c."""
-    from scipy.optimize import minimize
-    from test_hvp import hvp
-    from test_newton_prox import _phi, _prox_ref
-    P, y, w, o, (x, hist) = _psd_ref(kind)
-    for t, step in enumerate(hist):
-        nxt = hist[t + 1] if t + 1 < len(hist) else None
-        for s, r in enumerate(step):
-            after = nxt[s]["phi0"] if nxt else _phi(P, x, y.reshape(-1), w)[s]
-            assert after <= r["phi0"] + 1e-12 * abs(r["phi0"]), (t, s)
-            assert abs((after - r["phi0"]) - r["delta"]) <= 1e-9 * abs(r["phi0"]), (t, s)
-            assert r["pcg"] not in (2, 3), (t, s, r["pcg"])
-    conv = _converged_at(hist, P.S)
-    print(f"{kind}: converged at steps {conv}, k {[[h['k'] for h in step] for step in hist]}")
-    must = PSD_MUST[kind]
-    assert all(conv[s] is not None and conv[s] <= PSD_REF_STEPS[kind] for s in must), conv
-    for s in set(range(P.S)) - set(must):
-        assert all(step[s]["delta"] < 0 for step in hist), s
-    yf = y.reshape(-1)
-    wv = np.repeat(w, np.diff(P.vo) * 3)
-    jac = lambda z: P.grad(z) + wv * (z - yf)                                       # noqa: E731
-    gx = jac(x)
-    print(f"{kind}: |grad Phi_c| / gtol at the end {[float(np.linalg.norm(gx[3 * P.vo[s]:3 * P.vo[s + 1]]) / o['gtol']) for s in range(P.S)]}")
-    for s in must:
-        assert np.linalg.norm(gx[3 * P.vo[s]:3 * P.vo[s + 1]]) <= o["gtol"] * (1 + 1e-6), s
-    if kind == "small":
-        _, _, _, _, (xe, _) = _prox_ref("small")
-        ref = minimize(lambda z: float(_phi(P, z, yf, w).sum()), yf.copy(), jac=jac,
-                       hessp=lambda z, p: hvp(P.orc, z, p, P.c1, P.c2, P.order).reshape(-1) + wv * p, method="trust-ncg",
-                       options=dict(gtol=1e-3 * o["gtol"], maxiter=500))
-        for other in (xe, ref.x):
-            go = jac(other)
-            for s in must:
-                sl = slice(3 * P.vo[s], 3 * P.vo[s + 1])
-                bound = (np.linalg.norm(gx[sl]) + np.linalg.norm(go[sl])) / w[s]
-                assert np.linalg.norm(x[sl] - other[sl]) <= bound, (s, np.linalg.norm(x[sl] - other[sl]), bound)
-
-
-def _ref_pack_gpu(torch, ext):
-    from test_newton_prox import _prox_ref
-    P, x, w, o, _ = _prox_ref("small")
-    sp = _handle(ext, P.pk.verts, P.pk.tets, enable_amips=True, deterministic=True)
-    return P, x, w, o, sp
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("c3", [0.0, C3], ids=["amips-off", "amips-on"])
-def test_psd_steps_equal_their_composition(ext, c3):
-    """A PSD-mode tsb_newton_step and tsb_newton_prox_step against the public calls (on the PSD workspace: its solve
-    multiplies by H+) composed with the numpy rule: bitwise x, the same k, alpha and status, mu to fp64 rounding."""
-    torch = _torch()
-    from test_newton_lm import _compose_step, _labels, new_state, N_CONVERGED
-    from test_newton_prox import _compose_prox, _weights
-    from tssplat_b200.newton import DeviceNewton
-    pk, x_np = _pack("small")
-    sp = _handle(ext, pk.verts, pk.tets, enable_amips=True, deterministic=True)
-    sid_np, orph_np, S = _labels(pk.verts, pk.tets)
-    sid, orph = torch.from_numpy(sid_np).cuda(), torch.from_numpy(orph_np).cuda()
-    nw = DeviceNewton(sp, hessian="psd")
-    c1, c2 = COEF
-    o = dict(OPTS, gtol=0.05)
-    for prox in (False, True):
-        nw.reset()
-        x1 = _cuda(x_np)
-        x2 = x1.clone()
-        y = _cuda(perturb(pk, sigma_rel=0.01, seed=5))
-        w = _weights(torch, sp.hess_diag(x1, c1, c2, 2, c3=c3), sid, orph, S, [1e-3, 1e-1, 1.0])
-        st = new_state(S)
-        seen = set()
-        for t in range(6):
-            if prox:
-                r = nw.step(x1, c1, c2, 2, c3=c3, anchor=y, weight=w, **o)
-                x2, out = _compose_prox(torch, sp, nw.pcg, x2, y, w, st, c1, c2, c3, o, sid, orph, S)
-            else:
-                r = nw.step(x1, c1, c2, 2, c3=c3, **o)
-                x2, out = _compose_step(torch, sp, nw.pcg, x2, st, c1, c2, c3, o, sid, orph, S)
-            assert torch.equal(x1, x2), (prox, t)
-            assert r.k.cpu().tolist() == [q[1] for q in out] and r.alpha.cpu().tolist() == [q[0] for q in out], (prox, t)
-            assert r.status.cpu().tolist() == [s["status"] for s in st], (prox, t)
-            assert np.allclose(r.mu.cpu().numpy(), [s["mu"] for s in st], rtol=1e-12, atol=0)
-            seen |= set(r.status.cpu().tolist())
-        assert N_CONVERGED in seen, prox
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind", ["plain", "small"])
 def test_psd_steps_converge_within_the_reference_count(ext, kind):
     """On the projected reference's own pack, the spheres of PSD_MUST (with w = 0 all three, the rough one included) are
     CONVERGED within PSD_REF_STEPS + GPU_SLACK PSD-mode steps, no step raises Phi, and with the small weight the rough
     sphere's Phi falls at every step.  With the small weight the converged spheres' GPU fixed point is the fp64
-    exact-mode fixed point (test_newton_prox's reference) within the stationarity bound, using the oracle's gradient at
+    exact-mode fixed point (the proximal fp64 reference) within the stationarity bound, using the oracle's gradient at
     the GPU point."""
     torch = _torch()
-    from test_newton_lm import GPU_SLACK
-    from test_newton_prox import _prox_ref
     from tssplat_b200.newton import DeviceNewton
-    P, x0, w, o, sp = _ref_pack_gpu(torch, ext)
+    P, x0, w, o = reference_problem(scale="small")
+    sp = _handle(ext, P.pk.verts, P.pk.tets, enable_amips=True, deterministic=True)
     w = np.zeros_like(w) if kind == "plain" else w
     nw = DeviceNewton(sp, hessian="psd")
     x = _cuda(x0.reshape(-1, 3))
@@ -782,7 +533,7 @@ def test_psd_steps_converge_within_the_reference_count(ext, kind):
     print(f"{kind}: spheres {must} CONVERGED at GPU step {steps}, reference {PSD_REF_STEPS[kind]}, status {r.status.tolist()}")
     assert steps is not None and steps <= PSD_REF_STEPS[kind] + GPU_SLACK, r.status
     if kind == "small":
-        xe = _prox_ref("small")[4][0]
+        xe = reference_run("prox", "small")[6]
         xg = x.double().cpu().numpy().reshape(-1)
         yf = x0.reshape(-1)
         wv = np.repeat(w, np.diff(P.vo) * 3)
@@ -791,3 +542,19 @@ def test_psd_steps_converge_within_the_reference_count(ext, kind):
             sl = slice(3 * P.vo[s], 3 * P.vo[s + 1])
             bound = (np.linalg.norm(gx[sl]) + np.linalg.norm(ge[sl])) / w[s]
             assert np.linalg.norm(xg[sl] - xe[sl]) <= bound, (s, np.linalg.norm(xg[sl] - xe[sl]), bound)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the checks every Newton step shares (_newton_checks)
+
+
+@pytest.mark.parametrize("kind", ["plain", "small"])
+def test_psd_reference_mixed_pack(kind):
+    check_reference("psd", kind)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("c3", [0.0, C3], ids=["amips-off", "amips-on"])
+def test_psd_steps_equal_their_composition(ext, c3):
+    for prox in (False, True):
+        check_composition(ext, "psd", c3, prox)

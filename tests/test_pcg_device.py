@@ -1,9 +1,10 @@
 """The device-resident per-sphere PCG solver (tsb_pcg_*, tsb_sphere_axpy, newton.DevicePCG,
 SmoothnessBarrierEnergy.newton_direction).
 
-CPU: an fp64 numpy restatement of the batched state machine the kernels implement, against dense solves per component
-and step for step against newton.pcg; its status semantics; the kernel's 3x3 Jacobi eigen / clamp / inverse algorithm
-re-enacted in numpy against newton.block_jacobi; the host builder's component lists and chunk table.  GPU: the
+CPU: the fp64 numpy restatement of the batched state machine the kernels implement (_newton_model), against dense
+solves per component and step for step against newton.pcg; its status semantics; the kernel's 3x3 Jacobi eigen /
+clamp / inverse algorithm re-enacted in numpy against newton.block_jacobi; the host builder's component lists and chunk
+table.  GPU: the
 preconditioner kernel, the solve (true residuals, records, energy decrease, product counts), a mixed pack where the
 global CG is truncated by one sphere, independence and bitwise repeatability, handle variants, the per-sphere axpy,
 chaining, handle info, argument errors and the module route end to end."""
@@ -13,128 +14,9 @@ import numpy as np
 import pytest
 
 from _helpers import GOLDEN, PLAN_DEBUG_SO
+from _newton_model import (CHUNK, COEF, CONVERGED, MAXITER, NEGCURV, NEGCURV_FIRST, ZERO_RHS, _cuda, _handle,  # noqa: F401
+                           _shuffled_mesh, _spd, _torch, batched_pcg_reference, ext, jacobi_inverse_blocks, planes_of, sym6)
 from tssplat_b200.mesh import connected_components, make_pack, perturb
-
-MAXITER, CONVERGED, NEGCURV, NEGCURV_FIRST, ZERO_RHS = 0, 1, 2, 3, 4
-CHUNK = 256
-C3 = 0.5
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# fp64 restatement of the kernels' state machine
-
-
-def batched_pcg_reference(H_blocks, b, P, max_iter, rtol):
-    """Truncated PCG on every diagonal block at once, as pcg_init / pcg_curv / pcg_update / pcg_dir run it: all
-    components take part in every iteration, a stopped one idles with p = 0.  H_blocks, b, P: per component a dense
-    [m, m] matrix, a right-hand side [m] and a preconditioner (dense [m, m], or None).  Returns per component a dict
-    (d, status, n_hvp, rel_residual, b_dot_d, d_H_d) and the iterations run."""
-    S = len(H_blocks)
-    ap = lambda c, r: r.copy() if P[c] is None else P[c] @ r
-    st = []
-    for c in range(S):
-        r = np.array(b[c], np.float64)
-        z = ap(c, r)
-        bb = float(r @ r)
-        active = bb != 0.0
-        st.append(dict(r=r, z=z, p=z.copy() if active else np.zeros_like(z), d=np.zeros_like(r), rz=float(r @ z), bb=bb,
-                       rr=bb, dHd=0.0, n_hvp=0, status=None if active else ZERO_RHS))
-    for it in range(max_iter):
-        for c, s in enumerate(st):
-            if s["status"] is not None:
-                continue
-            Hp = H_blocks[c] @ s["p"]
-            pHp = float(s["p"] @ Hp)
-            s["n_hvp"] = it + 1
-            if not pHp > 0.0:
-                s["status"] = NEGCURV_FIRST if it == 0 else NEGCURV
-                if it == 0:
-                    s["d"] = s["z"].copy()
-                continue
-            a = s["rz"] / pHp
-            s["d"] = s["d"] + a * s["p"]
-            s["r"] = s["r"] - a * Hp
-            s["dHd"] += a * a * pHp
-            s["z"] = ap(c, s["r"])
-            rz, s["rr"] = float(s["r"] @ s["z"]), float(s["r"] @ s["r"])
-            if np.sqrt(s["rr"]) <= rtol * np.sqrt(s["bb"]):
-                s["status"] = CONVERGED
-            s["p"] = s["z"] + (rz / s["rz"]) * s["p"]
-            s["rz"] = rz
-    out = []
-    for c, s in enumerate(st):
-        status = MAXITER if s["status"] is None else s["status"]
-        rel = 0.0 if status == ZERO_RHS else 1.0 if status == NEGCURV_FIRST else float(np.sqrt(s["rr"] / s["bb"]))
-        out.append(dict(d=s["d"], status=status, n_hvp=s["n_hvp"], rel_residual=rel, b_dot_d=float(np.dot(b[c], s["d"])),
-                        d_H_d=s["dHd"]))
-    return out
-
-
-def jacobi_inverse_blocks(D, rel_floor, sweeps=8):
-    """pcg_blocks_kernel in numpy, operation for operation (fp64): cyclic Jacobi over (0,1), (0,2), (1,2), clamp,
-    invert.  D: [n, 3, 3] symmetric.  Returns [n, 6] = (xx, yy, zz, yz, xz, xy)."""
-    out = np.zeros((len(D), 6))
-    for i, A in enumerate(np.asarray(D, np.float64)):
-        a = {(0, 0): A[0, 0], (1, 1): A[1, 1], (2, 2): A[2, 2], (0, 1): A[0, 1], (0, 2): A[0, 2], (1, 2): A[1, 2]}
-        V = np.eye(3)
-        key = lambda i, j: (min(i, j), max(i, j))
-        for _ in range(sweeps):
-            if a[(0, 1)] == 0.0 and a[(0, 2)] == 0.0 and a[(1, 2)] == 0.0:
-                break
-            for p, q in ((0, 1), (0, 2), (1, 2)):
-                r = 3 - p - q
-                apq = a[(p, q)]
-                if apq == 0.0:
-                    continue
-                with np.errstate(over="ignore"):                     # a tiny a_pq: theta = inf, t = 0, as in the kernel
-                    theta = (a[(q, q)] - a[(p, p)]) / (2.0 * apq)
-                    t = np.copysign(1.0, theta) / (abs(theta) + np.sqrt(theta * theta + 1.0))
-                c = 1.0 / np.sqrt(t * t + 1.0)
-                s = t * c
-                a[(p, p)] -= t * apq
-                a[(q, q)] += t * apq
-                a[(p, q)] = 0.0
-                apr, aqr = a[key(p, r)], a[key(q, r)]
-                a[key(p, r)], a[key(q, r)] = c * apr - s * aqr, s * apr + c * aqr
-                vp, vq = V[:, p].copy(), V[:, q].copy()
-                V[:, p], V[:, q] = c * vp - s * vq, s * vp + c * vq
-        lam = np.array([a[(0, 0)], a[(1, 1)], a[(2, 2)]])
-        lmax = lam.max()
-        if lmax > 0.0:
-            inv = 1.0 / np.maximum(lam, rel_floor * lmax)
-            M = (V * inv) @ V.T
-            out[i] = [M[0, 0], M[1, 1], M[2, 2], M[1, 2], M[0, 2], M[0, 1]]
-    return out
-
-
-def sym6(P):
-    """[n, 3, 3] symmetric -> [n, 6] = (xx, yy, zz, yz, xz, xy)."""
-    P = np.asarray(P)
-    return np.stack([P[:, 0, 0], P[:, 1, 1], P[:, 2, 2], P[:, 1, 2], P[:, 0, 2], P[:, 0, 1]], axis=1)
-
-
-def planes_of(D):
-    D = np.asarray(D)
-    return np.stack([np.stack([D[:, 0, 0], D[:, 1, 1], D[:, 2, 2]], 1), np.stack([D[:, 1, 2], D[:, 0, 2], D[:, 0, 1]], 1)])
-
-
-def _spd(rng, m, lo=0.5, hi=20.0):
-    Q = np.linalg.qr(rng.normal(size=(m, m)))[0]
-    return (Q * rng.uniform(lo, hi, size=m)) @ Q.T
-
-
-def _shuffled_mesh():
-    """tests/test_hvp.py's "shuffled" mesh: a 3 x 1024 pack relabelled into a larger id space (500 orphans)."""
-    pk = make_pack(3, 1024, seed=1)
-    rng = np.random.default_rng(8)
-    n = len(pk.verts) + 500
-    ids = rng.permutation(n)[:len(pk.verts)]
-    V = rng.normal(size=(n, 3)).astype(np.float32)
-    V[ids] = pk.verts
-    T = ids[pk.tets].astype(np.int32)
-    x = V.copy()
-    x[ids] = perturb(pk, sigma_rel=0.02, seed=1)
-    return V, T, x
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -344,26 +226,6 @@ def test_component_lists_and_chunk_table(mesh):
 # GPU
 
 
-def _torch():
-    import torch
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch
-
-
-@pytest.fixture(scope="module")
-def ext():
-    _torch()
-    from tssplat_b200 import tet_spheres_ext
-    return tet_spheres_ext
-
-
-def _handle(ext, V, T, **kw):
-    return ext.TetSpheres(np.ascontiguousarray(V, np.float32).reshape(-1), np.ascontiguousarray(T, np.int32).reshape(-1), **kw)
-
-
-def _cuda(a):
-    return _torch().from_numpy(np.ascontiguousarray(a, np.float32)).cuda()
-
 
 _PACKS = {}
 
@@ -399,9 +261,6 @@ def _sphere_dots(torch, a, b, sid, S):
     return torch.zeros(S, dtype=torch.float64, device=a.device).index_add_(0, sid, (a.double() * b.double()).sum(dim=1))
 
 
-COEF = (2e-4 / 3, 2e-4)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("mesh", ["big", "shuffled"])
 def test_set_blocks_against_block_jacobi(ext, mesh):
@@ -413,7 +272,7 @@ def test_set_blocks_against_block_jacobi(ext, mesh):
     else:
         V, T, x = _shuffled_mesh()
     sp = _handle(ext, V, T, enable_amips=True)
-    planes = sp.hess_diag(_cuda(x), 2e-3, 0.8, 2, c3=C3)
+    planes = sp.hess_diag(_cuda(x), 2e-3, 0.8, 2, c3=0.5)
     ws = DevicePCG(sp)
     for rel_floor in (1e-6, 1e-2):
         got = ws.set_blocks(planes, rel_floor=rel_floor, want_inverse=True).double().cpu().numpy()
@@ -555,6 +414,8 @@ def test_independence_and_bitwise_repeatability(ext):
 @pytest.mark.gpu
 @pytest.mark.parametrize("kw", [dict(), dict(warps_per_cta=8), dict(deterministic=True), dict(warps_per_cta=8, deterministic=True)],
                          ids=["w16", "w8", "w16-det", "w8-det"])
+
+
 def test_staged_handle_variants(ext, kw):
     torch = _torch()
     from tssplat_b200.newton import DevicePCG

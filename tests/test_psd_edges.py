@@ -3,7 +3,7 @@
 CPU: project_reenact, the kernel's projection restated in fp64 numpy operation for operation (Jacobi eigen-system of
 F^T F, sort, proper V, one one-sided Jacobi sweep on the columns of F V, Gram-Schmidt, the closed forms, the clamp of A),
 its 30 stored floats rounded to fp32, against numpy.linalg.eigh of the 9 x 9 F-space Hessian, on random F (calibrating
-KAPPA), test_newton_psd's cases, needles, a collapsing plane, equal singular values with a negative s_3, a large stretch
+KAPPA), _newton_model's cases, needles, a collapsing plane, equal singular values with a negative s_3, a large stretch
 and a uniformly tiny F, in both signs of det F and rounded to fp32; the fp64 stage alone; the algorithm without the
 one-sided sweep fails the needles; apply_reenact, psd_apply_kernel's fp32 product, and its curvature.  GPU: a handle of
 disjoint single-tet components (unit right tets with B = I and a generic rest tet far from the origin), so every tet's F
@@ -12,9 +12,8 @@ record; flat and collapsed tets; AMIPS at rotations; inverted tets with AMIPS on
 import numpy as np
 import pytest
 
+from _newton_model import C3, COEF, _cases, _cuda, _handle, _rot, _torch, ext  # noqa: F401
 from test_hess_diag import psi_hessians
-from test_newton_lm import C3, COEF, _cuda, _handle, _torch, ext  # noqa: F401
-from test_newton_psd import _cases, _rot
 
 U32 = 2.0 ** -24                # fp32 unit roundoff
 FLT_MIN = 2.0 ** -126           # smallest normal fp32: the floor of an operator entry's absolute error
