@@ -456,6 +456,50 @@ int64_t tsb_hessian_device_bytes(tsb_hessian_t hs);
 int tsb_hessian_pattern(tsb_hessian_t hs, int64_t *nnzb, int32_t *crow_dev_out, int32_t *col_dev_out, void *stream);
 int tsb_hessian_assemble(tsb_hessian_t hs, const float *x_dev, const tsb_terms_t *terms, float *values_dev, void *stream);
 
+/* ---- Symmetric Gauss-Seidel preconditioner: multicolour block SGS from the assembled Hessian ------------------------
+ * Opt-in on a solver workspace, in place of block Jacobi.  Per component, with A the assembled matrix of hs (H, or H+ in
+ * PSD mode), Dt^-1 the clamped inverse diagonal blocks tsb_pcg_set_blocks(_ex) computes, and L, U = L^T the strict lower
+ * and upper block parts of A in a multicolour order (colours ascending; vertices that share a tet, or any other block of
+ * the pattern, never share a colour):
+ *   M^-1 = (Dt + U)^-1 Dt (Dt + L)^-1 = W^T Dt W,  W = (Dt + L)^-1
+ * applied as a forward sweep, colour by colour, y_i = Dt_i^-1 (r_i - sum_{col j < col i} A_ij y_j), then a backward sweep,
+ * colours in reverse, z_i = y_i - Dt_i^-1 sum_{col j > col i} A_ij z_j.  M^-1 is SPD wherever every Dt_i is, indefinite A
+ * included, so CG, Steihaug-Toint and every Newton step keep their rules; a vertex with the zero inverse block gets z_i = 0
+ * (it does not move, as with block Jacobi).  The symmetry rests on A_ij = A_ji^T bitwise, which the assembly guarantees.
+ * DESIGN.md section 5, "Symmetric Gauss-Seidel preconditioner".
+ *
+ * tsb_pcg_enable_sgs: hs must have been created over s (TSB_E_INVALID otherwise) and must outlive every later call on s.
+ * Colours every component greedily on the host (vertices ascending, smallest free colour: deterministic), builds each
+ * row's lists of earlier-colour and later-colour blocks and the per-component colour schedule, and allocates the
+ * workspace's own values buffer.  tsb_pcg_device_bytes grows by
+ *   36 nnzb + 8 (nnzb - rows) + 12 rows + 8 + 8 (n_components + 1) + 4 (total colours + n_components) + 4 n   bytes
+ * (values; the two block lists; list offsets and schedule; component and colour-table offsets; colour table; colours;
+ * rows = vertices some tet references, total colours = the sum over components).  A component whose
+ * vector does not fit one CTA's shared memory (12 bytes per vertex: about 19 k vertices on an H100) is TSB_E_INVALID,
+ * naming the component and its size.  A second call is TSB_E_INVALID.  Synchronous and allocating: not during a stream
+ * capture (detected on the legacy default stream only, as for tsb_pcg_enable_psd).  After a failure the workspace is as
+ * before.  From then on every tsb_pcg_solve(_ex, _tr) on s applies M^-1 where block Jacobi applied its blocks (one sweep
+ * kernel after the init and after every update kernel; the Jacobi z they write is overwritten), the trust-region
+ * radius start of tsb_newton_tr_step(_ex) uses b^T M^-1 b, and every Newton step on s calls tsb_pcg_set_matrix in place
+ * of tsb_hess_diag (the diagonal planes, and so the preconditioner and the first damping mu_c, then come from A).
+ *
+ * tsb_pcg_set_matrix: assembles A(x_dev) into the workspace's values buffer through hs (tsb_hessian_assemble's rules for
+ * *terms) and writes its diagonal blocks to diag_out_dev (device float32 [2][n][3], tsb_hess_diag's planes; orphan rows
+ * zero), to hand to tsb_pcg_set_blocks(_ex).  No host read, no allocation: capturable.
+ *
+ * tsb_pcg_apply_precond: z_dev = M^-1 r_dev on every component (device float32 [3n]; z on vertices no tet references is
+ * left as it is; z_dev must not alias r_dev).  One launch, one CTA per component, no atomics: bitwise repeatable, and a
+ * component's z does not depend on other components' r.
+ *
+ * tsb_pcg_sgs_colors: colors_out_dev (optional device int32 [n]) receives every vertex's colour (-1 for orphans), on the
+ * legacy default stream and synchronously; *n_colors_out (optional) the most colours of any component.
+ * Argument errors (TSB_E_INVALID, nothing launched): a null pointer that is required, SGS not enabled (set_matrix,
+ * apply_precond, colors). */
+int tsb_pcg_enable_sgs(tsb_pcg_t s, tsb_hessian_t hs);
+int tsb_pcg_set_matrix(tsb_pcg_t s, const float *x_dev, const tsb_terms_t *terms, float *diag_out_dev, void *stream);
+int tsb_pcg_apply_precond(tsb_pcg_t s, const float *r_dev, float *z_dev, void *stream);
+int tsb_pcg_sgs_colors(tsb_pcg_t s, int32_t *colors_out_dev, int32_t *n_colors_out);
+
 /* ---- Damped Newton step: one Levenberg-Marquardt iteration per sphere on the device (no counterpart in the reference)
  * A Newton workspace sits beside a solver workspace (which must outlive it; creating one changes nothing about the
  * handle or the solver workspace) and holds b, d and the two diagonal planes (12 floats per vertex), the per-sphere line

@@ -26,7 +26,7 @@ EXPORTED_SYMBOLS = (
     "tsb_pcg_set_blocks", "tsb_pcg_solve", "tsb_sphere_axpy", "tsb_pcg_set_blocks_ex", "tsb_pcg_solve_ex",
     "tsb_pcg_enable_psd", "tsb_pcg_hvp_psd", "tsb_pcg_solve_tr",
     "tsb_hessian_create", "tsb_hessian_destroy", "tsb_hessian_last_error", "tsb_hessian_device_bytes", "tsb_hessian_pattern",
-    "tsb_hessian_assemble",
+    "tsb_hessian_assemble", "tsb_pcg_enable_sgs", "tsb_pcg_set_matrix", "tsb_pcg_apply_precond", "tsb_pcg_sgs_colors",
     "tsb_newton_create", "tsb_newton_destroy", "tsb_newton_last_error", "tsb_newton_device_bytes", "tsb_newton_reset",
     "tsb_newton_step", "tsb_newton_prox_step", "tsb_newton_tr_step", "tsb_newton_tr_step_ex", "tsb_energy_grad_host", "tsb_scale",
     "tsb_grad_limit", "tsb_adam_uniform_step",
@@ -184,6 +184,14 @@ def _load() -> C.CDLL:
     lib.tsb_hessian_pattern.argtypes = [vp, C.POINTER(i64), vp, vp, vp]
     lib.tsb_hessian_assemble.restype = C.c_int
     lib.tsb_hessian_assemble.argtypes = [vp, vp, C.POINTER(tsb_terms_t), vp, vp]
+    lib.tsb_pcg_enable_sgs.restype = C.c_int
+    lib.tsb_pcg_enable_sgs.argtypes = [vp, vp]
+    lib.tsb_pcg_set_matrix.restype = C.c_int
+    lib.tsb_pcg_set_matrix.argtypes = [vp, vp, C.POINTER(tsb_terms_t), vp, vp]
+    lib.tsb_pcg_apply_precond.restype = C.c_int
+    lib.tsb_pcg_apply_precond.argtypes = [vp, vp, vp, vp]
+    lib.tsb_pcg_sgs_colors.restype = C.c_int
+    lib.tsb_pcg_sgs_colors.argtypes = [vp, vp, C.POINTER(C.c_int32)]
     lib.tsb_newton_create.restype = C.c_int
     lib.tsb_newton_create.argtypes = [vp, C.POINTER(vp)]
     lib.tsb_newton_destroy.restype = None

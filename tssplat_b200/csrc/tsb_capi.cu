@@ -12,6 +12,7 @@
 #include "tsb_kernels.cuh"
 #include "tsb_plan.h"
 #include "tsb_psd.cuh"
+#include "tsb_sgs.cuh"
 #include "tsb_solver.cuh"
 
 static_assert(sizeof(tsb_sphere_stats_t) == 40, "tsb_sphere_stats_t must be 40 bytes");
@@ -55,6 +56,11 @@ struct tsb_pcg_s {
   bool psd = false;                  // tsb_pcg_enable_psd: the solve multiplies by the projected Hessian
   tsb::PsdParams Q{};
   tsb::TrComp *tr = nullptr;         // [n_components] trust-region recurrences (allocated by the first tsb_pcg_solve_tr)
+  tsb_hessian_t sgs = nullptr;       // tsb_pcg_enable_sgs: the Hessian workspace that assembles A, and the sweep's tables
+  tsb::SgsParams G{};
+  float *sgs_values = nullptr;       // [9 nnzb] A, written by tsb_pcg_set_matrix
+  int32_t *sgs_color = nullptr;      // [n]
+  int32_t sgs_n_colors = 0;
   std::vector<void *> allocs;
   std::string err;
 };
@@ -780,7 +786,8 @@ int pcg_solve_impl(tsb_pcg_t s, const float *x_dev, const float *b_dev, const ts
     const int rc = psd_project(s, x_dev, *terms, st);
     if (rc != TSB_OK) return rc;
   }
-  cudaError_t e = tsb::launch_pcg_begin(P, b_dev, d_out_dev, tr, st);
+  const tsb::SgsParams *sgs = s->sgs ? &s->G : nullptr;
+  cudaError_t e = tsb::launch_pcg_begin(P, b_dev, d_out_dev, tr, st, sgs);
   if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver launch: ") + cudaGetErrorString(e));
   int32_t it = 0;
   while (it < opt->max_iter) {
@@ -791,7 +798,7 @@ int pcg_solve_impl(tsb_pcg_t s, const float *x_dev, const float *b_dev, const ts
       const int rc = hvp_impl(s->h, x_dev, P.p, terms->c1, terms->c2, terms->c3, terms->order, 1.f, nullptr, P.Hp, nullptr, 1, st);
       if (rc != TSB_OK) return pcg_fail(s, rc, s->h->err);
     }
-    e = tsb::launch_pcg_step(P, d_out_dev, it, opt->rtol, shift_dev, tr, st);
+    e = tsb::launch_pcg_step(P, d_out_dev, it, opt->rtol, shift_dev, tr, st, sgs);
     if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver launch: ") + cudaGetErrorString(e));
     ++it;
     if (opt->check_every > 0 && it % opt->check_every == 0 && it < opt->max_iter) {
@@ -1006,8 +1013,14 @@ int newton_run(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const flo
   const float *shift = k.damped ? W.shift : weight_dev;
   // b = -grad, the diagonal blocks; frozen spheres' b = 0 (prox: b -= w (x - y)); damped: mu on a first step
   rc = energy_grad_impl(h, x_dev, terms->c1, terms->c2, terms->c3, terms->order, -1.f, nullptr, nw->energy, 1, W.b, nullptr, st);
-  if (rc == TSB_OK) rc = tsb_hess_diag(h, x_dev, terms, 1.f, nullptr, W.diag, st);
   if (rc != TSB_OK) return newton_fail(nw, rc, h->err);
+  if (s->sgs) {         // the diagonal blocks of the matrix the sweep uses
+    rc = tsb_pcg_set_matrix(s, x_dev, terms, W.diag, st);
+    if (rc != TSB_OK) return newton_fail(nw, rc, s->err);
+  } else {
+    rc = tsb_hess_diag(h, x_dev, terms, 1.f, nullptr, W.diag, st);
+    if (rc != TSB_OK) return newton_fail(nw, rc, h->err);
+  }
   cudaError_t e = tsb::launch_newton_prep(s->P, W, prox, st);
   if (e == cudaSuccess && k.damped) e = tsb::launch_newton_shift(s->P, W, k.lm, prox, st);
   if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
@@ -1015,7 +1028,7 @@ int newton_run(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const flo
   rc = tsb_pcg_set_blocks_ex(s, W.diag, k.rel_floor, shift, nullptr, st);
   if (rc != TSB_OK) return newton_fail(nw, rc, s->err);
   if (!k.damped) {
-    e = tsb::launch_newton_tr_radius(s->P, W, T, k.tr, st);
+    e = tsb::launch_newton_tr_radius(s->P, W, T, k.tr, st, s->sgs ? &s->G : nullptr);
     if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
   }
   // the solve
@@ -1182,6 +1195,116 @@ int tsb_hessian_assemble(tsb_hessian_t hs, const float *x_dev, const tsb_terms_t
   if (e == cudaSuccess) e = tsb::launch_hessian_blocks(hs->P, x_dev, terms->order, terms->c2, terms->c3, hs->psd, st);
   if (e == cudaSuccess) e = tsb::launch_hessian_gather(hs->P, terms->c1, values_dev, st);
   if (e != cudaSuccess) return hessian_fail(hs, TSB_E_CUDA, std::string("hessian launch: ") + cudaGetErrorString(e));
+  return TSB_OK;
+}
+
+/* ---- Symmetric Gauss-Seidel preconditioner (tsb_sgs.cu) ---- */
+
+int tsb_pcg_enable_sgs(tsb_pcg_t s, tsb_hessian_t hs) {
+  if (!s) return TSB_E_INVALID;
+  if (s->sgs) return pcg_fail(s, TSB_E_INVALID, "the symmetric Gauss-Seidel preconditioner is already enabled on this workspace");
+  if (!hs) return pcg_fail(s, TSB_E_INVALID, "hs is null");
+  if (hs->s != s) return pcg_fail(s, TSB_E_INVALID, "hs was created over another solver workspace");
+  const tsb_handle_t h = s->h;
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(cudaStreamLegacy, &cap) != cudaSuccess || cap != cudaStreamCaptureStatusNone) {
+    cudaGetLastError();
+    return pcg_fail(s, TSB_E_INVALID, "tsb_pcg_enable_sgs allocates device memory and cannot run while a stream is being captured");
+  }
+  const size_t n = size_t(h->info.n), S = size_t(s->P.n_components);
+  std::vector<int32_t> crow(n + 1), col(size_t(hs->nnzb));
+  cudaError_t e = cudaMemcpy(crow.data(), hs->crow, crow.size() * sizeof(int32_t), cudaMemcpyDeviceToHost);
+  if (e == cudaSuccess && !col.empty()) e = cudaMemcpy(col.data(), hs->col, col.size() * sizeof(int32_t), cudaMemcpyDeviceToHost);
+  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("pattern download: ") + cudaGetErrorString(e));
+  tsb::PcgLists L;
+  tsb::build_pcg_lists(h->comp_label, int32_t(S), L);
+  int32_t big = 0;
+  for (size_t c = 0; c < S; ++c)
+    if (L.comp_off[c + 1] - L.comp_off[c] > L.comp_off[size_t(big) + 1] - L.comp_off[size_t(big)]) big = int32_t(c);
+  const int32_t max_verts = S ? L.comp_off[size_t(big) + 1] - L.comp_off[size_t(big)] : 0;
+  int limit = 0;
+  e = tsb::sgs_configure(max_verts, &limit);
+  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("sweep configuration: ") + cudaGetErrorString(e));
+  if (max_verts > limit)
+    return pcg_fail(s, TSB_E_INVALID, "component " + std::to_string(big) + " has " + std::to_string(max_verts) +
+                                          " vertices; the sweep keeps a component's vector in one CTA's shared memory, at most " +
+                                          std::to_string(limit) + " vertices on this device");
+  tsb::SgsTables T;
+  std::string err;
+  int rc = tsb::build_sgs_tables(crow, col, L, 0, T, err);
+  if (rc != TSB_OK) return pcg_fail(s, rc, err);
+  const size_t allocs0 = s->allocs.size();
+  const int64_t bytes0 = s->device_bytes;
+  tsb::SgsParams G{};
+  int32_t *comp_off = nullptr, *color_ptr = nullptr, *color_off = nullptr, *sched = nullptr, *lo_ptr = nullptr, *hi_ptr = nullptr,
+          *lo = nullptr, *hi = nullptr, *color = nullptr;
+  float *values = nullptr;
+  rc = ws_alloc<float>(s, 9 * std::max<size_t>(col.size(), 1), nullptr, &values);
+  if (rc == TSB_OK) rc = ws_alloc(s, L.comp_off.size(), L.comp_off.data(), &comp_off);
+  if (rc == TSB_OK) rc = ws_alloc(s, T.color_ptr.size(), T.color_ptr.data(), &color_ptr);
+  if (rc == TSB_OK) rc = ws_alloc(s, std::max<size_t>(T.color_off.size(), 1), T.color_off.empty() ? nullptr : T.color_off.data(), &color_off);
+  if (rc == TSB_OK) rc = ws_alloc(s, std::max<size_t>(T.sched.size(), 1), T.sched.empty() ? nullptr : T.sched.data(), &sched);
+  if (rc == TSB_OK) rc = ws_alloc(s, T.lo_ptr.size(), T.lo_ptr.data(), &lo_ptr);
+  if (rc == TSB_OK) rc = ws_alloc(s, T.hi_ptr.size(), T.hi_ptr.data(), &hi_ptr);
+  if (rc == TSB_OK) rc = ws_alloc(s, std::max<size_t>(T.lo.size(), 2), T.lo.empty() ? nullptr : T.lo.data(), &lo);
+  if (rc == TSB_OK) rc = ws_alloc(s, std::max<size_t>(T.hi.size(), 2), T.hi.empty() ? nullptr : T.hi.data(), &hi);
+  if (rc == TSB_OK) rc = ws_alloc(s, T.color.size(), T.color.data(), &color);
+  if (rc != TSB_OK) {            // leave the workspace as it was
+    for (size_t k = allocs0; k < s->allocs.size(); ++k) cudaFree(s->allocs[k]);
+    s->allocs.resize(allocs0);
+    s->device_bytes = bytes0;
+    return rc;
+  }
+  G.comp_off = comp_off; G.color_ptr = color_ptr; G.color_off = color_off; G.sched = sched;
+  G.lo_ptr = lo_ptr; G.hi_ptr = hi_ptr;
+  G.lo = reinterpret_cast<const int2 *>(lo); G.hi = reinterpret_cast<const int2 *>(hi);
+  G.values = values; G.crow = hs->crow; G.col = hs->col; G.max_verts = max_verts;
+  s->G = G;
+  s->sgs_values = values;
+  s->sgs_color = color;
+  s->sgs_n_colors = T.n_colors;
+  s->sgs = hs;
+  return TSB_OK;
+}
+
+int tsb_pcg_set_matrix(tsb_pcg_t s, const float *x_dev, const tsb_terms_t *terms, float *diag_out_dev, void *stream) {
+  if (!s) return TSB_E_INVALID;
+  if (!s->sgs) return pcg_fail(s, TSB_E_INVALID, "tsb_pcg_set_matrix needs a workspace after tsb_pcg_enable_sgs");
+  if (!x_dev || !terms || !diag_out_dev) return pcg_fail(s, TSB_E_INVALID, "x_dev, terms and diag_out_dev must be non-null");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int rc = tsb_hessian_assemble(s->sgs, x_dev, terms, s->sgs_values, st);
+  if (rc != TSB_OK) return pcg_fail(s, rc, s->sgs->err);
+  DeviceGuard guard(s->h->device);
+  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  const cudaError_t e = tsb::launch_sgs_diag(s->G, s->P.n, diag_out_dev, st);
+  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("diagonal launch: ") + cudaGetErrorString(e));
+  return TSB_OK;
+}
+
+int tsb_pcg_apply_precond(tsb_pcg_t s, const float *r_dev, float *z_dev, void *stream) {
+  if (!s) return TSB_E_INVALID;
+  if (!s->sgs) return pcg_fail(s, TSB_E_INVALID, "tsb_pcg_apply_precond needs a workspace after tsb_pcg_enable_sgs");
+  if (!r_dev || !z_dev) return pcg_fail(s, TSB_E_INVALID, "r_dev and z_dev must be non-null");
+  if (r_dev == z_dev) return pcg_fail(s, TSB_E_INVALID, "z_dev must not be r_dev: r is read after z is written");
+  DeviceGuard guard(s->h->device);
+  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  const cudaError_t e = tsb::launch_sgs_sweep(s->P, s->G, tsb::SgsSweep{r_dev, z_dev, nullptr, 0, 0, -1, nullptr, nullptr},
+                                              static_cast<cudaStream_t>(stream));
+  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("sweep launch: ") + cudaGetErrorString(e));
+  return TSB_OK;
+}
+
+int tsb_pcg_sgs_colors(tsb_pcg_t s, int32_t *colors_out_dev, int32_t *n_colors_out) {
+  if (!s) return TSB_E_INVALID;
+  if (!s->sgs) return pcg_fail(s, TSB_E_INVALID, "tsb_pcg_sgs_colors needs a workspace after tsb_pcg_enable_sgs");
+  if (n_colors_out) *n_colors_out = s->sgs_n_colors;
+  if (!colors_out_dev) return TSB_OK;
+  DeviceGuard guard(s->h->device);
+  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  const cudaError_t e = cudaMemcpy(colors_out_dev, s->sgs_color, size_t(s->P.n) * sizeof(int32_t), cudaMemcpyDeviceToDevice);
+  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("colour copy: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 

@@ -1220,6 +1220,95 @@ int build_hessian_pattern(const float *rest, const int32_t *tets, int32_t n, int
   return TSB_OK;
 }
 
+int build_sgs_tables(const std::vector<int32_t> &crow, const std::vector<int32_t> &col, const PcgLists &L, int nth,
+                     SgsTables &T, std::string &err) {
+  T = SgsTables();
+  const size_t n = crow.size() - 1, rows = L.vert.size(), S = L.comp_off.size() - 1;
+  if (nth <= 0) nth = std::clamp(int(std::thread::hardware_concurrency()), 1, kMaxHostThreads);
+  T.color.assign(n, -1);
+  std::vector<int32_t> pos(n, -1);               // entry of every vertex in L.vert
+  for (size_t e = 0; e < rows; ++e) pos[size_t(L.vert[e])] = int32_t(e);
+  // pass 1, per component: colours, and the lengths of every row's two lists
+  std::vector<int32_t> n_lo(rows, 0), n_hi(rows, 0), ncol(S, 0);
+  std::atomic<int64_t> bad{-1};
+  parallel_for(S, 1, nth, [&](size_t c0, size_t c1) {
+    std::vector<uint8_t> used;
+    for (size_t c = c0; c < c1; ++c) {
+      int32_t nc = 0;
+      for (int32_t e = L.comp_off[c]; e < L.comp_off[c + 1]; ++e) {
+        const int32_t v = L.vert[size_t(e)];
+        used.assign(size_t(nc) + 1, 0);
+        bool diag = false;
+        for (int32_t b = crow[size_t(v)]; b < crow[size_t(v) + 1]; ++b) {
+          const int32_t j = col[size_t(b)], pj = pos[size_t(j)];
+          if (pj < L.comp_off[c] || pj >= L.comp_off[c + 1]) { bad = int64_t(v); break; }
+          if (j == v) diag = true;
+          else if (pj < e) used[size_t(T.color[size_t(j)])] = 1;   // an earlier vertex of this component: coloured
+        }
+        if (!diag) bad = int64_t(v);
+        int32_t k = 0;
+        while (used[size_t(k)]) ++k;
+        T.color[size_t(v)] = k;
+        nc = std::max(nc, k + 1);
+      }
+      ncol[c] = nc;
+      for (int32_t e = L.comp_off[c]; e < L.comp_off[c + 1]; ++e) {
+        const int32_t v = L.vert[size_t(e)], k = T.color[size_t(v)];
+        for (int32_t b = crow[size_t(v)]; b < crow[size_t(v) + 1]; ++b) {
+          const int32_t j = col[size_t(b)];
+          if (pos[size_t(j)] < 0) continue;          // reported above
+          const int32_t kj = T.color[size_t(j)];
+          if (kj < k) ++n_lo[size_t(e)];
+          else if (kj > k) ++n_hi[size_t(e)];
+        }
+      }
+    }
+  });
+  if (bad.load() >= 0) {
+    err = "vertex " + std::to_string(bad.load()) + ": its pattern row has a column outside its component or no diagonal block";
+    return TSB_E_INVALID;
+  }
+  T.lo_ptr.assign(rows + 1, 0);
+  T.hi_ptr.assign(rows + 1, 0);
+  for (size_t e = 0; e < rows; ++e) { T.lo_ptr[e + 1] = T.lo_ptr[e] + n_lo[e]; T.hi_ptr[e + 1] = T.hi_ptr[e] + n_hi[e]; }
+  T.color_ptr.assign(S + 1, 0);
+  for (size_t c = 0; c < S; ++c) {
+    T.color_ptr[c + 1] = T.color_ptr[c] + ncol[c] + 1;
+    T.n_colors = std::max(T.n_colors, ncol[c]);
+  }
+  T.lo.resize(2 * size_t(T.lo_ptr[rows]));
+  T.hi.resize(2 * size_t(T.hi_ptr[rows]));
+  T.sched.resize(rows);
+  T.color_off.resize(size_t(T.color_ptr[S]));
+  // pass 2, per component: the lists and the schedule (a counting sort of the rows by colour keeps them ascending)
+  parallel_for(S, 1, nth, [&](size_t c0, size_t c1) {
+    for (size_t c = c0; c < c1; ++c) {
+      const int32_t e0 = L.comp_off[c], e1 = L.comp_off[c + 1];
+      int32_t *off = T.color_off.data() + T.color_ptr[c];
+      const int32_t nc = ncol[c];
+      std::fill(off, off + nc + 1, 0);
+      for (int32_t e = e0; e < e1; ++e) ++off[T.color[size_t(L.vert[size_t(e)])] + 1];
+      off[0] = e0;
+      for (int32_t k = 0; k < nc; ++k) off[k + 1] += off[k];
+      std::vector<int32_t> fill(off, off + nc);
+      for (int32_t e = e0; e < e1; ++e) {
+        const int32_t v = L.vert[size_t(e)], k = T.color[size_t(v)];
+        T.sched[size_t(fill[size_t(k)]++)] = e;
+        int32_t *lo = T.lo.data() + 2 * size_t(T.lo_ptr[size_t(e)]), *hi = T.hi.data() + 2 * size_t(T.hi_ptr[size_t(e)]);
+        for (int32_t b = crow[size_t(v)]; b < crow[size_t(v) + 1]; ++b) {
+          const int32_t j = col[size_t(b)], kj = T.color[size_t(j)];
+          if (kj == k) continue;
+          int32_t *&q = kj < k ? lo : hi;
+          q[0] = b;
+          q[1] = pos[size_t(j)] - e0;
+          q += 2;
+        }
+      }
+    }
+  });
+  return TSB_OK;
+}
+
 int build_plan(const float *rest, const int32_t *tets, int32_t n, int32_t nele, const PlanConfig &cfg,
                HostPlan &P, std::string &err) {
   if (!rest || !tets || n <= 0 || nele <= 0) { err = "null input or non-positive size"; return TSB_E_INVALID; }

@@ -183,6 +183,28 @@ struct HessPattern {
 int build_hessian_pattern(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele, int32_t laplacian_scale,
                           HessPattern &out, std::string &err);
 
+// Multicolour symmetric Gauss-Seidel tables of the per-component solve (tsb_pcg_enable_sgs), over the block pattern crow /
+// col of build_hessian_pattern and the solver's PcgLists.  Rows are numbered by their entry (position) in PcgLists::vert.
+// Every component is coloured greedily on its own, vertices ascending, each vertex taking the smallest colour none of its
+// earlier neighbours in the pattern holds; so the colours depend on neither the thread count nor the other components.
+// lo[lo_ptr[e] .. lo_ptr[e + 1]) lists row e's blocks whose column has an earlier colour, hi the later ones, in column
+// order, as (block index into the values array, position of the column in its component's vertex list).  sched holds the
+// rows of every component grouped by colour (colours ascending, rows ascending in each); colour k of component c is
+// sched[color_off[color_ptr[c] + k] .. color_off[color_ptr[c] + k + 1]).
+struct SgsTables {
+  int32_t n_colors = 0;             // the most colours any component uses
+  std::vector<int32_t> color;       // [n] colour of every vertex, -1 = orphan
+  std::vector<int32_t> lo_ptr, hi_ptr;   // [rows + 1]
+  std::vector<int32_t> lo, hi;      // [2 * entries] (block, column position) pairs
+  std::vector<int32_t> sched;       // [rows]
+  std::vector<int32_t> color_ptr;   // [n_components + 1]
+  std::vector<int32_t> color_off;   // [color_ptr[n_components]] (n_colors_c + 1 entries per component)
+};
+// nth: host threads (0: one per core, at most the plan builder's cap).  Returns 0 on success, TSB_E_* otherwise (message
+// in err): a row of a component whose pattern has a column outside the component, or no diagonal block.
+int build_sgs_tables(const std::vector<int32_t> &crow, const std::vector<int32_t> &col, const PcgLists &L, int nth,
+                     SgsTables &out, std::string &err);
+
 // Returns 0 on success, TSB_E_* otherwise (message in err).
 int build_plan(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele,
                const PlanConfig &cfg, HostPlan &plan, std::string &err);

@@ -3,6 +3,7 @@
 // GPU.  It lives beside the builder because it sets PlanConfig fields and must change with them.
 // Built into tests/native/libtsb_plan_debug.so by __graft_entry__.build(); never part of
 // libtssplat_b200.so.
+#include <algorithm>
 #include <cstring>
 #include <string>
 
@@ -107,5 +108,43 @@ int tsbdbg_hess_array(tsbdbg_hess *d, const char *name, const void **ptr, int64_
 }
 
 void tsbdbg_hess_free(tsbdbg_hess *d) { delete d; }
+
+/* The multicolour Gauss-Seidel tables tsb_pcg_enable_sgs builds (tsb::build_sgs_tables) over the pattern and the solver's
+   vertex lists of the mesh, with nth host threads (0: the default); arrays through tsbdbg_sgs_array: "color", "lo_ptr",
+   "hi_ptr", "lo", "hi", "sched", "color_ptr", "color_off", and the lists "crow", "col", "vert", "comp_off" it was built
+   from */
+struct tsbdbg_sgs { tsb::HessPattern H; tsb::PcgLists L; tsb::SgsTables T; };
+
+int tsbdbg_sgs_build(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele, int32_t laplacian_scale, int32_t nth,
+                     tsbdbg_sgs **out, int32_t *n_colors) {
+  if (!out || !n_colors) return TSB_E_INVALID;
+  *out = nullptr;
+  tsbdbg_sgs *d = new tsbdbg_sgs();
+  int rc = tsb::build_hessian_pattern(rest_xyz, tets, n, nele, laplacian_scale, d->H, g_err);
+  if (rc == TSB_OK) {
+    int32_t S = 0;
+    for (const int32_t c : d->H.comp_label) S = std::max(S, c + 1);
+    tsb::build_pcg_lists(d->H.comp_label, S, d->L);
+    rc = tsb::build_sgs_tables(d->H.crow, d->H.col, d->L, nth, d->T, g_err);
+  }
+  if (rc != TSB_OK) { delete d; return rc; }
+  *n_colors = d->T.n_colors;
+  *out = d;
+  return TSB_OK;
+}
+
+int tsbdbg_sgs_array(tsbdbg_sgs *d, const char *name, const void **ptr, int64_t *count) {
+  if (!d || !name || !ptr || !count) return TSB_E_INVALID;
+  const tsb::SgsTables &T = d->T;
+  const std::string k(name);
+#define ARR(nm, vec) if (k == nm) { *ptr = (vec).data(); *count = int64_t((vec).size()); return TSB_OK; }
+  ARR("color", T.color) ARR("lo_ptr", T.lo_ptr) ARR("hi_ptr", T.hi_ptr) ARR("lo", T.lo) ARR("hi", T.hi) ARR("sched", T.sched)
+  ARR("color_ptr", T.color_ptr) ARR("color_off", T.color_off)
+  ARR("crow", d->H.crow) ARR("col", d->H.col) ARR("vert", d->L.vert) ARR("comp_off", d->L.comp_off)
+#undef ARR
+  return TSB_E_INVALID;
+}
+
+void tsbdbg_sgs_free(tsbdbg_sgs *d) { delete d; }
 
 }  // extern "C"

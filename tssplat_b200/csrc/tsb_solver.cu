@@ -9,6 +9,7 @@
 // The fold is redundant across the chunks of a component, but it needs no ticket, no atomic and no fence, and every
 // chunk gets bitwise the same scalar.  All scalars stay in device memory.
 #include "tsb_jacobi.cuh"
+#include "tsb_sgs.cuh"
 #include "tsb_solver.cuh"
 
 namespace tsb {
@@ -692,19 +693,30 @@ cudaError_t launch_pcg_blocks_shift(const PcgParams &s, const float *diag, float
   return cudaGetLastError();
 }
 
-cudaError_t launch_pcg_begin(const PcgParams &s, const float *b, float *d, const TrParams *tr, cudaStream_t st) {
+// The symmetric Gauss-Seidel mode runs the init and update kernels as they are and overwrites the z and the r.z / r.r
+// partials they wrote (block Jacobi's) with the sweep's, before the direction kernel folds them.
+cudaError_t launch_pcg_begin(const PcgParams &s, const float *b, float *d, const TrParams *tr, cudaStream_t st,
+                             const SgsParams *sgs) {
   pcg_init_kernel<<<with_orphans(s), kT, 0, st>>>(s, b, d);
+  if (sgs) {
+    const cudaError_t e = launch_sgs_sweep(s, *sgs, SgsSweep{b, s.z, s.part, kPartCols, kRz, kRr, nullptr, nullptr}, st);
+    if (e != cudaSuccess) return e;
+  }
   (tr ? pcg_dir_kernel<true, true> : pcg_dir_kernel<true, false>)<<<unsigned(s.n_chunks), kT, 0, st>>>(s, 0.f, tr ? *tr : TrParams{});
   return cudaGetLastError();
 }
 
 cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, const float *shift, const TrParams *tr,
-                            cudaStream_t st) {
+                            cudaStream_t st, const SgsParams *sgs) {
   const TrParams t = tr ? *tr : TrParams{};
   (shift ? pcg_curv_kernel<true> : pcg_curv_kernel<false>)<<<unsigned(s.n_chunks), kT, 0, st>>>(s, shift);
   (shift ? (tr ? pcg_update_kernel<true, true> : pcg_update_kernel<true, false>)
          : (tr ? pcg_update_kernel<false, true> : pcg_update_kernel<false, false>))<<<unsigned(s.n_chunks), kT, 0, st>>>(
       s, d, iter, shift, t);
+  if (sgs) {
+    const cudaError_t e = launch_sgs_sweep(s, *sgs, SgsSweep{s.r, s.z, s.part, kPartCols, kRz, kRr, s.comp, nullptr}, st);
+    if (e != cudaSuccess) return e;
+  }
   (tr ? pcg_dir_kernel<false, true> : pcg_dir_kernel<false, false>)<<<unsigned(s.n_chunks), kT, 0, st>>>(s, rtol, t);
   return cudaGetLastError();
 }
@@ -749,8 +761,13 @@ cudaError_t launch_newton_decide(const PcgParams &s, const NewtonParams &w, cons
 }
 
 cudaError_t launch_newton_tr_radius(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t, const NewtonTrRule &r,
-                                    cudaStream_t st) {
-  newton_tr_bpb_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w, t);
+                                    cudaStream_t st, const SgsParams *sgs) {
+  if (sgs) {            // z is scratch here: the solve's init overwrites it
+    const cudaError_t e = launch_sgs_sweep(s, *sgs, SgsSweep{w.b, s.z, w.part, kNwCols, kNwMaxD, -1, nullptr, t.state}, st);
+    if (e != cudaSuccess) return e;
+  } else {
+    newton_tr_bpb_kernel<<<unsigned(s.n_chunks), kT, 0, st>>>(s, w, t);
+  }
   newton_tr_radius_kernel<<<comp_blocks(s), kT, 0, st>>>(s, w, t, r);
   return cudaGetLastError();
 }

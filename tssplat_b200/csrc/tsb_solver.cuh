@@ -116,17 +116,21 @@ struct NewtonBacktrack {      // the backtracking options of tsb_newton_tr_step_
   int32_t n_alpha;
 };
 
+struct SgsParams;   // tsb_sgs.cuh: with it, the launchers below apply the symmetric Gauss-Seidel sweep in place of P
+
 cudaError_t launch_pcg_blocks(const PcgParams &s, const float *diag, float rel_floor, float *inv_out, cudaStream_t st);
 // blocks D_v + shift[c] I (over the chunk table; orphan vertices unshifted)
 cudaError_t launch_pcg_blocks_shift(const PcgParams &s, const float *diag, float rel_floor, const float *shift, float *inv_out,
                                     cudaStream_t st);
 // r = b, z = P r, d = 0 and the first direction; leaves every component ACTIVE or ZERO_RHS
-// (tr != nullptr: also initialises the trust-region recurrences)
-cudaError_t launch_pcg_begin(const PcgParams &s, const float *b, float *d, const TrParams *tr, cudaStream_t st);
+// (tr != nullptr: also initialises the trust-region recurrences; sgs != nullptr: z = M^-1 r by one sweep)
+cudaError_t launch_pcg_begin(const PcgParams &s, const float *b, float *d, const TrParams *tr, cudaStream_t st,
+                             const SgsParams *sgs = nullptr);
 // after Hp = H p of iteration `iter` (0-based) is complete on the stream: curvature, update and next direction; with
-// shift != nullptr the operator is H + shift[c] I; with tr != nullptr every component stays inside its radius
+// shift != nullptr the operator is H + shift[c] I; with tr != nullptr every component stays inside its radius; with
+// sgs != nullptr z = M^-1 r by one sweep after the update
 cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, const float *shift, const TrParams *tr,
-                            cudaStream_t st);
+                            cudaStream_t st, const SgsParams *sgs = nullptr);
 cudaError_t launch_pcg_count(const PcgParams &s, cudaStream_t st);
 cudaError_t launch_pcg_records(const PcgParams &s, const float *b, const float *d, tsb_pcg_sphere_t *out, cudaStream_t st);
 cudaError_t launch_sphere_axpy(const PcgParams &s, const float *x, const float *a, const float *d, float *out, cudaStream_t st);
@@ -141,9 +145,10 @@ cudaError_t launch_newton_dots(const PcgParams &s, const NewtonParams &w, const 
 // damped step: step choice, damping update, records (out may be null)
 cudaError_t launch_newton_decide(const PcgParams &s, const NewtonParams &w, const NewtonRule &r, const ProxParams *p,
                                  tsb_newton_sphere_t *out, cudaStream_t st);
-// trust-region step, after the preconditioner is set: b^T P b per component, Delta_c on a first step, the fp32 radius
+// trust-region step, after the preconditioner is set: b^T P b per component (sgs != nullptr: b^T M^-1 b), Delta_c on a
+// first step, the fp32 radius
 cudaError_t launch_newton_tr_radius(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t, const NewtonTrRule &r,
-                                    cudaStream_t st);
+                                    cudaStream_t st, const SgsParams *sgs = nullptr);
 // trust-region step: acceptance, radius update, records (out may be null); bt != nullptr: a rejected step is backtracked
 // along the line search's n_alpha step sizes (tsb_newton_tr_step_ex)
 cudaError_t launch_newton_tr_decide(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t, const NewtonTrRule &r,

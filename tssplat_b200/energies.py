@@ -146,7 +146,9 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
     (one fused launch, twice differentiable under ``twice_differentiable``), and ``hvp`` and ``sphere_stats`` include
     the term.  With ``amips_coeff`` absent or 0 nothing changes.  ``newton_hessian`` (default ``"exact"``) selects the
     model of ``device_pcg``, which ``newton_direction``, ``newton_step`` and ``prox_step`` solve with: ``"psd"`` is the
-    projected Hessian (``newton.DevicePCG``).
+    projected Hessian (``newton.DevicePCG``).  ``newton_precond`` (default ``"jacobi"``) selects that workspace's
+    preconditioner: ``"sgs"`` is the multicolour block symmetric Gauss-Seidel preconditioner built from the assembled
+    Hessian, which ``newton_direction``, ``newton_step``, ``prox_step`` and ``hessian`` then share.
     """
 
     #: the AMIPS coefficient; a class default, so that a module assembled without ``__init__`` (as ``bench.py`` does)
@@ -218,7 +220,8 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         from .hessian import DeviceHessian
         hs = getattr(self, "device_hessian", None)
         if hs is None:
-            hs = self.device_hessian = DeviceHessian(self._device_pcg())
+            pcg = self._device_pcg()
+            hs = self.device_hessian = pcg.hessian_ws or DeviceHessian(pcg)
         c1, c2 = self.coeff_scheduler(it)
         return hs.assemble(x.detach(), c1, c2, self.order_at(it), c3=self.amips_coeff)
 
@@ -226,7 +229,8 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         from .newton import DevicePCG
         pcg = getattr(self, "device_pcg", None)
         if pcg is None:
-            pcg = self.device_pcg = DevicePCG(self.tet_sp, hessian=getattr(self.FLAGS, "newton_hessian", "exact") or "exact")
+            pcg = self.device_pcg = DevicePCG(self.tet_sp, hessian=getattr(self.FLAGS, "newton_hessian", "exact") or "exact",
+                                              precond=getattr(self.FLAGS, "newton_precond", "jacobi") or "jacobi")
         return pcg
 
     def newton_direction(self, x, it, b=None, **solve_kw):
@@ -242,7 +246,10 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         if b is None:
             _, g = self.tet_sp.energy_grad(xd, c1, c2, order, -1.0, c3=self.amips_coeff)
             b = g.reshape(x.shape)
-        pcg.set_blocks(self.tet_sp.hess_diag(xd, c1, c2, order, c3=self.amips_coeff))
+        if pcg.precond == "sgs":    # the diagonal of the matrix the sweep uses
+            pcg.set_blocks(pcg.set_matrix(xd, c1, c2, order, c3=self.amips_coeff))
+        else:
+            pcg.set_blocks(self.tet_sp.hess_diag(xd, c1, c2, order, c3=self.amips_coeff))
         return pcg.solve(xd, b.detach(), c1, c2, order, c3=self.amips_coeff, **solve_kw)
 
     def _device_newton(self):

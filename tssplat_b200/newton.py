@@ -138,24 +138,35 @@ class DevicePCGResult(NamedTuple):
 
 
 HESSIANS = ("exact", "psd")
+#: preconditioners of ``DevicePCG``: block Jacobi, or multicolour block symmetric Gauss-Seidel from the assembled Hessian
+PRECONDS = ("jacobi", "sgs")
 
 
 class DevicePCG:
     """Per-sphere block-Jacobi PCG workspace of one ``TetSpheres`` handle (``tsb_pcg_create``), which it keeps alive.
     Serves one stream at a time, like the handle.  ``hessian="psd"`` enables the projected Hessian on it
     (``tsb_pcg_enable_psd``, from the mesh the handle keeps): ``solve`` and every ``DeviceNewton`` step over this workspace
-    then multiply by ``H+``, and ``hvp_psd`` is available.  Creating it allocates, so not inside a CUDA graph capture."""
+    then multiply by ``H+``, and ``hvp_psd`` is available.  ``precond="sgs"`` replaces block Jacobi by the multicolour
+    block symmetric Gauss-Seidel preconditioner built from the assembled Hessian (``tsb_pcg_enable_sgs``): the workspace
+    creates and owns a ``DeviceHessian`` in its mode (``hessian_ws``, usable while the workspace lives), ``set_matrix``
+    assembles the matrix the sweep uses and returns its diagonal planes for ``set_blocks``, and ``apply_precond`` and
+    ``colors`` are available.  Creating it allocates, so not inside a CUDA graph capture."""
 
-    def __init__(self, tet_sp, hessian: str = "exact"):
+    def __init__(self, tet_sp, hessian: str = "exact", precond: str = "jacobi"):
         from . import _capi
         from .tet_spheres_ext import _stream_ptr
         self._capi, self._stream_ptr = _capi, _stream_ptr
         self._s = None
         if hessian not in HESSIANS:
             raise ValueError(f"hessian must be one of {HESSIANS}, got {hessian!r}")
+        if precond not in PRECONDS:
+            raise ValueError(f"precond must be one of {PRECONDS}, got {precond!r}")
         if hessian == "psd" and torch.cuda.is_current_stream_capturing():
             raise RuntimeError('DevicePCG(hessian="psd") allocates device memory and cannot be created during a CUDA graph capture')
-        self.tet_sp, self.hessian = tet_sp, hessian
+        if precond == "sgs" and torch.cuda.is_current_stream_capturing():
+            raise RuntimeError('DevicePCG(precond="sgs") allocates device memory and cannot be created during a CUDA graph capture')
+        self.tet_sp, self.hessian, self.precond = tet_sp, hessian, precond
+        self.hessian_ws = None
         s = C.c_void_p()
         rc = _capi.lib.tsb_pcg_create(tet_sp._h, C.byref(s))
         if rc:
@@ -165,6 +176,14 @@ class DevicePCG:
         if hessian == "psd":
             rc = _capi.lib.tsb_pcg_enable_psd(s, tet_sp.vertices.ctypes.data, tet_sp.elements.ctypes.data, int(tet_sp.nele))
             self._check(rc, "__init__")
+        if precond == "sgs":
+            import weakref
+            from .hessian import DeviceHessian
+            self.hessian_ws = DeviceHessian(self)
+            # the workspace owns its Hessian workspace; a weak link back keeps the pair out of a reference cycle, which
+            # the garbage collector could otherwise free (cudaFree) in the middle of a later CUDA graph capture
+            self.hessian_ws.pcg = weakref.proxy(self)
+            self._check(_capi.lib.tsb_pcg_enable_sgs(s, self.hessian_ws._hs), "__init__")
         self.device_bytes = int(_capi.lib.tsb_pcg_device_bytes(s))
 
     def __del__(self):
@@ -244,6 +263,60 @@ class DevicePCG:
         self._check(rc, "solve")
         f = self._capi.record_fields(raw, self._capi.tsb_pcg_sphere_t)
         return DevicePCGResult(d=d, iters_run=int(iters.value), **{k: f[k] for k in DevicePCGResult._fields if k in f})
+
+    def _need_sgs(self, what: str) -> None:
+        if self.precond != "sgs":
+            raise RuntimeError(f'DevicePCG.{what} needs a workspace created with precond="sgs"')
+
+    def set_matrix(self, x: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0,
+                   out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Assembles the Hessian at ``x`` (exact, or projected with ``hessian="psd"``) into the workspace's matrix, from
+        which the symmetric Gauss-Seidel sweep reads its off-diagonal blocks (``tsb_pcg_set_matrix``), and returns its
+        diagonal blocks as ``hess_diag``'s [2, n, 3] planes, to hand to ``set_blocks`` (with or without a shift).
+        ``out``: a contiguous float32 tensor of 6n entries, overwritten and returned (then capturable)."""
+        self._need_sgs("set_matrix")
+        n, dev = self.tet_sp.n, self.tet_sp.device
+        xc = self._f32(x, self.tet_sp.n3, "x")
+        if out is None:
+            out = torch.empty((2, n, 3), dtype=torch.float32, device=dev)
+        elif self._f32(out, 6 * n, "out") is not out:
+            raise RuntimeError("out must be contiguous")
+        terms = self._capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
+        rc = self._capi.lib.tsb_pcg_set_matrix(self._s, xc.data_ptr(), C.byref(terms), out.data_ptr(), self._stream_ptr(dev))
+        self._check(rc, "set_matrix")
+        return out
+
+    def apply_precond(self, r: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``M^-1 r`` on every sphere with the symmetric Gauss-Seidel preconditioner of the last ``set_matrix`` and
+        ``set_blocks`` (``tsb_pcg_apply_precond``), in ``r``'s shape; 0 on vertices no tet references.  ``out`` (not
+        ``r``): a contiguous float32 tensor of 3n entries, returned (then no allocation)."""
+        self._need_sgs("apply_precond")
+        n3 = self.tet_sp.n3
+        rc_ = self._f32(r, n3, "r")
+        if out is None:
+            out = torch.zeros_like(rc_)
+        elif self._f32(out, n3, "out") is not out:
+            raise RuntimeError("out must be contiguous")
+        rc = self._capi.lib.tsb_pcg_apply_precond(self._s, rc_.data_ptr(), out.data_ptr(), self._stream_ptr(self.tet_sp.device))
+        self._check(rc, "apply_precond")
+        return out.reshape(r.shape)
+
+    @property
+    def colors(self) -> torch.Tensor:
+        """int32 [n]: the colour of every vertex in the sweep's order (-1 for vertices no tet references)."""
+        self._need_sgs("colors")
+        out = torch.empty(self.tet_sp.n, dtype=torch.int32, device=self.tet_sp.device)
+        torch.cuda.synchronize(self.tet_sp.device)
+        self._check(self._capi.lib.tsb_pcg_sgs_colors(self._s, out.data_ptr(), None), "colors")
+        return out
+
+    @property
+    def n_colors(self) -> int:
+        """The most colours any sphere uses."""
+        self._need_sgs("n_colors")
+        k = C.c_int32(0)
+        self._check(self._capi.lib.tsb_pcg_sgs_colors(self._s, None, C.byref(k)), "n_colors")
+        return int(k.value)
 
     def hvp_psd(self, x: torch.Tensor, v: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0):
         """``H+(x) v`` of ``c1 * smooth + c2 * barrier (+ c3 * amips)`` with every tet's Hessian projected to PSD at ``x``
@@ -352,22 +425,29 @@ class DeviceNewton:
     the same handle) or creates one, and keeps it alive.  Every sphere runs its own Levenberg-Marquardt iteration;
     ``reset`` starts them all again.  Serves one stream at a time, like the handle.  ``hessian``: the solve's model,
     ``"exact"`` or ``"psd"`` (the projected Hessian, see ``DevicePCG``); ``None`` takes ``pcg``'s, or ``"exact"`` when a
-    workspace is created.  A given ``pcg`` of another mode is an error."""
+    workspace is created.  A given ``pcg`` of another mode is an error.  ``precond`` follows the same rules: ``"jacobi"``
+    or ``"sgs"`` (see ``DevicePCG``); on an SGS workspace every step assembles the Hessian and takes its preconditioner
+    diagonal from it."""
 
-    def __init__(self, tet_sp, pcg: Optional[DevicePCG] = None, hessian: Optional[str] = None):
+    def __init__(self, tet_sp, pcg: Optional[DevicePCG] = None, hessian: Optional[str] = None,
+                 precond: Optional[str] = None):
         from . import _capi
         from .tet_spheres_ext import _stream_ptr
         self._capi, self._stream_ptr = _capi, _stream_ptr
         self._nw = None
         if hessian is not None and hessian not in HESSIANS:
             raise ValueError(f"hessian must be one of {HESSIANS}, got {hessian!r}")
+        if precond is not None and precond not in PRECONDS:
+            raise ValueError(f"precond must be one of {PRECONDS}, got {precond!r}")
         if pcg is None:
-            pcg = DevicePCG(tet_sp, hessian=hessian or "exact")
+            pcg = DevicePCG(tet_sp, hessian=hessian or "exact", precond=precond or "jacobi")
         elif pcg.tet_sp is not tet_sp:
             raise RuntimeError("DeviceNewton: pcg belongs to another handle")
         elif hessian is not None and pcg.hessian != hessian:
             raise RuntimeError(f"DeviceNewton: hessian={hessian!r} but pcg was created with hessian={pcg.hessian!r}")
-        self.hessian = pcg.hessian
+        elif precond is not None and pcg.precond != precond:
+            raise RuntimeError(f"DeviceNewton: precond={precond!r} but pcg was created with precond={pcg.precond!r}")
+        self.hessian, self.precond = pcg.hessian, pcg.precond
         self.tet_sp, self.pcg, self.n_spheres = tet_sp, pcg, pcg.n_spheres
         nw = C.c_void_p()
         rc = _capi.lib.tsb_newton_create(pcg._s, C.byref(nw))
