@@ -94,7 +94,12 @@ struct tsb_hessian_s {
 
 namespace {
 
-thread_local std::string g_create_err;
+// What *_last_error reports for a null object: the message of the last failed create of that kind on this thread
+template <class O>
+std::string &create_err() {
+  thread_local std::string msg;
+  return msg;
+}
 
 struct DeviceGuard {
   int prev = -1;
@@ -117,80 +122,82 @@ int device_of(const void *p) {
   return d;
 }
 
-int fail(tsb_handle_t h, int code, const std::string &msg) {
-  if (h) h->err = msg; else g_create_err = msg;
+// The error path of every object kind (tsb_handle_t and the workspaces): the message goes to the object, or for a null
+// object to its kind's creation error.
+template <class O>
+int fail(O *o, int code, const std::string &msg) {
+  (o ? o->err : create_err<O>()) = msg;
   return code;
 }
 
-// Copies src to a new device array of at least min_elems elements and points dst (the kernel's typed view of
-// the data, e.g. float4 over 4 floats) at it.
-template <class T, class A, class D>
-int upload(tsb_handle_t h, const std::vector<T, A> &src, D *&dst, size_t min_elems = 1) {
-  const size_t bytes = std::max(src.size(), min_elems) * sizeof(T);
+int64_t &device_bytes(tsb_handle_t h) { return h->info.device_bytes; }
+template <class W>
+int64_t &device_bytes(W *w) { return w->device_bytes; }
+
+// what a failed initialisation of a new device array reports: the handle names the call
+std::string init_error(tsb_handle_t, bool copy) { return copy ? "cudaMemcpy: " : "cudaMemset: "; }
+template <class W>
+std::string init_error(W *, bool) { return "workspace initialisation: "; }
+
+// A device array of max(elems, n_src) elements of T owned by o: counted in its device bytes, freed by its destroy.  It
+// holds src[0, n_src) when src is set (the rest uninitialised), else zeros when zero is set, else whatever was there.
+// out is the kernel's typed view of the data (e.g. float4 over 4 floats).
+template <class O, class D, class T = D>
+int device_array(O *o, D *&out, size_t elems, const T *src = nullptr, size_t n_src = 0, bool zero = true) {
+  const size_t bytes = std::max(elems, n_src) * sizeof(T);
   void *d = nullptr;
   cudaError_t e = cudaMalloc(&d, bytes);
-  if (e != cudaSuccess) return fail(h, TSB_E_NOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e));
-  h->allocs.push_back(d);
-  h->info.device_bytes += int64_t(bytes);
-  if (!src.empty()) {
-    e = cudaMemcpy(d, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) return fail(h, TSB_E_CUDA, std::string("cudaMemcpy: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(o, TSB_E_NOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e));
+  o->allocs.push_back(d);
+  device_bytes(o) += int64_t(bytes);
+  if (src && n_src) e = cudaMemcpy(d, src, n_src * sizeof(T), cudaMemcpyHostToDevice);
+  else if (!src && zero) e = cudaMemset(d, 0, bytes);
+  if (e != cudaSuccess) return fail(o, TSB_E_CUDA, init_error(o, src != nullptr) + cudaGetErrorString(e));
+  out = static_cast<D *>(d);
+  return TSB_OK;
+}
+
+// Marks o's allocations and device bytes; unless commit() is called, going out of scope rolls them back.  With destroy
+// (a create), it destroys the new object instead, keeping its message as the creation error.
+template <class O>
+class Rollback {
+ public:
+  explicit Rollback(O *o, void (*destroy)(O *) = nullptr)
+      : o_(o), destroy_(destroy), allocs_(o->allocs.size()), bytes_(device_bytes(o)) {}
+  ~Rollback() {
+    if (committed_) return;
+    if (destroy_) {
+      create_err<O>() = o_->err;
+      destroy_(o_);
+      return;
+    }
+    for (size_t k = allocs_; k < o_->allocs.size(); ++k) cudaFree(o_->allocs[k]);
+    o_->allocs.resize(allocs_);
+    device_bytes(o_) = bytes_;
   }
-  dst = static_cast<D *>(d);
-  return TSB_OK;
-}
+  void commit() { committed_ = true; }
 
-template <class T>
-int alloc_zero(tsb_handle_t h, size_t elems, T **out) {
-  const size_t bytes = std::max<size_t>(elems, 1) * sizeof(T);
-  void *d = nullptr;
-  cudaError_t e = cudaMalloc(&d, bytes);
-  if (e != cudaSuccess) return fail(h, TSB_E_NOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e));
-  h->allocs.push_back(d);
-  h->info.device_bytes += int64_t(bytes);
-  e = cudaMemset(d, 0, bytes);
-  if (e != cudaSuccess) return fail(h, TSB_E_CUDA, std::string("cudaMemset: ") + cudaGetErrorString(e));
-  *out = static_cast<T *>(d);
-  return TSB_OK;
-}
+ private:
+  O *o_;
+  void (*destroy_)(O *);
+  size_t allocs_;
+  int64_t bytes_;
+  bool committed_ = false;
+};
 
-// the same for a solver workspace (tsb_pcg_t) ...
-thread_local std::string g_pcg_create_err;
-
-int pcg_fail(tsb_pcg_t s, int code, const std::string &msg) {
-  if (s) s->err = msg; else g_pcg_create_err = msg;
-  return code;
-}
-
-// ... and a Newton workspace (tsb_newton_t)
-thread_local std::string g_newton_create_err;
-
-int newton_fail(tsb_newton_t nw, int code, const std::string &msg) {
-  if (nw) nw->err = msg; else g_newton_create_err = msg;
-  return code;
-}
-
-// ... and a Hessian workspace (tsb_hessian_t)
-thread_local std::string g_hessian_create_err;
-
-int hessian_fail(tsb_hessian_t hs, int code, const std::string &msg) {
-  if (hs) hs->err = msg; else g_hessian_create_err = msg;
-  return code;
-}
-
-// Device array of a workspace (tsb_pcg_t, tsb_newton_t or tsb_hessian_t): copied from src, or zeroed
-template <class T, class W>
-int ws_alloc(W *s, size_t elems, const T *src, T **out) {
-  const size_t bytes = elems * sizeof(T);
-  void *d = nullptr;
-  cudaError_t e = cudaMalloc(&d, bytes);
-  if (e != cudaSuccess) { s->err = std::string("cudaMalloc: ") + cudaGetErrorString(e); return TSB_E_NOMEM; }
-  s->allocs.push_back(d);
-  s->device_bytes += int64_t(bytes);
-  e = src ? cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice) : cudaMemset(d, 0, bytes);
-  if (e != cudaSuccess) { s->err = std::string("workspace initialisation: ") + cudaGetErrorString(e); return TSB_E_CUDA; }
-  *out = static_cast<T *>(d);
-  return TSB_OK;
+// TSB_OK unless st is being captured, which is refused with `refusal`.  The legacy stream cannot be queried while another
+// stream is being captured, so that counts as a capture too; any other stream that cannot be queried is TSB_E_CUDA.
+template <class O>
+int refuse_capture(O *o, cudaStream_t st, const char *refusal) {
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  const bool queried = cudaStreamIsCapturing(st, &cap) == cudaSuccess;
+  if (st == cudaStreamLegacy) {
+    if (queried && cap == cudaStreamCaptureStatusNone) return TSB_OK;
+    cudaGetLastError();
+    return fail(o, TSB_E_INVALID, refusal);
+  }
+  if (!queried) { cudaGetLastError(); return fail(o, TSB_E_CUDA, "cannot query the stream"); }
+  return cap == cudaStreamCaptureStatusNone ? TSB_OK : fail(o, TSB_E_INVALID, refusal);
 }
 
 // Device array of a workspace that a call allocates on its first use, of max(elems, 1) elements (zero: cleared on st).
@@ -198,20 +205,14 @@ int ws_alloc(W *s, size_t elems, const T *src, T **out) {
 template <class T, class W>
 int alloc_once(W *s, size_t elems, T **out, cudaStream_t st, const char *refusal, bool zero = false) {
   if (*out) return TSB_OK;
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  if (cudaStreamIsCapturing(st, &cap) != cudaSuccess) { cudaGetLastError(); s->err = "cannot query the stream"; return TSB_E_CUDA; }
-  if (cap != cudaStreamCaptureStatusNone) { s->err = refusal; return TSB_E_INVALID; }
-  const size_t bytes = std::max<size_t>(elems, 1) * sizeof(T);
-  void *d = nullptr;
-  cudaError_t e = cudaMalloc(&d, bytes);
-  if (e != cudaSuccess) { s->err = std::string("cudaMalloc: ") + cudaGetErrorString(e); return TSB_E_NOMEM; }
-  s->allocs.push_back(d);
-  s->device_bytes += int64_t(bytes);
-  if (zero && (e = cudaMemsetAsync(d, 0, bytes, st)) != cudaSuccess) {
-    s->err = std::string("cudaMemsetAsync: ") + cudaGetErrorString(e);
-    return TSB_E_CUDA;
+  int rc = refuse_capture(s, st, refusal);
+  if (rc == TSB_OK) rc = device_array(s, *out, std::max<size_t>(elems, 1), static_cast<const T *>(nullptr), 0, false);
+  if (rc != TSB_OK || !zero) return rc;
+  const cudaError_t e = cudaMemsetAsync(*out, 0, std::max<size_t>(elems, 1) * sizeof(T), st);
+  if (e != cudaSuccess) {
+    *out = nullptr;
+    return fail(s, TSB_E_CUDA, std::string("cudaMemsetAsync: ") + cudaGetErrorString(e));
   }
-  *out = static_cast<T *>(d);
   return TSB_OK;
 }
 
@@ -232,7 +233,7 @@ extern "C" {
 
 int tsb_create(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele, const tsb_options_t *opt,
                int device, tsb_handle_t *out) {
-  if (!out) return fail(nullptr, TSB_E_INVALID, "out is null");
+  if (!out) return fail<tsb_handle_s>(nullptr, TSB_E_INVALID, "out is null");
   *out = nullptr;
   tsb::PlanConfig pc;
   int nw = 16, ring = 2;
@@ -245,8 +246,8 @@ int tsb_create(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t ne
     pc.enable_amips = opt->enable_amips ? 1 : 0;
     pc.deterministic = opt->deterministic ? 1 : 0;
   }
-  if (nw != 8 && nw != 16) return fail(nullptr, TSB_E_INVALID, "warps_per_cta must be 8 or 16");
-  if (ring < 2 || ring > 8) return fail(nullptr, TSB_E_INVALID, "ring_slots must be in [2, 8]");
+  if (nw != 8 && nw != 16) return fail<tsb_handle_s>(nullptr, TSB_E_INVALID, "warps_per_cta must be 8 or 16");
+  if (ring < 2 || ring > 8) return fail<tsb_handle_s>(nullptr, TSB_E_INVALID, "ring_slots must be in [2, 8]");
   pc.nw = nw;
   pc.ring_cells = ring * tsb::kCellsPerChunk;   // the requested ring, also when the callback below shrinks it
   const int cpc = tsb::kCellsPerChunk;
@@ -254,14 +255,14 @@ int tsb_create(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t ne
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev) {
     cudaGetLastError();
-    return fail(nullptr, TSB_E_CUDA, "no CUDA device " + std::to_string(device) + " (tssplat_b200 has no CPU path)");
+    return fail<tsb_handle_s>(nullptr, TSB_E_CUDA, "no CUDA device " + std::to_string(device) + " (tssplat_b200 has no CPU path)");
   }
   DeviceGuard guard(device);
-  if (!guard.ok) return fail(nullptr, TSB_E_CUDA, "cannot select CUDA device " + std::to_string(device));
+  if (!guard.ok) return fail<tsb_handle_s>(nullptr, TSB_E_CUDA, "cannot select CUDA device " + std::to_string(device));
   int sms = 0, smem_optin = 0;
   if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || sms <= 0 ||
       cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device) != cudaSuccess)
-    return fail(nullptr, TSB_E_CUDA, "cannot query the CUDA device");
+    return fail<tsb_handle_s>(nullptr, TSB_E_CUDA, "cannot query the CUDA device");
   pc.area_cap = std::min(tsb::kMaxStagedVerts, std::max(0, (smem_optin - tsb::energy_smem_bytes(nw, 2, cpc, 0, false) - 256) / 32));
 
   // Called by the plan builder once the component sizes are known: pick the ring size that lets the
@@ -290,63 +291,70 @@ int tsb_create(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t ne
   tsb::HostPlan plan;
   std::string err;
   int rc = tsb::build_plan(rest_xyz, tets, n, nele, pc, plan, err);
-  if (rc != TSB_OK) return fail(nullptr, rc, err);
+  if (rc != TSB_OK) return fail<tsb_handle_s>(nullptr, rc, err);
 
   tsb_handle_t h = new tsb_handle_s();
   h->device = device;
   tsb::KParams &kp = h->kp;
-#define TSB_TRY(expr) do { rc = (expr); if (rc != TSB_OK) { g_create_err = h->err; tsb_destroy(h); return rc; } } while (0)
-  TSB_TRY(upload(h, plan.stream, kp.stream, 16));
-  TSB_TRY(upload(h, plan.X4, kp.X4, 4));
-  TSB_TRY(upload(h, plan.segs, kp.segs));
-  TSB_TRY(upload(h, plan.cta_seg, kp.cta_seg, 2));
-  TSB_TRY(upload(h, plan.wdesc, kp.wdesc, 2));
-  TSB_TRY(upload(h, plan.wseg, kp.wseg, 2));
-  TSB_TRY(upload(h, plan.vlist, kp.vlist));
-  TSB_TRY(upload(h, plan.pos16, kp.pos16, 2));
-  TSB_TRY(upload(h, plan.pos_gid, kp.pos_gid));
-  TSB_TRY(upload(h, plan.orphans, kp.orphans));
+  Rollback<tsb_handle_s> undo(h, tsb_destroy);
+  // the plan's tables (at least min_elems elements) and zeroed scratch (at least one element), until one fails
+  auto up = [&](const auto &src, auto *&dst, size_t min_elems = 1) {
+    if (rc == TSB_OK) rc = device_array(h, dst, min_elems, src.data(), src.size(), false);
+  };
+  auto zero = [&](size_t elems, auto *&dst) {
+    if (rc == TSB_OK) rc = device_array(h, dst, std::max<size_t>(elems, 1));
+  };
+  up(plan.stream, kp.stream, 16);
+  up(plan.X4, kp.X4, 4);
+  up(plan.segs, kp.segs);
+  up(plan.cta_seg, kp.cta_seg, 2);
+  up(plan.wdesc, kp.wdesc, 2);
+  up(plan.wseg, kp.wseg, 2);
+  up(plan.vlist, kp.vlist);
+  up(plan.pos16, kp.pos16, 2);
+  up(plan.pos_gid, kp.pos_gid);
+  up(plan.orphans, kp.orphans);
   if (pc.enable_amips) {
-    TSB_TRY(upload(h, plan.Bt, kp.Bt, 4));
-    TSB_TRY(upload(h, plan.wtc0, kp.wtc0));
+    up(plan.Bt, kp.Bt, 4);
+    up(plan.wtc0, kp.wtc0);
   }
   if (pc.deterministic) {
     // 48 B of corner vectors per tet slot, 8 B of ballot per tet cell, the vertex lists (16 B per tet) and their rows
     const size_t slots = size_t(plan.n_tetcells) * (plan.mode_global ? 32 : 64);
     tsb::DetParams &dp = h->dp;
-    if (!pc.enable_amips) TSB_TRY(upload(h, plan.wtc0, kp.wtc0));
-    TSB_TRY(alloc_zero(h, slots * 3, &kp.det_scratch));
-    TSB_TRY(alloc_zero(h, size_t(plan.n_tetcells), &kp.det_ballot));
-    TSB_TRY(alloc_zero(h, size_t(plan.n_components), &kp.det_flag));
-    TSB_TRY(upload(h, plan.det_rowptr, dp.rowptr));
-    TSB_TRY(upload(h, plan.det_vert, dp.vert));
-    TSB_TRY(upload(h, plan.det_comp_row, dp.comp_row));
-    TSB_TRY(upload(h, plan.det_ent, dp.ent));
-    TSB_TRY(upload(h, plan.det_chunk, dp.chunk, 2));
+    if (!pc.enable_amips) up(plan.wtc0, kp.wtc0);
+    zero(slots * 3, kp.det_scratch);
+    zero(size_t(plan.n_tetcells), kp.det_ballot);
+    zero(size_t(plan.n_components), kp.det_flag);
+    up(plan.det_rowptr, dp.rowptr);
+    up(plan.det_vert, dp.vert);
+    up(plan.det_comp_row, dp.comp_row);
+    up(plan.det_ent, dp.ent);
+    up(plan.det_chunk, dp.chunk, 2);
     dp.scratch = kp.det_scratch;
     dp.ballot = kp.det_ballot;
     dp.flag = kp.det_flag;
     dp.n_chunks = int32_t(plan.det_chunk.size() / 2);
     dp.tpl_log = plan.mode_global ? 0 : 1;
   }
-  TSB_TRY(alloc_zero(h, size_t(plan.n_components), &kp.done));
+  zero(size_t(plan.n_components), kp.done);
   // per-sphere statistics: 12 B per component of tables, 32 B per (segment, warp) of records
-  TSB_TRY(upload(h, plan.comp_seg, h->sp.comp_seg));
-  TSB_TRY(upload(h, plan.comp_first_vertex, h->sp.comp_first_vertex));
-  TSB_TRY(upload(h, plan.comp_ntets, h->sp.comp_ntets));
-  TSB_TRY(alloc_zero(h, plan.segs.size() * size_t(nw), &kp.sph_rec));
+  up(plan.comp_seg, h->sp.comp_seg);
+  up(plan.comp_first_vertex, h->sp.comp_first_vertex);
+  up(plan.comp_ntets, h->sp.comp_ntets);
+  zero(plan.segs.size() * size_t(nw), kp.sph_rec);
   h->sp.rec = kp.sph_rec;
   h->sp.n_components = plan.n_components;
   h->sp.nw = nw;
-  TSB_TRY(upload(h, std::vector<unsigned long long>(size_t(plan.grid) * 4, tsb::kEnergySentinel), kp.cta_energy, 2));
+  up(std::vector<unsigned long long>(size_t(plan.grid) * 4, tsb::kEnergySentinel), kp.cta_energy, 2);
 #ifdef TSB_TRACE
-  TSB_TRY(alloc_zero(h, size_t(plan.grid) * tsb::kTraceSlots, &kp.trace));
+  zero(size_t(plan.grid) * tsb::kTraceSlots, kp.trace);
 #endif
   if (plan.mode_global) {
-    TSB_TRY(alloc_zero(h, size_t(plan.n), &kp.u4g));
-    TSB_TRY(alloc_zero(h, size_t(plan.n), &kp.x4g));
+    zero(size_t(plan.n), kp.u4g);
+    zero(size_t(plan.n), kp.x4g);
   }
-#undef TSB_TRY
+  if (rc != TSB_OK) return rc;
   kp.n_orphans = int32_t(plan.orphans.size());
   kp.n_components = plan.n_components;
   kp.n = plan.n;
@@ -371,6 +379,7 @@ int tsb_create(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t ne
   for (const tsb::SegHdr &s : plan.segs) staged += s.nv;
   I.stream_bytes = int64_t(plan.stream.size()) + (plan.mode_global ? int64_t(plan.n) * (12 + 16 + 64) : staged * (16 + 12 + 2)) +
                    int64_t(plan.n) * 12 + int64_t(plan.segs.size()) * 32 + int64_t(plan.grid) * (16 + 8 * nw);
+  undo.commit();
   *out = h;
   return TSB_OK;
 }
@@ -387,7 +396,7 @@ void tsb_destroy(tsb_handle_t h) {
   delete h;
 }
 
-const char *tsb_last_error(tsb_handle_t h) { return h ? h->err.c_str() : g_create_err.c_str(); }
+const char *tsb_last_error(tsb_handle_t h) { return h ? h->err.c_str() : create_err<tsb_handle_s>().c_str(); }
 
 int tsb_get_info(tsb_handle_t h, tsb_info_t *info) {
   if (!h || !info) return TSB_E_INVALID;
@@ -554,11 +563,11 @@ int tsb_hess_diag(tsb_handle_t h, const float *x_dev, const tsb_terms_t *terms, 
 /* ---- Newton-CG solve (tsb_solver.cu) ---- */
 
 int tsb_pcg_create(tsb_handle_t h, tsb_pcg_t *out) {
-  if (!out) return pcg_fail(nullptr, TSB_E_INVALID, "out is null");
+  if (!out) return fail<tsb_pcg_s>(nullptr, TSB_E_INVALID, "out is null");
   *out = nullptr;
-  if (!h) return pcg_fail(nullptr, TSB_E_INVALID, "handle is null");
+  if (!h) return fail<tsb_pcg_s>(nullptr, TSB_E_INVALID, "handle is null");
   DeviceGuard guard(h->device);
-  if (!guard.ok) return pcg_fail(nullptr, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  if (!guard.ok) return fail<tsb_pcg_s>(nullptr, TSB_E_CUDA, "cannot select the handle's CUDA device");
   tsb::PcgLists L;
   tsb::build_pcg_lists(h->comp_label, h->info.n_components, L);
   tsb_pcg_t s = new tsb_pcg_s();
@@ -566,33 +575,27 @@ int tsb_pcg_create(tsb_handle_t h, tsb_pcg_t *out) {
   s->device = h->device;
   tsb::PcgParams &P = s->P;
   const size_t n = size_t(h->info.n), n3 = 3 * n;
-  int32_t *vert = nullptr, *comp_chunk = nullptr, *chunk = nullptr;
-  int rc = TSB_OK;
-#define TSB_TRY(expr) do { rc = (expr); if (rc != TSB_OK) { g_pcg_create_err = s->err; tsb_pcg_destroy(s); return rc; } } while (0)
-  TSB_TRY(ws_alloc(s, L.vert.size(), L.vert.data(), &vert));
-  TSB_TRY(ws_alloc(s, L.comp_chunk.size(), L.comp_chunk.data(), &comp_chunk));
-  TSB_TRY(ws_alloc(s, L.chunk.size(), L.chunk.data(), &chunk));
-  TSB_TRY(ws_alloc<float>(s, n3, nullptr, &P.r));
-  TSB_TRY(ws_alloc<float>(s, n3, nullptr, &P.z));
-  TSB_TRY(ws_alloc<float>(s, n3, nullptr, &P.p));     // zero on vertices no tet references, and stays so
-  TSB_TRY(ws_alloc<float>(s, n3, nullptr, &P.Hp));
-  TSB_TRY(ws_alloc<float>(s, 2 * n3, nullptr, &P.pinv));
-  TSB_TRY(ws_alloc<double>(s, 3 * (L.chunk.size() / 3), nullptr, &P.part));
-  TSB_TRY(ws_alloc<tsb::PcgComp>(s, size_t(h->info.n_components), nullptr, &P.comp));
-  TSB_TRY(ws_alloc<int32_t>(s, 1, nullptr, &P.active));
-#undef TSB_TRY
-  P.vert = vert; P.comp_chunk = comp_chunk; P.chunk = chunk;
+  Rollback<tsb_pcg_s> undo(s, tsb_pcg_destroy);
+  int rc = device_array(s, P.vert, 0, L.vert.data(), L.vert.size());
+  if (rc == TSB_OK) rc = device_array(s, P.comp_chunk, 0, L.comp_chunk.data(), L.comp_chunk.size());
+  if (rc == TSB_OK) rc = device_array(s, P.chunk, 0, L.chunk.data(), L.chunk.size());
+  if (rc == TSB_OK) rc = device_array(s, P.r, n3);
+  if (rc == TSB_OK) rc = device_array(s, P.z, n3);
+  if (rc == TSB_OK) rc = device_array(s, P.p, n3);     // zero on vertices no tet references, and stays so
+  if (rc == TSB_OK) rc = device_array(s, P.Hp, n3);
+  if (rc == TSB_OK) rc = device_array(s, P.pinv, 2 * n3);
+  if (rc == TSB_OK) rc = device_array(s, P.part, 3 * (L.chunk.size() / 3));
+  if (rc == TSB_OK) rc = device_array(s, P.comp, size_t(h->info.n_components));
+  if (rc == TSB_OK) rc = device_array(s, P.active, 1);
+  if (rc != TSB_OK) return rc;
   P.orphans = h->kp.orphans; P.n_orphans = h->kp.n_orphans;
   P.n_chunks = int32_t(L.chunk.size() / 3); P.n_components = h->info.n_components; P.n = h->info.n;
   cudaError_t e = cudaMallocHost(reinterpret_cast<void **>(&s->active_host), sizeof(int32_t));
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->ev, cudaEventDisableTiming);
   if (e == cudaSuccess) e = tsb::launch_pcg_blocks(P, nullptr, 0.f, nullptr, nullptr);     // identity preconditioner
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
-  if (e != cudaSuccess) {
-    pcg_fail(nullptr, TSB_E_CUDA, std::string("tsb_pcg_create: ") + cudaGetErrorString(e));
-    tsb_pcg_destroy(s);
-    return TSB_E_CUDA;
-  }
+  if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("tsb_pcg_create: ") + cudaGetErrorString(e));
+  undo.commit();
   *out = s;
   return TSB_OK;
 }
@@ -606,7 +609,7 @@ void tsb_pcg_destroy(tsb_pcg_t s) {
   delete s;
 }
 
-const char *tsb_pcg_last_error(tsb_pcg_t s) { return s ? s->err.c_str() : g_pcg_create_err.c_str(); }
+const char *tsb_pcg_last_error(tsb_pcg_t s) { return s ? s->err.c_str() : create_err<tsb_pcg_s>().c_str(); }
 
 int64_t tsb_pcg_device_bytes(tsb_pcg_t s) { return s ? s->device_bytes : 0; }
 
@@ -617,13 +620,13 @@ int tsb_pcg_set_blocks(tsb_pcg_t s, const float *diag_dev, float rel_floor, floa
 int tsb_pcg_set_blocks_ex(tsb_pcg_t s, const float *diag_dev, float rel_floor, const float *shift_dev, float *inv_out_dev,
                           void *stream) {
   if (!s) return TSB_E_INVALID;
-  if (!(rel_floor >= 0.f)) return pcg_fail(s, TSB_E_INVALID, "rel_floor must be >= 0");
+  if (!(rel_floor >= 0.f)) return fail(s, TSB_E_INVALID, "rel_floor must be >= 0");
   DeviceGuard guard(s->h->device);
-  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  if (!guard.ok) return fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   const cudaError_t e = diag_dev && shift_dev ? tsb::launch_pcg_blocks_shift(s->P, diag_dev, rel_floor, shift_dev, inv_out_dev, st)
                                               : tsb::launch_pcg_blocks(s->P, diag_dev, rel_floor, inv_out_dev, st);
-  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("preconditioner launch: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("preconditioner launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 
@@ -636,16 +639,16 @@ namespace {
 int psd_product(tsb_pcg_t s, const float *x_dev, const float *v_dev, const tsb_terms_t &t, float *hv, float *curv,
                 cudaStream_t st) {
   const int rc = hvp_impl(s->h, x_dev, v_dev, t.c1, 0.f, 0.f, t.order, 1.f, nullptr, hv, curv ? s->Q.curv_m : nullptr, 1, st);
-  if (rc != TSB_OK) return pcg_fail(s, rc, s->h->err);
+  if (rc != TSB_OK) return fail(s, rc, s->h->err);
   cudaError_t e = tsb::launch_psd_apply(s->Q, v_dev, t.c2, t.c3, curv != nullptr, hv, st);
   if (e == cudaSuccess && curv) e = tsb::launch_psd_curv(s->Q, t.c1, t.c2, t.c3, curv, st);
-  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("projected product launch: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("projected product launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 
 int psd_project(tsb_pcg_t s, const float *x_dev, const tsb_terms_t &t, cudaStream_t st) {
   const cudaError_t e = tsb::launch_psd_project(s->Q, x_dev, t.order, t.c3 != 0.f ? 1 : 0, st);
-  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("projection launch: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("projection launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 
@@ -655,75 +658,36 @@ extern "C" {
 
 int tsb_pcg_enable_psd(tsb_pcg_t s, const float *rest_xyz, const int32_t *tets, int32_t nele) {
   if (!s) return TSB_E_INVALID;
-  if (s->psd) return pcg_fail(s, TSB_E_INVALID, "the projected Hessian is already enabled on this workspace");
-  if (!rest_xyz || !tets) return pcg_fail(s, TSB_E_INVALID, "rest_xyz and tets must be non-null");
+  if (s->psd) return fail(s, TSB_E_INVALID, "the projected Hessian is already enabled on this workspace");
+  if (!rest_xyz || !tets) return fail(s, TSB_E_INVALID, "rest_xyz and tets must be non-null");
   const tsb_handle_t h = s->h;
   if (nele != h->info.nele)
-    return pcg_fail(s, TSB_E_INVALID, "nele = " + std::to_string(nele) + " but the handle has " + std::to_string(h->info.nele) + " tets");
+    return fail(s, TSB_E_INVALID, "nele = " + std::to_string(nele) + " but the handle has " + std::to_string(h->info.nele) + " tets");
   DeviceGuard guard(h->device);
-  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  if (cudaStreamIsCapturing(cudaStreamLegacy, &cap) != cudaSuccess || cap != cudaStreamCaptureStatusNone) {
-    cudaGetLastError();
-    return pcg_fail(s, TSB_E_INVALID, "tsb_pcg_enable_psd allocates device memory and cannot run while a stream is being captured");
-  }
+  if (!guard.ok) return fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  int rc = refuse_capture(s, cudaStreamLegacy, "tsb_pcg_enable_psd allocates device memory and cannot run while a stream is being captured");
+  if (rc != TSB_OK) return rc;
   const int32_t n = h->info.n;
   const size_t ne = size_t(nele);
-  // the mesh: every vertex in range, every tet inside one component, B = Dm^-1 in fp64 stored as fp32 (row-major, one
-  // array per entry)
-  std::vector<float> B(9 * ne);
-  std::vector<int32_t> cnt(size_t(n) + 1, 0);
-  for (size_t t = 0; t < ne; ++t) {
-    const int32_t *q = tets + 4 * t;
-    for (int k = 0; k < 4; ++k)
-      if (q[k] < 0 || q[k] >= n)
-        return pcg_fail(s, TSB_E_MESH, "tet " + std::to_string(t) + " has vertex " + std::to_string(q[k]) + " outside [0, " + std::to_string(n) + ")");
-    const int32_t c = h->comp_label[size_t(q[0])];
-    if (c < 0 || h->comp_label[size_t(q[1])] != c || h->comp_label[size_t(q[2])] != c || h->comp_label[size_t(q[3])] != c)
-      return pcg_fail(s, TSB_E_MESH, "tet " + std::to_string(t) + " spans two components of the handle: not the mesh it was created from");
-    double D[3][3];
-    for (int k = 0; k < 3; ++k)
-      for (int r = 0; r < 3; ++r)
-        D[r][k] = double(rest_xyz[3 * size_t(q[k + 1]) + r]) - double(rest_xyz[3 * size_t(q[0]) + r]);
-    const double c00 = D[1][1] * D[2][2] - D[1][2] * D[2][1], c01 = D[1][2] * D[2][0] - D[1][0] * D[2][2],
-                 c02 = D[1][0] * D[2][1] - D[1][1] * D[2][0];
-    const double det = D[0][0] * c00 + D[0][1] * c01 + D[0][2] * c02;
-    if (!(std::fabs(det) > 0.0) || !std::isfinite(det))
-      return pcg_fail(s, TSB_E_MESH, "tet " + std::to_string(t) + " has a zero-volume or non-finite rest shape");
-    const double inv[3][3] = {
-        {c00 / det, (D[0][2] * D[2][1] - D[0][1] * D[2][2]) / det, (D[0][1] * D[1][2] - D[0][2] * D[1][1]) / det},
-        {c01 / det, (D[0][0] * D[2][2] - D[0][2] * D[2][0]) / det, (D[0][2] * D[1][0] - D[0][0] * D[1][2]) / det},
-        {c02 / det, (D[0][1] * D[2][0] - D[0][0] * D[2][1]) / det, (D[0][0] * D[1][1] - D[0][1] * D[1][0]) / det}};
-    for (int k = 0; k < 9; ++k) B[size_t(k) * ne + t] = float(inv[k / 3][k % 3]);
-    for (int k = 0; k < 4; ++k) ++cnt[size_t(q[k]) + 1];
-  }
-  // per-vertex incidence lists of 4 tet + corner, ascending (a counting sort over ascending entries keeps the order)
-  for (size_t v = 0; v < size_t(n); ++v) cnt[v + 1] += cnt[v];
-  std::vector<int32_t> inc(4 * ne), fill(cnt.begin(), cnt.end() - 1);
-  for (size_t t = 0; t < ne; ++t)
-    for (int k = 0; k < 4; ++k) inc[size_t(fill[size_t(tets[4 * t + k])]++)] = int32_t(4 * t + k);
+  // the mesh: every vertex in range, every tet inside one component, B = Dm^-1 in fp64 stored as fp32
+  tsb::TetTables T;
+  std::string err;
+  rc = tsb::build_tet_tables(rest_xyz, tets, n, nele, &h->comp_label, T, err);
+  if (rc != TSB_OK) return fail(s, rc, err);
   tsb::PsdParams Q{};
   Q.nele = nele; Q.n = n; Q.n_blocks = int32_t((ne + tsb::kPsdT - 1) / tsb::kPsdT);
-  const size_t allocs0 = s->allocs.size();
-  const int64_t bytes0 = s->device_bytes;
-  int32_t *tets_dev = nullptr, *inc_ptr = nullptr, *inc_dev = nullptr;
-  float *B_dev = nullptr;
-  int rc = ws_alloc(s, 4 * ne, tets, &tets_dev);
-  if (rc == TSB_OK) rc = ws_alloc(s, 9 * ne, B.data(), &B_dev);
-  if (rc == TSB_OK) rc = ws_alloc<float>(s, tsb::kPsdOpFloats * ne, nullptr, &Q.op);
-  if (rc == TSB_OK) rc = ws_alloc<uint8_t>(s, ne, nullptr, &Q.kind);
-  if (rc == TSB_OK) rc = ws_alloc<float>(s, 12 * ne, nullptr, &Q.corner);
-  if (rc == TSB_OK) rc = ws_alloc(s, cnt.size(), cnt.data(), &inc_ptr);
-  if (rc == TSB_OK) rc = ws_alloc(s, inc.size(), inc.data(), &inc_dev);
-  if (rc == TSB_OK) rc = ws_alloc<double>(s, 2 * size_t(Q.n_blocks), nullptr, &Q.part);
-  if (rc == TSB_OK) rc = ws_alloc<float>(s, 4, nullptr, &Q.curv_m);
-  if (rc != TSB_OK) {            // leave the workspace as it was
-    for (size_t k = allocs0; k < s->allocs.size(); ++k) cudaFree(s->allocs[k]);
-    s->allocs.resize(allocs0);
-    s->device_bytes = bytes0;
-    return rc;
-  }
-  Q.tets = reinterpret_cast<const int4 *>(tets_dev); Q.B = B_dev; Q.inc_ptr = inc_ptr; Q.inc = inc_dev;
+  Rollback<tsb_pcg_s> undo(s);
+  rc = device_array(s, Q.tets, 0, T.tets.data(), T.tets.size());
+  if (rc == TSB_OK) rc = device_array(s, Q.B, 0, T.B.data(), T.B.size());
+  if (rc == TSB_OK) rc = device_array(s, Q.op, tsb::kPsdOpFloats * ne);
+  if (rc == TSB_OK) rc = device_array(s, Q.kind, ne);
+  if (rc == TSB_OK) rc = device_array(s, Q.corner, 12 * ne);
+  if (rc == TSB_OK) rc = device_array(s, Q.inc_ptr, 0, T.inc_ptr.data(), T.inc_ptr.size());
+  if (rc == TSB_OK) rc = device_array(s, Q.inc, 0, T.inc.data(), T.inc.size());
+  if (rc == TSB_OK) rc = device_array(s, Q.part, 2 * size_t(Q.n_blocks));
+  if (rc == TSB_OK) rc = device_array(s, Q.curv_m, 4);
+  if (rc != TSB_OK) return rc;       // the rollback leaves the workspace as it was
+  undo.commit();
   s->Q = Q;
   s->psd = true;
   return TSB_OK;
@@ -732,13 +696,13 @@ int tsb_pcg_enable_psd(tsb_pcg_t s, const float *rest_xyz, const int32_t *tets, 
 int tsb_pcg_hvp_psd(tsb_pcg_t s, const float *x_dev, const float *v_dev, const tsb_terms_t *terms, float *hv_out_dev,
                     float *curv_out_dev, void *stream) {
   if (!s) return TSB_E_INVALID;
-  if (!s->psd) return pcg_fail(s, TSB_E_INVALID, "tsb_pcg_hvp_psd needs a workspace after tsb_pcg_enable_psd");
-  if (!x_dev || !v_dev || !terms || !hv_out_dev) return pcg_fail(s, TSB_E_INVALID, "x_dev, v_dev, terms and hv_out_dev must be non-null");
+  if (!s->psd) return fail(s, TSB_E_INVALID, "tsb_pcg_hvp_psd needs a workspace after tsb_pcg_enable_psd");
+  if (!x_dev || !v_dev || !terms || !hv_out_dev) return fail(s, TSB_E_INVALID, "x_dev, v_dev, terms and hv_out_dev must be non-null");
   if (hv_out_dev == v_dev || hv_out_dev == x_dev)
-    return pcg_fail(s, TSB_E_INVALID, "hv_out_dev must not be x_dev or v_dev: hv is written before v and x are read for the last time");
-  if (const char *m = check_terms(s->h, true, *terms)) return pcg_fail(s, TSB_E_INVALID, m);
+    return fail(s, TSB_E_INVALID, "hv_out_dev must not be x_dev or v_dev: hv is written before v and x are read for the last time");
+  if (const char *m = check_terms(s->h, true, *terms)) return fail(s, TSB_E_INVALID, m);
   DeviceGuard guard(s->h->device);
-  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  if (!guard.ok) return fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   int rc = psd_project(s, x_dev, *terms, st);
   if (rc == TSB_OK) rc = psd_product(s, x_dev, v_dev, *terms, hv_out_dev, curv_out_dev, st);
@@ -759,19 +723,17 @@ int pcg_solve_impl(tsb_pcg_t s, const float *x_dev, const float *b_dev, const ts
                    const float *shift_dev, const float *radius_dev, float *d_out_dev, tsb_pcg_sphere_t *spheres_out_dev,
                    int32_t *iters_run_out, void *stream) {
   if (!x_dev || !b_dev || !d_out_dev || !terms || !opt)
-    return pcg_fail(s, TSB_E_INVALID, "x_dev, b_dev, d_out_dev, terms and opt must be non-null");
-  if (opt->max_iter < 1) return pcg_fail(s, TSB_E_INVALID, "max_iter must be >= 1");
-  if (!(opt->rtol >= 0.f)) return pcg_fail(s, TSB_E_INVALID, "rtol must be >= 0");
-  if (opt->check_every < 0) return pcg_fail(s, TSB_E_INVALID, "check_every must be >= 0");
-  if (const char *m = check_terms(s->h, s->psd, *terms)) return pcg_fail(s, TSB_E_INVALID, m);
+    return fail(s, TSB_E_INVALID, "x_dev, b_dev, d_out_dev, terms and opt must be non-null");
+  if (opt->max_iter < 1) return fail(s, TSB_E_INVALID, "max_iter must be >= 1");
+  if (!(opt->rtol >= 0.f)) return fail(s, TSB_E_INVALID, "rtol must be >= 0");
+  if (opt->check_every < 0) return fail(s, TSB_E_INVALID, "check_every must be >= 0");
+  if (const char *m = check_terms(s->h, s->psd, *terms)) return fail(s, TSB_E_INVALID, m);
   DeviceGuard guard(s->h->device);
-  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  if (!guard.ok) return fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (opt->check_every > 0) {          // the termination check waits on the host: not possible inside a stream capture
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    if (cudaStreamIsCapturing(st, &cap) != cudaSuccess) { cudaGetLastError(); return pcg_fail(s, TSB_E_CUDA, "cannot query the stream"); }
-    if (cap != cudaStreamCaptureStatusNone)
-      return pcg_fail(s, TSB_E_INVALID, "check_every > 0 reads the host and cannot be captured in a CUDA graph: use check_every = 0");
+    const int rc = refuse_capture(s, st, "check_every > 0 reads the host and cannot be captured in a CUDA graph: use check_every = 0");
+    if (rc != TSB_OK) return rc;
   }
   if (radius_dev) {     // the recurrence state: the dir kernel of iteration 0 writes it before any kernel reads it
     const int rc = alloc_once(s, size_t(s->P.n_components), &s->tr, st,
@@ -788,7 +750,7 @@ int pcg_solve_impl(tsb_pcg_t s, const float *x_dev, const float *b_dev, const ts
   }
   const tsb::SgsParams *sgs = s->sgs ? &s->G : nullptr;
   cudaError_t e = tsb::launch_pcg_begin(P, b_dev, d_out_dev, tr, st, sgs);
-  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver launch: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("solver launch: ") + cudaGetErrorString(e));
   int32_t it = 0;
   while (it < opt->max_iter) {
     if (s->psd) {
@@ -796,24 +758,24 @@ int pcg_solve_impl(tsb_pcg_t s, const float *x_dev, const float *b_dev, const ts
       if (rc != TSB_OK) return rc;
     } else {
       const int rc = hvp_impl(s->h, x_dev, P.p, terms->c1, terms->c2, terms->c3, terms->order, 1.f, nullptr, P.Hp, nullptr, 1, st);
-      if (rc != TSB_OK) return pcg_fail(s, rc, s->h->err);
+      if (rc != TSB_OK) return fail(s, rc, s->h->err);
     }
     e = tsb::launch_pcg_step(P, d_out_dev, it, opt->rtol, shift_dev, tr, st, sgs);
-    if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver launch: ") + cudaGetErrorString(e));
+    if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("solver launch: ") + cudaGetErrorString(e));
     ++it;
     if (opt->check_every > 0 && it % opt->check_every == 0 && it < opt->max_iter) {
       e = tsb::launch_pcg_count(P, st);
       if (e == cudaSuccess) e = cudaMemcpyAsync(s->active_host, P.active, sizeof(int32_t), cudaMemcpyDeviceToHost, st);
       if (e == cudaSuccess) e = cudaEventRecord(s->ev, st);
       if (e == cudaSuccess) e = cudaEventSynchronize(s->ev);
-      if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver termination check: ") + cudaGetErrorString(e));
+      if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("solver termination check: ") + cudaGetErrorString(e));
       if (*s->active_host == 0) break;
     }
   }
   if (iters_run_out) *iters_run_out = it;
   if (spheres_out_dev) {
     e = tsb::launch_pcg_records(P, b_dev, d_out_dev, spheres_out_dev, st);
-    if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("solver record launch: ") + cudaGetErrorString(e));
+    if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("solver record launch: ") + cudaGetErrorString(e));
   }
   return TSB_OK;
 }
@@ -833,7 +795,7 @@ int tsb_pcg_solve_tr(tsb_pcg_t s, const float *x_dev, const float *b_dev, const 
                      const float *shift_dev, const float *radius_dev, float *d_out_dev, tsb_pcg_sphere_t *spheres_out_dev,
                      int32_t *iters_run_out, void *stream) {
   if (!s) return TSB_E_INVALID;
-  if (!radius_dev) return pcg_fail(s, TSB_E_INVALID, "radius_dev must be non-null");
+  if (!radius_dev) return fail(s, TSB_E_INVALID, "radius_dev must be non-null");
   return pcg_solve_impl(s, x_dev, b_dev, terms, opt, shift_dev, radius_dev, d_out_dev, spheres_out_dev, iters_run_out, stream);
 }
 
@@ -841,22 +803,22 @@ int tsb_sphere_axpy(tsb_pcg_t s, const float *x_dev, const float *a_sphere_dev, 
                     void *stream) {
   if (!s) return TSB_E_INVALID;
   if (!x_dev || !a_sphere_dev || !d_dev || !out_dev)
-    return pcg_fail(s, TSB_E_INVALID, "x_dev, a_sphere_dev, d_dev and out_dev must be non-null");
+    return fail(s, TSB_E_INVALID, "x_dev, a_sphere_dev, d_dev and out_dev must be non-null");
   DeviceGuard guard(s->h->device);
-  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  if (!guard.ok) return fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
   const cudaError_t e = tsb::launch_sphere_axpy(s->P, x_dev, a_sphere_dev, d_dev, out_dev, static_cast<cudaStream_t>(stream));
-  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("sphere axpy launch: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("sphere axpy launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 
 /* ---- Damped Newton step (tsb_solver.cu) ---- */
 
 int tsb_newton_create(tsb_pcg_t s, tsb_newton_t *out) {
-  if (!out) return newton_fail(nullptr, TSB_E_INVALID, "out is null");
+  if (!out) return fail<tsb_newton_s>(nullptr, TSB_E_INVALID, "out is null");
   *out = nullptr;
-  if (!s) return newton_fail(nullptr, TSB_E_INVALID, "solver workspace is null");
+  if (!s) return fail<tsb_newton_s>(nullptr, TSB_E_INVALID, "solver workspace is null");
   DeviceGuard guard(s->h->device);
-  if (!guard.ok) return newton_fail(nullptr, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  if (!guard.ok) return fail<tsb_newton_s>(nullptr, TSB_E_CUDA, "cannot select the handle's CUDA device");
   tsb_newton_t nw = new tsb_newton_s();
   nw->s = s;
   nw->device = s->h->device;
@@ -864,23 +826,21 @@ int tsb_newton_create(tsb_pcg_t s, tsb_newton_t *out) {
   const size_t n3 = 3 * size_t(s->P.n), S = size_t(s->P.n_components), K = TSB_LINE_MAX_ALPHA;
   std::vector<float> alphas(K);
   for (size_t k = 0; k < K; ++k) alphas[k] = std::ldexp(1.f, -int(k));
-  float *alphas_dev = nullptr;
-  int rc = TSB_OK;
-#define TSB_TRY(expr) do { rc = (expr); if (rc != TSB_OK) { g_newton_create_err = nw->err; tsb_newton_destroy(nw); return rc; } } while (0)
-  TSB_TRY(ws_alloc<float>(nw, n3, nullptr, &W.b));
-  TSB_TRY(ws_alloc<float>(nw, n3, nullptr, &W.d));
-  TSB_TRY(ws_alloc<float>(nw, 2 * n3, nullptr, &W.diag));
-  TSB_TRY(ws_alloc<float>(nw, S, nullptr, &W.shift));
-  TSB_TRY(ws_alloc<float>(nw, S, nullptr, &W.alpha_sphere));
-  TSB_TRY(ws_alloc<float>(nw, K, alphas.data(), &alphas_dev));
-  TSB_TRY(ws_alloc<float>(nw, S * K * 4, nullptr, &W.sphere_delta));
-  TSB_TRY(ws_alloc<float>(nw, S, nullptr, &W.sphere_step));
-  TSB_TRY(ws_alloc<double>(nw, 3 * size_t(s->P.n_chunks), nullptr, &W.part));
-  TSB_TRY(ws_alloc<tsb::NewtonComp>(nw, S, nullptr, &W.comp));     // zero: ACTIVE, mu not initialised
-  TSB_TRY(ws_alloc<float>(nw, 4, nullptr, &nw->energy));
-  TSB_TRY(ws_alloc<float>(nw, K * 4, nullptr, &nw->delta));
-#undef TSB_TRY
-  W.alphas = alphas_dev;
+  Rollback<tsb_newton_s> undo(nw, tsb_newton_destroy);
+  int rc = device_array(nw, W.b, n3);
+  if (rc == TSB_OK) rc = device_array(nw, W.d, n3);
+  if (rc == TSB_OK) rc = device_array(nw, W.diag, 2 * n3);
+  if (rc == TSB_OK) rc = device_array(nw, W.shift, S);
+  if (rc == TSB_OK) rc = device_array(nw, W.alpha_sphere, S);
+  if (rc == TSB_OK) rc = device_array(nw, W.alphas, 0, alphas.data(), K);
+  if (rc == TSB_OK) rc = device_array(nw, W.sphere_delta, S * K * 4);
+  if (rc == TSB_OK) rc = device_array(nw, W.sphere_step, S);
+  if (rc == TSB_OK) rc = device_array(nw, W.part, 3 * size_t(s->P.n_chunks));
+  if (rc == TSB_OK) rc = device_array(nw, W.comp, S);     // zero: ACTIVE, mu not initialised
+  if (rc == TSB_OK) rc = device_array(nw, nw->energy, 4);
+  if (rc == TSB_OK) rc = device_array(nw, nw->delta, K * 4);
+  if (rc != TSB_OK) return rc;
+  undo.commit();
   *out = nw;
   return TSB_OK;
 }
@@ -892,18 +852,18 @@ void tsb_newton_destroy(tsb_newton_t nw) {
   delete nw;
 }
 
-const char *tsb_newton_last_error(tsb_newton_t nw) { return nw ? nw->err.c_str() : g_newton_create_err.c_str(); }
+const char *tsb_newton_last_error(tsb_newton_t nw) { return nw ? nw->err.c_str() : create_err<tsb_newton_s>().c_str(); }
 
 int64_t tsb_newton_device_bytes(tsb_newton_t nw) { return nw ? nw->device_bytes : 0; }
 
 int tsb_newton_reset(tsb_newton_t nw, void *stream) {
   if (!nw) return TSB_E_INVALID;
   DeviceGuard guard(nw->s->h->device);
-  if (!guard.ok) return newton_fail(nw, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  if (!guard.ok) return fail(nw, TSB_E_CUDA, "cannot select the handle's CUDA device");
   const size_t S = size_t(nw->s->P.n_components);
   cudaError_t e = cudaMemsetAsync(nw->W.comp, 0, S * sizeof(tsb::NewtonComp), static_cast<cudaStream_t>(stream));
   if (e == cudaSuccess && nw->tr_state) e = cudaMemsetAsync(nw->tr_state, 0, S * sizeof(tsb::TrState), static_cast<cudaStream_t>(stream));
-  if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("reset: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(nw, TSB_E_CUDA, std::string("reset: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 
@@ -934,22 +894,22 @@ std::string rule_error(const tsb_newton_tr_options_t &o) {
 template <class O>
 int newton_check(tsb_newton_t nw, const float *x_dev, const float *anchor_dev, const float *weight_dev, const tsb_terms_t *terms,
                  const O *opt) {
-  if (!x_dev || !terms || !opt) return newton_fail(nw, TSB_E_INVALID, "x_dev, terms and opt must be non-null");
+  if (!x_dev || !terms || !opt) return fail(nw, TSB_E_INVALID, "x_dev, terms and opt must be non-null");
   if (!anchor_dev != !weight_dev)
-    return newton_fail(nw, TSB_E_INVALID, "anchor_dev and weight_dev must be both null (objective E) or both set (proximal objective)");
+    return fail(nw, TSB_E_INVALID, "anchor_dev and weight_dev must be both null (objective E) or both set (proximal objective)");
   if (anchor_dev && anchor_dev == x_dev)
-    return newton_fail(nw, TSB_E_INVALID, "anchor_dev must not be x_dev: x is updated in place while the anchor is read");
+    return fail(nw, TSB_E_INVALID, "anchor_dev must not be x_dev: x is updated in place while the anchor is read");
   const O &o = *opt;
-  if (o.max_iter < 1) return newton_fail(nw, TSB_E_INVALID, "max_iter must be >= 1");
-  if (!(o.rtol >= 0.f)) return newton_fail(nw, TSB_E_INVALID, "rtol must be >= 0");
-  if (!(o.rel_floor >= 0.f)) return newton_fail(nw, TSB_E_INVALID, "rel_floor must be >= 0");
-  if (!(o.gtol >= 0.f)) return newton_fail(nw, TSB_E_INVALID, "gtol must be >= 0");
-  if (!(o.eta > 0.f && o.eta <= 1.f)) return newton_fail(nw, TSB_E_INVALID, "eta must be in (0, 1]");
+  if (o.max_iter < 1) return fail(nw, TSB_E_INVALID, "max_iter must be >= 1");
+  if (!(o.rtol >= 0.f)) return fail(nw, TSB_E_INVALID, "rtol must be >= 0");
+  if (!(o.rel_floor >= 0.f)) return fail(nw, TSB_E_INVALID, "rel_floor must be >= 0");
+  if (!(o.gtol >= 0.f)) return fail(nw, TSB_E_INVALID, "gtol must be >= 0");
+  if (!(o.eta > 0.f && o.eta <= 1.f)) return fail(nw, TSB_E_INVALID, "eta must be in (0, 1]");
   for (int32_t r : o.reserved)
-    if (r != 0) return newton_fail(nw, TSB_E_INVALID, "reserved fields must be 0");
+    if (r != 0) return fail(nw, TSB_E_INVALID, "reserved fields must be 0");
   const std::string rule = rule_error(o);
-  if (!rule.empty()) return newton_fail(nw, TSB_E_INVALID, rule);
-  if (const char *m = check_terms(nw->s->h, nw->s->psd, *terms)) return newton_fail(nw, TSB_E_INVALID, m);
+  if (!rule.empty()) return fail(nw, TSB_E_INVALID, rule);
+  if (const char *m = check_terms(nw->s->h, nw->s->psd, *terms)) return fail(nw, TSB_E_INVALID, m);
   return TSB_OK;
 }
 
@@ -986,7 +946,7 @@ int newton_run(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const flo
   tsb_pcg_t s = nw->s;
   tsb_handle_t h = s->h;
   DeviceGuard guard(h->device);
-  if (!guard.ok) return newton_fail(nw, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  if (!guard.ok) return fail(nw, TSB_E_CUDA, "cannot select the handle's CUDA device");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   const char *refusal = k.damped ? "the first tsb_newton_prox_step of a workspace allocates device memory and cannot be "
                                    "captured in a CUDA graph: make one call outside any capture first"
@@ -1003,7 +963,7 @@ int newton_run(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const flo
   if (rc != TSB_OK) return rc;
   if (!k.damped) {      // the solve's recurrence state, as a first tsb_pcg_solve_tr allocates it
     rc = alloc_once(s, S, &s->tr, st, refusal);
-    if (rc != TSB_OK) return newton_fail(nw, rc, s->err);
+    if (rc != TSB_OK) return fail(nw, rc, s->err);
   }
   const tsb::NewtonParams &W = nw->W;
   const tsb::ProxParams pp{x_dev, anchor_dev, weight_dev, nw->prox_part};
@@ -1013,37 +973,37 @@ int newton_run(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const flo
   const float *shift = k.damped ? W.shift : weight_dev;
   // b = -grad, the diagonal blocks; frozen spheres' b = 0 (prox: b -= w (x - y)); damped: mu on a first step
   rc = energy_grad_impl(h, x_dev, terms->c1, terms->c2, terms->c3, terms->order, -1.f, nullptr, nw->energy, 1, W.b, nullptr, st);
-  if (rc != TSB_OK) return newton_fail(nw, rc, h->err);
+  if (rc != TSB_OK) return fail(nw, rc, h->err);
   if (s->sgs) {         // the diagonal blocks of the matrix the sweep uses
     rc = tsb_pcg_set_matrix(s, x_dev, terms, W.diag, st);
-    if (rc != TSB_OK) return newton_fail(nw, rc, s->err);
+    if (rc != TSB_OK) return fail(nw, rc, s->err);
   } else {
     rc = tsb_hess_diag(h, x_dev, terms, 1.f, nullptr, W.diag, st);
-    if (rc != TSB_OK) return newton_fail(nw, rc, h->err);
+    if (rc != TSB_OK) return fail(nw, rc, h->err);
   }
   cudaError_t e = tsb::launch_newton_prep(s->P, W, prox, st);
   if (e == cudaSuccess && k.damped) e = tsb::launch_newton_shift(s->P, W, k.lm, prox, st);
-  if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
   // the preconditioner; trust region: the radius on a first step
   rc = tsb_pcg_set_blocks_ex(s, W.diag, k.rel_floor, shift, nullptr, st);
-  if (rc != TSB_OK) return newton_fail(nw, rc, s->err);
+  if (rc != TSB_OK) return fail(nw, rc, s->err);
   if (!k.damped) {
     e = tsb::launch_newton_tr_radius(s->P, W, T, k.tr, st, s->sgs ? &s->G : nullptr);
-    if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
+    if (e != cudaSuccess) return fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
   }
   // the solve
   rc = pcg_solve_impl(s, x_dev, W.b, terms, &k.po, shift, k.damped ? nullptr : nw->tr_radius, W.d, nullptr, nullptr, st);
-  if (rc != TSB_OK) return newton_fail(nw, rc, s->err);
+  if (rc != TSB_OK) return fail(nw, rc, s->err);
   // b.d and |d|^2 (prox: and d.(x - y)) per chunk; the line search at 2^-k, k < n_alpha, per sphere
   e = tsb::launch_newton_dots(s->P, W, prox, st);
-  if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
   rc = tsb_line_search(h, x_dev, W.d, terms, W.alphas, k.n_alpha, nw->delta, nullptr, W.sphere_delta, W.sphere_step, st);
-  if (rc != TSB_OK) return newton_fail(nw, rc, h->err);
+  if (rc != TSB_OK) return fail(nw, rc, h->err);
   // decision, step
   e = k.damped ? tsb::launch_newton_decide(s->P, W, k.lm, prox, k.lm_out, st)
                : tsb::launch_newton_tr_decide(s->P, W, T, k.tr, prox, k.backtrack ? &k.bt : nullptr, k.tr_out, st);
   if (e == cudaSuccess) e = tsb::launch_sphere_axpy(s->P, x_dev, W.alpha_sphere, W.d, x_dev, st);
-  if (e != cudaSuccess) return newton_fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 
@@ -1063,7 +1023,7 @@ int tsb_newton_prox_step(tsb_newton_t nw, float *x_dev, const float *anchor_dev,
                          const tsb_terms_t *terms, const tsb_newton_options_t *opt, tsb_newton_sphere_t *records_out_dev,
                          void *stream) {
   if (!nw) return TSB_E_INVALID;
-  if (!anchor_dev || !weight_dev) return newton_fail(nw, TSB_E_INVALID, "anchor_dev and weight_dev must be non-null");
+  if (!anchor_dev || !weight_dev) return fail(nw, TSB_E_INVALID, "anchor_dev and weight_dev must be non-null");
   const int rc = newton_check(nw, x_dev, anchor_dev, weight_dev, terms, opt);
   if (rc != TSB_OK) return rc;
   return newton_run(nw, x_dev, anchor_dev, weight_dev, terms, NewtonStep(*opt, records_out_dev), stream);
@@ -1082,10 +1042,10 @@ int tsb_newton_tr_step_ex(tsb_newton_t nw, float *x_dev, const float *anchor_dev
   if (rc != TSB_OK) return rc;
   if (bt) {
     if (bt->n_alpha < 2 || bt->n_alpha > TSB_LINE_MAX_ALPHA)
-      return newton_fail(nw, TSB_E_INVALID, "n_alpha must be in [2, " + std::to_string(TSB_LINE_MAX_ALPHA) + "]");
-    if (!(bt->sigma > 0.f && bt->sigma < 0.5f)) return newton_fail(nw, TSB_E_INVALID, "sigma must be in (0, 1/2)");
+      return fail(nw, TSB_E_INVALID, "n_alpha must be in [2, " + std::to_string(TSB_LINE_MAX_ALPHA) + "]");
+    if (!(bt->sigma > 0.f && bt->sigma < 0.5f)) return fail(nw, TSB_E_INVALID, "sigma must be in (0, 1/2)");
     for (int32_t r : bt->reserved)
-      if (r != 0) return newton_fail(nw, TSB_E_INVALID, "reserved fields must be 0");
+      if (r != 0) return fail(nw, TSB_E_INVALID, "reserved fields must be 0");
   }
   return newton_run(nw, x_dev, anchor_dev, weight_dev, terms, NewtonStep(*opt, bt, records_out_dev), stream);
 }
@@ -1093,26 +1053,27 @@ int tsb_newton_tr_step_ex(tsb_newton_t nw, float *x_dev, const float *anchor_dev
 /* ---- Assembled Hessian (tsb_hessian.cu) ---- */
 
 int tsb_hessian_create(tsb_pcg_t s, const float *rest_xyz, const int32_t *tets, int32_t nele, tsb_hessian_t *out) {
-  if (!out) return hessian_fail(nullptr, TSB_E_INVALID, "out is null");
+  if (!out) return fail<tsb_hessian_s>(nullptr, TSB_E_INVALID, "out is null");
   *out = nullptr;
-  if (!s) return hessian_fail(nullptr, TSB_E_INVALID, "solver workspace is null");
-  if (!rest_xyz || !tets) return hessian_fail(nullptr, TSB_E_INVALID, "rest_xyz and tets must be non-null");
+  if (!s) return fail<tsb_hessian_s>(nullptr, TSB_E_INVALID, "solver workspace is null");
+  if (!rest_xyz || !tets) return fail<tsb_hessian_s>(nullptr, TSB_E_INVALID, "rest_xyz and tets must be non-null");
   const tsb_handle_t h = s->h;
   if (nele != h->info.nele)
-    return hessian_fail(nullptr, TSB_E_INVALID, "nele = " + std::to_string(nele) + " but the handle has " + std::to_string(h->info.nele) + " tets");
+    return fail<tsb_hessian_s>(nullptr, TSB_E_INVALID, "nele = " + std::to_string(nele) + " but the handle has " + std::to_string(h->info.nele) + " tets");
   DeviceGuard guard(h->device);
-  if (!guard.ok) return hessian_fail(nullptr, TSB_E_CUDA, "cannot select the handle's CUDA device");
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  if (cudaStreamIsCapturing(cudaStreamLegacy, &cap) != cudaSuccess || cap != cudaStreamCaptureStatusNone) {
-    cudaGetLastError();
-    return hessian_fail(nullptr, TSB_E_INVALID, "tsb_hessian_create allocates device memory and cannot run while a stream is being captured");
-  }
+  if (!guard.ok) return fail<tsb_hessian_s>(nullptr, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  int rc = refuse_capture<tsb_hessian_s>(nullptr, cudaStreamLegacy,
+                                         "tsb_hessian_create allocates device memory and cannot run while a stream is being captured");
+  if (rc != TSB_OK) return rc;
   tsb::HessPattern H;
   std::string err;
-  int rc = tsb::build_hessian_pattern(rest_xyz, tets, h->info.n, nele, h->lap_scale, H, err);
-  if (rc != TSB_OK) return hessian_fail(nullptr, rc, err);
+  rc = tsb::build_hessian_pattern(rest_xyz, tets, h->info.n, nele, h->lap_scale, H, err);
+  if (rc != TSB_OK) return fail<tsb_hessian_s>(nullptr, rc, err);
   if (H.comp_label != h->comp_label || H.nnz != h->info.nnz)
-    return hessian_fail(nullptr, TSB_E_MESH, "the mesh's components or operator differ from the handle's: not the mesh it was created from");
+    return fail<tsb_hessian_s>(nullptr, TSB_E_MESH, "the mesh's components or operator differ from the handle's: not the mesh it was created from");
+  tsb::TetTables T;
+  rc = tsb::build_tet_tables(rest_xyz, tets, h->info.n, nele, nullptr, T, err);
+  if (rc != TSB_OK) return fail<tsb_hessian_s>(nullptr, rc, err);
   tsb_hessian_t hs = new tsb_hessian_s();
   hs->s = s;
   hs->device = h->device;
@@ -1120,34 +1081,26 @@ int tsb_hessian_create(tsb_pcg_t s, const float *rest_xyz, const int32_t *tets, 
   hs->nnzb = H.nnzb;
   tsb::HessParams &P = hs->P;
   const size_t ne = size_t(nele);
-  int32_t *crow = nullptr, *tblk = nullptr, *inc_ptr = nullptr, *inc = nullptr;
-  float *w = nullptr;
-#define TSB_TRY(expr) do { rc = (expr); if (rc != TSB_OK) { g_hessian_create_err = hs->err; tsb_hessian_destroy(hs); return rc; } } while (0)
-  TSB_TRY(ws_alloc(hs, H.crow.size(), H.crow.data(), &crow));
-  TSB_TRY(ws_alloc(hs, H.col.size(), H.col.data(), &hs->col));
-  TSB_TRY(ws_alloc(hs, H.w.size(), H.w.data(), &w));
-  TSB_TRY(ws_alloc(hs, H.tblk.size(), H.tblk.data(), &tblk));
-  TSB_TRY(ws_alloc(hs, H.inc_ptr.size(), H.inc_ptr.data(), &inc_ptr));
-  TSB_TRY(ws_alloc(hs, H.inc.size(), H.inc.data(), &inc));
-  TSB_TRY(ws_alloc<uint8_t>(hs, ne, nullptr, &P.kind));
-  TSB_TRY(ws_alloc<float>(hs, ne * tsb::kHessTetFloats, nullptr, &P.blk));
+  Rollback<tsb_hessian_s> undo(hs, tsb_hessian_destroy);
+  rc = device_array(hs, hs->crow, 0, H.crow.data(), H.crow.size());
+  if (rc == TSB_OK) rc = device_array(hs, hs->col, 0, H.col.data(), H.col.size());
+  if (rc == TSB_OK) rc = device_array(hs, P.w, 0, H.w.data(), H.w.size());
+  if (rc == TSB_OK) rc = device_array(hs, P.tblk, 0, H.tblk.data(), H.tblk.size());
+  if (rc == TSB_OK) rc = device_array(hs, P.inc_ptr, 0, T.inc_ptr.data(), T.inc_ptr.size());
+  if (rc == TSB_OK) rc = device_array(hs, P.inc, 0, T.inc.data(), T.inc.size());
+  if (rc == TSB_OK) rc = device_array(hs, P.kind, ne);
+  if (rc == TSB_OK) rc = device_array(hs, P.blk, ne * tsb::kHessTetFloats);
   if (hs->psd) {                     // the projection's tets and rest inverses, a private operator
-    float *op = nullptr;
-    TSB_TRY(ws_alloc<float>(hs, ne * tsb::kPsdOpFloats, nullptr, &op));
-    P.op = op;
+    if (rc == TSB_OK) rc = device_array(hs, P.op, ne * tsb::kPsdOpFloats);
     P.tets = s->Q.tets;
     P.B = s->Q.B;
   } else {
-    int32_t *tets_dev = nullptr;
-    float *B = nullptr;
-    TSB_TRY(ws_alloc(hs, 4 * ne, tets, &tets_dev));
-    TSB_TRY(ws_alloc(hs, H.B.size(), H.B.data(), &B));
-    P.tets = reinterpret_cast<const int4 *>(tets_dev);
-    P.B = B;
+    if (rc == TSB_OK) rc = device_array(hs, P.tets, 0, T.tets.data(), T.tets.size());
+    if (rc == TSB_OK) rc = device_array(hs, P.B, 0, T.B.data(), T.B.size());
   }
-#undef TSB_TRY
-  hs->crow = crow;
-  P.crow = crow; P.w = w; P.tblk = tblk; P.inc_ptr = inc_ptr; P.inc = inc;
+  if (rc != TSB_OK) return rc;
+  undo.commit();
+  P.crow = hs->crow;
   P.n = h->info.n; P.nele = nele;
   *out = hs;
   return TSB_OK;
@@ -1160,7 +1113,7 @@ void tsb_hessian_destroy(tsb_hessian_t hs) {
   delete hs;
 }
 
-const char *tsb_hessian_last_error(tsb_hessian_t hs) { return hs ? hs->err.c_str() : g_hessian_create_err.c_str(); }
+const char *tsb_hessian_last_error(tsb_hessian_t hs) { return hs ? hs->err.c_str() : create_err<tsb_hessian_s>().c_str(); }
 
 int64_t tsb_hessian_device_bytes(tsb_hessian_t hs) { return hs ? hs->device_bytes : 0; }
 
@@ -1168,22 +1121,22 @@ int tsb_hessian_pattern(tsb_hessian_t hs, int64_t *nnzb, int32_t *crow_dev_out, 
   if (!hs) return TSB_E_INVALID;
   if (nnzb) *nnzb = hs->nnzb;
   DeviceGuard guard(hs->device);
-  if (!guard.ok) return hessian_fail(hs, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  if (!guard.ok) return fail(hs, TSB_E_CUDA, "cannot select the handle's CUDA device");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   cudaError_t e = cudaSuccess;
   if (crow_dev_out) e = cudaMemcpyAsync(crow_dev_out, hs->crow, (size_t(hs->P.n) + 1) * sizeof(int32_t), cudaMemcpyDeviceToDevice, st);
   if (e == cudaSuccess && col_dev_out)
     e = cudaMemcpyAsync(col_dev_out, hs->col, size_t(hs->nnzb) * sizeof(int32_t), cudaMemcpyDeviceToDevice, st);
-  if (e != cudaSuccess) return hessian_fail(hs, TSB_E_CUDA, std::string("pattern copy: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(hs, TSB_E_CUDA, std::string("pattern copy: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 
 int tsb_hessian_assemble(tsb_hessian_t hs, const float *x_dev, const tsb_terms_t *terms, float *values_dev, void *stream) {
   if (!hs) return TSB_E_INVALID;
-  if (!x_dev || !terms || !values_dev) return hessian_fail(hs, TSB_E_INVALID, "x_dev, terms and values_dev must be non-null");
-  if (const char *m = check_terms(hs->s->h, hs->psd, *terms)) return hessian_fail(hs, TSB_E_INVALID, m);
+  if (!x_dev || !terms || !values_dev) return fail(hs, TSB_E_INVALID, "x_dev, terms and values_dev must be non-null");
+  if (const char *m = check_terms(hs->s->h, hs->psd, *terms)) return fail(hs, TSB_E_INVALID, m);
   DeviceGuard guard(hs->device);
-  if (!guard.ok) return hessian_fail(hs, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  if (!guard.ok) return fail(hs, TSB_E_CUDA, "cannot select the handle's CUDA device");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   cudaError_t e = cudaSuccess;
   if (hs->psd) {                     // the workspace's projection kernel, into this workspace's operator and activity
@@ -1194,7 +1147,7 @@ int tsb_hessian_assemble(tsb_hessian_t hs, const float *x_dev, const tsb_terms_t
   }
   if (e == cudaSuccess) e = tsb::launch_hessian_blocks(hs->P, x_dev, terms->order, terms->c2, terms->c3, hs->psd, st);
   if (e == cudaSuccess) e = tsb::launch_hessian_gather(hs->P, terms->c1, values_dev, st);
-  if (e != cudaSuccess) return hessian_fail(hs, TSB_E_CUDA, std::string("hessian launch: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(hs, TSB_E_CUDA, std::string("hessian launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 
@@ -1202,22 +1155,19 @@ int tsb_hessian_assemble(tsb_hessian_t hs, const float *x_dev, const tsb_terms_t
 
 int tsb_pcg_enable_sgs(tsb_pcg_t s, tsb_hessian_t hs) {
   if (!s) return TSB_E_INVALID;
-  if (s->sgs) return pcg_fail(s, TSB_E_INVALID, "the symmetric Gauss-Seidel preconditioner is already enabled on this workspace");
-  if (!hs) return pcg_fail(s, TSB_E_INVALID, "hs is null");
-  if (hs->s != s) return pcg_fail(s, TSB_E_INVALID, "hs was created over another solver workspace");
+  if (s->sgs) return fail(s, TSB_E_INVALID, "the symmetric Gauss-Seidel preconditioner is already enabled on this workspace");
+  if (!hs) return fail(s, TSB_E_INVALID, "hs is null");
+  if (hs->s != s) return fail(s, TSB_E_INVALID, "hs was created over another solver workspace");
   const tsb_handle_t h = s->h;
   DeviceGuard guard(h->device);
-  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  if (cudaStreamIsCapturing(cudaStreamLegacy, &cap) != cudaSuccess || cap != cudaStreamCaptureStatusNone) {
-    cudaGetLastError();
-    return pcg_fail(s, TSB_E_INVALID, "tsb_pcg_enable_sgs allocates device memory and cannot run while a stream is being captured");
-  }
+  if (!guard.ok) return fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  int rc = refuse_capture(s, cudaStreamLegacy, "tsb_pcg_enable_sgs allocates device memory and cannot run while a stream is being captured");
+  if (rc != TSB_OK) return rc;
   const size_t n = size_t(h->info.n), S = size_t(s->P.n_components);
   std::vector<int32_t> crow(n + 1), col(size_t(hs->nnzb));
   cudaError_t e = cudaMemcpy(crow.data(), hs->crow, crow.size() * sizeof(int32_t), cudaMemcpyDeviceToHost);
   if (e == cudaSuccess && !col.empty()) e = cudaMemcpy(col.data(), hs->col, col.size() * sizeof(int32_t), cudaMemcpyDeviceToHost);
-  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("pattern download: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("pattern download: ") + cudaGetErrorString(e));
   tsb::PcgLists L;
   tsb::build_pcg_lists(h->comp_label, int32_t(S), L);
   int32_t big = 0;
@@ -1226,40 +1176,31 @@ int tsb_pcg_enable_sgs(tsb_pcg_t s, tsb_hessian_t hs) {
   const int32_t max_verts = S ? L.comp_off[size_t(big) + 1] - L.comp_off[size_t(big)] : 0;
   int limit = 0;
   e = tsb::sgs_configure(max_verts, &limit);
-  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("sweep configuration: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("sweep configuration: ") + cudaGetErrorString(e));
   if (max_verts > limit)
-    return pcg_fail(s, TSB_E_INVALID, "component " + std::to_string(big) + " has " + std::to_string(max_verts) +
-                                          " vertices; the sweep keeps a component's vector in one CTA's shared memory, at most " +
-                                          std::to_string(limit) + " vertices on this device");
+    return fail(s, TSB_E_INVALID, "component " + std::to_string(big) + " has " + std::to_string(max_verts) +
+                                      " vertices; the sweep keeps a component's vector in one CTA's shared memory, at most " +
+                                      std::to_string(limit) + " vertices on this device");
   tsb::SgsTables T;
   std::string err;
-  int rc = tsb::build_sgs_tables(crow, col, L, 0, T, err);
-  if (rc != TSB_OK) return pcg_fail(s, rc, err);
-  const size_t allocs0 = s->allocs.size();
-  const int64_t bytes0 = s->device_bytes;
+  rc = tsb::build_sgs_tables(crow, col, L, 0, T, err);
+  if (rc != TSB_OK) return fail(s, rc, err);
   tsb::SgsParams G{};
-  int32_t *comp_off = nullptr, *color_ptr = nullptr, *color_off = nullptr, *sched = nullptr, *lo_ptr = nullptr, *hi_ptr = nullptr,
-          *lo = nullptr, *hi = nullptr, *color = nullptr;
+  Rollback<tsb_pcg_s> undo(s);
   float *values = nullptr;
-  rc = ws_alloc<float>(s, 9 * std::max<size_t>(col.size(), 1), nullptr, &values);
-  if (rc == TSB_OK) rc = ws_alloc(s, L.comp_off.size(), L.comp_off.data(), &comp_off);
-  if (rc == TSB_OK) rc = ws_alloc(s, T.color_ptr.size(), T.color_ptr.data(), &color_ptr);
-  if (rc == TSB_OK) rc = ws_alloc(s, std::max<size_t>(T.color_off.size(), 1), T.color_off.empty() ? nullptr : T.color_off.data(), &color_off);
-  if (rc == TSB_OK) rc = ws_alloc(s, std::max<size_t>(T.sched.size(), 1), T.sched.empty() ? nullptr : T.sched.data(), &sched);
-  if (rc == TSB_OK) rc = ws_alloc(s, T.lo_ptr.size(), T.lo_ptr.data(), &lo_ptr);
-  if (rc == TSB_OK) rc = ws_alloc(s, T.hi_ptr.size(), T.hi_ptr.data(), &hi_ptr);
-  if (rc == TSB_OK) rc = ws_alloc(s, std::max<size_t>(T.lo.size(), 2), T.lo.empty() ? nullptr : T.lo.data(), &lo);
-  if (rc == TSB_OK) rc = ws_alloc(s, std::max<size_t>(T.hi.size(), 2), T.hi.empty() ? nullptr : T.hi.data(), &hi);
-  if (rc == TSB_OK) rc = ws_alloc(s, T.color.size(), T.color.data(), &color);
-  if (rc != TSB_OK) {            // leave the workspace as it was
-    for (size_t k = allocs0; k < s->allocs.size(); ++k) cudaFree(s->allocs[k]);
-    s->allocs.resize(allocs0);
-    s->device_bytes = bytes0;
-    return rc;
-  }
-  G.comp_off = comp_off; G.color_ptr = color_ptr; G.color_off = color_off; G.sched = sched;
-  G.lo_ptr = lo_ptr; G.hi_ptr = hi_ptr;
-  G.lo = reinterpret_cast<const int2 *>(lo); G.hi = reinterpret_cast<const int2 *>(hi);
+  int32_t *color = nullptr;
+  rc = device_array(s, values, 9 * std::max<size_t>(col.size(), 1));
+  if (rc == TSB_OK) rc = device_array(s, G.comp_off, 0, L.comp_off.data(), L.comp_off.size());
+  if (rc == TSB_OK) rc = device_array(s, G.color_ptr, 0, T.color_ptr.data(), T.color_ptr.size());
+  if (rc == TSB_OK) rc = device_array(s, G.color_off, 1, T.color_off.empty() ? nullptr : T.color_off.data(), T.color_off.size());
+  if (rc == TSB_OK) rc = device_array(s, G.sched, 1, T.sched.empty() ? nullptr : T.sched.data(), T.sched.size());
+  if (rc == TSB_OK) rc = device_array(s, G.lo_ptr, 0, T.lo_ptr.data(), T.lo_ptr.size());
+  if (rc == TSB_OK) rc = device_array(s, G.hi_ptr, 0, T.hi_ptr.data(), T.hi_ptr.size());
+  if (rc == TSB_OK) rc = device_array(s, G.lo, 2, T.lo.empty() ? nullptr : T.lo.data(), T.lo.size());
+  if (rc == TSB_OK) rc = device_array(s, G.hi, 2, T.hi.empty() ? nullptr : T.hi.data(), T.hi.size());
+  if (rc == TSB_OK) rc = device_array(s, color, 0, T.color.data(), T.color.size());
+  if (rc != TSB_OK) return rc;       // the rollback leaves the workspace as it was
+  undo.commit();
   G.values = values; G.crow = hs->crow; G.col = hs->col; G.max_verts = max_verts;
   s->G = G;
   s->sgs_values = values;
@@ -1271,40 +1212,40 @@ int tsb_pcg_enable_sgs(tsb_pcg_t s, tsb_hessian_t hs) {
 
 int tsb_pcg_set_matrix(tsb_pcg_t s, const float *x_dev, const tsb_terms_t *terms, float *diag_out_dev, void *stream) {
   if (!s) return TSB_E_INVALID;
-  if (!s->sgs) return pcg_fail(s, TSB_E_INVALID, "tsb_pcg_set_matrix needs a workspace after tsb_pcg_enable_sgs");
-  if (!x_dev || !terms || !diag_out_dev) return pcg_fail(s, TSB_E_INVALID, "x_dev, terms and diag_out_dev must be non-null");
+  if (!s->sgs) return fail(s, TSB_E_INVALID, "tsb_pcg_set_matrix needs a workspace after tsb_pcg_enable_sgs");
+  if (!x_dev || !terms || !diag_out_dev) return fail(s, TSB_E_INVALID, "x_dev, terms and diag_out_dev must be non-null");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int rc = tsb_hessian_assemble(s->sgs, x_dev, terms, s->sgs_values, st);
-  if (rc != TSB_OK) return pcg_fail(s, rc, s->sgs->err);
+  if (rc != TSB_OK) return fail(s, rc, s->sgs->err);
   DeviceGuard guard(s->h->device);
-  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  if (!guard.ok) return fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
   const cudaError_t e = tsb::launch_sgs_diag(s->G, s->P.n, diag_out_dev, st);
-  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("diagonal launch: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("diagonal launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 
 int tsb_pcg_apply_precond(tsb_pcg_t s, const float *r_dev, float *z_dev, void *stream) {
   if (!s) return TSB_E_INVALID;
-  if (!s->sgs) return pcg_fail(s, TSB_E_INVALID, "tsb_pcg_apply_precond needs a workspace after tsb_pcg_enable_sgs");
-  if (!r_dev || !z_dev) return pcg_fail(s, TSB_E_INVALID, "r_dev and z_dev must be non-null");
-  if (r_dev == z_dev) return pcg_fail(s, TSB_E_INVALID, "z_dev must not be r_dev: r is read after z is written");
+  if (!s->sgs) return fail(s, TSB_E_INVALID, "tsb_pcg_apply_precond needs a workspace after tsb_pcg_enable_sgs");
+  if (!r_dev || !z_dev) return fail(s, TSB_E_INVALID, "r_dev and z_dev must be non-null");
+  if (r_dev == z_dev) return fail(s, TSB_E_INVALID, "z_dev must not be r_dev: r is read after z is written");
   DeviceGuard guard(s->h->device);
-  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  if (!guard.ok) return fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
   const cudaError_t e = tsb::launch_sgs_sweep(s->P, s->G, tsb::SgsSweep{r_dev, z_dev, nullptr, 0, 0, -1, nullptr, nullptr},
                                               static_cast<cudaStream_t>(stream));
-  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("sweep launch: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("sweep launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 
 int tsb_pcg_sgs_colors(tsb_pcg_t s, int32_t *colors_out_dev, int32_t *n_colors_out) {
   if (!s) return TSB_E_INVALID;
-  if (!s->sgs) return pcg_fail(s, TSB_E_INVALID, "tsb_pcg_sgs_colors needs a workspace after tsb_pcg_enable_sgs");
+  if (!s->sgs) return fail(s, TSB_E_INVALID, "tsb_pcg_sgs_colors needs a workspace after tsb_pcg_enable_sgs");
   if (n_colors_out) *n_colors_out = s->sgs_n_colors;
   if (!colors_out_dev) return TSB_OK;
   DeviceGuard guard(s->h->device);
-  if (!guard.ok) return pcg_fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  if (!guard.ok) return fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
   const cudaError_t e = cudaMemcpy(colors_out_dev, s->sgs_color, size_t(s->P.n) * sizeof(int32_t), cudaMemcpyDeviceToDevice);
-  if (e != cudaSuccess) return pcg_fail(s, TSB_E_CUDA, std::string("colour copy: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("colour copy: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 
@@ -1319,9 +1260,9 @@ int tsb_energy_grad_host(tsb_handle_t h, const float *x_host, float c1, float c2
   if (!h->stage_x[0]) {
     int rc = TSB_OK;
     for (int k = 0; k < 2 && rc == TSB_OK; ++k) {
-      rc = alloc_zero(h, size_t(h->info.n) * 3, &h->stage_x[k]);
-      if (rc == TSB_OK) rc = alloc_zero(h, size_t(h->info.n) * 3, &h->stage_grad[k]);
-      if (rc == TSB_OK) rc = alloc_zero(h, 4, &h->stage_energy[k]);
+      rc = device_array(h, h->stage_x[k], size_t(h->info.n) * 3);
+      if (rc == TSB_OK) rc = device_array(h, h->stage_grad[k], size_t(h->info.n) * 3);
+      if (rc == TSB_OK) rc = device_array(h, h->stage_energy[k], 4);
     }
     if (rc != TSB_OK) return rc;
     cudaError_t e = cudaSuccess;
@@ -1381,32 +1322,32 @@ int tsb_energy_grad_host(tsb_handle_t h, const float *x_host, float c1, float c2
 }
 
 int tsb_scale(const float *g_dev, int64_t count, float gradH, const float *gradH_dev, float *out_dev, void *stream) {
-  if (!g_dev || !out_dev || count < 0) return fail(nullptr, TSB_E_INVALID, "tsb_scale: null pointer or negative count");
+  if (!g_dev || !out_dev || count < 0) return fail<tsb_handle_s>(nullptr, TSB_E_INVALID, "tsb_scale: null pointer or negative count");
   if (count == 0) return TSB_OK;
   DeviceGuard guard(device_of(g_dev));
   cudaError_t e = tsb::launch_scale(g_dev, count, gradH, gradH_dev, out_dev, static_cast<cudaStream_t>(stream));
-  if (e != cudaSuccess) return fail(nullptr, TSB_E_CUDA, std::string("scale launch: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail<tsb_handle_s>(nullptr, TSB_E_CUDA, std::string("scale launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 
 int tsb_grad_limit(float *grad_dev, int64_t count, float s_threshold, float s, float *work_dev, void *stream) {
-  if (!grad_dev || !work_dev || count < 0) return fail(nullptr, TSB_E_INVALID, "tsb_grad_limit: null pointer or negative count");
+  if (!grad_dev || !work_dev || count < 0) return fail<tsb_handle_s>(nullptr, TSB_E_INVALID, "tsb_grad_limit: null pointer or negative count");
   if (count == 0) return TSB_OK;
   DeviceGuard guard(device_of(grad_dev));
   cudaError_t e = tsb::launch_grad_limit(grad_dev, count, s_threshold, s, work_dev, static_cast<cudaStream_t>(stream));
-  if (e != cudaSuccess) return fail(nullptr, TSB_E_CUDA, std::string("grad_limit launch: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail<tsb_handle_s>(nullptr, TSB_E_CUDA, std::string("grad_limit launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 
 int tsb_adam_uniform_step(float *p_dev, const float *grad_dev, float *g1_dev, float *g2_dev, int64_t count, double lr,
                           double beta1, double beta2, int32_t step, double grad_limit, float *work_dev, void *stream) {
   if (!p_dev || !grad_dev || !g1_dev || !g2_dev || !work_dev || count < 0 || step < 1)
-    return fail(nullptr, TSB_E_INVALID, "tsb_adam_uniform_step: null pointer, negative count or step < 1");
+    return fail<tsb_handle_s>(nullptr, TSB_E_INVALID, "tsb_adam_uniform_step: null pointer, negative count or step < 1");
   if (count == 0) return TSB_OK;
   DeviceGuard guard(device_of(p_dev));
   cudaError_t e = tsb::launch_adam_uniform(p_dev, grad_dev, g1_dev, g2_dev, count, lr, beta1, beta2, step, grad_limit,
                                            work_dev, static_cast<cudaStream_t>(stream));
-  if (e != cudaSuccess) return fail(nullptr, TSB_E_CUDA, std::string("adam_uniform launch: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail<tsb_handle_s>(nullptr, TSB_E_CUDA, std::string("adam_uniform launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 

@@ -9,7 +9,7 @@
 //   AMIPS (J > 0, psi = I1 / (3 J^(2/3)) - 1, a = 2 / (3 J^(2/3))):  al = a, be = -2a / (3J), ga = 5 a I1 / (9 J^2),
 //                                                                     sk = -a I1 / (3J)
 // PSD: column (l, s) of P(H) is P(H)[e_s a_l^T]; in the rotated frame Dh = u_s (V^T a_l)^T (u_s = row s of U), and
-// entry (k r, l s) = u_r . (D'(Dh) V^T a_k), with D' the clamped scaling and pair rule of psd_apply_kernel.
+// entry (k r, l s) = u_r . (D'(Dh) V^T a_k), with D' = L+(Dh) of psd_frame_product (tsb_psd.cuh).
 #include "tsb_hessian.cuh"
 #include "tsb_psd.cuh"
 
@@ -147,16 +147,7 @@ __global__ void __launch_bounds__(kHessT) hessian_blocks_kernel(const HessParams
           for (int i = 0; i < 3; ++i)
 #pragma unroll
             for (int j = 0; j < 3; ++j) Dh[i][j] = U[s][i] * at[l][j];
-          Dp[0][0] = Ap[0] * Dh[0][0] + Ap[5] * Dh[1][1] + Ap[4] * Dh[2][2];
-          Dp[1][1] = Ap[5] * Dh[0][0] + Ap[1] * Dh[1][1] + Ap[3] * Dh[2][2];
-          Dp[2][2] = Ap[4] * Dh[0][0] + Ap[3] * Dh[1][1] + Ap[2] * Dh[2][2];
-#pragma unroll
-          for (int P = 0; P < 3; ++P) {
-            const int i = P == 2 ? 1 : 0, j = P == 0 ? 1 : 2;      // pairs (0,1), (0,2), (1,2)
-            const float sy = 0.5f * (Dh[i][j] + Dh[j][i]), an = 0.5f * (Dh[i][j] - Dh[j][i]);
-            Dp[i][j] = ls[P] * sy + la[P] * an;
-            Dp[j][i] = ls[P] * sy - la[P] * an;
-          }
+          psd_frame_product([&](int k) { return k < 24 ? Ap[k - 18] : k < 27 ? ls[k - 24] : la[k - 27]; }, Dh, Dp);
 #pragma unroll
           for (int k = 0; k <= l; ++k) {
             float y[3];

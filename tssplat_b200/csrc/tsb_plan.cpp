@@ -1201,22 +1201,35 @@ int build_hessian_pattern(const float *rest, const int32_t *tets, int32_t n, int
     err = "internal: tet " + std::to_string(missing.load()) + " has a corner pair that is not an entry of the operator";
     return TSB_E_MESH;
   }
-  // incidence lists (a counting sort over ascending entries keeps them ascending) and the rest inverses
-  H.inc_ptr.assign(size_t(n) + 1, 0);
-  for (size_t e = 0; e < 4 * size_t(nele); ++e) ++H.inc_ptr[size_t(tets[e]) + 1];
-  for (int32_t v = 0; v < n; ++v) H.inc_ptr[size_t(v) + 1] += H.inc_ptr[size_t(v)];
-  H.inc.resize(4 * size_t(nele));
-  std::vector<int32_t> fill(H.inc_ptr.begin(), H.inc_ptr.end() - 1);
-  for (size_t e = 0; e < 4 * size_t(nele); ++e) H.inc[size_t(fill[size_t(tets[e])]++)] = int32_t(e);
-  H.B.resize(9 * size_t(nele));
-  parallel_for(size_t(nele), 8192, nth, [&](size_t b, size_t e) {
-    for (size_t t = b; t < e; ++t) {
-      double Bi[9], det;
-      rest_inverse(rest, tets + 4 * t, Bi, &det);     // validated above
-      for (int k = 0; k < 9; ++k) H.B[size_t(k) * size_t(nele) + t] = float(Bi[k]);
-    }
-  });
   H.comp_label = std::move(P.comp_label);
+  return TSB_OK;
+}
+
+int build_tet_tables(const float *rest, const int32_t *tets, int32_t n, int32_t nele, const std::vector<int32_t> *comp_label,
+                     TetTables &T, std::string &err) {
+  const size_t ne = size_t(nele);
+  T.tets.assign(tets, tets + 4 * ne);
+  T.B.resize(9 * ne);
+  T.inc_ptr.assign(size_t(n) + 1, 0);
+  const int32_t *lab = comp_label ? comp_label->data() : nullptr;
+  size_t t = 0;
+  const auto bad = [&](const std::string &what) { err = "tet " + std::to_string(t) + " " + what; return TSB_E_MESH; };
+  for (; t < ne; ++t) {
+    const int32_t *q = tets + 4 * t;
+    for (int k = 0; k < 4; ++k)
+      if (q[k] < 0 || q[k] >= n) return bad("has vertex " + std::to_string(q[k]) + " outside [0, " + std::to_string(n) + ")");
+    if (lab && (lab[q[0]] < 0 || lab[q[1]] != lab[q[0]] || lab[q[2]] != lab[q[0]] || lab[q[3]] != lab[q[0]]))
+      return bad("spans two components of the handle: not the mesh it was created from");
+    double Bi[9], det;
+    if (!rest_inverse(rest, q, Bi, &det)) return bad("has a zero-volume or non-finite rest shape");
+    for (int k = 0; k < 9; ++k) T.B[size_t(k) * ne + t] = float(Bi[k]);
+    for (int k = 0; k < 4; ++k) ++T.inc_ptr[size_t(q[k]) + 1];
+  }
+  // incidence lists (a counting sort over ascending entries keeps them ascending)
+  for (int32_t v = 0; v < n; ++v) T.inc_ptr[size_t(v) + 1] += T.inc_ptr[size_t(v)];
+  T.inc.resize(4 * ne);
+  std::vector<int32_t> fill(T.inc_ptr.begin(), T.inc_ptr.end() - 1);
+  for (size_t e = 0; e < 4 * ne; ++e) T.inc[size_t(fill[size_t(tets[e])]++)] = int32_t(e);
   return TSB_OK;
 }
 

@@ -173,15 +173,25 @@ struct HessPattern {
   std::vector<int32_t> col;         // [nnzb] global vertex ids
   std::vector<float> w;             // [nnzb] fp32 M_ij as the plan streams it; diagonal -sum_j M_ij (fp64, column order)
   std::vector<int32_t> tblk;        // [16 nele] block of corner pair (k, l) of tet t at 16 t + 4 k + l
-  std::vector<int32_t> inc_ptr;     // [n + 1]
-  std::vector<int32_t> inc;         // [4 nele] 4 tet + corner, ascending within a vertex row
-  std::vector<float> B;             // [9][nele] rest inverse Dm^-1 (fp64, rounded), row-major entries
   std::vector<int32_t> comp_label;  // [n] component of every vertex, -1 = orphan
 };
 
 // Returns 0 on success, TSB_E_* otherwise (message in err).
 int build_hessian_pattern(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele, int32_t laplacian_scale,
                           HessPattern &out, std::string &err);
+
+// The per-tet tables of the projected Hessian (tsb_pcg_enable_psd) and the assembled one (tsb_hessian_create).
+struct TetTables {
+  std::vector<int32_t> tets;        // [4 nele] the caller's vertex ids
+  std::vector<float> B;             // [9][nele] rest inverse Dm^-1 (fp64, rounded), row-major entries
+  std::vector<int32_t> inc_ptr;     // [n + 1]
+  std::vector<int32_t> inc;         // [4 nele] 4 tet + corner, ascending within a vertex row
+};
+
+// Checks every tet in order: its vertices in [0, n), with comp_label (may be null) all four in one component, and a
+// nonzero, finite rest volume.  Returns 0 on success, TSB_E_MESH for the first tet that fails (message in err).
+int build_tet_tables(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele, const std::vector<int32_t> *comp_label,
+                     TetTables &out, std::string &err);
 
 // Multicolour symmetric Gauss-Seidel tables of the per-component solve (tsb_pcg_enable_sgs), over the block pattern crow /
 // col of build_hessian_pattern and the solver's PcgLists.  Rows are numbered by their entry (position) in PcgLists::vert.

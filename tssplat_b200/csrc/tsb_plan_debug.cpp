@@ -80,16 +80,17 @@ int tsbdbg_scalars(tsbdbg_plan *d, int64_t *out16) {   /* out16: 20 entries */
 
 void tsbdbg_free(tsbdbg_plan *d) { delete d; }
 
-/* The block pattern tsb_hessian_create uploads (tsb::build_hessian_pattern); arrays through tsbdbg_hess_array:
-   "crow", "col", "w", "tblk", "inc_ptr", "inc", "B", "comp_label" */
-struct tsbdbg_hess { tsb::HessPattern H; };
+/* The block pattern and tet tables tsb_hessian_create uploads (tsb::build_hessian_pattern, tsb::build_tet_tables);
+   arrays through tsbdbg_hess_array: "crow", "col", "w", "tblk", "inc_ptr", "inc", "B", "comp_label" */
+struct tsbdbg_hess { tsb::HessPattern H; tsb::TetTables T; };
 
 int tsbdbg_hess_build(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele, int32_t laplacian_scale,
                       tsbdbg_hess **out, int64_t *nnzb) {
   if (!out || !nnzb) return TSB_E_INVALID;
   *out = nullptr;
   tsbdbg_hess *d = new tsbdbg_hess();
-  const int rc = tsb::build_hessian_pattern(rest_xyz, tets, n, nele, laplacian_scale, d->H, g_err);
+  int rc = tsb::build_hessian_pattern(rest_xyz, tets, n, nele, laplacian_scale, d->H, g_err);
+  if (rc == TSB_OK) rc = tsb::build_tet_tables(rest_xyz, tets, n, nele, nullptr, d->T, g_err);
   if (rc != TSB_OK) { delete d; return rc; }
   *nnzb = d->H.nnzb;
   *out = d;
@@ -101,8 +102,8 @@ int tsbdbg_hess_array(tsbdbg_hess *d, const char *name, const void **ptr, int64_
   const tsb::HessPattern &H = d->H;
   const std::string k(name);
 #define ARR(nm, vec) if (k == nm) { *ptr = (vec).data(); *count = int64_t((vec).size()); return TSB_OK; }
-  ARR("crow", H.crow) ARR("col", H.col) ARR("w", H.w) ARR("tblk", H.tblk) ARR("inc_ptr", H.inc_ptr) ARR("inc", H.inc)
-  ARR("B", H.B) ARR("comp_label", H.comp_label)
+  ARR("crow", H.crow) ARR("col", H.col) ARR("w", H.w) ARR("tblk", H.tblk) ARR("inc_ptr", d->T.inc_ptr) ARR("inc", d->T.inc)
+  ARR("B", d->T.B) ARR("comp_label", H.comp_label)
 #undef ARR
   return TSB_E_INVALID;
 }

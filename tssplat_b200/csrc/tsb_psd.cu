@@ -7,6 +7,7 @@
 // lambda_a.  The projection clamps A's eigenvalues and the six pair eigenvalues at 0.  The product in the rotated frame,
 // Dh = U^T dF V, D' = L+(Dh), P(H)[dF] = U D' V^T, gives dF : P(H)[dF] = Dh : L+(Dh) >= 0 whatever rounding U and V
 // carry, so the stored operator stays PSD in fp32 (A+ up to its own rounding).
+#include "tsb_device.cuh"
 #include "tsb_jacobi.cuh"
 #include "tsb_psd.cuh"
 
@@ -224,20 +225,6 @@ __global__ void __launch_bounds__(kPsdProjectT) psd_project_kernel(const PsdPara
   for (int k = 0; k < kPsdOpFloats; ++k) p.op[k * ne + t] = o[k];
 }
 
-// Sum of v over the CTA in a fixed order (shuffle tree, then the warps in order); valid in thread 0.
-__device__ __forceinline__ double cta_sum(double v, double *sh) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, o);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0.0;
-  if (threadIdx.x == 0)
-#pragma unroll
-    for (int w = 0; w < kPsdT / 32; ++w) s += sh[w];
-  return s;
-}
-
 // One thread per tet: corner vectors of w P(H_t)[dF] with dF = dDs B, w = c2 (barrier) or c3 (AMIPS); inactive tets
 // write nothing (the gather skips them).  CURV: per-CTA fp64 partials of v^T P(H_t) v (unweighted) per term.
 template <bool CURV>
@@ -275,20 +262,8 @@ __global__ void __launch_bounds__(kPsdT) psd_apply_kernel(const PsdParams p, con
     for (int i = 0; i < 3; ++i)
 #pragma unroll
       for (int j = 0; j < 3; ++j) Dh[i][j] = T[i][0] * V[0][j] + T[i][1] * V[1][j] + T[i][2] * V[2][j];
-    const float a00 = p.op[18 * ne + t], a11 = p.op[19 * ne + t], a22 = p.op[20 * ne + t];
-    const float a12 = p.op[21 * ne + t], a02 = p.op[22 * ne + t], a01 = p.op[23 * ne + t];
     float Dp[3][3];
-    Dp[0][0] = a00 * Dh[0][0] + a01 * Dh[1][1] + a02 * Dh[2][2];
-    Dp[1][1] = a01 * Dh[0][0] + a11 * Dh[1][1] + a12 * Dh[2][2];
-    Dp[2][2] = a02 * Dh[0][0] + a12 * Dh[1][1] + a22 * Dh[2][2];
-#pragma unroll
-    for (int P = 0; P < 3; ++P) {
-      const int i = kPi[P], j = kPj[P];
-      const float s = 0.5f * (Dh[i][j] + Dh[j][i]), a = 0.5f * (Dh[i][j] - Dh[j][i]);
-      const float ls = p.op[(24 + P) * ne + t], la = p.op[(27 + P) * ne + t];
-      Dp[i][j] = ls * s + la * a;
-      Dp[j][i] = ls * s - la * a;
-    }
+    psd_frame_product([&](int k) { return p.op[k * ne + t]; }, Dh, Dp);
     if constexpr (CURV) {
       float q = 0.f;
 #pragma unroll
@@ -325,9 +300,9 @@ __global__ void __launch_bounds__(kPsdT) psd_apply_kernel(const PsdParams p, con
   }
   if constexpr (CURV) {
     __shared__ double sh[kPsdT / 32];
-    const double sb = cta_sum(qb, sh);
+    const double sb = block_sum<kPsdT>(qb, sh);
     if (threadIdx.x == 0) p.part[2 * size_t(blockIdx.x)] = sb;
-    const double sa = cta_sum(qa, sh);
+    const double sa = block_sum<kPsdT>(qa, sh);
     if (threadIdx.x == 0) p.part[2 * size_t(blockIdx.x) + 1] = sa;
   }
 }
@@ -361,8 +336,8 @@ __global__ void __launch_bounds__(kPsdT) psd_curv_kernel(const PsdParams p, floa
     b += p.part[2 * size_t(k)];
     a += p.part[2 * size_t(k) + 1];
   }
-  const double sb = cta_sum(b, sh);
-  const double sa = cta_sum(a, sh);
+  const double sb = block_sum<kPsdT>(b, sh);
+  const double sa = block_sum<kPsdT>(a, sh);
   if (threadIdx.x == 0) {
     const float vmv = p.curv_m[1];
     out[0] = float(double(c1) * double(vmv) + double(c2) * sb + double(c3) * sa);

@@ -26,6 +26,26 @@ struct PsdParams {
   int32_t nele, n, n_blocks;
 };
 
+// The product in the rotated frame, D' = L+(Dh): the clamped scaling block A+ on the diagonal, and for the pairs (0,1),
+// (0,2), (1,2) lambda_s+ on the symmetric and lambda_a+ on the antisymmetric part.  op(k) is entry k of the tet's
+// operator (18 + 00 11 22 12 02 01 for A+, 24 + pair for lambda_s+, 27 + pair for lambda_a+), read where it is first
+// needed.  Shared by the projected product (tsb_psd.cu) and the projected assembly (tsb_hessian.cu).
+template <class Op>
+__device__ __forceinline__ void psd_frame_product(Op op, const float (&Dh)[3][3], float (&Dp)[3][3]) {
+  const float a00 = op(18), a11 = op(19), a22 = op(20), a12 = op(21), a02 = op(22), a01 = op(23);
+  Dp[0][0] = a00 * Dh[0][0] + a01 * Dh[1][1] + a02 * Dh[2][2];
+  Dp[1][1] = a01 * Dh[0][0] + a11 * Dh[1][1] + a12 * Dh[2][2];
+  Dp[2][2] = a02 * Dh[0][0] + a12 * Dh[1][1] + a22 * Dh[2][2];
+#pragma unroll
+  for (int P = 0; P < 3; ++P) {
+    const int i = P == 2 ? 1 : 0, j = P == 0 ? 1 : 2;
+    const float s = 0.5f * (Dh[i][j] + Dh[j][i]), a = 0.5f * (Dh[i][j] - Dh[j][i]);
+    const float ls = op(24 + P), la = op(27 + P);
+    Dp[i][j] = ls * s + la * a;
+    Dp[j][i] = ls * s - la * a;
+  }
+}
+
 // Signed SVD and clamped eigen-system of every tet at x: barrier-active where det F < 0, AMIPS-active where det F > 0 and
 // amips != 0.
 cudaError_t launch_psd_project(const PsdParams &p, const float *x, int order, int amips, cudaStream_t st);

@@ -9,37 +9,13 @@
 // order (one thread per entry of the chunk, a shuffle tree per warp, the warps in order), so the direction kernel folds
 // them as it folds block Jacobi's.  No atomics, and no launch reads what
 // another CTA of it writes: bitwise repeatable, and a component's z depends on its own r only.
+#include "tsb_device.cuh"
 #include "tsb_sgs.cuh"
 
 namespace tsb {
 namespace {
 
 constexpr int kT = kSgsT, kW = kT / 32;
-
-struct F3 { float x, y, z; };
-__device__ __forceinline__ F3 ld3(const float *a, int v) { return F3{a[3 * size_t(v)], a[3 * size_t(v) + 1], a[3 * size_t(v) + 2]}; }
-__device__ __forceinline__ void st3(float *a, int v, F3 q) { a[3 * size_t(v)] = q.x; a[3 * size_t(v) + 1] = q.y; a[3 * size_t(v) + 2] = q.z; }
-__device__ __forceinline__ double dot3(F3 a, F3 b) { return double(a.x) * double(b.x) + double(a.y) * double(b.y) + double(a.z) * double(b.z); }
-// P r with the symmetric block stored as xx yy zz yz xz xy (as the solver's apply_block)
-__device__ __forceinline__ F3 apply_block(const float *pinv, int v, F3 r) {
-  const float *q = pinv + 6 * size_t(v);
-  const float xx = q[0], yy = q[1], zz = q[2], yz = q[3], xz = q[4], xy = q[5];
-  return F3{xx * r.x + xy * r.y + xz * r.z, xy * r.x + yy * r.y + yz * r.z, xz * r.x + yz * r.y + zz * r.z};
-}
-
-// Sum of v over the CTA in a fixed order (the solver's block_sum over this CTA's warps); valid in thread 0.
-__device__ __forceinline__ double block_sum(double v, double *sh) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, o);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0.0;
-  if (threadIdx.x == 0)
-#pragma unroll
-    for (int w = 0; w < kW; ++w) s += sh[w];
-  return s;
-}
 
 // sum over the list [b0, b1) of A_ij v_j (v in shared memory), lanes over the entries, summed by a fixed shuffle tree;
 // valid in every lane
@@ -112,8 +88,8 @@ __global__ void __launch_bounds__(kT) pcg_sgs_kernel(const PcgParams s, const Sg
       rz = dot3(r, z);
       rr = dot3(r, r);
     }
-    rz = block_sum(rz, sh);
-    if (w.col_rr >= 0) rr = block_sum(rr, sh);
+    rz = block_sum<kT>(rz, sh);
+    if (w.col_rr >= 0) rr = block_sum<kT>(rr, sh);
     if (threadIdx.x == 0) {
       w.part[size_t(w.stride) * size_t(ch) + w.col_rz] = rz;
       if (w.col_rr >= 0) w.part[size_t(w.stride) * size_t(ch) + w.col_rr] = rr;

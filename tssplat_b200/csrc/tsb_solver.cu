@@ -8,6 +8,7 @@
 // component's partials itself, in chunk order, from a column of the partial table that no CTA of that kernel writes.
 // The fold is redundant across the chunks of a component, but it needs no ticket, no atomic and no fence, and every
 // chunk gets bitwise the same scalar.  All scalars stay in device memory.
+#include "tsb_device.cuh"
 #include "tsb_jacobi.cuh"
 #include "tsb_sgs.cuh"
 #include "tsb_solver.cuh"
@@ -16,20 +17,6 @@ namespace tsb {
 namespace {
 
 constexpr int kT = kPcgChunkVerts;   // threads per CTA
-
-// Sum of v over the CTA in a fixed order; the result is valid in thread 0.
-__device__ __forceinline__ double block_sum(double v, double *sh) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, o);
-  __syncthreads();                                  // sh may still be read from the previous sum
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0.0;
-  if (threadIdx.x == 0)
-#pragma unroll
-    for (int w = 0; w < kT / 32; ++w) s += sh[w];
-  return s;
-}
 
 // The partial table has three columns per chunk, each with one writing kernel per iteration and read only by the kernel
 // after it, so no launch folds a column it also writes: kPHp (pcg_curv_kernel -> pcg_update_kernel; pcg_bdotd_kernel ->
@@ -50,17 +37,6 @@ __device__ __forceinline__ double fold(const double *part, int col, int c0, int 
   const double out = sh[0];
   __syncthreads();                                  // sh is reused by the next fold and by block_sum
   return out;
-}
-
-struct F3 { float x, y, z; };
-__device__ __forceinline__ F3 ld3(const float *a, int v) { return F3{a[3 * size_t(v)], a[3 * size_t(v) + 1], a[3 * size_t(v) + 2]}; }
-__device__ __forceinline__ void st3(float *a, int v, F3 q) { a[3 * size_t(v)] = q.x; a[3 * size_t(v) + 1] = q.y; a[3 * size_t(v) + 2] = q.z; }
-__device__ __forceinline__ double dot3(F3 a, F3 b) { return double(a.x) * double(b.x) + double(a.y) * double(b.y) + double(a.z) * double(b.z); }
-// z = P r with the symmetric block stored as xx yy zz yz xz xy
-__device__ __forceinline__ F3 apply_block(const float *pinv, int v, F3 r) {
-  const float *q = pinv + 6 * size_t(v);
-  const float xx = q[0], yy = q[1], zz = q[2], yz = q[3], xz = q[4], xy = q[5];
-  return F3{xx * r.x + xy * r.y + xz * r.z, xy * r.x + yy * r.y + yz * r.z, xz * r.x + yz * r.y + zz * r.z};
 }
 
 // Inverse preconditioner block of vertex v: cyclic Jacobi eigen-decomposition in fp64 registers, eigenvalues clamped
@@ -148,8 +124,8 @@ __global__ void __launch_bounds__(kT) pcg_init_kernel(const PcgParams s, const f
     st3(s.r, v, r); st3(s.z, v, z); st3(d, v, F3{0.f, 0.f, 0.f});
     rz = dot3(r, z); rr = dot3(r, r);
   }
-  rz = block_sum(rz, sh);
-  rr = block_sum(rr, sh);
+  rz = block_sum<kT>(rz, sh);
+  rr = block_sum<kT>(rr, sh);
   if (threadIdx.x == 0) { s.part[kPartCols * size_t(blockIdx.x) + kRz] = rz; s.part[kPartCols * size_t(blockIdx.x) + kRr] = rr; }
 }
 
@@ -172,7 +148,7 @@ __global__ void __launch_bounds__(kT) pcg_curv_kernel(const PcgParams s, const f
     const F3 p = ld3(s.p, v);
     q = dot3(p, SHIFT ? shifted(ld3(s.Hp, v), p, shift[c]) : ld3(s.Hp, v));
   }
-  q = block_sum(q, sh);
+  q = block_sum<kT>(q, sh);
   if (threadIdx.x == 0) s.part[kPartCols * size_t(blockIdx.x) + kPHp] = q;
 }
 
@@ -252,8 +228,8 @@ __global__ void __launch_bounds__(kT) pcg_update_kernel(const PcgParams s, float
     st3(d, v, x); st3(s.r, v, r); st3(s.z, v, z);
     nrz = dot3(r, z); nrr = dot3(r, r);
   }
-  nrz = block_sum(nrz, sh);
-  nrr = block_sum(nrr, sh);
+  nrz = block_sum<kT>(nrz, sh);
+  nrr = block_sum<kT>(nrr, sh);
   if (threadIdx.x == 0) { s.part[kPartCols * size_t(blockIdx.x) + kRz] = nrz; s.part[kPartCols * size_t(blockIdx.x) + kRr] = nrr; }
   if (lead) { C.st_upd = kPcgActive; C.idle = 0; C.n_hvp = iter + 1; C.rz_prev = rz; C.dHd += alpha * alpha * pHp; }
   if (TR && lead) t.comp[c].step = alpha;
@@ -331,7 +307,7 @@ __global__ void __launch_bounds__(kT) pcg_bdotd_kernel(const PcgParams s, const 
   const int e = begin + int(threadIdx.x);
   double q = 0.0;
   if (e < end) { const int v = s.vert[e]; q = dot3(ld3(b, v), ld3(d, v)); }
-  q = block_sum(q, sh);
+  q = block_sum<kT>(q, sh);
   if (threadIdx.x == 0) s.part[kPartCols * size_t(blockIdx.x) + kPHp] = q;
 }
 
@@ -461,9 +437,9 @@ __global__ void __launch_bounds__(kT) newton_dots_kernel(const PcgParams s, cons
            double(d.z) * (double(x.z) - double(y.z));
     }
   }
-  bd = block_sum(bd, sh);
-  dd = block_sum(dd, sh);
-  if (PROX) dx = block_sum(dx, sh);
+  bd = block_sum<kT>(bd, sh);
+  dd = block_sum<kT>(dd, sh);
+  if (PROX) dx = block_sum<kT>(dx, sh);
   if (threadIdx.x == 0) {
     w.part[kNwCols * size_t(blockIdx.x) + kNwBd] = bd;
     w.part[kNwCols * size_t(blockIdx.x) + kNwDd] = dd;
@@ -568,7 +544,7 @@ __global__ void __launch_bounds__(kT) newton_tr_bpb_kernel(const PcgParams s, co
     const F3 b = ld3(w.b, v);
     q = dot3(b, apply_block(s.pinv, v, b));
   }
-  q = block_sum(q, sh);
+  q = block_sum<kT>(q, sh);
   if (threadIdx.x == 0) w.part[kNwCols * size_t(blockIdx.x) + kNwMaxD] = q;
 }
 
