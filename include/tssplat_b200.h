@@ -20,7 +20,7 @@
 extern "C" {
 #endif
 
-#define TSB_VERSION 11
+#define TSB_VERSION 12
 #define TSB_LINE_MAX_ALPHA 8   /* step sizes one tsb_line_search call may evaluate */
 
 enum {
@@ -499,6 +499,53 @@ int tsb_pcg_enable_sgs(tsb_pcg_t s, tsb_hessian_t hs);
 int tsb_pcg_set_matrix(tsb_pcg_t s, const float *x_dev, const tsb_terms_t *terms, float *diag_out_dev, void *stream);
 int tsb_pcg_apply_precond(tsb_pcg_t s, const float *r_dev, float *z_dev, void *stream);
 int tsb_pcg_sgs_colors(tsb_pcg_t s, int32_t *colors_out_dev, int32_t *n_colors_out);
+
+/* ---- Affine coarse space: a two-level preconditioner for the per-sphere solve --------------------------------------
+ * Opt-in on a solver workspace, on top of block Jacobi or SGS (P below: the blocks, or the sweep's M^-1).  Per sphere c,
+ * with Y_i = X_i - mean_c X (rest positions, the mean in fp64, Y stored in fp32) and the 9 coarse unknowns a 3 x 3 matrix
+ * A, (Z a)_i = A Y_i spans the linear affine motions of the sphere, and the preconditioner is
+ *   P + Z E+ Z^T,   E = E_c + shift_c (S_c (x) I3),   S_c = sum_i Y_i Y_i^T,
+ * E_c = Z^T H Z = sum_t [c2 d2psi_b + c3 d2psi_a](F_t) (the c1 M term vanishes: M annihilates affine maps; translations
+ * have no curvature), in PSD mode with the projected operator the solve multiplies by.  E+ is E's pseudo-inverse: cyclic
+ * Jacobi in fp64, eigenvalues <= coarse_floor * lambda_max give 0, lambda_max <= 0 gives the zero matrix.  So the
+ * preconditioner is SPD wherever P is, indefinite H included, and CG, Steihaug-Toint and every Newton rule keep their
+ * meaning: with R = Z^T r, r.z becomes r.P r + R^T E+ R and z = P r + Z E+ R wherever the solve uses z (the first
+ * direction, NEGCURV_FIRST's d, and tsb_pcg_solve_tr's norm).  It removes the near-null global modes
+ * (rotations, scaling, shears with AMIPS or in PSD mode) that block Jacobi leaves to CG.  The R partials ride in the init
+ * and update kernels and the fold in the direction kernel: no launch per iteration.  DESIGN.md section 5, "Affine coarse
+ * space".
+ *
+ * tsb_pcg_enable_coarse: rest_xyz (host float32 [3n]) and tets (host int32 [4 nele]) must be the mesh the handle was
+ * created from; coarse_floor >= 0.  Builds Y in the solver's vertex order, S_c, and per sphere a table of tet chunks of
+ * <= 256 tets (tets grouped by sphere, ascending), and allocates, added to tsb_pcg_device_bytes:
+ *   12 rows + 72 chunks + 372 tet_chunks + 700 n_components + 56 nele + 4   bytes
+ * (Y; R partials; E_c partials and the chunk table; S_c, E+ and the chunk offsets; tet ids, vertices and Dm^-1 in chunk
+ * order).  A workspace that never enables keeps its size.  E+ starts at 0 (no correction) until set_coarse.  Synchronous
+ * and allocating: not during a stream capture (detected on the legacy default stream only, as for tsb_pcg_enable_psd).
+ * A second call is TSB_E_INVALID; after a failure the workspace is as before.
+ *
+ * tsb_pcg_set_coarse: forms E_c at x_dev (tsb_hessian_assemble's rules for *terms; exact mode: barrier where det F < 0,
+ * AMIPS where det F > 0 and c3 != 0, det F in fp64 from the fp32 x; PSD mode: runs the solve's projection launch first,
+ * so the same x gives the same operator bits) and E+ of the unshifted E_c.  One thread per tet writes each tet chunk's
+ * fp64 partials, summed in a fixed order; one thread per sphere folds them in chunk order and factors.
+ * tsb_pcg_set_blocks(_ex) factors again with its shift, so the solve's E includes shift_c.  No host read, no
+ * allocation, no atomics: capturable and bitwise repeatable; a sphere's E depends on its own x only.  Every damped or
+ * proximal Newton step on a coarse workspace forms E_c after the diagonal blocks (or tsb_pcg_set_matrix) and leaves the
+ * factorisation to its tsb_pcg_set_blocks_ex.  tsb_newton_tr_step(_ex) refuses a coarse workspace with TSB_E_INVALID:
+ * the two-level norm is near-singular along the coarse modes, so the radius admits long affine moves that the gain
+ * ratio rejects, and the steps stall (DESIGN.md section 5).
+ *
+ * tsb_pcg_coarse_matrix: E_out_dev (device double [n_components][81], component order) = the unshifted E_c of the last
+ * set_coarse, on the legacy default stream and synchronously.
+ *
+ * tsb_pcg_apply_precond applies P + Z E+ Z^T at the current E+ on a coarse workspace (z on vertices no tet references is
+ * left as it is).
+ * Argument errors (TSB_E_INVALID, nothing launched): a null pointer that is required, coarse not enabled, a negative or
+ * NaN coarse_floor, another nele, tets that do not match the handle's mesh (a vertex out of range, a tet across two of
+ * its spheres, a zero-volume rest tet), the rules of *terms. */
+int tsb_pcg_enable_coarse(tsb_pcg_t s, const float *rest_xyz, const int32_t *tets, int32_t nele, float coarse_floor);
+int tsb_pcg_set_coarse(tsb_pcg_t s, const float *x_dev, const tsb_terms_t *terms, void *stream);
+int tsb_pcg_coarse_matrix(tsb_pcg_t s, double *E_out_dev);
 
 /* ---- Damped Newton step: one Levenberg-Marquardt iteration per sphere on the device (no counterpart in the reference)
  * A Newton workspace sits beside a solver workspace (which must outlive it; creating one changes nothing about the

@@ -27,6 +27,7 @@ EXPORTED_SYMBOLS = (
     "tsb_pcg_enable_psd", "tsb_pcg_hvp_psd", "tsb_pcg_solve_tr",
     "tsb_hessian_create", "tsb_hessian_destroy", "tsb_hessian_last_error", "tsb_hessian_device_bytes", "tsb_hessian_pattern",
     "tsb_hessian_assemble", "tsb_pcg_enable_sgs", "tsb_pcg_set_matrix", "tsb_pcg_apply_precond", "tsb_pcg_sgs_colors",
+    "tsb_pcg_enable_coarse", "tsb_pcg_set_coarse", "tsb_pcg_coarse_matrix",
     "tsb_newton_create", "tsb_newton_destroy", "tsb_newton_last_error", "tsb_newton_device_bytes", "tsb_newton_reset",
     "tsb_newton_step", "tsb_newton_prox_step", "tsb_newton_tr_step", "tsb_newton_tr_step_ex", "tsb_energy_grad_host", "tsb_scale",
     "tsb_grad_limit", "tsb_adam_uniform_step",
@@ -192,6 +193,12 @@ def _load() -> C.CDLL:
     lib.tsb_pcg_apply_precond.argtypes = [vp, vp, vp, vp]
     lib.tsb_pcg_sgs_colors.restype = C.c_int
     lib.tsb_pcg_sgs_colors.argtypes = [vp, vp, C.POINTER(C.c_int32)]
+    lib.tsb_pcg_enable_coarse.restype = C.c_int
+    lib.tsb_pcg_enable_coarse.argtypes = [vp, vp, vp, i32, C.c_float]
+    lib.tsb_pcg_set_coarse.restype = C.c_int
+    lib.tsb_pcg_set_coarse.argtypes = [vp, vp, C.POINTER(tsb_terms_t), vp]
+    lib.tsb_pcg_coarse_matrix.restype = C.c_int
+    lib.tsb_pcg_coarse_matrix.argtypes = [vp, vp]
     lib.tsb_newton_create.restype = C.c_int
     lib.tsb_newton_create.argtypes = [vp, C.POINTER(vp)]
     lib.tsb_newton_destroy.restype = None

@@ -61,6 +61,8 @@ struct tsb_pcg_s {
   float *sgs_values = nullptr;       // [9 nnzb] A, written by tsb_pcg_set_matrix
   int32_t *sgs_color = nullptr;      // [n]
   int32_t sgs_n_colors = 0;
+  bool coarse = false;               // tsb_pcg_enable_coarse: the two-level preconditioner with the affine coarse space
+  tsb::CoarseParams co{};
   std::vector<void *> allocs;
   std::string err;
 };
@@ -624,8 +626,9 @@ int tsb_pcg_set_blocks_ex(tsb_pcg_t s, const float *diag_dev, float rel_floor, c
   DeviceGuard guard(s->h->device);
   if (!guard.ok) return fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const cudaError_t e = diag_dev && shift_dev ? tsb::launch_pcg_blocks_shift(s->P, diag_dev, rel_floor, shift_dev, inv_out_dev, st)
-                                              : tsb::launch_pcg_blocks(s->P, diag_dev, rel_floor, inv_out_dev, st);
+  cudaError_t e = diag_dev && shift_dev ? tsb::launch_pcg_blocks_shift(s->P, diag_dev, rel_floor, shift_dev, inv_out_dev, st)
+                                        : tsb::launch_pcg_blocks(s->P, diag_dev, rel_floor, inv_out_dev, st);
+  if (e == cudaSuccess && s->coarse) e = tsb::launch_coarse_factor(s->P, s->co, diag_dev ? shift_dev : nullptr, nullptr, st);
   if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("preconditioner launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
@@ -649,6 +652,20 @@ int psd_product(tsb_pcg_t s, const float *x_dev, const float *v_dev, const tsb_t
 int psd_project(tsb_pcg_t s, const float *x_dev, const tsb_terms_t &t, cudaStream_t st) {
   const cudaError_t e = tsb::launch_psd_project(s->Q, x_dev, t.order, t.c3 != 0.f ? 1 : 0, st);
   if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("projection launch: ") + cudaGetErrorString(e));
+  return TSB_OK;
+}
+
+// The coarse matrix's partials at x (PSD mode: after the solve's projection launch, so the same x gives the same
+// operator bits) and, with factor, its unshifted E+.  A Newton step leaves the factorisation to tsb_pcg_set_blocks_ex,
+// which follows with the step's shift.
+int coarse_form(tsb_pcg_t s, const float *x_dev, const tsb_terms_t &t, bool factor, cudaStream_t st) {
+  if (s->psd) {
+    const int rc = psd_project(s, x_dev, t, st);
+    if (rc != TSB_OK) return rc;
+  }
+  cudaError_t e = tsb::launch_coarse_tets(s->co, x_dev, t.order, t.c2, t.c3, s->psd ? &s->Q : nullptr, st);
+  if (e == cudaSuccess && factor) e = tsb::launch_coarse_factor(s->P, s->co, nullptr, nullptr, st);
+  if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("coarse launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 
@@ -749,7 +766,8 @@ int pcg_solve_impl(tsb_pcg_t s, const float *x_dev, const float *b_dev, const ts
     if (rc != TSB_OK) return rc;
   }
   const tsb::SgsParams *sgs = s->sgs ? &s->G : nullptr;
-  cudaError_t e = tsb::launch_pcg_begin(P, b_dev, d_out_dev, tr, st, sgs);
+  const tsb::CoarseParams *co = s->coarse ? &s->co : nullptr;
+  cudaError_t e = tsb::launch_pcg_begin(P, b_dev, d_out_dev, tr, st, sgs, co);
   if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("solver launch: ") + cudaGetErrorString(e));
   int32_t it = 0;
   while (it < opt->max_iter) {
@@ -760,7 +778,7 @@ int pcg_solve_impl(tsb_pcg_t s, const float *x_dev, const float *b_dev, const ts
       const int rc = hvp_impl(s->h, x_dev, P.p, terms->c1, terms->c2, terms->c3, terms->order, 1.f, nullptr, P.Hp, nullptr, 1, st);
       if (rc != TSB_OK) return fail(s, rc, s->h->err);
     }
-    e = tsb::launch_pcg_step(P, d_out_dev, it, opt->rtol, shift_dev, tr, st, sgs);
+    e = tsb::launch_pcg_step(P, d_out_dev, it, opt->rtol, shift_dev, tr, st, sgs, co);
     if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("solver launch: ") + cudaGetErrorString(e));
     ++it;
     if (opt->check_every > 0 && it % opt->check_every == 0 && it < opt->max_iter) {
@@ -981,6 +999,10 @@ int newton_run(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const flo
     rc = tsb_hess_diag(h, x_dev, terms, 1.f, nullptr, W.diag, st);
     if (rc != TSB_OK) return fail(nw, rc, h->err);
   }
+  if (s->coarse) {      // E_c at x; tsb_pcg_set_blocks_ex below factors it with the step's shift
+    rc = coarse_form(s, x_dev, *terms, false, st);
+    if (rc != TSB_OK) return fail(nw, rc, s->err);
+  }
   cudaError_t e = tsb::launch_newton_prep(s->P, W, prox, st);
   if (e == cudaSuccess && k.damped) e = tsb::launch_newton_shift(s->P, W, k.lm, prox, st);
   if (e != cudaSuccess) return fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
@@ -1040,6 +1062,9 @@ int tsb_newton_tr_step_ex(tsb_newton_t nw, float *x_dev, const float *anchor_dev
   if (!nw) return TSB_E_INVALID;
   const int rc = newton_check(nw, x_dev, anchor_dev, weight_dev, terms, opt);
   if (rc != TSB_OK) return rc;
+  if (nw->s->coarse)    // the two-level norm is near-singular along the coarse modes: the radius then admits long affine
+                        // moves the gain ratio rejects, and the steps stall (DESIGN.md section 5, "Affine coarse space")
+    return fail(nw, TSB_E_INVALID, "the trust-region steps do not take a workspace with the coarse space (tsb_pcg_enable_coarse)");
   if (bt) {
     if (bt->n_alpha < 2 || bt->n_alpha > TSB_LINE_MAX_ALPHA)
       return fail(nw, TSB_E_INVALID, "n_alpha must be in [2, " + std::to_string(TSB_LINE_MAX_ALPHA) + "]");
@@ -1226,14 +1251,83 @@ int tsb_pcg_set_matrix(tsb_pcg_t s, const float *x_dev, const tsb_terms_t *terms
 
 int tsb_pcg_apply_precond(tsb_pcg_t s, const float *r_dev, float *z_dev, void *stream) {
   if (!s) return TSB_E_INVALID;
-  if (!s->sgs) return fail(s, TSB_E_INVALID, "tsb_pcg_apply_precond needs a workspace after tsb_pcg_enable_sgs");
+  if (!s->sgs && !s->coarse)
+    return fail(s, TSB_E_INVALID, "tsb_pcg_apply_precond needs a workspace after tsb_pcg_enable_sgs or tsb_pcg_enable_coarse");
   if (!r_dev || !z_dev) return fail(s, TSB_E_INVALID, "r_dev and z_dev must be non-null");
   if (r_dev == z_dev) return fail(s, TSB_E_INVALID, "z_dev must not be r_dev: r is read after z is written");
   DeviceGuard guard(s->h->device);
   if (!guard.ok) return fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
-  const cudaError_t e = tsb::launch_sgs_sweep(s->P, s->G, tsb::SgsSweep{r_dev, z_dev, nullptr, 0, 0, -1, nullptr, nullptr},
-                                              static_cast<cudaStream_t>(stream));
-  if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("sweep launch: ") + cudaGetErrorString(e));
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaError_t e = cudaSuccess;
+  if (s->sgs) e = tsb::launch_sgs_sweep(s->P, s->G, tsb::SgsSweep{r_dev, z_dev, nullptr, 0, 0, -1, nullptr, nullptr}, st);
+  if (e == cudaSuccess && s->coarse) e = tsb::launch_coarse_restrict(s->P, s->co, r_dev, st);
+  if (e == cudaSuccess && s->coarse) e = tsb::launch_coarse_apply(s->P, s->co, r_dev, z_dev, !s->sgs, st);
+  if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("preconditioner launch: ") + cudaGetErrorString(e));
+  return TSB_OK;
+}
+
+/* ---- Affine coarse space (tsb_coarse.cu) ---- */
+
+int tsb_pcg_enable_coarse(tsb_pcg_t s, const float *rest_xyz, const int32_t *tets, int32_t nele, float coarse_floor) {
+  if (!s) return TSB_E_INVALID;
+  if (s->coarse) return fail(s, TSB_E_INVALID, "the coarse space is already enabled on this workspace");
+  if (!rest_xyz || !tets) return fail(s, TSB_E_INVALID, "rest_xyz and tets must be non-null");
+  if (!(coarse_floor >= 0.f)) return fail(s, TSB_E_INVALID, "coarse_floor must be >= 0");
+  const tsb_handle_t h = s->h;
+  if (nele != h->info.nele)
+    return fail(s, TSB_E_INVALID, "nele = " + std::to_string(nele) + " but the handle has " + std::to_string(h->info.nele) + " tets");
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  int rc = refuse_capture(s, cudaStreamLegacy, "tsb_pcg_enable_coarse allocates device memory and cannot run while a stream is being captured");
+  if (rc != TSB_OK) return rc;
+  tsb::TetTables T;
+  std::string err;
+  rc = tsb::build_tet_tables(rest_xyz, tets, h->info.n, nele, &h->comp_label, T, err);
+  if (rc != TSB_OK) return fail(s, TSB_E_INVALID, err + " (tets must be the mesh the handle was created from)");
+  tsb::PcgLists L;
+  tsb::build_pcg_lists(h->comp_label, s->P.n_components, L);
+  tsb::CoarseTables CT;
+  tsb::build_coarse_tables(rest_xyz, T, h->comp_label, L, CT);
+  tsb::CoarseParams co{};
+  co.n_tchunks = int32_t(CT.tchunk.size() / 3); co.nele = nele; co.floor = coarse_floor;
+  const size_t S = size_t(s->P.n_components);
+  Rollback<tsb_pcg_s> undo(s);
+  rc = device_array(s, co.Y, 1, CT.Y.empty() ? nullptr : CT.Y.data(), CT.Y.size());
+  if (rc == TSB_OK) rc = device_array(s, co.rpart, 9 * std::max<size_t>(size_t(s->P.n_chunks), 1));
+  if (rc == TSB_OK) rc = device_array(s, co.tchunk, 3, CT.tchunk.empty() ? nullptr : CT.tchunk.data(), CT.tchunk.size());
+  if (rc == TSB_OK) rc = device_array(s, co.comp_tchunk, 0, CT.comp_tchunk.data(), CT.comp_tchunk.size());
+  if (rc == TSB_OK) rc = device_array(s, co.tet, 1, CT.tet.empty() ? nullptr : CT.tet.data(), CT.tet.size());
+  if (rc == TSB_OK) rc = device_array(s, co.tets, 4, CT.tets.empty() ? nullptr : CT.tets.data(), CT.tets.size());
+  if (rc == TSB_OK) rc = device_array(s, co.B, 9, CT.B.empty() ? nullptr : CT.B.data(), CT.B.size());
+  if (rc == TSB_OK) rc = device_array(s, co.epart, size_t(tsb::kCoarseUpper) * std::max<size_t>(size_t(co.n_tchunks), 1));
+  if (rc == TSB_OK) rc = device_array(s, co.S, 6, CT.S.empty() ? nullptr : CT.S.data(), CT.S.size());
+  if (rc == TSB_OK) rc = device_array(s, co.Einv, 81 * std::max<size_t>(S, 1));
+  if (rc != TSB_OK) return rc;       // the rollback leaves the workspace as it was
+  undo.commit();
+  s->co = co;
+  s->coarse = true;
+  return TSB_OK;
+}
+
+int tsb_pcg_set_coarse(tsb_pcg_t s, const float *x_dev, const tsb_terms_t *terms, void *stream) {
+  if (!s) return TSB_E_INVALID;
+  if (!s->coarse) return fail(s, TSB_E_INVALID, "tsb_pcg_set_coarse needs a workspace after tsb_pcg_enable_coarse");
+  if (!x_dev || !terms) return fail(s, TSB_E_INVALID, "x_dev and terms must be non-null");
+  if (const char *m = check_terms(s->h, s->psd, *terms)) return fail(s, TSB_E_INVALID, m);
+  DeviceGuard guard(s->h->device);
+  if (!guard.ok) return fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  return coarse_form(s, x_dev, *terms, true, static_cast<cudaStream_t>(stream));
+}
+
+int tsb_pcg_coarse_matrix(tsb_pcg_t s, double *E_out_dev) {
+  if (!s) return TSB_E_INVALID;
+  if (!s->coarse) return fail(s, TSB_E_INVALID, "tsb_pcg_coarse_matrix needs a workspace after tsb_pcg_enable_coarse");
+  if (!E_out_dev) return fail(s, TSB_E_INVALID, "E_out_dev must be non-null");
+  DeviceGuard guard(s->h->device);
+  if (!guard.ok) return fail(s, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  cudaError_t e = tsb::launch_coarse_factor(s->P, s->co, nullptr, E_out_dev, cudaStreamLegacy);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(cudaStreamLegacy);
+  if (e != cudaSuccess) return fail(s, TSB_E_CUDA, std::string("coarse launch: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
 

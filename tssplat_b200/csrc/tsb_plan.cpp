@@ -1233,6 +1233,53 @@ int build_tet_tables(const float *rest, const int32_t *tets, int32_t n, int32_t 
   return TSB_OK;
 }
 
+void build_coarse_tables(const float *rest, const TetTables &T, const std::vector<int32_t> &comp_label, const PcgLists &L,
+                         CoarseTables &C) {
+  C = CoarseTables();
+  const size_t ne = T.tets.size() / 4, S = L.comp_off.size() - 1;
+  // tets grouped by component: a counting sort keeps tet ids ascending in each
+  std::vector<int32_t> off(S + 1, 0);
+  for (size_t t = 0; t < ne; ++t) ++off[size_t(comp_label[size_t(T.tets[4 * t])]) + 1];
+  for (size_t c = 0; c < S; ++c) off[c + 1] += off[c];
+  C.tet.resize(ne);
+  std::vector<int32_t> fill(off.begin(), off.end() - 1);
+  for (size_t t = 0; t < ne; ++t) C.tet[size_t(fill[size_t(comp_label[size_t(T.tets[4 * t])])]++)] = int32_t(t);
+  C.tets.resize(4 * ne);
+  C.B.resize(9 * ne);
+  for (size_t e = 0; e < ne; ++e) {
+    const size_t t = size_t(C.tet[e]);
+    for (int k = 0; k < 4; ++k) C.tets[4 * e + size_t(k)] = T.tets[4 * t + size_t(k)];
+    for (int k = 0; k < 9; ++k) C.B[size_t(k) * ne + e] = T.B[size_t(k) * ne + t];
+  }
+  C.comp_tchunk.assign(S + 1, 0);
+  for (size_t c = 0; c < S; ++c) {
+    C.comp_tchunk[c] = int32_t(C.tchunk.size() / 3);
+    for (int32_t b = off[c]; b < off[c + 1]; b += kCoarseTetChunk) {
+      C.tchunk.push_back(int32_t(c));
+      C.tchunk.push_back(b);
+      C.tchunk.push_back(std::min(off[c + 1], b + kCoarseTetChunk));
+    }
+  }
+  C.comp_tchunk[S] = int32_t(C.tchunk.size() / 3);
+  // Y and S_c
+  C.Y.resize(3 * L.vert.size());
+  C.S.assign(6 * S, 0.0);
+  for (size_t c = 0; c < S; ++c) {
+    const int32_t e0 = L.comp_off[c], e1 = L.comp_off[c + 1];
+    double m[3] = {0.0, 0.0, 0.0};
+    for (int32_t e = e0; e < e1; ++e)
+      for (int k = 0; k < 3; ++k) m[k] += double(rest[3 * size_t(L.vert[size_t(e)]) + size_t(k)]);
+    for (int k = 0; k < 3; ++k) m[k] /= double(std::max(e1 - e0, 1));
+    double *Sc = C.S.data() + 6 * c;
+    for (int32_t e = e0; e < e1; ++e) {
+      float *y = C.Y.data() + 3 * size_t(e);
+      for (int k = 0; k < 3; ++k) y[k] = float(double(rest[3 * size_t(L.vert[size_t(e)]) + size_t(k)]) - m[k]);
+      const double y0 = y[0], y1 = y[1], y2 = y[2];
+      Sc[0] += y0 * y0; Sc[1] += y1 * y1; Sc[2] += y2 * y2; Sc[3] += y1 * y2; Sc[4] += y0 * y2; Sc[5] += y0 * y1;
+    }
+  }
+}
+
 int build_sgs_tables(const std::vector<int32_t> &crow, const std::vector<int32_t> &col, const PcgLists &L, int nth,
                      SgsTables &T, std::string &err) {
   T = SgsTables();

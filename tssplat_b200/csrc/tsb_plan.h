@@ -193,6 +193,26 @@ struct TetTables {
 int build_tet_tables(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele, const std::vector<int32_t> *comp_label,
                      TetTables &out, std::string &err);
 
+// The affine coarse space of the per-component solve (tsb_pcg_enable_coarse), over the tables of build_tet_tables and the
+// solver's PcgLists.  The tets are grouped by component (components in order, tet ids ascending in each) and cut into
+// chunks of <= kCoarseTetChunk tets of one component: tchunk holds (component, begin, end) into tet, comp_tchunk[c] the
+// first chunk of component c.  Y[3 e .. 3 e + 2] = X_v - mean_c X for entry e of PcgLists::vert (v its vertex, the mean
+// over the component's vertices in fp64, the difference rounded to fp32); S[6 c ..] = sum_e Y_e Y_e^T of component c in
+// fp64 from the fp32 Y, as 00 11 22 12 02 01.
+constexpr int kCoarseTetChunk = 256;
+struct CoarseTables {
+  std::vector<int32_t> tet;          // [nele] tet ids grouped by component
+  std::vector<int32_t> tets;         // [4 nele] their vertices
+  std::vector<float> B;              // [9][nele] their Dm^-1, row-major entries
+  std::vector<int32_t> tchunk;       // [3 * tet chunks]
+  std::vector<int32_t> comp_tchunk;  // [n_components + 1]
+  std::vector<float> Y;              // [3 rows]
+  std::vector<double> S;             // [6 n_components]
+};
+// comp_label: the component of every vertex (every tet's vertices in one component, as build_tet_tables checks)
+void build_coarse_tables(const float *rest_xyz, const TetTables &T, const std::vector<int32_t> &comp_label, const PcgLists &L,
+                         CoarseTables &out);
+
 // Multicolour symmetric Gauss-Seidel tables of the per-component solve (tsb_pcg_enable_sgs), over the block pattern crow /
 // col of build_hessian_pattern and the solver's PcgLists.  Rows are numbered by their entry (position) in PcgLists::vert.
 // Every component is coloured greedily on its own, vertices ascending, each vertex taking the smallest colour none of its

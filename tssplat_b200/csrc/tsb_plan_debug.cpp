@@ -148,4 +148,41 @@ int tsbdbg_sgs_array(tsbdbg_sgs *d, const char *name, const void **ptr, int64_t 
 
 void tsbdbg_sgs_free(tsbdbg_sgs *d) { delete d; }
 
+/* The coarse-space tables tsb_pcg_enable_coarse builds (tsb::build_coarse_tables) over build_tet_tables and the solver's
+   vertex lists of the mesh; arrays through tsbdbg_coarse_array: "tet", "tets", "B", "tchunk", "comp_tchunk", "Y", "S",
+   and the lists "vert", "comp_off", "comp_label" it was built from */
+struct tsbdbg_coarse { tsb::HessPattern H; tsb::PcgLists L; tsb::TetTables T; tsb::CoarseTables C; };
+
+int tsbdbg_coarse_build(const float *rest_xyz, const int32_t *tets, int32_t n, int32_t nele, tsbdbg_coarse **out,
+                        int32_t *n_components) {
+  if (!out || !n_components) return TSB_E_INVALID;
+  *out = nullptr;
+  tsbdbg_coarse *d = new tsbdbg_coarse();
+  int rc = tsb::build_hessian_pattern(rest_xyz, tets, n, nele, 0, d->H, g_err);
+  int32_t S = 0;
+  if (rc == TSB_OK) {
+    for (const int32_t c : d->H.comp_label) S = std::max(S, c + 1);
+    tsb::build_pcg_lists(d->H.comp_label, S, d->L);
+    rc = tsb::build_tet_tables(rest_xyz, tets, n, nele, &d->H.comp_label, d->T, g_err);
+  }
+  if (rc != TSB_OK) { delete d; return rc; }
+  tsb::build_coarse_tables(rest_xyz, d->T, d->H.comp_label, d->L, d->C);
+  *n_components = S;
+  *out = d;
+  return TSB_OK;
+}
+
+int tsbdbg_coarse_array(tsbdbg_coarse *d, const char *name, const void **ptr, int64_t *count) {
+  if (!d || !name || !ptr || !count) return TSB_E_INVALID;
+  const tsb::CoarseTables &C = d->C;
+  const std::string k(name);
+#define ARR(nm, vec) if (k == nm) { *ptr = (vec).data(); *count = int64_t((vec).size()); return TSB_OK; }
+  ARR("tet", C.tet) ARR("tets", C.tets) ARR("B", C.B) ARR("tchunk", C.tchunk) ARR("comp_tchunk", C.comp_tchunk) ARR("Y", C.Y)
+  ARR("S", C.S) ARR("vert", d->L.vert) ARR("comp_off", d->L.comp_off) ARR("comp_label", d->H.comp_label)
+#undef ARR
+  return TSB_E_INVALID;
+}
+
+void tsbdbg_coarse_free(tsbdbg_coarse *d) { delete d; }
+
 }  // extern "C"

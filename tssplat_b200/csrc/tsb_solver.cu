@@ -8,6 +8,7 @@
 // component's partials itself, in chunk order, from a column of the partial table that no CTA of that kernel writes.
 // The fold is redundant across the chunks of a component, but it needs no ticket, no atomic and no fence, and every
 // chunk gets bitwise the same scalar.  All scalars stay in device memory.
+#include "tsb_coarse.cuh"
 #include "tsb_device.cuh"
 #include "tsb_jacobi.cuh"
 #include "tsb_sgs.cuh"
@@ -107,8 +108,12 @@ __global__ void __launch_bounds__(kT) pcg_blocks_shift_kernel(const PcgParams s,
   block_inverse<true>(diag, s.n, v, rel_floor, mu, s.pinv, inv_out);
 }
 
-// r = b, z = P r, d = 0, partials of r.z and r.r.  CTAs past the chunk table zero d on the orphan vertices.
-__global__ void __launch_bounds__(kT) pcg_init_kernel(const PcgParams s, const float *__restrict__ b, float *__restrict__ d) {
+// r = b, z = P r, d = 0, partials of r.z and r.r.  CTAs past the chunk table zero d on the orphan vertices.  COARSE:
+// also the partials of R = Z^T r.  Each kernel is a body instantiated by a __global__ of its own name, so the block-Jacobi
+// kernels keep the machine code they had before the coarse variants existed.
+template <bool COARSE>
+__device__ __forceinline__ void pcg_init_body(const PcgParams &s, const float *__restrict__ b, float *__restrict__ d,
+                                              const CoarseParams &co) {
   __shared__ double sh[kT / 32];
   if (int(blockIdx.x) >= s.n_chunks) {
     const int k = (int(blockIdx.x) - s.n_chunks) * kT + int(threadIdx.x);
@@ -118,15 +123,30 @@ __global__ void __launch_bounds__(kT) pcg_init_kernel(const PcgParams s, const f
   const int begin = s.chunk[3 * blockIdx.x + 1], end = s.chunk[3 * blockIdx.x + 2];
   const int e = begin + int(threadIdx.x);
   double rz = 0.0, rr = 0.0;
+  double q[9] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
   if (e < end) {
     const int v = s.vert[e];
     const F3 r = ld3(b, v), z = apply_block(s.pinv, v, r);
     st3(s.r, v, r); st3(s.z, v, z); st3(d, v, F3{0.f, 0.f, 0.f});
     rz = dot3(r, z); rr = dot3(r, r);
+    if constexpr (COARSE) coarse_outer(r, co.Y, e, q);
   }
   rz = block_sum<kT>(rz, sh);
   rr = block_sum<kT>(rr, sh);
   if (threadIdx.x == 0) { s.part[kPartCols * size_t(blockIdx.x) + kRz] = rz; s.part[kPartCols * size_t(blockIdx.x) + kRr] = rr; }
+  if constexpr (COARSE) {
+    __shared__ double sh9[kT / 32 * 9];
+    block_sum9<kT>(q, sh9, co.rpart + 9 * size_t(blockIdx.x));
+  }
+}
+
+__global__ void __launch_bounds__(kT) pcg_init_kernel(const PcgParams s, const float *__restrict__ b, float *__restrict__ d) {
+  pcg_init_body<false>(s, b, d, CoarseParams{});
+}
+
+__global__ void __launch_bounds__(kT) pcg_init_coarse_kernel(const PcgParams s, const float *__restrict__ b, float *__restrict__ d,
+                                                             const CoarseParams co) {
+  pcg_init_body<true>(s, b, d, co);
 }
 
 // Hp + mu p with one rounding per entry, in curvature and update alike
@@ -164,10 +184,11 @@ __device__ __forceinline__ double boundary_tau(double pMp, double dMp, double dM
 // d += alpha p, r -= alpha Hp, z = P r and the partials of the new r.z and r.r.  SHIFT: Hp + mu_c p in place of Hp.
 // TR, with a finite radius Delta_c: p.Hp <= 0, or a step that would end at |d + alpha p|_M >= Delta_c, stops the component
 // on the boundary instead, d += tau p (NEGCURV_BOUNDARY, BOUNDARY); r and z are then left as they were.  With Delta_c =
-// +inf every value written is the one TR = false writes.
-template <bool SHIFT, bool TR>
-__global__ void __launch_bounds__(kT) pcg_update_kernel(const PcgParams s, float *__restrict__ d, int iter,
-                                                        const float *__restrict__ shift, const TrParams t) {
+// +inf every value written is the one TR = false writes.  COARSE: also the partials of R = Z^T r, and NEGCURV_FIRST takes
+// d = p, the first direction (the two-level z).
+template <bool SHIFT, bool TR, bool COARSE>
+__device__ __forceinline__ void pcg_update_body(const PcgParams &s, float *__restrict__ d, int iter, const float *__restrict__ shift,
+                                                const TrParams &t, const CoarseParams &co) {
   __shared__ double sh[kT / 32];
   const int c = s.chunk[3 * blockIdx.x];
   const bool lead = int(blockIdx.x) == s.comp_chunk[c] && threadIdx.x == 0;
@@ -210,7 +231,7 @@ __global__ void __launch_bounds__(kT) pcg_update_kernel(const PcgParams s, float
     }
   }
   if (!(pHp > 0.0)) {
-    if (iter == 0 && e < end) { const int v = s.vert[e]; st3(d, v, ld3(s.z, v)); }
+    if (iter == 0 && e < end) { const int v = s.vert[e]; st3(d, v, ld3(COARSE ? s.p : s.z, v)); }
     if (lead) { C.st_upd = iter == 0 ? TSB_PCG_NEGCURV_FIRST : TSB_PCG_NEGCURV; C.idle = 0; C.n_hvp = iter + 1; }
     if (TR && lead) t.comp[c].step = iter == 0 ? 1.0 : 0.0;
     return;
@@ -218,6 +239,7 @@ __global__ void __launch_bounds__(kT) pcg_update_kernel(const PcgParams s, float
   const double alpha = rz / pHp;
   const float a = float(alpha);
   double nrz = 0.0, nrr = 0.0;
+  double q[9] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
   if (e < end) {
     const int v = s.vert[e];
     const F3 p = ld3(s.p, v), hp = SHIFT ? shifted(ld3(s.Hp, v), p, shift[c]) : ld3(s.Hp, v);
@@ -227,12 +249,29 @@ __global__ void __launch_bounds__(kT) pcg_update_kernel(const PcgParams s, float
     const F3 z = apply_block(s.pinv, v, r);
     st3(d, v, x); st3(s.r, v, r); st3(s.z, v, z);
     nrz = dot3(r, z); nrr = dot3(r, r);
+    if constexpr (COARSE) coarse_outer(r, co.Y, e, q);
   }
   nrz = block_sum<kT>(nrz, sh);
   nrr = block_sum<kT>(nrr, sh);
   if (threadIdx.x == 0) { s.part[kPartCols * size_t(blockIdx.x) + kRz] = nrz; s.part[kPartCols * size_t(blockIdx.x) + kRr] = nrr; }
   if (lead) { C.st_upd = kPcgActive; C.idle = 0; C.n_hvp = iter + 1; C.rz_prev = rz; C.dHd += alpha * alpha * pHp; }
   if (TR && lead) t.comp[c].step = alpha;
+  if constexpr (COARSE) {
+    __shared__ double sh9[kT / 32 * 9];
+    block_sum9<kT>(q, sh9, co.rpart + 9 * size_t(blockIdx.x));
+  }
+}
+
+template <bool SHIFT, bool TR>
+__global__ void __launch_bounds__(kT) pcg_update_kernel(const PcgParams s, float *__restrict__ d, int iter,
+                                                        const float *__restrict__ shift, const TrParams t) {
+  pcg_update_body<SHIFT, TR, false>(s, d, iter, shift, t, CoarseParams{});
+}
+
+template <bool SHIFT, bool TR>
+__global__ void __launch_bounds__(kT) pcg_update_coarse_kernel(const PcgParams s, float *__restrict__ d, int iter,
+                                                               const float *__restrict__ shift, const TrParams t, const CoarseParams co) {
+  pcg_update_body<SHIFT, TR, true>(s, d, iter, shift, t, co);
 }
 
 // The trust-region recurrences (TR), advanced by the lead (Steihaug; r^T p_k = 0 and d_k^T M z_{k+1} = r_{k+1}^T d_k = 0):
@@ -249,9 +288,10 @@ __device__ __forceinline__ void tr_advance(TrComp &T, bool active, double beta, 
 
 // Folds r.z and r.r, tests convergence and sets the next direction p = z + beta p; a stopped component gets p = 0, so
 // later products leave it untouched.  FIRST: the direction of iteration 0 (p = z), which also initialises the state.
-// TR: the lead also advances the trust-region recurrences.
-template <bool FIRST, bool TR>
-__global__ void __launch_bounds__(kT) pcg_dir_kernel(const PcgParams s, float rtol, const TrParams t) {
+// TR: the lead also advances the trust-region recurrences.  COARSE: z is the two-level z + Z E+ R, so r.z gains R^T E+ R
+// (R = Z^T r folded from the chunk partials, every chunk for itself) and p gains (Z E+ R)_v.
+template <bool FIRST, bool TR, bool COARSE>
+__device__ __forceinline__ void pcg_dir_body(const PcgParams s, float rtol, const TrParams t, const CoarseParams co) {
   __shared__ double sh[kT / 32];
   const int c = s.chunk[3 * blockIdx.x];
   const bool lead = int(blockIdx.x) == s.comp_chunk[c] && threadIdx.x == 0;
@@ -260,8 +300,10 @@ __global__ void __launch_bounds__(kT) pcg_dir_kernel(const PcgParams s, float rt
   int st = FIRST ? kPcgActive : C.st_upd;
   float beta = 0.f;
   if (st == kPcgActive) {
-    const double2 f = make_double2(fold(s.part, kRz, s.comp_chunk[c], s.comp_chunk[c + 1], sh),
-                                   fold(s.part, kRr, s.comp_chunk[c], s.comp_chunk[c + 1], sh));   // (r.z, r.r)
+    const double2 f0 = make_double2(fold(s.part, kRz, s.comp_chunk[c], s.comp_chunk[c + 1], sh),
+                                    fold(s.part, kRr, s.comp_chunk[c], s.comp_chunk[c + 1], sh));   // (r.z, r.r)
+    const double2 f = COARSE ? make_double2(f0.x + coarse_fold(co, c, s.comp_chunk[c], s.comp_chunk[c + 1], coarse_shared()), f0.y)
+                             : f0;
     if (FIRST) {
       if (f.y == 0.0) st = TSB_PCG_ZERO_RHS;
       if (lead) { C.rz = f.x; C.rz_prev = f.x; C.bb = f.y; C.rr = f.y; C.dHd = 0.0; C.st_upd = st; C.idle = 0; C.n_hvp = 0; }
@@ -282,10 +324,21 @@ __global__ void __launch_bounds__(kT) pcg_dir_kernel(const PcgParams s, float rt
     F3 p{0.f, 0.f, 0.f};
     if (st == kPcgActive) {
       p = ld3(s.z, v);
+      if constexpr (COARSE) { const F3 g = coarse_prolong(coarse_shared() + 9, co.Y, e); p.x += g.x; p.y += g.y; p.z += g.z; }
       if (!FIRST) { const F3 q = ld3(s.p, v); p.x += beta * q.x; p.y += beta * q.y; p.z += beta * q.z; }
     }
     st3(s.p, v, p);
   }
+}
+
+template <bool FIRST, bool TR>
+__global__ void __launch_bounds__(kT) pcg_dir_kernel(const PcgParams s, float rtol, const TrParams t) {
+  pcg_dir_body<FIRST, TR, false>(s, rtol, t, CoarseParams{});
+}
+
+template <bool FIRST, bool TR>
+__global__ void __launch_bounds__(kT) pcg_dir_coarse_kernel(const PcgParams s, float rtol, const TrParams t, const CoarseParams co) {
+  pcg_dir_body<FIRST, TR, true>(s, rtol, t, co);
 }
 
 // Components still active, for the host's termination test every check_every iterations.
@@ -671,29 +724,40 @@ cudaError_t launch_pcg_blocks_shift(const PcgParams &s, const float *diag, float
 
 // The symmetric Gauss-Seidel mode runs the init and update kernels as they are and overwrites the z and the r.z / r.r
 // partials they wrote (block Jacobi's) with the sweep's, before the direction kernel folds them.
+// The coarse space adds its term in the direction kernel, after the sweep: the init and update kernels' R partials are
+// of r, which the sweep does not change.
 cudaError_t launch_pcg_begin(const PcgParams &s, const float *b, float *d, const TrParams *tr, cudaStream_t st,
-                             const SgsParams *sgs) {
-  pcg_init_kernel<<<with_orphans(s), kT, 0, st>>>(s, b, d);
+                             const SgsParams *sgs, const CoarseParams *co) {
+  if (co) pcg_init_coarse_kernel<<<with_orphans(s), kT, 0, st>>>(s, b, d, *co);
+  else pcg_init_kernel<<<with_orphans(s), kT, 0, st>>>(s, b, d);
   if (sgs) {
     const cudaError_t e = launch_sgs_sweep(s, *sgs, SgsSweep{b, s.z, s.part, kPartCols, kRz, kRr, nullptr, nullptr}, st);
     if (e != cudaSuccess) return e;
   }
-  (tr ? pcg_dir_kernel<true, true> : pcg_dir_kernel<true, false>)<<<unsigned(s.n_chunks), kT, 0, st>>>(s, 0.f, tr ? *tr : TrParams{});
+  const TrParams t = tr ? *tr : TrParams{};
+  if (co) (tr ? pcg_dir_coarse_kernel<true, true> : pcg_dir_coarse_kernel<true, false>)<<<unsigned(s.n_chunks), kT, 0, st>>>(s, 0.f, t, *co);
+  else (tr ? pcg_dir_kernel<true, true> : pcg_dir_kernel<true, false>)<<<unsigned(s.n_chunks), kT, 0, st>>>(s, 0.f, t);
   return cudaGetLastError();
 }
 
 cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, const float *shift, const TrParams *tr,
-                            cudaStream_t st, const SgsParams *sgs) {
+                            cudaStream_t st, const SgsParams *sgs, const CoarseParams *co) {
   const TrParams t = tr ? *tr : TrParams{};
-  (shift ? pcg_curv_kernel<true> : pcg_curv_kernel<false>)<<<unsigned(s.n_chunks), kT, 0, st>>>(s, shift);
-  (shift ? (tr ? pcg_update_kernel<true, true> : pcg_update_kernel<true, false>)
-         : (tr ? pcg_update_kernel<false, true> : pcg_update_kernel<false, false>))<<<unsigned(s.n_chunks), kT, 0, st>>>(
-      s, d, iter, shift, t);
+  const unsigned g = unsigned(s.n_chunks);
+  (shift ? pcg_curv_kernel<true> : pcg_curv_kernel<false>)<<<g, kT, 0, st>>>(s, shift);
+  if (co)
+    (shift ? (tr ? pcg_update_coarse_kernel<true, true> : pcg_update_coarse_kernel<true, false>)
+           : (tr ? pcg_update_coarse_kernel<false, true> : pcg_update_coarse_kernel<false, false>))<<<g, kT, 0, st>>>(
+        s, d, iter, shift, t, *co);
+  else
+    (shift ? (tr ? pcg_update_kernel<true, true> : pcg_update_kernel<true, false>)
+           : (tr ? pcg_update_kernel<false, true> : pcg_update_kernel<false, false>))<<<g, kT, 0, st>>>(s, d, iter, shift, t);
   if (sgs) {
     const cudaError_t e = launch_sgs_sweep(s, *sgs, SgsSweep{s.r, s.z, s.part, kPartCols, kRz, kRr, s.comp, nullptr}, st);
     if (e != cudaSuccess) return e;
   }
-  (tr ? pcg_dir_kernel<false, true> : pcg_dir_kernel<false, false>)<<<unsigned(s.n_chunks), kT, 0, st>>>(s, rtol, t);
+  if (co) (tr ? pcg_dir_coarse_kernel<false, true> : pcg_dir_coarse_kernel<false, false>)<<<g, kT, 0, st>>>(s, rtol, t, *co);
+  else (tr ? pcg_dir_kernel<false, true> : pcg_dir_kernel<false, false>)<<<g, kT, 0, st>>>(s, rtol, t);
   return cudaGetLastError();
 }
 

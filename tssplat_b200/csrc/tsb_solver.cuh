@@ -118,19 +118,40 @@ struct NewtonBacktrack {      // the backtracking options of tsb_newton_tr_step_
 
 struct SgsParams;   // tsb_sgs.cuh: with it, the launchers below apply the symmetric Gauss-Seidel sweep in place of P
 
+// Affine coarse space of the two-level preconditioner P + Z E+ Z^T (tsb_pcg_enable_coarse; tsb_coarse.cu).  Per component
+// c the 9 coarse unknowns are a 3 x 3 matrix A, (Z a)_i = A Y_i with Y_i = X_i - mean_c X (rest positions), so
+// R = Z^T r = sum_i r_i Y_i^T, entry 3 a + b = sum_i r_i[a] Y_i[b].  E+ is the pseudo-inverse of E_c + shift_c (S_c (x) I3).
+constexpr int kCoarseTetT = 256;   // tets per tet chunk (one CTA of the tet pass)
+constexpr int kCoarseUpper = 45;   // unique entries of a symmetric 9 x 9: (a, b), a <= b, rows in order
+struct CoarseParams {
+  const float *Y;              // [rows][3] Y of every entry of PcgParams::vert
+  double *rpart;               // [n_chunks][9] per-chunk partials of R (init / update / restrict write, dir / apply fold)
+  const int32_t *tchunk;       // [3 * n_tchunks] (component, begin, end) into the component-sorted tet list
+  const int32_t *comp_tchunk;  // [n_components + 1] first tet chunk of every component
+  const int32_t *tet;          // [nele] tet ids grouped by component
+  const int4 *tets;            // [nele] their vertex ids
+  const float *B;              // [9][nele] their rest inverse Dm^-1
+  double *epart;               // [n_tchunks][45] per-chunk partials of E_c (upper triangle)
+  const double *S;             // [n_components][6] sum_i Y_i Y_i^T: 00 11 22 12 02 01
+  double *Einv;                // [n_components][81] E+
+  int32_t n_tchunks, nele;
+  float floor;                 // eigenvalues <= floor * lambda_max give 0
+};
+
 cudaError_t launch_pcg_blocks(const PcgParams &s, const float *diag, float rel_floor, float *inv_out, cudaStream_t st);
 // blocks D_v + shift[c] I (over the chunk table; orphan vertices unshifted)
 cudaError_t launch_pcg_blocks_shift(const PcgParams &s, const float *diag, float rel_floor, const float *shift, float *inv_out,
                                     cudaStream_t st);
 // r = b, z = P r, d = 0 and the first direction; leaves every component ACTIVE or ZERO_RHS
 // (tr != nullptr: also initialises the trust-region recurrences; sgs != nullptr: z = M^-1 r by one sweep)
+// (co != nullptr: the two-level preconditioner, z + Z E+ Z^T r, in the direction and in r.z)
 cudaError_t launch_pcg_begin(const PcgParams &s, const float *b, float *d, const TrParams *tr, cudaStream_t st,
-                             const SgsParams *sgs = nullptr);
+                             const SgsParams *sgs = nullptr, const CoarseParams *co = nullptr);
 // after Hp = H p of iteration `iter` (0-based) is complete on the stream: curvature, update and next direction; with
 // shift != nullptr the operator is H + shift[c] I; with tr != nullptr every component stays inside its radius; with
 // sgs != nullptr z = M^-1 r by one sweep after the update
 cudaError_t launch_pcg_step(const PcgParams &s, float *d, int iter, float rtol, const float *shift, const TrParams *tr,
-                            cudaStream_t st, const SgsParams *sgs = nullptr);
+                            cudaStream_t st, const SgsParams *sgs = nullptr, const CoarseParams *co = nullptr);
 cudaError_t launch_pcg_count(const PcgParams &s, cudaStream_t st);
 cudaError_t launch_pcg_records(const PcgParams &s, const float *b, const float *d, tsb_pcg_sphere_t *out, cudaStream_t st);
 cudaError_t launch_sphere_axpy(const PcgParams &s, const float *x, const float *a, const float *d, float *out, cudaStream_t st);
@@ -149,6 +170,19 @@ cudaError_t launch_newton_decide(const PcgParams &s, const NewtonParams &w, cons
 // first step, the fp32 radius
 cudaError_t launch_newton_tr_radius(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t, const NewtonTrRule &r,
                                     cudaStream_t st, const SgsParams *sgs = nullptr);
+// Coarse space (tsb_coarse.cu).  Per-chunk partials of E_c at x: exact (activity from det F in fp64; c2, c3 weights) or,
+// with q != nullptr, the projected operators of q's last projection
+struct PsdParams;
+cudaError_t launch_coarse_tets(const CoarseParams &co, const float *x, int order, float c2, float c3, const PsdParams *q,
+                               cudaStream_t st);
+// E+ of every component from the partials, with E_c + shift_c (S_c (x) I3) (shift may be null: unshifted); with
+// E_out != nullptr the unshifted E_c (81 per component) goes there instead and E+ is left as it is
+cudaError_t launch_coarse_factor(const PcgParams &s, const CoarseParams &co, const float *shift, double *E_out, cudaStream_t st);
+// the R partials of v, per chunk
+cudaError_t launch_coarse_restrict(const PcgParams &s, const CoarseParams &co, const float *v, cudaStream_t st);
+// z = P r + Z E+ Z^T r (jacobi) or z += Z E+ Z^T r (after the sweep wrote z), on the vertices of the chunk table; the R
+// partials of r must be in place (launch_coarse_restrict)
+cudaError_t launch_coarse_apply(const PcgParams &s, const CoarseParams &co, const float *r, float *z, bool jacobi, cudaStream_t st);
 // trust-region step: acceptance, radius update, records (out may be null); bt != nullptr: a rejected step is backtracked
 // along the line search's n_alpha step sizes (tsb_newton_tr_step_ex)
 cudaError_t launch_newton_tr_decide(const PcgParams &s, const NewtonParams &w, const NewtonTrParams &t, const NewtonTrRule &r,

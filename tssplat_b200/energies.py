@@ -148,7 +148,8 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
     model of ``device_pcg``, which ``newton_direction``, ``newton_step`` and ``prox_step`` solve with: ``"psd"`` is the
     projected Hessian (``newton.DevicePCG``).  ``newton_precond`` (default ``"jacobi"``) selects that workspace's
     preconditioner: ``"sgs"`` is the multicolour block symmetric Gauss-Seidel preconditioner built from the assembled
-    Hessian, which ``newton_direction``, ``newton_step``, ``prox_step`` and ``hessian`` then share.
+    Hessian, which ``newton_direction``, ``newton_step``, ``prox_step`` and ``hessian`` then share.  ``newton_coarse``
+    (default ``None``) set to ``"affine"`` adds the affine coarse space to that preconditioner (``newton.DevicePCG``).
     """
 
     #: the AMIPS coefficient; a class default, so that a module assembled without ``__init__`` (as ``bench.py`` does)
@@ -230,7 +231,8 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         pcg = getattr(self, "device_pcg", None)
         if pcg is None:
             pcg = self.device_pcg = DevicePCG(self.tet_sp, hessian=getattr(self.FLAGS, "newton_hessian", "exact") or "exact",
-                                              precond=getattr(self.FLAGS, "newton_precond", "jacobi") or "jacobi")
+                                              precond=getattr(self.FLAGS, "newton_precond", "jacobi") or "jacobi",
+                                              coarse=getattr(self.FLAGS, "newton_coarse", None) or None)
         return pcg
 
     def newton_direction(self, x, it, b=None, **solve_kw):
@@ -246,6 +248,8 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         if b is None:
             _, g = self.tet_sp.energy_grad(xd, c1, c2, order, -1.0, c3=self.amips_coeff)
             b = g.reshape(x.shape)
+        if pcg.coarse is not None:
+            pcg.set_coarse(xd, c1, c2, order, c3=self.amips_coeff)
         if pcg.precond == "sgs":    # the diagonal of the matrix the sweep uses
             pcg.set_blocks(pcg.set_matrix(xd, c1, c2, order, c3=self.amips_coeff))
         else:

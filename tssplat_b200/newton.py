@@ -140,6 +140,8 @@ class DevicePCGResult(NamedTuple):
 HESSIANS = ("exact", "psd")
 #: preconditioners of ``DevicePCG``: block Jacobi, or multicolour block symmetric Gauss-Seidel from the assembled Hessian
 PRECONDS = ("jacobi", "sgs")
+#: coarse spaces of ``DevicePCG``: none, or the 9 linear affine motions of every sphere
+COARSES = (None, "affine")
 
 
 class DevicePCG:
@@ -150,9 +152,14 @@ class DevicePCG:
     block symmetric Gauss-Seidel preconditioner built from the assembled Hessian (``tsb_pcg_enable_sgs``): the workspace
     creates and owns a ``DeviceHessian`` in its mode (``hessian_ws``, usable while the workspace lives), ``set_matrix``
     assembles the matrix the sweep uses and returns its diagonal planes for ``set_blocks``, and ``apply_precond`` and
-    ``colors`` are available.  Creating it allocates, so not inside a CUDA graph capture."""
+    ``colors`` are available.  ``coarse="affine"`` adds the affine coarse space on top of that preconditioner
+    (``tsb_pcg_enable_coarse``): ``P + Z E+ Z^T`` with the sphere's 9 linear affine motions as ``Z`` and ``E+`` the
+    pseudo-inverse of ``Z^T H Z`` (eigenvalues at or below ``coarse_floor * lambda_max`` dropped); ``set_coarse`` forms it at
+    a point, ``set_blocks`` refactors it with its shift, ``coarse_matrix`` returns ``Z^T H Z`` and ``apply_precond`` applies
+    the whole two-level preconditioner.  Creating it allocates, so not inside a CUDA graph capture."""
 
-    def __init__(self, tet_sp, hessian: str = "exact", precond: str = "jacobi"):
+    def __init__(self, tet_sp, hessian: str = "exact", precond: str = "jacobi", coarse: Optional[str] = None,
+                 coarse_floor: float = 1e-8):
         from . import _capi
         from .tet_spheres_ext import _stream_ptr
         self._capi, self._stream_ptr = _capi, _stream_ptr
@@ -165,7 +172,11 @@ class DevicePCG:
             raise RuntimeError('DevicePCG(hessian="psd") allocates device memory and cannot be created during a CUDA graph capture')
         if precond == "sgs" and torch.cuda.is_current_stream_capturing():
             raise RuntimeError('DevicePCG(precond="sgs") allocates device memory and cannot be created during a CUDA graph capture')
-        self.tet_sp, self.hessian, self.precond = tet_sp, hessian, precond
+        if coarse not in COARSES:
+            raise ValueError(f"coarse must be one of {COARSES}, got {coarse!r}")
+        if coarse is not None and torch.cuda.is_current_stream_capturing():
+            raise RuntimeError('DevicePCG(coarse="affine") allocates device memory and cannot be created during a CUDA graph capture')
+        self.tet_sp, self.hessian, self.precond, self.coarse = tet_sp, hessian, precond, coarse
         self.hessian_ws = None
         s = C.c_void_p()
         rc = _capi.lib.tsb_pcg_create(tet_sp._h, C.byref(s))
@@ -184,6 +195,10 @@ class DevicePCG:
             # the garbage collector could otherwise free (cudaFree) in the middle of a later CUDA graph capture
             self.hessian_ws.pcg = weakref.proxy(self)
             self._check(_capi.lib.tsb_pcg_enable_sgs(s, self.hessian_ws._hs), "__init__")
+        if coarse is not None:
+            rc = _capi.lib.tsb_pcg_enable_coarse(s, tet_sp.vertices.ctypes.data, tet_sp.elements.ctypes.data, int(tet_sp.nele),
+                                                 float(coarse_floor))
+            self._check(rc, "__init__")
         self.device_bytes = int(_capi.lib.tsb_pcg_device_bytes(s))
 
     def __del__(self):
@@ -288,9 +303,11 @@ class DevicePCG:
 
     def apply_precond(self, r: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``M^-1 r`` on every sphere with the symmetric Gauss-Seidel preconditioner of the last ``set_matrix`` and
-        ``set_blocks`` (``tsb_pcg_apply_precond``), in ``r``'s shape; 0 on vertices no tet references.  ``out`` (not
-        ``r``): a contiguous float32 tensor of 3n entries, returned (then no allocation)."""
-        self._need_sgs("apply_precond")
+        ``set_blocks`` (``tsb_pcg_apply_precond``), in ``r``'s shape.  Vertices no tet references are 0 in a new tensor and
+        left as they are in ``out`` (not ``r``): a contiguous float32 tensor of 3n entries, returned (then no allocation).  On a ``coarse`` workspace it is
+        the two-level ``P r + Z E+ Z^T r`` (``P`` block Jacobi or the sweep) at the last ``set_coarse`` and ``set_blocks``."""
+        if self.precond != "sgs" and self.coarse is None:
+            raise RuntimeError('DevicePCG.apply_precond needs a workspace created with precond="sgs" or coarse="affine"')
         n3 = self.tet_sp.n3
         rc_ = self._f32(r, n3, "r")
         if out is None:
@@ -300,6 +317,29 @@ class DevicePCG:
         rc = self._capi.lib.tsb_pcg_apply_precond(self._s, rc_.data_ptr(), out.data_ptr(), self._stream_ptr(self.tet_sp.device))
         self._check(rc, "apply_precond")
         return out.reshape(r.shape)
+
+    def _need_coarse(self, what: str) -> None:
+        if self.coarse is None:
+            raise RuntimeError(f'DevicePCG.{what} needs a workspace created with coarse="affine"')
+
+    def set_coarse(self, x: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0) -> None:
+        """Forms every sphere's coarse matrix ``Z^T H Z`` at ``x`` (exact, or projected with ``hessian="psd"``) and its
+        unshifted pseudo-inverse (``tsb_pcg_set_coarse``); a following ``set_blocks`` with a shift refactors it with
+        ``shift_c (S_c (x) I3)``.  No host sync, no allocation: capturable."""
+        self._need_coarse("set_coarse")
+        xc = self._f32(x, self.tet_sp.n3, "x")
+        terms = self._capi.tsb_terms_t(c1=float(c1), c2=float(c2), order=int(order), c3=float(c3))
+        rc = self._capi.lib.tsb_pcg_set_coarse(self._s, xc.data_ptr(), C.byref(terms), self._stream_ptr(self.tet_sp.device))
+        self._check(rc, "set_coarse")
+
+    def coarse_matrix(self) -> torch.Tensor:
+        """float64 [S, 9, 9]: every sphere's unshifted ``Z^T H Z`` of the last ``set_coarse``, coarse unknowns the 3 x 3
+        matrix ``A`` row-major (``tsb_pcg_coarse_matrix``; synchronises the device)."""
+        self._need_coarse("coarse_matrix")
+        out = torch.empty((self.n_spheres, 9, 9), dtype=torch.float64, device=self.tet_sp.device)
+        torch.cuda.synchronize(self.tet_sp.device)
+        self._check(self._capi.lib.tsb_pcg_coarse_matrix(self._s, out.data_ptr()), "coarse_matrix")
+        return out
 
     @property
     def colors(self) -> torch.Tensor:
@@ -427,10 +467,13 @@ class DeviceNewton:
     ``"exact"`` or ``"psd"`` (the projected Hessian, see ``DevicePCG``); ``None`` takes ``pcg``'s, or ``"exact"`` when a
     workspace is created.  A given ``pcg`` of another mode is an error.  ``precond`` follows the same rules: ``"jacobi"``
     or ``"sgs"`` (see ``DevicePCG``); on an SGS workspace every step assembles the Hessian and takes its preconditioner
-    diagonal from it."""
+    diagonal from it.  ``coarse``: ``None`` or ``"affine"`` (see ``DevicePCG``), taken from ``pcg`` when one is given (a
+    different value is an error); on a coarse workspace every damped and proximal step forms the coarse matrix at its
+    point, and ``tr_step`` / ``trls_step`` are refused (``tsb_newton_tr_step``: the two-level norm is near-singular along
+    the coarse modes and the trust-region steps stall)."""
 
     def __init__(self, tet_sp, pcg: Optional[DevicePCG] = None, hessian: Optional[str] = None,
-                 precond: Optional[str] = None):
+                 precond: Optional[str] = None, coarse: Optional[str] = None):
         from . import _capi
         from .tet_spheres_ext import _stream_ptr
         self._capi, self._stream_ptr = _capi, _stream_ptr
@@ -439,15 +482,19 @@ class DeviceNewton:
             raise ValueError(f"hessian must be one of {HESSIANS}, got {hessian!r}")
         if precond is not None and precond not in PRECONDS:
             raise ValueError(f"precond must be one of {PRECONDS}, got {precond!r}")
+        if coarse not in COARSES:
+            raise ValueError(f"coarse must be one of {COARSES}, got {coarse!r}")
         if pcg is None:
-            pcg = DevicePCG(tet_sp, hessian=hessian or "exact", precond=precond or "jacobi")
+            pcg = DevicePCG(tet_sp, hessian=hessian or "exact", precond=precond or "jacobi", coarse=coarse)
         elif pcg.tet_sp is not tet_sp:
             raise RuntimeError("DeviceNewton: pcg belongs to another handle")
         elif hessian is not None and pcg.hessian != hessian:
             raise RuntimeError(f"DeviceNewton: hessian={hessian!r} but pcg was created with hessian={pcg.hessian!r}")
         elif precond is not None and pcg.precond != precond:
             raise RuntimeError(f"DeviceNewton: precond={precond!r} but pcg was created with precond={pcg.precond!r}")
-        self.hessian, self.precond = pcg.hessian, pcg.precond
+        elif coarse is not None and pcg.coarse != coarse:
+            raise RuntimeError(f"DeviceNewton: coarse={coarse!r} but pcg was created with coarse={pcg.coarse!r}")
+        self.hessian, self.precond, self.coarse = pcg.hessian, pcg.precond, pcg.coarse
         self.tet_sp, self.pcg, self.n_spheres = tet_sp, pcg, pcg.n_spheres
         nw = C.c_void_p()
         rc = _capi.lib.tsb_newton_create(pcg._s, C.byref(nw))
