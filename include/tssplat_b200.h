@@ -20,7 +20,7 @@
 extern "C" {
 #endif
 
-#define TSB_VERSION 12
+#define TSB_VERSION 13
 #define TSB_LINE_MAX_ALPHA 8   /* step sizes one tsb_line_search call may evaluate */
 
 enum {
@@ -565,7 +565,8 @@ const char *tsb_newton_last_error(tsb_newton_t nw);   /* nw may be NULL: last ts
 int64_t tsb_newton_device_bytes(tsb_newton_t nw);
 
 /* Marks every sphere ACTIVE with mu not initialised (one memset on the stream; capturable); after a tsb_newton_tr_step
- * also the trust-region radius (a second memset). */
+ * also the trust-region radius (a second memset), and after a tsb_newton_lbfgs_step every sphere's L-BFGS history is
+ * emptied (another memset). */
 int tsb_newton_reset(tsb_newton_t nw, void *stream);
 
 enum {
@@ -757,6 +758,74 @@ typedef struct {            /* 32 bytes */
 int tsb_newton_tr_step_ex(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const float *weight_dev,
                           const tsb_terms_t *terms, const tsb_newton_tr_options_t *opt, const tsb_newton_backtrack_t *bt,
                           tsb_newton_tr_sphere_t *records_out_dev, void *stream);
+
+/* ---- L-BFGS step: per-sphere quasi-Newton steps from gradients and the line search, no Hessian products -----------
+ * Minimises E (anchor_dev = weight_dev = NULL) or the proximal objective Phi_c = E_c + (w_c / 2)|x_c - y_c|^2 (both set,
+ * with tsb_newton_prox_step's semantics for the right-hand side, the d.(x - y) term and an unusable weight) by one
+ * limited-memory BFGS step per sphere.  Every sphere keeps its own history of up to m pairs (s_i, y_i) (the Hessian is
+ * block diagonal by sphere), and the initial inverse Hessian is H0 = P, the block-Jacobi preconditioner a damped step
+ * on this workspace builds with mu = 0, rebuilt at every step's x.  On one stream, without any host read (capturable in
+ * a CUDA graph after the first call):
+ *   1. b = -grad Phi(x) (one gradient launch, gradH = -1; b_c = 0 on frozen spheres and where w_c is unusable);
+ *   2. tsb_hess_diag and tsb_pcg_set_blocks_ex with shift w_c (prox) or none: H0 = P;
+ *   3. the direction kernel, one CTA per sphere, the history in global memory (no limit on a sphere's size):
+ *      if the sphere moved on the previous step, s = x - x_prev (from a stored fp32 copy of x, so an x edited between
+ *      calls is still right) and y = b_prev - b; the pair is kept, the oldest dropped from a full ring, when
+ *      s.y > curv_eps |s| |y| (fp64);  the two-loop recursion with H0 = P, fp32 vectors and fp64 rho_i = 1 / s_i.y_i,
+ *      alpha_i and dots;  if b.d <= 0 on a sphere with a history, the history is cleared and d = P b;  then x_prev, b_prev
+ *      and the per-sphere b.b, b.d, |d|^2 (prox: d.(x - y)) in fp64;
+ *   4. tsb_line_search at alpha_k = 2^-k, k < n_alpha, per sphere;  5. the decision below;  6. tsb_sphere_axpy in place.
+ * Decision per sphere c, in fp64, with g = |b_c|, bd = b.d, dd = |d|^2, dPhi_k = dE_k + w_c (alpha_k d.(x - y) +
+ * alpha_k^2 dd / 2) (dE_k for the plain objective; tsb_newton_prox_step's dPhi) and alpha^ the inversion-free step:
+ *   frozen: alpha = 0.  An unusable w_c: STALLED, frozen.  g <= gtol: CONVERGED, frozen.
+ *   k* = the smallest k with alpha_k < eta alpha^ and dPhi_k <= -sigma alpha_k bd (tsb_newton_step's Armijo test);
+ *   none (or bd <= 0): no step, and the history is cleared; no step from an empty history (d = P b): STALLED, frozen.
+ * records_out_dev (optional, device [info.n_components]) receives one tsb_newton_lbfgs_sphere_t per sphere.  No
+ * floating-point atomics in the new kernels and every fold in a fixed order (one CTA owns a sphere: a fixed shuffle tree,
+ * then the warps in order): on a deterministic handle x and the records are bitwise identical across calls, streams and
+ * graph replays, and a sphere's trajectory depends on its own start, anchor and weight only.  Vertices no tet references
+ * never move.  With every w_c = 0 the call gives bitwise the x and records of the call without an anchor.
+ * State: the pairs (m + 1 slots of s and y per vertex: the slot being filled never holds a kept pair), x_prev, b_prev,
+ * rho and a 64-byte record per sphere (ring head, count, whether it moved, the direction's dots), allocated by the first
+ * call; tsb_newton_device_bytes grows by
+ *   24 (m + 2) rows + 8 (m + 1) n_components + 64 n_components   bytes
+ * (rows = vertices some tet references).  tsb_newton_reset empties every history (on a workspace that has one).  Make the
+ * first call outside any stream capture: on a stream being captured it returns TSB_E_INVALID.  m is fixed by that call.
+ * Argument errors (TSB_E_INVALID, nothing launched): a null nw, x_dev, terms or opt, exactly one of anchor_dev and
+ * weight_dev null, anchor_dev == x_dev, an option outside its range (NaN included), nonzero reserved words, an m other
+ * than the workspace's first one, an order other than 2 or 4, terms->c3 != 0 on a handle without enable_amips, a
+ * negative coefficient on a projected-Hessian workspace, a workspace with the SGS preconditioner or the coarse space (H0
+ * is block Jacobi only).  DESIGN.md section 5, "L-BFGS step". */
+#define TSB_LBFGS_MAX_M 16
+typedef struct {            /* 64 bytes */
+  int32_t m;                /* 1..TSB_LBFGS_MAX_M: pairs kept per sphere; fixed by the workspace's first L-BFGS call    */
+  float gtol;               /* >= 0: a sphere with |grad_c| <= gtol is CONVERGED                                     */
+  float sigma;              /* in (0, 1): Armijo constant                                                            */
+  float eta;                /* in (0, 1]: a step must lie below eta times the sphere's inversion-free step            */
+  int32_t n_alpha;          /* 1..TSB_LINE_MAX_ALPHA: step sizes 1, 1/2, ..., 2^-(n_alpha - 1)                       */
+  float rel_floor;          /* >= 0: H0's eigenvalue floor (tsb_pcg_set_blocks)                                      */
+  float curv_eps;           /* >= 0, finite: a pair is kept only if s.y > curv_eps |s| |y| (fp64)                    */
+  int32_t reserved[9];      /* must be 0                                                                             */
+} tsb_newton_lbfgs_options_t;
+
+typedef struct {            /* one per component, component order of tsb_energy_grad_spheres; 64 bytes               */
+  float grad_norm;          /* |grad_c| at x before the step (0 on a sphere already frozen)                          */
+  float alpha;              /* the step taken (0: none)                                                              */
+  float delta;              /* Phi_c(x + alpha d) - Phi_c(x) of the step taken (0 if none)                            */
+  float b_dot_d;            /* b_c . d_c, b = -grad                                                                   */
+  float d_norm;             /* |d_c|                                                                                  */
+  int32_t k;                /* index of the step size taken, -1 when none                                            */
+  int32_t status;           /* TSB_NEWTON_* after the step                                                           */
+  int32_t n_pairs;          /* pairs held after the step                                                             */
+  int32_t pair_kept;        /* -1: no pair this step (the sphere did not move), 0: rejected by the curvature test, 1: kept */
+  int32_t history_cleared;  /* 1: the history was cleared this step (b.d <= 0, or no step)                            */
+  int32_t first_vertex;     /* its lowest vertex id                                                                  */
+  int32_t reserved[5];
+} tsb_newton_lbfgs_sphere_t;
+
+int tsb_newton_lbfgs_step(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const float *weight_dev,
+                          const tsb_terms_t *terms, const tsb_newton_lbfgs_options_t *opt,
+                          tsb_newton_lbfgs_sphere_t *records_out_dev, void *stream);
 
 /* Same computation for callers whose vertex positions live in HOST memory (e.g. a CPU-side
  * optimiser): copies x_host -> device, runs the fused launch, copies energy[3] and grad back,

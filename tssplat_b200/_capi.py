@@ -15,6 +15,7 @@ LIB_PATH = os.environ.get("TSSPLAT_B200_LIB") or _build.LIB_PATH
 
 TSB_OK, TSB_E_INVALID, TSB_E_MESH, TSB_E_CUDA, TSB_E_NOMEM = 0, -1, -2, -3, -4
 TSB_LINE_MAX_ALPHA = 8
+TSB_LBFGS_MAX_M = 16
 TSB_PCG_MAXITER, TSB_PCG_CONVERGED, TSB_PCG_NEGCURV, TSB_PCG_NEGCURV_FIRST, TSB_PCG_ZERO_RHS = 0, 1, 2, 3, 4
 TSB_PCG_BOUNDARY, TSB_PCG_NEGCURV_BOUNDARY = 5, 6
 TSB_NEWTON_ACTIVE, TSB_NEWTON_CONVERGED, TSB_NEWTON_STALLED = 0, 1, 2
@@ -29,7 +30,8 @@ EXPORTED_SYMBOLS = (
     "tsb_hessian_assemble", "tsb_pcg_enable_sgs", "tsb_pcg_set_matrix", "tsb_pcg_apply_precond", "tsb_pcg_sgs_colors",
     "tsb_pcg_enable_coarse", "tsb_pcg_set_coarse", "tsb_pcg_coarse_matrix",
     "tsb_newton_create", "tsb_newton_destroy", "tsb_newton_last_error", "tsb_newton_device_bytes", "tsb_newton_reset",
-    "tsb_newton_step", "tsb_newton_prox_step", "tsb_newton_tr_step", "tsb_newton_tr_step_ex", "tsb_energy_grad_host", "tsb_scale",
+    "tsb_newton_step", "tsb_newton_prox_step", "tsb_newton_tr_step", "tsb_newton_tr_step_ex", "tsb_newton_lbfgs_step",
+    "tsb_energy_grad_host", "tsb_scale",
     "tsb_grad_limit", "tsb_adam_uniform_step",
     "tsb_surface_create", "tsb_surface_destroy", "tsb_surface_last_error", "tsb_surface_forward", "tsb_surface_backward",
     "tsb_surface_extract", "tsb_free_host", "tsb_setup_last_error",
@@ -87,6 +89,18 @@ class tsb_newton_tr_sphere_t(C.Structure):
 
 class tsb_newton_backtrack_t(C.Structure):
     _fields_ = [("n_alpha", C.c_int32), ("sigma", C.c_float), ("reserved", C.c_int32 * 6)]
+
+
+class tsb_newton_lbfgs_options_t(C.Structure):
+    _fields_ = [("m", C.c_int32), ("gtol", C.c_float), ("sigma", C.c_float), ("eta", C.c_float), ("n_alpha", C.c_int32),
+                ("rel_floor", C.c_float), ("curv_eps", C.c_float), ("reserved", C.c_int32 * 9)]
+
+
+class tsb_newton_lbfgs_sphere_t(C.Structure):
+    _fields_ = [("grad_norm", C.c_float), ("alpha", C.c_float), ("delta", C.c_float), ("b_dot_d", C.c_float),
+                ("d_norm", C.c_float), ("k", C.c_int32), ("status", C.c_int32), ("n_pairs", C.c_int32),
+                ("pair_kept", C.c_int32), ("history_cleared", C.c_int32), ("first_vertex", C.c_int32),
+                ("reserved", C.c_int32 * 5)]
 
 
 class tsb_info_t(C.Structure):
@@ -218,6 +232,8 @@ def _load() -> C.CDLL:
     lib.tsb_newton_tr_step_ex.restype = C.c_int
     lib.tsb_newton_tr_step_ex.argtypes = [vp, vp, vp, vp, C.POINTER(tsb_terms_t), C.POINTER(tsb_newton_tr_options_t),
                                           C.POINTER(tsb_newton_backtrack_t), vp, vp]
+    lib.tsb_newton_lbfgs_step.restype = C.c_int
+    lib.tsb_newton_lbfgs_step.argtypes = [vp, vp, vp, vp, C.POINTER(tsb_terms_t), C.POINTER(tsb_newton_lbfgs_options_t), vp, vp]
     lib.tsb_energy_grad_host.restype = C.c_int
     lib.tsb_energy_grad_host.argtypes = [vp, vp, f32, f32, i32, f32, vp, vp, vp]
     lib.tsb_scale.restype = C.c_int

@@ -13,8 +13,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_PATH = os.path.join(HERE, "libtssplat_b200.so")
-SOURCES = ["tsb_plan.cpp", "tsb_kernels.cu", "tsb_capi.cu", "tsb_solver.cu", "tsb_psd.cu", "tsb_hessian.cu", "tsb_sgs.cu", "tsb_coarse.cu", "tsb_surface.cu", "tsb_setup.cu"]
-HEADERS = ["tsb_plan.h", "tsb_kernels.cuh", "tsb_solver.cuh", "tsb_device.cuh", "tsb_jacobi.cuh", "tsb_psd.cuh", "tsb_hessian.cuh", "tsb_sgs.cuh", "tsb_coarse.cuh", os.path.join("..", "..", "include", "tssplat_b200.h")]
+SOURCES = ["tsb_plan.cpp", "tsb_kernels.cu", "tsb_capi.cu", "tsb_solver.cu", "tsb_psd.cu", "tsb_hessian.cu", "tsb_sgs.cu", "tsb_coarse.cu", "tsb_lbfgs.cu", "tsb_surface.cu", "tsb_setup.cu"]
+HEADERS = ["tsb_plan.h", "tsb_kernels.cuh", "tsb_solver.cuh", "tsb_device.cuh", "tsb_jacobi.cuh", "tsb_psd.cuh", "tsb_hessian.cuh", "tsb_sgs.cuh", "tsb_coarse.cuh", "tsb_lbfgs.cuh", os.path.join("..", "..", "include", "tssplat_b200.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",

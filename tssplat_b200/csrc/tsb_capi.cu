@@ -10,6 +10,7 @@
 #include "../../include/tssplat_b200.h"
 #include "tsb_hessian.cuh"
 #include "tsb_kernels.cuh"
+#include "tsb_lbfgs.cuh"
 #include "tsb_plan.h"
 #include "tsb_psd.cuh"
 #include "tsb_sgs.cuh"
@@ -22,6 +23,8 @@ static_assert(sizeof(tsb_newton_sphere_t) == 64, "tsb_newton_sphere_t must be 64
 static_assert(sizeof(tsb_newton_tr_options_t) == 64, "tsb_newton_tr_options_t must be 64 bytes");
 static_assert(sizeof(tsb_newton_tr_sphere_t) == 64, "tsb_newton_tr_sphere_t must be 64 bytes");
 static_assert(sizeof(tsb_newton_backtrack_t) == 32, "tsb_newton_backtrack_t must be 32 bytes");
+static_assert(sizeof(tsb_newton_lbfgs_options_t) == 64, "tsb_newton_lbfgs_options_t must be 64 bytes");
+static_assert(sizeof(tsb_newton_lbfgs_sphere_t) == 64, "tsb_newton_lbfgs_sphere_t must be 64 bytes");
 
 struct tsb_handle_s {
   int device = 0;
@@ -77,6 +80,7 @@ struct tsb_newton_s {
   double *prox_part = nullptr;       // [chunks] d.(x - y) partials of tsb_newton_prox_step (allocated by its first call)
   tsb::TrState *tr_state = nullptr;  // [n_components] trust-region radius state (allocated by the first tsb_newton_tr_step)
   float *tr_radius = nullptr;        // [n_components] its fp32 radius, handed to tsb_pcg_solve_tr
+  tsb::LbfgsParams lb{};             // L-BFGS history and state (allocated by the first tsb_newton_lbfgs_step; lb.m = 0 before)
   int64_t device_bytes = 0;
   std::vector<void *> allocs;
   std::string err;
@@ -881,6 +885,7 @@ int tsb_newton_reset(tsb_newton_t nw, void *stream) {
   const size_t S = size_t(nw->s->P.n_components);
   cudaError_t e = cudaMemsetAsync(nw->W.comp, 0, S * sizeof(tsb::NewtonComp), static_cast<cudaStream_t>(stream));
   if (e == cudaSuccess && nw->tr_state) e = cudaMemsetAsync(nw->tr_state, 0, S * sizeof(tsb::TrState), static_cast<cudaStream_t>(stream));
+  if (e == cudaSuccess && nw->lb.comp) e = cudaMemsetAsync(nw->lb.comp, 0, S * sizeof(tsb::LbfgsComp), static_cast<cudaStream_t>(stream));
   if (e != cudaSuccess) return fail(nw, TSB_E_CUDA, std::string("reset: ") + cudaGetErrorString(e));
   return TSB_OK;
 }
@@ -907,16 +912,25 @@ std::string rule_error(const tsb_newton_tr_options_t &o) {
   return "";
 }
 
-// The argument rules of every Newton step: the pointers, the proximal pair (anchor_dev and weight_dev both null: objective
-// E, or both set, the anchor not x), the options all steps have, those of the step's kind (O), and the terms.
-template <class O>
-int newton_check(tsb_newton_t nw, const float *x_dev, const float *anchor_dev, const float *weight_dev, const tsb_terms_t *terms,
-                 const O *opt) {
+// The pointer rules of every Newton step: x, terms and opt set, the proximal pair (anchor_dev and weight_dev both null:
+// objective E, or both set, the anchor not x).
+int newton_pointers_check(tsb_newton_t nw, const float *x_dev, const float *anchor_dev, const float *weight_dev,
+                          const tsb_terms_t *terms, const void *opt) {
   if (!x_dev || !terms || !opt) return fail(nw, TSB_E_INVALID, "x_dev, terms and opt must be non-null");
   if (!anchor_dev != !weight_dev)
     return fail(nw, TSB_E_INVALID, "anchor_dev and weight_dev must be both null (objective E) or both set (proximal objective)");
   if (anchor_dev && anchor_dev == x_dev)
     return fail(nw, TSB_E_INVALID, "anchor_dev must not be x_dev: x is updated in place while the anchor is read");
+  return TSB_OK;
+}
+
+// The argument rules of every Newton step: the pointers, the options all steps have, those of the step's kind (O), and
+// the terms.
+template <class O>
+int newton_check(tsb_newton_t nw, const float *x_dev, const float *anchor_dev, const float *weight_dev, const tsb_terms_t *terms,
+                 const O *opt) {
+  const int rc = newton_pointers_check(nw, x_dev, anchor_dev, weight_dev, terms, opt);
+  if (rc != TSB_OK) return rc;
   const O &o = *opt;
   if (o.max_iter < 1) return fail(nw, TSB_E_INVALID, "max_iter must be >= 1");
   if (!(o.rtol >= 0.f)) return fail(nw, TSB_E_INVALID, "rtol must be >= 0");
@@ -956,6 +970,30 @@ struct NewtonStep {
         rel_floor(o.rel_floor), n_alpha(b ? b->n_alpha : 1) {}
 };
 
+// The first phases of every Newton step: b = -grad at x, the diagonal blocks (from the assembled matrix on an SGS
+// workspace), E_c on a coarse workspace, then the prep kernel: b_c = 0 on frozen spheres (prox: b -= w (x - y)).
+int newton_rhs(tsb_newton_t nw, const float *x_dev, const tsb_terms_t *terms, const tsb::ProxParams *prox, cudaStream_t st) {
+  tsb_pcg_t s = nw->s;
+  tsb_handle_t h = s->h;
+  const tsb::NewtonParams &W = nw->W;
+  int rc = energy_grad_impl(h, x_dev, terms->c1, terms->c2, terms->c3, terms->order, -1.f, nullptr, nw->energy, 1, W.b, nullptr, st);
+  if (rc != TSB_OK) return fail(nw, rc, h->err);
+  if (s->sgs) {         // the diagonal blocks of the matrix the sweep uses
+    rc = tsb_pcg_set_matrix(s, x_dev, terms, W.diag, st);
+    if (rc != TSB_OK) return fail(nw, rc, s->err);
+  } else {
+    rc = tsb_hess_diag(h, x_dev, terms, 1.f, nullptr, W.diag, st);
+    if (rc != TSB_OK) return fail(nw, rc, h->err);
+  }
+  if (s->coarse) {      // E_c at x; the step's tsb_pcg_set_blocks_ex factors it with the step's shift
+    rc = coarse_form(s, x_dev, *terms, false, st);
+    if (rc != TSB_OK) return fail(nw, rc, s->err);
+  }
+  const cudaError_t e = tsb::launch_newton_prep(s->P, W, prox, st);
+  if (e != cudaSuccess) return fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
+  return TSB_OK;
+}
+
 // One Newton step of every sphere after its arguments are checked: the first call's allocations, then gradient, diagonal
 // blocks, prep (damped: and the shift), preconditioner, (trust region: the radius), solve, dots, line search, decision and
 // the step itself.
@@ -990,21 +1028,10 @@ int newton_run(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const flo
   // the trust-region step's shift w_c: an unusable w_c only reaches a sphere whose b_c is 0
   const float *shift = k.damped ? W.shift : weight_dev;
   // b = -grad, the diagonal blocks; frozen spheres' b = 0 (prox: b -= w (x - y)); damped: mu on a first step
-  rc = energy_grad_impl(h, x_dev, terms->c1, terms->c2, terms->c3, terms->order, -1.f, nullptr, nw->energy, 1, W.b, nullptr, st);
-  if (rc != TSB_OK) return fail(nw, rc, h->err);
-  if (s->sgs) {         // the diagonal blocks of the matrix the sweep uses
-    rc = tsb_pcg_set_matrix(s, x_dev, terms, W.diag, st);
-    if (rc != TSB_OK) return fail(nw, rc, s->err);
-  } else {
-    rc = tsb_hess_diag(h, x_dev, terms, 1.f, nullptr, W.diag, st);
-    if (rc != TSB_OK) return fail(nw, rc, h->err);
-  }
-  if (s->coarse) {      // E_c at x; tsb_pcg_set_blocks_ex below factors it with the step's shift
-    rc = coarse_form(s, x_dev, *terms, false, st);
-    if (rc != TSB_OK) return fail(nw, rc, s->err);
-  }
-  cudaError_t e = tsb::launch_newton_prep(s->P, W, prox, st);
-  if (e == cudaSuccess && k.damped) e = tsb::launch_newton_shift(s->P, W, k.lm, prox, st);
+  rc = newton_rhs(nw, x_dev, terms, prox, st);
+  if (rc != TSB_OK) return rc;
+  cudaError_t e = cudaSuccess;
+  if (k.damped) e = tsb::launch_newton_shift(s->P, W, k.lm, prox, st);
   if (e != cudaSuccess) return fail(nw, TSB_E_CUDA, std::string("newton launch: ") + cudaGetErrorString(e));
   // the preconditioner; trust region: the radius on a first step
   rc = tsb_pcg_set_blocks_ex(s, W.diag, k.rel_floor, shift, nullptr, st);
@@ -1073,6 +1100,94 @@ int tsb_newton_tr_step_ex(tsb_newton_t nw, float *x_dev, const float *anchor_dev
       if (r != 0) return fail(nw, TSB_E_INVALID, "reserved fields must be 0");
   }
   return newton_run(nw, x_dev, anchor_dev, weight_dev, terms, NewtonStep(*opt, bt, records_out_dev), stream);
+}
+
+}  // extern "C"
+
+namespace {
+
+// The L-BFGS options: "" when they hold, or the message of the first broken
+std::string lbfgs_rule_error(const tsb_newton_lbfgs_options_t &o) {
+  if (o.m < 1 || o.m > TSB_LBFGS_MAX_M) return "m must be in [1, " + std::to_string(TSB_LBFGS_MAX_M) + "]";
+  if (!(o.gtol >= 0.f)) return "gtol must be >= 0";
+  if (!(o.sigma > 0.f && o.sigma < 1.f)) return "sigma must be in (0, 1)";
+  if (!(o.eta > 0.f && o.eta <= 1.f)) return "eta must be in (0, 1]";
+  if (o.n_alpha < 1 || o.n_alpha > TSB_LINE_MAX_ALPHA) return "n_alpha must be in [1, " + std::to_string(TSB_LINE_MAX_ALPHA) + "]";
+  if (!(o.rel_floor >= 0.f)) return "rel_floor must be >= 0";
+  if (!(o.curv_eps >= 0.f) || !std::isfinite(o.curv_eps)) return "curv_eps must be finite and >= 0";
+  for (int32_t r : o.reserved)
+    if (r != 0) return "reserved fields must be 0";
+  return "";
+}
+
+// The L-BFGS state of a workspace, allocated by its first L-BFGS step (every history empty, no sphere moved).
+int lbfgs_alloc(tsb_newton_t nw, int32_t m, cudaStream_t st) {
+  if (nw->lb.m) return TSB_OK;
+  const char *refusal = "the first tsb_newton_lbfgs_step of a workspace allocates device memory and cannot be captured in a "
+                        "CUDA graph: make one call outside any capture first";
+  const tsb::PcgParams &P = nw->s->P;
+  const size_t rows = size_t(P.n - P.n_orphans), S = size_t(P.n_components), M1 = size_t(m) + 1;
+  // all or nothing, so the arrays are sized for one m.  Nothing in the slots, x_prev, b_prev or rho is used before a
+  // step writes it; comp is zero: every history empty
+  Rollback<tsb_newton_s> undo(nw);
+  tsb::LbfgsParams L{};
+  int rc = alloc_once(nw, M1 * rows * 3, &L.s, st, refusal);
+  if (rc == TSB_OK) rc = alloc_once(nw, M1 * rows * 3, &L.y, st, refusal);
+  if (rc == TSB_OK) rc = alloc_once(nw, rows * 3, &L.x_prev, st, refusal);
+  if (rc == TSB_OK) rc = alloc_once(nw, rows * 3, &L.b_prev, st, refusal);
+  if (rc == TSB_OK) rc = alloc_once(nw, M1 * S, &L.rho, st, refusal);
+  if (rc == TSB_OK) rc = alloc_once(nw, S, &L.comp, st, refusal, true);
+  if (rc != TSB_OK) return rc;
+  undo.commit();
+  L.m = m;
+  L.rows = int32_t(rows);
+  nw->lb = L;
+  return TSB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int tsb_newton_lbfgs_step(tsb_newton_t nw, float *x_dev, const float *anchor_dev, const float *weight_dev,
+                          const tsb_terms_t *terms, const tsb_newton_lbfgs_options_t *opt,
+                          tsb_newton_lbfgs_sphere_t *records_out_dev, void *stream) {
+  if (!nw) return TSB_E_INVALID;
+  int rc = newton_pointers_check(nw, x_dev, anchor_dev, weight_dev, terms, opt);
+  if (rc != TSB_OK) return rc;
+  const std::string rule = lbfgs_rule_error(*opt);
+  if (!rule.empty()) return fail(nw, TSB_E_INVALID, rule);
+  if (nw->lb.m && opt->m != nw->lb.m)
+    return fail(nw, TSB_E_INVALID, "m = " + std::to_string(opt->m) + " but this workspace's L-BFGS history was sized for m = " +
+                                       std::to_string(nw->lb.m) + " by its first L-BFGS step");
+  tsb_pcg_t s = nw->s;
+  if (const char *m = check_terms(s->h, s->psd, *terms)) return fail(nw, TSB_E_INVALID, m);
+  if (s->sgs || s->coarse)     // H0 is the block-Jacobi preconditioner alone
+    return fail(nw, TSB_E_INVALID, "the L-BFGS step takes H0 from block Jacobi: not on a workspace with the SGS preconditioner "
+                                   "(tsb_pcg_enable_sgs) or the coarse space (tsb_pcg_enable_coarse)");
+  DeviceGuard guard(s->h->device);
+  if (!guard.ok) return fail(nw, TSB_E_CUDA, "cannot select the handle's CUDA device");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  rc = lbfgs_alloc(nw, opt->m, st);
+  if (rc != TSB_OK) return rc;
+  const tsb::NewtonParams &W = nw->W;
+  const tsb::ProxParams pp{x_dev, anchor_dev, weight_dev, nullptr};
+  const tsb::ProxParams *prox = anchor_dev ? &pp : nullptr;
+  const tsb::LbfgsRule r{opt->gtol, opt->sigma, opt->eta, opt->curv_eps, opt->n_alpha};
+  // b = -grad (prox: b -= w (x - y)), frozen spheres' b = 0; H0 = P from the diagonal blocks with the shift w_c (prox)
+  rc = newton_rhs(nw, x_dev, terms, prox, st);
+  if (rc != TSB_OK) return rc;
+  rc = tsb_pcg_set_blocks_ex(s, W.diag, opt->rel_floor, weight_dev, nullptr, st);
+  if (rc != TSB_OK) return fail(nw, rc, s->err);
+  // the direction, the line search at 2^-k, k < n_alpha, per sphere, the decision and the step
+  cudaError_t e = tsb::launch_lbfgs_dir(s->P, W, nw->lb, r, x_dev, prox, st);
+  if (e != cudaSuccess) return fail(nw, TSB_E_CUDA, std::string("lbfgs launch: ") + cudaGetErrorString(e));
+  rc = tsb_line_search(s->h, x_dev, W.d, terms, W.alphas, opt->n_alpha, nw->delta, nullptr, W.sphere_delta, W.sphere_step, st);
+  if (rc != TSB_OK) return fail(nw, rc, s->h->err);
+  e = tsb::launch_lbfgs_decide(s->P, W, nw->lb, r, prox, records_out_dev, st);
+  if (e == cudaSuccess) e = tsb::launch_sphere_axpy(s->P, x_dev, W.alpha_sphere, W.d, x_dev, st);
+  if (e != cudaSuccess) return fail(nw, TSB_E_CUDA, std::string("lbfgs launch: ") + cudaGetErrorString(e));
+  return TSB_OK;
 }
 
 /* ---- Assembled Hessian (tsb_hessian.cu) ---- */

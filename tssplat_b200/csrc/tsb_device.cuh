@@ -1,5 +1,6 @@
-// Small device helpers shared by the solver (tsb_solver.cu), the Gauss-Seidel sweep (tsb_sgs.cu) and the projected
-// Hessian (tsb_psd.cu): the fixed-order CTA sum and the per-vertex 3-vector access.
+// Small device helpers shared by the solver (tsb_solver.cu), the Gauss-Seidel sweep (tsb_sgs.cu), the projected
+// Hessian (tsb_psd.cu) and the L-BFGS step (tsb_lbfgs.cu): the fixed-order CTA sum, the per-vertex 3-vector access and
+// the proximal step's weight test and objective change.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -31,6 +32,16 @@ __device__ __forceinline__ F3 apply_block(const float *pinv, int v, F3 r) {
   const float *q = pinv + 6 * size_t(v);
   const float xx = q[0], yy = q[1], zz = q[2], yz = q[3], xz = q[4], xy = q[5];
   return F3{xx * r.x + xy * r.y + xz * r.z, xy * r.x + yy * r.y + yz * r.z, xz * r.x + yz * r.y + zz * r.z};
+}
+
+// The proximal weight of a component is usable when it is finite and >= 0 (NaN fails both tests).
+__device__ __forceinline__ bool prox_weight_ok(float wc) { return wc >= 0.f && wc < INFINITY; }
+
+// Phi_c(x + a d) - Phi_c(x) from the line search's dE = E_c(x + a d) - E_c(x): dE + w_c (a d.(x - y) + a^2 |d|^2 / 2).
+// Without PROX, or with w_c = 0, it is dE itself.
+template <bool PROX>
+__device__ __forceinline__ double step_change(float dE, double wc, double a, double dx, double dd) {
+  return PROX && wc > 0.0 ? double(dE) + wc * (a * dx + 0.5 * a * a * dd) : double(dE);
 }
 
 }  // namespace tsb

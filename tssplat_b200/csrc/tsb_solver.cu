@@ -420,9 +420,6 @@ __device__ __forceinline__ double block_max(double v, double *sh) {
   return m;
 }
 
-// The proximal weight of a component is usable when it is finite and >= 0 (NaN fails both tests).
-__device__ __forceinline__ bool prox_weight_ok(float wc) { return wc >= 0.f && wc < INFINITY; }
-
 // b_c = 0 on the components already frozen; per-chunk maximum of the diagonal entries (D_v)_ii.  PROX: b_c = 0 also where
 // w_c is unusable, and elsewhere b_v += (-w_c)(x_v - y_v), each operation rounded on its own (no contraction), as eager
 // torch rounds b + (-w) * (x - y); w_c = 0 leaves b as it is.
@@ -498,13 +495,6 @@ __global__ void __launch_bounds__(kT) newton_dots_kernel(const PcgParams s, cons
     w.part[kNwCols * size_t(blockIdx.x) + kNwDd] = dd;
     if (PROX) p.part[blockIdx.x] = dx;
   }
-}
-
-// Phi_c(x + a d) - Phi_c(x) from the line search's dE = E_c(x + a d) - E_c(x): dE + w_c (a d.(x - y) + a^2 |d|^2 / 2).
-// Without PROX, or with w_c = 0, it is dE itself.
-template <bool PROX>
-__device__ __forceinline__ double step_change(float dE, double wc, double a, double dx, double dd) {
-  return PROX && wc > 0.0 ? double(dE) + wc * (a * dx + 0.5 * a * a * dd) : double(dE);
 }
 
 // The step choice and the damping update of every component (thread = component); see tsb_newton_step and

@@ -270,8 +270,10 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         ``newton.NEWTON_DEFAULTS``.  The workspace, ``self.device_newton``, is created on first use (sharing
         ``self.device_pcg``); its ``reset()`` restarts every sphere.  Returns the ``NewtonStepResult``.
         ``FLAGS.newton_method = "tr"`` takes the trust-region step instead (``DeviceNewton.tr_step``; ``opts`` then the
-        fields of ``newton.NEWTON_TR_DEFAULTS``; returns a ``NewtonTRStepResult``), and ``"trls"`` the backtracking
-        trust-region step (``DeviceNewton.trls_step``; the fields of ``newton.NEWTON_TRLS_DEFAULTS``)."""
+        fields of ``newton.NEWTON_TR_DEFAULTS``; returns a ``NewtonTRStepResult``), ``"trls"`` the backtracking
+        trust-region step (``DeviceNewton.trls_step``; the fields of ``newton.NEWTON_TRLS_DEFAULTS``), and ``"lbfgs"``
+        the L-BFGS step (``DeviceNewton.lbfgs_step``; the fields of ``newton.NEWTON_LBFGS_DEFAULTS``; returns a
+        ``NewtonLBFGSStepResult``)."""
         nw = self._device_newton()
         c1, c2 = self.coeff_scheduler(it)
         return nw._step(self._newton_method(), x.data, c1, c2, self.order_at(it), self.amips_coeff, None, None, opts)
@@ -292,7 +294,9 @@ class SmoothnessBarrierEnergy(torch.nn.Module):
         ``NewtonStepResult``.  ``restart`` resets the workspace first: a new anchor is a new problem, and a sphere frozen
         on the old one must not stay frozen.  ``opts``: the fields of ``newton.NEWTON_DEFAULTS`` (of
         ``newton.NEWTON_TR_DEFAULTS`` with ``FLAGS.newton_method = "tr"``, which takes trust-region steps, and of
-        ``newton.NEWTON_TRLS_DEFAULTS`` with ``"trls"``, which takes backtracking trust-region steps)."""
+        ``newton.NEWTON_TRLS_DEFAULTS`` with ``"trls"``, which takes backtracking trust-region steps, and of
+        ``newton.NEWTON_LBFGS_DEFAULTS`` with ``"lbfgs"``, which takes L-BFGS steps; the reset then also empties every
+        sphere's L-BFGS history, which belongs to the old anchor)."""
         if n_steps < 1:
             raise ValueError("n_steps must be >= 1")
         nw = self._device_newton()

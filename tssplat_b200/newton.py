@@ -21,7 +21,10 @@ data term keeps its first-order optimiser.  ``DeviceNewton.tr_step`` is the trus
 (``tsb_newton_tr_step``): no damping shift, a per-sphere radius in the preconditioner norm inside which the solve
 (``DevicePCG.solve(..., radius=)``, ``tsb_pcg_solve_tr``) follows negative curvature to the boundary.
 ``DeviceNewton.trls_step`` (``tsb_newton_tr_step_ex``) is the same step, but one the trust-region rule rejects is
-backtracked along ``2^-k`` with the Armijo test instead of being dropped whole.
+backtracked along ``2^-k`` with the Armijo test instead of being dropped whole.  ``DeviceNewton.lbfgs_step``
+(``tsb_newton_lbfgs_step``) is the quasi-Newton alternative: a per-sphere L-BFGS direction from the gradients of earlier
+steps with the block-Jacobi preconditioner as its initial inverse Hessian, and the damped step's line search; no
+Hessian-vector products and no solve.
 """
 from __future__ import annotations
 
@@ -32,7 +35,7 @@ import torch
 
 __all__ = ["hess_blocks", "block_jacobi", "apply_blocks", "pcg", "PCGResult", "DevicePCG", "DevicePCGResult", "DeviceNewton",
            "NewtonStepResult", "NEWTON_DEFAULTS", "HESSIANS", "NewtonTRStepResult", "NEWTON_TR_DEFAULTS", "NEWTON_TRLS_DEFAULTS",
-           "METHODS"]
+           "NEWTON_LBFGS_DEFAULTS", "NewtonLBFGSStepResult", "METHODS"]
 
 
 def hess_blocks(planes: torch.Tensor) -> torch.Tensor:
@@ -435,6 +438,26 @@ class NewtonTRStepResult(NamedTuple):
     first_vertex: torch.Tensor      # i32: lowest vertex id of the sphere
 
 
+#: options of ``DeviceNewton.lbfgs_step`` (``tsb_newton_lbfgs_options_t``)
+NEWTON_LBFGS_DEFAULTS = dict(m=8, sigma=1e-4, eta=0.9, n_alpha=8, rel_floor=1e-6, gtol=0.0, curv_eps=1e-8)
+
+
+class NewtonLBFGSStepResult(NamedTuple):
+    """What ``DeviceNewton.lbfgs_step`` returns: device tensors [S], spheres in the order of their lowest vertex ids
+    (``tsb_newton_lbfgs_sphere_t`` in ``include/tssplat_b200.h``)."""
+    grad_norm: torch.Tensor         # f32: |grad_c| before the step (0 once the sphere is frozen)
+    alpha: torch.Tensor             # f32: step taken (0: none)
+    k: torch.Tensor                 # i32: index of the step size 2^-k taken, -1 when none
+    delta: torch.Tensor             # f32: objective change of the step taken (0 if none)
+    b_dot_d: torch.Tensor           # f32: b_c . d_c, b = -grad
+    d_norm: torch.Tensor            # f32: |d_c|
+    n_pairs: torch.Tensor           # i32: (s, y) pairs held after the step
+    pair_kept: torch.Tensor         # i32: -1 no pair this step, 0 rejected by the curvature test, 1 kept
+    history_cleared: torch.Tensor   # i32: 1 when the history was cleared this step
+    status: torch.Tensor            # i32: 0 active, 1 converged, 2 stalled (both frozen)
+    first_vertex: torch.Tensor      # i32: lowest vertex id of the sphere
+
+
 class _Method(NamedTuple):
     defaults: dict                  # the options and their defaults
     what: str                       # what an unknown option's error calls them
@@ -453,10 +476,12 @@ _STEPS = {
                   "tsb_newton_tr_sphere_t", NewtonTRStepResult, "tr_step"),
     "trls": _Method(NEWTON_TRLS_DEFAULTS, "backtracking trust-region", ("tsb_newton_tr_options_t", "tsb_newton_backtrack_t"),
                     "tsb_newton_tr_step_ex", None, "tsb_newton_tr_sphere_t", NewtonTRStepResult, "trls_step"),
+    "lbfgs": _Method(NEWTON_LBFGS_DEFAULTS, "L-BFGS", ("tsb_newton_lbfgs_options_t",), "tsb_newton_lbfgs_step", None,
+                     "tsb_newton_lbfgs_sphere_t", NewtonLBFGSStepResult, "lbfgs_step"),
 }
 
-#: the steps of ``DeviceNewton.minimize``: Levenberg-Marquardt (``step``), trust region (``tr_step``) or backtracking
-#: trust region (``trls_step``)
+#: the steps of ``DeviceNewton.minimize``: Levenberg-Marquardt (``step``), trust region (``tr_step``), backtracking
+#: trust region (``trls_step``) or L-BFGS (``lbfgs_step``)
 METHODS = tuple(_STEPS)
 
 
@@ -470,7 +495,8 @@ class DeviceNewton:
     diagonal from it.  ``coarse``: ``None`` or ``"affine"`` (see ``DevicePCG``), taken from ``pcg`` when one is given (a
     different value is an error); on a coarse workspace every damped and proximal step forms the coarse matrix at its
     point, and ``tr_step`` / ``trls_step`` are refused (``tsb_newton_tr_step``: the two-level norm is near-singular along
-    the coarse modes and the trust-region steps stall)."""
+    the coarse modes and the trust-region steps stall).  ``lbfgs_step`` takes block Jacobi alone as its initial inverse
+    Hessian, so it is refused on an SGS or coarse workspace."""
 
     def __init__(self, tet_sp, pcg: Optional[DevicePCG] = None, hessian: Optional[str] = None,
                  precond: Optional[str] = None, coarse: Optional[str] = None):
@@ -504,8 +530,8 @@ class DeviceNewton:
 
     @property
     def device_bytes(self) -> int:
-        """``tsb_newton_device_bytes``: grows by 8 bytes per chunk at the first proximal step and by 20 bytes per sphere
-        at the first trust-region step."""
+        """``tsb_newton_device_bytes``: grows by 8 bytes per chunk at the first proximal step, by 20 bytes per sphere
+        at the first trust-region step and by the L-BFGS history at the first ``lbfgs_step``."""
         return int(self._capi.lib.tsb_newton_device_bytes(self._nw))
 
     def __del__(self):
@@ -525,7 +551,8 @@ class DeviceNewton:
             raise RuntimeError(f"DeviceNewton.{what}: {self._error(self._nw)} (code {rc})")
 
     def reset(self) -> None:
-        """Every sphere ACTIVE again, its damping (and trust radius) re-initialised at the next step."""
+        """Every sphere ACTIVE again, its damping (and trust radius) re-initialised at the next step and its L-BFGS
+        history emptied."""
         self._check(self._capi.lib.tsb_newton_reset(self._nw, self._stream_ptr(self.tet_sp.device)), "reset")
 
     def _options(self, method: str, opts: dict) -> list:
@@ -549,6 +576,10 @@ class DeviceNewton:
     def trls_options(self, **opts):
         """(``tsb_newton_tr_options_t``, ``tsb_newton_backtrack_t``) from ``NEWTON_TRLS_DEFAULTS`` updated with ``opts``."""
         return tuple(self._options("trls", opts))
+
+    def lbfgs_options(self, **opts):
+        """``tsb_newton_lbfgs_options_t`` from ``NEWTON_LBFGS_DEFAULTS`` updated with ``opts``."""
+        return self._options("lbfgs", opts)[0]
 
     def _x_anchor(self, x, anchor, weight):
         """Checks x (updated in place) and the proximal pair; returns the weight tensor or None."""
@@ -584,6 +615,18 @@ class DeviceNewton:
         self._check(rc, m.name)
         f = self._capi.record_fields(raw, rec)
         return m.result(*(f[k] for k in m.result._fields))
+
+    def lbfgs_step(self, x: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0,
+                   anchor: Optional[torch.Tensor] = None, weight=None, **opts) -> NewtonLBFGSStepResult:
+        """One L-BFGS step (``tsb_newton_lbfgs_step``) of ``c1 * smooth + c2 * barrier (+ c3 * amips)`` on every sphere,
+        or of the proximal objective with ``anchor`` and ``weight`` as in ``step``; ``x`` is updated in place without a
+        host read.  Each sphere keeps up to ``m`` pairs ``(s, y)`` of its own earlier steps (a pair is kept when
+        ``s.y > curv_eps |s| |y|``); the direction is the two-loop recursion with the block-Jacobi preconditioner at
+        ``x`` as the initial inverse Hessian, and the step is the largest ``2^-k`` with the damped step's Armijo test
+        below the inversion bound.  No step clears the sphere's history, and no step from an empty history stalls it.
+        ``opts``: the fields of ``NEWTON_LBFGS_DEFAULTS``; ``m`` is fixed by the first call.  ``reset`` empties every
+        history.  The first call on a workspace allocates, so it cannot be captured in a CUDA graph; later ones can."""
+        return self._step("lbfgs", x, c1, c2, order, c3, anchor, weight, opts)
 
     def trls_step(self, x: torch.Tensor, c1: float, c2: float, order: int, c3: float = 0.0,
                   anchor: Optional[torch.Tensor] = None, weight=None, **opts) -> NewtonTRStepResult:
@@ -622,7 +665,8 @@ class DeviceNewton:
     def minimize(self, x: torch.Tensor, n_steps: int, c1: float, c2: float, order: int, c3: float = 0.0,
                  check_every: int = 0, anchor: Optional[torch.Tensor] = None, weight=None, method: str = "lm", **opts):
         """Up to ``n_steps`` calls of ``step`` (``method="lm"``), ``tr_step`` (``method="tr"``, ``opts`` then the fields
-        of ``NEWTON_TR_DEFAULTS``) or ``trls_step`` (``method="trls"``, the fields of ``NEWTON_TRLS_DEFAULTS``); returns
+        of ``NEWTON_TR_DEFAULTS``), ``trls_step`` (``method="trls"``, the fields of ``NEWTON_TRLS_DEFAULTS``) or
+        ``lbfgs_step`` (``method="lbfgs"``, the fields of ``NEWTON_LBFGS_DEFAULTS``); returns
         (steps run, the last result).  ``check_every = 0`` never touches the host
         (capturable); ``k > 0`` reads one integer, the number of spheres still active, every ``k`` steps and stops when
         it is 0 (refused while the stream is being captured).  ``anchor`` and ``weight``: the proximal step of
