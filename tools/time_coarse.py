@@ -15,54 +15,33 @@ card, its power limit and maximum SM clock are read in the same process.
 Usage: python tools/time_coarse.py [--rounds 5] [--big] [--max-steps 60] [--out DIR]"""
 import argparse
 import json
-import os
-import sys
 
-import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-from time_hvp import card  # noqa: E402
-from time_sgs import pack_x, sphere_gnorm  # noqa: E402
-from tssplat_b200 import tet_spheres_ext as ext  # noqa: E402
-from tssplat_b200.newton import DeviceNewton, DevicePCG  # noqa: E402
+from _timing import alternate, card, mixed_pack, sphere_gnorm, sphere_ids, steps_until, summary, write_json
+from tssplat_b200 import tet_spheres_ext as ext
+from tssplat_b200.newton import DeviceNewton, DevicePCG
 
 C3 = 1e-4
 METHODS = {"lm": ("exact", "step"), "psd": ("psd", "step")}   # the trust-region steps refuse a coarse workspace
 
 
-def event_us(fns, rounds, reps=5):
-    """{name: median, min, max over rounds of us per call}: every round times each fn in turn, reps calls between two
-    CUDA events, so the arms share the machine's state"""
-    for fn in fns.values():
-        fn()
-    torch.cuda.synchronize()
-    out = {k: [] for k in fns}
-    for _ in range(rounds):
-        for k, fn in fns.items():
-            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            a.record()
-            for _ in range(reps):
-                fn()
-            b.record()
-            b.synchronize()
-            out[k].append(1e3 * a.elapsed_time(b) / reps)
-    return {k: dict(median=float(np.median(v)), min=float(np.min(v)), max=float(np.max(v))) for k, v in out.items()}
+def rounds_us(fns, rounds):
+    """{name: median, min, max over rounds of us per call}: one untimed call of each fn, then every round times each fn in
+    turn, 5 calls between two CUDA events, so the arms share the machine's state"""
+    return {k: summary(v) for k, v in alternate(fns, rounds, reps=5, warmup=1).items()}
 
 
 def run_pack(S, amips, args):
-    pk, x_np, quiet = pack_x(S, "mixed")
-    sp = ext.TetSpheres(pk.verts.astype(np.float32).reshape(-1), pk.tets.astype(np.int32).reshape(-1),
-                        enable_amips=True, deterministic=True)
+    pk, x_np, quiet = mixed_pack(S, 1, 3, 4)
+    sp = ext.TetSpheres(pk.verts.reshape(-1), pk.tets.reshape(-1), enable_amips=True, deterministic=True)
     c1, c2, c3 = 2e-4 / S, 2e-4, (C3 if amips else 0.0)
-    x = torch.from_numpy(x_np.astype(np.float32)).cuda()
+    x = torch.from_numpy(x_np).cuda()
     q = torch.from_numpy(quiet).cuda()
     _, g = sp.energy_grad(x, c1, c2, 2, -1.0, c3=c3)
     b = g.reshape(-1, 3).contiguous()
     planes = sp.hess_diag(x, c1, c2, 2, c3=c3)
-    sid = torch.from_numpy(np.repeat(np.arange(S), np.diff(pk.vert_offsets))).cuda()
+    sid = sphere_ids(pk).cuda()
     dmax = torch.zeros(S, dtype=torch.float32, device="cuda").index_reduce_(0, sid, planes[0].max(1).values, "amax",
                                                                            include_self=False)
     mu = (1e-3 * dmax).contiguous()       # the damped step's first shift, tau max (D_v)_ii per sphere
@@ -75,11 +54,11 @@ def run_pack(S, amips, args):
             p.set_blocks(planes, shift=sh)
         r = {name: dict(products=p.solve(x, b, c1, c2, 2, c3=c3, max_iter=400, rtol=1e-3, shift=sh).n_hvp[q].double().mean().item())
              for name, p in (("jacobi", pj), ("coarse", pc))}
-        t = event_us({name: (lambda p=p: p.solve(x, b, c1, c2, 2, c3=c3, max_iter=20, rtol=1e-2, shift=sh))
+        t = rounds_us({name: (lambda p=p: p.solve(x, b, c1, c2, 2, c3=c3, max_iter=20, rtol=1e-2, shift=sh))
                       for name, p in (("jacobi", pj), ("coarse", pc))}, args.rounds)
         for name in t:
             r[name]["solve_us"] = t[name]
-        r["set_coarse_us"] = event_us({"coarse": lambda: pc.set_coarse(x, c1, c2, 2, c3=c3)}, args.rounds)["coarse"]
+        r["set_coarse_us"] = rounds_us({"coarse": lambda: pc.set_coarse(x, c1, c2, 2, c3=c3)}, args.rounds)["coarse"]
         res[hessian] = r
     steps = {}
     for m, (hessian, fn) in METHODS.items():
@@ -93,7 +72,7 @@ def run_pack(S, amips, args):
                 nw.reset()
                 getattr(nw, fn)(xs, c1, c2, 2, c3=c3)
             arms[name] = one
-        steps[m] = event_us(arms, args.rounds)
+        steps[m] = rounds_us(arms, args.rounds)
     res["step_us"] = steps
     return res, (sp, pk, x, quiet, c1, c2, c3)
 
@@ -101,29 +80,17 @@ def run_pack(S, amips, args):
 def time_to_solution(ctx, args):
     sp, pk, x0, quiet, c1, c2, c3 = ctx
     S = pk.num_spheres
-    sid_np = np.repeat(np.arange(S), np.diff(pk.vert_offsets))
-    keep = torch.ones(len(sid_np), dtype=torch.bool, device="cuda")
-    sid = torch.from_numpy(sid_np).cuda()
+    sid = sphere_ids(pk).cuda()
     q = torch.from_numpy(quiet).cuda()
     out = {}
     for m, (hessian, fn) in METHODS.items():
         for name, coarse in (("jacobi", None), ("coarse", "affine")):
             nw = DeviceNewton(sp, hessian=hessian, coarse=coarse)
             x = x0.clone()
-            g0 = sphere_gnorm(sp, x, c1, c2, c3, sid, keep, S)
-            total, k = 0.0, 0
-            while k < args.max_steps:
-                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                a.record()
-                getattr(nw, fn)(x, c1, c2, 2, c3=c3)
-                b.record()
-                b.synchronize()
-                total += 1e3 * a.elapsed_time(b)
-                k += 1
-                if bool((sphere_gnorm(sp, x, c1, c2, c3, sid, keep, S)[q] <= 1e-3 * g0[q]).all()):
-                    break
-            out[f"{m}/{name}"] = dict(steps=k, us=total, reached=k < args.max_steps or
-                                      bool((sphere_gnorm(sp, x, c1, c2, c3, sid, keep, S)[q] <= 1e-3 * g0[q]).all()))
+            g0 = sphere_gnorm(sp, x, c1, c2, c3, sid, S)
+            k, total, reached = steps_until(lambda: getattr(nw, fn)(x, c1, c2, 2, c3=c3), lambda: bool(
+                (sphere_gnorm(sp, x, c1, c2, c3, sid, S)[q] <= 1e-3 * g0[q]).all()), args.max_steps)
+            out[f"{m}/{name}"] = dict(steps=k, us=total, reached=reached)
     return out
 
 
@@ -147,10 +114,7 @@ def main():
                 ctx64 = ctx
     result["time_to_solution_64x4096_amips_on"] = time_to_solution(ctx64, args)
     print(json.dumps({"card": result["card"], "time_to_solution": result["time_to_solution_64x4096_amips_on"]}), flush=True)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "time_coarse.json"), "w") as f:
-            json.dump(result, f, indent=1)
+    write_json(args.out, "time_coarse.json", result)
 
 
 if __name__ == "__main__":

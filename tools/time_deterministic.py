@@ -4,41 +4,18 @@ one process with CUDA events, alternating.  Each timed unit is a CUDA graph of `
 
 Usage: python tools/time_deterministic.py [--rounds 30] [--launches 50] [--out DIR]"""
 import argparse
-import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from tssplat_b200 import tet_spheres_ext as ext  # noqa: E402
-from tssplat_b200.mesh import make_pack, perturb  # noqa: E402
+from _timing import TETS, alternate, capture, card, p10_p90, write_json
+from tssplat_b200 import tet_spheres_ext as ext
+from tssplat_b200.mesh import make_pack, perturb
 
-TETS = 4096
 # (name, spheres, sigma relative to the edge length h, AMIPS coefficient)
 CASES = [("64x4096 benign (0.02 h)", 64, 0.02, 0.0), ("64x4096 inverted (0.35 h)", 64, 0.35, 0.0),
          ("64x4096 AMIPS on (0.02 h)", 64, 0.02, 1e-4), ("1024x4096 benign (0.02 h)", 1024, 0.02, 0.0),
          ("1024x4096 AMIPS on (0.02 h)", 1024, 0.02, 1e-4)]
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
-
-
-def graph_of(sp, x, c1, c2, c3, launches):
-    for _ in range(3):                                    # warm-up outside the capture
-        sp.energy_grad(x, c1, c2, 2, 1.0, c3=c3)
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        for _ in range(launches):
-            sp.energy_grad(x, c1, c2, 2, 1.0, c3=c3)
-    return g
 
 
 def main():
@@ -62,20 +39,13 @@ def main():
         ed, gd = d.energy_grad(x, c1, c2, 2, 1.0, c3=c3)
         torch.cuda.synchronize()
         rel = float((gd - ga).norm() / ga.norm())
-        graphs = {"default": graph_of(a, x, c1, c2, c3, args.launches), "deterministic": graph_of(d, x, c1, c2, c3, args.launches)}
-        times = {k: [] for k in graphs}
-        for _ in range(args.rounds):
-            for k, g in graphs.items():                   # alternating
-                t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                t0.record()
-                g.replay()
-                t1.record()
-                t1.synchronize()
-                times[k].append(t0.elapsed_time(t1) * 1e3 / args.launches)
+        graphs = {k: capture(lambda h=h: h.energy_grad(x, c1, c2, 2, 1.0, c3=c3), None, args.launches, 3, k)
+                  for k, h in (("default", a), ("deterministic", d))}
+        times = alternate(graphs, args.rounds, calls=args.launches)
         r = {"case": name, "spheres": S, "tets": S * TETS, "sigma_rel": sig, "c3": c3, "barrier_energy": float(ea[2]),
              "grad_rel_diff": rel, "energies_bitwise_equal": bool(torch.equal(ea, ed)),
              "us_per_step": {k: float(np.median(v)) for k, v in times.items()},
-             "us_per_step_p10_p90": {k: [float(np.percentile(v, 10)), float(np.percentile(v, 90))] for k, v in times.items()},
+             "us_per_step_p10_p90": {k: p10_p90(v) for k, v in times.items()},
              "device_bytes": {"default": a.info["device_bytes"], "deterministic": d.info["device_bytes"]}, "device": dev}
         us = r["us_per_step"]
         print(f"{name:30s} default {us['default']:8.2f} us  deterministic {us['deterministic']:8.2f} us "
@@ -84,10 +54,7 @@ def main():
         results.append(r)
         del graphs, a, d
         torch.cuda.empty_cache()
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "time_deterministic.json"), "w") as f:
-            json.dump(results, f, indent=1)
+    write_json(args.out, "time_deterministic.json", results)
 
 
 if __name__ == "__main__":

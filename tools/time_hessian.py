@@ -1,5 +1,5 @@
 """Cost of assembling the Hessian: tsb_hessian_assemble against tsb_hvp_ex and tsb_hess_diag on the SAME handle, timed in
-one process with CUDA events over CUDA-graph replays, alternating (time_hvp.time_kinds: median over rounds, us per call).
+one process with CUDA events over CUDA-graph replays, alternating (as time_hvp.py: median over rounds, us per call).
 Also reports the values' bytes (36 per block) over the assembly time against the H100 SXM data sheet's 3.35 TB/s.
 
 Rows: 64 x 4096 and 1024 x 4096, benign (0.02 h) and inverted (0.35 h) inputs, AMIPS off and on (c3 = 1e-4), exact and
@@ -8,24 +8,16 @@ PSD Hessians, on a default handle.
 Usage: python tools/time_hessian.py [--rounds 20] [--launches 20] [--sizes 64,1024] [--out DIR]"""
 import argparse
 import ctypes as C
-import json
-import os
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-from time_hvp import card, time_kinds  # noqa: E402
-from tssplat_b200 import _capi  # noqa: E402
-from tssplat_b200 import tet_spheres_ext as ext  # noqa: E402
-from tssplat_b200.hessian import DeviceHessian  # noqa: E402
-from tssplat_b200.mesh import make_pack, perturb  # noqa: E402
-from tssplat_b200.newton import DevicePCG  # noqa: E402
-
-TETS = 4096
+from _timing import TETS, alternate, capture, card, p10_p90, write_json
+from tssplat_b200 import _capi
+from tssplat_b200 import tet_spheres_ext as ext
+from tssplat_b200.hessian import DeviceHessian
+from tssplat_b200.mesh import make_pack, perturb
+from tssplat_b200.newton import DevicePCG
 C3 = 1e-4
 HBM = 3.35e12
 
@@ -67,12 +59,13 @@ def main():
                                                                hv.data_ptr(), None, s.cuda_stream),
                         "hess_diag": lambda: _capi.lib.tsb_hess_diag(sp._h, x.data_ptr(), C.byref(terms), 1.0, None,
                                                                      planes.data_ptr(), s.cuda_stream)}
-                    times = time_kinds(fns, s, args.rounds, args.launches)
+                    times = alternate({k: capture(fn, s, args.launches, 3, k) for k, fn in fns.items()}, args.rounds,
+                                      calls=args.launches)
                     us = {k: float(np.median(t)) for k, t in times.items()}
                     bw = 36 * hs.nnzb / (us["assemble"] * 1e-6)
                     r = {"spheres": S, "tets": S * TETS, "hessian": hessian, "sigma_rel": sig, "amips_c3": c3, "nnzb": hs.nnzb,
                          "us_per_call": us,
-                         "us_per_call_p10_p90": {k: [float(np.percentile(t, 10)), float(np.percentile(t, 90))] for k, t in times.items()},
+                         "us_per_call_p10_p90": {k: p10_p90(t) for k, t in times.items()},
                          "values_bytes_per_s": bw, "share_of_3_35_TBps": bw / HBM, "device": dev}
                     print(f"{S}x{TETS} {hessian:5s} sigma {sig:<5g} c3={c3:<6g} assemble {us['assemble']:9.1f}  hvp_ex "
                           f"{us['hvp_ex']:8.1f}  hess_diag {us['hess_diag']:8.1f} us   values {bw / 1e12:.2f} TB/s "
@@ -82,10 +75,7 @@ def main():
             torch.cuda.empty_cache()
         del sp
         torch.cuda.empty_cache()
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "time_hessian.json"), "w") as f:
-            json.dump(results, f, indent=1)
+    write_json(args.out, "time_hessian.json", results)
 
 
 if __name__ == "__main__":

@@ -8,59 +8,21 @@ with the gradient against tsb_hvp_ex, on default and deterministic handles.
 Usage: python tools/time_hvp.py [--rounds 30] [--launches 50] [--out DIR]"""
 import argparse
 import ctypes as C
-import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from tssplat_b200 import _capi  # noqa: E402
-from tssplat_b200 import tet_spheres_ext as ext  # noqa: E402
-from tssplat_b200.mesh import make_pack, perturb  # noqa: E402
+from _timing import TETS, alternate, capture, card, p10_p90, write_json
+from tssplat_b200 import _capi
+from tssplat_b200 import tet_spheres_ext as ext
+from tssplat_b200.mesh import make_pack, perturb
 
-TETS = 4096
 # (name, spheres, sigma relative to the edge length h)
 CASES = [("64x4096 benign (0.02 h)", 64, 0.02), ("64x4096 inverted (0.35 h)", 64, 0.35), ("1024x4096 benign (0.02 h)", 1024, 0.02)]
 # AMIPS rows: (name, spheres, sigma, deterministic handle)
 AMIPS_CASES = [("64x4096 AMIPS default", 64, 0.02, False), ("64x4096 AMIPS det", 64, 0.02, True),
                ("1024x4096 AMIPS default", 1024, 0.02, False), ("1024x4096 AMIPS det", 1024, 0.02, True)]
 C3 = 1e-4
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
-
-
-def time_kinds(fns, s, rounds, launches):
-    """{kind: [us per launch of each round]}: one CUDA graph of `launches` calls per kind, replayed alternately."""
-    graphs = {}
-    for k, fn in fns.items():
-        with torch.cuda.stream(s):
-            for _ in range(3):                        # warm-up outside the capture
-                assert fn() == 0
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g, stream=s):
-            for _ in range(launches):
-                assert fn() == 0
-        graphs[k] = g
-    times = {k: [] for k in graphs}
-    for _ in range(rounds):
-        for k, g in graphs.items():                   # alternating
-            t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            t0.record()
-            g.replay()
-            t1.record()
-            t1.synchronize()
-            times[k].append(t0.elapsed_time(t1) * 1e3 / launches)
-    del graphs
-    return times
 
 
 def main():
@@ -104,13 +66,15 @@ def main():
                 return _capi.lib.tsb_hvp(sp._h, x.data_ptr(), v.data_ptr(), c1, c2, 2, 1.0, None, hv.data_ptr(),
                                          curv.data_ptr(), s.cuda_stream)
 
-        times = time_kinds({"gradient": gradient, "hvp": hvp}, s, args.rounds, args.launches)
+        graphs = {k: capture(fn, s, args.launches, 3, k) for k, fn in (("gradient", gradient), ("hvp", hvp))}
+        times = alternate(graphs, args.rounds, calls=args.launches)
+        del graphs
         _, _, st = sp.energy_grad_spheres(x, c1, c2, 2, want_grad=False)
         n_inv = int(st.n_inverted.sum())
         r = {"case": name, "spheres": S, "tets": S * TETS, "sigma_rel": sig, "grid": sp.info["grid"],
              "amips_c3": C3 if amips else 0.0, "deterministic": bool(det),
              "inverted_tets": n_inv, "us_per_launch": {k: float(np.median(t)) for k, t in times.items()},
-             "us_per_launch_p10_p90": {k: [float(np.percentile(t, 10)), float(np.percentile(t, 90))] for k, t in times.items()},
+             "us_per_launch_p10_p90": {k: p10_p90(t) for k, t in times.items()},
              "device": dev}
         us = r["us_per_launch"]
         print(f"{name:28s} gradient {us['gradient']:8.2f} us  hvp {us['hvp']:8.2f} us "
@@ -118,10 +82,7 @@ def main():
         results.append(r)
         del sp
         torch.cuda.empty_cache()
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "time_hvp.json"), "w") as f:
-            json.dump(results, f, indent=1)
+    write_json(args.out, "time_hvp.json", results)
 
 
 if __name__ == "__main__":

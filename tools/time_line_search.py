@@ -8,22 +8,14 @@ Rows: 64 x 4096 benign (0.02 h) and inverted (0.35 h), 1024 x 4096 benign, each 
 Usage: python tools/time_line_search.py [--rounds 30] [--launches 50] [--out DIR]"""
 import argparse
 import ctypes as C
-import json
-import os
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-from time_hvp import card, time_kinds  # noqa: E402
-from tssplat_b200 import _capi  # noqa: E402
-from tssplat_b200 import tet_spheres_ext as ext  # noqa: E402
-from tssplat_b200.mesh import make_pack, perturb  # noqa: E402
-
-TETS = 4096
+from _timing import TETS, alternate, capture, card, p10_p90, write_json
+from tssplat_b200 import _capi
+from tssplat_b200 import tet_spheres_ext as ext
+from tssplat_b200.mesh import make_pack, perturb
 CASES = [("64x4096 benign (0.02 h)", 64, 0.02), ("64x4096 inverted (0.35 h)", 64, 0.35), ("1024x4096 benign (0.02 h)", 1024, 0.02)]
 C3 = 1e-4
 
@@ -65,11 +57,12 @@ def main():
                 return lambda: _capi.lib.tsb_line_search(sp._h, x.data_ptr(), d.data_ptr(), C.byref(terms), alphas.data_ptr(), K,
                                                          delta.data_ptr(), step.data_ptr(), None, None, s.cuda_stream)
 
-            times = time_kinds({"energy": energy_only, "gradient": gradient, "line_K1": line(1), "line_K8": line(8)}, s,
-                               args.rounds, args.launches)
+            fns = {"energy": energy_only, "gradient": gradient, "line_K1": line(1), "line_K8": line(8)}
+            times = alternate({k: capture(fn, s, args.launches, 3, k) for k, fn in fns.items()}, args.rounds,
+                              calls=args.launches)
             r = {"case": name, "spheres": S, "tets": S * TETS, "sigma_rel": sig, "amips_c3": c3, "grid": sp.info["grid"],
                  "us_per_call": {k: float(np.median(t)) for k, t in times.items()},
-                 "us_per_call_p10_p90": {k: [float(np.percentile(t, 10)), float(np.percentile(t, 90))] for k, t in times.items()},
+                 "us_per_call_p10_p90": {k: p10_p90(t) for k, t in times.items()},
                  "device": dev}
             us = r["us_per_call"]
             print(f"{name:28s} c3={c3:<6g} energy {us['energy']:8.2f}  gradient {us['gradient']:8.2f}  "
@@ -77,10 +70,7 @@ def main():
             results.append(r)
         del sp
         torch.cuda.empty_cache()
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "time_line_search.json"), "w") as f:
-            json.dump(results, f, indent=1)
+    write_json(args.out, "time_line_search.json", results)
 
 
 if __name__ == "__main__":

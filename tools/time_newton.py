@@ -20,33 +20,20 @@ Usage: python tools/time_newton.py [--rounds 10] [--out DIR]"""
 import argparse
 import ctypes as C
 import json
-import os
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-from time_hvp import card  # noqa: E402
-from time_pcg import graph_of, timed  # noqa: E402
-from tssplat_b200 import _capi  # noqa: E402
-from tssplat_b200 import tet_spheres_ext as ext  # noqa: E402
-from tssplat_b200.mesh import make_pack, perturb  # noqa: E402
-from tssplat_b200.newton import DeviceNewton  # noqa: E402
-from tssplat_b200.optimizer import AdamUniform  # noqa: E402
+from _timing import (TETS, alternate, capture, card, mixed_pack, p10_p90, sphere_gnorm, sphere_ids, steps_until, timed,
+                     write_json)
+from tssplat_b200 import _capi
+from tssplat_b200 import tet_spheres_ext as ext
+from tssplat_b200.mesh import make_pack, perturb
+from tssplat_b200.newton import DeviceNewton
+from tssplat_b200.optimizer import AdamUniform
 
-TETS = 4096
 C3 = 1e-4
 ALPHAS = [2.0 ** -k for k in range(8)]
-
-
-def checked(f, what):
-    def run():
-        if f() != 0:
-            raise RuntimeError(what)
-    return run
 
 
 def step_cost(S, args, dev, results):
@@ -75,11 +62,8 @@ def step_cost(S, args, dev, results):
             st = s.cuda_stream
             L = _capi.lib
 
-            def steps(n):
-                def run():
-                    for _ in range(n):
-                        assert L.tsb_newton_step(nw._nw, x.data_ptr(), C.byref(terms), C.byref(nwo), None, st) == 0
-                return run
+            def step():
+                return L.tsb_newton_step(nw._nw, x.data_ptr(), C.byref(terms), C.byref(nwo), None, st)
 
             phases = {
                 "gradient": lambda: L.tsb_energy_grad_ex(sp._h, x.data_ptr(), C.byref(terms), -1.0, None, energy.data_ptr(),
@@ -93,44 +77,30 @@ def step_cost(S, args, dev, results):
                 "axpy": lambda: L.tsb_sphere_axpy(ws._s, x.data_ptr(), aS.data_ptr(), d.data_ptr(), xo.data_ptr(), st),
             }
             nw.reset()
-            graphs = {"step": graph_of(steps(1), s), "10 steps": graph_of(steps(10), s)}
-            graphs.update({k: graph_of(checked(f, k), s) for k, f in phases.items()})
-            t = {k: [] for k in graphs}
-            for _ in range(args.rounds):                      # alternating; x restarts from the same point every round
-                for k, g in graphs.items():
-                    x.copy_(x0)
-                    nw.reset()
-                    torch.cuda.synchronize()
-                    us = timed(g.replay)[0]
-                    t[k].append(us / 10 if k == "10 steps" else us)
+            graphs = {"step": capture(step, s, 1, 2, "step"), "10 steps": capture(step, s, 10, 20, "10 steps")}
+            graphs.update({k: capture(f, s, 1, 2, k) for k, f in phases.items()})
+            # alternating; x restarts from the same point every round
+            t = alternate(graphs, args.rounds, before=lambda k: (x.copy_(x0), nw.reset()))
+            del graphs
+            t["10 steps"] = [us / 10 for us in t["10 steps"]]
             med = {k: float(np.median(v)) for k, v in t.items()}
             med["small kernels (step - phases)"] = med["step"] - sum(med[k] for k in phases)
             r = {"case": f"{S}x{TETS} benign (0.02 h)", "amips_c3": c3, "max_iter": K, "us": med,
-                 "us_p10_p90": {k: [float(np.percentile(v, 10)), float(np.percentile(v, 90))] for k, v in t.items()},
+                 "us_p10_p90": {k: p10_p90(v) for k, v in t.items()},
                  "newton_workspace_bytes": nw.device_bytes, "device": dev}
             print(f"{r['case']:26s} c3={c3:<6g} max_iter={K:<3d} " + "  ".join(f"{k} {v:.1f}" for k, v in med.items()), flush=True)
             results.append(r)
-            del graphs
     del nw, ws, sp
     torch.cuda.empty_cache()
 
 
-def sphere_gnorm(sp, x, c1, c2, c3, sid, S):
-    _, g = sp.energy_grad(x, c1, c2, 2, c3=c3)
-    return torch.zeros(S, dtype=torch.float64, device="cuda").index_add_(0, sid, (g.double() ** 2).sum(1)).sqrt()
-
-
 def time_to_solution(args, dev, results):
     S = 64
-    pack = make_pack(S, TETS, seed=0, unique=8)
-    x_np, rough = perturb(pack, sigma_rel=0.02, seed=0), perturb(pack, sigma_rel=0.35, seed=0)
-    vo = pack.vert_offsets
-    for k in range(0, S, 4):
-        x_np[vo[k]:vo[k + 1]] = rough[vo[k]:vo[k + 1]]
+    pack, x_np, quiet = mixed_pack(S, 0, 0, 4)
     x0 = torch.from_numpy(x_np).cuda()
     c1, c2 = 2e-4 / S, 2e-4
-    sid = torch.from_numpy(np.repeat(np.arange(S), np.diff(vo))).cuda()
-    quiet = torch.arange(S, device="cuda") % 4 != 0
+    sid = sphere_ids(pack).cuda()
+    quiet = torch.from_numpy(quiet).cuda()
     alphas = torch.tensor(ALPHAS, device="cuda")
     for c3 in (0.0, C3):
         sp = ext.TetSpheres(pack.verts.reshape(-1), pack.tets.reshape(-1), enable_amips=True, deterministic=True)
@@ -158,12 +128,8 @@ def time_to_solution(args, dev, results):
             for name, (fn, n_max) in arms.items():
                 x = x0.clone()
                 nw.reset()
-                total, steps, done = 0.0, 0, False
-                for steps in range(1, n_max + 1):
-                    total += timed(lambda: fn(x))[0]
-                    if bool((sphere_gnorm(sp, x, c1, c2, c3, sid, S)[quiet] <= target[quiet]).all()):
-                        done = True
-                        break
+                steps, total, done = steps_until(lambda: fn(x), lambda: bool(
+                    (sphere_gnorm(sp, x, c1, c2, c3, sid, S)[quiet] <= target[quiet]).all()), n_max)
                 out[name].append((steps if done else None, total))
             p = torch.nn.Parameter(x0.clone())
             opt = AdamUniform([p], lr=1e-3)
@@ -205,10 +171,7 @@ def main():
     for S in (int(v) for v in args.sizes.split(",")):
         step_cost(S, args, dev, results)
     time_to_solution(args, dev, results)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "time_newton.json"), "w") as f:
-            json.dump(results, f, indent=1)
+    write_json(args.out, "time_newton.json", results)
 
 
 if __name__ == "__main__":

@@ -16,22 +16,16 @@ Usage: python tools/time_pcg.py [--rounds 10] [--iters 20] [--out DIR]"""
 import argparse
 import ctypes as C
 import json
-import os
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-from time_hvp import card  # noqa: E402
-from tssplat_b200 import _capi  # noqa: E402
-from tssplat_b200 import tet_spheres_ext as ext  # noqa: E402
-from tssplat_b200.mesh import make_pack, perturb  # noqa: E402
-from tssplat_b200.newton import DevicePCG, hess_blocks, pcg  # noqa: E402
+from _timing import TETS, capture, card, mixed_pack, p10_p90, timed, write_json
+from tssplat_b200 import _capi
+from tssplat_b200 import tet_spheres_ext as ext
+from tssplat_b200.mesh import make_pack, perturb
+from tssplat_b200.newton import DevicePCG, hess_blocks, pcg
 
-TETS = 4096
 CASES = [("64x4096 benign (0.02 h)", 64, 0.02), ("64x4096 inverted (0.35 h)", 64, 0.35),
          ("1024x4096 benign (0.02 h)", 1024, 0.02), ("1024x4096 inverted (0.35 h)", 1024, 0.35)]
 C3 = 1e-4
@@ -43,26 +37,6 @@ def torch_blocks(ws, planes):
     this size reliably)."""
     q = ws.set_blocks(planes, want_inverse=True)
     return hess_blocks(torch.stack([q[:, :3], q[:, 3:]]))
-
-
-def graph_of(fn, s):
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            fn()
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g, stream=s):
-        fn()
-    return g
-
-
-def timed(run):
-    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    t0.record()
-    out = run()
-    t1.record()
-    t1.synchronize()
-    return t0.elapsed_time(t1) * 1e3, out
 
 
 def main():
@@ -92,16 +66,15 @@ def main():
             P = torch_blocks(ws, planes)
             torch.cuda.synchronize()
 
-            def hvps():
-                for _ in range(K):
-                    assert _capi.lib.tsb_hvp_ex(sp._h, x.data_ptr(), b.data_ptr(), C.byref(terms), 1.0, None, hv.data_ptr(), None,
-                                                s.cuda_stream) == 0
+            def hvp():
+                return _capi.lib.tsb_hvp_ex(sp._h, x.data_ptr(), b.data_ptr(), C.byref(terms), 1.0, None, hv.data_ptr(), None,
+                                            s.cuda_stream)
 
             def solve():
-                assert _capi.lib.tsb_pcg_solve(ws._s, x.data_ptr(), b.data_ptr(), C.byref(terms), C.byref(opt), d.data_ptr(), None,
-                                               None, s.cuda_stream) == 0
+                return _capi.lib.tsb_pcg_solve(ws._s, x.data_ptr(), b.data_ptr(), C.byref(terms), C.byref(opt), d.data_ptr(),
+                                               None, None, s.cuda_stream)
 
-            g_hvp, g_solve = graph_of(hvps, s), graph_of(solve, s)
+            g_hvp, g_solve = capture(hvp, s, K, 2 * K, "hvp"), capture(solve, s, 1, 2, "solve")
             torch_pcg = lambda: pcg(lambda p: sp.hvp(x, p, c1, c2, 2, c3=c3)[0], b, P, max_iter=K, rtol=0.0)
             torch_pcg()
             t = {"hvp": [], "device_pcg": [], "torch_pcg": []}
@@ -112,7 +85,7 @@ def main():
                 t["torch_pcg"].append(us / ref.n_hvp)
             r = {"case": name, "spheres": S, "sigma_rel": sig, "amips_c3": c3, "iters": K, "torch_pcg_products": ref.n_hvp,
                  "us_per_iteration": {k: float(np.median(v)) for k, v in t.items()},
-                 "us_per_iteration_p10_p90": {k: [float(np.percentile(v, 10)), float(np.percentile(v, 90))] for k, v in t.items()},
+                 "us_per_iteration_p10_p90": {k: p10_p90(v) for k, v in t.items()},
                  "workspace_bytes": ws.device_bytes, "device": dev}
             u = r["us_per_iteration"]
             print(f"{name:28s} c3={c3:<6g} hvp {u['hvp']:8.2f}  device pcg {u['device_pcg']:8.2f}  torch pcg {u['torch_pcg']:9.2f} "
@@ -124,16 +97,11 @@ def main():
 
     # products to reach rtol: one Krylov space over all spheres against one per sphere
     S, rtol = 64, 1e-3
-    pack = make_pack(S, TETS, seed=0, unique=8)
-    x_np, rough = perturb(pack, sigma_rel=0.02, seed=0), perturb(pack, sigma_rel=0.35, seed=0)
-    vo = pack.vert_offsets
-    for k in range(0, S, 4):
-        x_np[vo[k]:vo[k + 1]] = rough[vo[k]:vo[k + 1]]
+    pack, x_np, quiet = mixed_pack(S, 0, 0, 4)
     x = torch.from_numpy(x_np).cuda()
     c1, c2 = 2e-4 / S, 2e-4
     sp = ext.TetSpheres(pack.verts.reshape(-1), pack.tets.reshape(-1), enable_amips=True, deterministic=True)
     ws = DevicePCG(sp)
-    quiet = np.arange(S) % 4 != 0
     for c3 in (0.0, C3):
         _, g = sp.energy_grad(x, c1, c2, 2, c3=c3)
         planes = sp.hess_diag(x, c1, c2, 2, c3=c3)
@@ -154,10 +122,7 @@ def main():
                  "device": dev}
         print(json.dumps(mixed, indent=1), flush=True)
         results.append(mixed)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "time_pcg.json"), "w") as f:
-            json.dump(results, f, indent=1)
+    write_json(args.out, "time_pcg.json", results)
 
 
 if __name__ == "__main__":

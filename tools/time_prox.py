@@ -21,49 +21,20 @@ renderer and image data this says nothing about reconstruction quality.
 Usage: python tools/time_prox.py [--rounds 6] [--replays 5] [--iters 200] [--loop-rounds 5] [--out DIR]"""
 import argparse
 import json
-import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-from time_hvp import card  # noqa: E402
-from time_pcg import timed  # noqa: E402
-from tssplat_b200 import tet_spheres_ext as ext  # noqa: E402
-from tssplat_b200.energies import SmoothnessBarrierEnergy  # noqa: E402
-from tssplat_b200.mesh import make_pack, perturb, surface_vf  # noqa: E402
-from tssplat_b200.newton import DeviceNewton  # noqa: E402
-from tssplat_b200.optimizer import AdamUniform  # noqa: E402
+from _timing import TETS, alternate, capture, card, sm_clock_under_load, summary, write_json
+from tssplat_b200 import tet_spheres_ext as ext
+from tssplat_b200.energies import SmoothnessBarrierEnergy
+from tssplat_b200.mesh import make_pack, perturb, surface_vf
+from tssplat_b200.newton import DeviceNewton
+from tssplat_b200.optimizer import AdamUniform
 
-TETS = 4096
 C3 = 1e-4
-
-
-def sm_clock():
-    """The current SM clock in MHz (nvidia-smi clocks.sm), or None where it cannot be read."""
-    q = subprocess.run(["nvidia-smi", "--query-gpu=clocks.sm", "--format=csv,noheader,nounits"], capture_output=True, text=True)
-    try:
-        return int(q.stdout.strip().splitlines()[torch.cuda.current_device()])
-    except (ValueError, IndexError):
-        return None
-
-
-def sm_clock_under_load(g, us_per_replay):
-    """clocks.sm read while about 0.5 s of replays of the graph g is queued (enqueue, read, synchronise)."""
-    for _ in range(max(1, int(5e5 / us_per_replay))):
-        g.replay()
-    mhz = sm_clock()
-    torch.cuda.synchronize()
-    return mhz
-
-
-def stats(v):
-    return dict(median=float(np.median(v)), min=float(np.min(v)), max=float(np.max(v)))
 
 
 def step_cost(S, args, results):
@@ -83,23 +54,10 @@ def step_cost(S, args, results):
                 x.copy_(x0)
                 nw.reset()
                 nw.step(x, c1, c2, 2, c3=c3, max_iter=10, **kw)
-            with torch.cuda.stream(s):
-                for _ in range(2):                    # warm-up outside the capture (the first prox step allocates)
-                    fn()
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, stream=s):
-                fn()
-            graphs[name] = g
-        times = {k: [] for k in graphs}
-        for _ in range(args.rounds):
-            for k, g in graphs.items():
-                g.replay()
-                torch.cuda.synchronize()
-                us, _ = timed(lambda g=g: [g.replay() for _ in range(args.replays)])
-                times[k].append(us / args.replays)
+            graphs[name] = capture(fn, s, 1, 2, name)        # two warm-up calls: the first prox step allocates
+        times = alternate(graphs, args.rounds, reps=args.replays, before=lambda k: graphs[k].replay())
         key = f"{S}x{TETS} c3={c3:g}"
-        results["cost"][key] = {k: stats(v) for k, v in times.items()}
+        results["cost"][key] = {k: summary(v) for k, v in times.items()}
         r = results["cost"][key]
         clock = r["sm_mhz_under_load"] = sm_clock_under_load(graphs["prox"], r["prox"]["median"])
         for name, kw in arms.items():                 # what the solve did in one step of each arm
@@ -166,7 +124,7 @@ def split_loop(args, results):
     st0 = E.sphere_stats(x0, it)
     results["split_loop"] = dict(iters=args.iters, rounds=args.loop_rounds, weight=args.weight, start=dict(
         data=float(data(x0)), E=float((c1 * st0.smooth + c2 * st0.barrier).sum()), inverted=int(st0.n_inverted.sum())),
-        **{k: dict(ms_per_iter=stats(times[k]), **final[k]) for k in times})
+        **{k: dict(ms_per_iter=summary(times[k]), **final[k]) for k in times})
     print(json.dumps(results["split_loop"], indent=1), flush=True)
 
 
@@ -187,10 +145,7 @@ def main():
     for S in (64, 1024):
         step_cost(S, args, results)
     split_loop(args, results)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "time_prox.json"), "w") as f:
-            json.dump(results, f, indent=1)
+    write_json(args.out, "time_prox.json", results)
 
 
 if __name__ == "__main__":

@@ -23,34 +23,18 @@ Usage: python tools/time_psd.py [--rounds 5] [--launches 10] [--big] [--tts] [--
 import argparse
 import ctypes as C
 import json
-import os
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-from time_hvp import card, time_kinds  # noqa: E402
-from time_prox import sm_clock_under_load  # noqa: E402
-from tssplat_b200 import _capi  # noqa: E402
-from tssplat_b200 import tet_spheres_ext as ext  # noqa: E402
-from tssplat_b200.mesh import make_pack, perturb  # noqa: E402
-from tssplat_b200.newton import DeviceNewton, DevicePCG  # noqa: E402
+from _timing import (TETS, alternate, capture, card, mixed_pack, sm_clock_under_load, sphere_gnorm, sphere_ids, summary,
+                     timed, write_json)
+from tssplat_b200 import _capi
+from tssplat_b200 import tet_spheres_ext as ext
+from tssplat_b200.newton import DeviceNewton, DevicePCG
 
-TETS = 4096
 C3 = 1e-4
-
-
-def pack_x(S, kind):
-    pk = make_pack(S, TETS, seed=0, unique=8)
-    x = perturb(pk, sigma_rel=0.02, seed=1)
-    if kind == "inverted":
-        rough = perturb(pk, sigma_rel=0.35, seed=3)
-        for s in range(0, S, 4):
-            x[pk.vert_offsets[s]:pk.vert_offsets[s + 1]] = rough[pk.vert_offsets[s]:pk.vert_offsets[s + 1]]
-    return pk, x
+ROUGH_EVERY = {"benign": None, "inverted": 4}      # "inverted": every fourth sphere at 0.35 h
 
 
 def project_us(wp, x, v, terms, hv, curv, launches):
@@ -65,23 +49,13 @@ def project_us(wp, x, v, terms, hv, curv, launches):
     return float(np.mean(ts)) if ts else None
 
 
-def sphere_gnorm(sp, x, c1, c2, c3, sid, S):
-    _, g = sp.energy_grad(x, c1, c2, 2, c3=c3)
-    return torch.zeros(S, dtype=torch.float64, device="cuda").index_add_(0, sid, (g.double() ** 2).sum(1)).sqrt()
-
-
 def time_to_solution(args, dev, results):
-    from time_pcg import timed
     S = 64
-    pack = make_pack(S, TETS, seed=0, unique=8)
-    x_np, rough = perturb(pack, sigma_rel=0.02, seed=0), perturb(pack, sigma_rel=0.35, seed=0)
-    vo = pack.vert_offsets
-    for k in range(0, S, 4):
-        x_np[vo[k]:vo[k + 1]] = rough[vo[k]:vo[k + 1]]
+    pack, x_np, quiet = mixed_pack(S, 0, 0, 4)
     x0 = torch.from_numpy(x_np).cuda()
     c1, c2 = 2e-4 / S, 2e-4
-    sid = torch.from_numpy(np.repeat(np.arange(S), np.diff(vo))).cuda()
-    quiet = torch.arange(S, device="cuda") % 4 != 0
+    sid = sphere_ids(pack).cuda()
+    quiet = torch.from_numpy(quiet).cuda()
     for c3 in (0.0, C3):
         sp = ext.TetSpheres(pack.verts.reshape(-1), pack.tets.reshape(-1), enable_amips=True, deterministic=True)
         arms = {"exact": DeviceNewton(sp), "psd": DeviceNewton(sp, hessian="psd")}
@@ -113,10 +87,6 @@ def time_to_solution(args, dev, results):
         torch.cuda.empty_cache()
 
 
-def stats(v):
-    return dict(median=float(np.median(v)), min=float(np.min(v)), max=float(np.max(v)))
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rounds", type=int, default=5)
@@ -134,9 +104,8 @@ def main():
     results = []
     for S in (() if args.tts_only else (64, 1024) if args.big else (64,)):
         for kind in ("benign", "inverted"):
-            pk, x_np = pack_x(S, kind)
-            sp = ext.TetSpheres(np.ascontiguousarray(pk.verts, np.float32).reshape(-1),
-                                np.ascontiguousarray(pk.tets, np.int32).reshape(-1), enable_amips=True, deterministic=True)
+            pk, x_np, _ = mixed_pack(S, 1, 3, ROUGH_EVERY[kind])
+            sp = ext.TetSpheres(pk.verts.reshape(-1), pk.tets.reshape(-1), enable_amips=True, deterministic=True)
             we, wp = DevicePCG(sp), DevicePCG(sp, hessian="psd")
             ne, npd = DeviceNewton(sp, we), DeviceNewton(sp, wp)
             x0 = torch.from_numpy(x_np).cuda()
@@ -160,7 +129,6 @@ def main():
                         xs[key].copy_(x0)
                         nw.reset()
                         nw.step(xs[key], c1, c2, 2, c3=c3, max_iter=it)
-                        return 0
                     return f
 
                 fns = {
@@ -177,10 +145,13 @@ def main():
                     "solve20_psd": lambda: L.tsb_pcg_solve(wp._s, x0.data_ptr(), b.data_ptr(), C.byref(terms), C.byref(o20),
                                                            d.data_ptr(), None, None, st),
                 }
-                t = {k: stats(vv) for k, vv in time_kinds(fns, s, args.rounds, args.launches).items()}
+                t = alternate({k: capture(f, s, args.launches, 3, k) for k, f in fns.items()}, args.rounds,
+                              calls=args.launches)
+                t = {k: summary(vv) for k, vv in t.items()}
                 steps = {"step10_exact": step(ne, "e10", 10), "step20_exact": step(ne, "e20", 20),
                          "step10_psd": step(npd, "p10", 10), "step20_psd": step(npd, "p20", 20)}
-                t.update({k: stats(vv) for k, vv in time_kinds(steps, s, args.rounds, 1).items()})
+                tv = alternate({k: capture(f, s, 1, 3, k) for k, f in steps.items()}, args.rounds)
+                t.update({k: summary(vv) for k, vv in tv.items()})
                 r = dict(S=S, kind=kind, c3=c3, times_us=t)
                 iter_e = (t["solve20_exact"]["median"] - t["solve10_exact"]["median"]) / 10
                 iter_p = (t["solve20_psd"]["median"] - t["solve10_psd"]["median"]) / 10
@@ -192,22 +163,14 @@ def main():
                       f"{t['step10_exact']['median']:.1f} psd {t['step10_psd']['median']:.1f}; step20 exact "
                       f"{t['step20_exact']['median']:.1f} psd {t['step20_psd']['median']:.1f} us", flush=True)
                 results.append(r)
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.stream(s):
-                step(npd, "p10", 10)()
-            torch.cuda.synchronize()
-            with torch.cuda.graph(g, stream=s):
-                step(npd, "p10", 10)()
+            g = capture(step(npd, "p10", 10), s, 1, 1)
             results[-1]["sm_mhz_under_load"] = sm_clock_under_load(g, results[-1]["times_us"]["step10_psd"]["median"])
             print(f"SM clock under load {results[-1]['sm_mhz_under_load']} MHz", flush=True)
             del g, ne, npd, we, wp, sp
             torch.cuda.empty_cache()
     if args.tts or args.tts_only:
         time_to_solution(args, dev, results)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "time_psd.json"), "w") as f:
-            json.dump(dict(device=dev, results=results), f, indent=1)
+    write_json(args.out, "time_psd.json", dict(device=dev, results=results))
 
 
 if __name__ == "__main__":

@@ -19,45 +19,21 @@ are read in the same process.
 Usage: python tools/time_sgs.py [--rounds 5] [--launches 10] [--big] [--out DIR]"""
 import argparse
 import json
-import os
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-from time_hvp import card, time_kinds  # noqa: E402
-from time_prox import sm_clock_under_load  # noqa: E402
-from tssplat_b200 import tet_spheres_ext as ext  # noqa: E402
-from tssplat_b200.mesh import make_pack, perturb  # noqa: E402
-from tssplat_b200.newton import DeviceNewton, DevicePCG  # noqa: E402
+from _timing import (TETS, alternate, capture, card, mixed_pack, sm_clock_under_load, sphere_gnorm, sphere_ids, steps_until,
+                     write_json)
+from tssplat_b200 import tet_spheres_ext as ext
+from tssplat_b200.newton import DeviceNewton, DevicePCG
 
-TETS = 4096
 C3 = 1e-4
-
-
-def pack_x(S, kind):
-    pk = make_pack(S, TETS, seed=0, unique=8)
-    x = perturb(pk, sigma_rel=0.02, seed=1)
-    rough = perturb(pk, sigma_rel=0.35, seed=3)
-    quiet = np.ones(S, bool)
-    for s in range(S):
-        if kind == "inverted" or (kind == "mixed" and s % 4 == 0):
-            x[pk.vert_offsets[s]:pk.vert_offsets[s + 1]] = rough[pk.vert_offsets[s]:pk.vert_offsets[s + 1]]
-            quiet[s] = False
-    return pk, x, quiet
-
-
-def sphere_gnorm(sp, x, c1, c2, c3, sid, keep, S):
-    _, g = sp.energy_grad(x, c1, c2, 2, -1.0, c3=c3)
-    g = g.reshape(-1, 3).double()
-    return torch.zeros(S, dtype=torch.float64, device="cuda").index_add_(0, sid, (g * g).sum(1)[keep]).sqrt()
+ROUGH_EVERY = {"benign": None, "inverted": 1, "mixed": 4}     # the spheres at 0.35 h: none, all, every fourth
 
 
 def run_pack(S, kind, args, out):
-    pk, x_np, quiet = pack_x(S, kind)
+    pk, x_np, quiet = mixed_pack(S, 1, 3, ROUGH_EVERY[kind])
     x = torch.from_numpy(x_np).cuda()
     c1, c2 = 2e-4 / S, 2e-4
     sp = ext.TetSpheres(pk.verts.reshape(-1), pk.tets.reshape(-1), enable_amips=True, deterministic=True)
@@ -78,14 +54,14 @@ def run_pack(S, kind, args, out):
         planes_out = torch.empty_like(planes)
 
         def solve(p, k):
-            return lambda: (p.solve(x, b, c1, c2, 2, c3=c3, max_iter=k, rtol=0.0), 0)[1]
+            return lambda: p.solve(x, b, c1, c2, 2, c3=c3, max_iter=k, rtol=0.0)
 
-        fns = {"apply": lambda: (ps.apply_precond(b, out=z), 0)[1],
-               "set_matrix": lambda: (ps.set_matrix(x, c1, c2, 2, c3=c3, out=planes_out), 0)[1],
+        fns = {"apply": lambda: ps.apply_precond(b, out=z),
+               "set_matrix": lambda: ps.set_matrix(x, c1, c2, 2, c3=c3, out=planes_out),
                "jacobi10": solve(pj, 10), "jacobi20": solve(pj, 20), "sgs10": solve(ps, 10), "sgs20": solve(ps, 20)}
         with torch.cuda.stream(s):
             ps.set_blocks(planes)
-        t = time_kinds(fns, s, args.rounds, args.launches)
+        t = alternate({k: capture(f, s, args.launches, 3, k) for k, f in fns.items()}, args.rounds, calls=args.launches)
         med = {k: float(np.median(v)) for k, v in t.items()}
         res.update(apply_us=med["apply"], set_matrix_us=med["set_matrix"],
                    iter_us_jacobi=(med["jacobi20"] - med["jacobi10"]) / 10, iter_us_sgs=(med["sgs20"] - med["sgs10"]) / 10)
@@ -114,9 +90,14 @@ def run_pack(S, kind, args, out):
 
         def step(name):
             nw, xs = arms[name]
-            return lambda: (xs.copy_(x0), nw.reset(), nw.step(xs, c1, c2, 2, c3=c3, **o), 0)[3]
 
-        t = time_kinds({"step_jacobi": step("jacobi"), "step_sgs": step("sgs")}, s, args.rounds, 1)
+            def f():
+                xs.copy_(x0)
+                nw.reset()
+                nw.step(xs, c1, c2, 2, c3=c3, **o)
+            return f
+
+        t = alternate({f"step_{k}": capture(step(k), s, 1, 3, k) for k in ("jacobi", "sgs")}, args.rounds)
         res.update({k + "_us": float(np.median(v)) for k, v in t.items()})
         if kind == "mixed":
             res["tts"] = time_to_solution(sp, pk, x0, quiet, c1, c2, c3, {k: v[0] for k, v in arms.items()}, args)
@@ -126,34 +107,19 @@ def run_pack(S, kind, args, out):
 
 
 def time_to_solution(sp, pk, x0, quiet, c1, c2, c3, nws, args):
-    from tssplat_b200.mesh import connected_components
     S = len(quiet)
-    lab = connected_components(len(pk.verts), pk.tets)
-    used = np.zeros(len(pk.verts), bool)
-    used[np.unique(pk.tets)] = True
-    sid = torch.from_numpy(np.searchsorted(np.unique(lab[used]), lab[used])).cuda()
-    keep = torch.from_numpy(used).cuda()
-    g0 = sphere_gnorm(sp, x0, c1, c2, c3, sid, keep, S).cpu().numpy()
+    sid = sphere_ids(pk).cuda()
+    g0 = sphere_gnorm(sp, x0, c1, c2, c3, sid, S).cpu().numpy()
     o = dict(max_iter=20, rtol=1e-2, gtol=float(1e-3 * g0[quiet].min()))
     out = {k: dict(steps=[], ms=[]) for k in nws}
     for _ in range(args.tts_rounds):
         for name, nw in nws.items():          # alternating
             x = x0.clone()
             nw.reset()
-            tot, steps = 0.0, None
-            for k in range(args.max_steps):
-                t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                t0.record()
-                nw.step(x, c1, c2, 2, c3=c3, **o)
-                t1.record()
-                t1.synchronize()
-                tot += t0.elapsed_time(t1)
-                gn = sphere_gnorm(sp, x, c1, c2, c3, sid, keep, S).cpu().numpy()
-                if (gn[quiet] <= 1e-3 * g0[quiet]).all():
-                    steps = k + 1
-                    break
-            out[name]["steps"].append(steps)
-            out[name]["ms"].append(tot if steps else None)
+            steps, us, done = steps_until(lambda: nw.step(x, c1, c2, 2, c3=c3, **o), lambda: bool(
+                (sphere_gnorm(sp, x, c1, c2, c3, sid, S).cpu().numpy()[quiet] <= 1e-3 * g0[quiet]).all()), args.max_steps)
+            out[name]["steps"].append(steps if done else None)
+            out[name]["ms"].append(us / 1e3 if done else None)
     return {k: dict(steps=v["steps"][0], ms=float(np.median([m for m in v["ms"] if m is not None])) if all(v["ms"]) else None)
             for k, v in out.items()}
 
@@ -173,7 +139,7 @@ def main():
         for kind in ("benign", "inverted", "mixed"):
             run_pack(S, kind, args, out)
     # the SM clock while the last pack's Jacobi solve is replayed
-    pk, x_np, _ = pack_x(64, "mixed")
+    pk, x_np, _ = mixed_pack(64, 1, 3, ROUGH_EVERY["mixed"])
     sp = ext.TetSpheres(pk.verts.reshape(-1), pk.tets.reshape(-1), deterministic=True)
     p = DevicePCG(sp, precond="sgs")
     x = torch.from_numpy(x_np).cuda()
@@ -181,18 +147,10 @@ def main():
     b = torch.ones_like(x)
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        p.solve(x, b, 2e-4 / 64, 2e-4, 2, max_iter=20, rtol=0.0)
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g, stream=s):
-        p.solve(x, b, 2e-4 / 64, 2e-4, 2, max_iter=20, rtol=0.0)
+    g = capture(lambda: p.solve(x, b, 2e-4 / 64, 2e-4, 2, max_iter=20, rtol=0.0), s, 1, 1)
     out["sm_clock_mhz_under_load"] = sm_clock_under_load(g, 500.0)
     print(json.dumps(out, indent=1))
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "time_sgs.json"), "w") as f:
-            json.dump(out, f, indent=1)
+    write_json(args.out, "time_sgs.json", out)
 
 
 if __name__ == "__main__":

@@ -6,29 +6,17 @@ in one process with CUDA events, alternating.  Each timed unit is a CUDA graph o
 Usage: python tools/time_sphere_stats.py [--rounds 30] [--launches 50] [--out DIR]"""
 import argparse
 import ctypes as C
-import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from tssplat_b200 import _capi  # noqa: E402
-from tssplat_b200 import tet_spheres_ext as ext  # noqa: E402
-from tssplat_b200.mesh import make_pack, perturb  # noqa: E402
+from _timing import TETS, alternate, capture, card, p10_p90, write_json
+from tssplat_b200 import _capi
+from tssplat_b200 import tet_spheres_ext as ext
+from tssplat_b200.mesh import make_pack, perturb
 
-TETS = 4096
 # (name, spheres, sigma relative to the edge length h)
 CASES = [("64x4096 benign (0.02 h)", 64, 0.02), ("64x4096 inverted (0.35 h)", 64, 0.35), ("1024x4096 benign (0.02 h)", 1024, 0.02)]
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
 
 
 def main():
@@ -58,31 +46,13 @@ def main():
             return _capi.lib.tsb_energy_grad_spheres(sp._h, x.data_ptr(), C.byref(terms), 1.0, None, energy.data_ptr(),
                                                      grad.data_ptr(), stats.data_ptr(), s.cuda_stream)
 
-        graphs = {}
-        for k, fn in (("default", default), ("spheres", spheres)):
-            with torch.cuda.stream(s):
-                for _ in range(3):                        # warm-up outside the capture
-                    assert fn() == 0
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, stream=s):
-                for _ in range(args.launches):
-                    assert fn() == 0
-            graphs[k] = g
-        times = {k: [] for k in graphs}
-        for _ in range(args.rounds):
-            for k, g in graphs.items():                   # alternating
-                t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                t0.record()
-                g.replay()
-                t1.record()
-                t1.synchronize()
-                times[k].append(t0.elapsed_time(t1) * 1e3 / args.launches)
+        graphs = {k: capture(fn, s, args.launches, 3, k) for k, fn in (("default", default), ("spheres", spheres))}
+        times = alternate(graphs, args.rounds, calls=args.launches)
         st = stats.view(-1)
         n_inv = int(st.view(-1, 40)[:, 28:32].contiguous().view(torch.int32).sum())
         r = {"case": name, "spheres": S, "tets": S * TETS, "sigma_rel": sig, "grid": sp.info["grid"],
              "inverted_tets": n_inv, "us_per_step": {k: float(np.median(v)) for k, v in times.items()},
-             "us_per_step_p10_p90": {k: [float(np.percentile(v, 10)), float(np.percentile(v, 90))] for k, v in times.items()},
+             "us_per_step_p10_p90": {k: p10_p90(v) for k, v in times.items()},
              "device": dev}
         us = r["us_per_step"]
         print(f"{name:28s} default {us['default']:8.2f} us  spheres {us['spheres']:8.2f} us "
@@ -90,10 +60,7 @@ def main():
         results.append(r)
         del graphs, sp
         torch.cuda.empty_cache()
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "time_sphere_stats.json"), "w") as f:
-            json.dump(results, f, indent=1)
+    write_json(args.out, "time_sphere_stats.json", results)
 
 
 if __name__ == "__main__":

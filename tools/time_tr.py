@@ -20,28 +20,17 @@ exact solve and of the trust-region solve at the step's initial radius.
 Usage: python tools/time_tr.py [--rounds 7] [--steps 40] [--tts-rounds 2] [--out DIR]"""
 import argparse
 import json
-import os
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-from time_hvp import card, time_kinds  # noqa: E402
-from time_pcg import timed  # noqa: E402
-from time_prox import sm_clock_under_load  # noqa: E402
-from tssplat_b200 import tet_spheres_ext as ext  # noqa: E402
-from tssplat_b200.mesh import make_pack, perturb  # noqa: E402
-from tssplat_b200.newton import DeviceNewton  # noqa: E402
+from _timing import (TETS, alternate, capture, card, mixed_pack, sm_clock_under_load, sphere_gnorm, sphere_ids, summary,
+                     timed, write_json)
+from tssplat_b200 import tet_spheres_ext as ext
+from tssplat_b200.mesh import make_pack, perturb
+from tssplat_b200.newton import DeviceNewton
 
-TETS = 4096
 C3 = 1e-4
-
-
-def stats(v):
-    return dict(median=float(np.median(v)), min=float(np.min(v)), max=float(np.max(v)))
 
 
 def step_cost(args, results):
@@ -64,12 +53,12 @@ def step_cost(args, results):
                         nw.tr_step(xs[key], c1, c2, 2, c3=c3, max_iter=it)
                     else:
                         nw.step(xs[key], c1, c2, 2, c3=c3, max_iter=it)
-                    return 0
                 return f
 
             s = torch.cuda.Stream()
             fns = {k: arm(k) for k in xs}
-            t = {k: stats(v) for k, v in time_kinds(fns, s, args.rounds, 1).items()}
+            t = alternate({k: capture(f, s, 1, 3, k) for k, f in fns.items()}, args.rounds)
+            t = {k: summary(v) for k, v in t.items()}
             solves = {}
             for k in ("lm20", "tr20"):
                 x = x0.clone()
@@ -77,12 +66,7 @@ def step_cost(args, results):
                 r = (nw.tr_step if k.startswith("tr") else nw.step)(x, c1, c2, 2, c3=c3, max_iter=20)
                 solves[k] = dict(mean_hvp=float(r.n_hvp.float().mean()), status=torch.bincount(r.pcg_status, minlength=7).tolist(),
                                  accepted=int((r.alpha > 0).sum()))
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.stream(s):
-                fns["tr20"]()
-            torch.cuda.synchronize()
-            with torch.cuda.graph(g, stream=s):
-                fns["tr20"]()
+            g = capture(fns["tr20"], s, 1, 1)
             mhz = sm_clock_under_load(g, t["tr20"]["median"])
             del g
             r = dict(S=S, c3=c3, times_us=t, solves=solves, sm_mhz_under_load=mhz,
@@ -94,22 +78,13 @@ def step_cost(args, results):
         torch.cuda.empty_cache()
 
 
-def sphere_gnorm(sp, x, c1, c2, c3, sid, S):
-    _, g = sp.energy_grad(x, c1, c2, 2, c3=c3)
-    return torch.zeros(S, dtype=torch.float64, device="cuda").index_add_(0, sid, (g.double() ** 2).sum(1)).sqrt()
-
-
 def time_to_solution(args, dev, results):
     S = 64
-    pack = make_pack(S, TETS, seed=0, unique=8)
-    x_np, rough = perturb(pack, sigma_rel=0.02, seed=0), perturb(pack, sigma_rel=0.35, seed=0)
-    vo = pack.vert_offsets
-    for k in range(0, S, 4):
-        x_np[vo[k]:vo[k + 1]] = rough[vo[k]:vo[k + 1]]
+    pack, x_np, quiet = mixed_pack(S, 0, 0, 4)
     x0 = torch.from_numpy(x_np).cuda()
     c1, c2 = 2e-4 / S, 2e-4
-    sid = torch.from_numpy(np.repeat(np.arange(S), np.diff(vo))).cuda()
-    quiet = torch.arange(S, device="cuda") % 4 != 0
+    sid = sphere_ids(pack).cuda()
+    quiet = torch.from_numpy(quiet).cuda()
     for c3 in (0.0, C3):
         sp = ext.TetSpheres(pack.verts.reshape(-1), pack.tets.reshape(-1), enable_amips=True, deterministic=True)
         arms = {"lm": DeviceNewton(sp), "psd": DeviceNewton(sp, hessian="psd"), "tr": None}
@@ -173,10 +148,7 @@ def main():
         step_cost(args, results)
     if not args.no_tts:
         time_to_solution(args, dev, results)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "time_tr.json"), "w") as f:
-            json.dump(dict(device=dev, results=results), f, indent=1)
+    write_json(args.out, "time_tr.json", dict(device=dev, results=results))
 
 
 if __name__ == "__main__":

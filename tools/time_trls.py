@@ -20,24 +20,16 @@ the per-sphere statuses, and how many of the rough spheres' steps were backtrack
 Usage: python tools/time_trls.py [--rounds 7] [--steps 40] [--tts-rounds 2] [--out DIR]"""
 import argparse
 import json
-import os
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-from time_hvp import card, time_kinds  # noqa: E402
-from time_pcg import timed  # noqa: E402
-from time_prox import sm_clock_under_load  # noqa: E402
-from time_tr import sphere_gnorm, stats  # noqa: E402
-from tssplat_b200 import tet_spheres_ext as ext  # noqa: E402
-from tssplat_b200.mesh import make_pack, perturb  # noqa: E402
-from tssplat_b200.newton import DeviceNewton  # noqa: E402
+from _timing import (TETS, alternate, capture, card, mixed_pack, sm_clock_under_load, sphere_gnorm, sphere_ids, summary,
+                     timed, write_json)
+from tssplat_b200 import tet_spheres_ext as ext
+from tssplat_b200.mesh import make_pack, perturb
+from tssplat_b200.newton import DeviceNewton
 
-TETS = 4096
 C3 = 1e-4
 
 
@@ -59,12 +51,12 @@ def step_cost(args, results):
                     xs[key].copy_(x0)
                     nw.reset()
                     run(xs[key], c1, c2, 2, c3=c3, max_iter=it)
-                    return 0
                 return f
 
             s = torch.cuda.Stream()
             fns = {k: arm(k) for k in xs}
-            t = {k: stats(v) for k, v in time_kinds(fns, s, args.rounds, 1).items()}
+            t = alternate({k: capture(f, s, 1, 3, k) for k, f in fns.items()}, args.rounds)
+            t = {k: summary(v) for k, v in t.items()}
             # the line search alone along the first trust-region direction, at 8 sizes and at 1
             d = torch.zeros_like(x0)
             nw.reset()
@@ -77,15 +69,10 @@ def step_cost(args, results):
             def ls(alphas):
                 def f():
                     sp.line_search(x0, d, alphas, c1, c2, 2, c3=c3, per_sphere=True)
-                    return 0
                 return f
-            tl = {k: stats(v) for k, v in time_kinds({"ls8": ls(a8), "ls1": ls(a1)}, s, args.rounds, 20).items()}
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.stream(s):
-                fns["trls20"]()
-            torch.cuda.synchronize()
-            with torch.cuda.graph(g, stream=s):
-                fns["trls20"]()
+            tl = alternate({k: capture(ls(a), s, 20, 3, k) for k, a in (("ls8", a8), ("ls1", a1))}, args.rounds, calls=20)
+            tl = {k: summary(v) for k, v in tl.items()}
+            g = capture(fns["trls20"], s, 1, 1)
             mhz = sm_clock_under_load(g, t["trls20"]["median"])
             del g
             r = dict(S=S, c3=c3, times_us=t, line_search_us=tl, sm_mhz_under_load=mhz,
@@ -99,15 +86,11 @@ def step_cost(args, results):
 
 def time_to_solution(args, dev, results):
     S = 64
-    pack = make_pack(S, TETS, seed=0, unique=8)
-    x_np, rough = perturb(pack, sigma_rel=0.02, seed=0), perturb(pack, sigma_rel=0.35, seed=0)
-    vo = pack.vert_offsets
-    for k in range(0, S, 4):
-        x_np[vo[k]:vo[k + 1]] = rough[vo[k]:vo[k + 1]]
+    pack, x_np, quiet = mixed_pack(S, 0, 0, 4)
     x0 = torch.from_numpy(x_np).cuda()
     c1, c2 = 2e-4 / S, 2e-4
-    sid = torch.from_numpy(np.repeat(np.arange(S), np.diff(vo))).cuda()
-    quiet = torch.arange(S, device="cuda") % 4 != 0
+    sid = sphere_ids(pack).cuda()
+    quiet = torch.from_numpy(quiet).cuda()
     for c3 in (0.0, C3):
         sp = ext.TetSpheres(pack.verts.reshape(-1), pack.tets.reshape(-1), enable_amips=True, deterministic=True)
         lm = DeviceNewton(sp)
@@ -169,10 +152,7 @@ def main():
         step_cost(args, results)
     if not args.no_tts:
         time_to_solution(args, dev, results)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "time_trls.json"), "w") as f:
-            json.dump(dict(device=dev, results=results), f, indent=1)
+    write_json(args.out, "time_trls.json", dict(device=dev, results=results))
 
 
 if __name__ == "__main__":
